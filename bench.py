@@ -1,6 +1,6 @@
-"""bench.py -- headline benchmark of the B200-native tensorflow/compression hot path.
+"""bench.py -- headline benchmark of the tensorflow/compression hot path on the H100 (sm_90a).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extras]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--no-extras] [--dump-outputs DIR]
     (N > 1: launched by `python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...`)
 
 Workload (BASELINE.json configs[1], "cfg2"): bls2017 compress path at batch 256, 256x256x3 images,
@@ -21,6 +21,9 @@ the `decode` / `gdn` / `cfg3_bmshj2018` / `model_path` objects of the JSON line 
             table builder); this arm never imports compression_b200.
 Parity: outside the timed region every rank checks its first batch against the oracle, byte for byte, and
 cross-decodes it (`parity_checked`).
+`--dump-outputs DIR` (rank 0) writes what the last timed step returned -- the packed strings' bytes and offsets --
+as DIR/strings_bytes.npy (float32) and DIR/strings_offsets.npy (float64); the inputs are seeded, so two builds
+can be compared output for output.
 
 Weak scaling: every rank codes its own 256-stream batch; rank 0 builds the tables and broadcasts them
 (NCCL); there is no data-path collective.
@@ -53,7 +56,7 @@ def _peaks():
     with open(path) as f:
       p = json.load(f)
     return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-  return 6650.0, "fallback (B200_PROFILING.md)"
+  return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -222,6 +225,7 @@ class ClockSampler:
 
   def __init__(self, index, uuid=None):
     self.index, self.uuid, self.rows, self._stop = index, uuid, [], threading.Event()
+    self._ready = threading.Event()  # set once sampling runs: NVML start-up inside the timed region stalls the launches
     self._t = threading.Thread(target=self._run, daemon=True)
 
   def _run_nvml(self):
@@ -245,6 +249,7 @@ class ClockSampler:
       r = int(get_reasons(h))
       self.rows.append([str(sm), str(mx)] + [("Active" if r & bits[n] else "Not Active")
                                               for n in ("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap")])
+      self._ready.set()
       self._stop.wait(0.05)
 
   def _run(self):
@@ -260,10 +265,12 @@ class ClockSampler:
         self.rows.append([c.strip() for c in out.strip().split(",")])
       except Exception:  # pylint:disable=broad-except
         pass
+      self._ready.set()
       self._stop.wait(0.5)
 
   def __enter__(self):
     self._t.start()
+    self._ready.wait(timeout=15)
     return self
 
   def __exit__(self, *a):
@@ -467,6 +474,7 @@ def main():
   ap.add_argument("--warmup", type=int, default=5)
   ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
   ap.add_argument("--no-extras", action="store_true", help="skip the decode / GDN / cfg3 / model-path / CPU side measurements")
+  ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
   args = ap.parse_args()
   if args.impl == "reference":
     return run_reference(args)
@@ -550,12 +558,14 @@ def main():
   tables_match = None if fixture is None else bool(np.array_equal(fixture["lookup"], model._lookup_host()))
 
   # ---- the timed region: exactly K steps, CUDA events, max over ranks ----
+  last = {}
+
   def timed_region(k):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     ev0.record()
     for i in range(k):
-      step(i)
+      last["strings"] = step(i)
     ev1.record()
     barrier()
     return allmax(ev0.elapsed_time(ev1))
@@ -569,6 +579,8 @@ def main():
   elapsed_ms = timed_region(args.steps)
   if clocks:
     clocks.__exit__()
+  if rank == 0 and args.dump_outputs:
+    dump_outputs(args.dump_outputs, last["strings"])
   launches = _lib.launch_count() - launches0
   value = world * sym_per_step * args.steps / (elapsed_ms * 1e-3) / 1e6
   more = [timed_region(args.steps) for _ in range(4)]   # informational spread of the same region
@@ -634,7 +646,7 @@ def main():
       "config": {
           "workload": WORKLOAD,
           "bits_per_symbol": round(bits_per_symbol, 4), "streams_per_gpu": S, "symbols_per_stream": N,
-          "l2": f"inputs rotate over {n_rot} distinct batches ({n_rot * 33.5:.0f} MB > 126 MB L2)",
+          "l2": f"inputs rotate over {n_rot} distinct batches ({n_rot * 33.5:.0f} MB > 50 MB L2)",
           "parallelism": f"batch-shard x{world}, tables broadcast from rank 0",
           "tables_match_fixture": tables_match,
       },
@@ -667,6 +679,26 @@ def main():
     dist.barrier()
     dist.destroy_process_group()
   faulthandler.cancel_dump_traceback_later()
+
+
+DUMP_LIMIT = 64 << 20  # bytes of .npy payload per dump
+
+
+def dump_outputs(out_dir, strings):
+  """The packed strings of one step as float arrays: bytes (float32, exact for uint8) and offsets (float64, exact
+  below 2^53).  A byte array over the budget is replaced by a fixed, seeded sample (indices beside it)."""
+  os.makedirs(out_dir, exist_ok=True)
+  offsets = strings.offsets_dev.cpu().numpy()
+  raw = strings.bytes_dev[:int(offsets[-1])].cpu().numpy()
+  arrays = {"strings_offsets": offsets.astype(np.float64)}
+  budget = DUMP_LIMIT - offsets.size * 8
+  if raw.size * 4 > budget:
+    idx = np.sort(np.random.default_rng(0).choice(raw.size, size=budget // 12, replace=False))
+    raw = raw[idx]
+    arrays["strings_bytes_sample_index"] = idx.astype(np.float64)
+  arrays["strings_bytes"] = raw.astype(np.float32)
+  for name, a in arrays.items():
+    np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
@@ -706,7 +738,8 @@ def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
       traffic, traffic_note = tj.get("dram_bytes_per_launch"), tj.get("note", "ncu --set full capture of this build")
     else:
       traffic_note = "profiles/encode_kernel_traffic.json was captured on another build of range_coder.cu: not reported"
-  sm_clock = (result.get("clocks") or {}).get("sm_mhz") or 1965
+  sm_clock = (result.get("clocks") or {}).get("sm_mhz") or 1980
+  sms = torch.cuda.get_device_properties(dev).multi_processor_count
   result["roofline"] = {
       "kernel": "encode_kernel (fused quantise + range encode; gather / chain / drain warps per stream)", "bound": "hbm",
       "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
@@ -714,7 +747,7 @@ def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
       "peak_source": peak_src, "kernel_ms": enc_ms, "algorithmic_bytes": alg_bytes,
       "kernel_msym_s": sym_per_step / (enc_ms * 1e-3) / 1e6,
       "chain_cycles_per_symbol": enc_ms * 1e-3 * sm_clock * 1e6 / N,
-      "note": "latency-bound serial recurrence per stream (256 streams on 148 SMs); the HBM fraction is small by "
+      "note": f"latency-bound serial recurrence per stream (256 streams on {sms} SMs); the HBM fraction is small by "
               "construction, chain_cycles_per_symbol is the figure that bounds it",
   }
   # --- decode path (create + fused decode/dequantise + finalize), same strings
@@ -724,7 +757,7 @@ def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
                       "roundtrip_equals_quantize": bool(torch.equal(out, model.quantize(ys[0])))}
   if int(os.environ.get("WORLD_SIZE", "1")) > 1:
     # N > 1 is the scaling measurement: the other ranks wait at a barrier while rank 0 is here, so the long side
-    # measurements (cfg3, GDN at 12 GiB tensors, the model path, the CPU baselines -- rank 0 at N = 1 only) stay
+    # measurements (cfg3, GDN at 3 GiB tensors, the model path, the CPU baselines -- rank 0 at N = 1 only) stay
     # with the single-GPU run
     result["extras_note"] = "N > 1: cfg3 / GDN / model-path / CPU side measurements are taken by the N = 1 run"
     return
@@ -764,10 +797,10 @@ def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
       gdn[name].update({"bwd_ms": ms, "bwd_GBps": gbs, "bwd_frac_of_hbm_peak": gbs / peak})
       del dy
     del x
-  # --- configs[3]: GDN microbench, 192 channels, 64x64 tiles (batch 4096 if memory allows, else 1024)
+  # --- configs[3]: GDN microbench, 192 channels, 64x64 tiles, batch 1024 (x, dy, dx and the backward's workspace,
+  # 3.2 GB each, fit an 80 GB card beside the rest of the run)
   try:
-    free_b, _ = torch.cuda.mem_get_info(dev)
-    batch4 = 4096 if free_b > 90e9 else 1024
+    batch4 = 1024
     npix = batch4 * 64 * 64
     gamma192 = (0.1 * torch.eye(192) + (0.02 * torch.randn(192, 192)).abs()).to(dev)
     beta192 = (1 + 0.5 * torch.rand(192)).to(dev)
@@ -783,7 +816,7 @@ def extras(result, model, ys, ys_host, strings, dev, args, sym_per_step, S, N):
     gdn[f"cfg4 [{batch4},64,64,192]"] = entry
     del x, dy
   except Exception as e:  # pylint:disable=broad-except
-    gdn["cfg4 [4096,64,64,192]"] = {"error": repr(e)}
+    gdn["cfg4 [1024,64,64,192]"] = {"error": repr(e)}
   result["gdn"] = gdn
   torch.cuda.empty_cache()
   # --- the model path as configs[1]/[2] name it: images -> analysis transform (conv glue + GDN) -> strings

@@ -1,4 +1,4 @@
-"""compression_b200 -- B200-native (sm_100a) implementation of tensorflow/compression's data-parallel hot
+"""compression_b200 -- H100-native (sm_90a) implementation of tensorflow/compression's data-parallel hot
 path: range coding (multi-stream and legacy ops), PMF->CDF integerisation and GDN/IGDN, behind the
 reference's own operator API (``gen_ops``, ``ContinuousBatchedEntropyModel``,
 ``LocationScaleIndexedEntropyModel``, ``GDN``).  All compute runs in hand-written CUDA kernels reached

@@ -23,7 +23,7 @@ class CudaError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-  """Compiles libtfcb200.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+  """Compiles libtfcb200.so for sm_90a with nvcc (cross-compiles without a GPU)."""
   cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
   if not verbose:
     cmd.insert(1, "-s")

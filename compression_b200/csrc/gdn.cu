@@ -10,7 +10,7 @@
 // Kernel shape (persistent, one CTA per SM): gamma lives in shared memory for the whole launch; a
 // CTA walks 64-pixel tiles; warp w owns 8 pixels, lane l owns output channels {l + 32 m}; the pool
 // tile is read with 128-bit broadcast loads (4 input channels at a time), gamma rows with
-// conflict-free scalar loads.  The tcgen05 tensor-core path lives in gdn_tc.cu.
+// conflict-free scalar loads.  The wgmma tensor-core path lives in gdn_tc.cu.
 #include <algorithm>
 
 #include "common.cuh"
@@ -437,7 +437,7 @@ __global__ void __launch_bounds__(128) gdn_bwd_exponents_kernel(const float* __r
     part[(long long)blockIdx.x * 2 + threadIdx.x] = red[0][threadIdx.x] + red[1][threadIdx.x] + red[2][threadIdx.x] + red[3][threadIdx.x];
 }
 
-constexpr int kExpGrid = 1184;  // blocks of the exponent-gradient kernel (8 per SM)
+constexpr int kExpGrid = 1184;  // blocks of the exponent-gradient kernel (fixed: the reduction order does not depend on the GPU)
 
 int parse_flags(int flags, float alpha, float eps, GdnFlags* f) {
   f->inverse = (flags & TFCB_GDN_INVERSE) != 0;
@@ -459,7 +459,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

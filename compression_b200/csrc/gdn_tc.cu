@@ -1,32 +1,37 @@
-// GDN / IGDN forward on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.
+// GDN / IGDN forward and backward on the Hopper tensor cores (wgmma), sm_90a.
 //
 //   n[pix, i] = sum_j p[pix, j] * gamma[j, i]      p = |x|, x^2 or relu(x) variants (py/layers/gdn.py:377-398)
 //
-// is a [n_pix x C] x [C x C] GEMM with 2*C^2 FLOP per 8*C bytes of HBM traffic: on fp32 CUDA cores it is
-// compute bound at ~1/3 of the HBM roofline.  Here the contraction runs as  tcgen05.mma kind::f16  on an
-// error-compensated bf16 split (3 products: hi*hi + lo*hi + hi*lo, fp32 accumulation in TMEM), which keeps the
-// result within ~4e-6 of fp32 (SURVEY.md App. D; the contract is 1e-5) at bf16 tensor throughput.
+// is a [n_pix x C] x [C x C] GEMM with 2*C^2 FLOP per 8*C bytes of HBM traffic: on fp32 CUDA cores it is compute
+// bound well below the HBM roofline.  Here every contraction runs as  wgmma.mma_async .f32.bf16.bf16  on an
+// error-compensated bf16 split (3 products: hi*hi + lo*hi + hi*lo, fp32 accumulation), which keeps the result within
+// ~4e-6 of fp32 (SURVEY.md App. D; the contract is 1e-5) at bf16 tensor throughput.
 //
-// One CTA per SM, persistent over 128-pixel tiles.  gamma's hi/lo planes live in shared memory for the whole
-// launch in the UMMA "K-major, no swizzle" core-matrix layout ([K/8][N][8] bf16, LBO = N*16 B, SBO = 128 B).
-// Per tile, K is consumed in chunks of 64 channels:
-//   cp.async x[128, 64] fp32 -> staging  ->  threads split |x| into bf16 hi/lo operand planes
-//   ([8][128][8] bf16 each, LBO = 2048 B, SBO = 128 B)  ->  fence.proxy.async  ->  one thread issues 4 K-steps x
-//   3 MMAs (M=128, N=C, K=16)  ->  tcgen05.commit -> mbarrier.
-// Epilogue, 64 output channels at a time: tcgen05.ld (warp w owns TMEM lanes 32*(w%4)..) -> staging ->
-// coalesced pass  y = x / (beta + n)  with x re-read from L2.
+// Forward and the dx half of the backward: persistent CTAs of 2 (C = 192) or 3 (C = 128) warpgroups; each warpgroup
+// walks its own 64-pixel tiles (wgmma M = 64) with no block-level synchronisation after the prologue.  gamma's hi / lo
+// bf16 planes are built once per CTA in shared memory in the no-swizzle core-matrix layout [j / 8][i][j % 8]: read
+// K-major they are the B operand of p . gamma, read MN-major (transposed) the B operand of q . gamma^T, so one copy
+// serves both products (two copies would not fit next to each other at C = 192).  The pixel-side operand comes from
+// registers: a thread loads x at the positions of its wgmma A fragment, which are also the positions of its
+// accumulator fragment, so q = dL/dn is turned into the A operand of q . gamma^T without leaving registers.
+//
+// dgamma = p^T . q reduces over pixels: a second kernel stages 64-pixel chunks of p and q as bf16 planes in shared
+// memory (double-buffered, the next chunk is staged while the tensor cores work on the current one) and accumulates
+// one [64 x C] slice of dgamma per warpgroup.
 //
 // Everything outside {C in {128, 192}, alpha in {1, 2}, eps in {1, 0.5}} falls back to the fp32 kernels in gdn.cu.
-#include <cuda.h>  // CUtensorMap (types only; cuTensorMapEncodeTiled is fetched through the runtime)
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 
 namespace tfcb {
 namespace {
 
-constexpr int kTileM = 128;    // pixels per tile (UMMA M)
+constexpr int kTileM = 64;     // pixels per warpgroup tile (wgmma M)
+constexpr int kMaxParts = 148;  // per-CTA dgamma partials the workspace holds (kDgammaGrid, gdn.cu)
 
 struct TcFlags {
   int inverse, rectify, alpha_mode, eps_mode;  // alpha_mode: 1 |u|, 2 u^2; eps_mode: 1 identity, 2 sqrt
@@ -34,51 +39,53 @@ struct TcFlags {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// UMMA shared-memory descriptor, K-major, SWIZZLE_NONE (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// bits [0,14) start >> 4, [16,30) leading byte offset >> 4 (between the two 8-element K chunks of one MMA),
-// [32,46) stride byte offset >> 4 (between 8-row groups), [46,48) version = 1, [61,64) layout = 0.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+// wgmma shared-memory matrix descriptor, no swizzle: bits [0,14) start >> 4, [16,30) leading-dimension byte offset >> 4
+// (between core matrices along K), [32,46) stride-dimension byte offset >> 4 (between core matrices along M / N).
+// A core matrix is 8 rows of 16 contiguous bytes.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | (1ull << 46);
+         ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
 
-// Instruction descriptor for kind::f16: D = f32 (bits [4,6) = 1), A = B = bf16 ([7,10) = [10,13) = 1), both
-// K-major ([15], [16] = 0), N >> 3 at [17,23), M >> 4 at [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// Keeps reads of the accumulators after the wait for the MMAs that write them.
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&d)[N][32]) {
+#pragma unroll
+  for (int n = 0; n < N; ++n)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[n][i])::"memory");
 }
 
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+#define TFCB_WGMMA_D32                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, " \
+  "%23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define TFCB_WGMMA_D32_OPS                                                                                         \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),    \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),     \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),    \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// d[64 x 64] += A[64 x 16] . B[16 x 64].  A: four bf16x2 registers per thread (the m16n8k16 A fragment of the
+// warp's 16 rows); B: shared memory, K-major (TB = 0) or MN-major (TB = 1).
+template <int TB>
+__device__ __forceinline__ void wgmma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " TFCB_WGMMA_D32
+               ", {%32, %33, %34, %35}, %36, 1, 1, 1, %37;"
+               : TFCB_WGMMA_D32_OPS
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB)
+               : "memory");
 }
 
-__device__ __forceinline__ void umma_commit(uint32_t mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(mbar) : "memory");
-}
-
-__device__ __forceinline__ bool mbar_wait(uint32_t mbar, uint32_t parity) {
-  for (int spin = 0; spin < (1 << 24); ++spin) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(done)
-        : "r"(mbar), "r"(parity)
-        : "memory");
-    if (done) return true;
-  }
-  return false;  // never spin forever on a bad descriptor: the host reports an error instead of hanging
+// d[64 x 64] += A[64 x 16] . B[16 x 64], both MN-major in shared memory.
+__device__ __forceinline__ void wgmma_ss_mn(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " TFCB_WGMMA_D32 ", %32, %33, 1, 1, 1, 1, 1;"
+               : TFCB_WGMMA_D32_OPS
+               : "l"(a), "l"(b)
+               : "memory");
 }
 
 // FAST = the default GDN / IGDN of bls2017 / bmshj2018 (alpha = 1, epsilon = 1, no rectification): no
@@ -91,15 +98,15 @@ __device__ __forceinline__ float tc_pool(float x, const TcFlags& f) {
   return f.rectify ? u : fabsf(u);
 }
 
-// y = u / m (GDN) or u * m (IGDN).  The quotient uses the hardware reciprocal (MUFU.RCP, <= 2 ulp): an IEEE
-// divide costs ~20 instructions per element, which made the whole kernel ALU bound (ncu, profiles/), and
-// 2.4e-7 is far inside the 1e-5 contract.
+// The quotients use the hardware reciprocal (MUFU.RCP, <= 1 ulp): an IEEE divide costs ~20 instructions per element,
+// and 2.4e-7 is far inside the 1e-5 contract.  n = beta + pool is a normal, moderate number.
 __device__ __forceinline__ float rcp_approx(float v) {
   float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));  // MUFU.RCP, <= 1 ulp; n = beta + pool is a normal, moderate number
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
   return r;
 }
 
+// y = u / m (GDN) or u * m (IGDN), m = n or sqrt(n).
 template <bool FAST>
 __device__ __forceinline__ float tc_out(float x, float n, const TcFlags& f) {
   if (FAST) return f.inverse ? x * n : x * rcp_approx(n);
@@ -108,3092 +115,448 @@ __device__ __forceinline__ float tc_out(float x, float n, const TcFlags& f) {
   return f.inverse ? u * m : u * rcp_approx(m);
 }
 
-// bf16 split of 8 consecutive values -> two 16-byte rows of the hi / lo operand planes.
-// Packed conversions (cvt.rn.bf16x2.f32) and integer re-expansion of the hi part keep this at ~3
-// instructions per element.
+// Upstream gradient g at one element: *q = dL/dn, *d = the direct part of dL/du (through the division or product).
+template <bool FAST>
+__device__ __forceinline__ void tc_bwd_point(float x, float g, float n, const TcFlags& f, float* q, float* d) {
+  if (FAST) {
+    if (f.inverse) {
+      *d = g * n;
+      *q = g * x;
+    } else {
+      const float r = rcp_approx(n);
+      *d = g * r;
+      *q = -(*d) * x * r;
+    }
+    return;
+  }
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  if (f.eps_mode == 2) {
+    const float m = sqrtf(n);
+    *d = f.inverse ? g * m : g / m;
+    *q = f.inverse ? 0.5f * g * u / m : -0.5f * g * u / (n * m);
+  } else {
+    *d = f.inverse ? g * n : g / n;
+    *q = f.inverse ? g * u : -g * u / (n * n);
+  }
+}
+
+// d pool / d x, with the rectifier's mask folded in by the caller.
+template <bool FAST>
+__device__ __forceinline__ float tc_dpool(float x, const TcFlags& f) {
+  if (FAST) return (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f);  // TF's abs gradient is sign()
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  if (f.alpha_mode == 2) return 2.f * u;
+  if (f.rectify) return 1.f;
+  return (u > 0.f) ? 1.f : ((u < 0.f) ? -1.f : 0.f);
+}
+
+// Two floats -> bf16x2, the first in the low half (the lower column of a fragment).
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
   return r;
 }
 
+// Error-compensated split of two values: hi = bf16(v), lo = bf16(v - hi).
+__device__ __forceinline__ void split2(float a, float b, uint32_t* hi, uint32_t* lo) {
+  *hi = pack_bf16x2(a, b);
+  *lo = pack_bf16x2(a - __uint_as_float(*hi << 16), b - __uint_as_float(*hi & 0xFFFF0000u));
+}
+
 __device__ __forceinline__ void split8(const float (&v)[8], uint4* hi, uint4* lo) {
   uint32_t h[4], l[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    h[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
-    const float h0 = __uint_as_float(h[i] << 16), h1 = __uint_as_float(h[i] & 0xFFFF0000u);
-    l[i] = pack_bf16x2(v[2 * i] - h0, v[2 * i + 1] - h1);
-  }
+  for (int i = 0; i < 4; ++i) split2(v[2 * i], v[2 * i + 1], &h[i], &l[i]);
   *hi = make_uint4(h[0], h[1], h[2], h[3]);
   *lo = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-// gamma [C, C] fp32 (gamma[j, i]) -> hi / lo bf16 planes in the B-operand layout [j / 8][i][j % 8].
-__global__ void gdn_tc_prep_kernel(const float* __restrict__ gamma, int C, __nv_bfloat16* __restrict__ planes) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // over (j / 8, i)
-  if (idx >= (C / 8) * C) return;
-  const int jc = idx / C, i = idx % C;
-  float v[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) v[e] = gamma[(jc * 8 + e) * C + i];
-  uint4 hi, lo;
-  split8(v, &hi, &lo);
-  reinterpret_cast<uint4*>(planes)[idx] = hi;
-  reinterpret_cast<uint4*>(planes + (size_t)C * C)[idx] = lo;
-}
-
-template <int N>
-__device__ __forceinline__ void tmem_load(uint32_t taddr, uint32_t (&r)[N]);
-
-template <>
-__device__ __forceinline__ void tmem_load<32>(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-
-template <>
-__device__ __forceinline__ void tmem_load<8>(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-
-template <>
-__device__ __forceinline__ void tmem_load<16>(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
-// =============================================================================================
-// Forward, second generation (C = 128): the whole x tile lives in shared memory.
-//
-//   bulk async copies (cp.async.bulk, one 512-byte pixel row each, completion on an mbarrier) bring tile t+1
-//   into a padded [128][132] fp32 buffer while tile t is processed; the same buffer is the epilogue's x source
-//   and, rewritten in place with y, the source of the bulk stores.  Nothing is re-read from L2, no thread ever
-//   waits on a global load, and the 528-byte row stride makes the thread-per-pixel-row accesses (the mapping
-//   tcgen05.ld imposes) bank-conflict free, so no staging transposes and no barriers inside the epilogue.
-//   K is consumed in chunks of 16 channels through two small operand-plane buffers.
-// =============================================================================================
-constexpr int kStLd = 36;  // floats per staging row (32 + 4: conflict-free 128-bit access)
-
-__device__ __forceinline__ void stage_store16(float* dst, const uint32_t (&a)[16]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(__uint_as_float(a[4 * i]), __uint_as_float(a[4 * i + 1]),
-                                                           __uint_as_float(a[4 * i + 2]), __uint_as_float(a[4 * i + 3]));
-}
-
-// dgamma accumulates in TMEM across a CTA's tiles.  The tensor core adds every MMA into the fp32 accumulator with
-// TRUNCATION, so a long-running accumulator shrinks by ~2^-25 per accumulation step: measured 6e-6 of max |dgamma|
-// after one tile per CTA, 6.4e-5 after 110 (2 M pixels), linear in the tile count.  The accumulator is therefore
-// flushed into the CTA's fp32 partial in global memory (round-to-nearest adds, L2 resident) every kDgFlush tiles
-// and restarted; the drift stays below 3e-6 at any pixel count.
-constexpr int kDgFlush = 4;
-
-__device__ __forceinline__ void accum_store16(float* dst, const uint32_t (&a)[16], bool accumulate) {
-  float4 o[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) o[i] = accumulate ? *reinterpret_cast<const float4*>(dst + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-    *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(o[i].x + __uint_as_float(a[4 * i]), o[i].y + __uint_as_float(a[4 * i + 1]),
-                                                           o[i].z + __uint_as_float(a[4 * i + 2]), o[i].w + __uint_as_float(a[4 * i + 3]));
-}
-
-constexpr int kF2Threads = 320;   // 8 compute warps + 1 copy warp + 1 MMA-issue warp
-constexpr int kF2Compute = 256;
-constexpr int kF2XBuf = kTileM * 128 * 4;          // one x / y tile, dense [128][128] fp32 (one bulk copy)
-constexpr int kF2Kg = kTileM * 16 + 160;           // plane group stride: padding = 2 (mod 8) 16-byte units -> conflict-free
-                                                   // stores; sized so that the epilogue's [128][68] staging fits in the planes
-constexpr int kF2StLd = 68;                        // floats per staging row (64 + 4)
-constexpr int kF2Plane = 4 * kF2Kg;                // one hi or lo plane of a 32-channel chunk
-
-struct Fwd2Smem {
-  static constexpr int C = 128;
-  static constexpr int kOffBh = 0;
-  static constexpr int kOffBl = kOffBh + C * C * 2;
-  static constexpr int kOffX = kOffBl + C * C * 2;            // [2] x / y tiles
-  static constexpr int kOffP = kOffX + 2 * kF2XBuf;           // [2 buffers][hi, lo]; the epilogue's staging aliases it
-  static constexpr int kOffBar = kOffP + 4 * kF2Plane;        // full[2], plane[2], y ready[2], TMEM slot
-  static constexpr int kBytes = kOffBar + 64;
-  static_assert(4 * kF2Plane >= kTileM * kF2StLd * 4, "staging must fit in the operand-plane area");
-  static_assert(kBytes <= 232448, "shared memory budget");
-};
-
 // Element type of x / y in memory: 0 float32, 1 float16, 2 bfloat16 (the reference's mixed-precision policy keeps the
 // variables in float32 and the activations in 16 bits, gdn_test.py:200-210; arithmetic is float32 here either way).
+// Pairs of consecutive channels of one pixel; idx is the (even) element index.
 template <int IO>
-struct IoBytes { static constexpr int value = IO == 0 ? 4 : 2; };
-
-template <int IO>
-__device__ __forceinline__ void io_load8(const uint8_t* src, float (&v)[8]) {  // 8 consecutive 16-bit elements
-  const uint4 raw = *reinterpret_cast<const uint4*>(src);
-  const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    if (IO == 2) {
-      v[2 * i] = __uint_as_float(w[i] << 16);
-      v[2 * i + 1] = __uint_as_float(w[i] & 0xFFFF0000u);
-    } else {
-      const __half2 hh = *reinterpret_cast<const __half2*>(&w[i]);
-      const float2 ff = __half22float2(hh);
-      v[2 * i] = ff.x;
-      v[2 * i + 1] = ff.y;
-    }
-  }
+__device__ __forceinline__ float2 ld_pair(const void* base, long long idx) {
+  if (IO == 0) return __ldg(reinterpret_cast<const float2*>(static_cast<const float*>(base) + idx));
+  const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(static_cast<const uint16_t*>(base) + idx));
+  if (IO == 2) return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
+  return __half22float2(*reinterpret_cast<const __half2*>(&w));
 }
 
 template <int IO>
-__device__ __forceinline__ void io_store8(uint8_t* dst, const float (&v)[8]) {
-  uint32_t w[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    if (IO == 2) {
-      w[i] = pack_bf16x2(v[2 * i], v[2 * i + 1]);
-    } else {
-      const __half2 hh = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-      w[i] = *reinterpret_cast<const uint32_t*>(&hh);
-    }
+__device__ __forceinline__ void st_pair(void* base, long long idx, float a, float b) {
+  if (IO == 0) {
+    *reinterpret_cast<float2*>(static_cast<float*>(base) + idx) = make_float2(a, b);
+    return;
   }
-  *reinterpret_cast<uint4*>(dst) = make_uint4(w[0], w[1], w[2], w[3]);
+  uint32_t w;
+  if (IO == 2) {
+    w = pack_bf16x2(a, b);
+  } else {
+    const __half2 h = __floats2half2_rn(a, b);
+    w = *reinterpret_cast<const uint32_t*>(&h);
+  }
+  *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(base) + idx) = w;
 }
 
-template <bool FAST, int IO>
-__global__ void __launch_bounds__(kF2Threads, 1)
-gdn_tc_fwd2_kernel(const void* __restrict__ x_, const float* __restrict__ gamma,
-                   const float* __restrict__ beta, void* __restrict__ y_, long long n_pix, TcFlags f) {
-  using L = Fwd2Smem;
-  constexpr int C = 128;
-  constexpr int EB = IoBytes<IO>::value, kRowB = C * EB;  // bytes per element / per pixel row
-  const uint8_t* x = static_cast<const uint8_t*>(x_);
-  uint8_t* y = static_cast<uint8_t*>(y_);
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* stage = reinterpret_cast<float*>(smem + L::kOffP);          // [128][68] fp32, only during the epilogue
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);  // [0,1] full, [2,3] plane, [4,5] y tile ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + 56);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = tid >> 7, gwarp = warp & 3;
-  constexpr uint32_t kIdesc = umma_idesc(kTileM, C);
+template <int C>
+struct TcCfg {
+  static constexpr int kWG = C == 128 ? 3 : 2;  // warpgroups per CTA: as many as the registers allow
+  static constexpr int kThreads = 128 * kWG;
+  static constexpr int kSmem = 2 * C * C * 2;   // gamma hi / lo planes
+  static_assert(kSmem <= 232448, "shared memory budget");
+};
 
-  // gamma [C, C] fp32 (64 KB, L2 resident) -> hi / lo bf16 planes [j / 8][i][j % 8], converted by every CTA in its
-  // prologue: no per-call allocation and no separate preparation launch (they cost the small shapes 10 %)
-  for (int idx = tid; idx < (C / 8) * C; idx += kF2Threads) {
+// gamma [C, C] fp32 (L2 resident) -> hi / lo bf16 planes [j / 8][i][j % 8] at smem, smem + C * C * 2.  Every CTA
+// converts its own copy in the prologue: no per-call allocation and no separate preparation launch.
+template <int C>
+__device__ __forceinline__ void fill_planes(const float* __restrict__ gamma, uint8_t* smem) {
+  for (int idx = threadIdx.x; idx < (C / 8) * C; idx += blockDim.x) {
     const int jc = idx / C, i = idx % C;
     float v[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) v[e] = __ldg(gamma + (jc * 8 + e) * C + i);
     uint4 hi, lo;
     split8(v, &hi, &lo);
-    reinterpret_cast<uint4*>(smem + L::kOffBh)[idx] = hi;
-    reinterpret_cast<uint4*>(smem + L::kOffBl)[idx] = lo;
+    reinterpret_cast<uint4*>(smem)[idx] = hi;
+    reinterpret_cast<uint4*>(smem + C * C * 2)[idx] = lo;
   }
-  if (tid == 0) {
-    for (int i = 0; i < 6; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbars + i)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(128));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the planes are read by the tensor cores
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_n = *tmem_slot;
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const uint32_t b_hi = smem_u32(smem + L::kOffBh), b_lo = smem_u32(smem + L::kOffBl);
-  const uint32_t xs = smem_u32(smem + L::kOffX);
-  uint32_t par_full[2] = {0u, 0u}, par_plane[2] = {0u, 0u};
+}
 
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  // thread 0 moves the tiles: a tile is one contiguous block of rows * 512 bytes
-  auto issue_load = [&](long long tile, int b) {
-    const long long p0 = tile * kTileM;
-    const uint32_t bytes = (uint32_t)min((long long)kTileM, n_pix - p0) * (uint32_t)kRowB;
-    const uint32_t mbar = smem_u32(mbars + b);
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     xs + b * kF2XBuf),
-                 "l"(x + p0 * kRowB), "r"(bytes), "r"(mbar)
-                 : "memory");
-  };
-  if (warp == kF2Compute / 32) {
-    // ------------------------------ copy warp ------------------------------
-    // Both buffers are filled up front; afterwards, per tile: wait until the compute warps have rewritten the
-    // buffer with y, store it, and as soon as the store has read the buffer refill it with the tile after next.
-    if (lane == 0) {
-      uint32_t par_y[2] = {0u, 0u};
-      if (blockIdx.x < n_tiles) issue_load(blockIdx.x, 0);
-      if (blockIdx.x + (long long)gridDim.x < n_tiles) issue_load(blockIdx.x + gridDim.x, 1);
-      int it = 0;
-      for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-        const int b = it & 1;
-        const long long p0 = tile * kTileM;
-        const uint32_t bytes = (uint32_t)min((long long)kTileM, n_pix - p0) * (uint32_t)kRowB;
-        if (!mbar_wait(smem_u32(mbars + 4 + b), par_y[b])) __trap();
-        par_y[b] ^= 1u;
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(y + p0 * kRowB),
-                     "r"(xs + b * kF2XBuf), "r"(bytes)
-                     : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        const long long nxt = tile + 2ll * gridDim.x;
-        if (nxt < n_tiles) {
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          issue_load(nxt, b);
-        }
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-    __syncwarp();
-  } else if (warp == kF2Compute / 32 + 1) {
-    // ---------------------------- MMA-issue warp ----------------------------
-    // The compute warps only ARRIVE on the chunk's named barrier once their operand planes are written and
-    // fenced; this warp waits on it, issues the chunk's MMAs and commits to the plane mbarrier.  (Barrier ids
-    // alternate with the plane buffer: a buffer is rewritten only after its commit has been waited for.)
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+// A fragments of pool(x) for one tile: k-step kk covers channels 16 kk .. 16 kk + 15; register r of a step holds
+// (row g, cols c, c+1), (row g+8, c, c+1), (row g, c+8, c+9), (row g+8, c+8, c+9), c = 16 kk + 2 t.
+template <int C, bool FAST, int IO>
+__device__ __forceinline__ void pool_frags(const void* __restrict__ x, long long r0, long long r1, bool ok0, bool ok1,
+                                           int t, const TcFlags& f, uint32_t (&ah)[C / 16][4],
+                                           uint32_t (&al)[C / 16][4]) {
 #pragma unroll
-      for (int c = 0; c < C / 32; ++c) {
-        const int pb = c & 1;
-        asm volatile("bar.sync %0, %1;" ::"r"(2 + pb), "n"(kF2Compute + 32) : "memory");
-        if (lane == 0) {
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t ph = smem_u32(smem + L::kOffP + pb * 2 * kF2Plane), pl = ph + kF2Plane;
+  for (int kk = 0; kk < C / 16; ++kk) {
+    const int c = 16 * kk + 2 * t;
+    const float2 z = make_float2(0.f, 0.f);
+    const float2 v[4] = {ok0 ? ld_pair<IO>(x, r0 * C + c) : z, ok1 ? ld_pair<IO>(x, r1 * C + c) : z,
+                         ok0 ? ld_pair<IO>(x, r0 * C + c + 8) : z, ok1 ? ld_pair<IO>(x, r1 * C + c + 8) : z};
 #pragma unroll
-          for (int s2 = 0; s2 < 2; ++s2) {
-            const uint64_t dah = umma_desc(ph + (uint32_t)(2 * s2) * kF2Kg, kF2Kg, 128);
-            const uint64_t dal = umma_desc(pl + (uint32_t)(2 * s2) * kF2Kg, kF2Kg, 128);
-            const uint32_t b_off = (uint32_t)(c * 4 + 2 * s2) * (C * 16);
-            const uint64_t dbh = umma_desc(b_hi + b_off, C * 16, 128);
-            const uint64_t dbl = umma_desc(b_lo + b_off, C * 16, 128);
-            umma_bf16(tmem_n, dah, dbh, kIdesc, (c | s2) ? 1u : 0u);
-            umma_bf16(tmem_n, dal, dbh, kIdesc, 1u);
-            umma_bf16(tmem_n, dah, dbl, kIdesc, 1u);
-          }
-          umma_commit(smem_u32(mbars + 2 + pb));
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-  // ----------------------------- compute warps -----------------------------
-
-  // memory-side items of a 32-channel chunk: (row, kg) = 8 channels of one pixel, two per thread.  Odd rows touch
-  // the two 16-byte halves of their 32 bytes in the opposite order: with the dense 512-byte row stride two
-  // neighbouring rows would otherwise hit the same banks.
-  const int ckg = tid & 3, crow = tid >> 2;
-  const int swap = crow & 1;
-
-  auto compute_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kF2Compute) : "memory"); };
-  int it = 0;
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-    const int b = it & 1;
-    // (b) this tile has landed
-    if (!mbar_wait(smem_u32(mbars + b), par_full[b])) __trap();
-    par_full[b] ^= 1u;
-    uint8_t* xt = smem + L::kOffX + b * kF2XBuf;
-    // (c) pool + bf16 split, 32 channels at a time
-#pragma unroll
-    for (int c = 0; c < C / 32; ++c) {
-      const int pb = c & 1;
-      if (c >= 2) {
-        if (!mbar_wait(smem_u32(mbars + 2 + pb), par_plane[pb])) __trap();
-        par_plane[pb] ^= 1u;
-      }
-      uint8_t* ph = smem + L::kOffP + pb * 2 * kF2Plane;
-      uint8_t* pl = ph + kF2Plane;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = crow + 64 * i;
-        const uint8_t* src = xt + row * kRowB + (c * 32 + ckg * 8) * EB;
-        float v[8];
-        if (IO == 0) {
-          const float4 va = *reinterpret_cast<const float4*>(src + (swap ? 16 : 0));
-          const float4 vb = *reinterpret_cast<const float4*>(src + (swap ? 0 : 16));
-          const float4 v0 = swap ? vb : va, v1 = swap ? va : vb;
-          v[0] = v0.x; v[1] = v0.y; v[2] = v0.z; v[3] = v0.w;
-          v[4] = v1.x; v[5] = v1.y; v[6] = v1.z; v[7] = v1.w;
-        } else {
-          io_load8<IO>(src, v);
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = tc_pool<FAST>(v[e], f);
-        uint4 hi, lo;
-        split8(v, &hi, &lo);
-        *reinterpret_cast<uint4*>(ph + ckg * kF2Kg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(pl + ckg * kF2Kg + row * 16) = lo;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(2 + pb), "n"(kF2Compute + 32) : "memory");
-    }
-    // (d) epilogue in place: y = x / (beta + n).  The last two commits cover every MMA of the tile, after which
-    // the operand planes are dead and their memory is the staging buffer for the TMEM -> row-major transpose.
-#pragma unroll
-    for (int pb = 0; pb < 2; ++pb) {
-      if (!mbar_wait(smem_u32(mbars + 2 + pb), par_plane[pb])) __trap();
-      par_plane[pb] ^= 1u;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // 64 output channels at a time: thread (r, h) moves 32 accumulator columns of its row to the staging buffer,
-    // then every thread finishes four (row, 8-channel) items; lanes 4..7 of each 8-lane group touch the two
-    // 16-byte halves in the opposite order (a row's eight items span 256 B = two passes over the banks).
-    const int ekg = tid & 7, erow = tid >> 3, eswap = (ekg >> 2) & 1;
-#pragma unroll
-    for (int cc = 0; cc < C / 64; ++cc) {
-      {
-        uint32_t acc[32];
-        tmem_load<32>(tmem_n + lane_sel + (uint32_t)(cc * 64 + h * 32), acc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float* dst = stage + r * kF2StLd + h * 32;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(__uint_as_float(acc[4 * i]), __uint_as_float(acc[4 * i + 1]),
-                                                                 __uint_as_float(acc[4 * i + 2]), __uint_as_float(acc[4 * i + 3]));
-      }
-      compute_sync();
-      const float4 bv0 = __ldg(reinterpret_cast<const float4*>(beta + cc * 64 + ekg * 8));
-      const float4 bv1 = __ldg(reinterpret_cast<const float4*>(beta + cc * 64 + ekg * 8) + 1);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int row = erow + 32 * i;
-        uint8_t* src = xt + row * kRowB + (cc * 64 + ekg * 8) * EB;
-        const uint8_t* nsrc = reinterpret_cast<const uint8_t*>(stage + row * kF2StLd + ekg * 8);
-        if (IO != 0) {  // 16-bit elements: one 16-byte load and store per item
-          float xv[8], o[8];
-          io_load8<IO>(src, xv);
-          const float4 na = *reinterpret_cast<const float4*>(nsrc), nb = *reinterpret_cast<const float4*>(nsrc + 16);
-          const float nn[8] = {bv0.x + na.x, bv0.y + na.y, bv0.z + na.z, bv0.w + na.w,
-                               bv1.x + nb.x, bv1.y + nb.y, bv1.z + nb.z, bv1.w + nb.w};
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] = tc_out<FAST>(xv[e], nn[e], f);
-          io_store8<IO>(src, o);
-          continue;
-        }
-        float4* pa = reinterpret_cast<float4*>(src + (eswap ? 16 : 0));
-        float4* pb2 = reinterpret_cast<float4*>(src + (eswap ? 0 : 16));
-        const float4 va = *pa, vb = *pb2;
-        const float4 na = *reinterpret_cast<const float4*>(nsrc + (eswap ? 16 : 0));
-        const float4 nb = *reinterpret_cast<const float4*>(nsrc + (eswap ? 0 : 16));
-        const float4 ba = eswap ? bv1 : bv0, bb = eswap ? bv0 : bv1;
-        float4 oa, ob;
-        oa.x = tc_out<FAST>(va.x, ba.x + na.x, f);
-        oa.y = tc_out<FAST>(va.y, ba.y + na.y, f);
-        oa.z = tc_out<FAST>(va.z, ba.z + na.z, f);
-        oa.w = tc_out<FAST>(va.w, ba.w + na.w, f);
-        ob.x = tc_out<FAST>(vb.x, bb.x + nb.x, f);
-        ob.y = tc_out<FAST>(vb.y, bb.y + nb.y, f);
-        ob.z = tc_out<FAST>(vb.z, bb.z + nb.z, f);
-        ob.w = tc_out<FAST>(vb.w, bb.w + nb.w, f);
-        *pa = oa;
-        *pb2 = ob;
-      }
-      if (cc == C / 64 - 1) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // y tile -> bulk store
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      compute_sync();  // staging free again (and, after the last chunk, for the next tile's operand planes)
-    }
-    // (e) hand the y tile to the copy warp
-    if (tid == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(mbars + 4 + b)) : "memory");
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(128));
+    for (int r = 0; r < 4; ++r) split2(tc_pool<FAST>(v[r].x, f), tc_pool<FAST>(v[r].y, f), &ah[kk][r], &al[kk][r]);
   }
 }
 
-template <bool FAST, int IO>
-int launch_tc_fwd2(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, TcFlags f,
-                   cudaStream_t s) {
-  constexpr int C = 128;
-  using L = Fwd2Smem;
-  {  // the attribute is per device: set it on every launch (microseconds)
-    cudaError_t e = cudaFuncSetAttribute(gdn_tc_fwd2_kernel<FAST, IO>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      return fail(TFCB_CUDA_ERROR, "cannot reserve %d bytes of shared memory: %s", L::kBytes, cudaGetErrorString(e));
+// acc[64 x C] = A . gamma (TB = 0) or A . gamma^T (TB = 1), A = ah + al, gamma = hi + lo planes at bh, bl; the
+// lo . lo product is below fp32 resolution and skipped.  Issues the MMAs and waits for them.
+template <int C, int TB>
+__device__ __forceinline__ void gemm3(float (&acc)[C / 64][32], const uint32_t (&ah)[C / 16][4],
+                                      const uint32_t (&al)[C / 16][4], uint32_t bh, uint32_t bl) {
+#pragma unroll
+  for (int n = 0; n < C / 64; ++n)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[n][i] = 0.f;
+  // K-major: core matrix (k / 8, n / 8) at (k / 8) * C * 16 + (n / 8) * 128 bytes; MN-major (the same planes read as
+  // gamma^T, k = i, n = j): at (n / 8) * C * 16 + (k / 8) * 128.
+  constexpr uint32_t kLbo = TB ? 128 : C * 16, kSbo = TB ? C * 16 : 128;
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < C / 16; ++kk)
+#pragma unroll
+    for (int n = 0; n < C / 64; ++n) {
+      const uint32_t off = TB ? (256u * kk + (uint32_t)n * C * 128) : ((uint32_t)kk * C * 32 + 1024u * n);
+      wgmma_rs<TB>(acc[n], ah[kk], gmma_desc(bh + off, kLbo, kSbo));
+      wgmma_rs<TB>(acc[n], al[kk], gmma_desc(bh + off, kLbo, kSbo));
+      wgmma_rs<TB>(acc[n], ah[kk], gmma_desc(bl + off, kLbo, kSbo));
     }
-  }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>(n_tiles, sms);
-  gdn_tc_fwd2_kernel<FAST, IO><<<grid, kF2Threads, L::kBytes, s>>>(x, gamma, beta, y, n_pix, f);
-  TFCB_LAUNCHED();
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core kernel launch failed: %s", cudaGetErrorString(e));
-  return TFCB_OK;
+  wgmma_commit();
+  wgmma_wait_all();
+  fence_acc(acc);
 }
 
+// Accumulator element (n, jj, h, e) of a thread: row g + 8 h of its warp's 16, column 64 n + 8 jj + 2 t + e.
+#define TFCB_FOR_ACC_PAIRS(C)            \
+  _Pragma("unroll") for (int n = 0; n < (C) / 64; ++n) \
+  _Pragma("unroll") for (int jj = 0; jj < 8; ++jj)     \
+  _Pragma("unroll") for (int h = 0; h < 2; ++h)
 
-// =============================================================================================
-// Forward, C = 192, fourth kernel shape: everything that touches HBM is asynchronous, and the epilogue of one
-// tile runs between the conversion chunks of the next.
-//
-// gamma's hi + lo planes (144 KB) leave no room for x, and feeding the conversion and the epilogue from registers
-// (the round-1 kernel, 52 % of the HBM roofline) leaves every compute thread waiting on its own loads and stores
-// (clock64 trace of a ring-fed variant with register stores: 5.2 k of 15.9 k cycles per tile in the epilogue's store
-// back-pressure, 3 k waiting for boxes of a three-slot ring, 1.7 k waiting for the tensor pipe).  So:
-//   * only gamma's HI plane is resident (72 KB); the LO plane is needed by one of the three products only and is
-//     streamed from L2 per 32-channel K chunk (12 KB bulk copies, double buffered) by a "gamma" warp;
-//   * x arrives as [128 rows x 32 channels] 2-D TMA boxes (128-byte swizzle) in two three-slot rings, twice per
-//     tile: boxes C0..C5 feed the pool + bf16 split, boxes E0..E5 (L2 hits) feed the epilogue; the whole next tile is
-//     prefetched into L2 with one bulk prefetch;
-//   * the epilogue needs no transpose: thread (r, h) takes 16 accumulator columns of ITS pixel row from TMEM,
-//     reads the same 64 bytes of x from its row of the E box (the swizzle makes the row-per-lane access conflict
-//     free), overwrites them with y = x / (beta + n), and a "store" warp sends the box out with a 2-D TMA store;
-//   * two accumulators in TMEM: while the tensor pipe works on tile t + 1 (it is the slower side of the conversion
-//     phase), the compute warps finish box c - 1 of tile t after converting chunk c of tile t + 1.
-// No compute thread ever waits on a global load or store, and there is no CTA-wide barrier in the steady state.
-// Rows past n_pix: zero-filled on load, clipped on store.
-// =============================================================================================
-// L2 eviction-priority descriptors for bulk / tensor copies (the values createpolicy.fractional.L2::evict_* produces
-// for fraction 1.0; same constants as CUTLASS's TMA::CacheHintSm90)
-constexpr unsigned long long kEvictFirst = 0x12F0000000000000ull, kEvictLast = 0x14F0000000000000ull;
-
-constexpr int kF4Compute = 512;                  // 16 compute warps: four per scheduler, the work is latency bound
-constexpr int kF4Threads = kF4Compute + 160;     // + MMA-issue, C-copy, E-copy, gamma and store warps
-constexpr int kF4Sync = kF4Compute + 32;         // compute + issue warps (the named barriers of the plane hand-off)
-constexpr int kF4Box = kTileM * 32 * 4;          // one x box: [128][32] fp32, 128-byte rows, 128B-swizzled
-constexpr int kF4Kg = kTileM * 16 + 32;          // plane group stride: padding = 2 (mod 8) 16-byte units (see kF2Kg)
-constexpr int kF4Plane = 4 * kF4Kg;              // hi or lo plane of a 32-channel chunk
-
-template <int C>
-struct Fwd4Smem {
-  static constexpr int kPlaneB = C * C * 2;                 // gamma hi (resident)
-  static constexpr int kGlo = 4 * C * 16;                   // one 32-channel K chunk of gamma lo
-  static constexpr int kOffBh = 0;
-  static constexpr int kOffRing = kOffBh + kPlaneB;         // [3] C boxes, [3] E boxes (1024-byte aligned: swizzle atom)
-  static constexpr int kOffGlo = kOffRing + 6 * kF4Box;     // [2] gamma lo chunks
-  static constexpr int kOffP = kOffGlo + 2 * kGlo;          // [2 buffers][hi, lo] operand planes
-  static constexpr int kOffBeta = kOffP + 4 * kF4Plane;
-  static constexpr int kOffBar = kOffBeta + C * 4;
-  // mbarriers: plane[2], gfull[2], cfull[3], cempty[3], efull[3], eempty[3], yready[3]; then the TMEM slot
-  static constexpr int kBarPlane = 0, kBarGfull = 2, kBarCfull = 4, kBarCempty = 7, kBarEfull = 10, kBarEempty = 13,
-                       kBarY = 16, kNumBars = 19;
-  static constexpr int kBytes = kOffBar + kNumBars * 8 + 16;
-  static_assert(kOffRing % 1024 == 0 && kOffGlo % 128 == 0 && kOffP % 128 == 0, "alignment");
-  static_assert(kBytes <= 232448, "shared memory budget");
-};
-
-template <int C, bool FAST>
-__global__ void __launch_bounds__(kF4Threads, 1)
-gdn_tc_fwd4_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap y_map,
-                   const float* __restrict__ x, const __nv_bfloat16* __restrict__ planes,
-                   const float* __restrict__ beta, long long n_pix, TcFlags f) {
-  using L = Fwd4Smem<C>;
-  constexpr int NCH = C / 32;  // 6 boxes per pass over a tile
+template <int C, bool FAST, int IO>
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                  void* __restrict__ y, long long n_pix, TcFlags f) {
+  using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* beta_s = reinterpret_cast<float*>(smem + L::kOffBeta);
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + L::kNumBars * 8);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 3, gwarp = warp & 3;  // compute thread (r, h): pixel row r, column quarter h
-  constexpr uint32_t kIdesc = umma_idesc(kTileM, C);
-  auto bar = [&](int i) { return smem_u32(mbars + i); };
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(planes);  // hi plane first
-    uint4* dst = reinterpret_cast<uint4*>(smem + L::kOffBh);
-    for (int i = tid; i < L::kPlaneB / 16; i += kF4Threads) dst[i] = src[i];
-    for (int i = tid; i < C; i += kF4Threads) beta_s[i] = beta[i];
-  }
-  if (tid == 0) {
-    for (int i = 0; i < L::kNumBars; ++i) {
-      const int count = (i >= L::kBarY) ? kF4Compute / 32 : 1;  // y ready: one arrival per compute warp
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar(i)), "r"(count));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;            // accumulator of tile t: columns (t & 1) * 256 ..
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const uint32_t b_hi = smem_u32(smem + L::kOffBh);
+  fill_planes<C>(gamma, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * C * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-
-  // A box ring of three slots: request n uses slot n % 3 in its (n / 3)-th round.
-  auto load_boxes = [&](int ring, bool prefetch_l2) {  // ring 0: C boxes, 1: E boxes
-    const int full0 = ring ? L::kBarEfull : L::kBarCfull, empty0 = ring ? L::kBarEempty : L::kBarCempty;
-    uint32_t n = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int row0 = (int)(tile * kTileM);
-      if (prefetch_l2) {  // the next tile of this CTA -> L2 (one contiguous block): its boxes become L2 hits
-        const long long pn = (tile + gridDim.x) * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - pn);
-        if (rows > 0)
-          asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(x + pn * C),
-                       "r"((uint32_t)(rows * C * 4)), "l"(kEvictLast)
-                       : "memory");
-      }
-#pragma unroll 1
-      for (int k = 0; k < NCH; ++k, ++n) {
-        const uint32_t slot = n % 3u, round = n / 3u;
-        if (round > 0) {
-          if (!mbar_wait(bar(empty0 + slot), (round - 1u) & 1u)) __trap();
-        }
-        const uint32_t full = bar(full0 + slot);
-        const uint32_t dst = smem_u32(smem + L::kOffRing + (ring * 3 + slot) * kF4Box);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "n"(kF4Box) : "memory");
-        // x is read twice (C box, then E box about a tile later): the first read asks L2 to keep the lines, the
-        // second releases them (ncu before the hints: 1.54x the algorithmic DRAM reads at 16.7 M pixels)
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(dst),
-            "l"(&x_map), "r"(k * 32), "r"(row0), "r"(full), "l"(ring ? kEvictFirst : kEvictLast)
-            : "memory");
-      }
+  for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    uint32_t ah[C / 16][4], al[C / 16][4];
+    pool_frags<C, FAST, IO>(x, r0, r1, ok0, ok1, t, f, ah, al);
+    float acc[C / 64][32];
+    gemm3<C, 0>(acc, ah, al, bh, bl);
+    // accumulators are read on every thread (only the memory accesses are predicated): a read inside a divergent
+    // branch makes ptxas serialise the MMAs
+    TFCB_FOR_ACC_PAIRS(C) {
+      const bool ok = h ? ok1 : ok0;
+      const int col = 64 * n + 8 * jj + 2 * t;
+      const long long idx = (h ? r1 : r0) * C + col;
+      const float2 xv = ok ? ld_pair<IO>(x, idx) : make_float2(0.f, 0.f);
+      const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
+      const float y0 = tc_out<FAST>(xv.x, b.x + acc[n][4 * jj + 2 * h], f);
+      const float y1 = tc_out<FAST>(xv.y, b.y + acc[n][4 * jj + 2 * h + 1], f);
+      if (ok) st_pair<IO>(y, idx, y0, y1);
     }
-  };
-
-  constexpr int W0 = kF4Compute / 32;  // first auxiliary warp
-  if (warp == W0 + 1 || warp == W0 + 2) {
-    // ---------------------------------- copy warps: C boxes / E boxes ----------------------------------
-    if (lane == 0) load_boxes(warp - (W0 + 1), warp == W0 + 1);
-    __syncwarp();
-  } else if (warp == W0 + 3) {
-    // ---------------------------------- gamma warp: lo-plane chunks ----------------------------------
-    if (lane == 0) {
-      const uint8_t* lo_plane = reinterpret_cast<const uint8_t*>(planes) + L::kPlaneB;
-      uint32_t n = 0;  // chunks requested so far; chunk n uses buffer n & 1
-      for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c, ++n) {
-          const uint32_t buf = n & 1u;
-          if (n >= 2) {  // the MMAs of chunk n - 2 (same buffer, same plane mbarrier) have completed
-            if (!mbar_wait(bar(L::kBarPlane + buf), ((n >> 1) - 1u) & 1u)) __trap();
-          }
-          const uint32_t gfull = bar(L::kBarGfull + buf);
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(gfull), "n"(L::kGlo) : "memory");
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                           smem_u32(smem + L::kOffGlo + buf * L::kGlo)),
-                       "l"(lo_plane + (size_t)c * L::kGlo), "n"(L::kGlo), "r"(gfull)
-                       : "memory");
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0 + 4) {
-    // ---------------------------------- store warp: y boxes ----------------------------------
-    if (lane == 0) {
-      uint32_t n = 0;
-      for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int row0 = (int)(tile * kTileM);
-#pragma unroll 1
-        for (int k = 0; k < NCH; ++k, ++n) {
-          const uint32_t slot = n % 3u, round = n / 3u;
-          if (!mbar_wait(bar(L::kBarY + slot), round & 1u)) __trap();
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(&y_map),
-                       "r"(k * 32), "r"(row0), "r"(smem_u32(smem + L::kOffRing + (3 + slot) * kF4Box)), "l"(kEvictFirst)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the box has been read: the slot is free
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarEempty + slot)) : "memory");
-        }
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-    __syncwarp();
-  } else if (warp == W0) {
-    // ------------------------------- MMA-issue warp -------------------------------
-    uint32_t parg[2] = {0u, 0u};
-    uint32_t n = 0;  // chunk counter = C box counter
-    int t = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t tmem_n = tmem_base + (uint32_t)(t & 1) * 256u;
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, ++n) {
-        const int pb = c & 1;
-        asm volatile("bar.sync %0, %1;" ::"r"(2 + pb), "n"(kF4Sync) : "memory");  // planes of chunk c are written
-        if (lane == 0) {
-          // every compute thread is done with this C box: hand its slot back to the copy warp
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarCempty + n % 3u)) : "memory");
-          if (!mbar_wait(bar(L::kBarGfull + pb), parg[pb])) __trap();
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t ph = smem_u32(smem + L::kOffP + pb * 2 * kF4Plane), pl = ph + kF4Plane;
-          const uint32_t g_lo = smem_u32(smem + L::kOffGlo + pb * L::kGlo);
-#pragma unroll
-          for (int s2 = 0; s2 < 2; ++s2) {
-            const uint64_t dah = umma_desc(ph + (uint32_t)(2 * s2) * kF4Kg, kF4Kg, 128);
-            const uint64_t dal = umma_desc(pl + (uint32_t)(2 * s2) * kF4Kg, kF4Kg, 128);
-            const uint64_t dbh = umma_desc(b_hi + (uint32_t)(c * 4 + 2 * s2) * (C * 16), C * 16, 128);
-            const uint64_t dbl = umma_desc(g_lo + (uint32_t)(2 * s2) * (C * 16), C * 16, 128);
-            umma_bf16(tmem_n, dah, dbh, kIdesc, (c | s2) ? 1u : 0u);
-            umma_bf16(tmem_n, dal, dbh, kIdesc, 1u);
-            umma_bf16(tmem_n, dah, dbl, kIdesc, 1u);
-          }
-          umma_commit(bar(L::kBarPlane + pb));
-        }
-        parg[pb] ^= 1u;
-        __syncwarp();
-      }
-    }
-  } else {
-  // --------------------------------- compute warps ---------------------------------
-  uint32_t parp[2] = {0u, 0u};
-  uint32_t nc = 0, ne = 0;                     // C boxes converted / E boxes finished so far
-  const int ckg = tid & 3, crow = tid >> 2;    // conversion item of a box: row crow, 8 channels
-  // 128-byte swizzle: the 16-byte chunk j of box row `row` sits at chunk j ^ (row & 7)
-  auto chunk_at = [](uint8_t* box, int row, int j) { return reinterpret_cast<float4*>(box + row * 128 + ((j ^ (row & 7)) << 4)); };
-
-  auto convert = [&](int c, bool wait_planes) {
-    const int pb = c & 1;
-    const uint32_t slot = nc % 3u, round = nc / 3u;
-    uint8_t* box = smem + L::kOffRing + slot * kF4Box;
-    if (!mbar_wait(bar(L::kBarCfull + slot), round & 1u)) __trap();
-    const float4 a = *chunk_at(box, crow, 2 * ckg), b = *chunk_at(box, crow, 2 * ckg + 1);
-    if (wait_planes) {  // the plane buffer is still being read by the MMAs of the chunk two before this one
-      if (!mbar_wait(bar(L::kBarPlane + pb), parp[pb])) __trap();
-      parp[pb] ^= 1u;
-    }
-    uint8_t* ph = smem + L::kOffP + pb * 2 * kF4Plane;
-    {
-      float v[8] = {tc_pool<FAST>(a.x, f), tc_pool<FAST>(a.y, f), tc_pool<FAST>(a.z, f), tc_pool<FAST>(a.w, f),
-                    tc_pool<FAST>(b.x, f), tc_pool<FAST>(b.y, f), tc_pool<FAST>(b.z, f), tc_pool<FAST>(b.w, f)};
-      uint4 hi, lo;
-      split8(v, &hi, &lo);
-      *reinterpret_cast<uint4*>(ph + ckg * kF4Kg + crow * 16) = hi;
-      *reinterpret_cast<uint4*>(ph + kF4Plane + ckg * kF4Kg + crow * 16) = lo;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    asm volatile("bar.arrive %0, %1;" ::"r"(2 + pb), "n"(kF4Sync) : "memory");  // (also releases the box, see issue warp)
-    ++nc;
-  };
-
-  // y = x / (beta + n) for box k (channels 32 k ..) of the tile whose accumulator starts at column `acc`:
-  // thread (r, h) owns pixel row r and the 8 channels 32 k + 8 h ..
-  auto finish_box = [&](int k, uint32_t acc) {
-    const uint32_t slot = ne % 3u, round = ne / 3u;
-    uint8_t* box = smem + L::kOffRing + (3 + slot) * kF4Box;
-    uint32_t nacc[8];
-    tmem_load<8>(tmem_base + acc + lane_sel + (uint32_t)(k * 32 + h * 8), nacc);
-    if (!mbar_wait(bar(L::kBarEfull + slot), round & 1u)) __trap();
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    const float* bs = beta_s + k * 32 + h * 8;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      float4* px = chunk_at(box, r, 2 * h + j);
-      const float4 xv = *px;
-      const float4 bv = *reinterpret_cast<const float4*>(bs + 4 * j);  // same address in every lane: broadcast
-      float4 o;
-      o.x = tc_out<FAST>(xv.x, bv.x + __uint_as_float(nacc[4 * j]), f);
-      o.y = tc_out<FAST>(xv.y, bv.y + __uint_as_float(nacc[4 * j + 1]), f);
-      o.z = tc_out<FAST>(xv.z, bv.z + __uint_as_float(nacc[4 * j + 2]), f);
-      o.w = tc_out<FAST>(xv.w, bv.w + __uint_as_float(nacc[4 * j + 3]), f);
-      *px = o;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // y box -> TMA store
-    __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarY + slot)) : "memory");
-    ++ne;
-  };
-
-  int t = 0;
-  for (long long tile = blockIdx.x;; tile += gridDim.x, ++t) {
-    const bool has_cur = tile < n_tiles;   // tile t: converted now, accumulator (t & 1)
-    const bool has_prev = t > 0;           // tile t - 1: finished now, accumulator ((t - 1) & 1)
-    if (!has_cur && !has_prev) break;
-    const uint32_t acc_prev = (uint32_t)((t - 1) & 1) * 256u;
-    if (!has_cur) {  // drain: the last two commits cover every MMA of the last tile
-#pragma unroll
-      for (int pb = 0; pb < 2; ++pb) {
-        if (!mbar_wait(bar(L::kBarPlane + pb), parp[pb])) __trap();
-        parp[pb] ^= 1u;
-      }
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // Chunks 0 and 1 of this tile first: their plane-buffer waits are the commits of the previous tile's last two
-    // chunks, i.e. after them every MMA of the previous tile has completed.  Then box c - 2 of the previous tile is
-    // finished BEFORE chunk c is converted, which gives the tensor pipe (the slower side) a box worth of slack.
-    if (has_cur) {
-      convert(0, t > 0);
-      convert(1, t > 0);
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c = 2; c < NCH; ++c) {
-      if (has_prev) finish_box(c - 2, acc_prev);
-      if (has_cur) convert(c, true);
-    }
-    if (has_prev) {
-      finish_box(NCH - 2, acc_prev);
-      finish_box(NCH - 1, acc_prev);
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // accumulator reads precede its next MMAs
-    if (!has_cur) break;
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
   }
 }
 
-// 2-D tensor map of a row-major fp32 [rows, cols] array with [box_rows x box_cols] boxes (zero fill; optionally the
-// 128-byte swizzle: 16-byte chunk j of box row i lands at chunk j ^ (i & 7); needs 128-byte box rows).
-// cuTensorMapEncodeTiled is a driver entry point; it is looked up through the runtime so that the library keeps
-// linking against libcudart only.
-int make_tensor_map_2d(CUtensorMap* map, const float* base, long long rows, int cols, int box_rows, int box_cols,
-                       bool swizzle128 = false) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-        st != cudaDriverEntryPointSuccess)
-      fn = nullptr;
-    (void)cudaGetLastError();
-    return reinterpret_cast<EncodeFn>(fn);
-  }();
-  if (!encode) return fail(TFCB_CUDA_ERROR, "cuTensorMapEncodeTiled is not available from this driver");
-  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(float)};
-  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1u, 1u};
-  const CUresult rc = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (rc != CUDA_SUCCESS) return fail(TFCB_CUDA_ERROR, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
-  return TFCB_OK;
-}
-
-// 3-D view of a row-major fp32 [rows, cols] array as (32 channels, rows, cols / 32 chunks) with boxes of
-// [chunks_per_box][box_rows][32 channels], 128-byte swizzle: ONE copy instruction moves several of the kernels'
-// [128 rows x 32 channels] boxes, which land back to back in shared memory exactly as separate 2-D boxes would.
-// (The SM's async-copy engine retires ~2.5 copy instructions per microsecond whatever their size -- 0.39 us per 16 KB
-// box, tools/tma_probe.py -- so the number of instructions per tile, not the bytes, bounded the box-fed kernels.)
-int make_tensor_map_3d(CUtensorMap* map, const float* base, long long rows, int cols, int box_rows, int chunks_per_box) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-        st != cudaDriverEntryPointSuccess)
-      fn = nullptr;
-    (void)cudaGetLastError();
-    return reinterpret_cast<EncodeFn>(fn);
-  }();
-  if (!encode) return fail(TFCB_CUDA_ERROR, "cuTensorMapEncodeTiled is not available from this driver");
-  const cuuint64_t dims[3] = {32u, (cuuint64_t)rows, (cuuint64_t)(cols / 32)};
-  const cuuint64_t strides[2] = {(cuuint64_t)cols * sizeof(float), 32u * sizeof(float)};  // row stride, chunk stride
-  const cuuint32_t box[3] = {32u, (cuuint32_t)box_rows, (cuuint32_t)chunks_per_box};
-  const cuuint32_t estr[3] = {1u, 1u, 1u};
-  const CUresult rc = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (rc != CUDA_SUCCESS) return fail(TFCB_CUDA_ERROR, "cuTensorMapEncodeTiled (3-D) failed (%d)", (int)rc);
-  return TFCB_OK;
-}
-
-template <bool FAST>
-int launch_tc_fwd4(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, TcFlags f,
-                   cudaStream_t s) {
-  constexpr int C = 192;
-  using L = Fwd4Smem<C>;
-  CUtensorMap x_map, y_map;
-  TFCB_TRY(make_tensor_map_2d(&x_map, x, n_pix, C, kTileM, 32, true));
-  TFCB_TRY(make_tensor_map_2d(&y_map, y, n_pix, C, kTileM, 32, true));
-  __nv_bfloat16* planes = nullptr;
-  TFCB_TRY(dev_alloc((void**)&planes, (size_t)2 * C * C * sizeof(__nv_bfloat16), s));
-  gdn_tc_prep_kernel<<<((C / 8) * C + 255) / 256, 256, 0, s>>>(gamma, C, planes);
-  TFCB_LAUNCHED();
-  cudaError_t e = cudaFuncSetAttribute(gdn_tc_fwd4_kernel<C, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    dev_free(planes, s);
-    return fail(TFCB_CUDA_ERROR, "cannot reserve %d bytes of shared memory: %s", L::kBytes, cudaGetErrorString(e));
-  }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>(n_tiles, sms);
-  gdn_tc_fwd4_kernel<C, FAST><<<grid, kF4Threads, L::kBytes, s>>>(x_map, y_map, x, planes, beta, n_pix, f);
-  TFCB_LAUNCHED();
-  e = cudaGetLastError();
-  dev_free(planes, s);
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core kernel launch failed: %s", cudaGetErrorString(e));
-  return TFCB_OK;
-}
-
-// =============================================================================================
-// Backward (C = 128): one fused kernel per launch instead of three fp32 passes.
-//
-//   n  = beta + p . gamma                 MMA1   A = p planes (K-major),        B = gamma planes (K-major)
-//   q  = dL/dn (elementwise, from g, x, n)
-//   dp = q . gamma^T                      MMA2   A = q planes (K-major),        B = gamma planes (MN-major view)
-//   dx = g / m + dpool/du * dp            (IGDN: g * m + ...)
-//   dgamma[j, i] += sum_pix p[pix, j] q[pix, i]
-//                                         MMA3   A = p planes (MN-major view),  B = q planes (MN-major view)
-//   dbeta[i] += sum_pix q[pix, i]         warp transpose-reduce of the q registers
-//
-// The MN-major views reuse the very same shared-memory planes: a K-major plane [k / 8][row][8] read with the
-// "transposed" descriptor (instruction-descriptor bits 15 / 16) is the operand with the roles of row and k
-// swapped (core matrix = 8 k-rows of 16 bytes, LBO = 128 B between k groups, SBO = plane row-group stride).
-// TMEM: columns [0, C) n, [C, 2C) dp, [2C, 3C) this CTA's dgamma partial (accumulates over all its tiles).
-// HBM traffic per element: x and dy once (their re-reads in the two epilogues are L2 hits), dx once.
-// =============================================================================================
-constexpr int kBwdThreads = 288;  // 8 compute warps + 1 MMA-issue warp
-constexpr int kKg = kTileM * 16 + 16;  // byte stride between 8-channel groups of an operand plane: one 16-byte row
-                                       // of padding makes the coalesced (row, group) stores bank-conflict free;
-                                       // the descriptors take it as LBO (K-major view) or SBO (MN-major view)
-
-template <int C>
-struct BwdSmem {
-  static constexpr int kPlaneB = C * C * 2;            // gamma hi / lo
-  static constexpr int kPlaneP = (C / 8) * kKg;        // p hi / lo (whole K)
-  static constexpr int kPlaneQ = 4 * kKg;              // q hi / lo, one 32-channel chunk
-  static constexpr int kStage = kTileM * kStLd * 4;    // fp32 [128][36]
-  static constexpr int kOffBh = 0;
-  static constexpr int kOffBl = kOffBh + kPlaneB;
-  static constexpr int kOffPh = kOffBl + kPlaneB;
-  static constexpr int kOffPl = kOffPh + kPlaneP;
-  static constexpr int kOffQ = kOffPl + kPlaneP;       // [2 buffers][hi, lo]
-  static constexpr int kOffStage = kOffQ + 4 * kPlaneQ;  // [2]: n, dp
-  static constexpr int kOffBeta = kOffStage + 2 * kStage;
-  static constexpr int kOffDbeta = kOffBeta + C * 4;
-  static constexpr int kOffBar = kOffDbeta + C * 4;
-  static constexpr int kBytes = kOffBar + 64;
-};
-
-template <bool FAST>
-__device__ __forceinline__ float tc_dl_dn(float g, float x, float n, const TcFlags& f) {
-  const float u = (!FAST && f.rectify) ? fmaxf(x, 0.f) : x;
-  const float r = rcp_approx(n);
-  if (FAST || f.eps_mode == 1) return f.inverse ? g * u : -g * u * r * r;
-  const float rs = rsqrtf(n);
-  return f.inverse ? 0.5f * g * u * rs : -0.5f * g * u * r * rs;
-}
-
-template <bool FAST>
-__device__ __forceinline__ float tc_dx(float g, float x, float n, float dp, const TcFlags& f) {
-  const float u = (!FAST && f.rectify) ? fmaxf(x, 0.f) : x;
-  float direct;
-  if (FAST || f.eps_mode == 1) direct = f.inverse ? g * n : g * rcp_approx(n);
-  else direct = f.inverse ? g * sqrtf(n) : g * rsqrtf(n);
-  float dpool;
-  if (FAST || f.alpha_mode == 1) dpool = (!FAST && f.rectify) ? 1.f : ((u > 0.f) ? 1.f : ((u < 0.f) ? -1.f : 0.f));
-  else dpool = 2.f * u;
-  float d = direct + dpool * dp;
-  if (!FAST && f.rectify && !(x > 0.f)) d = 0.f;
-  return d;
-}
-
-// Warp roles: 8 compute warps + 1 MMA-issue warp.  Compute threads never block on a CTA-wide barrier to hand
-// operands over: they ARRIVE on a named barrier once their planes are written and fenced; the issue warp waits
-// on it, issues the MMAs and commits to an mbarrier.  TMEM side, compute thread (r = tid % 128, h = tid / 128)
-// owns pixel row r (= TMEM lane) and half of the columns being moved; memory side, item (row, kg) = 8
-// consecutive channels of one pixel, items enumerated row-major so that a warp reads whole 128-byte lines.
-constexpr int kBwdCompute = 256;
-constexpr int kBwdStLd2 = 68;    // staging row of the 64-column n passes (P2)
-constexpr int kBwdStLd3 = 132;   // staging row of the full n / dp tiles (P3; aliases the dead operand planes)
-
+// Backward, part 1: per 64-pixel tile
+//   n = beta + p . gamma  ->  q = dL/dn (stored for part 2), dx = direct term (stored)
+//   dp = q . gamma^T      ->  dx += dpool/dx * dp (read back from the same thread's stores, L2 resident).
 template <int C, bool FAST>
-__global__ void __launch_bounds__(kBwdThreads, 1)
-gdn_tc_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, const __nv_bfloat16* __restrict__ planes,
-                  const float* __restrict__ beta, float* __restrict__ dx, float* __restrict__ part_g,
-                  float* __restrict__ part_b, long long n_pix, TcFlags f) {
-  using L = BwdSmem<C>;
-  static_assert(C == 128, "TMEM holds n, dp and the dgamma partial only for C = 128");
-  static_assert(2 * L::kStage >= kTileM * kBwdStLd2 * 4, "P2 staging");
-  static_assert(2 * L::kPlaneP + 4 * L::kPlaneQ + 2 * L::kStage >= 2 * kTileM * kBwdStLd3 * 4, "P3 staging");
-  constexpr int NCH = C / 32;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* beta_s = reinterpret_cast<float*>(smem + L::kOffBeta);
-  float* dbeta_s = reinterpret_cast<float*>(smem + L::kOffDbeta);
-  float* stage2 = reinterpret_cast<float*>(smem + L::kOffStage);                 // [128][68]
-  float* stage3n = reinterpret_cast<float*>(smem + L::kOffPh);                   // [128][132], planes are dead
-  float* stage3d = stage3n + kTileM * kBwdStLd3;
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);  // [0,1] MMA1 halves, [2,3] q buffers
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + 40);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 1, gwarp = warp & 3;
-  constexpr uint32_t kIdesc1 = umma_idesc(kTileM, 64);                         // MMA1, one 64-column half of n
-  constexpr uint32_t kIdesc2 = umma_idesc(kTileM, C) | (1u << 16);             // B = gamma^T (MN-major view)
-  constexpr uint32_t kIdesc3 = umma_idesc(C, 32) | (1u << 15) | (1u << 16);    // A = p^T, B = q chunk (both views)
-
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(planes);
-    uint4* dst = reinterpret_cast<uint4*>(smem + L::kOffBh);
-    for (int i = tid; i < 2 * L::kPlaneB / 16; i += kBwdThreads) dst[i] = src[i];
-    for (int i = tid; i < C; i += kBwdThreads) {
-      beta_s[i] = beta[i];
-      dbeta_s[i] = 0.f;
-    }
-  }
-  if (tid == 0) {
-    for (int i = 0; i < 4; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbars + i)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_n = *tmem_slot, tmem_dp = tmem_n + C, tmem_dg = tmem_n + 2 * C;
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const uint32_t b_hi = smem_u32(smem + L::kOffBh), b_lo = smem_u32(smem + L::kOffBl);
-  const uint32_t p_hi = smem_u32(smem + L::kOffPh), p_lo = smem_u32(smem + L::kOffPl);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  int t_idx = 0;  // this CTA's tile counter (both roles count alike)
-
-  if (warp == kBwdCompute / 32) {
-    // ------------------------------- MMA-issue warp -------------------------------
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t_idx) {
-      // next tile of this CTA -> L2 (one bulk prefetch per array: the tile is contiguous)
-      if (lane == 1) {
-        const long long pn = (tile + gridDim.x) * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - pn);
-        if (rows > 0) {
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(x + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(dy + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-        }
-      }
-      // MMA1: n = p . gamma, the two 64-column halves one after the other so that P2 can start on the first
-      asm volatile("bar.sync 2, %0;" ::"n"(kBwdThreads) : "memory");
-      if (lane == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-#pragma unroll
-          for (int s = 0; s < C / 16; ++s) {
-            const uint64_t dah = umma_desc(p_hi + (uint32_t)(2 * s) * kKg, kKg, 128);
-            const uint64_t dal = umma_desc(p_lo + (uint32_t)(2 * s) * kKg, kKg, 128);
-            const uint32_t boff = (uint32_t)(2 * s) * (C * 16) + (uint32_t)(half * 64) * 16u;
-            const uint64_t dbh = umma_desc(b_hi + boff, C * 16, 128);
-            const uint64_t dbl = umma_desc(b_lo + boff, C * 16, 128);
-            umma_bf16(tmem_n + (uint32_t)(half * 64), dah, dbh, kIdesc1, s ? 1u : 0u);
-            umma_bf16(tmem_n + (uint32_t)(half * 64), dal, dbh, kIdesc1, 1u);
-            umma_bf16(tmem_n + (uint32_t)(half * 64), dah, dbl, kIdesc1, 1u);
-          }
-          umma_commit(smem_u32(mbars + half));
-        }
-      }
-      __syncwarp();
-#pragma unroll
-      for (int c = 0; c < NCH; ++c) {
-        const int b = c & 1;
-        asm volatile("bar.sync %0, %1;" ::"r"(3 + b), "n"(kBwdThreads) : "memory");
-        if (lane == 0) {
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t q_hi = smem_u32(smem + L::kOffQ + b * 2 * L::kPlaneQ), q_lo = q_hi + L::kPlaneQ;
-          // MMA2: dp[pix, j] += sum_{i in chunk} q[pix, i] gamma[j, i]   (K = i: 2 steps of 16)
-#pragma unroll
-          for (int s = 0; s < 2; ++s) {
-            const uint64_t dah = umma_desc(q_hi + (uint32_t)(2 * s) * kKg, kKg, 128);
-            const uint64_t dal = umma_desc(q_lo + (uint32_t)(2 * s) * kKg, kKg, 128);
-            // gamma plane viewed with n = j, k = i: k rows are 16 B apart, k groups 128 B, n groups C * 16 B
-            const uint32_t koff = (uint32_t)(c * 32 + s * 16) * 16u;
-            const uint64_t dbh = umma_desc(b_hi + koff, 128, C * 16);
-            const uint64_t dbl = umma_desc(b_lo + koff, 128, C * 16);
-            umma_bf16(tmem_dp, dah, dbh, kIdesc2, (c | s) ? 1u : 0u);
-            umma_bf16(tmem_dp, dal, dbh, kIdesc2, 1u);
-            umma_bf16(tmem_dp, dah, dbl, kIdesc2, 1u);
-          }
-          // MMA3: dgamma[j, i in chunk] += sum_pix p[pix, j] q[pix, i]   (K = pix: 8 steps of 16)
-#pragma unroll
-          for (int s = 0; s < kTileM / 16; ++s) {
-            const uint32_t koff = (uint32_t)(s * 16) * 16u;
-            const uint64_t dah = umma_desc(p_hi + koff, 128, kKg);
-            const uint64_t dal = umma_desc(p_lo + koff, 128, kKg);
-            const uint64_t dbh = umma_desc(q_hi + koff, 128, kKg);
-            const uint64_t dbl = umma_desc(q_lo + koff, 128, kKg);
-            const uint32_t acc_on = ((t_idx % kDgFlush) == 0 && s == 0) ? 0u : 1u;  // restarted after every flush
-            umma_bf16(tmem_dg + (uint32_t)(c * 32), dah, dbh, kIdesc3, acc_on);
-            umma_bf16(tmem_dg + (uint32_t)(c * 32), dal, dbh, kIdesc3, 1u);
-            umma_bf16(tmem_dg + (uint32_t)(c * 32), dah, dbl, kIdesc3, 1u);
-          }
-          umma_commit(smem_u32(mbars + 2 + b));
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-  // --------------------------------- compute warps ---------------------------------
-  uint32_t parn[2] = {0u, 0u}, parq[2] = {0u, 0u};
-  float dbeta_acc[NCH][8];  // channels c * 32 + (tid % 4) * 8 + e, summed over this thread's rows
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) dbeta_acc[c][e] = 0.f;
-  const int ckg = tid & 3;         // 8-channel group inside a 32-channel chunk
-  const int crow = tid >> 2;       // rows crow and crow + 64
-  auto compute_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kBwdCompute) : "memory"); };
-  bool flushed = false;  // the global partial holds earlier flushes
-  // adds the TMEM dgamma accumulator (lane r = input channel j, this thread's 64 columns) into the CTA's partial
-  auto flush_dgamma = [&]() {
-    float* pg = part_g + (long long)blockIdx.x * C * C + (long long)r * C + h * 64;
-#pragma unroll
-    for (int cb = 0; cb < 4; ++cb) {
-      uint32_t a[16];
-      tmem_load<16>(tmem_dg + lane_sel + (uint32_t)(h * 64 + cb * 16), a);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      accum_store16(pg + cb * 16, a, flushed);
-    }
-    flushed = true;
-  };
-
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t_idx) {
-    const long long p0 = tile * kTileM;
-    // ---- P1: p = pool(x) -> hi / lo planes [j / 8][row][8]; item = (row, kg), 16 groups per row ----
-    {
-      constexpr int ITEMS = kTileM * (C / 8) / kBwdCompute;  // 8
-      float4 xv[ITEMS][2];
-#pragma unroll
-      for (int it = 0; it < ITEMS; ++it) {
-        const int id = it * kBwdCompute + tid;
-        const int row = id / (C / 8), kg = id % (C / 8);
-        const bool live = p0 + row < n_pix;
-        const float4* src = reinterpret_cast<const float4*>(x + (p0 + row) * C + kg * 8);
-        xv[it][0] = live ? __ldg(src) : make_float4(0.f, 0.f, 0.f, 0.f);
-        xv[it][1] = live ? __ldg(src + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int it = 0; it < ITEMS; ++it) {
-        const int id = it * kBwdCompute + tid;
-        const int row = id / (C / 8), kg = id % (C / 8);
-        const float4 a = xv[it][0], b = xv[it][1];
-        float v[8] = {tc_pool<FAST>(a.x, f), tc_pool<FAST>(a.y, f), tc_pool<FAST>(a.z, f), tc_pool<FAST>(a.w, f),
-                      tc_pool<FAST>(b.x, f), tc_pool<FAST>(b.y, f), tc_pool<FAST>(b.z, f), tc_pool<FAST>(b.w, f)};
-        uint4 hi, lo;
-        split8(v, &hi, &lo);
-        *reinterpret_cast<uint4*>(smem + L::kOffPh + kg * kKg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(smem + L::kOffPl + kg * kKg + row * 16) = lo;
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    asm volatile("bar.arrive 2, %0;" ::"n"(kBwdThreads) : "memory");
-    // x and dy of a chunk for this thread's two items (coalesced; L2 hits after the prefetch / P1).  Two register
-    // sets: the loads of the next chunk are issued a whole chunk ahead of their use.
-    float4 xq[2][2][2], gq[2][2][2];  // [set][item][half]
-    auto load_xg = [&](int set, int c) {
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const bool live = p0 + row < n_pix;
-        const long long off = (p0 + row) * C + c * 32 + ckg * 8;
-        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-        xq[set][it][0] = live ? __ldg(reinterpret_cast<const float4*>(x + off)) : z;
-        xq[set][it][1] = live ? __ldg(reinterpret_cast<const float4*>(x + off) + 1) : z;
-        gq[set][it][0] = live ? __ldg(reinterpret_cast<const float4*>(dy + off)) : z;
-        gq[set][it][1] = live ? __ldg(reinterpret_cast<const float4*>(dy + off) + 1) : z;
-      }
-    };
-    // ---- P2: q = dL/dn -> q planes (32-channel chunks); n is staged 64 columns at a time ----
-    load_xg(0, 0);
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int b = c & 1;
-      load_xg(b ^ 1, (c + 1) % NCH);  // next chunk; after the last one: chunk 0 again, for the dx pass
-      if ((c & 1) == 0) {
-        const int half = c >> 1;
-        if (c) compute_sync();  // everyone is done reading the previous 64 staged columns
-        if (!mbar_wait(smem_u32(mbars + half), parn[half])) __trap();
-        parn[half] ^= 1u;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t acc[32];
-        tmem_load<32>(tmem_n + lane_sel + (uint32_t)(half * 64 + h * 32), acc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float* dst = stage2 + r * kBwdStLd2 + h * 32;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(__uint_as_float(acc[4 * i]), __uint_as_float(acc[4 * i + 1]),
-                                                                 __uint_as_float(acc[4 * i + 2]), __uint_as_float(acc[4 * i + 3]));
-        compute_sync();
-      }
-      // the q buffer was read by the MMAs of chunk c - 2 (chunks 2, 3 of the previous tile: waited for before its dx pass)
-      if (c >= 2) {
-        if (!mbar_wait(smem_u32(mbars + 2 + b), parq[b])) __trap();
-        parq[b] ^= 1u;
-      }
-      uint8_t* qh = smem + L::kOffQ + b * 2 * L::kPlaneQ;
-      uint8_t* ql = qh + L::kPlaneQ;
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8);
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8 + 4);
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const float* ns = stage2 + row * kBwdStLd2 + (c & 1) * 32 + ckg * 8;
-        const float4 n0 = *reinterpret_cast<const float4*>(ns);
-        const float4 n1 = *reinterpret_cast<const float4*>(ns + 4);
-        const float4 x0 = xq[b][it][0], x1 = xq[b][it][1], g0 = gq[b][it][0], g1 = gq[b][it][1];
-        float q[8];
-        q[0] = tc_dl_dn<FAST>(g0.x, x0.x, bv0.x + n0.x, f);
-        q[1] = tc_dl_dn<FAST>(g0.y, x0.y, bv0.y + n0.y, f);
-        q[2] = tc_dl_dn<FAST>(g0.z, x0.z, bv0.z + n0.z, f);
-        q[3] = tc_dl_dn<FAST>(g0.w, x0.w, bv0.w + n0.w, f);
-        q[4] = tc_dl_dn<FAST>(g1.x, x1.x, bv1.x + n1.x, f);
-        q[5] = tc_dl_dn<FAST>(g1.y, x1.y, bv1.y + n1.y, f);
-        q[6] = tc_dl_dn<FAST>(g1.z, x1.z, bv1.z + n1.z, f);
-        q[7] = tc_dl_dn<FAST>(g1.w, x1.w, bv1.w + n1.w, f);
-        uint4 hi, lo;
-        split8(q, &hi, &lo);
-        *reinterpret_cast<uint4*>(qh + ckg * kKg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(ql + ckg * kKg + row * 16) = lo;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dbeta_acc[c][e] += q[e];
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(3 + b), "n"(kBwdThreads) : "memory");
-    }
-    // ---- P3: dx = g / m + dpool/du * dp  (chunk 0 is already in register set 0) ----
-#pragma unroll
-    for (int b = 0; b < 2; ++b) {  // commits of chunks 2 and 3: all MMAs of this tile are done, the planes are dead
-      if (!mbar_wait(smem_u32(mbars + 2 + b), parq[b])) __trap();
-      parq[b] ^= 1u;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // whole n and dp tiles -> staging (over the dead operand planes), thread (r, h) moves 64 columns of each
-#pragma unroll
-    for (int part = 0; part < 4; ++part) {
-      const uint32_t col = (uint32_t)(h * 64 + (part & 1) * 32);
-      uint32_t acc[32];
-      tmem_load<32>(((part >> 1) ? tmem_dp : tmem_n) + lane_sel + col, acc);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float* dst = ((part >> 1) ? stage3d : stage3n) + r * kBwdStLd3 + col;
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        *reinterpret_cast<float4*>(dst + 4 * i) = make_float4(__uint_as_float(acc[4 * i]), __uint_as_float(acc[4 * i + 1]),
-                                                               __uint_as_float(acc[4 * i + 2]), __uint_as_float(acc[4 * i + 3]));
-    }
-    compute_sync();
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int b = c & 1;
-      if (c + 1 < NCH) load_xg(b ^ 1, c + 1);
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8);
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8 + 4);
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const float* ns = stage3n + row * kBwdStLd3 + c * 32 + ckg * 8;
-        const float* ds = stage3d + row * kBwdStLd3 + c * 32 + ckg * 8;
-        const float4 n0 = *reinterpret_cast<const float4*>(ns), n1 = *reinterpret_cast<const float4*>(ns + 4);
-        const float4 d0 = *reinterpret_cast<const float4*>(ds), d1 = *reinterpret_cast<const float4*>(ds + 4);
-        const float4 x0 = xq[b][it][0], x1 = xq[b][it][1], g0 = gq[b][it][0], g1 = gq[b][it][1];
-        float4 o0, o1;
-        o0.x = tc_dx<FAST>(g0.x, x0.x, bv0.x + n0.x, d0.x, f);
-        o0.y = tc_dx<FAST>(g0.y, x0.y, bv0.y + n0.y, d0.y, f);
-        o0.z = tc_dx<FAST>(g0.z, x0.z, bv0.z + n0.z, d0.z, f);
-        o0.w = tc_dx<FAST>(g0.w, x0.w, bv0.w + n0.w, d0.w, f);
-        o1.x = tc_dx<FAST>(g1.x, x1.x, bv1.x + n1.x, d1.x, f);
-        o1.y = tc_dx<FAST>(g1.y, x1.y, bv1.y + n1.y, d1.y, f);
-        o1.z = tc_dx<FAST>(g1.z, x1.z, bv1.z + n1.z, d1.z, f);
-        o1.w = tc_dx<FAST>(g1.w, x1.w, bv1.w + n1.w, d1.w, f);
-        if (p0 + row < n_pix) {
-          float4* dst = reinterpret_cast<float4*>(dx + (p0 + row) * C + c * 32 + ckg * 8);
-          __stcs(dst, o0);  // streaming stores: keep x / dy (re-read from L2) resident instead of the outputs
-          __stcs(dst + 1, o1);
-        }
-      }
-    }
-    // every MMA of this tile has completed (the two waits above): flush the dgamma accumulator when due
-    if ((t_idx % kDgFlush) == kDgFlush - 1) flush_dgamma();
-    // the staging (= operand planes) and the n / dp columns are rewritten by the next tile
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    compute_sync();
-  }
-
-  // ---- this CTA's partial sums ----
-  if (t_idx > 0) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if ((t_idx % kDgFlush) != 0) flush_dgamma();  // tiles since the last flush
-    // dbeta: lanes with the same tid % 4 hold the same channels
-#pragma unroll
-    for (int c = 0; c < NCH; ++c)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        float v = dbeta_acc[c][e];
-        v += __shfl_xor_sync(0xFFFFFFFFu, v, 4);
-        v += __shfl_xor_sync(0xFFFFFFFFu, v, 8);
-        v += __shfl_xor_sync(0xFFFFFFFFu, v, 16);
-        if (lane < 4) atomicAdd(dbeta_s + c * 32 + lane * 8 + e, v);
-      }
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < C) part_b[(long long)blockIdx.x * C + tid] = dbeta_s[tid];
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
-  }
-}
-
-// =============================================================================================
-// Backward for C = 192: two kernels.  n, dp and a dgamma accumulator would need 3 x 192 TMEM columns and the
-// gamma planes plus a full-K p plane 243 KB of shared memory, so the dgamma contraction moves to its own
-// kernel and q = dL/dn travels through global memory (fp32, the caller's workspace):
-//   K1  gdn_tc_bwd_dx_kernel     : n = beta + p.gamma (p converted 16 channels at a time) -> q (stored) ->
-//                                  dp = q.gamma^T -> dx.   TMEM: n | dp (2 x 192 columns).
-//   K2  gdn_tc_bwd_dgamma_kernel : dgamma += p^T q over all tiles of the CTA, dbeta = column sums of q.  No gamma:
-//                                  the full-K p and q planes fill the shared memory.  M = 192 does not exist, so
-//                                  rows j in [0,128) and [64,192) are two overlapping M = 128 blocks.
-// HBM traffic: K1 x, dy in; dx, q out.  K2 x, q in.  (6 passes against the fused kernel's 3.)
-// =============================================================================================
-template <int C>
-struct Bwd2Smem {
-  static constexpr int kPlaneB = C * C * 2;          // gamma hi / lo
-  static constexpr int kPlaneP = 2 * kKg;            // p hi or lo, one 16-channel chunk
-  static constexpr int kPlaneQ = 4 * kKg;            // q hi or lo, one 32-channel chunk
-  static constexpr int kStage = kTileM * kStLd * 4;  // fp32 [128][36]
-  static constexpr int kOffBh = 0;
-  static constexpr int kOffBl = kOffBh + kPlaneB;
-  static constexpr int kOffP = kOffBl + kPlaneB;     // [2 buffers][hi, lo]
-  static constexpr int kOffQ = kOffP + 4 * kPlaneP;  // [2 buffers][hi, lo]; the dx pass stages dp here
-  static constexpr int kOffStage = kOffQ + 4 * kPlaneQ;
-  static constexpr int kOffBeta = kOffStage + kStage;
-  static constexpr int kOffBar = kOffBeta + C * 4;
-  static constexpr int kBytes = kOffBar + 64;
-  static_assert(4 * kPlaneQ >= kStage, "dp staging aliases the q planes");
-  static_assert(kBytes <= 232448, "shared memory budget");
-};
-
-template <int C, bool FAST>
-__global__ void __launch_bounds__(kBwdThreads, 1)
-gdn_tc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ dy, const __nv_bfloat16* __restrict__ planes,
-                     const float* __restrict__ beta, float* __restrict__ dx, float* __restrict__ q_out, long long n_pix,
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
                      TcFlags f) {
-  using L = Bwd2Smem<C>;
-  constexpr int NCH = C / 32;   // q / dx chunks
-  constexpr int NK = C / 16;    // p chunks (one MMA K step each)
-  static_assert(2 * C <= 512 && NK % 2 == 0 && NCH % 2 == 0, "layout");
+  using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* beta_s = reinterpret_cast<float*>(smem + L::kOffBeta);
-  float* stage_n = reinterpret_cast<float*>(smem + L::kOffStage);
-  float* stage_d = reinterpret_cast<float*>(smem + L::kOffQ);
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);  // [0,1] p buffers, [2,3] q buffers
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + 40);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 1, gwarp = warp & 3;
-  constexpr uint32_t kIdesc1 = umma_idesc(kTileM, C);
-  constexpr uint32_t kIdesc2 = umma_idesc(kTileM, C) | (1u << 16);  // B = gamma^T (MN-major view)
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(planes);
-    uint4* dst = reinterpret_cast<uint4*>(smem + L::kOffBh);
-    for (int i = tid; i < 2 * L::kPlaneB / 16; i += kBwdThreads) dst[i] = src[i];
-    for (int i = tid; i < C; i += kBwdThreads) beta_s[i] = beta[i];
-  }
-  if (tid == 0) {
-    for (int i = 0; i < 4; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbars + i)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_n = *tmem_slot, tmem_dp = tmem_n + C;
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const uint32_t b_hi = smem_u32(smem + L::kOffBh), b_lo = smem_u32(smem + L::kOffBl);
+  fill_planes<C>(gamma, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * C * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-
-  if (warp == kBwdCompute / 32) {
-    // ------------------------------- MMA-issue warp -------------------------------
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      if (lane == 1) {
-        const long long pn = (tile + gridDim.x) * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - pn);
-        if (rows > 0) {
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(x + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(dy + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-        }
+  for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    uint32_t ah[C / 16][4], al[C / 16][4];
+    pool_frags<C, FAST, 0>(x, r0, r1, ok0, ok1, t, f, ah, al);
+    float acc[C / 64][32];
+    gemm3<C, 0>(acc, ah, al, bh, bl);
+    TFCB_FOR_ACC_PAIRS(C) {
+      float* a = &acc[n][4 * jj + 2 * h];
+      if (!(h ? ok1 : ok0)) {
+        a[0] = a[1] = 0.f;
+        continue;
       }
-#pragma unroll 1
-      for (int c = 0; c < NK; ++c) {  // MMA1: one K step per 16-channel p chunk
-        const int pb = c & 1;
-        asm volatile("bar.sync %0, %1;" ::"r"(2 + pb), "n"(kBwdThreads) : "memory");
-        if (lane == 0) {
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t ph = smem_u32(smem + L::kOffP + pb * 2 * L::kPlaneP), pl = ph + L::kPlaneP;
-          const uint64_t dah = umma_desc(ph, kKg, 128), dal = umma_desc(pl, kKg, 128);
-          const uint64_t dbh = umma_desc(b_hi + (uint32_t)(2 * c) * (C * 16), C * 16, 128);
-          const uint64_t dbl = umma_desc(b_lo + (uint32_t)(2 * c) * (C * 16), C * 16, 128);
-          umma_bf16(tmem_n, dah, dbh, kIdesc1, c ? 1u : 0u);
-          umma_bf16(tmem_n, dal, dbh, kIdesc1, 1u);
-          umma_bf16(tmem_n, dah, dbl, kIdesc1, 1u);
-          umma_commit(smem_u32(mbars + pb));
-        }
-        __syncwarp();
-      }
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c) {  // MMA2: dp += q chunk . gamma^T
-        const int b = c & 1;
-        asm volatile("bar.sync %0, %1;" ::"r"(4 + b), "n"(kBwdThreads) : "memory");
-        if (lane == 0) {
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t q_hi = smem_u32(smem + L::kOffQ + b * 2 * L::kPlaneQ), q_lo = q_hi + L::kPlaneQ;
-#pragma unroll
-          for (int s2 = 0; s2 < 2; ++s2) {
-            const uint64_t dah = umma_desc(q_hi + (uint32_t)(2 * s2) * kKg, kKg, 128);
-            const uint64_t dal = umma_desc(q_lo + (uint32_t)(2 * s2) * kKg, kKg, 128);
-            const uint32_t koff = (uint32_t)(c * 32 + s2 * 16) * 16u;
-            const uint64_t dbh = umma_desc(b_hi + koff, 128, C * 16);
-            const uint64_t dbl = umma_desc(b_lo + koff, 128, C * 16);
-            umma_bf16(tmem_dp, dah, dbh, kIdesc2, (c | s2) ? 1u : 0u);
-            umma_bf16(tmem_dp, dal, dbh, kIdesc2, 1u);
-            umma_bf16(tmem_dp, dah, dbl, kIdesc2, 1u);
-          }
-          umma_commit(smem_u32(mbars + 2 + b));
-        }
-        __syncwarp();
-      }
+      const int col = 64 * n + 8 * jj + 2 * t;
+      const long long idx = (h ? r1 : r0) * C + col;
+      const float2 xv = __ldg(reinterpret_cast<const float2*>(x + idx));
+      const float2 gv = __ldg(reinterpret_cast<const float2*>(dy + idx));
+      const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
+      float2 q, d;
+      tc_bwd_point<FAST>(xv.x, gv.x, b.x + a[0], f, &q.x, &d.x);
+      tc_bwd_point<FAST>(xv.y, gv.y, b.y + a[1], f, &q.y, &d.y);
+      *reinterpret_cast<float2*>(q_ws + idx) = q;
+      *reinterpret_cast<float2*>(dx + idx) = d;
+      a[0] = q.x;
+      a[1] = q.y;
     }
-  } else {
-  // --------------------------------- compute warps ---------------------------------
-  uint32_t parp[2] = {0u, 0u}, parq[2] = {0u, 0u};
-  const int ckg = tid & 3, crow = tid >> 2;   // items of a 32-channel chunk: rows crow, crow + 64
-  const int pkg = tid & 1, prow = tid >> 1;   // item of a 16-channel p chunk
-  auto compute_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kBwdCompute) : "memory"); };
-
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const long long p0 = tile * kTileM;
-    // ---- P1: p chunks -> planes -> MMA1, the loads of six chunks in flight at a time ----
-    {
-      const bool live = p0 + prow < n_pix;
-      const float* xr = x + (p0 + prow) * C + pkg * 8;
+    // q's accumulator fragment is, register for register, the A fragment of q . gamma^T
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float4 xv[NK / 2][2];
+    for (int kk = 0; kk < C / 16; ++kk) {
+      const float* a = &acc[kk / 4][8 * (kk % 4)];
 #pragma unroll
-        for (int k = 0; k < NK / 2; ++k) {
-          const float4* src = reinterpret_cast<const float4*>(xr + (half * (NK / 2) + k) * 16);
-          xv[k][0] = live ? __ldg(src) : make_float4(0.f, 0.f, 0.f, 0.f);
-          xv[k][1] = live ? __ldg(src + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int k = 0; k < NK / 2; ++k) {
-          const int c = half * (NK / 2) + k, pb = c & 1;
-          if (c >= 2) {
-            if (!mbar_wait(smem_u32(mbars + pb), parp[pb])) __trap();
-            parp[pb] ^= 1u;
-          }
-          const float4 a = xv[k][0], b = xv[k][1];
-          float v[8] = {tc_pool<FAST>(a.x, f), tc_pool<FAST>(a.y, f), tc_pool<FAST>(a.z, f), tc_pool<FAST>(a.w, f),
-                        tc_pool<FAST>(b.x, f), tc_pool<FAST>(b.y, f), tc_pool<FAST>(b.z, f), tc_pool<FAST>(b.w, f)};
-          uint4 hi, lo;
-          split8(v, &hi, &lo);
-          uint8_t* ph = smem + L::kOffP + pb * 2 * L::kPlaneP;
-          *reinterpret_cast<uint4*>(ph + pkg * kKg + prow * 16) = hi;
-          *reinterpret_cast<uint4*>(ph + L::kPlaneP + pkg * kKg + prow * 16) = lo;
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          asm volatile("bar.arrive %0, %1;" ::"r"(2 + pb), "n"(kBwdThreads) : "memory");
-        }
-      }
+      for (int r = 0; r < 4; ++r) split2(a[2 * r], a[2 * r + 1], &ah[kk][r], &al[kk][r]);
     }
-    float4 xq[2][2][2], gq[2][2][2];  // [set][item][half]
-    auto load_xg = [&](int set, int c) {
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const bool live = p0 + row < n_pix;
-        const long long off = (p0 + row) * C + c * 32 + ckg * 8;
-        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-        xq[set][it][0] = live ? __ldg(reinterpret_cast<const float4*>(x + off)) : z;
-        xq[set][it][1] = live ? __ldg(reinterpret_cast<const float4*>(x + off) + 1) : z;
-        gq[set][it][0] = live ? __ldg(reinterpret_cast<const float4*>(dy + off)) : z;
-        gq[set][it][1] = live ? __ldg(reinterpret_cast<const float4*>(dy + off) + 1) : z;
+    gemm3<C, 1>(acc, ah, al, bh, bl);
+    TFCB_FOR_ACC_PAIRS(C) {
+      if (!(h ? ok1 : ok0)) continue;
+      const long long idx = (h ? r1 : r0) * C + 64 * n + 8 * jj + 2 * t;
+      const float2 xv = __ldg(reinterpret_cast<const float2*>(x + idx));
+      float2 d = *reinterpret_cast<const float2*>(dx + idx);
+      d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
+      d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
+      if (!FAST && f.rectify) {
+        if (!(xv.x > 0.f)) d.x = 0.f;
+        if (!(xv.y > 0.f)) d.y = 0.f;
       }
-    };
-    load_xg(0, 0);
-    // the last two p commits cover every MMA1 step: n is complete
-#pragma unroll
-    for (int pb = 0; pb < 2; ++pb) {
-      if (!mbar_wait(smem_u32(mbars + pb), parp[pb])) __trap();
-      parp[pb] ^= 1u;
+      *reinterpret_cast<float2*>(dx + idx) = d;
     }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- P2: q = dL/dn per 32-channel chunk -> q planes + global q; MMA2 ----
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int b = c & 1;
-      load_xg(b ^ 1, (c + 1) % NCH);
-      {
-        uint32_t acc[16];
-        tmem_load<16>(tmem_n + lane_sel + (uint32_t)(c * 32 + h * 16), acc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        stage_store16(stage_n + r * kStLd + h * 16, acc);
-      }
-      if (c >= 2) {
-        if (!mbar_wait(smem_u32(mbars + 2 + b), parq[b])) __trap();
-        parq[b] ^= 1u;
-      }
-      compute_sync();
-      uint8_t* qh = smem + L::kOffQ + b * 2 * L::kPlaneQ;
-      uint8_t* ql = qh + L::kPlaneQ;
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8);
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8 + 4);
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const float4 n0 = *reinterpret_cast<const float4*>(stage_n + row * kStLd + ckg * 8);
-        const float4 n1 = *reinterpret_cast<const float4*>(stage_n + row * kStLd + ckg * 8 + 4);
-        const float4 x0 = xq[b][it][0], x1 = xq[b][it][1], g0 = gq[b][it][0], g1 = gq[b][it][1];
-        float q[8];
-        q[0] = tc_dl_dn<FAST>(g0.x, x0.x, bv0.x + n0.x, f);
-        q[1] = tc_dl_dn<FAST>(g0.y, x0.y, bv0.y + n0.y, f);
-        q[2] = tc_dl_dn<FAST>(g0.z, x0.z, bv0.z + n0.z, f);
-        q[3] = tc_dl_dn<FAST>(g0.w, x0.w, bv0.w + n0.w, f);
-        q[4] = tc_dl_dn<FAST>(g1.x, x1.x, bv1.x + n1.x, f);
-        q[5] = tc_dl_dn<FAST>(g1.y, x1.y, bv1.y + n1.y, f);
-        q[6] = tc_dl_dn<FAST>(g1.z, x1.z, bv1.z + n1.z, f);
-        q[7] = tc_dl_dn<FAST>(g1.w, x1.w, bv1.w + n1.w, f);
-        uint4 hi, lo;
-        split8(q, &hi, &lo);
-        *reinterpret_cast<uint4*>(qh + ckg * kKg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(ql + ckg * kKg + row * 16) = lo;
-        if (p0 + row < n_pix) {
-          float4* dst = reinterpret_cast<float4*>(q_out + (p0 + row) * C + c * 32 + ckg * 8);
-          __stcs(dst, make_float4(q[0], q[1], q[2], q[3]));
-          __stcs(dst + 1, make_float4(q[4], q[5], q[6], q[7]));
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(4 + b), "n"(kBwdThreads) : "memory");
-      compute_sync();  // staging free again
-    }
-    // ---- P3: dx = g / m + dpool/du * dp ----
-#pragma unroll
-    for (int b = 0; b < 2; ++b) {
-      if (!mbar_wait(smem_u32(mbars + 2 + b), parq[b])) __trap();
-      parq[b] ^= 1u;
-    }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const int b = c & 1;
-      if (c + 1 < NCH) load_xg(b ^ 1, c + 1);
-      {
-        uint32_t an[16], ad[16];
-        tmem_load<16>(tmem_n + lane_sel + (uint32_t)(c * 32 + h * 16), an);
-        tmem_load<16>(tmem_dp + lane_sel + (uint32_t)(c * 32 + h * 16), ad);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        stage_store16(stage_n + r * kStLd + h * 16, an);
-        stage_store16(stage_d + r * kStLd + h * 16, ad);
-      }
-      compute_sync();
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8);
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + ckg * 8 + 4);
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = crow + 64 * it;
-        const float4 n0 = *reinterpret_cast<const float4*>(stage_n + row * kStLd + ckg * 8);
-        const float4 n1 = *reinterpret_cast<const float4*>(stage_n + row * kStLd + ckg * 8 + 4);
-        const float4 d0 = *reinterpret_cast<const float4*>(stage_d + row * kStLd + ckg * 8);
-        const float4 d1 = *reinterpret_cast<const float4*>(stage_d + row * kStLd + ckg * 8 + 4);
-        const float4 x0 = xq[b][it][0], x1 = xq[b][it][1], g0 = gq[b][it][0], g1 = gq[b][it][1];
-        float4 o0, o1;
-        o0.x = tc_dx<FAST>(g0.x, x0.x, bv0.x + n0.x, d0.x, f);
-        o0.y = tc_dx<FAST>(g0.y, x0.y, bv0.y + n0.y, d0.y, f);
-        o0.z = tc_dx<FAST>(g0.z, x0.z, bv0.z + n0.z, d0.z, f);
-        o0.w = tc_dx<FAST>(g0.w, x0.w, bv0.w + n0.w, d0.w, f);
-        o1.x = tc_dx<FAST>(g1.x, x1.x, bv1.x + n1.x, d1.x, f);
-        o1.y = tc_dx<FAST>(g1.y, x1.y, bv1.y + n1.y, d1.y, f);
-        o1.z = tc_dx<FAST>(g1.z, x1.z, bv1.z + n1.z, d1.z, f);
-        o1.w = tc_dx<FAST>(g1.w, x1.w, bv1.w + n1.w, d1.w, f);
-        if (p0 + row < n_pix) {
-          float4* dst = reinterpret_cast<float4*>(dx + (p0 + row) * C + c * 32 + ckg * 8);
-          __stcs(dst, o0);  // streaming stores: keep x / dy (re-read from L2) resident instead of the outputs
-          __stcs(dst + 1, o1);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      compute_sync();
-    }
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
   }
 }
 
+// Backward, part 2: per-CTA partials dgamma[j, i] = sum_pix p[pix, j] q[pix, i] and dbeta[i] = sum_pix q[pix, i].
+// C / 64 warpgroups; warpgroup w accumulates rows 64 w .. 64 w + 63 of dgamma.  A 64-pixel chunk of p and q is staged
+// as bf16 hi / lo planes [C / 8][64][8] (MN-major core matrices: 8 channels x 8 pixels); thread t stages channels
+// 8 (t / 16) .. + 7 of pixels t % 16 + 16 s, s < 4, and keeps the dbeta sums of those channels.
 template <int C>
-struct Bwd3Smem {
-  static constexpr int kPlane = (C / 8) * kKg;       // one full-K plane
-  static constexpr int kOffPh = 0;
-  static constexpr int kOffPl = kOffPh + kPlane;
-  static constexpr int kOffQh = kOffPl + kPlane;
-  static constexpr int kOffQl = kOffQh + kPlane;
-  static constexpr int kOffDbeta = kOffQl + kPlane;
-  static constexpr int kOffBar = kOffDbeta + C * 4;
-  static constexpr int kBytes = kOffBar + 64;
-  static_assert(kBytes <= 232448, "shared memory budget");
+struct DgCfg {
+  static constexpr int kThreads = 2 * C;
+  static constexpr int kPlane = C * kTileM * 2;
+  static constexpr int kStage = 4 * kPlane;  // p hi, p lo, q hi, q lo
+  static constexpr int kSmem = 2 * kStage;
+  static_assert(kSmem <= 232448, "shared memory budget");
 };
+
+// The tensor core's fp32 accumulation is not round-to-nearest: a long-running accumulator drifts with the number of
+// accumulation steps.  The accumulator is therefore added into the CTA's fp32 partial in global memory (round-to-
+// nearest adds, L2 resident) every kDgFlush chunks and restarted.
+constexpr int kDgFlush = 8;
 
 template <int C, bool FAST>
-__global__ void __launch_bounds__(kBwdThreads, 1)
-gdn_tc_bwd_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                         float* __restrict__ part_b, long long n_pix, TcFlags f) {
-  using L = Bwd3Smem<C>;
-  constexpr int KG = C / 8;                                     // 8-channel groups per row
-  constexpr int ITEMS = kTileM * KG / kBwdCompute;              // (row, kg) items per thread and array: 12
-  constexpr int PERIOD = 3;                                     // kg of a thread's items repeats with this period
-  static_assert(C == 192 && (kTileM * KG) % kBwdCompute == 0 && ITEMS % 4 == 0, "item mapping");
+__global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
+gdn_tc_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                     float* __restrict__ part_b, long long n_pix, TcFlags f) {
+  using L = DgCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* dbeta_s = reinterpret_cast<float*>(smem + L::kOffDbeta);
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + 16);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 1, gwarp = warp & 3;
-  constexpr uint32_t kIdesc = umma_idesc(kTileM, C) | (1u << 15) | (1u << 16);  // A = p^T, B = q, both MN-major views
-  for (int i = tid; i < C; i += kBwdThreads) dbeta_s[i] = 0.f;
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbar)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_a = *tmem_slot, tmem_b = tmem_a + C;  // rows j in [0,128) | rows j in [64,192)
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  int t_idx = 0;  // this CTA's tile counter (both roles count alike)
+  const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int jc = tid >> 4, pl = tid & 15;
+  const long long n_chunks = (n_pix + kTileM - 1) / kTileM;
+  float bsum[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) bsum[e] = 0.f;
 
-  if (warp == kBwdCompute / 32) {
-    const uint32_t p_hi = smem_u32(smem + L::kOffPh), p_lo = smem_u32(smem + L::kOffPl);
-    const uint32_t q_hi = smem_u32(smem + L::kOffQh), q_lo = smem_u32(smem + L::kOffQl);
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t_idx) {
-      if (lane == 1) {
-        const long long pn = (tile + gridDim.x) * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - pn);
-        if (rows > 0) {
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(x + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q + pn * C), "r"((uint32_t)(rows * C * 4)) : "memory");
-        }
-      }
-      asm volatile("bar.sync 2, %0;" ::"n"(kBwdThreads) : "memory");
-      if (lane == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-        for (int blk = 0; blk < 2; ++blk) {
-          const uint32_t moff = (uint32_t)(blk * 8) * kKg;  // second block starts at channel 64 = m group 8
-          const uint32_t td = blk ? tmem_b : tmem_a;
+  auto stage = [&](long long chunk, int buf) {
+    uint8_t* base = smem + buf * L::kStage;
 #pragma unroll
-          for (int s = 0; s < kTileM / 16; ++s) {
-            const uint32_t koff = (uint32_t)(s * 16) * 16u;
-            const uint64_t dah = umma_desc(p_hi + moff + koff, 128, kKg);
-            const uint64_t dal = umma_desc(p_lo + moff + koff, 128, kKg);
-            const uint64_t dbh = umma_desc(q_hi + koff, 128, kKg);
-            const uint64_t dbl = umma_desc(q_lo + koff, 128, kKg);
-            umma_bf16(td, dah, dbh, kIdesc, ((t_idx % kDgFlush) == 0 && s == 0) ? 0u : 1u);  // restarted after a flush
-            umma_bf16(td, dal, dbh, kIdesc, 1u);
-            umma_bf16(td, dah, dbl, kIdesc, 1u);
-          }
-        }
-        umma_commit(smem_u32(mbar));
-      }
-      __syncwarp();
-    }
-  } else {
-  uint32_t par = 0u;
-  bool flushed = false;  // the global partial holds earlier flushes
-  // block a: lane r = channel j = r; block b: lane r = channel 64 + r (only its rows >= 128 are new)
-  auto flush_dgamma = [&]() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int blk = 0; blk < 2; ++blk) {
-      const int j = blk ? 64 + r : r;
-      float* pg = part_g + (long long)blockIdx.x * C * C + (long long)j * C + h * (C / 2);
+    for (int s = 0; s < 4; ++s) {
+      const int p = pl + 16 * s;
+      const long long row = chunk * kTileM + p;
+      float v[8], w[8];
+      if (row < n_pix) {
+        const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
+        const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
+        const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1), q0 = __ldg(qr), q1 = __ldg(qr + 1);
+        v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
+        w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+      } else {
 #pragma unroll
-      for (int cb = 0; cb < C / 32; ++cb) {
-        uint32_t a[16];
-        tmem_load<16>((blk ? tmem_b : tmem_a) + lane_sel + (uint32_t)(h * (C / 2) + cb * 16), a);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (!blk || r >= 64) accum_store16(pg + cb * 16, a, flushed);
+        for (int e = 0; e < 8; ++e) v[e] = w[e] = 0.f;
       }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[e] = tc_pool<FAST>(v[e], f);
+        bsum[e] += w[e];
+      }
+      const int slot = (jc * kTileM + p) * 16;
+      uint4 hi, lo;
+      split8(v, &hi, &lo);
+      *reinterpret_cast<uint4*>(base + slot) = hi;
+      *reinterpret_cast<uint4*>(base + L::kPlane + slot) = lo;
+      split8(w, &hi, &lo);
+      *reinterpret_cast<uint4*>(base + 2 * L::kPlane + slot) = hi;
+      *reinterpret_cast<uint4*>(base + 3 * L::kPlane + slot) = lo;
     }
-    flushed = true;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   };
-  float dbeta_acc[PERIOD][8];
+
+  float acc[C / 64][32];
+  float* pg = part_g + (long long)blockIdx.x * C * C;
+  bool first_flush = true;
+  stage(blockIdx.x, 0);
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+  int k = 0;
+  for (long long chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x, ++k) {
+    if (k % kDgFlush == 0) {
 #pragma unroll
-  for (int a = 0; a < PERIOD; ++a)
+      for (int n = 0; n < C / 64; ++n)
 #pragma unroll
-    for (int e = 0; e < 8; ++e) dbeta_acc[a][e] = 0.f;
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t_idx) {
-    const long long p0 = tile * kTileM;
-    bool waited = t_idx == 0;
+        for (int i = 0; i < 32; ++i) acc[n][i] = 0.f;
+    }
+    // core matrix (channel / 8, pixel / 8) at (channel / 8) * 1024 + (pixel / 8) * 128 bytes of a plane
+    const uint32_t base = smem_u32(smem + (k & 1) * L::kStage);
+    const uint32_t planes[3][2] = {{0, 2}, {1, 2}, {0, 3}};  // (p, q) plane pairs: hi.hi, lo.hi, hi.lo
+    wgmma_fence();
 #pragma unroll
-    for (int pass = 0; pass < ITEMS / 4; ++pass) {
-      float4 xv[4][2], qv[4][2];
+    for (int kk = 0; kk < kTileM / 16; ++kk)
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int id = (pass * 4 + i) * kBwdCompute + tid;
-        const int row = id / KG, kg = id % KG;
-        const bool live = p0 + row < n_pix;
-        const long long off = (p0 + row) * C + kg * 8;
-        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-        xv[i][0] = live ? __ldg(reinterpret_cast<const float4*>(x + off)) : z;
-        xv[i][1] = live ? __ldg(reinterpret_cast<const float4*>(x + off) + 1) : z;
-        qv[i][0] = live ? __ldg(reinterpret_cast<const float4*>(q + off)) : z;
-        qv[i][1] = live ? __ldg(reinterpret_cast<const float4*>(q + off) + 1) : z;
+      for (int pr = 0; pr < 3; ++pr) {
+        const uint64_t a = gmma_desc(base + planes[pr][0] * L::kPlane + wg * 8 * 1024 + 256 * kk, 128, 1024);
+#pragma unroll
+        for (int n = 0; n < C / 64; ++n)
+          wgmma_ss_mn(acc[n], a, gmma_desc(base + planes[pr][1] * L::kPlane + n * 8 * 1024 + 256 * kk, 128, 1024));
       }
-      if (!waited) {  // the planes are being read by the previous tile's MMAs
-        if (!mbar_wait(smem_u32(mbar), par)) __trap();
-        par ^= 1u;
-        waited = true;
-        if ((t_idx % kDgFlush) == 0) flush_dgamma();  // t_idx tiles are in the accumulator and complete
+    wgmma_commit();
+    const bool last = chunk + gridDim.x >= n_chunks;
+    if (!last) stage(chunk + gridDim.x, (k + 1) & 1);
+    wgmma_wait_all();
+    fence_acc(acc);
+    if ((k + 1) % kDgFlush == 0 || last) {
+      TFCB_FOR_ACC_PAIRS(C) {
+        float2* dst = reinterpret_cast<float2*>(pg + (64 * wg + 16 * warp + g + 8 * h) * C + 64 * n + 8 * jj + 2 * t);
+        float2 v = make_float2(acc[n][4 * jj + 2 * h], acc[n][4 * jj + 2 * h + 1]);
+        if (!first_flush) {
+          const float2 o = *dst;
+          v.x += o.x;
+          v.y += o.y;
+        }
+        *dst = v;
       }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int j = pass * 4 + i;
-        const int id = j * kBwdCompute + tid;
-        const int row = id / KG, kg = id % KG;
-        const float4 a = xv[i][0], b = xv[i][1];
-        float v[8] = {tc_pool<FAST>(a.x, f), tc_pool<FAST>(a.y, f), tc_pool<FAST>(a.z, f), tc_pool<FAST>(a.w, f),
-                      tc_pool<FAST>(b.x, f), tc_pool<FAST>(b.y, f), tc_pool<FAST>(b.z, f), tc_pool<FAST>(b.w, f)};
-        uint4 hi, lo;
-        split8(v, &hi, &lo);
-        *reinterpret_cast<uint4*>(smem + L::kOffPh + kg * kKg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(smem + L::kOffPl + kg * kKg + row * 16) = lo;
-        float w[8] = {qv[i][0].x, qv[i][0].y, qv[i][0].z, qv[i][0].w, qv[i][1].x, qv[i][1].y, qv[i][1].z, qv[i][1].w};
-        split8(w, &hi, &lo);
-        *reinterpret_cast<uint4*>(smem + L::kOffQh + kg * kKg + row * 16) = hi;
-        *reinterpret_cast<uint4*>(smem + L::kOffQl + kg * kKg + row * 16) = lo;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dbeta_acc[j % PERIOD][e] += w[e];
-      }
+      first_flush = false;
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    asm volatile("bar.arrive 2, %0;" ::"n"(kBwdThreads) : "memory");
+    __syncthreads();
   }
-  if (t_idx > 0) {
-    if (!mbar_wait(smem_u32(mbar), par)) __trap();
-    // the tiles since the last flush (a flush is due at the top of a NEXT tile, so a full period may be pending)
-    flush_dgamma();
 #pragma unroll
-    for (int a = 0; a < PERIOD; ++a) {
-      const int kg = (a * kBwdCompute + tid) % KG;
+  for (int e = 0; e < 8; ++e)
 #pragma unroll
-      for (int e = 0; e < 8; ++e) atomicAdd(dbeta_s + kg * 8 + e, dbeta_acc[a][e]);
-    }
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  for (int i = tid; i < C; i += kBwdThreads) part_b[(long long)blockIdx.x * C + i] = dbeta_s[i];
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
+    for (int o = 8; o > 0; o >>= 1) bsum[e] += __shfl_xor_sync(0xFFFFFFFFu, bsum[e], o);
+  if (pl == 0) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) part_b[(long long)blockIdx.x * C + 8 * jc + e] = bsum[e];
   }
 }
 
-// =============================================================================================
-// Backward, C = 128, second kernel shape (the default GDN / IGDN: alpha = 1, epsilon = 1, no rectification).
-//
-// Same mathematics and the same operand planes / MN-major views as gdn_tc_bwd_kernel above, rebuilt along the
-// lines of the C = 192 forward: everything that touches HBM is an asynchronous 2-D TMA box, every compute thread
-// (r, h) owns pixel row r (= its TMEM lane) and 8 of the 32 channels of a box, so there are no staging
-// transposes and no CTA-wide barriers, and x and dy are read exactly once:
-//
-//   conv(t)   x boxes -> p = |x| hi / lo planes (whole K)                -> MMA1  n = p . gamma
-//             the raw x values are parked in 128 spare TMEM columns (tcgen05.st) for pass 2
-//   pass2(t)  g boxes + n, x from TMEM -> q hi / lo planes (whole tile, written 32 channels at a time)
-//                                                                         -> MMA2  dp += q_chunk . gamma^T  per chunk
-//             the direct term g / n (IGDN: g * n) goes back into n's TMEM columns with sign(x) in the two low
-//             mantissa bits (2 ulp, the contract is 1e-5): the dx pass needs neither x nor g again
-//   pass3(t)  dx = direct + sign(x) * dp  from TMEM only -> box -> TMA store;  meanwhile
-//                                                                         -> MMA3  dgamma += p^T q, 24 full-width MMAs
-//
-// (With 32-channel q buffers MMA3 was 96 MMAs of N = 32 per tile, each re-reading its 4 KB A operand from shared
-// memory for 16 cycles of math: switching them off saved 20 % of the kernel.)  The whole-tile q planes take the
-// place of the resident gamma planes: gamma (and gamma^T for MMA2) is streamed from L2 in 32-channel K chunks
-// (16 KB hi + lo, double buffered) by a "gamma" warp, 128 KB per tile.
-// One ring of four 16 KB boxes serves every box request in program order: g x 4 (pass 2), output x 4 (pass 3),
-// x x 4 (conversion of the CTA's next tile).  TMEM: n | dp | dgamma partial | parked x (4 x 128 columns).
-// HBM traffic: x, dy in, dx out, nothing else.
-// =============================================================================================
-__device__ __forceinline__ void tmem_store8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-// gamma [C, C] -> bf16 K chunks for the streamed kernels: for t in {gamma (MMA1: K = j), gamma^T (MMA2: K = i)} and each
-// 32-channel K chunk c one block [hi: 4 groups x C x 8][lo: the same], i.e. chunk (t, c) is ONE contiguous copy of
-// C * 128 bytes (a copy instruction costs the SM's copy engine ~0.35 us whatever its size).  INTERLEAVED = false keeps
-// four whole planes [gamma hi, gamma lo, gamma^T hi, gamma^T lo] (the C = 192 dx kernel keeps a whole hi plane resident).
-template <bool INTERLEAVED>
-__global__ void gdn_tc_prep2_kernel(const float* __restrict__ gamma, int C, __nv_bfloat16* __restrict__ planes) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // over (k / 8, n)
-  if (idx >= (C / 8) * C) return;
-  const int kc = idx / C, n = idx % C;
-  float v[8], w[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    v[e] = gamma[(kc * 8 + e) * C + n];  // k = j (input channel), n = i
-    w[e] = gamma[n * C + kc * 8 + e];    // k = i, n = j
-  }
-  uint4* out = reinterpret_cast<uint4*>(planes);
-  const size_t plane16 = (size_t)C * C / 8;  // 16-byte units per plane
-  uint4 hi, lo;
-  split8(v, &hi, &lo);
-  if (INTERLEAVED) {
-    const size_t chunk16 = (size_t)4 * C;  // units of one chunk of one plane
-    const size_t at = ((size_t)(kc / 4) * 2) * chunk16 + (size_t)(kc % 4) * C + n;
-    out[at] = hi;
-    out[at + chunk16] = lo;
-    split8(w, &hi, &lo);
-    out[2 * plane16 + at] = hi;
-    out[2 * plane16 + at + chunk16] = lo;
-  } else {
-    out[idx] = hi;
-    out[plane16 + idx] = lo;
-    split8(w, &hi, &lo);
-    out[2 * plane16 + idx] = hi;
-    out[3 * plane16 + idx] = lo;
-  }
-}
-
-constexpr int kB3Compute = 512;                // 16 compute warps
-constexpr int kB3Threads = kB3Compute + 160;   // + two MMA-issue warps, box-copy, gamma and store warps
-constexpr int kB3SyncA = kB3Compute + 32;      // compute + first issue warp
-constexpr int kB3SyncB = kB3Compute + 64;      // compute + both issue warps (last q chunk of a tile)
-constexpr int kB3Slots = 4;
-
-struct BwdFusedSmem {
-  static constexpr int C = 128;
-  static constexpr int kGChunk = 4 * C * 16;                      // one 32-channel K chunk of one gamma plane (8 KB)
-  static constexpr int kOffRing = 0;                              // [4] boxes (1024-byte aligned: swizzle atom)
-  static constexpr int kOffG = kOffRing + kB3Slots * kF4Box;      // [2 buffers][hi, lo] gamma K chunks
-  static constexpr int kPlane = (C / 8) * kKg;                    // one whole-K operand plane (p or q, hi or lo)
-  static constexpr int kOffPh = kOffG + 4 * kGChunk;
-  static constexpr int kOffPl = kOffPh + kPlane;
-  static constexpr int kOffQh = kOffPl + kPlane;
-  static constexpr int kOffQl = kOffQh + kPlane;
-  static constexpr int kOffBeta = kOffQl + kPlane;
-  static constexpr int kOffDbeta = kOffBeta + C * 4;
-  static constexpr int kOffBar = kOffDbeta + C * 4;
-  // mbarriers: full[4], empty[4], yready[4], gfull[2], gfree[2], nfull, dpfull, m3done; then the TMEM slot
-  static constexpr int kBarFull = 0, kBarEmpty = 4, kBarY = 8, kBarGfull = 12, kBarGfree = 14, kBarN = 16, kBarDp = 17,
-                       kBarM3 = 18, kNumBars = 19;
-  static constexpr int kBytes = kOffBar + kNumBars * 8 + 16;
-  static_assert(kOffG % 128 == 0 && kOffPh % 16 == 0 && kOffQh % 16 == 0 && kOffBar % 8 == 0, "alignment");
-  static_assert(kBytes <= 232448, "shared memory budget");
-};
-
-__global__ void __launch_bounds__(kB3Threads, 1)
-gdn_tc_bwd3_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap g_map,
-                   const __grid_constant__ CUtensorMap dx_map, const float* __restrict__ x, const float* __restrict__ dy,
-                   const __nv_bfloat16* __restrict__ planes, const float* __restrict__ beta, float* __restrict__ part_g,
-                   float* __restrict__ part_b, long long n_pix, int inverse, int dbg) {
-  using L = BwdFusedSmem;
-  constexpr int C = L::C, NCH = C / 32;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* beta_s = reinterpret_cast<float*>(smem + L::kOffBeta);
-  float* dbeta_s = reinterpret_cast<float*>(smem + L::kOffDbeta);
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + L::kNumBars * 8);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 3, gwarp = warp & 3;  // compute thread (r, h): pixel row r, channel octet h of a box
-  auto bar = [&](int i) { return smem_u32(mbars + i); };
-  for (int i = tid; i < C; i += kB3Threads) {
-    beta_s[i] = beta[i];
-    dbeta_s[i] = 0.f;
-  }
-  if (tid == 0) {
-    for (int i = 0; i < L::kNumBars; ++i) {
-      const int count = (i >= L::kBarY && i < L::kBarGfull) ? kB3Compute / 32 : 1;  // y ready: one arrival per compute warp
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar(i)), "r"(count));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_n = *tmem_slot, tmem_dp = tmem_n + C, tmem_dg = tmem_n + 2 * C, tmem_x = tmem_n + 3 * C;
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const uint32_t p_hi = smem_u32(smem + L::kOffPh), p_lo = smem_u32(smem + L::kOffPl);
-  const uint32_t q_hi = smem_u32(smem + L::kOffQh), q_lo = smem_u32(smem + L::kOffQl);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const long long first = blockIdx.x;
-  // The dgamma accumulator is flushed every kDgFlush tiles; CTAs take turns (all 148 flushing in the same
-  // microsecond made the L2 the bottleneck of the flush)
-  const int fphase = (int)(blockIdx.x % kDgFlush);
-  // Box requests are numbered in program order; request n uses ring slot n % 4 in its (n / 4)-th round:
-  //   4 x boxes (conversion of the CTA's first tile), then per tile  g x 4, out x 4, (x of the next tile) x 4.
-  // Gamma K chunks likewise, buffer m % 2:  4 chunks of gamma (MMA1 of the first tile), then per tile 4 chunks of
-  // gamma^T (MMA2), 4 chunks of gamma (MMA1 of the next tile).
-  constexpr int W0 = kB3Compute / 32;  // first auxiliary warp
-
-  if (warp == W0 + 2) {
-    // ---------------------------------- box-copy warp ----------------------------------
-    if (lane == 0) {
-      uint32_t n = 0;
-      auto acquire = [&]() {
-        const uint32_t slot = n & 3u, round = n >> 2;
-        if (round > 0) {
-          if (!mbar_wait(bar(L::kBarEmpty + slot), (round - 1u) & 1u)) __trap();
-        }
-        return slot;
-      };
-      auto load = [&](const CUtensorMap* map, int c, int row0) {
-        const uint32_t slot = acquire();
-        const uint32_t full = bar(L::kBarFull + slot);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "n"(kF4Box) : "memory");
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(
-                smem_u32(smem + L::kOffRing + slot * kF4Box)),
-            "l"(map), "r"(c * 32), "r"(row0), "r"(full), "l"(kEvictFirst)
-            : "memory");
-        ++n;
-      };
-      auto prefetch_tile = [&](const float* base, long long tile) {  // one contiguous block -> L2
-        const long long p0 = tile * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - p0);
-        if (rows > 0)
-          asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(base + p0 * C),
-                       "r"((uint32_t)(rows * C * 4)), "l"(kEvictLast)
-                       : "memory");
-      };
-      if (first < n_tiles) {
-        prefetch_tile(dy, first);
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) load(&x_map, c, (int)(first * kTileM));
-      }
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-        const long long next = tile + gridDim.x;
-        const bool has_next = next < n_tiles;
-        const int row0 = (int)(tile * kTileM);
-        if (has_next) {  // the next tile of this CTA -> L2: its boxes become L2 hits
-          prefetch_tile(x, next);
-          prefetch_tile(dy, next);
-        }
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) load(&g_map, c, row0);
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) {
-          const uint32_t slot = acquire();      // output box: nothing to load, the slot only has to be free
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarFull + slot)) : "memory");
-          ++n;
-        }
-        if (has_next) {
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c) load(&x_map, c, (int)(next * kTileM));
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0 + 3) {
-    // ---------------------------------- gamma warp: K chunks of gamma / gamma^T ----------------------------------
-    if (lane == 0) {
-      const uint8_t* gp = reinterpret_cast<const uint8_t*>(planes);
-      constexpr size_t kPlaneBytes = (size_t)C * C * 2;
-      uint32_t m = 0;
-      auto chunk = [&](int transposed, int c) {
-        const uint32_t buf = m & 1u;
-        if (m >= 2) {  // the MMAs of chunk m - 2 (same buffer) have completed
-          if (!mbar_wait(bar(L::kBarGfree + buf), ((m >> 1) - 1u) & 1u)) __trap();
-        }
-        const uint32_t gfull = bar(L::kBarGfull + buf);
-        const uint32_t dst = smem_u32(smem + L::kOffG + buf * 2 * L::kGChunk);
-        // chunk (t, c) = [hi 8 KB][lo 8 KB], contiguous in the prepared buffer: one copy
-        const uint8_t* src = gp + (size_t)(2 * transposed) * kPlaneBytes + (size_t)c * (2 * L::kGChunk);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(gfull), "n"(2 * L::kGChunk) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-                     "l"(src), "n"(2 * L::kGChunk), "r"(gfull), "l"(kEvictLast)
-                     : "memory");
-        ++m;
-      };
-      if (first < n_tiles) {
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) chunk(0, c);
-      }
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) chunk(1, c);
-        if (tile + gridDim.x < n_tiles) {
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c) chunk(0, c);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0 + 4) {
-    // ---------------------------------- store warp: dx boxes ----------------------------------
-    if (lane == 0) {
-      uint32_t n = (first < n_tiles) ? (uint32_t)NCH : 0u;
-      uint32_t ypar = 0u;  // per-slot phase of the y-ready barrier (a slot is an output box only now and then)
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-        const bool has_next = tile + gridDim.x < n_tiles;
-        const int row0 = (int)(tile * kTileM);
-        n += NCH;
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c, ++n) {
-          const uint32_t slot = n & 3u;
-          if (!mbar_wait(bar(L::kBarY + slot), (ypar >> slot) & 1u)) __trap();
-          ypar ^= 1u << slot;
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(&dx_map),
-                       "r"(c * 32), "r"(row0), "r"(smem_u32(smem + L::kOffRing + slot * kF4Box)), "l"(kEvictFirst)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the box has been read: the slot is free
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarEmpty + slot)) : "memory");
-        }
-        if (has_next) n += NCH;
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-    __syncwarp();
-  } else if (warp == W0) {
-    // ------------------------------- first MMA-issue warp: MMA1, MMA2 (K-chunked, gamma streamed) ------------------
-    constexpr uint32_t kIdesc = umma_idesc(kTileM, C);  // A, B both K-major
-    uint32_t n = 0, m = 0;
-    // six MMAs of one 32-channel K chunk: A planes (hi, lo) x gamma chunk (hi, lo), three products
-    auto chunk_mmas = [&](uint32_t a_hi, uint32_t a_lo, uint32_t acc, bool first_chunk) {
-      const uint32_t buf = m & 1u;
-      if (!mbar_wait(bar(L::kBarGfull + buf), (m >> 1) & 1u)) __trap();
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t g_hi = smem_u32(smem + L::kOffG + buf * 2 * L::kGChunk), g_lo = g_hi + L::kGChunk;
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        const uint64_t dah = umma_desc(a_hi + (uint32_t)(2 * s2) * kKg, kKg, 128);
-        const uint64_t dal = umma_desc(a_lo + (uint32_t)(2 * s2) * kKg, kKg, 128);
-        const uint64_t dbh = umma_desc(g_hi + (uint32_t)(2 * s2) * (C * 16), C * 16, 128);
-        const uint64_t dbl = umma_desc(g_lo + (uint32_t)(2 * s2) * (C * 16), C * 16, 128);
-        umma_bf16(acc, dah, dbh, kIdesc, (first_chunk && s2 == 0) ? 0u : 1u);
-        umma_bf16(acc, dal, dbh, kIdesc, 1u);
-        umma_bf16(acc, dah, dbl, kIdesc, 1u);
-      }
-      umma_commit(bar(L::kBarGfree + buf));
-      ++m;
-    };
-    auto release = [&](uint32_t req) {
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarEmpty + (req & 3u))) : "memory");
-    };
-    auto mma1_tile = [&]() {  // n = p . gamma of the tile being converted, K chunk by K chunk
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, ++n) {
-        asm volatile("bar.sync %0, %1;" ::"r"(2 + c), "n"(kB3SyncA) : "memory");  // p planes of chunk c are written
-        if (lane == 0) {
-          release(n);
-          chunk_mmas(p_hi + (uint32_t)(4 * c) * kKg, p_lo + (uint32_t)(4 * c) * kKg, tmem_n, c == 0);
-          if (c == NCH - 1) umma_commit(bar(L::kBarN));
-        }
-        __syncwarp();
-      }
-    };
-    if (first < n_tiles) mma1_tile();
-    for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-      const bool has_next = tile + gridDim.x < n_tiles;
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, ++n) {
-        if (c == NCH - 1) asm volatile("bar.sync %0, %1;" ::"r"(6 + c), "n"(kB3SyncB) : "memory");
-        else asm volatile("bar.sync %0, %1;" ::"r"(6 + c), "n"(kB3SyncA) : "memory");  // q planes of chunk c are written
-        if (lane == 0) {
-          release(n);  // the g box of this chunk
-          // MMA2: dp[pix, j] += sum_{i in chunk} q[pix, i] gamma[j, i]
-          chunk_mmas(q_hi + (uint32_t)(4 * c) * kKg, q_lo + (uint32_t)(4 * c) * kKg, tmem_dp, c == 0);
-          if (c == NCH - 1) umma_commit(bar(L::kBarDp));  // dp is complete: the dx pass may start
-        }
-        __syncwarp();
-      }
-      n += NCH;  // the output boxes: handed back by the store warp
-      if (has_next) mma1_tile();
-    }
-  } else if (warp == W0 + 1) {
-    // ------------------------------- second MMA-issue warp: MMA3, once per tile -------------------------------
-    constexpr uint32_t kIdesc3 = umma_idesc(C, C) | (1u << 15) | (1u << 16);    // A = p^T, B = q (both MN-major views)
-    int t = 0;
-    for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-      asm volatile("bar.sync %0, %1;" ::"r"(6 + NCH - 1), "n"(kB3SyncB) : "memory");  // the whole tile of q is written
-      if (lane == 0) {
-        // let the tile's last MMA2s through first: the dx pass waits for them, nothing waits for MMA3 until the next
-        // conversion (both issue warps leave the same barrier; 24 MMAs ahead of 6 cost the dx pass ~0.8 us per tile)
-        if (!(dbg & 8)) {
-          if (!mbar_wait(bar(L::kBarDp), (uint32_t)t & 1u)) __trap();
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // dgamma[j, i] += sum_pix p[pix, j] q[pix, i]   (K = pix: 8 steps of 16)
-        if (!(dbg & 1)) {
-          const bool restart = (t == 0) || (((t + fphase) % kDgFlush) == 0);  // first MMA after a flush
-#pragma unroll
-          for (int s = 0; s < kTileM / 16; ++s) {
-            const uint32_t koff = (uint32_t)(s * 16) * 16u;
-            const uint64_t dah = umma_desc(p_hi + koff, 128, kKg);
-            const uint64_t dal = umma_desc(p_lo + koff, 128, kKg);
-            const uint64_t dbh = umma_desc(q_hi + koff, 128, kKg);
-            const uint64_t dbl = umma_desc(q_lo + koff, 128, kKg);
-            umma_bf16(tmem_dg, dah, dbh, kIdesc3, (restart && s == 0) ? 0u : 1u);
-            umma_bf16(tmem_dg, dal, dbh, kIdesc3, 1u);
-            umma_bf16(tmem_dg, dah, dbl, kIdesc3, 1u);
-          }
-        }
-        umma_commit(bar(L::kBarM3));
-      }
-      __syncwarp();
-    }
-  } else if (warp < W0) {
-  // --------------------------------- compute warps ---------------------------------
-  uint32_t n = 0;
-  float dbeta_acc[NCH][8];  // channels 32 c + 8 h + e, summed over this thread's rows
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) dbeta_acc[c][e] = 0.f;
-  // 128-byte swizzle: the 16-byte chunk j of box row `row` sits at chunk j ^ (row & 7)
-  auto chunk_at = [](uint8_t* box, int row, int j) { return reinterpret_cast<float4*>(box + row * 128 + ((j ^ (row & 7)) << 4)); };
-  bool flushed = false;  // the global partial holds earlier flushes
-  // The accumulator (TMEM lane = input channel j, 32 columns per thread) is transposed through the dead q planes
-  // ([128][128] fp32, 16-byte units XOR-swizzled by the row) so that every warp adds 512 contiguous bytes to the CTA's
-  // partial: with one row per lane each vector add touched 32 different L2 lines (8 % of the kernel).
-  auto flush_dgamma = [&]() {
-    uint8_t* stage = smem + L::kOffQh;
-#pragma unroll
-    for (int cb = 0; cb < 2; ++cb) {
-      uint32_t a[16];
-      tmem_load<16>(tmem_dg + lane_sel + (uint32_t)(h * 32 + cb * 16), a);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        *reinterpret_cast<uint4*>(stage + r * 512 + (((h * 8 + cb * 4 + i) ^ (r & 7)) << 4)) =
-            make_uint4(a[4 * i], a[4 * i + 1], a[4 * i + 2], a[4 * i + 3]);
-    }
-    asm volatile("bar.sync 1, %0;" ::"n"(kB3Compute) : "memory");
-    float* pg = part_g + (long long)blockIdx.x * C * C;
-#pragma unroll
-    for (int it = 0; it < (C * C / 4) / kB3Compute; ++it) {
-      const int item = it * kB3Compute + tid, row = item >> 5, c4 = item & 31;
-      const uint4 v = *reinterpret_cast<const uint4*>(stage + row * 512 + ((c4 ^ (row & 7)) << 4));
-      float* dst = pg + row * C + c4 * 4;
-      // first flush: plain stores; later ones: fire-and-forget vector adds in L2
-      if (!flushed)
-        asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-      else
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-    }
-    flushed = true;
-  };
-
-  // One tile: p = |x| -> hi / lo planes chunk by chunk (each chunk arrives on its own named barrier), raw x -> TMEM
-  auto conv_tile = [&]() {
-#pragma unroll 1
-    for (int c = 0; c < NCH; ++c, ++n) {
-      const uint32_t slot = n & 3u, round = n >> 2;
-      uint8_t* box = smem + L::kOffRing + slot * kF4Box;
-      if (!mbar_wait(bar(L::kBarFull + slot), round & 1u)) __trap();
-      const float4 a = *chunk_at(box, r, 2 * h), b = *chunk_at(box, r, 2 * h + 1);
-      const uint32_t raw[8] = {__float_as_uint(a.x), __float_as_uint(a.y), __float_as_uint(a.z), __float_as_uint(a.w),
-                               __float_as_uint(b.x), __float_as_uint(b.y), __float_as_uint(b.z), __float_as_uint(b.w)};
-      tmem_store8(tmem_x + lane_sel + (uint32_t)(c * 32 + h * 8), raw);
-      float v[8] = {fabsf(a.x), fabsf(a.y), fabsf(a.z), fabsf(a.w), fabsf(b.x), fabsf(b.y), fabsf(b.z), fabsf(b.w)};
-      uint4 hi, lo;
-      split8(v, &hi, &lo);
-      *reinterpret_cast<uint4*>(smem + L::kOffPh + (4 * c + h) * kKg + r * 16) = hi;
-      *reinterpret_cast<uint4*>(smem + L::kOffPl + (4 * c + h) * kKg + r * 16) = lo;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(2 + c), "n"(kB3SyncA) : "memory");  // (also releases the box, see issue warp)
-    }
-  };
-
-  if (first < n_tiles) conv_tile();
-  int t = 0;
-  for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-    const bool has_next = tile + gridDim.x < n_tiles;
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");  // this thread's parked x values are in TMEM
-    if (!mbar_wait(bar(L::kBarN), (uint32_t)t & 1u)) __trap();  // MMA1 of this tile has completed
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- pass 2: q = dL/dn -> q planes; the direct term and sign(x) go back into n's columns ----
-#pragma unroll
-    for (int c = 0; c < NCH; ++c, ++n) {
-      const uint32_t slot = n & 3u;
-      const uint32_t col = lane_sel + (uint32_t)(c * 32 + h * 8);
-      uint32_t nacc[8], xraw[8];
-      tmem_load<8>(tmem_n + col, nacc);
-      tmem_load<8>(tmem_x + col, xraw);
-      if (!mbar_wait(bar(L::kBarFull + slot), (n >> 2) & 1u)) __trap();
-      uint8_t* bg = smem + L::kOffRing + slot * kF4Box;
-      const float4 g0 = *chunk_at(bg, r, 2 * h), g1 = *chunk_at(bg, r, 2 * h + 1);
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + h * 8);      // same address in every lane
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + h * 8 + 4);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const float gs[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      const float bs[8] = {bv0.x, bv0.y, bv0.z, bv0.w, bv1.x, bv1.y, bv1.z, bv1.w};
-      float q[8];
-      uint32_t dbits[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float xe = __uint_as_float(xraw[e]);
-        const float nn = bs[e] + __uint_as_float(nacc[e]);
-        float direct;
-        if (inverse) {
-          direct = gs[e] * nn;
-          q[e] = gs[e] * xe;
-        } else {
-          const float rn = rcp_approx(nn);
-          direct = gs[e] * rn;
-          q[e] = -gs[e] * xe * rn * rn;
-        }
-        const uint32_t code = (xe > 0.f) ? 1u : ((xe < 0.f) ? 2u : 0u);
-        dbits[e] = (__float_as_uint(direct) & ~3u) | code;
-        dbeta_acc[c][e] += q[e];
-      }
-      uint4 hi, lo;
-      split8(q, &hi, &lo);
-      *reinterpret_cast<uint4*>(smem + L::kOffQh + (4 * c + h) * kKg + r * 16) = hi;
-      *reinterpret_cast<uint4*>(smem + L::kOffQl + (4 * c + h) * kKg + r * 16) = lo;
-      tmem_store8(tmem_n + col, dbits);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      if (c == NCH - 1) asm volatile("bar.arrive %0, %1;" ::"r"(6 + c), "n"(kB3SyncB) : "memory");
-      else asm volatile("bar.arrive %0, %1;" ::"r"(6 + c), "n"(kB3SyncA) : "memory");  // (also releases the g box)
-    }
-    // ---- pass 3: dx = direct + sign(x) * dp, from TMEM only ----
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");  // this thread's direct terms are in TMEM
-    if (!mbar_wait(bar(L::kBarDp), (uint32_t)t & 1u)) __trap();  // every MMA2 of this tile has completed
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c = 0; c < NCH; ++c, ++n) {
-      const uint32_t slot = n & 3u, round = n >> 2;
-      uint32_t d[8], p[8];
-      tmem_load<8>(tmem_n + lane_sel + (uint32_t)(c * 32 + h * 8), d);
-      tmem_load<8>(tmem_dp + lane_sel + (uint32_t)(c * 32 + h * 8), p);
-      uint8_t* box = smem + L::kOffRing + slot * kF4Box;
-      if (!mbar_wait(bar(L::kBarFull + slot), round & 1u)) __trap();  // the slot's previous user has left
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float o[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const uint32_t code = d[e] & 3u;
-        const float s = (code == 1u) ? 1.f : ((code == 2u) ? -1.f : 0.f);
-        o[e] = fmaf(s, __uint_as_float(p[e]), __uint_as_float(d[e]));
-      }
-      *chunk_at(box, r, 2 * h) = make_float4(o[0], o[1], o[2], o[3]);
-      *chunk_at(box, r, 2 * h + 1) = make_float4(o[4], o[5], o[6], o[7]);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // dx box -> TMA store
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarY + slot)) : "memory");
-    }
-    // MMA3 of this tile has completed: the p and q planes are dead, the dgamma accumulator is up to date
-    if (!mbar_wait(bar(L::kBarM3), (uint32_t)t & 1u)) __trap();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (((t + fphase) % kDgFlush) == kDgFlush - 1 && !(dbg & 4)) flush_dgamma();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // TMEM reads precede the next tile's MMAs
-    if (has_next) conv_tile();
-  }
-
-  // ---- this CTA's partial sums ----
-  if (t > 0) {
-    if (((t + fphase) % kDgFlush) != 0) flush_dgamma();  // tiles since the last flush
-    // dbeta: the 32 lanes of a warp hold the same channels (32 c + 8 h + e) for 32 different rows
-#pragma unroll
-    for (int c = 0; c < NCH; ++c)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        float v = dbeta_acc[c][e];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
-        if (lane == 0) atomicAdd(dbeta_s + c * 32 + h * 8 + e, v);
-      }
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < C) part_b[(long long)blockIdx.x * C + tid] = dbeta_s[tid];
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
-  }
-}
-
-int launch_tc_bwd3(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* part_g,
-                   float* part_b, int* n_parts, long long n_pix, int inverse, cudaStream_t s) {
-  constexpr int C = 128;
-  using L = BwdFusedSmem;
-  CUtensorMap x_map, g_map, dx_map;
-  TFCB_TRY(make_tensor_map_2d(&x_map, x, n_pix, C, kTileM, 32, true));
-  TFCB_TRY(make_tensor_map_2d(&g_map, dy, n_pix, C, kTileM, 32, true));
-  TFCB_TRY(make_tensor_map_2d(&dx_map, dx, n_pix, C, kTileM, 32, true));
-  __nv_bfloat16* planes = nullptr;
-  TFCB_TRY(dev_alloc((void**)&planes, (size_t)4 * C * C * sizeof(__nv_bfloat16), s));
-  gdn_tc_prep2_kernel<true><<<((C / 8) * C + 255) / 256, 256, 0, s>>>(gamma, C, planes);
-  TFCB_LAUNCHED();
-  cudaError_t e = cudaFuncSetAttribute(gdn_tc_bwd3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kBytes);
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    dev_free(planes, s);
-    return fail(TFCB_CUDA_ERROR, "cannot reserve %d bytes of shared memory: %s", L::kBytes, cudaGetErrorString(e));
-  }
-  int dev = 0, sms = 148;
+int sm_count_tc() {
+  int dev = 0, n = 0;
   cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>(n_tiles, std::min(sms, 148));
-  int dbg = 0;  // timing experiments only (results are wrong with any bit set): 1 no MMA3, 4 no dgamma flushes
-  if (const char* env = getenv("TFCB_GDN_DBG")) dbg = atoi(env);
-  gdn_tc_bwd3_kernel<<<grid, kB3Threads, L::kBytes, s>>>(x_map, g_map, dx_map, x, dy, planes, beta, part_g, part_b, n_pix,
-                                                        inverse, dbg);
-  TFCB_LAUNCHED();
-  e = cudaGetLastError();
-  dev_free(planes, s);
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core backward launch failed: %s", cudaGetErrorString(e));
-  *n_parts = grid;
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 1;
+}
+
+template <typename Kern>
+int reserve_smem(Kern kernel, int bytes) {
+  TFCB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   return TFCB_OK;
 }
 
-// =============================================================================================
-// Backward, C = 192, first of the two kernels (dx and q), box-fed like gdn_tc_bwd3_kernel.
-//
-// n, dp and a dgamma accumulator need 3 x 192 TMEM columns and whole-tile p and q planes 198 KB of shared memory, so
-// C = 192 keeps the two-kernel split: this kernel produces dx and q = dL/dn, and gdn_tc_bwd_dgamma2_kernel contracts
-// x and q into dgamma / dbeta.  q travels through the workspace AS THE bf16 hi / lo OPERAND PLANES the second kernel
-// needs ([tile][hi, lo][24 groups][128 rows][8], 4 B/element like fp32): this kernel's q chunk buffers are bulk-stored
-// as they are, the second kernel bulk-loads a tile's planes with one copy and converts nothing.  Per 128-pixel tile:
-//
-//   conv(t)   x boxes -> p = |x| hi / lo planes, one 32-channel K chunk at a time (two chunk buffers)  -> MMA1  n += p_c . gamma_c
-//   pass2(t)  x (L2 hit), g boxes + n from TMEM -> q hi / lo planes of the chunk (also bulk-stored to the workspace)
-//                                                                                                      -> MMA2  dp += q_c . gammaT_c
-//             the direct term g / n (IGDN: g * n) goes back into n's columns with sign(x) in the two low mantissa bits
-//   pass3(t)  dx = direct + sign(x) * dp, from TMEM only -> output box -> TMA store
-//
-// gamma's hi plane is resident (72 KB; MMA2 reads it through the MN-major view); the lo planes of gamma (MMA1) and
-// gamma^T (MMA2) arrive as 12 KB K chunks, double buffered, from a "gamma" warp, and each chunk's two hi products are
-// issued before the one that needs the streamed chunk.  Chunk m of the stream uses operand buffer and gamma buffer
-// m % 2, so ONE commit per chunk frees both (a q chunk's buffer additionally waits for its bulk store to have read
-// it).  A ring of six 16 KB boxes serves every box request in program order.
-// TMEM: n | dp (2 x 192 columns).
-// =============================================================================================
-constexpr int kD2Compute = 512;
-constexpr int kD2Threads = kD2Compute + 128;   // + MMA-issue, box-copy, gamma and store warps
-constexpr int kD2Sync = kD2Compute + 32;
-constexpr int kD2Slots = 6;
-constexpr int kDKg = kTileM * 16;  // dense group stride of the operand planes (row-per-lane stores need no padding)
-
-struct BwdDx2Smem {
-  static constexpr int C = 192;
-  static constexpr int kGChunk = 4 * C * 16;                      // one 32-channel K chunk of one gamma plane (12 KB)
-  static constexpr int kOpPlane = 4 * kDKg;                       // hi or lo plane of one 32-channel operand chunk (8 KB)
-  static constexpr int kOffRing = 0;                              // [7] boxes (1024-byte aligned: swizzle atom)
-  static constexpr int kOffGh = kOffRing + kD2Slots * kF4Box;     // gamma hi plane [j / 8][i][8], resident
-  static constexpr int kOffG = kOffGh + C * C * 2;                // [2 buffers] lo K chunks of gamma / gamma^T
-  static constexpr int kOffOp = kOffG + 2 * kGChunk;              // [2 buffers][hi, lo] operand (p or q) chunks
-  static constexpr int kOffBeta = kOffOp + 4 * kOpPlane;
-  static constexpr int kOffBar = kOffBeta + C * 4;
-  // mbarriers: full[7], empty[7], yready[7], gfull[2], cfree[2], nfull, dpfull, qready[2], sfree[2]; then the TMEM slot
-  static constexpr int kBarFull = 0, kBarEmpty = 7, kBarY = 14, kBarGfull = 21, kBarCfree = 23, kBarN = 25, kBarDp = 26,
-                       kBarQready = 27, kBarSfree = 29, kNumBars = 31;
-  static constexpr int kBytes = kOffBar + kNumBars * 8 + 16;
-  static_assert(kOffGh % 128 == 0 && kOffG % 128 == 0 && kOffOp % 16 == 0 && kOffBar % 8 == 0, "alignment");
-  static_assert(kBytes <= 232448, "shared memory budget");
-};
-
-__global__ void __launch_bounds__(kD2Threads, 1)
-gdn_tc_bwd_dx2_kernel(const __grid_constant__ CUtensorMap x_map, const __grid_constant__ CUtensorMap g_map,
-                      const __grid_constant__ CUtensorMap dx_map, const float* __restrict__ x,
-                      const float* __restrict__ dy, const __nv_bfloat16* __restrict__ planes,
-                      const float* __restrict__ beta, uint8_t* __restrict__ q_planes, long long n_pix, int inverse) {
-  using L = BwdDx2Smem;
-  constexpr int C = L::C, NCH = C / 32;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* beta_s = reinterpret_cast<float*>(smem + L::kOffBeta);
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + L::kNumBars * 8);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 3, gwarp = warp & 3;  // compute thread (r, h): pixel row r, channel octet h of a box
-  auto bar = [&](int i) { return smem_u32(mbars + i); };
-  for (int i = tid; i < C; i += kD2Threads) beta_s[i] = beta[i];
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(planes);  // first plane: gamma hi, [j / 8][i][8]
-    uint4* dst = reinterpret_cast<uint4*>(smem + L::kOffGh);
-    for (int i = tid; i < C * C * 2 / 16; i += kD2Threads) dst[i] = src[i];
-  }
-  if (tid == 0) {
-    for (int i = 0; i < L::kNumBars; ++i) {
-      // y ready / q ready: one arrival per compute warp
-      const int count = ((i >= L::kBarY && i < L::kBarGfull) || (i >= L::kBarQready && i < L::kBarSfree)) ? kD2Compute / 32 : 1;
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar(i)), "r"(count));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_n = *tmem_slot, tmem_dp = tmem_n + C;
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
+template <int C, bool FAST, int IO>
+int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, TcFlags f,
+                  cudaStream_t s) {
+  using K = TcCfg<C>;
+  TFCB_TRY(reserve_smem(gdn_tc_fwd_kernel<C, FAST, IO>, K::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const long long first = blockIdx.x;
-  // Box request n uses ring slot n % 7 in its (n / 7)-th round:
-  //   6 x boxes (conversion of the CTA's first tile), then per tile {x, g} x 6 (pass 2), dx-out x 6 (pass 3),
-  //   (x of the next tile) x 6.
-  // Chunk m of the operand / gamma stream uses buffers m % 2: 6 conversion chunks of the first tile, then per tile 6 q
-  // chunks, 6 conversion chunks of the next tile.
-  constexpr int W0 = kD2Compute / 32;  // first auxiliary warp
-  auto slot_of = [](uint32_t n) { return n % (uint32_t)kD2Slots; };
-  auto round_of = [](uint32_t n) { return n / (uint32_t)kD2Slots; };
-
-  if (warp == W0 + 1) {
-    // ---------------------------------- box-copy warp ----------------------------------
-    if (lane == 0) {
-      uint32_t n = 0;
-      auto acquire = [&]() {
-        const uint32_t slot = slot_of(n), round = round_of(n);
-        if (round > 0) {
-          if (!mbar_wait(bar(L::kBarEmpty + slot), (round - 1u) & 1u)) __trap();
-        }
-        return slot;
-      };
-      auto load = [&](const CUtensorMap* map, int c, int row0) {
-        const uint32_t slot = acquire();
-        const uint32_t full = bar(L::kBarFull + slot);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "n"(kF4Box) : "memory");
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(
-                smem_u32(smem + L::kOffRing + slot * kF4Box)),
-            "l"(map), "r"(c * 32), "r"(row0), "r"(full), "l"(kEvictFirst)
-            : "memory");
-        ++n;
-      };
-      auto reserve = [&]() {  // output box: nothing to load, the slot only has to be free
-        const uint32_t slot = acquire();
-        asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarFull + slot)) : "memory");
-        ++n;
-      };
-      auto prefetch_tile = [&](const float* base, long long tile) {  // one contiguous block -> L2
-        const long long p0 = tile * kTileM;
-        const long long rows = min((long long)kTileM, n_pix - p0);
-        if (rows > 0)
-          asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(base + p0 * C),
-                       "r"((uint32_t)(rows * C * 4)), "l"(kEvictLast)
-                       : "memory");
-      };
-      if (first < n_tiles) {
-        prefetch_tile(x, first);
-        prefetch_tile(dy, first);
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) load(&x_map, c, (int)(first * kTileM));
-      }
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-        const long long next = tile + gridDim.x;
-        const bool has_next = next < n_tiles;
-        const int row0 = (int)(tile * kTileM);
-        if (has_next) {  // the next tile of this CTA -> L2: its boxes become L2 hits
-          prefetch_tile(x, next);
-          prefetch_tile(dy, next);
-        }
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) {
-          load(&x_map, c, row0);  // second read of x: an L2 hit
-          load(&g_map, c, row0);
-        }
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) reserve();  // dx out
-        if (has_next) {
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c) load(&x_map, c, (int)(next * kTileM));
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0 + 2) {
-    // ---------------------------------- gamma warp: K chunks of gamma / gamma^T ----------------------------------
-    if (lane == 0) {
-      const uint8_t* gp = reinterpret_cast<const uint8_t*>(planes);
-      constexpr size_t kPlaneBytes = (size_t)C * C * 2;
-      uint32_t m = 0;
-      auto chunk = [&](int transposed, int c) {
-        const uint32_t buf = m & 1u;
-        if (m >= 2) {  // the MMAs of chunk m - 2 (same buffers) have completed
-          if (!mbar_wait(bar(L::kBarCfree + buf), ((m >> 1) - 1u) & 1u)) __trap();
-        }
-        const uint32_t gfull = bar(L::kBarGfull + buf);
-        const uint32_t dst = smem_u32(smem + L::kOffG + buf * L::kGChunk);
-        const uint8_t* src = gp + (size_t)(2 * transposed + 1) * kPlaneBytes + (size_t)c * L::kGChunk;  // the lo plane
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(gfull), "n"(L::kGChunk) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-                     "l"(src), "n"(L::kGChunk), "r"(gfull), "l"(kEvictLast)
-                     : "memory");
-        ++m;
-      };
-      if (first < n_tiles) {
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) chunk(0, c);
-      }
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c) chunk(1, c);
-        if (tile + gridDim.x < n_tiles) {
-#pragma unroll 1
-          for (int c = 0; c < NCH; ++c) chunk(0, c);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0 + 3) {
-    // ---------------------------------- store warp: q planes and dx boxes ----------------------------------
-    if (lane == 0) {
-      uint32_t n = (first < n_tiles) ? (uint32_t)NCH : 0u;
-      uint32_t m = (first < n_tiles) ? (uint32_t)NCH : 0u;  // operand chunk counter (q chunks are stored, p chunks skipped)
-      uint32_t ypar = 0u;  // per-slot phase of the y-ready barrier (a slot is an output box only now and then)
-      uint32_t qcnt[2] = {0u, 0u};
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-        const bool has_next = tile + gridDim.x < n_tiles;
-        const int row0 = (int)(tile * kTileM);
-        uint8_t* qt = q_planes + (size_t)tile * (2 * (C / 8) * kDKg);  // this tile's [hi, lo][24][128][8] planes
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c, ++m) {
-          const uint32_t buf = m & 1u;
-          if (!mbar_wait(bar(L::kBarQready + buf), qcnt[buf] & 1u)) __trap();
-          ++qcnt[buf];
-          const uint32_t src = smem_u32(smem + L::kOffOp + buf * 2 * L::kOpPlane);
-#pragma unroll
-          for (int pl = 0; pl < 2; ++pl)
-            asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(
-                             qt + (size_t)pl * ((C / 8) * kDKg) + (size_t)c * L::kOpPlane),
-                         "r"(src + pl * L::kOpPlane), "n"(L::kOpPlane), "l"(kEvictLast)
-                         : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the buffer has been read
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarSfree + buf)) : "memory");
-        }
-        n += 2 * NCH;  // x and g boxes of pass 2
-#pragma unroll 1
-        for (int c = 0; c < NCH; ++c, ++n) {
-          const uint32_t slot = slot_of(n);
-          if (!mbar_wait(bar(L::kBarY + slot), (ypar >> slot) & 1u)) __trap();
-          ypar ^= 1u << slot;
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2}], [%3], %4;" ::"l"(&dx_map),
-                       "r"(c * 32), "r"(row0), "r"(smem_u32(smem + L::kOffRing + slot * kF4Box)), "l"(kEvictFirst)
-                       : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the box has been read: the slot is free
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarEmpty + slot)) : "memory");
-        }
-        if (has_next) {
-          n += NCH;
-          m += NCH;
-        }
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-    __syncwarp();
-  } else if (warp == W0) {
-    // ------------------------------- MMA-issue warp: MMA1, MMA2 (K-chunked, everything streamed) -------------------
-    constexpr uint32_t kIdesc = umma_idesc(kTileM, C);  // A, B both K-major
-    uint32_t n = 0, m = 0;
-    constexpr uint32_t kIdescT = umma_idesc(kTileM, C) | (1u << 16);  // B = resident gamma hi read transposed (MMA2)
-    const uint32_t gh = smem_u32(smem + L::kOffGh);
-    // Six MMAs of chunk m (K chunk c of the tile): the four that only need the resident hi plane first, then the two
-    // against the streamed lo chunk.  MMA1: B = gamma[j in chunk, :] (K-major); MMA2: B = gamma[:, i in chunk]^T, the
-    // same plane through the MN-major view (hi) / the gamma^T lo chunk (K-major).
-    auto chunk_mmas = [&](uint32_t acc, int c, bool transposed) {
-      const uint32_t buf = m & 1u;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_hi = smem_u32(smem + L::kOffOp + buf * 2 * L::kOpPlane), a_lo = a_hi + L::kOpPlane;
-      const uint32_t g_lo = smem_u32(smem + L::kOffG + buf * L::kGChunk);
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        const uint64_t dah = umma_desc(a_hi + (uint32_t)(2 * s2) * kDKg, kDKg, 128);
-        const uint64_t dal = umma_desc(a_lo + (uint32_t)(2 * s2) * kDKg, kDKg, 128);
-        const uint64_t dbh = transposed ? umma_desc(gh + (uint32_t)(c * 32 + s2 * 16) * 16u, 128, C * 16)
-                                        : umma_desc(gh + (uint32_t)(c * 4 + 2 * s2) * (C * 16), C * 16, 128);
-        const uint32_t idesc = transposed ? kIdescT : kIdesc;
-        umma_bf16(acc, dah, dbh, idesc, (c == 0 && s2 == 0) ? 0u : 1u);
-        umma_bf16(acc, dal, dbh, idesc, 1u);
-      }
-      if (!mbar_wait(bar(L::kBarGfull + buf), (m >> 1) & 1u)) __trap();
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        const uint64_t dah = umma_desc(a_hi + (uint32_t)(2 * s2) * kDKg, kDKg, 128);
-        const uint64_t dbl = umma_desc(g_lo + (uint32_t)(2 * s2) * (C * 16), C * 16, 128);
-        umma_bf16(acc, dah, dbl, kIdesc, 1u);
-      }
-      umma_commit(bar(L::kBarCfree + buf));
-      ++m;
-    };
-    auto release = [&](uint32_t req) {
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarEmpty + slot_of(req))) : "memory");
-    };
-    auto mma1_tile = [&]() {
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, ++n) {
-        asm volatile("bar.sync %0, %1;" ::"r"(2 + (int)(m & 1u)), "n"(kD2Sync) : "memory");  // p planes of this chunk are written
-        if (lane == 0) {
-          release(n);
-          chunk_mmas(tmem_n, c, false);
-          if (c == NCH - 1) umma_commit(bar(L::kBarN));
-        } else {
-          ++m;
-        }
-        m = __shfl_sync(0xFFFFFFFFu, m, 0);
-      }
-    };
-    if (first < n_tiles) mma1_tile();
-    for (long long tile = first; tile < n_tiles; tile += gridDim.x) {
-      const bool has_next = tile + gridDim.x < n_tiles;
-#pragma unroll 1
-      for (int c = 0; c < NCH; ++c, n += 2) {
-        asm volatile("bar.sync %0, %1;" ::"r"(4 + (int)(m & 1u)), "n"(kD2Sync) : "memory");  // q planes of this chunk are written
-        if (lane == 0) {
-          release(n);      // x box
-          release(n + 1);  // g box
-          chunk_mmas(tmem_dp, c, true);
-          if (c == NCH - 1) umma_commit(bar(L::kBarDp));  // dp is complete: the dx pass may start
-        } else {
-          ++m;
-        }
-        m = __shfl_sync(0xFFFFFFFFu, m, 0);
-      }
-      n += NCH;  // dx-out boxes
-      if (has_next) mma1_tile();
-    }
-  } else if (warp < W0) {
-  // --------------------------------- compute warps ---------------------------------
-  uint32_t n = 0, m = 0;
-  // 128-byte swizzle: the 16-byte chunk j of box row `row` sits at chunk j ^ (row & 7)
-  auto chunk_at = [](uint8_t* box, int row, int j) { return reinterpret_cast<float4*>(box + row * 128 + ((j ^ (row & 7)) << 4)); };
-  auto wait_full = [&](uint32_t req) {
-    if (!mbar_wait(bar(L::kBarFull + slot_of(req)), round_of(req) & 1u)) __trap();
-    return smem + L::kOffRing + slot_of(req) * kF4Box;
-  };
-  // this thread's 16-byte rows of the hi / lo planes of operand chunk m: waits until the MMAs of chunk m - 2 are done
-  // and, if that chunk was a q chunk, until its bulk store has read the buffer
-  uint32_t scnt[2] = {0u, 0u};
-  auto operand_rows = [&](uint4** hi, uint4** lo, bool prev_was_q) {
-    const uint32_t buf = m & 1u;
-    if (m >= 2) {
-      if (!mbar_wait(bar(L::kBarCfree + buf), ((m >> 1) - 1u) & 1u)) __trap();
-    }
-    if (prev_was_q) {
-      if (!mbar_wait(bar(L::kBarSfree + buf), scnt[buf] & 1u)) __trap();
-      ++scnt[buf];
-    }
-    uint8_t* base = smem + L::kOffOp + buf * 2 * L::kOpPlane + h * kDKg + r * 16;
-    *hi = reinterpret_cast<uint4*>(base);
-    *lo = reinterpret_cast<uint4*>(base + L::kOpPlane);
-  };
-
-  auto conv_tile = [&](bool after_pass2) {
-#pragma unroll 1
-    for (int c = 0; c < NCH; ++c, ++n) {
-      uint8_t* box = wait_full(n);
-      const float4 a = *chunk_at(box, r, 2 * h), b = *chunk_at(box, r, 2 * h + 1);
-      float v[8] = {fabsf(a.x), fabsf(a.y), fabsf(a.z), fabsf(a.w), fabsf(b.x), fabsf(b.y), fabsf(b.z), fabsf(b.w)};
-      uint4 hi, lo, *ph, *pl;
-      split8(v, &hi, &lo);
-      operand_rows(&ph, &pl, after_pass2 && c < 2);  // chunks 0, 1 reuse the buffers of the tile's last two q chunks
-      *ph = hi;
-      *pl = lo;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(2 + (int)(m & 1u)), "n"(kD2Sync) : "memory");  // (also releases the box, see issue warp)
-      ++m;
-    }
-  };
-
-  if (first < n_tiles) conv_tile(false);
-  int t = 0;
-  for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-    const bool has_next = tile + gridDim.x < n_tiles;
-    if (!mbar_wait(bar(L::kBarN), (uint32_t)t & 1u)) __trap();  // MMA1 of this tile has completed
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    // ---- pass 2: q = dL/dn -> output box + q planes; the direct term and sign(x) go back into n's columns ----
-#pragma unroll 1
-    for (int c = 0; c < NCH; ++c, n += 2) {
-      const uint32_t col = tmem_n + lane_sel + (uint32_t)(c * 32 + h * 8);
-      uint32_t nacc[8];
-      tmem_load<8>(col, nacc);
-      uint8_t* bx = wait_full(n);
-      uint8_t* bg = wait_full(n + 1);
-      const float4 x0 = *chunk_at(bx, r, 2 * h), x1 = *chunk_at(bx, r, 2 * h + 1);
-      const float4 g0 = *chunk_at(bg, r, 2 * h), g1 = *chunk_at(bg, r, 2 * h + 1);
-      const float4 bv0 = *reinterpret_cast<const float4*>(beta_s + c * 32 + h * 8);      // same address in every lane
-      const float4 bv1 = *reinterpret_cast<const float4*>(beta_s + c * 32 + h * 8 + 4);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const float xs[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-      const float gs[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      const float bs[8] = {bv0.x, bv0.y, bv0.z, bv0.w, bv1.x, bv1.y, bv1.z, bv1.w};
-      float q[8];
-      uint32_t dbits[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float nn = bs[e] + __uint_as_float(nacc[e]);
-        float direct;
-        if (inverse) {
-          direct = gs[e] * nn;
-          q[e] = gs[e] * xs[e];
-        } else {
-          const float rn = rcp_approx(nn);
-          direct = gs[e] * rn;
-          q[e] = -gs[e] * xs[e] * rn * rn;
-        }
-        const uint32_t code = (xs[e] > 0.f) ? 1u : ((xs[e] < 0.f) ? 2u : 0u);
-        dbits[e] = (__float_as_uint(direct) & ~3u) | code;
-      }
-      uint4 hi, lo, *qh, *ql;
-      split8(q, &hi, &lo);
-      operand_rows(&qh, &ql, c >= 2);
-      *qh = hi;
-      *ql = lo;
-      tmem_store8(col, dbits);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // q planes -> MMA and -> bulk store
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      asm volatile("bar.arrive %0, %1;" ::"r"(4 + (int)(m & 1u)), "n"(kD2Sync) : "memory");  // (also releases the x and g boxes)
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarQready + (m & 1u))) : "memory");
-      ++m;
-    }
-    // ---- pass 3: dx = direct + sign(x) * dp, from TMEM only ----
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");  // this thread's direct terms are in TMEM
-    if (!mbar_wait(bar(L::kBarDp), (uint32_t)t & 1u)) __trap();  // every MMA2 of this tile has completed
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c = 0; c < NCH; ++c, ++n) {
-      uint32_t d[8], p[8];
-      tmem_load<8>(tmem_n + lane_sel + (uint32_t)(c * 32 + h * 8), d);
-      tmem_load<8>(tmem_dp + lane_sel + (uint32_t)(c * 32 + h * 8), p);
-      uint8_t* box = wait_full(n);  // the slot's previous user has left
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      float o[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const uint32_t code = d[e] & 3u;
-        const float s = (code == 1u) ? 1.f : ((code == 2u) ? -1.f : 0.f);
-        o[e] = fmaf(s, __uint_as_float(p[e]), __uint_as_float(d[e]));
-      }
-      *chunk_at(box, r, 2 * h) = make_float4(o[0], o[1], o[2], o[3]);
-      *chunk_at(box, r, 2 * h + 1) = make_float4(o[4], o[5], o[6], o[7]);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // dx box -> TMA store
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarY + slot_of(n))) : "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // TMEM reads precede the next tile's MMAs
-    if (has_next) conv_tile(true);
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
-  }
-}
-
-// =============================================================================================
-// Backward, C = 192, second kernel: dgamma += p^T q, dbeta += column sums of q, box-fed.
-//
-// Per 128-pixel tile: the tile's q hi / lo planes arrive from the workspace with ONE bulk copy (96 KB, written in
-// exactly this layout by gdn_tc_bwd_dx2_kernel); the x tile (six TMA boxes, 96 KB) lands IN THE MEMORY OF THE p PLANES
-// (same size), every compute thread (r, h) takes its 48 values into registers, and after a barrier the p = |x| hi / lo
-// planes are written over the boxes; 48 MMAs (two overlapping M = 128 row blocks [0,128) and [64,192) of p^T, N = 192,
-// K = 128 pixels) accumulate into TMEM.  Nothing is double buffered (4 x 48 KB of planes): a tile costs one load
-// latency + the conversion + the MMAs.  dbeta comes from the planes (q = hi + lo to 2^-17): warp w sums 8-channel
-// groups w and w + 16, lane = pixel row mod 32.  The accumulator is flushed every kDgFlush tiles (CTAs take turns),
-// transposed through the dead p planes one row block at a time into coalesced L2 adds.
-// =============================================================================================
-constexpr int kG2Compute = 512;
-constexpr int kG2Threads = kG2Compute + 64;   // + MMA-issue and copy warps
-constexpr int kG2Sync = kG2Compute + 32;
-
-struct BwdDg2Smem {
-  static constexpr int C = 192;
-  static constexpr int kPlane = (C / 8) * kDKg;          // 49 152: one whole-K plane, dense groups
-  static constexpr int kOffPh = 0;                       // p hi, lo: also the landing area of the six x boxes
-  static constexpr int kOffPl = kOffPh + kPlane;
-  static constexpr int kOffQh = kOffPl + kPlane;         // q hi, lo contiguous: one bulk copy per tile
-  static constexpr int kOffQl = kOffQh + kPlane;
-  static constexpr int kOffDbeta = kOffQl + kPlane;
-  static constexpr int kOffBar = kOffDbeta + C * 4;
-  // mbarriers: xfull, pfree, qfull, qdone, m3done; then the TMEM slot
-  static constexpr int kBarXfull = 0, kBarPfree = 1, kBarQfull = 2, kBarQdone = 3, kBarM3 = 4, kNumBars = 5;
-  static constexpr int kBytes = kOffBar + kNumBars * 8 + 16;
-  static_assert(kBytes <= 232448, "shared memory budget");
-  static_assert(2 * kPlane == 6 * kF4Box && 2 * kPlane >= kTileM * C * 4, "x tile / flush staging fit in the p planes");
-};
-
-__global__ void __launch_bounds__(kG2Threads, 1)
-gdn_tc_bwd_dgamma2_kernel(const __grid_constant__ CUtensorMap x_map, const float* __restrict__ x,
-                          const uint8_t* __restrict__ q_planes, float* __restrict__ part_g, float* __restrict__ part_b,
-                          long long n_pix) {
-  using L = BwdDg2Smem;
-  constexpr int C = L::C, NCH = C / 32;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* dbeta_s = reinterpret_cast<float*>(smem + L::kOffDbeta);
-  uint64_t* mbars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::kOffBar + L::kNumBars * 8);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int r = tid & 127, h = (tid >> 7) & 3, gwarp = warp & 3;
-  auto bar = [&](int i) { return smem_u32(mbars + i); };
-  for (int i = tid; i < C; i += kG2Threads) dbeta_s[i] = 0.f;
-  if (tid == 0) {
-    for (int i = 0; i < L::kNumBars; ++i) {
-      const int count = (i == L::kBarQdone || i == L::kBarPfree) ? kG2Compute / 32 : 1;
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar(i)), "r"(count));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (tid < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_a = *tmem_slot, tmem_b = tmem_a + C;  // rows j in [0,128) | rows j in [64,192)
-  const uint32_t lane_sel = (uint32_t)(gwarp * 32) << 16;
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const long long first = blockIdx.x;
-  const int fphase = (int)(blockIdx.x % kDgFlush);
-  constexpr int W0 = kG2Compute / 32;
-
-  if (warp == W0 + 1) {
-    // ---------------------------------- copy warp: q planes and the x tile ----------------------------------
-    if (lane == 0) {
-      int t = 0;
-      for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-        const long long next = tile + gridDim.x;
-        if (next < n_tiles) {  // the next tile of this CTA -> L2
-          const long long p0 = next * kTileM;
-          const long long rows = min((long long)kTileM, n_pix - p0);
-          asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(x + p0 * C),
-                       "r"((uint32_t)(rows * C * 4)), "l"(kEvictLast)
-                       : "memory");
-          asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(q_planes + (size_t)next * (2 * L::kPlane)),
-                       "n"(2 * L::kPlane), "l"(kEvictLast)
-                       : "memory");
-        }
-        if (t > 0) {  // the q planes are free once the previous tile's MMAs and dbeta reads are done
-          if (!mbar_wait(bar(L::kBarM3), (uint32_t)(t - 1) & 1u)) __trap();
-          if (!mbar_wait(bar(L::kBarQdone), (uint32_t)(t - 1) & 1u)) __trap();
-        }
-        const uint32_t qfull = bar(L::kBarQfull);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(qfull), "n"(2 * L::kPlane) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                         smem_u32(smem + L::kOffQh)),
-                     "l"(q_planes + (size_t)tile * (2 * L::kPlane)), "n"(2 * L::kPlane), "r"(qfull), "l"(kEvictFirst)
-                     : "memory");
-        // the p planes are free once the compute warps say so (previous MMAs done, flush staging consumed)
-        if (!mbar_wait(bar(L::kBarPfree), (uint32_t)t & 1u)) __trap();
-        const uint32_t xfull = bar(L::kBarXfull);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(xfull), "n"(6 * kF4Box) : "memory");
-        // ONE 3-D box: all six [128 x 32] boxes of the tile, back to back (a copy instruction costs the SM's copy
-        // engine ~0.35 us whatever its size, tools/tma_probe.py)
-        asm volatile(
-            "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4}], [%5], %6;" ::"r"(
-                smem_u32(smem + L::kOffPh)),
-            "l"(&x_map), "r"(0), "r"((int)(tile * kTileM)), "r"(0), "r"(xfull), "l"(kEvictFirst)
-            : "memory");
-      }
-    }
-    __syncwarp();
-  } else if (warp == W0) {
-    // ------------------------------- MMA-issue warp -------------------------------
-    constexpr uint32_t kIdesc = umma_idesc(kTileM, C) | (1u << 15) | (1u << 16);  // A = p^T, B = q, both MN-major views
-    const uint32_t p_hi = smem_u32(smem + L::kOffPh), p_lo = smem_u32(smem + L::kOffPl);
-    const uint32_t q_hi = smem_u32(smem + L::kOffQh), q_lo = smem_u32(smem + L::kOffQl);
-    int t = 0;
-    for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-      asm volatile("bar.sync 2, %0;" ::"n"(kG2Sync) : "memory");  // the p planes are written
-      if (lane == 0) {
-        if (!mbar_wait(bar(L::kBarQfull), (uint32_t)t & 1u)) __trap();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const bool restart = (t == 0) || (((t + fphase) % kDgFlush) == 0);
-#pragma unroll 1
-        for (int blk = 0; blk < 2; ++blk) {
-          const uint32_t moff = (uint32_t)(blk * 8) * kDKg;  // second block starts at channel 64 = m group 8
-          const uint32_t td = blk ? tmem_b : tmem_a;
-#pragma unroll
-          for (int s = 0; s < kTileM / 16; ++s) {
-            const uint32_t koff = (uint32_t)(s * 16) * 16u;
-            const uint64_t dah = umma_desc(p_hi + moff + koff, 128, kDKg);
-            const uint64_t dal = umma_desc(p_lo + moff + koff, 128, kDKg);
-            const uint64_t dbh = umma_desc(q_hi + koff, 128, kDKg);
-            const uint64_t dbl = umma_desc(q_lo + koff, 128, kDKg);
-            umma_bf16(td, dah, dbh, kIdesc, (restart && s == 0) ? 0u : 1u);
-            umma_bf16(td, dal, dbh, kIdesc, 1u);
-            umma_bf16(td, dah, dbl, kIdesc, 1u);
-          }
-        }
-        umma_commit(bar(L::kBarM3));
-      }
-      __syncwarp();
-    }
-  } else if (warp < W0) {
-  // --------------------------------- compute warps ---------------------------------
-  float dbeta_acc[2][8];  // 8-channel groups warp and warp + 16, summed over rows lane, lane + 32, ...
-#pragma unroll
-  for (int k = 0; k < 2; ++k)
-#pragma unroll
-    for (int e = 0; e < 8; ++e) dbeta_acc[k][e] = 0.f;
-  auto chunk_at = [](uint8_t* box, int row, int j) { return reinterpret_cast<float4*>(box + row * 128 + ((j ^ (row & 7)) << 4)); };
-  bool flushed = false;
-  // one row block of the accumulator (lane r = row, 48 columns per thread) -> swizzled [128][192] fp32 staging in
-  // the dead p planes -> 768 contiguous bytes per row added to the CTA's partial
-  auto flush_dgamma = [&]() {
-    uint8_t* stage = smem + L::kOffPh;
-#pragma unroll 1
-    for (int blk = 0; blk < 2; ++blk) {
-#pragma unroll
-      for (int cb = 0; cb < 3; ++cb) {
-        uint32_t a[16];
-        tmem_load<16>((blk ? tmem_b : tmem_a) + lane_sel + (uint32_t)(h * 48 + cb * 16), a);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          *reinterpret_cast<uint4*>(stage + r * 768 + (((h * 12 + cb * 4 + i) ^ (r & 7)) << 4)) =
-              make_uint4(a[4 * i], a[4 * i + 1], a[4 * i + 2], a[4 * i + 3]);
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(kG2Compute) : "memory");
-      float* pg = part_g + (long long)blockIdx.x * C * C + (long long)(blk * 64) * C;  // block b: lane r = channel 64 + r
-#pragma unroll 1
-      for (int it = 0; it < (kTileM * C / 4) / kG2Compute; ++it) {
-        const int item = it * kG2Compute + tid, row = item / 48, u = item % 48;
-        if (blk && row < 64) continue;  // rows [64,128) of block b repeat block a's
-        const uint4 v = *reinterpret_cast<const uint4*>(stage + row * 768 + ((u ^ (row & 7)) << 4));
-        float* dst = pg + row * C + u * 4;
-        if (!flushed)
-          asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-        else
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(kG2Compute) : "memory");  // the staging is rewritten (next block / the x tile)
-    }
-    flushed = true;
-  };
-
-  int t = 0;
-  for (long long tile = first; tile < n_tiles; tile += gridDim.x, ++t) {
-    if (t > 0) {  // the previous tile's MMAs have completed: the p planes are dead, the accumulator is up to date
-      if (!mbar_wait(bar(L::kBarM3), (uint32_t)(t - 1) & 1u)) __trap();
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (((t - 1 + fphase) % kDgFlush) == kDgFlush - 1) flush_dgamma();
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic accesses of the p planes precede the TMA writes
-    __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarPfree)) : "memory");
-    // the x tile has landed in the p planes: take this thread's 48 values, then overwrite the boxes with the planes
-    if (!mbar_wait(bar(L::kBarXfull), (uint32_t)t & 1u)) __trap();
-    float4 xa[NCH], xb[NCH];
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      uint8_t* box = smem + L::kOffPh + c * kF4Box;
-      xa[c] = *chunk_at(box, r, 2 * h);
-      xb[c] = *chunk_at(box, r, 2 * h + 1);
-    }
-    asm volatile("bar.sync 1, %0;" ::"n"(kG2Compute) : "memory");  // every thread holds its values
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      float v[8] = {fabsf(xa[c].x), fabsf(xa[c].y), fabsf(xa[c].z), fabsf(xa[c].w),
-                    fabsf(xb[c].x), fabsf(xb[c].y), fabsf(xb[c].z), fabsf(xb[c].w)};
-      uint4 hi, lo;
-      split8(v, &hi, &lo);
-      *reinterpret_cast<uint4*>(smem + L::kOffPh + (4 * c + h) * kDKg + r * 16) = hi;
-      *reinterpret_cast<uint4*>(smem + L::kOffPl + (4 * c + h) * kDKg + r * 16) = lo;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    asm volatile("bar.arrive 2, %0;" ::"n"(kG2Sync) : "memory");
-    // dbeta from the q planes (q = hi + lo to 2^-17 relative): groups warp and warp + 16, rows lane + 32 k
-    if (!mbar_wait(bar(L::kBarQfull), (uint32_t)t & 1u)) __trap();
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const int grp = warp + 16 * k;
-      if (grp < C / 8) {
-#pragma unroll
-        for (int rq = 0; rq < 4; ++rq) {
-          const int row = lane + 32 * rq;
-          const uint4 qh = *reinterpret_cast<const uint4*>(smem + L::kOffQh + grp * kDKg + row * 16);
-          const uint4 ql = *reinterpret_cast<const uint4*>(smem + L::kOffQl + grp * kDKg + row * 16);
-          const uint32_t wh[4] = {qh.x, qh.y, qh.z, qh.w}, wl[4] = {ql.x, ql.y, ql.z, ql.w};
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            dbeta_acc[k][2 * i] += __uint_as_float(wh[i] << 16) + __uint_as_float(wl[i] << 16);
-            dbeta_acc[k][2 * i + 1] += __uint_as_float(wh[i] & 0xFFFF0000u) + __uint_as_float(wl[i] & 0xFFFF0000u);
-          }
-        }
-      }
-    }
-    __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar(L::kBarQdone)) : "memory");
-  }
-  if (t > 0) {
-    if (!mbar_wait(bar(L::kBarM3), (uint32_t)(t - 1) & 1u)) __trap();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    flush_dgamma();  // the tiles since the last restart (a turn that falls on the last tile is flushed here as well)
-#pragma unroll
-    for (int k = 0; k < 2; ++k)
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        float v = dbeta_acc[k][e];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
-        const int grp = warp + 16 * k;
-        if (lane == 0 && grp < C / 8) dbeta_s[grp * 8 + e] = v;  // one warp per group: no atomics
-      }
-  }
-  }  // compute warps
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  for (int i = tid; i < C; i += kG2Threads) part_b[(long long)blockIdx.x * C + i] = dbeta_s[i];
-  if (tid < 32) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_slot), "n"(512));
-  }
-}
-
-template <bool FAST>
-int launch_tc_bwd192(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                     float* part_g, float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
-  constexpr int C = 192;
-  __nv_bfloat16* planes = nullptr;
-  TFCB_TRY(dev_alloc((void**)&planes, (size_t)2 * C * C * sizeof(__nv_bfloat16), s));
-  gdn_tc_prep_kernel<<<((C / 8) * C + 255) / 256, 256, 0, s>>>(gamma, C, planes);
+  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sm_count_tc());
+  gdn_tc_fwd_kernel<C, FAST, IO><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
   TFCB_LAUNCHED();
-  bool attr_set = false;  // the attribute is per device: set it on every launch (microseconds)
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gdn_tc_bwd_dx_kernel<C, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Bwd2Smem<C>::kBytes);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gdn_tc_bwd_dgamma_kernel<C, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               Bwd3Smem<C>::kBytes);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      dev_free(planes, s);
-      return fail(TFCB_CUDA_ERROR, "cannot reserve shared memory for the C=192 backward: %s", cudaGetErrorString(e));
-    }
-    attr_set = true;
-  }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>(n_tiles, std::min(sms, 148));
-  const char* v1 = getenv("TFCB_GDN_BWD_V1");  // A/B timing: the register-fed kernels
-  if (FAST && n_pix < (1ll << 31) && !(v1 && v1[0] == '1')) {
-    // box-fed pair: q travels as bf16 hi / lo planes ([tile][2][24][128][8], 4 B/element; the workspace is sized in
-    // whole tiles, tfcb_gdn_backward_workspace_bytes)
-    using L2 = BwdDx2Smem;
-    using L3 = BwdDg2Smem;
-    CUtensorMap x_map, g_map, dx_map;
-    __nv_bfloat16* planes4 = nullptr;
-    int rc = make_tensor_map_2d(&x_map, x, n_pix, C, kTileM, 32, true);
-    if (rc == TFCB_OK) rc = make_tensor_map_2d(&g_map, dy, n_pix, C, kTileM, 32, true);
-    if (rc == TFCB_OK) rc = make_tensor_map_2d(&dx_map, dx, n_pix, C, kTileM, 32, true);
-    if (rc == TFCB_OK) rc = dev_alloc((void**)&planes4, (size_t)4 * C * C * sizeof(__nv_bfloat16), s);
-    if (rc == TFCB_OK && (cudaFuncSetAttribute(gdn_tc_bwd_dx2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L2::kBytes) != cudaSuccess ||
-                          cudaFuncSetAttribute(gdn_tc_bwd_dgamma2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3::kBytes) != cudaSuccess)) {
-      (void)cudaGetLastError();
-      rc = fail(TFCB_CUDA_ERROR, "cannot reserve shared memory for the C=192 backward");
-    }
-    if (rc != TFCB_OK) {
-      dev_free(planes4, s);
-      dev_free(planes, s);
-      return rc;
-    }
-    gdn_tc_prep2_kernel<false><<<((C / 8) * C + 255) / 256, 256, 0, s>>>(gamma, C, planes4);
-    TFCB_LAUNCHED();
-    gdn_tc_bwd_dx2_kernel<<<grid, kD2Threads, L2::kBytes, s>>>(x_map, g_map, dx_map, x, dy, planes4, beta,
-                                                              reinterpret_cast<uint8_t*>(q_ws), n_pix, f.inverse);
-    TFCB_LAUNCHED();
-    CUtensorMap x_map3;  // the whole [128 x 192] x tile as one 3-D box
-    rc = make_tensor_map_3d(&x_map3, x, n_pix, C, kTileM, C / 32);
-    if (rc != TFCB_OK) {
-      dev_free(planes4, s);
-      dev_free(planes, s);
-      return rc;
-    }
-    gdn_tc_bwd_dgamma2_kernel<<<grid, kG2Threads, L3::kBytes, s>>>(x_map3, x, reinterpret_cast<const uint8_t*>(q_ws), part_g,
-                                                                   part_b, n_pix);
-    TFCB_LAUNCHED();
-    cudaError_t e2 = cudaGetLastError();
-    dev_free(planes4, s);
-    dev_free(planes, s);
-    if (e2 != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core backward (C=192) launch failed: %s", cudaGetErrorString(e2));
-    *n_parts = grid;
-    return TFCB_OK;
-  }
-  gdn_tc_bwd_dx_kernel<C, FAST><<<grid, kBwdThreads, Bwd2Smem<C>::kBytes, s>>>(x, dy, planes, beta, dx, q_ws, n_pix, f);
-  TFCB_LAUNCHED();
-  gdn_tc_bwd_dgamma_kernel<C, FAST><<<grid, kBwdThreads, Bwd3Smem<C>::kBytes, s>>>(x, q_ws, part_g, part_b, n_pix, f);
-  TFCB_LAUNCHED();
-  cudaError_t e = cudaGetLastError();
-  dev_free(planes, s);
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core backward (C=192) launch failed: %s", cudaGetErrorString(e));
-  *n_parts = grid;
+  TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
 }
 
-template <bool FAST>
-int launch_tc_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* part_g,
-                  float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
-  constexpr int C = 128;
-  using L = BwdSmem<C>;
-  __nv_bfloat16* planes = nullptr;
-  TFCB_TRY(dev_alloc((void**)&planes, (size_t)2 * C * C * sizeof(__nv_bfloat16), s));
-  gdn_tc_prep_kernel<<<((C / 8) * C + 255) / 256, 256, 0, s>>>(gamma, C, planes);
-  TFCB_LAUNCHED();
-  bool attr_set = false;  // the attribute is per device: set it on every launch (microseconds)
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gdn_tc_bwd_kernel<C, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::kBytes);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      dev_free(planes, s);
-      return fail(TFCB_CUDA_ERROR, "cannot reserve %d bytes of shared memory: %s", L::kBytes, cudaGetErrorString(e));
-    }
-    attr_set = true;
-  }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+template <int C, bool FAST>
+int launch_tc_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
+                  float* part_g, float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
+  using K = TcCfg<C>;
+  using L = DgCfg<C>;
+  TFCB_TRY(reserve_smem(gdn_tc_bwd_dx_kernel<C, FAST>, K::kSmem));
+  TFCB_TRY(reserve_smem(gdn_tc_dgamma_kernel<C, FAST>, L::kSmem));
+  const int sms = sm_count_tc();
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>(n_tiles, std::min(sms, 148));
-  gdn_tc_bwd_kernel<C, FAST><<<grid, kBwdThreads, L::kBytes, s>>>(x, dy, planes, beta, dx, part_g, part_b, n_pix, f);
+  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sms);
+  gdn_tc_bwd_dx_kernel<C, FAST><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
   TFCB_LAUNCHED();
-  cudaError_t e = cudaGetLastError();
-  dev_free(planes, s);
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "GDN tensor-core backward launch failed: %s", cudaGetErrorString(e));
-  *n_parts = grid;
+  const int grid_g = (int)std::min<long long>(n_tiles, std::min(sms, kMaxParts));
+  gdn_tc_dgamma_kernel<C, FAST><<<grid_g, L::kThreads, L::kSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  *n_parts = grid_g;
   return TFCB_OK;
+}
+
+// Which configurations have a tensor-core kernel; fills *f.
+bool tc_config(int C, int flags, float alpha, float eps, TcFlags* f) {
+  if (!(C == 128 || C == 192)) return false;
+  if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return false;
+  if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return false;  // trainable exponents: literal pow
+  if (const char* env = getenv("TFCB_GDN_FP32")) {
+    if (env[0] == '1') return false;  // debugging aid: force the CUDA-core kernels
+  }
+  f->inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
+  f->rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
+  f->alpha_mode = (alpha == 2.f) ? 2 : 1;
+  f->eps_mode = (eps == 0.5f) ? 2 : 1;
+  return true;
+}
+
+bool tc_fast(const TcFlags& f) { return f.alpha_mode == 1 && f.eps_mode == 1 && !f.rectify; }
+
+bool misaligned(const void* a, const void* b, const void* c) {
+  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) != 0;
 }
 
 }  // namespace
@@ -3201,83 +564,49 @@ int launch_tc_bwd(const float* x, const float* gamma, const float* beta, const f
 int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
                    int flags, float alpha, float eps, cudaStream_t s, bool* handled) {
   *handled = false;
-  if (!(C == 128 || C == 192)) return TFCB_OK;
-  if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return TFCB_OK;
-  if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return TFCB_OK;  // trainable exponents: literal pow
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(beta)) & 15) return TFCB_OK;  // 16-byte rows
-  if (const char* env = getenv("TFCB_GDN_FP32")) {
-    if (env[0] == '1') return TFCB_OK;  // debugging aid: force the CUDA-core kernels
-  }
   TcFlags f;
-  f.inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
-  f.rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
-  f.alpha_mode = (alpha == 2.f) ? 2 : 1;
-  f.eps_mode = (eps == 0.5f) ? 2 : 1;
+  if (misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
-  const bool fast = (alpha == 1.f) && (eps == 1.f) && !f.rectify;
-  if (C == 128)  // x tile resident in shared memory, bulk async copies
-    return fast ? launch_tc_fwd2<true, 0>(x, gamma, beta, y, n_pix, f, s) : launch_tc_fwd2<false, 0>(x, gamma, beta, y, n_pix, f, s);
-  // C == 192: x through rings of 2-D TMA boxes, gamma's lo plane streamed, y through TMA stores
-  if (n_pix >= (1ll << 31)) return fail(TFCB_INVALID_ARGUMENT, "GDN: more than 2^31 pixels in one call");
-  return fast ? launch_tc_fwd4<true>(x, gamma, beta, y, n_pix, f, s) : launch_tc_fwd4<false>(x, gamma, beta, y, n_pix, f, s);
+  const bool fast = tc_fast(f);
+  if (C == 128)
+    return fast ? launch_tc_fwd<128, true, 0>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_fwd<128, false, 0>(x, gamma, beta, y, n_pix, f, s);
+  return fast ? launch_tc_fwd<192, true, 0>(x, gamma, beta, y, n_pix, f, s)
+              : launch_tc_fwd<192, false, 0>(x, gamma, beta, y, n_pix, f, s);
 }
 
-// 16-bit activations (float16 / bfloat16 in, same type out; parameters and arithmetic float32): the C = 128 resident
-// tile kernel with 256-byte rows.  *handled = false -> the caller converts and runs the float32 path.
+// 16-bit activations (float16 / bfloat16 in, same type out; parameters and arithmetic float32): the C = 128 kernel
+// reading and writing the 16-bit elements itself.  *handled = false -> the caller reports the configuration.
 int gdn_tc_forward16(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, int C, int flags,
                      float alpha, float eps, int dtype, cudaStream_t s, bool* handled) {
   *handled = false;
-  if (C != 128 || (dtype != 1 && dtype != 2)) return TFCB_OK;
-  if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return TFCB_OK;
-  if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return TFCB_OK;
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(beta)) & 15) return TFCB_OK;
   TcFlags f;
-  f.inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
-  f.rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
-  f.alpha_mode = (alpha == 2.f) ? 2 : 1;
-  f.eps_mode = (eps == 0.5f) ? 2 : 1;
+  if (C != 128 || (dtype != 1 && dtype != 2) || misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f))
+    return TFCB_OK;
   *handled = true;
-  const bool fast = (alpha == 1.f) && (eps == 1.f) && !f.rectify;
+  const bool fast = tc_fast(f);
   if (dtype == 1)
-    return fast ? launch_tc_fwd2<true, 1>(x, gamma, beta, y, n_pix, f, s) : launch_tc_fwd2<false, 1>(x, gamma, beta, y, n_pix, f, s);
-  return fast ? launch_tc_fwd2<true, 2>(x, gamma, beta, y, n_pix, f, s) : launch_tc_fwd2<false, 2>(x, gamma, beta, y, n_pix, f, s);
+    return fast ? launch_tc_fwd<128, true, 1>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_fwd<128, false, 1>(x, gamma, beta, y, n_pix, f, s);
+  return fast ? launch_tc_fwd<128, true, 2>(x, gamma, beta, y, n_pix, f, s)
+              : launch_tc_fwd<128, false, 2>(x, gamma, beta, y, n_pix, f, s);
 }
 
-}  // namespace tfcb
-
-namespace tfcb {
-
-// Fused tensor-core backward; fills the per-CTA partial sums (part_g [n_parts][C][C], part_b [n_parts][C]) that
-// the caller reduces.  *handled = false -> the caller runs the fp32 kernels.
+// Tensor-core backward: dx, q (workspace) and the per-CTA partial sums (part_g [n_parts][C][C], part_b [n_parts][C])
+// that the caller reduces.  *handled = false -> the caller runs the fp32 kernels.
 int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
                     float* part_g, float* part_b, int* n_parts, long long n_pix, int C, int flags, float alpha,
                     float eps, cudaStream_t s, bool* handled) {
   *handled = false;
-  if (C != 128 && C != 192) return TFCB_OK;
-  if (C == 192 && (reinterpret_cast<uintptr_t>(q_ws) & 15)) return TFCB_OK;
-  if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return TFCB_OK;
-  if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return TFCB_OK;  // trainable exponents: literal pow
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15) return TFCB_OK;
-  if (const char* env = getenv("TFCB_GDN_FP32")) {
-    if (env[0] == '1') return TFCB_OK;
-  }
   TcFlags f;
-  f.inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
-  f.rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
-  f.alpha_mode = (alpha == 2.f) ? 2 : 1;
-  f.eps_mode = (eps == 0.5f) ? 2 : 1;
+  if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
-  const bool fast = (alpha == 1.f) && (eps == 1.f) && !f.rectify;
-  if (C == 192)
-    return fast ? launch_tc_bwd192<true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
-                : launch_tc_bwd192<false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
-  // C == 128.  The default GDN / IGDN goes through the box-fed kernel; TFCB_GDN_BWD_V1=1 keeps the register-fed one
-  // (A/B timing), which also serves the alpha = 2 / epsilon = 1/2 / rectified variants.
-  const char* v1 = getenv("TFCB_GDN_BWD_V1");
-  if (fast && n_pix < (1ll << 31) && !(v1 && v1[0] == '1'))
-    return launch_tc_bwd3(x, gamma, beta, dy, dx, part_g, part_b, n_parts, n_pix, f.inverse, s);
-  return fast ? launch_tc_bwd<true>(x, gamma, beta, dy, dx, part_g, part_b, n_parts, n_pix, f, s)
-              : launch_tc_bwd<false>(x, gamma, beta, dy, dx, part_g, part_b, n_parts, n_pix, f, s);
+  const bool fast = tc_fast(f);
+  if (C == 128)
+    return fast ? launch_tc_bwd<128, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
+                : launch_tc_bwd<128, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
+  return fast ? launch_tc_bwd<192, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
+              : launch_tc_bwd<192, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
 }
 
 }  // namespace tfcb

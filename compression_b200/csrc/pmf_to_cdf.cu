@@ -1,4 +1,4 @@
-// PmfToQuantizedCdf on sm_100a: one thread block per PMF row.
+// PmfToQuantizedCdf on sm_90a: one thread block per PMF row.
 //
 // Replaces tensorflow_compression/cc/kernels/pmf_to_cdf_kernels.cc:58-208 (Compute / PerShard /
 // PenaltyItem / GainItem) and, through tfcb_build_lookup, the per-row tf.while_loop of

@@ -1,4 +1,4 @@
-// Range coder for sm_100a: one CTA per code stream, the serial recurrence alone on one warp.
+// Range coder for sm_90a: one CTA per code stream, the serial recurrence alone on one warp.
 //
 // Replaces (paths relative to /root/reference/tensorflow_compression):
 //   cc/lib/range_coder.cc:37-307, cc/lib/range_coder.h:79-282          the coder
@@ -552,7 +552,6 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
   //   six warps per CTA (P.rot < 0): warp 0 chain, 1 gather, 5 drain, 2..4 idle -- the first CTA of an SM takes slots
   //     0..5 (chain on sub-partition 0, gather + drain on 1), the second slots 6..11 (chain on 2, gather + drain on 3);
   //   four warps per CTA (P.rot = 0..3): roles rotated by P.rot in the CTAs launched after the first wave.
-  // Measured: profiles/r2_encode_notes.md.
   const int warp = threadIdx.x >> 5;
   int role;
   if (P.rot < 0) {
@@ -1612,7 +1611,7 @@ int device_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -1818,7 +1817,7 @@ int enc_role_rotation() {
   static int rot = [] {
     const char* e = getenv("TFCB_ENC_ROT");
     if (e && e[0] >= '0' && e[0] <= '3') return e[0] - '0';
-    return -1;  // default: the six-warp layout (11.7 vs 11.2 Gsym/s at cfg2, profiles/r2_encode_notes.md)
+    return -1;  // default: the six-warp layout
   }();
   return rot;
 }

@@ -96,12 +96,15 @@ extern "C" int tfcb_debug_tma_probe(const float* x_dev, float* y_dev, long long 
   if (depth < 1 || depth > 14 || smem > 227 * 1024) return fail(TFCB_INVALID_ARGUMENT, "bad depth");
   TFCB_CUDA_TRY(cudaFuncSetAttribute(tma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaStream_t s = as_stream(stream);
+  int dev = 0, sms = 0;
+  TFCB_CUDA_TRY(cudaGetDevice(&dev));
+  TFCB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   cudaEvent_t a, b;
   cudaEventCreate(&a);
   cudaEventCreate(&b);
-  tma_probe_kernel<<<148, 32, smem, s>>>(maps[0], maps[1], x_dev, n_rows, C, mode, depth, 8);  // warm
+  tma_probe_kernel<<<sms, 32, smem, s>>>(maps[0], maps[1], x_dev, n_rows, C, mode, depth, 8);  // warm
   cudaEventRecord(a, s);
-  tma_probe_kernel<<<148, 32, smem, s>>>(maps[0], maps[1], x_dev, n_rows, C, mode, depth, iters);
+  tma_probe_kernel<<<sms, 32, smem, s>>>(maps[0], maps[1], x_dev, n_rows, C, mode, depth, iters);
   cudaEventRecord(b, s);
   TFCB_CUDA_TRY(cudaStreamSynchronize(s));
   cudaEventElapsedTime(ms_out, a, b);

@@ -1,4 +1,4 @@
-"""Entropy models of the reference on the B200 range coder.
+"""Entropy models of the reference on the CUDA range coder.
 
 Mirrors tensorflow_compression/python/entropy_models:
   continuous_base.py:36-370     ContinuousEntropyModelBase (table build, storage, config)

@@ -1,4 +1,4 @@
-/* tfcb200.h -- C ABI of libtfcb200.so: the B200-native replacement for the data-parallel hot path of
+/* tfcb200.h -- C ABI of libtfcb200.so: the H100-native (sm_90a) replacement for the data-parallel hot path of
  * tensorflow/compression (range coder ops, PmfToQuantizedCdf, GDN/IGDN forward + backward).
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / TF types.  Every entry point

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+  config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

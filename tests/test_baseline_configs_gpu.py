@@ -104,24 +104,31 @@ def test_cfg1_legacy_op_exactly_as_stated(per_channel):
   assert dec.dtype == torch.int16 and np.array_equal(dec.cpu().numpy(), data)
 
 
+def tie_row_pmfs():
+  """Every 7th symmetric NoisyNormal table of cfg3 as a [1, n] float32 PMF."""
+  from scipy.stats import norm
+  sig = np.exp(np.log(.11) + np.arange(64) * (np.log(256.) - np.log(.11)) / 63)
+  out = []
+  for s in sig[::7]:
+    half = int(np.ceil(s * 2.8)) + 1
+    k = np.arange(-half, half + 1, dtype=np.float64)
+    out.append((norm.cdf((k + .5) / s) - norm.cdf((k - .5) / s)).astype(np.float32)[None])
+  return out
+
+
 def test_pmf_to_cdf_tie_rows_distance_to_the_compiled_reference():
   """a-7 on tie rows (every symmetric NoisyNormal table of cfg3): the kernel equals the C port (lowest-index tie
   break); against the compiled-reference flavour (libstdc++ std::sort order) the tables may differ only by moving
   single counts between bins of EQUAL mass -- recorded here: identical bin-count multiset, |difference| <= 1 per
   bin, and a coding-cost difference of exactly zero under the table's own PMF."""
-  if not oracle.have_ref():
-    pytest.skip("compiled reference not present")
+  import golden_util
   from compression_b200 import gen_ops
-  sig = np.exp(np.log(.11) + np.arange(64) * (np.log(256.) - np.log(.11)) / 63)
   worst = 0
-  for s in sig[::7]:
-    half = int(np.ceil(s * 2.8)) + 1
-    k = np.arange(-half, half + 1, dtype=np.float64)
-    from scipy.stats import norm
-    pmf = (norm.cdf((k + .5) / s) - norm.cdf((k - .5) / s)).astype(np.float32)[None]
+  refs = golden_util.split_rows(golden_util.load_reference(), "pmf_tie_cdf")
+  for pmf, ref in zip(tie_row_pmfs(), refs, strict=True):
     got = gen_ops.pmf_to_quantized_cdf(torch.from_numpy(pmf).cuda(), 12).cpu().numpy()
     assert np.array_equal(got, oracle.port().pmf_to_cdf(pmf, 12))
-    ref = oracle.ref().pmf_to_cdf(pmf, 12)
+    ref = ref[None]
     a, b = np.diff(got[0]), np.diff(ref[0])
     assert sorted(a) == sorted(b)
     assert np.abs(a - b).max() <= 1

@@ -18,6 +18,6 @@ for n_pix in (256 * 64 * 64, 256 * 32 * 32):
     xd = x.to(dt)
     ms = med_ms(lambda: F.gdn_forward(xd, gamma, beta))
     b = 2 * n_pix * C * xd.element_size()
-    print(f"n_pix={n_pix} {str(dt):16s} {ms:.4f} ms  {b/ms/1e6:.0f} GB/s of its own traffic ({b/ms/1e6/6569.6:.3f} of peak)", flush=True)
+    print(f"n_pix={n_pix} {str(dt):16s} {ms:.4f} ms  {b/ms/1e6:.0f} GB/s of its own traffic ({b/ms/1e6/3350:.3f} of peak)", flush=True)
   ms = med_ms(lambda: F.gdn_forward(x.to(torch.bfloat16).float(), gamma, beta).to(torch.bfloat16))
   print(f"n_pix={n_pix} bf16 via convert + float32 kernel + convert: {ms:.4f} ms")
