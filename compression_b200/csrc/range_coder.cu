@@ -191,6 +191,15 @@ struct EncState {
   uint32_t raw;   // size - 1 BEFORE the renormalisation that followed the last symbol (what the chain resumes from)
 };
 
+__host__ __device__ inline EncState enc_initial_state() {
+  EncState s;
+  s.base = 0;
+  s.span = 0xFFFFFFFFu;
+  s.cnt = 0;
+  s.raw = 0xFFFFFFFFu;
+  return s;
+}
+
 // THE RECURRENCE.  The reference keeps (base, size - 1) and, after every Encode, multiplies both by 2^16 when
 // size - 1 < 2^16 (range_coder.cc:69-84).  Only the interval SIZE feeds back into the next symbol, and the
 // renormalisation is a select between two multiplies on that dependent chain.  Here the chain carries the
@@ -226,7 +235,9 @@ struct EncChain {
     const uint32_t shift = (s < 65536u) ? 0u : 16u;
     const uint32_t L = __funnelshift_r((uint32_t)ql, (uint32_t)(ql >> 32), shift);
     const uint32_t U = __funnelshift_r((uint32_t)qu, (uint32_t)(qu >> 32), shift);
-    s = U - L - 1u;
+    // s' = U - L - 1 as ONE IADD3 (U, -L, -1).  Written in C the compiler turns it into U + ~L: a LOP3 and an add,
+    // two dependent instructions on the chain instead of one.
+    asm("{\n\t.reg .u32 t;\n\tsub.u32 t, %1, %2;\n\tsub.u32 %0, t, 1;\n\t}" : "=r"(s) : "r"(U), "r"(L));
     return make_uint2(L, s);
   }
   __device__ __forceinline__ uint2 step(uint4 o) { return step(make_uint2(o.x, o.y), make_uint2(o.z, o.w)); }
@@ -349,6 +360,7 @@ struct EncParams {
   const int32_t* coff;     // f32 modes: cdf_offset [n_rows]
   long long n;
   long long n_streams;
+  int fresh;  // first encode of the handle: start from the initial state instead of reading `state`
   EncState* state;
   uint16_t* words;
   uint32_t* cbits;
@@ -474,8 +486,16 @@ struct BlockInfo {
   uint32_t last;  // nonzero: no further block follows
 };
 
+#ifndef TFCB_ENC_PREFETCH
+#define TFCB_ENC_PREFETCH 4
+#endif
+// Records the chain warp loads ahead of the one it codes: enough to cover the shared-memory load latency while the
+// gather and drain warps keep the SM's shared-memory pipe busy.
+constexpr int kPrefetch = TFCB_ENC_PREFETCH;
+static_assert(kPrefetch == 2 || kPrefetch == 4 || kPrefetch == 8, "the chain loop unrolls by 8 records");
+
 struct EncShared {
-  uint4 ops[2][kBlock + 2];   // (+2: the chain's operand prefetch may run two records past the block)
+  uint4 ops[2][kBlock + kPrefetch];  // (the chain's operand prefetch may run kPrefetch records past the block)
   uint2 ent[2][kBlock];
   BlockInfo ops_info[2];
   BlockInfo ent_info[2];
@@ -631,7 +651,8 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
   if (role == 2) {
     // ------------------------------- drain warp -------------------------------
     EncDrain d;
-    d.begin(P.state[s], P.words + s * P.cap, P.cbits + s * (P.cap >> 5), (uint32_t)P.cap, lane);
+    d.begin(P.fresh ? enc_initial_state() : P.state[s], P.words + s * P.cap, P.cbits + s * (P.cap >> 5),
+            (uint32_t)P.cap, lane);
     for (long long k = 0;; ++k) {
       const int b = (int)(k & 1);
       bar_sync(kBarEntFull + b, 64);
@@ -650,30 +671,36 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
 
   // --------------------------------- chain warp ---------------------------------
   EncChain c;
-  c.s = P.state[s].raw;
+  c.s = P.fresh ? enc_initial_state().raw : P.state[s].raw;
   for (long long k = 0;; ++k) {
     const int b = (int)(k & 1);
     bar_sync(kBarOpsFull + b, 64);
     const BlockInfo bi = sh.ops_info[b];
     if (k >= 2) bar_sync(kBarEntEmpty + b, 64);  // the drain warp is done with this entry buffer
-    // operands are fetched two records ahead so that the shared-memory latency stays off the chain; two 64-bit
+    // operands are fetched kPrefetch records ahead so that the shared-memory latency stays off the chain; two 64-bit
     // loads per record: each multiply-add gets its addend in a register pair of its own
     const uint2* q = reinterpret_cast<const uint2*>(sh.ops[b]);
     uint2* e = sh.ent[b];
     const int n = (int)bi.n;
     int kk = 0;
-    uint2 l0 = q[0], h0 = q[1], l1 = q[2], h1 = q[3];
+    uint2 lo[kPrefetch], hi[kPrefetch];  // records kk .. kk + kPrefetch - 1
+#pragma unroll
+    for (int r = 0; r < kPrefetch; ++r) {
+      lo[r] = q[2 * r];
+      hi[r] = q[2 * r + 1];
+    }
 #pragma unroll 1
     for (; kk + 8 <= n; kk += 8) {
       const uint2* p = q + 2 * kk;
       uint2* const eo = e + kk;
 #pragma unroll
       for (int j = 0; j < 8; j += 2) {  // immediates only
-        const uint2 a0 = l0, b0 = h0, a1 = l1, b1 = h1;
-        l0 = p[2 * j + 4];
-        h0 = p[2 * j + 5];
-        l1 = p[2 * j + 6];
-        h1 = p[2 * j + 7];
+        const int r0 = j % kPrefetch, r1 = (j + 1) % kPrefetch;
+        const uint2 a0 = lo[r0], b0 = hi[r0], a1 = lo[r1], b1 = hi[r1];
+        lo[r0] = p[2 * (j + kPrefetch)];
+        hi[r0] = p[2 * (j + kPrefetch) + 1];
+        lo[r1] = p[2 * (j + 1 + kPrefetch)];
+        hi[r1] = p[2 * (j + 1 + kPrefetch) + 1];
         eo[j] = c.step(a0, b0);
         eo[j + 1] = c.step(a1, b1);
       }
@@ -695,14 +722,7 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
 // ---------------------------------------------------------------------------------------------
 __global__ void enc_init_state_kernel(EncState* st, long long n) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < n) {
-    EncState s;
-    s.base = 0;
-    s.span = 0xFFFFFFFFu;
-    s.cnt = 0;
-    s.raw = 0xFFFFFFFFu;
-    st[i] = s;
-  }
+  if (i < n) st[i] = enc_initial_state();
 }
 
 // Tail rule of RangeEncoder::Finalize (range_coder.cc:266-307) expressed on (words, state).
@@ -747,8 +767,9 @@ __global__ void enc_lengths_kernel(const EncState* state, const uint16_t* words,
   lens[s] = enc_final_length(state[s], words + s * cap, &straddle, &tail, &ntail);
 }
 
-// Single-block exclusive scan: offsets[0..n] from lens[0..n-1].
-__global__ void exclusive_scan_kernel(const long long* lens, long long n, long long* offsets) {
+// Single-block exclusive scan: offsets[0..n] from len(0) .. len(n-1); returns the total to every thread.
+template <typename F>
+__device__ __forceinline__ long long block_exclusive_scan(F len, long long n, long long* offsets) {
   __shared__ long long warp_sums[32];
   __shared__ long long carry_s;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -756,7 +777,7 @@ __global__ void exclusive_scan_kernel(const long long* lens, long long n, long l
   __syncthreads();
   for (long long base = 0; base < n; base += blockDim.x) {
     const long long i = base + tid;
-    long long v = (i < n) ? lens[i] : 0;
+    long long v = (i < n) ? len(i) : 0;
     long long x = v;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -782,6 +803,38 @@ __global__ void exclusive_scan_kernel(const long long* lens, long long n, long l
     __syncthreads();
   }
   if (tid == 0) offsets[n] = carry_s;
+  return carry_s;
+}
+
+__global__ void exclusive_scan_kernel(const long long* lens, long long n, long long* offsets) {
+  block_exclusive_scan([&](long long i) { return lens[i]; }, n, offsets);
+}
+
+// What finalize needs on the host before it can size the output: the total and the first deferred error.
+struct EncResult {
+  long long total;
+  DevError err;
+};
+
+// Finalize in one block: every stream's string length (enc_final_length), their exclusive scan into `offsets`,
+// and {total, error} written straight into host-mapped memory, so that one stream synchronisation is the only
+// round trip.  `reset_err` clears the error record for the next user of a recycled encoder.
+__global__ void __launch_bounds__(1024) enc_offsets_kernel(const EncState* state, const uint16_t* words,
+                                                           long long cap, long long n_streams, long long* offsets,
+                                                           DevError* err, int reset_err, EncResult* res) {
+  const long long total = block_exclusive_scan(
+      [&](long long i) {
+        bool straddle;
+        uint32_t tail;
+        int ntail;
+        return enc_final_length(state[i], words + i * cap, &straddle, &tail, &ntail);
+      },
+      n_streams, offsets);
+  if (threadIdx.x == 0) {
+    res->total = total;
+    res->err = *err;
+    if (reset_err) *err = DevError{};
+  }
 }
 
 // One warp per stream: resolve carries right-to-left, 32 words per step, and write the bytes.
@@ -1695,6 +1748,16 @@ struct LookupCache {
     return TFCB_OK;
   }
 
+  // Whether the entry pinned by `token` holds exactly this encoder table.  (A pinned entry is never evicted, and
+  // its fields do not change after it became visible.)
+  bool same(const void* token, const int32_t* host, int64_t len, int64_t cols) {
+    const Entry* e = static_cast<const Entry*>(token);
+    if (!e || e->for_decoder || e->cols != cols || (int64_t)e->host.size() != len || (len > 0 && !host)) return false;
+    int device = 0;
+    cudaGetDevice(&device);
+    return e->device == device && (len == 0 || std::memcmp(e->host.data(), host, len * sizeof(int32_t)) == 0);
+  }
+
   void release(void* token) {
     if (!token) return;
     std::lock_guard<std::mutex> lock(mu);
@@ -1705,18 +1768,6 @@ struct LookupCache {
 LookupCache& lookup_cache() {
   static LookupCache* c = new LookupCache;  // leaked on purpose: no destructor order problems at exit
   return *c;
-}
-
-// Small pinned scratch per host thread for the device -> host words read at finalize.
-void* pinned_scratch() {
-  thread_local void* p = nullptr;
-  if (!p) {
-    if (cudaHostAlloc(&p, 256, cudaHostAllocDefault) != cudaSuccess) {
-      (void)cudaGetLastError();
-      p = nullptr;
-    }
-  }
-  return p;
 }
 
 int decode_error(const DevError& e, const char* what);
@@ -1770,12 +1821,16 @@ struct tfcb_encoder {
   long long cap = 0;    // words per stream (multiple of 32)
   long long bound = 0;  // worst-case words emitted so far per stream
   DevError* err = nullptr;
-  long long* lens = nullptr;
   long long* offsets = nullptr;
   uint8_t* out = nullptr;
   long long total = 0;
+  bool fresh = true;  // no encode yet: `state` is not initialised (the first encode starts from the initial state)
   bool finalized = false;
   cudaStream_t home = nullptr;
+  // tfcb_compress recycles its encoders: `device` keys the pool, `done` is recorded after the last kernel that
+  // reads the word arena, and the next user's stream waits for it
+  int device = 0;
+  cudaEvent_t done = nullptr;
 };
 
 namespace {
@@ -1848,6 +1903,7 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.coff = coff;
   P.n = n;
   P.n_streams = h->n_streams;
+  P.fresh = h->fresh ? 1 : 0;
   P.state = h->state;
   P.words = h->words;
   P.cbits = h->cbits;
@@ -1857,7 +1913,62 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   encode_kernel<MODE><<<(unsigned)h->n_streams, P.rot < 0 ? 192 : 128, 0, s>>>(P);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
+  h->fresh = false;
   return TFCB_OK;
+}
+
+// Initial state of a handle that finalizes without having encoded anything.
+int init_state_if_fresh(tfcb_encoder* h, cudaStream_t s) {
+  if (!h->fresh) return TFCB_OK;
+  if (h->n_streams > 0) {
+    enc_init_state_kernel<<<(unsigned)((h->n_streams + 255) / 256), 256, 0, s>>>(h->state, h->n_streams);
+    TFCB_LAUNCHED();
+    TFCB_CUDA_TRY(cudaGetLastError());
+  }
+  h->fresh = false;
+  return TFCB_OK;
+}
+
+// Host-mapped {total, error} per host thread: written by enc_offsets_kernel, read after the stream synchronises.
+EncResult* mapped_result(EncResult** dev) {
+  thread_local EncResult* host = nullptr;
+  thread_local EncResult* devp = nullptr;
+  if (!host) {
+    void* p = nullptr;
+    if (cudaHostAlloc(&p, sizeof(EncResult), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess ||
+        cudaHostGetDevicePointer((void**)&devp, p, 0) != cudaSuccess) {
+      (void)cudaGetLastError();
+      if (p) cudaFreeHost(p);
+      return nullptr;
+    }
+    host = static_cast<EncResult*>(p);
+  }
+  *dev = devp;
+  return host;
+}
+
+// Lengths, offsets (into `offsets`), the one host round trip, then the deferred argument errors and the total.
+int enc_offsets(tfcb_encoder* h, long long* offsets, bool reset_err, cudaStream_t s, long long* total) {
+  EncResult* dres = nullptr;
+  EncResult* res = mapped_result(&dres);
+  if (!res) return fail(TFCB_CUDA_ERROR, "could not allocate host-mapped memory for the finalize result");
+  enc_offsets_kernel<<<1, 1024, 0, s>>>(h->state, h->words, h->cap, h->n_streams, offsets, h->err,
+                                         reset_err ? 1 : 0, dres);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  TFCB_CUDA_TRY(cudaStreamSynchronize(s));
+  EncResult r;
+  std::memcpy(&r, res, sizeof r);
+  *total = r.total;
+  return decode_error(r.err, "encode");
+}
+
+void enc_write(tfcb_encoder* h, const long long* offsets, uint8_t* out, cudaStream_t s) {
+  if (h->n_streams > 0) {
+    enc_write_kernel<<<(unsigned)h->n_streams, 32 * kWriteWarps, 0, s>>>(h->state, h->words, h->cbits, h->cap,
+                                                                        h->n_streams, offsets, out);
+    TFCB_LAUNCHED();
+  }
 }
 
 }  // namespace
@@ -1880,14 +1991,11 @@ int tfcb_encoder_create(const int32_t* lookup_host, int64_t lookup_len, int64_t 
     tfcb_encoder_destroy(h);
     return rc;
   }
-  cudaMemsetAsync(h->err, 0, sizeof(DevError), s);
-  if (n_streams > 0) {
-    enc_init_state_kernel<<<(unsigned)((n_streams + 255) / 256), 256, 0, s>>>(h->state, n_streams);
-    TFCB_LAUNCHED();
-  }
-  if (cudaGetLastError() != cudaSuccess) {
+  // (the state is initialised by the first encode, or by finalize when nothing was encoded)
+  if (cudaMemsetAsync(h->err, 0, sizeof(DevError), s) != cudaSuccess) {
+    (void)cudaGetLastError();
     tfcb_encoder_destroy(h);
-    return fail(TFCB_CUDA_ERROR, "encoder state initialisation failed");
+    return fail(TFCB_CUDA_ERROR, "encoder initialisation failed");
   }
   *out = h;
   return TFCB_OK;
@@ -1928,39 +2036,15 @@ int tfcb_encode_finalize(tfcb_encoder* h, void* stream, int64_t* total_bytes_hos
   cudaStream_t s = as_stream(stream);
   const long long S = h->n_streams;
   // (a finalize retried after a deferred argument error reuses the buffers of the first attempt)
-  if (!h->lens) TFCB_TRY(dev_alloc((void**)&h->lens, std::max<long long>(S, 1) * sizeof(long long), s));
   if (!h->offsets) TFCB_TRY(dev_alloc((void**)&h->offsets, (S + 1) * sizeof(long long), s));
   if (h->cap == 0) TFCB_TRY(ensure_capacity(h, 0, s));
-  if (S > 0) {
-    enc_lengths_kernel<<<(unsigned)((S + 127) / 128), 128, 0, s>>>(h->state, h->words, h->cap, S, h->lens);
-    TFCB_LAUNCHED();
-  }
-  exclusive_scan_kernel<<<1, 1024, 0, s>>>(h->lens, S, h->offsets);
-  TFCB_LAUNCHED();
-  TFCB_CUDA_TRY(cudaGetLastError());
-  // one host round trip for both the deferred argument errors and the total size
+  TFCB_TRY(init_state_if_fresh(h, s));
   long long total = 0;
-  DevError err;
-  if (char* scratch = static_cast<char*>(pinned_scratch())) {
-    TFCB_CUDA_TRY(cudaMemcpyAsync(scratch, h->offsets + S, sizeof total, cudaMemcpyDeviceToHost, s));
-    TFCB_CUDA_TRY(cudaMemcpyAsync(scratch + 64, h->err, sizeof err, cudaMemcpyDeviceToHost, s));
-    TFCB_CUDA_TRY(cudaStreamSynchronize(s));
-    std::memcpy(&total, scratch, sizeof total);
-    std::memcpy(&err, scratch + 64, sizeof err);
-  } else {
-    TFCB_CUDA_TRY(cudaMemcpyAsync(&total, h->offsets + S, sizeof total, cudaMemcpyDeviceToHost, s));
-    TFCB_CUDA_TRY(cudaMemcpyAsync(&err, h->err, sizeof err, cudaMemcpyDeviceToHost, s));
-    TFCB_CUDA_TRY(cudaStreamSynchronize(s));
-  }
-  TFCB_TRY(decode_error(err, "encode"));
+  TFCB_TRY(enc_offsets(h, h->offsets, /*reset_err=*/false, s, &total));
   h->total = total;
   TFCB_TRY(dev_alloc((void**)&h->out, (size_t)std::max<long long>(total, 1), s));
-  if (S > 0) {
-    enc_write_kernel<<<(unsigned)S, 32 * kWriteWarps, 0, s>>>(h->state, h->words, h->cbits, h->cap, S,
-                                                             h->offsets, h->out);
-    TFCB_LAUNCHED();
-    TFCB_CUDA_TRY(cudaGetLastError());
-  }
+  enc_write(h, h->offsets, h->out, s);
+  TFCB_CUDA_TRY(cudaGetLastError());
   // the word arena is no longer needed
   dev_free(h->words, s);
   dev_free(h->cbits, s);
@@ -1998,10 +2082,154 @@ void tfcb_encoder_destroy(tfcb_encoder* h) {
   dev_free(h->words, s);
   dev_free(h->cbits, s);
   dev_free(h->err, s);
-  dev_free(h->lens, s);
   dev_free(h->offsets, s);
   dev_free(h->out, s);
+  if (h->done) cudaEventDestroy(h->done);
   delete h;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Idle encoders of tfcb_compress, with their state, error record and word arena: a model compresses batch after
+// batch of the same shape, and a recycled encoder saves the allocations and the initialisation of each call.
+struct EncoderPool {
+  static constexpr size_t kMaxIdle = 4;
+  std::mutex mu;
+  std::vector<tfcb_encoder*> idle;
+
+  tfcb_encoder* take(long long n_streams, int device) {
+    std::lock_guard<std::mutex> lock(mu);
+    for (size_t i = idle.size(); i-- > 0;) {
+      if (idle[i]->n_streams == n_streams && idle[i]->device == device) {
+        tfcb_encoder* h = idle[i];
+        idle.erase(idle.begin() + i);
+        return h;
+      }
+    }
+    return nullptr;
+  }
+  void give(tfcb_encoder* h) {
+    {
+      std::lock_guard<std::mutex> lock(mu);
+      if (idle.size() < kMaxIdle) {
+        idle.push_back(h);
+        return;
+      }
+    }
+    tfcb_encoder_destroy(h);
+  }
+};
+
+EncoderPool& encoder_pool() {
+  static EncoderPool* p = new EncoderPool;  // leaked on purpose, like the lookup cache
+  return *p;
+}
+
+// A pooled encoder reset to a fresh handle for `lookup` on stream `s`.
+int checkout_encoder(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                     cudaStream_t s, tfcb_encoder** out) {
+  int device = 0;
+  cudaGetDevice(&device);
+  tfcb_encoder* h = encoder_pool().take(n_streams, device);
+  if (!h) {
+    TFCB_TRY(tfcb_encoder_create(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
+    h->device = device;
+    if (cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming) != cudaSuccess) {
+      (void)cudaGetLastError();
+      h->done = nullptr;
+      tfcb_encoder_destroy(h);
+      return fail(TFCB_CUDA_ERROR, "encoder event creation failed");
+    }
+    *out = h;
+    return TFCB_OK;
+  }
+  // Same table as the previous user (the common case: one model, batch after batch): a compare with the cache
+  // entry the encoder already pins is cheaper than hashing the table again.
+  if (!lookup_cache().same(h->lut_token, lookup_host, lookup_len, lookup_cols)) {
+    DeviceLookup lut;
+    void* token = nullptr;
+    const int rc =
+        lookup_cache().acquire(lookup_host, lookup_len, lookup_cols, /*for_decoder=*/false, s, &lut, &token);
+    if (rc != TFCB_OK) {
+      encoder_pool().give(h);
+      return rc;
+    }
+    lookup_cache().release(h->lut_token);
+    h->lut = lut;
+    h->lut_token = token;
+  }
+  // the previous user's last kernel (enc_write_kernel) may still read the arena on another stream (on the same
+  // stream, stream order is enough)
+  if (h->home != s && cudaStreamWaitEvent(s, h->done, 0) != cudaSuccess) {
+    (void)cudaGetLastError();
+    tfcb_encoder_destroy(h);
+    return fail(TFCB_CUDA_ERROR, "cudaStreamWaitEvent failed");
+  }
+  h->home = s;
+  h->bound = 0;
+  h->total = 0;
+  h->fresh = true;
+  h->finalized = false;
+  *out = h;
+  return TFCB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                  const int32_t* index_dev, const void* value_dev, int32_t value_is_f32, const float* qoff_dev,
+                  const int32_t* cdf_offset_dev, int64_t n, int64_t* offsets_dev, void* stream,
+                  tfcb_encoder** out, int64_t* total_bytes_host) {
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  *out = nullptr;
+  *total_bytes_host = 0;
+  if (n_streams < 0) return fail(TFCB_INVALID_ARGUMENT, "negative stream count");
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  cudaStream_t s = as_stream(stream);
+  tfcb_encoder* h = nullptr;
+  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
+  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0);
+  int rc;
+  switch (mode) {
+    case 0: rc = launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, s); break;
+    case kModeIndex: rc = launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, s); break;
+    case kModeF32: rc = launch_encode<kModeF32>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s); break;
+    default:
+      rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s);
+      break;
+  }
+  if (rc == TFCB_OK && h->cap == 0) rc = ensure_capacity(h, 0, s);
+  if (rc == TFCB_OK) rc = init_state_if_fresh(h, s);
+  long long total = 0;
+  if (rc == TFCB_OK)
+    rc = enc_offsets(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
+  if (rc != TFCB_OK) {
+    // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
+    if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
+    else tfcb_encoder_destroy(h);
+    return rc;
+  }
+  *out = h;
+  *total_bytes_host = total;
+  return TFCB_OK;
+}
+
+int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
+  cudaStream_t s = as_stream(stream);
+  enc_write(h, reinterpret_cast<const long long*>(offsets_dev), bytes_dev, s);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || cudaEventRecord(h->done, s) != cudaSuccess) {
+    (void)cudaGetLastError();
+    tfcb_encoder_destroy(h);
+    return fail(TFCB_CUDA_ERROR, "enc_write_kernel launch failed: %s", cudaGetErrorString(e));
+  }
+  encoder_pool().give(h);
+  return TFCB_OK;
 }
 
 }  // extern "C"

@@ -321,17 +321,16 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     if rank_p and shape[-rank_p:] != self.prior_shape:
       bottleneck = torch.broadcast_to(bottleneck, shape[:-rank_p] + self.prior_shape)
     coff, qoff = self._flat_tables(bottleneck.device)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
     if fused and bottleneck.dtype == torch.float32:
-      F.encode_channel_f32(handle, bottleneck.contiguous(), qoff, coff)
-    else:
-      b = bottleneck.to(torch.float32)
-      if qoff is not None:
-        b = b - qoff.reshape(self.prior_shape)
-      symbols = torch.round(b).to(torch.int32)
-      iid = shape[:len(shape) - rank_p] if rank_p else shape
-      symbols = symbols.reshape(iid + (-1,)) - coff
-      gen_ops.entropy_encode_channel(handle, symbols)
+      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, qoff, coff)
+    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
+    b = bottleneck.to(torch.float32)
+    if qoff is not None:
+      b = b - qoff.reshape(self.prior_shape)
+    symbols = torch.round(b).to(torch.int32)
+    iid = shape[:len(shape) - rank_p] if rank_p else shape
+    symbols = symbols.reshape(iid + (-1,)) - coff
+    gen_ops.entropy_encode_channel(handle, symbols)
     return gen_ops.entropy_encode_finalize(handle)
 
   def decompress(self, strings, broadcast_shape, fused=True):
@@ -475,13 +474,12 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     fshape = tuple(flat.shape)
     batch_shape = fshape[:len(fshape) - self.coding_rank]
     coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
     if fused and bottleneck.dtype == torch.float32:
-      F.encode_index_f32(handle, flat, bottleneck.contiguous(), _loc, coff)
-    else:
-      b = bottleneck if _loc is None else bottleneck - _loc
-      symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
-      gen_ops.entropy_encode_index(handle, flat, symbols)
+      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, _loc, coff, index=flat)
+    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
+    b = bottleneck if _loc is None else bottleneck - _loc
+    symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
+    gen_ops.entropy_encode_index(handle, flat, symbols)
     return gen_ops.entropy_encode_finalize(handle)
 
   def decompress(self, strings, indexes, fused=True, _loc=None):
@@ -669,12 +667,12 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
     indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
     indexes = torch.broadcast_to(indexes, shape).contiguous()
     coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
     if fused and bottleneck.dtype == torch.float32:
-      F.encode_index_f32(handle, indexes, bottleneck.contiguous(), torch.broadcast_to(offset, shape).contiguous(), coff)
-    else:
-      symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[indexes.long()]
-      gen_ops.entropy_encode_index(handle, indexes, symbols)
+      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck,
+                            torch.broadcast_to(offset, shape).contiguous(), coff, index=indexes)
+    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
+    symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[indexes.long()]
+    gen_ops.entropy_encode_index(handle, indexes, symbols)
     return gen_ops.entropy_encode_finalize(handle)
 
   def decompress(self, strings, broadcast_shape, fused=True):
@@ -800,12 +798,11 @@ class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
     fshape = tuple(flat.shape)
     batch_shape = fshape[:len(fshape) - self.coding_rank]
     coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
     if fused and bottleneck.dtype == torch.float32:
-      F.encode_index_f32(handle, flat, bottleneck.contiguous(), offset, coff)
-    else:
-      symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[flat.long()]
-      gen_ops.entropy_encode_index(handle, flat, symbols)
+      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, offset, coff, index=flat)
+    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
+    symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[flat.long()]
+    gen_ops.entropy_encode_index(handle, flat, symbols)
     return gen_ops.entropy_encode_finalize(handle)
 
   def decompress(self, strings, indexes, fused=True):

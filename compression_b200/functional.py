@@ -167,6 +167,37 @@ def encode_index_f32(handle, index, y, loc, cdf_offset):
   return handle
 
 
+def compress_f32(batch_shape, lookup, y, quant_offset, cdf_offset, index=None):
+  """create_range_encoder + encode_channel_f32 (index None) or encode_index_f32 (`quant_offset` is then the loc
+  tensor) + entropy_encode_finalize, as two library calls with one host synchronisation.  The strings are
+  written into tensors this call allocates, so each result owns its memory."""
+  from compression_b200 import gen_ops
+  shape = tuple(int(d) for d in batch_shape)
+  lookup = gen_ops._host_i32(lookup)
+  if lookup.ndim not in (1, 2):
+    raise _lib.InvalidArgumentError(f"`lookup` must be rank 1 or 2: {lookup.shape}")
+  n_streams = gen_ops._prod(shape)
+  if n_streams == 0:
+    raise _lib.InvalidArgumentError(f"`handle` is empty: handle.shape={shape}")
+  y = _f32(y, y.device)
+  dev = y.device
+  index = _i32(index, dev)
+  offsets = torch.empty(n_streams + 1, dtype=torch.int64, device=dev)
+  h, total = C.c_void_p(), C.c_int64(0)
+  stream = _stream()
+  L = _lib.lib()
+  check(L.tfcb_compress(lookup.ctypes.data_as(C.c_void_p), lookup.size, 0 if lookup.ndim == 1 else lookup.shape[1],
+                        n_streams, _p(index), _p(y), 1, _p(_f32(quant_offset, dev)), _p(_i32(cdf_offset, dev)),
+                        y.numel() // n_streams, _p(offsets), stream, C.byref(h), C.byref(total)))
+  try:
+    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
+  except BaseException:
+    L.tfcb_encoder_destroy(h)
+    raise
+  check(L.tfcb_compress_write(h, _p(offsets), _p(out), stream))
+  return gen_ops.Strings(out, offsets, shape)
+
+
 def decode_channel_f32(handle, out_shape, quant_offset, cdf_offset):
   """Decodes and dequantises: float(sym + cdf_offset[c]) + quant_offset[c] (continuous_batched.py:416-421)."""
   dev = handle._encoded.bytes_dev.device

@@ -97,6 +97,21 @@ int tfcb_encoder_copy_output(tfcb_encoder* h, uint8_t* bytes_host, int64_t* offs
                              void* stream);
 void tfcb_encoder_destroy(tfcb_encoder* h);
 
+/* One whole compress() in two calls: create + one encode + finalize, with the result written into
+ * caller-owned device memory.  tfcb_compress encodes `n_per_stream` symbols of every stream (channel mode when
+ * `index_dev` is NULL, else index mode; `value_dev` is int32, or float32 quantised as in the *_f32 calls when
+ * `value_is_f32` is nonzero), writes the offsets int64 [n_streams + 1] to `offsets_dev`, synchronises `stream`
+ * once, reports argument errors like tfcb_encode_finalize and returns the total size and an encoder that holds
+ * the unpacked streams.  tfcb_compress_write packs them into `bytes_dev` [total] and takes the encoder back;
+ * the caller must not use it afterwards (tfcb_encoder_destroy releases one that is never written).
+ * The library keeps such encoders, with their device buffers, between calls and reuses them in stream
+ * order. */
+int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                  const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
+                  const float* quant_offset_dev, const int32_t* cdf_offset_dev, int64_t n_per_stream,
+                  int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host);
+int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Range DECODER.  Replaces CreateRangeDecoder / EntropyDecodeChannel / EntropyDecodeIndex /
  * EntropyDecodeFinalize:
