@@ -137,18 +137,30 @@ REGISTER_KERNEL_BUILDER(Name("EntropyEncodeIndex").Device(tf::DEVICE_GPU).HostMe
                         EntropyEncodeGpuOp<true>);
 
 // ---- EntropyEncodeFinalize (range_coder_kernels.cc:594-619): device-side range errors surface here ----
+// The strings are packed on the device into temporaries and copied out, as RunLengthEncode does below.
 class EntropyEncodeFinalizeGpuOp : public tf::OpKernel {
  public:
   using tf::OpKernel::OpKernel;
   void Compute(tf::OpKernelContext* ctx) override {
     GpuEncoderVariant* v;
     OP_REQUIRES_OK(ctx, GetEncoder(ctx, &v));
-    int64_t total = 0;
-    OP_REQUIRES_OK(ctx, FromRc(tfcb_encode_finalize(v->handle.get(), CudaStream(ctx), &total)));
     const int64_t streams = v->shape.num_elements();
+    tf::Tensor offsets_dev, bytes_dev;
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(tf::DT_INT64, tf::TensorShape({streams + 1}), &offsets_dev));
+    int64_t total = 0;
+    OP_REQUIRES_OK(ctx, FromRc(tfcb_encode_finalize(v->handle.get(), offsets_dev.flat<int64_t>().data(), CudaStream(ctx),
+                                                   &total)));
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(tf::DT_UINT8, tf::TensorShape({total > 0 ? total : 1}), &bytes_dev));
+    OP_REQUIRES_OK(ctx, FromRc(tfcb_encode_write(v->handle.get(), offsets_dev.flat<int64_t>().data(),
+                                                bytes_dev.flat<uint8_t>().data(), CudaStream(ctx))));
     std::vector<uint8_t> bytes(total > 0 ? total : 1);
     std::vector<int64_t> offsets(streams + 1);
-    OP_REQUIRES_OK(ctx, FromRc(tfcb_encoder_copy_output(v->handle.get(), bytes.data(), offsets.data(), CudaStream(ctx))));
+    auto* stream = ctx->op_device_context()->stream();
+    stream_executor::DeviceMemoryBase src_bytes(bytes_dev.flat<uint8_t>().data(), static_cast<uint64_t>(total));
+    stream_executor::DeviceMemoryBase src_offsets(offsets_dev.flat<int64_t>().data(), offsets.size() * sizeof(int64_t));
+    if (total > 0) OP_REQUIRES_OK(ctx, stream->Memcpy(bytes.data(), src_bytes, static_cast<uint64_t>(total)));
+    OP_REQUIRES_OK(ctx, stream->Memcpy(offsets.data(), src_offsets, offsets.size() * sizeof(int64_t)));
+    OP_REQUIRES_OK(ctx, stream->BlockHostUntilDone());
     tf::Tensor* out;
     OP_REQUIRES_OK(ctx, ctx->allocate_output(0, v->shape, &out));
     auto flat = out->flat<tf::tstring>();

@@ -46,9 +46,8 @@ SIGNATURES = {
     "tfcb_encode_channel_f32": (_int, [_vp, _vp, _vp, _vp, _i64, _vp]),
     "tfcb_encode_index_f32": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "tfcb_encoder_check": (_int, [_vp, _vp]),
-    "tfcb_encode_finalize": (_int, [_vp, _vp, _p(_i64)]),
-    "tfcb_encoder_output": (_int, [_vp, _p(_vp), _p(_vp)]),
-    "tfcb_encoder_copy_output": (_int, [_vp, _vp, _vp, _vp]),
+    "tfcb_encode_finalize": (_int, [_vp, _vp, _vp, _p(_i64)]),
+    "tfcb_encode_write": (_int, [_vp, _vp, _vp, _vp]),
     "tfcb_encoder_destroy": (None, [_vp]),
     "tfcb_compress": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _p(_vp), _p(_i64)]),
     "tfcb_compress_write": (_int, [_vp, _vp, _vp, _vp]),
@@ -90,7 +89,7 @@ def lib():
       fn = getattr(handle, name)
       fn.restype = res
       fn.argtypes = args
-    if handle.tfcb_abi_version() != 1:
+    if handle.tfcb_abi_version() != 2:
       raise ImportError("libtfcb200.so ABI version mismatch")
     _lib = handle
   return _lib

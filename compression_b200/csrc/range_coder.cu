@@ -352,8 +352,6 @@ struct EncParams {
   const int2* rows;
   int n_rows;
   int uniform_prec;        // > 0: every row has this precision
-  int n_sms;
-  int rot;                 // warp-role rotation of the CTAs of the second wave (see encode_kernel)
   const void* value;       // int32 or float [S, n]
   const int32_t* index;    // [S, n] or null
   const float* qoff;       // channel+f32: [n_rows] or null; index+f32: loc [S, n] or null
@@ -476,22 +474,16 @@ __device__ __forceinline__ void bar_arrive(int id, int count) {
 // block and direction.  The gather warp writes the record stream the chain consumes blindly: an escaping symbol
 // is followed by the records of its Elias-gamma bits (OverflowEncode, range_coder_kernels.cc:306-321), so the
 // chain warp has no special cases at all.
-#ifndef TFCB_ENC_BLOCK
-#define TFCB_ENC_BLOCK 256
-#endif
-constexpr int kBlock = TFCB_ENC_BLOCK;
+constexpr int kBlock = 256;
 
 struct BlockInfo {
   uint32_t n;     // records / entries in this block (kBlock except for the last one)
   uint32_t last;  // nonzero: no further block follows
 };
 
-#ifndef TFCB_ENC_PREFETCH
-#define TFCB_ENC_PREFETCH 4
-#endif
 // Records the chain warp loads ahead of the one it codes: enough to cover the shared-memory load latency while the
 // gather and drain warps keep the SM's shared-memory pipe busy.
-constexpr int kPrefetch = TFCB_ENC_PREFETCH;
+constexpr int kPrefetch = 4;
 static_assert(kPrefetch == 2 || kPrefetch == 4 || kPrefetch == 8, "the chain loop unrolls by 8 records");
 
 struct EncShared {
@@ -566,23 +558,14 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
   __shared__ __align__(16) EncShared sh;
   const long long s = blockIdx.x;
   const int lane = threadIdx.x & 31;
-  // Roles: 0 chain, 1 gather, 2 drain, 3 idle (exits at once).  Only the per-stream latency of the chain warp
-  // matters (there are more schedulers than streams), so the layout's job is to keep a chain warp alone on its
-  // sub-partition (warp slot mod 4) when two CTAs share an SM:
-  //   six warps per CTA (P.rot < 0): warp 0 chain, 1 gather, 5 drain, 2..4 idle -- the first CTA of an SM takes slots
-  //     0..5 (chain on sub-partition 0, gather + drain on 1), the second slots 6..11 (chain on 2, gather + drain on 3);
-  //   four warps per CTA (P.rot = 0..3): roles rotated by P.rot in the CTAs launched after the first wave.
+  // Warp 0 chain, 1 gather, 5 drain; 2..4 exit at once.  Only the per-stream latency of the chain warp matters
+  // (there are more schedulers than streams), so the layout keeps a chain warp alone on its sub-partition (warp slot
+  // mod 4) when two CTAs share an SM: the first takes slots 0..5 (chain on sub-partition 0, gather + drain on 1), the
+  // second slots 6..11 (chain on 2, gather + drain on 3).
   const int warp = threadIdx.x >> 5;
-  int role;
-  if (P.rot < 0) {
-    role = warp == 0 ? 0 : (warp == 1 ? 1 : (warp == 5 ? 2 : 3));
-  } else {
-    const int rot = (blockIdx.x >= (unsigned)P.n_sms) ? P.rot : 0;
-    role = (warp - rot) & 3;
-  }
-  if (role == 3) return;
+  if (warp != 0 && warp != 1 && warp != 5) return;
 
-  if (role == 1) {
+  if (warp == 1) {
     // ------------------------------- gather warp -------------------------------
     uint32_t row_a = 0, chan_step = 0;
     if (!(MODE & kModeIndex)) {
@@ -648,7 +631,7 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
     return;
   }
 
-  if (role == 2) {
+  if (warp == 5) {
     // ------------------------------- drain warp -------------------------------
     EncDrain d;
     d.begin(P.fresh ? enc_initial_state() : P.state[s], P.words + s * P.cap, P.cbits + s * (P.cap >> 5),
@@ -757,27 +740,44 @@ __device__ __forceinline__ long long enc_final_length(const EncState& st, const 
   return 2ll * st.cnt + *ntail;
 }
 
-__global__ void enc_lengths_kernel(const EncState* state, const uint16_t* words, long long cap,
-                                   long long n_streams, long long* lens) {
-  const long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (s >= n_streams) return;
-  bool straddle;
-  uint32_t tail;
-  int ntail;
-  lens[s] = enc_final_length(state[s], words + s * cap, &straddle, &tail, &ntail);
-}
+// What finalize needs on the host before it can size the output: the total and the first deferred error.
+struct EncResult {
+  long long total;
+  DevError err;
+};
 
-// Single-block exclusive scan: offsets[0..n] from len(0) .. len(n-1); returns the total to every thread.
-template <typename F>
-__device__ __forceinline__ long long block_exclusive_scan(F len, long long n, long long* offsets) {
+// What finalize reads: the coded streams' state, unresolved words and carry bits, and the deferred error record.
+// An encoder handle holds one; the legacy single-stream op sets one up per call.
+struct EncArena {
+  long long n_streams = 0;
+  EncState* state = nullptr;
+  uint16_t* words = nullptr;
+  uint32_t* cbits = nullptr;
+  long long cap = 0;  // words per stream (multiple of 32)
+  DevError* err = nullptr;
+};
+
+// Finalize in one block: every stream's string length (enc_final_length), their exclusive scan into
+// offsets[0..n_streams], and {total, error} written straight into host-mapped memory, so that one stream
+// synchronisation is the only round trip.  `reset_err` clears the error record for the next user of a recycled
+// encoder.
+__global__ void __launch_bounds__(1024) enc_offsets_kernel(const EncState* state, const uint16_t* words,
+                                                           long long cap, long long n_streams, long long* offsets,
+                                                           DevError* err, int reset_err, EncResult* res) {
   __shared__ long long warp_sums[32];
   __shared__ long long carry_s;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   if (tid == 0) carry_s = 0;
   __syncthreads();
-  for (long long base = 0; base < n; base += blockDim.x) {
+  for (long long base = 0; base < n_streams; base += blockDim.x) {
     const long long i = base + tid;
-    long long v = (i < n) ? len(i) : 0;
+    long long v = 0;
+    if (i < n_streams) {
+      bool straddle;
+      uint32_t tail;
+      int ntail;
+      v = enc_final_length(state[i], words + i * cap, &straddle, &tail, &ntail);
+    }
     long long x = v;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -797,47 +797,19 @@ __device__ __forceinline__ long long block_exclusive_scan(F len, long long n, lo
     }
     __syncthreads();
     const long long before = carry_s + (wid ? warp_sums[wid - 1] : 0) + (x - v);
-    if (i < n) offsets[i] = before;
+    if (i < n_streams) offsets[i] = before;
     __syncthreads();
     if (tid == blockDim.x - 1) carry_s = before + v;
     __syncthreads();
   }
-  if (tid == 0) offsets[n] = carry_s;
-  return carry_s;
-}
-
-__global__ void exclusive_scan_kernel(const long long* lens, long long n, long long* offsets) {
-  block_exclusive_scan([&](long long i) { return lens[i]; }, n, offsets);
-}
-
-// What finalize needs on the host before it can size the output: the total and the first deferred error.
-struct EncResult {
-  long long total;
-  DevError err;
-};
-
-// Finalize in one block: every stream's string length (enc_final_length), their exclusive scan into `offsets`,
-// and {total, error} written straight into host-mapped memory, so that one stream synchronisation is the only
-// round trip.  `reset_err` clears the error record for the next user of a recycled encoder.
-__global__ void __launch_bounds__(1024) enc_offsets_kernel(const EncState* state, const uint16_t* words,
-                                                           long long cap, long long n_streams, long long* offsets,
-                                                           DevError* err, int reset_err, EncResult* res) {
-  const long long total = block_exclusive_scan(
-      [&](long long i) {
-        bool straddle;
-        uint32_t tail;
-        int ntail;
-        return enc_final_length(state[i], words + i * cap, &straddle, &tail, &ntail);
-      },
-      n_streams, offsets);
-  if (threadIdx.x == 0) {
-    res->total = total;
+  if (tid == 0) {
+    offsets[n_streams] = carry_s;
+    res->total = carry_s;
     res->err = *err;
     if (reset_err) *err = DevError{};
   }
 }
 
-// One warp per stream: resolve carries right-to-left, 32 words per step, and write the bytes.
 // One CTA of kWriteWarps warps per stream.  The carry chain runs right to left over 32-word groups; it is cut into
 // kWriteWarps segments: every warp first runs its segment's chain for BOTH possible carries entering it (two adds per
 // group instead of one), the segments' carry-ins are then resolved through shared memory (a chain of kWriteWarps
@@ -1658,18 +1630,6 @@ __global__ void __launch_bounds__(32) legacy_decode_kernel(const uint8_t* bytes,
 // ---------------------------------------------------------------------------------------------
 // Host-side handles
 // ---------------------------------------------------------------------------------------------
-int device_sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
-// ---------------------------------------------------------------------------------------------
 // Device-table cache.  A model creates a handle per compress()/decompress() call with the same `lookup`
 // every time (continuous_batched.py:381, :408): parsing and uploading it again (plus the stream
 // synchronisation that keeps the host staging alive) would sit on the host's critical path of every step.
@@ -1686,8 +1646,7 @@ struct LookupCache {
     int pins = 0;
     uint64_t last_use = 0;
     std::vector<int32_t> host;
-    DeviceLookup lut;      // shallow copy of a cache entry's tables
-  void* lut_token = nullptr;
+    DeviceLookup lut;
   };
   static constexpr size_t kMaxEntries = 16;
   std::mutex mu;
@@ -1811,21 +1770,12 @@ int decode_error(const DevError& e, const char* what) {
 
 using namespace tfcb;
 
-struct tfcb_encoder {
+struct tfcb_encoder : EncArena {
   DeviceLookup lut;      // shallow copy of a cache entry's tables
   void* lut_token = nullptr;
-  long long n_streams = 0;
-  EncState* state = nullptr;
-  uint16_t* words = nullptr;
-  uint32_t* cbits = nullptr;
-  long long cap = 0;    // words per stream (multiple of 32)
   long long bound = 0;  // worst-case words emitted so far per stream
-  DevError* err = nullptr;
-  long long* offsets = nullptr;
-  uint8_t* out = nullptr;
-  long long total = 0;
   bool fresh = true;  // no encode yet: `state` is not initialised (the first encode starts from the initial state)
-  bool finalized = false;
+  bool finalized = false;  // tfcb_encode_finalize succeeded: only tfcb_encode_write (once) and destroy remain
   cudaStream_t home = nullptr;
   // tfcb_compress recycles its encoders: `device` keys the pool, `done` is recorded after the last kernel that
   // reads the word arena, and the next user's stream waits for it
@@ -1867,16 +1817,6 @@ int ensure_capacity(tfcb_encoder* h, long long extra_words, cudaStream_t s) {
   return TFCB_OK;
 }
 
-// Warp-role rotation of the second-wave CTAs (0..3); TFCB_ENC_ROT overrides the default for experiments.
-int enc_role_rotation() {
-  static int rot = [] {
-    const char* e = getenv("TFCB_ENC_ROT");
-    if (e && e[0] >= '0' && e[0] <= '3') return e[0] - '0';
-    return -1;  // default: the six-warp layout
-  }();
-  return rot;
-}
-
 template <int MODE>
 int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, const float* qoff,
                   const int32_t* coff, long long n, cudaStream_t s) {
@@ -1895,8 +1835,6 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.rows = h->lut.rows;
   P.n_rows = h->lut.n_rows;
   P.uniform_prec = h->lut.uniform_prec;
-  P.n_sms = device_sm_count();
-  P.rot = enc_role_rotation();
   P.value = value;
   P.index = index;
   P.qoff = qoff;
@@ -1910,21 +1848,9 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.cap = h->cap;
   P.err = h->err;
   if (h->n_streams > 0x7FFFFFFFll) return fail(TFCB_INVALID_ARGUMENT, "too many streams");
-  encode_kernel<MODE><<<(unsigned)h->n_streams, P.rot < 0 ? 192 : 128, 0, s>>>(P);
+  encode_kernel<MODE><<<(unsigned)h->n_streams, 192, 0, s>>>(P);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
-  h->fresh = false;
-  return TFCB_OK;
-}
-
-// Initial state of a handle that finalizes without having encoded anything.
-int init_state_if_fresh(tfcb_encoder* h, cudaStream_t s) {
-  if (!h->fresh) return TFCB_OK;
-  if (h->n_streams > 0) {
-    enc_init_state_kernel<<<(unsigned)((h->n_streams + 255) / 256), 256, 0, s>>>(h->state, h->n_streams);
-    TFCB_LAUNCHED();
-    TFCB_CUDA_TRY(cudaGetLastError());
-  }
   h->fresh = false;
   return TFCB_OK;
 }
@@ -1947,28 +1873,43 @@ EncResult* mapped_result(EncResult** dev) {
   return host;
 }
 
-// Lengths, offsets (into `offsets`), the one host round trip, then the deferred argument errors and the total.
-int enc_offsets(tfcb_encoder* h, long long* offsets, bool reset_err, cudaStream_t s, long long* total) {
+// Lengths, offsets (into `offsets`), the one host round trip, then the deferred argument errors (`what` selects their
+// wording, see decode_error) and the total.
+int enc_offsets(const EncArena& a, long long* offsets, bool reset_err, const char* what, cudaStream_t s,
+                long long* total) {
   EncResult* dres = nullptr;
   EncResult* res = mapped_result(&dres);
   if (!res) return fail(TFCB_CUDA_ERROR, "could not allocate host-mapped memory for the finalize result");
-  enc_offsets_kernel<<<1, 1024, 0, s>>>(h->state, h->words, h->cap, h->n_streams, offsets, h->err,
-                                         reset_err ? 1 : 0, dres);
+  enc_offsets_kernel<<<1, 1024, 0, s>>>(a.state, a.words, a.cap, a.n_streams, offsets, a.err, reset_err ? 1 : 0,
+                                         dres);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   TFCB_CUDA_TRY(cudaStreamSynchronize(s));
   EncResult r;
   std::memcpy(&r, res, sizeof r);
   *total = r.total;
-  return decode_error(r.err, "encode");
+  return decode_error(r.err, what);
 }
 
-void enc_write(tfcb_encoder* h, const long long* offsets, uint8_t* out, cudaStream_t s) {
-  if (h->n_streams > 0) {
-    enc_write_kernel<<<(unsigned)h->n_streams, 32 * kWriteWarps, 0, s>>>(h->state, h->words, h->cbits, h->cap,
-                                                                        h->n_streams, offsets, out);
+void enc_write(const EncArena& a, const long long* offsets, uint8_t* out, cudaStream_t s) {
+  if (a.n_streams > 0) {
+    enc_write_kernel<<<(unsigned)a.n_streams, 32 * kWriteWarps, 0, s>>>(a.state, a.words, a.cbits, a.cap,
+                                                                       a.n_streams, offsets, out);
     TFCB_LAUNCHED();
   }
+}
+
+// Finalize of an encoder handle up to its output size: the initial state if nothing was encoded, an arena for
+// enc_write_kernel to read even then, and enc_offsets.
+int finalize_encoder(tfcb_encoder* h, long long* offsets, bool reset_err, cudaStream_t s, long long* total) {
+  if (h->cap == 0) TFCB_TRY(ensure_capacity(h, 0, s));
+  if (h->fresh && h->n_streams > 0) {
+    enc_init_state_kernel<<<(unsigned)((h->n_streams + 255) / 256), 256, 0, s>>>(h->state, h->n_streams);
+    TFCB_LAUNCHED();
+    TFCB_CUDA_TRY(cudaGetLastError());
+  }
+  h->fresh = false;
+  return enc_offsets(*h, offsets, reset_err, "encode", s, total);
 }
 
 }  // namespace
@@ -2030,47 +1971,31 @@ int tfcb_encoder_check(tfcb_encoder* h, void* stream) {
   return fetch_error(h->err, as_stream(stream), "encode");
 }
 
-int tfcb_encode_finalize(tfcb_encoder* h, void* stream, int64_t* total_bytes_host) {
+int tfcb_encode_finalize(tfcb_encoder* h, int64_t* offsets_dev, void* stream, int64_t* total_bytes_host) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
   if (h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
-  cudaStream_t s = as_stream(stream);
-  const long long S = h->n_streams;
-  // (a finalize retried after a deferred argument error reuses the buffers of the first attempt)
-  if (!h->offsets) TFCB_TRY(dev_alloc((void**)&h->offsets, (S + 1) * sizeof(long long), s));
-  if (h->cap == 0) TFCB_TRY(ensure_capacity(h, 0, s));
-  TFCB_TRY(init_state_if_fresh(h, s));
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
   long long total = 0;
-  TFCB_TRY(enc_offsets(h, h->offsets, /*reset_err=*/false, s, &total));
-  h->total = total;
-  TFCB_TRY(dev_alloc((void**)&h->out, (size_t)std::max<long long>(total, 1), s));
-  enc_write(h, h->offsets, h->out, s);
-  TFCB_CUDA_TRY(cudaGetLastError());
-  // the word arena is no longer needed
-  dev_free(h->words, s);
-  dev_free(h->cbits, s);
-  h->words = nullptr;
-  h->cbits = nullptr;
+  // (the error record is not reset: a finalize retried after an argument error fails again)
+  TFCB_TRY(finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/false, as_stream(stream),
+                            &total));
   h->finalized = true;
   if (total_bytes_host) *total_bytes_host = total;
   return TFCB_OK;
 }
 
-int tfcb_encoder_output(tfcb_encoder* h, const uint8_t** bytes_dev, const int64_t** offsets_dev) {
-  if (!h || !h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle is not finalized");
-  if (bytes_dev) *bytes_dev = h->out;
-  if (offsets_dev) *offsets_dev = reinterpret_cast<const int64_t*>(h->offsets);
-  return TFCB_OK;
-}
-
-int tfcb_encoder_copy_output(tfcb_encoder* h, uint8_t* bytes_host, int64_t* offsets_host, void* stream) {
-  if (!h || !h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle is not finalized");
+int tfcb_encode_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
+  if (!h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle is not finalized");
+  // (the first write frees the word arena)
+  if (!h->words) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
   cudaStream_t s = as_stream(stream);
-  if (bytes_host && h->total > 0)
-    TFCB_CUDA_TRY(cudaMemcpyAsync(bytes_host, h->out, (size_t)h->total, cudaMemcpyDeviceToHost, s));
-  if (offsets_host)
-    TFCB_CUDA_TRY(cudaMemcpyAsync(offsets_host, h->offsets, (h->n_streams + 1) * sizeof(long long),
-                                  cudaMemcpyDeviceToHost, s));
-  TFCB_CUDA_TRY(cudaStreamSynchronize(s));
+  enc_write(*h, reinterpret_cast<const long long*>(offsets_dev), bytes_dev, s);
+  TFCB_CUDA_TRY(cudaGetLastError());
+  dev_free(h->words, s);
+  dev_free(h->cbits, s);
+  h->words = nullptr;
+  h->cbits = nullptr;
   return TFCB_OK;
 }
 
@@ -2082,8 +2007,6 @@ void tfcb_encoder_destroy(tfcb_encoder* h) {
   dev_free(h->words, s);
   dev_free(h->cbits, s);
   dev_free(h->err, s);
-  dev_free(h->offsets, s);
-  dev_free(h->out, s);
   if (h->done) cudaEventDestroy(h->done);
   delete h;
 }
@@ -2169,7 +2092,6 @@ int checkout_encoder(const int32_t* lookup_host, int64_t lookup_len, int64_t loo
   }
   h->home = s;
   h->bound = 0;
-  h->total = 0;
   h->fresh = true;
   h->finalized = false;
   *out = h;
@@ -2202,11 +2124,9 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
       rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s);
       break;
   }
-  if (rc == TFCB_OK && h->cap == 0) rc = ensure_capacity(h, 0, s);
-  if (rc == TFCB_OK) rc = init_state_if_fresh(h, s);
   long long total = 0;
   if (rc == TFCB_OK)
-    rc = enc_offsets(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
+    rc = finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
   if (rc != TFCB_OK) {
     // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
     if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
@@ -2221,7 +2141,7 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
   cudaStream_t s = as_stream(stream);
-  enc_write(h, reinterpret_cast<const long long*>(offsets_dev), bytes_dev, s);
+  enc_write(*h, reinterpret_cast<const long long*>(offsets_dev), bytes_dev, s);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || cudaEventRecord(h->done, s) != cudaSuccess) {
     (void)cudaGetLastError();
@@ -2441,74 +2361,58 @@ int tfcb_range_encode(const int16_t* data_dev, const int64_t* data_shape_host, i
   long long n = 0, rows = 0;
   TFCB_TRY(legacy_prepare(data_shape_host, rank, cdf_shape_host, cdf_rank, precision, debug_level, &dims,
                           &n, &rows));
-  const long long cap = (((n * precision + 15) / 16 + 2 + 32) + 31) & ~31ll;
-  if (cap >= (1ll << 31) - 64) return fail(TFCB_INVALID_ARGUMENT, "input too large for one code stream");
-  EncState* state = nullptr;
-  uint16_t* words = nullptr;
-  uint32_t* cbits = nullptr;
-  DevError* err = nullptr;
-  long long* lens = nullptr;
+  EncArena a;
+  a.n_streams = 1;
+  a.cap = (((n * precision + 15) / 16 + 2 + 32) + 31) & ~31ll;
+  if (a.cap >= (1ll << 31) - 64) return fail(TFCB_INVALID_ARGUMENT, "input too large for one code stream");
+  long long* offsets = nullptr;
   uint8_t* out = nullptr;
-  int rc = dev_alloc((void**)&state, sizeof(EncState), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&words, cap * sizeof(uint16_t), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&cbits, (cap >> 5) * sizeof(uint32_t), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&err, sizeof(DevError), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&lens, 3 * sizeof(long long), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&out, (size_t)(2 * cap + 8), s);
+  int rc = dev_alloc((void**)&a.state, sizeof(EncState), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&a.words, a.cap * sizeof(uint16_t), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&a.cbits, (a.cap >> 5) * sizeof(uint32_t), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&a.err, sizeof(DevError), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&offsets, 2 * sizeof(long long), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&out, (size_t)(2 * a.cap + 8), s);
   auto cleanup = [&]() {
-    dev_free(state, s);
-    dev_free(words, s);
-    dev_free(cbits, s);
-    dev_free(err, s);
-    dev_free(lens, s);
+    dev_free(a.state, s);
+    dev_free(a.words, s);
+    dev_free(a.cbits, s);
+    dev_free(a.err, s);
+    dev_free(offsets, s);
     dev_free(out, s);
   };
   if (rc != TFCB_OK) {
     cleanup();
     return rc;
   }
-  cudaMemsetAsync(err, 0, sizeof(DevError), s);
+  cudaMemsetAsync(a.err, 0, sizeof(DevError), s);
   if (debug_level > 0 && rows > 0) {
     legacy_check_cdf_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, s>>>(cdf_dev, rows, dims.chip,
-                                                                          precision, err);
+                                                                          precision, a.err);
     TFCB_LAUNCHED();
-    rc = fetch_error(err, s, "legacy");
+    rc = fetch_error(a.err, s, "legacy");
     if (rc != TFCB_OK) {
       cleanup();
       return rc;
     }
   }
-  legacy_encode_kernel<<<1, 32, 0, s>>>(data_dev, n, cdf_dev, dims, precision, debug_level, state, words,
-                                        cbits, cap, err);
-  TFCB_LAUNCHED();
-  rc = fetch_error(err, s, "legacy");
-  if (rc != TFCB_OK) {
-    cleanup();
-    return rc;
-  }
-  enc_lengths_kernel<<<1, 32, 0, s>>>(state, words, cap, 1, lens);
-  exclusive_scan_kernel<<<1, 32, 0, s>>>(lens, 1, lens + 1);
-  enc_write_kernel<<<1, 32 * kWriteWarps, 0, s>>>(state, words, cbits, cap, 1, lens + 1, out);
-  TFCB_LAUNCHED();
-  TFCB_LAUNCHED();
+  legacy_encode_kernel<<<1, 32, 0, s>>>(data_dev, n, cdf_dev, dims, precision, debug_level, a.state, a.words,
+                                        a.cbits, a.cap, a.err);
   TFCB_LAUNCHED();
   long long total = 0;
-  cudaMemcpyAsync(&total, lens, sizeof total, cudaMemcpyDeviceToHost, s);
-  cudaError_t e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) {
-    cleanup();
-    return fail(TFCB_CUDA_ERROR, "CUDA error '%s' in tfcb_range_encode", cudaGetErrorString(e));
+  rc = enc_offsets(a, offsets, /*reset_err=*/false, "legacy", s, &total);
+  if (rc == TFCB_OK) {
+    if (n_bytes_host) *n_bytes_host = total;
+    if (total > out_cap) rc = fail(TFCB_INVALID_ARGUMENT, "output buffer too small: need %lld bytes", total);
   }
-  if (n_bytes_host) *n_bytes_host = total;
-  if (total > out_cap) {
-    cleanup();
-    return fail(TFCB_INVALID_ARGUMENT, "output buffer too small: need %lld bytes", total);
+  if (rc == TFCB_OK) {
+    enc_write(a, offsets, out, s);
+    if (total > 0) cudaMemcpyAsync(out_host, out, (size_t)total, cudaMemcpyDeviceToHost, s);
+    const cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) rc = fail(TFCB_CUDA_ERROR, "CUDA error '%s' in tfcb_range_encode", cudaGetErrorString(e));
   }
-  if (total > 0) cudaMemcpyAsync(out_host, out, (size_t)total, cudaMemcpyDeviceToHost, s);
-  e = cudaStreamSynchronize(s);
   cleanup();
-  if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "CUDA error '%s' in tfcb_range_encode", cudaGetErrorString(e));
-  return TFCB_OK;
+  return rc;
 }
 
 int tfcb_range_decode(const uint8_t* encoded_host, int64_t n_bytes, const int64_t* shape_host, int rank,

@@ -81,11 +81,10 @@ class Strings:
   them.  ``tolist()`` / ``numpy()`` copy to the host lazily.
   """
 
-  def __init__(self, bytes_dev: torch.Tensor, offsets_dev: torch.Tensor, shape, owner=None):
+  def __init__(self, bytes_dev: torch.Tensor, offsets_dev: torch.Tensor, shape):
     self.bytes_dev = bytes_dev
     self.offsets_dev = offsets_dev
     self.shape = tuple(int(d) for d in shape)
-    self._owner = owner  # keeps the producing handle (and its device memory) alive
     self._host = None
 
   @classmethod
@@ -242,34 +241,13 @@ def entropy_encode_index(handle: EncoderHandle, index, value) -> EncoderHandle:
 def entropy_encode_finalize(handle: EncoderHandle) -> Strings:
   """EntropyEncodeFinalize (cc/ops/range_coder_ops.cc:123-135): one string per handle element."""
   handle._require()
-  total = C.c_int64(0)
-  check(_lib.lib().tfcb_encode_finalize(handle._h, _stream(), C.byref(total)))
-  bp, op = C.c_void_p(), C.c_void_p()
-  check(_lib.lib().tfcb_encoder_output(handle._h, C.byref(bp), C.byref(op)))
   dev = _device()
-  nbytes = max(int(total.value), 1)
-  bytes_dev = _wrap(bp.value, nbytes, torch.uint8, dev)
-  offsets_dev = _wrap(op.value, handle.n_streams + 1, torch.int64, dev)
-  return Strings(bytes_dev, offsets_dev, handle.shape, owner=handle)
-
-
-def _wrap(ptr: int, n: int, dtype, dev) -> torch.Tensor:
-  """Zero-copy torch view of library-owned device memory (kept alive by the owning handle)."""
-  itemsize = torch.empty((), dtype=dtype).element_size()
-
-  class _Mem:  # __cuda_array_interface__ provider
-    pass
-
-  m = _Mem()
-  m.__cuda_array_interface__ = {
-      "shape": (n,),
-      "typestr": {torch.uint8: "|u1", torch.int64: "<i8", torch.int32: "<i4"}[dtype],
-      "data": (int(ptr), False),
-      "version": 2,
-      "strides": None,
-  }
-  del itemsize
-  return torch.as_tensor(m, device=dev)
+  offsets = torch.empty(handle.n_streams + 1, dtype=torch.int64, device=dev)
+  total = C.c_int64(0)
+  check(_lib.lib().tfcb_encode_finalize(handle._h, _ptr(offsets), _stream(), C.byref(total)))
+  out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
+  check(_lib.lib().tfcb_encode_write(handle._h, _ptr(offsets), _ptr(out), _stream()))
+  return Strings(out, offsets, handle.shape)
 
 
 # ------------------------------------------------------------------------------------------------

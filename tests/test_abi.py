@@ -18,10 +18,12 @@ def _declared():
   return sorted(set(PROTO.findall(text)))
 
 
-def test_library_exists_and_loads():
+def test_library_loads_and_reports_the_header_abi_version():
   assert os.path.exists(_lib.LIB_PATH), "run `python -c 'import __graft_entry__ as g; g.build()'` first"
   lib = _lib.lib()
-  assert lib.tfcb_abi_version() == 1
+  with open(_lib.HEADER_PATH) as f:
+    declared = int(re.search(r"^#define TFCB_ABI_VERSION (\d+)$", f.read(), re.M).group(1))
+  assert lib.tfcb_abi_version() == declared == 2
   assert _lib.last_error() == ""
   assert _lib.launch_count() >= 0
 
