@@ -364,7 +364,21 @@ struct EncParams {
   uint32_t* cbits;
   long long cap;  // words per stream
   DevError* err;
+  // Ragged batches: stream s is symbols [sym_off[s], sym_off[s+1]) and arena words [arena_off[s], arena_off[s+1])
+  // (multiples of 32).  Null: stream s is symbols [s * n, s * n + n) and words [s * cap, s * cap + cap).
+  const long long* sym_off;
+  const long long* arena_off;
 };
+
+// Where one stream's symbols (or arena words) are: resolved once per CTA from the offsets array when there is one,
+// else from the uniform stride.
+struct Extent {
+  long long base, len;
+};
+__device__ __forceinline__ Extent stream_extent(const long long* off, long long s, long long stride) {
+  if (off) return Extent{off[s], off[s + 1] - off[s]};
+  return Extent{s * stride, stride};
+}
 
 // The gather of one pass of 32 symbols is split in two stages so that no global-memory latency is
 // ever exposed to the (in-order) warp:
@@ -389,8 +403,9 @@ struct Gathered {
   uint32_t sign;
 };
 
+// `at`: absolute symbol position; the stream's symbols end at `end`.
 template <int MODE>
-__device__ __forceinline__ Fetched enc_fetch(const EncParams& P, long long s, long long j, uint32_t chan_row) {
+__device__ __forceinline__ Fetched enc_fetch(const EncParams& P, long long end, long long at, uint32_t chan_row) {
   Fetched f;
   f.y = 0.f;
   f.v = 0;
@@ -398,9 +413,8 @@ __device__ __forceinline__ Fetched enc_fetch(const EncParams& P, long long s, lo
   f.coff = 0;
   f.row = (int)chan_row;
   f.ri = make_int2(0, 0);
-  f.valid = j < P.n;
+  f.valid = at < end;
   if (!f.valid) return f;
-  const long long at = s * P.n + j;
   if (MODE & kModeF32) {
     f.y = __ldg(reinterpret_cast<const float*>(P.value) + at);
   } else {
@@ -419,8 +433,10 @@ __device__ __forceinline__ Fetched enc_fetch(const EncParams& P, long long s, lo
   return f;
 }
 
+// `at`: absolute symbol position.  Errors name the stream and the position inside it (the stream's start is looked
+// up again there rather than kept live beside the gather loop).
 template <int MODE>
-__device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, long long j, Fetched f) {
+__device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, long long at, Fetched f) {
   Gathered g;
   g.ops = make_uint4(0u, 0u, 0u, 0u);
   g.prec = 0;
@@ -429,7 +445,7 @@ __device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, 
   if (!f.valid) return g;
   if (MODE & kModeIndex) {
     if (f.row < 0 || f.row >= P.n_rows) {
-      report(P.err, kErrIndex, s, j, f.row, P.n_rows);
+      report(P.err, kErrIndex, s, at - stream_extent(P.sym_off, s, P.n).base, f.row, P.n_rows);
       return g;
     }
     f.ri = __ldg(P.rows + f.row);
@@ -440,7 +456,7 @@ __device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, 
   const int ncdf = row_ncdf(f.ri.y);
   if (!row_ovf(f.ri.y)) {
     if (v < 0 || v >= ncdf - 1) {
-      report(P.err, kErrValue, s, j, v, ncdf - 1);
+      report(P.err, kErrValue, s, at - stream_extent(P.sym_off, s, P.n).base, v, ncdf - 1);
       return g;
     }
   } else {
@@ -578,26 +594,27 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
         if (row_a >= (uint32_t)P.n_rows) row_a -= (uint32_t)P.n_rows;
       }
     };
+    // absolute symbol positions: only the stream's end stays live beside the loop
+    const Extent x = stream_extent(P.sym_off, s, P.n);
+    const long long end = x.base + x.len;
     // stage A (symbol loads) runs three 32-symbol passes ahead of stage B: no global latency is waited for
-    Fetched f0 = enc_fetch<MODE>(P, s, lane, row_a);
+    Fetched f0 = enc_fetch<MODE>(P, end, x.base + lane, row_a);
     advance_row();
-    Fetched f1 = enc_fetch<MODE>(P, s, 32 + lane, row_a);
+    Fetched f1 = enc_fetch<MODE>(P, end, x.base + 32 + lane, row_a);
     advance_row();
-    Fetched f2 = enc_fetch<MODE>(P, s, 64 + lane, row_a);
+    Fetched f2 = enc_fetch<MODE>(P, end, x.base + 64 + lane, row_a);
     advance_row();
     RecordWriter w;
     w.begin(&sh);
-    const long long n_pass = (P.n + 31) / 32;
     bool stop = false;
-    for (long long pass = 0; pass < n_pass && !stop; ++pass) {
+    for (long long j0 = x.base; j0 < end && !stop; j0 += 32) {
       const Fetched fcur = f0;
       f0 = f1;
       f1 = f2;
-      f2 = enc_fetch<MODE>(P, s, (pass + 3) * 32 + lane, row_a);
+      f2 = enc_fetch<MODE>(P, end, j0 + 96 + lane, row_a);
       advance_row();
-      const long long j0 = pass * 32;
       const Gathered cur = enc_gather<MODE>(P, s, j0 + lane, fcur);
-      const int count = (int)min(32ll, P.n - j0);
+      const int count = (int)min(32ll, end - j0);
       const bool has = lane < count;
       const unsigned esc_mask = __ballot_sync(kFull, cur.gamma != 0);
       const unsigned bad_mask = __ballot_sync(kFull, cur.prec == 0 && has);
@@ -634,8 +651,9 @@ __global__ void __launch_bounds__(192) encode_kernel(const EncParams P) {
   if (warp == 5) {
     // ------------------------------- drain warp -------------------------------
     EncDrain d;
-    d.begin(P.fresh ? enc_initial_state() : P.state[s], P.words + s * P.cap, P.cbits + s * (P.cap >> 5),
-            (uint32_t)P.cap, lane);
+    const Extent a = stream_extent(P.arena_off, s, P.cap);
+    d.begin(P.fresh ? enc_initial_state() : P.state[s], P.words + a.base, P.cbits + (a.base >> 5), (uint32_t)a.len,
+            lane);
     for (long long k = 0;; ++k) {
       const int b = (int)(k & 1);
       bar_sync(kBarEntFull + b, 64);
@@ -755,6 +773,7 @@ struct EncArena {
   uint32_t* cbits = nullptr;
   long long cap = 0;  // words per stream (multiple of 32)
   DevError* err = nullptr;
+  const long long* arena_off = nullptr;  // device [n_streams + 1]: per-stream word ranges of a ragged batch (else cap)
 };
 
 // Finalize in one block: every stream's string length (enc_final_length), their exclusive scan into
@@ -762,7 +781,8 @@ struct EncArena {
 // synchronisation is the only round trip.  `reset_err` clears the error record for the next user of a recycled
 // encoder.
 __global__ void __launch_bounds__(1024) enc_offsets_kernel(const EncState* state, const uint16_t* words,
-                                                           long long cap, long long n_streams, long long* offsets,
+                                                           long long cap, const long long* arena_off,
+                                                           long long n_streams, long long* offsets,
                                                            DevError* err, int reset_err, EncResult* res) {
   __shared__ long long warp_sums[32];
   __shared__ long long carry_s;
@@ -776,7 +796,7 @@ __global__ void __launch_bounds__(1024) enc_offsets_kernel(const EncState* state
       bool straddle;
       uint32_t tail;
       int ntail;
-      v = enc_final_length(state[i], words + i * cap, &straddle, &tail, &ntail);
+      v = enc_final_length(state[i], words + (arena_off ? arena_off[i] : i * cap), &straddle, &tail, &ntail);
     }
     long long x = v;
 #pragma unroll
@@ -819,15 +839,16 @@ constexpr int kWriteWarps = 8;
 
 __global__ void __launch_bounds__(32 * kWriteWarps) enc_write_kernel(const EncState* state, const uint16_t* words,
                                                                     const uint32_t* cbits, long long cap,
-                                                                    long long n_streams,
+                                                                    const long long* arena_off, long long n_streams,
                                                                     const long long* offsets, uint8_t* out) {
   __shared__ uint32_t seg_out[kWriteWarps][2];
   const long long s = blockIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (s >= n_streams) return;
   const EncState st = state[s];
-  const uint16_t* w = words + s * cap;
-  const uint32_t* cb = cbits + s * (cap >> 5);
+  const long long abase = arena_off ? arena_off[s] : s * cap;
+  const uint16_t* w = words + abase;
+  const uint32_t* cb = cbits + (abase >> 5);
   uint8_t* dst = out + offsets[s];
   bool straddle;
   uint32_t tail;
@@ -940,6 +961,7 @@ struct DecParams {
   long long n_streams;
   DecState* state;
   DevError* err;
+  const long long* sym_off;  // ragged batches: stream s is symbols [sym_off[s], sym_off[s+1]); null: [s * n, s * n + n)
 };
 
 struct ByteWindow {
@@ -1170,7 +1192,8 @@ __global__ void __launch_bounds__(96) decode_kernel(const DecParams P) {
   const long long s = blockIdx.x;
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;  // 0 chain, 1 prepare, 2 resolve
-  const long long n_groups = (P.n + kDecGroup - 1) / kDecGroup;
+  const Extent x = stream_extent(P.sym_off, s, P.n);
+  const long long n_groups = (x.len + kDecGroup - 1) / kDecGroup;
 
   // tables: shared memory when they fit (loaded by all three warps), global (L1/L2) otherwise
   const uint2* pairs = P.pairs;
@@ -1211,8 +1234,8 @@ __global__ void __launch_bounds__(96) decode_kernel(const DecParams P) {
         int row = (int)chan_row;
         if (MODE & kModeIndex) {
           row = 0;
-          if (j < P.n) {
-            row = __ldg(P.index + s * P.n + j);
+          if (j < x.len) {
+            row = __ldg(P.index + x.base + j);
             if (row < 0 || row >= P.n_rows) {
               report(P.err, kErrIndex, s, j, row, P.n_rows);
               row = -1;
@@ -1235,7 +1258,7 @@ __global__ void __launch_bounds__(96) decode_kernel(const DecParams P) {
       }
       if (lane == 0) {
         sh.bad[b] = bad;
-        sh.count[b] = (unsigned)min((long long)kDecGroup, P.n - g * kDecGroup);
+        sh.count[b] = (unsigned)min((long long)kDecGroup, x.len - g * kDecGroup);
       }
       bar_arrive(kBarDescFull + b, 64);
       if (bad) break;
@@ -1254,7 +1277,7 @@ __global__ void __launch_bounds__(96) decode_kernel(const DecParams P) {
         const int k = sub * 32 + lane;
         const long long j = g * kDecGroup + k;
         if (k < count) {
-          const long long at = s * P.n + j;
+          const long long at = x.base + j;
           int row;
           if (MODE & kModeIndex) row = __ldg(P.index + at);
           else row = (int)(j % P.n_rows);
@@ -1781,21 +1804,25 @@ struct tfcb_encoder : EncArena {
   // reads the word arena, and the next user's stream waits for it
   int device = 0;
   cudaEvent_t done = nullptr;
+  long long arena_words = 0;  // words allocated in `words` (cbits: arena_words / 32): n_streams * cap, or more
+  long long* ext = nullptr;   // ragged batches, device [2 * (n_streams + 1)]: symbol offsets, then arena offsets
 };
 
 namespace {
 
 // Worst-case 16-bit words one call can append per stream: every Encode(.., p) shrinks the interval by
 // at most 2^p, i.e. consumes at most p bits; an escape adds at most 65 one-bit symbols.
+long long bits_bound(int max_prec, bool any_overflow) { return max_prec + (any_overflow ? 65 : 0); }
+long long words_for(long long bits, long long n) { return (n * bits + 15) / 16 + 2; }
 long long words_bound(const tfcb_encoder* h, long long n) {
-  const long long bits = h->lut.max_prec + (h->lut.any_overflow ? 65 : 0);
-  return (n * bits + 15) / 16 + 2;
+  return words_for(bits_bound(h->lut.max_prec, h->lut.any_overflow), n);
 }
+constexpr long long kMaxStreamWords = (1ll << 31) - 64;  // a stream's word count and positions fit 32 bits
 
 int ensure_capacity(tfcb_encoder* h, long long extra_words, cudaStream_t s) {
   const long long need = h->bound + extra_words + 32;
   if (need <= h->cap) return TFCB_OK;
-  if (need >= (1ll << 31) - 64)
+  if (need >= kMaxStreamWords)
     return fail(TFCB_INVALID_ARGUMENT, "a single code stream may not exceed 2^31 16-bit words");
   const long long new_cap = (std::max(need, h->cap * 2) + 31) & ~31ll;
   uint16_t* nw = nullptr;
@@ -1814,12 +1841,63 @@ int ensure_capacity(tfcb_encoder* h, long long extra_words, cudaStream_t s) {
   h->words = nw;
   h->cbits = nc;
   h->cap = new_cap;
+  h->arena_words = S * new_cap;
   return TFCB_OK;
 }
 
+// Host-side checks of a ragged batch's symbol offsets [n_streams + 1].
+int check_symbol_offsets(const int64_t* off, long long n_streams) {
+  if (n_streams <= 0) return fail(TFCB_INVALID_ARGUMENT, "`n_streams` must be positive: %lld", n_streams);
+  if (!off) return fail(TFCB_INVALID_ARGUMENT, "`symbol_offsets` is null");
+  if (off[0] != 0) return fail(TFCB_INVALID_ARGUMENT, "symbol_offsets[0] must be 0: %lld", (long long)off[0]);
+  for (long long i = 0; i < n_streams; ++i)
+    if (off[i + 1] < off[i])
+      return fail(TFCB_INVALID_ARGUMENT,
+                  "symbol_offsets must be non-decreasing: symbol_offsets[%lld]=%lld > symbol_offsets[%lld]=%lld", i,
+                  (long long)off[i], i + 1, (long long)off[i + 1]);
+  return TFCB_OK;
+}
+
+// Lays out a ragged batch's arena on a fresh (pooled) encoder: stream s gets its own worst case rounded to 32
+// words, so the arena is the sum of the per-stream bounds rather than n_streams times the longest one.  Uploads the
+// symbol and arena offsets in one copy and points the encoder at them.  The arena only grows.
+int prepare_ragged(tfcb_encoder* h, const int64_t* sym_off, cudaStream_t s) {
+  const long long S = h->n_streams;
+  std::vector<long long> off(2 * (S + 1));
+  long long* arena = off.data() + S + 1;
+  long long total = 0;
+  for (long long i = 0; i <= S; ++i) {
+    off[i] = sym_off[i];
+    arena[i] = total;
+    if (i < S) total += (words_bound(h, sym_off[i + 1] - sym_off[i]) + 32 + 31) & ~31ll;
+  }
+  if (total > h->arena_words) {
+    uint16_t* nw = nullptr;
+    uint32_t* nc = nullptr;
+    TFCB_TRY(dev_alloc((void**)&nw, (size_t)total * sizeof(uint16_t), s));
+    const int rc = dev_alloc((void**)&nc, (size_t)(total >> 5) * sizeof(uint32_t), s);
+    if (rc != TFCB_OK) {
+      dev_free(nw, s);
+      return rc;
+    }
+    dev_free(h->words, s);
+    dev_free(h->cbits, s);
+    h->words = nw;
+    h->cbits = nc;
+    h->arena_words = total;
+    h->cap = (total / S) & ~31ll;  // what a later uniform batch of this pooled encoder may use of the same arena
+  }
+  if (!h->ext) TFCB_TRY(dev_alloc((void**)&h->ext, off.size() * sizeof(long long), s));
+  // (pageable source: staged before the call returns)
+  TFCB_CUDA_TRY(cudaMemcpyAsync(h->ext, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice, s));
+  h->arena_off = h->ext + S + 1;
+  return TFCB_OK;
+}
+
+// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all, laid out by prepare_ragged.
 template <int MODE>
 int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s) {
+                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr) {
   if (h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
@@ -1827,9 +1905,11 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   if (value == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`value` is null");
   if ((MODE & kModeIndex) && index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
   if ((MODE & kModeF32) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
-  const long long extra = words_bound(h, n);
-  TFCB_TRY(ensure_capacity(h, extra, s));
-  h->bound += extra;
+  if (!sym_off) {
+    const long long extra = words_bound(h, n);
+    TFCB_TRY(ensure_capacity(h, extra, s));
+    h->bound += extra;
+  }
   EncParams P;
   P.lookup = h->lut.lookup;
   P.rows = h->lut.rows;
@@ -1847,6 +1927,8 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.cbits = h->cbits;
   P.cap = h->cap;
   P.err = h->err;
+  P.sym_off = sym_off;
+  P.arena_off = h->arena_off;
   if (h->n_streams > 0x7FFFFFFFll) return fail(TFCB_INVALID_ARGUMENT, "too many streams");
   encode_kernel<MODE><<<(unsigned)h->n_streams, 192, 0, s>>>(P);
   TFCB_LAUNCHED();
@@ -1880,8 +1962,8 @@ int enc_offsets(const EncArena& a, long long* offsets, bool reset_err, const cha
   EncResult* dres = nullptr;
   EncResult* res = mapped_result(&dres);
   if (!res) return fail(TFCB_CUDA_ERROR, "could not allocate host-mapped memory for the finalize result");
-  enc_offsets_kernel<<<1, 1024, 0, s>>>(a.state, a.words, a.cap, a.n_streams, offsets, a.err, reset_err ? 1 : 0,
-                                         dres);
+  enc_offsets_kernel<<<1, 1024, 0, s>>>(a.state, a.words, a.cap, a.arena_off, a.n_streams, offsets, a.err,
+                                         reset_err ? 1 : 0, dres);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   TFCB_CUDA_TRY(cudaStreamSynchronize(s));
@@ -1894,7 +1976,7 @@ int enc_offsets(const EncArena& a, long long* offsets, bool reset_err, const cha
 void enc_write(const EncArena& a, const long long* offsets, uint8_t* out, cudaStream_t s) {
   if (a.n_streams > 0) {
     enc_write_kernel<<<(unsigned)a.n_streams, 32 * kWriteWarps, 0, s>>>(a.state, a.words, a.cbits, a.cap,
-                                                                       a.n_streams, offsets, out);
+                                                                       a.arena_off, a.n_streams, offsets, out);
     TFCB_LAUNCHED();
   }
 }
@@ -2007,6 +2089,7 @@ void tfcb_encoder_destroy(tfcb_encoder* h) {
   dev_free(h->words, s);
   dev_free(h->cbits, s);
   dev_free(h->err, s);
+  dev_free(h->ext, s);
   if (h->done) cudaEventDestroy(h->done);
   delete h;
 }
@@ -2094,7 +2177,37 @@ int checkout_encoder(const int32_t* lookup_host, int64_t lookup_len, int64_t loo
   h->bound = 0;
   h->fresh = true;
   h->finalized = false;
+  h->arena_off = nullptr;
   *out = h;
+  return TFCB_OK;
+}
+
+// The common part of tfcb_compress and tfcb_compress_ragged: one encode of a checked-out encoder, finalize, and
+// the encoder either handed to the caller or taken back.
+int compress_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
+                         const float* qoff_dev, const int32_t* cdf_offset_dev, long long n, const long long* sym_off,
+                         int64_t* offsets_dev, cudaStream_t s, tfcb_encoder** out, int64_t* total_bytes_host) {
+  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0);
+  int rc;
+  switch (mode) {
+    case 0: rc = launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, s, sym_off); break;
+    case kModeIndex: rc = launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, s, sym_off); break;
+    case kModeF32: rc = launch_encode<kModeF32>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s, sym_off); break;
+    default:
+      rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s, sym_off);
+      break;
+  }
+  long long total = 0;
+  if (rc == TFCB_OK)
+    rc = finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
+  if (rc != TFCB_OK) {
+    // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
+    if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
+    else tfcb_encoder_destroy(h);
+    return rc;
+  }
+  *out = h;
+  *total_bytes_host = total;
   return TFCB_OK;
 }
 
@@ -2114,28 +2227,44 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
   cudaStream_t s = as_stream(stream);
   tfcb_encoder* h = nullptr;
   TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
-  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0);
-  int rc;
-  switch (mode) {
-    case 0: rc = launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, s); break;
-    case kModeIndex: rc = launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, s); break;
-    case kModeF32: rc = launch_encode<kModeF32>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s); break;
-    default:
-      rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s);
-      break;
+  return compress_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev, n, nullptr,
+                              offsets_dev, s, out, total_bytes_host);
+}
+
+int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                         const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                         int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
+                         int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  *out = nullptr;
+  *total_bytes_host = 0;
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
+  // the per-stream size limit needs the table's worst case bits per symbol: parsed here, before any device work
+  {
+    std::vector<HostRow> rows;
+    TFCB_TRY(parse_lookup(lookup_host, lookup_len, lookup_cols, &rows));
+    int max_prec = 0;
+    bool any_overflow = false;
+    for (const HostRow& r : rows) {
+      max_prec = std::max(max_prec, r.prec < 0 ? -r.prec : r.prec);
+      any_overflow |= r.prec < 0;
+    }
+    const long long bits = bits_bound(max_prec, any_overflow);
+    for (long long i = 0; i < n_streams; ++i)
+      if (words_for(bits, symbol_offsets_host[i + 1] - symbol_offsets_host[i]) + 32 >= kMaxStreamWords)
+        return fail(TFCB_INVALID_ARGUMENT, "a single code stream may not exceed 2^31 16-bit words (stream %lld)", i);
   }
-  long long total = 0;
-  if (rc == TFCB_OK)
-    rc = finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
+  cudaStream_t s = as_stream(stream);
+  tfcb_encoder* h = nullptr;
+  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
+  const int rc = prepare_ragged(h, symbol_offsets_host, s);
   if (rc != TFCB_OK) {
-    // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
-    if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
-    else tfcb_encoder_destroy(h);
+    tfcb_encoder_destroy(h);
     return rc;
   }
-  *out = h;
-  *total_bytes_host = total;
-  return TFCB_OK;
+  return compress_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev,
+                              symbol_offsets_host[n_streams], h->ext, offsets_dev, s, out, total_bytes_host);
 }
 
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
@@ -2164,13 +2293,15 @@ struct tfcb_decoder {
   DevError* err = nullptr;
   uint8_t* ok = nullptr;
   cudaStream_t home = nullptr;
+  long long* sym_off = nullptr;  // ragged decodes: device copy of the symbol offsets [n_streams + 1]
 };
 
 namespace {
 
+// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all.
 template <int MODE>
 int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s) {
+                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr) {
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
   if (h->lut.n_rows == 0) return fail(TFCB_INVALID_ARGUMENT, "index=0 not in range [0, 0)");
@@ -2196,6 +2327,7 @@ int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float*
   P.n_streams = h->n_streams;
   P.state = h->state;
   P.err = h->err;
+  P.sym_off = sym_off;
   // Search keys live in shared memory whenever they fit beside the kernel's static 16 KB: up to 96 KB two CTAs
   // (streams) still share an SM; up to 200 KB one CTA per SM (cfg3's 64 NoisyNormal tables up to sigma = 256 take
   // 118 KB: from L1/L2 every slow-path search round cost a global-memory latency on the chain warp).
@@ -2271,6 +2403,28 @@ int tfcb_decode_index_f32(tfcb_decoder* h, const int32_t* index_dev, float* out_
                                               as_stream(stream));
 }
 
+int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev, void* out_dev,
+                       int32_t out_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev,
+                       void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, h->n_streams));
+  const long long n = symbol_offsets_host[h->n_streams];
+  if (n == 0) return TFCB_OK;
+  cudaStream_t s = as_stream(stream);
+  if (!h->sym_off) TFCB_TRY(dev_alloc((void**)&h->sym_off, (h->n_streams + 1) * sizeof(long long), s));
+  // (pageable source: staged before the call returns; an earlier decode on this stream has read the old offsets)
+  TFCB_CUDA_TRY(cudaMemcpyAsync(h->sym_off, symbol_offsets_host, (h->n_streams + 1) * sizeof(long long),
+                                cudaMemcpyHostToDevice, s));
+  const float* q = quant_offset_dev;
+  const int32_t* c = cdf_offset_dev;
+  switch ((index_dev ? kModeIndex : 0) | (out_is_f32 ? kModeF32 : 0)) {
+    case 0: return launch_decode<0>(h, nullptr, out_dev, nullptr, nullptr, n, s, h->sym_off);
+    case kModeIndex: return launch_decode<kModeIndex>(h, index_dev, out_dev, nullptr, nullptr, n, s, h->sym_off);
+    case kModeF32: return launch_decode<kModeF32>(h, nullptr, out_dev, q, c, n, s, h->sym_off);
+    default: return launch_decode<kModeIndex | kModeF32>(h, index_dev, out_dev, q, c, n, s, h->sym_off);
+  }
+}
+
 int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
   cudaStream_t s = as_stream(stream);
@@ -2291,6 +2445,7 @@ void tfcb_decoder_destroy(tfcb_decoder* h) {
   dev_free(h->state, s);
   dev_free(h->err, s);
   dev_free(h->ok, s);
+  dev_free(h->sym_off, s);
   delete h;
 }
 

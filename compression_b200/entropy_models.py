@@ -31,6 +31,28 @@ def _cuda():
   return torch.device("cuda", torch.cuda.current_device())
 
 
+def _numel(shape):
+  return int(np.prod(shape)) if len(shape) else 1
+
+
+def _split_items(flat, shapes):
+  """Views of a flat tensor holding items of the given shapes back to back."""
+  out, at = [], 0
+  for shape in shapes:
+    n = _numel(shape)
+    out.append(flat[at:at + n].reshape(shape))
+    at += n
+  return out
+
+
+def _ragged_strings(strings, k):
+  if not isinstance(strings, gen_ops.Strings):
+    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+  if strings.numel() != k:
+    raise ValueError(f"{strings.numel()} strings for {k} items")
+  return strings
+
+
 class ContinuousEntropyModelBase(nn.Module):
   """continuous_base.py:36-370."""
 
@@ -360,6 +382,57 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
       outputs = outputs + qoff.reshape(self.prior_shape).to(outputs.dtype)
     return outputs
 
+  # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
+  def compress_ragged(self, bottlenecks):
+    """Compresses a list of coding units of different shapes in one range-coder launch.  Each item has exactly
+    `coding_rank` dimensions ending in `prior_shape` (no broadcasting).  Returns a Strings of shape (k,) whose string
+    i equals `compress(bottlenecks[i])`."""
+    self._check_compression()
+    dev = _cuda()
+    items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
+    rank_p = len(self.prior_shape)
+    for b in items:
+      if b.dim() != self.coding_rank or (rank_p and tuple(b.shape[-rank_p:]) != self.prior_shape):
+        raise ValueError(f"each item needs {self.coding_rank} dimensions ending in {self.prior_shape}: "
+                         f"received shape {tuple(b.shape)}")
+    if not items:
+      raise ValueError("`bottlenecks` is empty")
+    lengths = [b.numel() for b in items]
+    coff, qoff = self._flat_tables(dev)
+    flat = torch.cat([b.reshape(-1) for b in items])
+    if self.bottleneck_dtype == torch.float32:
+      return F.compress_ragged(self._lookup_host(), lengths, flat, qoff, coff)
+    # compress()'s unfused arithmetic; every item holds whole rows of prior_shape, so the rows line up
+    b = flat.to(torch.float32).reshape(-1, coff.numel())
+    if qoff is not None:
+      b = b - qoff
+    symbols = torch.round(b).to(torch.int32) - coff
+    return F.compress_ragged(self._lookup_host(), lengths, symbols.reshape(-1))
+
+  def decompress_ragged(self, strings, broadcast_shapes):
+    """Inverse of compress_ragged: item i has shape `broadcast_shapes[i] + prior_shape` and equals
+    `decompress(strings[i:i+1], broadcast_shapes[i])[0]`.  The items are views into one allocation."""
+    self._check_compression()
+    shapes = [tuple(int(d) for d in np.asarray(s).reshape(-1)) + self.prior_shape for s in broadcast_shapes]
+    strings = _ragged_strings(strings, len(shapes))
+    dev = strings.bytes_dev.device
+    coff, qoff = self._flat_tables(dev)
+    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
+    lengths = [_numel(s) for s in shapes]
+    if self.bottleneck_dtype == torch.float32:
+      outputs = F.decode_ragged(handle, lengths, quant_offset=qoff, cdf_offset=coff)
+    else:
+      symbols = F.decode_ragged(handle, lengths)
+    sanity = gen_ops.entropy_decode_finalize(handle)
+    if self.decode_sanity_check and not bool(sanity.all()):
+      raise gen_ops.InvalidArgumentError("Sanity check failed.")
+    if self.bottleneck_dtype != torch.float32:
+      outputs = (symbols.reshape(-1, coff.numel()) + coff).to(self.bottleneck_dtype)
+      if qoff is not None:
+        outputs = outputs + qoff.to(outputs.dtype)
+      outputs = outputs.reshape(-1)
+    return _split_items(outputs, shapes)
+
   def get_config(self):
     """continuous_batched.py:424-436."""
     config = super().get_config()
@@ -507,6 +580,72 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     out = (symbols + coff[flat.long()]).to(self.bottleneck_dtype)
     return out if _loc is None else out + _loc
 
+  # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
+  def _ragged_indexes(self, indexes, dev):
+    """Normalised, flattened table indexes of every item, concatenated, and the items' coding shapes."""
+    indexes = [torch.as_tensor(i).to(device=dev, dtype=self.prior_dtype) for i in indexes]
+    if not indexes:
+      raise ValueError("`indexes` is empty")
+    if self.channel_axis is None:  # elementwise: normalise all items at once
+      flat = self._flatten_indexes(self._normalize_indexes(torch.cat([i.reshape(-1) for i in indexes])))
+      shapes = [tuple(i.shape) for i in indexes]
+    else:
+      per_item = [self._flatten_indexes(self._normalize_indexes(i)) for i in indexes]
+      flat = torch.cat([f.reshape(-1) for f in per_item])
+      shapes = [tuple(f.shape) for f in per_item]
+    for s in shapes:
+      if len(s) != self.coding_rank:
+        raise ValueError(f"each item needs {self.coding_rank} dimensions: received indexes for shape {s}")
+    return flat, shapes
+
+  def compress_ragged(self, bottlenecks, indexes, _loc=None):
+    """Compresses a list of coding units of different shapes (each with exactly `coding_rank` dimensions) in one
+    range-coder launch.  Returns a Strings of shape (k,) whose string i equals `compress(bottlenecks[i],
+    indexes[i])`."""
+    self._check_compression()
+    dev = _cuda()
+    items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
+    flat, shapes = self._ragged_indexes(indexes, dev)
+    if len(items) != len(shapes) or any(tuple(b.shape) != s for b, s in zip(items, shapes)):
+      raise ValueError(f"bottleneck shapes {[tuple(b.shape) for b in items]} do not match the indexes' {shapes}")
+    loc = None if _loc is None else torch.cat([torch.as_tensor(l).to(dev).reshape(-1) for l in _loc])
+    b = torch.cat([b.reshape(-1) for b in items])
+    if loc is not None and loc.numel() != b.numel():
+      raise ValueError("each `loc` item must have the shape of its bottleneck")
+    coff = self.cdf_offset.to(dev)
+    lengths = [b.numel() for b in items]
+    if self.bottleneck_dtype == torch.float32:
+      return F.compress_ragged(self._lookup_host(), lengths, b, loc, coff, index=flat)
+    if loc is not None:
+      b = b - loc
+    symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
+    return F.compress_ragged(self._lookup_host(), lengths, symbols, index=flat)
+
+  def decompress_ragged(self, strings, indexes, _loc=None):
+    """Inverse of compress_ragged: item i has the coding shape of `indexes[i]`.  The items are views into one
+    allocation."""
+    self._check_compression()
+    strings = _ragged_strings(strings, len(indexes))
+    dev = strings.bytes_dev.device
+    flat, shapes = self._ragged_indexes(indexes, dev)
+    loc = None if _loc is None else torch.cat([torch.as_tensor(l).to(dev).reshape(-1) for l in _loc])
+    coff = self.cdf_offset.to(dev)
+    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
+    lengths = [_numel(s) for s in shapes]
+    fused = self.bottleneck_dtype == torch.float32
+    if fused:
+      out = F.decode_ragged(handle, lengths, index=flat, quant_offset=loc, cdf_offset=coff)
+    else:
+      symbols = F.decode_ragged(handle, lengths, index=flat)
+    sanity = gen_ops.entropy_decode_finalize(handle)
+    if self.decode_sanity_check and not bool(sanity.all()):
+      raise gen_ops.InvalidArgumentError("Sanity check failed.")
+    if not fused:
+      out = (symbols + coff[flat.long()]).to(self.bottleneck_dtype)
+      if loc is not None:
+        out = out + loc
+    return _split_items(out, shapes)
+
   def get_config(self):
     raise NotImplementedError("Serializing indexed entropy models is not yet implemented.")
 
@@ -543,6 +682,13 @@ class LocationScaleIndexedEntropyModel(ContinuousIndexedEntropyModel):
 
   def decompress(self, strings, scale_indexes, loc=None, fused=True):
     return super().decompress(strings, scale_indexes, fused=fused, _loc=loc)
+
+  def compress_ragged(self, bottlenecks, scale_indexes, loc=None):
+    """`loc`: None or a list with one tensor per item."""
+    return super().compress_ragged(bottlenecks, scale_indexes, _loc=loc)
+
+  def decompress_ragged(self, strings, scale_indexes, loc=None):
+    return super().decompress_ragged(strings, scale_indexes, _loc=loc)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -198,6 +198,68 @@ def compress_f32(batch_shape, lookup, y, quant_offset, cdf_offset, index=None):
   return gen_ops.Strings(out, offsets, shape)
 
 
+def _symbol_offsets(lengths):
+  import numpy as np
+  lengths = np.asarray([int(n) for n in lengths], dtype=np.int64)
+  if lengths.size == 0:
+    raise _lib.InvalidArgumentError("a ragged batch needs at least one stream")
+  return np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64))
+
+
+def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, index=None):
+  """One compress over streams of different lengths: stream i is the next `lengths[i]` elements of the flat
+  `value`.  `value` int32 holds symbols; float32 is quantised in the kernel like compress_f32 (`quant_offset` per
+  row in channel mode, the loc tensor in index mode; `cdf_offset` required).  Channel mode (index None) restarts
+  at row 0 in every stream.  Returns a Strings of shape (len(lengths),) whose string i equals what compress_f32 /
+  entropy_encode_* give for stream i alone."""
+  from compression_b200 import gen_ops
+  offs = _symbol_offsets(lengths)
+  lookup = gen_ops._host_i32(lookup)
+  if lookup.ndim not in (1, 2):
+    raise _lib.InvalidArgumentError(f"`lookup` must be rank 1 or 2: {lookup.shape}")
+  k = offs.size - 1
+  dev = value.device
+  is_f32 = value.dtype != torch.int32
+  value = (_f32 if is_f32 else _i32)(value, dev).reshape(-1)
+  index = _i32(index, dev)
+  if value.numel() != offs[-1] or (index is not None and index.numel() != offs[-1]):
+    raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} symbols, but `value` has {value.numel()}"
+                                    + ("" if index is None else f" and `index` {index.numel()}"))
+  offsets = torch.empty(k + 1, dtype=torch.int64, device=dev)
+  h, total = C.c_void_p(), C.c_int64(0)
+  stream = _stream()
+  L = _lib.lib()
+  check(L.tfcb_compress_ragged(lookup.ctypes.data_as(C.c_void_p), lookup.size,
+                               0 if lookup.ndim == 1 else lookup.shape[1], k, offs.ctypes.data_as(C.c_void_p),
+                               _p(index), _p(value), int(is_f32), _p(_f32(quant_offset, dev)),
+                               _p(_i32(cdf_offset, dev)), _p(offsets), stream, C.byref(h), C.byref(total)))
+  try:
+    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
+  except BaseException:
+    L.tfcb_encoder_destroy(h)
+    raise
+  check(L.tfcb_compress_write(h, _p(offsets), _p(out), stream))
+  return gen_ops.Strings(out, offsets, (k,))
+
+
+def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=None):
+  """Decodes `lengths[i]` more symbols of stream i of a decoder handle into one flat tensor, stream after stream.
+  With `cdf_offset` the symbols are dequantised as decode_channel_f32 / decode_index_f32 do (float32), without it
+  they are returned as int32.  Channel mode (index None) restarts at row 0 in every stream."""
+  offs = _symbol_offsets(lengths)
+  if offs.size - 1 != handle.n_streams:
+    raise _lib.InvalidArgumentError(f"{offs.size - 1} lengths for {handle.n_streams} strings")
+  dev = handle._encoded.bytes_dev.device
+  index = _i32(index, dev)
+  if index is not None and index.numel() != offs[-1]:
+    raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} symbols, but `index` has {index.numel()}")
+  f32 = cdf_offset is not None
+  out = torch.empty(int(offs[-1]), dtype=torch.float32 if f32 else torch.int32, device=dev)
+  check(_lib.lib().tfcb_decode_ragged(handle._h, offs.ctypes.data_as(C.c_void_p), _p(index), _p(out), int(f32),
+                                      _p(_f32(quant_offset, dev)), _p(_i32(cdf_offset, dev)), _stream()))
+  return out
+
+
 def decode_channel_f32(handle, out_shape, quant_offset, cdf_offset):
   """Decodes and dequantises: float(sym + cdf_offset[c]) + quant_offset[c] (continuous_batched.py:416-421)."""
   dev = handle._encoded.bytes_dev.device

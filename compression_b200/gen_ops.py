@@ -123,6 +123,32 @@ class Strings:
   def nbytes(self) -> int:
     return int(self.offsets_dev[-1].item())
 
+  def split(self) -> List["Strings"]:
+    """Every string on its own, as a Strings of shape (1,) that views this one's bytes (one host synchronisation)."""
+    offs = self.offsets_dev.cpu().tolist()
+    ends = self.offsets_dev[1:] - self.offsets_dev[:-1]
+    local = torch.stack([torch.zeros_like(ends), ends], dim=1)  # row i: offsets of string i in its own view
+    return [Strings(self.bytes_dev[offs[i]:offs[i + 1]], local[i], (1,)) for i in range(len(offs) - 1)]
+
+  @classmethod
+  def concat(cls, parts: Sequence["Strings"]) -> "Strings":
+    """The strings of `parts`, in order, as one Strings of shape (total,) (one host synchronisation)."""
+    parts = list(parts)
+    if not parts:
+      raise InvalidArgumentError("nothing to concatenate")
+    counts = [p.numel() for p in parts]
+    offs = torch.cat([p.offsets_dev for p in parts]).cpu().numpy()
+    out_offs, chunks, base, at = [0], [], 0, 0
+    for p, n in zip(parts, counts):
+      o = offs[at:at + n + 1]
+      at += n + 1
+      out_offs.extend(int(base + v - o[0]) for v in o[1:])
+      chunks.append(p.bytes_dev[int(o[0]):int(o[-1])])
+      base += int(o[-1] - o[0])
+    dev = parts[0].bytes_dev.device
+    data = torch.cat(chunks + [torch.zeros(1, dtype=torch.uint8, device=dev)])
+    return cls(data, torch.tensor(out_offs, dtype=torch.int64).to(dev), (len(out_offs) - 1,))
+
   def __len__(self):
     return self.shape[0] if self.shape else 1
 

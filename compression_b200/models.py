@@ -10,7 +10,9 @@ bytes of the container.
 
 Batches: the reference's `compress` takes ONE image `[H, W, 3]` uint8 (it adds the batch dimension itself);
 `compress_batch` / `decompress_batch` take `[B, H, W, 3]` and code B streams in one launch -- what
-BASELINE.json configs[1]/[2] ("batch=256 / 128") time.
+BASELINE.json configs[1]/[2] ("batch=256 / 128") time.  `compress_images` / `decompress_images` take a list of
+images of different sizes: the transforms run per image (grouping equal shapes into one conv batch could let cuDNN
+pick another algorithm and change the strings), the range coder once for all of them (ragged batches).
 """
 import math
 
@@ -20,6 +22,7 @@ from torch import nn
 
 from compression_b200 import distributions as D
 from compression_b200 import entropy_models as E
+from compression_b200 import gen_ops
 from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
@@ -103,6 +106,13 @@ def _as_batch(x):
   return x
 
 
+def _as_image(x):
+  x = torch.as_tensor(x)
+  if x.dim() != 3 or x.shape[-1] != 3:
+    raise ValueError(f"expected one image [H, W, 3], received shape {tuple(x.shape)}")
+  return x
+
+
 class _Model(nn.Module):
 
   def _device(self):
@@ -176,6 +186,31 @@ class BLS2017Model(_Model):
     x_hat = self.synthesis_transform(y_hat)
     x_hat = x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :]
     return _to_uint8(x_hat)
+
+  # -- lists of differently sized images: transforms per image, one range-coder launch for all --
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element."""
+    ys, shapes = [], []
+    for x in images:
+      x = _as_image(x)[None].to(device=self._device(), dtype=torch.float32)
+      y = self.analysis_transform(x)
+      ys.append(y[0])
+      shapes.append((torch.tensor(x.shape[1:-1], dtype=torch.int32), torch.tensor(y.shape[1:-1], dtype=torch.int32)))
+    strings = self.entropy_model.compress_ragged(ys).split()
+    return [(s,) + sh for s, sh in zip(strings, shapes)]
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
+    items = list(items)
+    y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]),
+                                                  [tuple(int(v) for v in it[2]) for it in items])
+    out = []
+    for y_hat, (_, x_shape, _) in zip(y_hats, items):
+      x_hat = self.synthesis_transform(y_hat[None])
+      out.append(_to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0])
+    return out
 
   # -- .tfci container (bls2017.py:262-282 `compress`, :308-321 `decompress`) --
   def compress_to_tfci(self, x):
@@ -265,6 +300,40 @@ class BMSHJ2018Model(_Model):
     x_hat = self.synthesis_transform(y_hat)
     x_hat = x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :]
     return _to_uint8(x_hat)
+
+  # -- lists of differently sized images: transforms per image, one range-coder launch for z and one for y --
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element."""
+    ys, zs, idxs, shapes = [], [], [], []
+    for x in images:
+      x = _as_image(x)[None].to(device=self._device(), dtype=torch.float32)
+      y = self.analysis_transform(x)
+      z = self.hyper_analysis_transform(y.abs())
+      indexes = self.hyper_synthesis_transform(self.side_entropy_model.quantize(z))
+      ys.append(y[0])
+      zs.append(z[0])
+      idxs.append(indexes[0, :y.shape[1], :y.shape[2], :])
+      shapes.append(tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z)))
+    side_strings = self.side_entropy_model.compress_ragged(zs).split()
+    strings = self.entropy_model.compress_ragged(ys, idxs).split()
+    return [(s, side) + sh for s, side, sh in zip(strings, side_strings, shapes)]
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
+    items = list(items)
+    z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
+                                                       [tuple(int(v) for v in it[4]) for it in items])
+    idxs = []
+    for z_hat, (_, _, _, y_shape, _) in zip(z_hats, items):
+      idxs.append(self.hyper_synthesis_transform(z_hat[None])[0, :int(y_shape[0]), :int(y_shape[1]), :])
+    y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]), idxs)
+    out = []
+    for y_hat, (_, _, x_shape, _, _) in zip(y_hats, items):
+      x_hat = self.synthesis_transform(y_hat[None])
+      out.append(_to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0])
+    return out
 
   def compress_to_tfci(self, x):
     packed = PackedTensors()

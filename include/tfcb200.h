@@ -110,6 +110,19 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
                   int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host);
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream);
 
+/* Ragged batch: one compress() over n_streams streams of different lengths (e.g. the latents of differently sized
+ * images): stream s is symbols [symbol_offsets_host[s], symbol_offsets_host[s+1]) of value_dev (and of index_dev /
+ * quant_offset_dev in index mode; in channel mode its rows restart at 0).  Otherwise exactly tfcb_compress: writes
+ * offsets_dev [n_streams + 1], synchronises once, returns the total size and an encoder that tfcb_compress_write
+ * packs and takes back.  String s is byte-identical to what tfcb_compress makes of stream s alone; a stream with
+ * no symbols gives the empty string.  The offsets are host memory and are checked before any device work
+ * (TFCB_INVALID_ARGUMENT): n_streams > 0, symbol_offsets_host[0] == 0, non-decreasing, every stream within the
+ * per-stream limit.  The word arena is the sum of the streams' own worst cases. */
+int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                         const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                         int32_t value_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev,
+                         int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host);
+
 /* ------------------------------------------------------------------------------------------------
  * Range DECODER.  Replaces CreateRangeDecoder / EntropyDecodeChannel / EntropyDecodeIndex /
  * EntropyDecodeFinalize:
@@ -139,6 +152,13 @@ int tfcb_decode_channel_f32(tfcb_decoder* h, float* out_dev, const float* quant_
 int tfcb_decode_index_f32(tfcb_decoder* h, const int32_t* index_dev, float* out_dev,
                           const float* loc_dev, const int32_t* cdf_offset_dev, int64_t n_per_stream,
                           void* stream);
+/* Ragged batch: decodes symbol_offsets_host[s+1] - symbol_offsets_host[s] more symbols of stream s into out_dev
+ * at symbol_offsets_host[s], int32 (out_is_f32 == 0) or dequantised float as tfcb_decode_{channel,index}_f32;
+ * index_dev NULL = channel mode (rows restart at 0 in every stream).  The offsets ([n_streams + 1], host memory)
+ * are checked like tfcb_compress_ragged's.  State persists like the other decode calls; tfcb_decode_finalize
+ * reports. */
+int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev, void* out_dev,
+                       int32_t out_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev, void* stream);
 /* EntropyDecodeFinalize: ok_host[s] = RangeDecoder::Finalize() of stream s (range_coder.h:144-169).
  * Synchronises; also reports a pending out-of-range index as TFCB_INVALID_ARGUMENT. */
 int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream);
