@@ -67,6 +67,10 @@ SIGNATURES = {
     "tfcb_build_lookup": (_int, [_vp, _i64, _i64, _vp, _int, _vp, _vp]),
     "tfcb_run_length_encode": (_int, [_vp, _i64, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_run_length_decode": (_int, [_vp, _i64, _int, _int, _int, _vp, _i64, _vp]),
+    "tfcb_run_length_encode_ragged": (_int, [_vp, _i64, _vp, _int, _int, _int, _vp, _vp, _p(_vp), _p(_i64)]),
+    "tfcb_run_length_write": (_int, [_vp, _vp, _vp]),
+    "tfcb_run_length_encoder_destroy": (None, [_vp]),
+    "tfcb_run_length_decode_ragged": (_int, [_vp, _vp, _i64, _vp, _int, _int, _int, _vp, _vp]),
     "tfcb_stochastic_round": (_int, [_vp, _int, _i64, _f32, _vp, _i64, _vp, _vp]),
     "tfcb_gdn_forward": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _f32, _f32, _vp]),
     "tfcb_gdn_forward_16bit": (_int, [_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _f32, _f32, _vp]),

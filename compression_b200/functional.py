@@ -260,6 +260,52 @@ def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=Non
   return out
 
 
+def run_length_encode_ragged(values, lengths, run_length_code, magnitude_code, use_run_length_for_non_zeros):
+  """RunLengthEncode of many strings in one launch: string i codes the next `lengths[i]` elements of the flat int32
+  `values`.  Returns a Strings of shape (len(lengths),) whose string i equals gen_ops.run_length_encode of those
+  elements alone (the empty string for a length of 0)."""
+  from compression_b200 import gen_ops
+  offs = _symbol_offsets(lengths)
+  k = offs.size - 1
+  dev = gen_ops._device()
+  values = _i32(values, dev).reshape(-1)
+  if values.numel() != offs[-1]:
+    raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} elements, but `values` has {values.numel()}")
+  offsets = torch.empty(k + 1, dtype=torch.int64, device=dev)
+  h, total = C.c_void_p(), C.c_int64(0)
+  stream = _stream()
+  L = _lib.lib()
+  check(L.tfcb_run_length_encode_ragged(_p(values), k, offs.ctypes.data_as(C.c_void_p), int(run_length_code),
+                                        int(magnitude_code), int(bool(use_run_length_for_non_zeros)), _p(offsets),
+                                        stream, C.byref(h), C.byref(total)))
+  try:
+    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
+  except BaseException:
+    L.tfcb_run_length_encoder_destroy(h)
+    raise
+  check(L.tfcb_run_length_write(h, _p(out), stream))
+  return gen_ops.Strings(out, offsets, (k,))
+
+
+def run_length_decode_ragged(strings, lengths, run_length_code, magnitude_code, use_run_length_for_non_zeros):
+  """Inverse of run_length_encode_ragged, one thread per string in one launch: `strings` (a Strings or a list of
+  bytes) holds len(lengths) strings; returns int32 [sum(lengths)], string after string.  A damaged string raises
+  InvalidArgumentError naming the lowest-numbered failing string and the message gen_ops.run_length_decode gives."""
+  from compression_b200 import gen_ops
+  offs = _symbol_offsets(lengths)
+  k = offs.size - 1
+  if not isinstance(strings, gen_ops.Strings):
+    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+  if strings.numel() != k:
+    raise _lib.InvalidArgumentError(f"{strings.numel()} strings for {k} lengths")
+  dev = strings.bytes_dev.device
+  out = torch.empty(int(offs[-1]), dtype=torch.int32, device=dev)
+  check(_lib.lib().tfcb_run_length_decode_ragged(
+      _p(strings.bytes_dev), _p(strings.offsets_dev), k, offs.ctypes.data_as(C.c_void_p), int(run_length_code),
+      int(magnitude_code), int(bool(use_run_length_for_non_zeros)), _p(out), _stream()))
+  return out
+
+
 def decode_channel_f32(handle, out_shape, quant_offset, cdf_offset):
   """Decodes and dequantises: float(sym + cdf_offset[c]) + quant_offset[c] (continuous_batched.py:416-421)."""
   dev = handle._encoded.bytes_dev.device

@@ -4,12 +4,14 @@ Host-side mirror of the reference's two callers of ``RunLength{Gamma}Encode/Deco
 (python/entropy_models/power_law.py:27-209, python/entropy_models/laplace.py:25-233): no tables, no prior --
 rounding, one bit string per coding unit through ``gen_ops.run_length_encode`` (the CUDA coder of
 csrc/run_length.cu), and a differentiable penalty standing in for the code length during training.
+``compress_ragged`` / ``decompress_ragged`` code a list of differently shaped coding units in one launch each.
 """
-from typing import Sequence
+from typing import List, Sequence
 
 import numpy as np
 import torch
 
+from compression_b200 import functional
 from compression_b200 import gen_ops
 from compression_b200 import math_ops
 
@@ -106,6 +108,39 @@ class _RunLengthEntropyModel(torch.nn.Module):
     if not units:
       return torch.zeros(arr.shape + code_shape, dtype=self.bottleneck_dtype)
     return torch.stack(units).reshape(arr.shape + code_shape).to(self.bottleneck_dtype)
+
+  def _code(self):
+    return self.run_length_code, self.magnitude_code, self.use_run_length_for_non_zeros
+
+  def compress_ragged(self, bottlenecks) -> gen_ops.Strings:
+    """Compresses a list of coding units of different shapes in one coder launch.  Each item has exactly
+    `coding_rank` dimensions.  Returns a Strings of shape (k,) whose string i equals `compress(bottlenecks[i])[()]`;
+    a uniform batch ``x`` is ``compress_ragged(list(x.reshape(-1, *code_shape)))``."""
+    items = [self._as_bottleneck(b) for b in bottlenecks]
+    if not items:
+      raise ValueError("`bottlenecks` is empty")
+    for b in items:
+      if b.dim() != self.coding_rank:
+        raise ValueError(f"each item needs exactly {self.coding_rank} dimensions: received shape {tuple(b.shape)}")
+    dev = gen_ops._device()
+    symbols = torch.cat([torch.round(b.to(dev)).to(torch.int32).reshape(-1) for b in items])
+    return functional.run_length_encode_ragged(symbols, [b.numel() for b in items], *self._code())
+
+  def decompress_ragged(self, strings, code_shapes) -> List[torch.Tensor]:
+    """Inverse of compress_ragged in one coder launch: item i has shape `code_shapes[i]` (exactly `coding_rank`
+    dimensions), equals `decompress(strings[i], code_shapes[i])` and is in `bottleneck_dtype`.  The items are views
+    into one allocation."""
+    shapes = [tuple(int(d) for d in s) for s in code_shapes]
+    for s in shapes:
+      if len(s) != self.coding_rank:
+        raise ValueError(f"each code shape needs exactly {self.coding_rank} dimensions: received {s}")
+    lengths = [_prod(s) for s in shapes]
+    flat = functional.run_length_decode_ragged(strings, lengths, *self._code()).to(self.bottleneck_dtype)
+    out, at = [], 0
+    for s, n in zip(shapes, lengths):
+      out.append(flat[at:at + n].reshape(s))
+      at += n
+    return out
 
 
 class PowerLawEntropyModel(_RunLengthEntropyModel):

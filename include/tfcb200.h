@@ -207,14 +207,37 @@ int tfcb_build_lookup(const float* pmf_dev, int64_t rows, int64_t max_len, const
  * data int32 [n] (flattened) <-> one bit string.  run_length_code / magnitude_code >= 0: Rice code with that parameter,
  * < 0: Elias gamma.  Encode: `code_dev` has room for `capacity` bytes (a multiple of 4 is used); *n_bytes_host receives
  * the length of the code; TFCB_INVALID_ARGUMENT with the needed size in the message (and in *n_bytes_host) when it
- * does not fit.  The encoder is data parallel (scans + atomics); the decoder is serial, as in the reference.
- * Decode errors carry the reference's DataLoss messages.
+ * does not fit.  The encoder is data parallel (scans + atomics); the decoder is serial within a string, as in the
+ * reference.  Decode errors carry the reference's DataLoss messages.  Both calls synchronise `stream`.
  * ---------------------------------------------------------------------------------------------- */
 int tfcb_run_length_encode(const int32_t* data_dev, int64_t n, int run_length_code, int magnitude_code,
                            int use_run_length_for_non_zeros, uint8_t* code_dev, int64_t capacity,
                            int64_t* n_bytes_host, void* stream);
 int tfcb_run_length_decode(const uint8_t* code_dev, int64_t n_bytes, int run_length_code, int magnitude_code,
                            int use_run_length_for_non_zeros, int32_t* data_dev, int64_t n, void* stream);
+
+/* Many strings in one launch (the reference has no batched op; this is an extension, e.g. for all coding units of
+ * a tensor, or differently sized items).  Unit u is data_dev[unit_offsets_host[u] .. unit_offsets_host[u+1]); string u
+ * is byte-identical to what tfcb_run_length_encode makes of unit u alone, and a unit with no elements gives the empty
+ * string.  The host offsets are checked before any device work (TFCB_INVALID_ARGUMENT): n_units > 0, non-null
+ * pointers, unit_offsets_host[0] == 0, non-decreasing, fewer than 2^31 elements in all, Rice parameters <= 31.
+ * tfcb_run_length_encode_ragged writes where each string starts to `offsets_dev` int64 [n_units + 1], synchronises
+ * once and returns the total size and a handle; data_dev must stay valid until tfcb_run_length_write packs the
+ * strings back to back into `bytes_dev` [total] (asynchronous; only [0, total) is written) and takes the handle back,
+ * also when it fails.  tfcb_run_length_encoder_destroy releases a handle that is never written. */
+typedef struct tfcb_rl_encoder tfcb_rl_encoder;
+int tfcb_run_length_encode_ragged(const int32_t* data_dev, int64_t n_units, const int64_t* unit_offsets_host,
+                                  int run_length_code, int magnitude_code, int use_run_length_for_non_zeros,
+                                  int64_t* offsets_dev, void* stream, tfcb_rl_encoder** out, int64_t* total_bytes_host);
+int tfcb_run_length_write(tfcb_rl_encoder* h, uint8_t* bytes_dev, void* stream);
+void tfcb_run_length_encoder_destroy(tfcb_rl_encoder* h);
+/* Decodes string u (bytes_dev[offsets_dev[u] .. offsets_dev[u+1]), device offsets) into
+ * data_dev[unit_offsets_host[u] .. unit_offsets_host[u+1]), one thread per string, and synchronises once.  The
+ * unit offsets are checked like the encoder's.  A damaged string gives TFCB_INVALID_ARGUMENT naming the
+ * lowest-numbered failing unit ("unit k: Out of bits to read.", as tfcb_run_length_decode would say of it). */
+int tfcb_run_length_decode_ragged(const uint8_t* bytes_dev, const int64_t* offsets_dev, int64_t n_units,
+                                  const int64_t* unit_offsets_host, int run_length_code, int magnitude_code,
+                                  int use_run_length_for_non_zeros, int32_t* data_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * StochasticRound:
