@@ -13,7 +13,9 @@
 // among equal keys the item that has waited longest goes first; the initial order among equal keys
 // comes from an unstable std::sort.  Here: waited-longest first as well, initial ties broken by
 // LOWEST BIN INDEX.  log2 of the integer arguments comes from a table computed on the host with the
-// same libm the reference would use, so every double comparison is identical.
+// same libm the reference would use, so every double comparison is identical.  The shared table covers
+// counts up to 65537; a row whose counts reach past it (a bin with mass above 1, or with a large
+// multiple of 2^-p) is rerun with a larger table built for that call, up to kMaxLogTab entries.
 #include <cmath>
 #include <mutex>
 #include <vector>
@@ -24,17 +26,23 @@ namespace tfcb {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kLogTab = 65538;  // log2(v) for v in [0, 65537]
+constexpr int kLogTab = 65538;       // shared table: log2(v) for v in [0, 65537]
+constexpr int kMaxLogTab = 1 << 24;  // largest per-call table (128 MiB): counts up to 2^24 - 1
 
 double* g_log2_dev = nullptr;
 std::mutex g_log2_mu;
 
+std::vector<double> log_table(int entries) {
+  std::vector<double> tab(entries);
+  tab[0] = 0.0;
+  for (int v = 1; v < entries; ++v) tab[v] = std::log2(static_cast<double>(v));
+  return tab;
+}
+
 int ensure_log_table(cudaStream_t s) {
   std::lock_guard<std::mutex> lock(g_log2_mu);
   if (g_log2_dev) return TFCB_OK;
-  std::vector<double> tab(kLogTab);
-  tab[0] = 0.0;
-  for (int v = 1; v < kLogTab; ++v) tab[v] = std::log2(static_cast<double>(v));
+  const std::vector<double> tab = log_table(kLogTab);
   double* d = nullptr;
   TFCB_CUDA_TRY(cudaMalloc((void**)&d, kLogTab * sizeof(double)));
   cudaError_t e = cudaMemcpyAsync(d, tab.data(), kLogTab * sizeof(double), cudaMemcpyHostToDevice, s);
@@ -46,6 +54,17 @@ int ensure_log_table(cudaStream_t s) {
   g_log2_dev = d;
   return TFCB_OK;
 }
+
+// What one launch reports to the host.  `err`: the first non-finite or negative mass.  Counts the
+// log2 table does not cover: the largest one, and the lowest (row, bin) whose count is kMaxLogTab or
+// more, stored complemented as ~(row << 20 | bin) so that atomicMax keeps the lowest and 0 means none.
+// Only the DOWN adjustment can read past the table: a count of 65538 or more makes the row sum exceed
+// 2^precision, and DOWN steps only lower counts.
+struct RowsStatus {
+  DevError err;
+  unsigned long long max_count;
+  unsigned long long first_over_cap;
+};
 
 struct Cand {
   double key;
@@ -145,12 +164,13 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
     const float* __restrict__ pmf_all, long long row_stride, int n_fixed, const int* __restrict__ lens,
     const long long* __restrict__ out_off, int precision, int* __restrict__ out_all,
     double* __restrict__ key_all, int* __restrict__ age_all, long long scratch_stride,
-    const double* __restrict__ lg, DevError* err) {
+    const double* __restrict__ lg, int lg_n, RowsStatus* st) {
   __shared__ long long s_red[kThreads / 32];
   __shared__ float s_redf[kThreads / 32];
   __shared__ long long s_sum;
   __shared__ float s_extra;
   __shared__ int s_bad;
+  __shared__ int s_big;
   const long long r = blockIdx.x;
   const int tid = threadIdx.x;
   const float* pmf = pmf_all + r * row_stride;
@@ -172,7 +192,10 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
   int* age = age_all + r * scratch_stride;
   const int total = 1 << precision;
 
-  if (tid == 0) s_bad = 0;
+  if (tid == 0) {
+    s_bad = 0;
+    s_big = 0;
+  }
   __syncthreads();
   // validation (pmf_to_cdf_kernels.cc:77-86) and, for ragged rows, the overflow mass
   float part = 0.f;
@@ -180,7 +203,7 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
     const float m = pmf[i];
     if (!(isfinite(m) && m >= 0.f)) {
       s_bad = 1;
-      report(err, kErrValue, r, i, (long long)__float_as_int(m), 0);
+      report(&st->err, kErrValue, r, i, (long long)__float_as_int(m), 0);
     }
     part += m;
   }
@@ -210,6 +233,11 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
     v = max(v, 1);
     q[i] = v;
     local += v;
+    if (v >= lg_n) {  // beyond the table: the host reruns with a larger one
+      s_big = 1;
+      atomicMax(&st->max_count, (unsigned long long)v);
+      if (v >= kMaxLogTab) atomicMax(&st->first_over_cap, ~((unsigned long long)r << 20 | (unsigned)i));
+    }
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) local += __shfl_xor_sync(0xFFFFFFFFu, local, d);
@@ -222,6 +250,7 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
   }
   __syncthreads();
   const long long sum = s_sum;
+  if (s_big) return;
   if (sum > total) {
     adjust<true>(q, pmf, len, extra, n, sum - total, key, age, lg);
   } else if (sum < total) {
@@ -266,39 +295,74 @@ __global__ void __launch_bounds__(kThreads) pmf_rows_kernel(
   }
 }
 
+// One launch over all rows with the log2 table `lg` of `lg_n` entries; copies the status back and
+// synchronises.
+int launch_rows(const float* pmf, long long rows, long long row_stride, int n_fixed, const int* lens_dev,
+                const long long* out_off_dev, long long max_n, int precision, int* out, double* key, int* age,
+                const double* lg, int lg_n, RowsStatus* st_dev, RowsStatus* st, cudaStream_t s) {
+  cudaMemsetAsync(st_dev, 0, sizeof(RowsStatus), s);
+  pmf_rows_kernel<<<(unsigned)rows, kThreads, 0, s>>>(pmf, row_stride, n_fixed, lens_dev, out_off_dev, precision,
+                                                      out, key, age, max_n, lg, lg_n, st_dev);
+  TFCB_LAUNCHED();
+  cudaError_t ce = cudaMemcpyAsync(st, st_dev, sizeof *st, cudaMemcpyDeviceToHost, s);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+  if (ce != cudaSuccess) {
+    (void)cudaGetLastError();
+    return fail(TFCB_CUDA_ERROR, "CUDA error '%s' in PmfToQuantizedCdf", cudaGetErrorString(ce));
+  }
+  if (st->err.code != kErrNone) {
+    const int bits = (int)st->err.value;
+    float f;
+    memcpy(&f, &bits, sizeof f);
+    return fail(TFCB_INVALID_ARGUMENT,
+                "`pmf` has non-finite or negative element: %g (row %lld, bin %lld). Please check for "
+                "numerical problems in the probability computation.",
+                (double)f, st->err.stream, st->err.pos);
+  }
+  return TFCB_OK;
+}
+
 int run_rows(const float* pmf, long long rows, long long row_stride, int n_fixed, const int* lens_dev,
              const long long* out_off_dev, long long max_n, int precision, int* out, cudaStream_t s) {
   TFCB_TRY(ensure_log_table(s));
   double* key = nullptr;
   int* age = nullptr;
-  DevError* err = nullptr;
+  RowsStatus* st_dev = nullptr;
+  double* big_lg = nullptr;
+  RowsStatus st;
   int rc = dev_alloc((void**)&key, (size_t)rows * max_n * sizeof(double), s);
   if (rc == TFCB_OK) rc = dev_alloc((void**)&age, (size_t)rows * max_n * sizeof(int), s);
-  if (rc == TFCB_OK) rc = dev_alloc((void**)&err, sizeof(DevError), s);
-  if (rc == TFCB_OK) {
-    cudaMemsetAsync(err, 0, sizeof(DevError), s);
-    pmf_rows_kernel<<<(unsigned)rows, kThreads, 0, s>>>(pmf, row_stride, n_fixed, lens_dev, out_off_dev,
-                                                        precision, out, key, age, max_n, g_log2_dev, err);
-    TFCB_LAUNCHED();
-    DevError e;
-    cudaError_t ce = cudaMemcpyAsync(&e, err, sizeof e, cudaMemcpyDeviceToHost, s);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
-    if (ce != cudaSuccess) {
-      (void)cudaGetLastError();
-      rc = fail(TFCB_CUDA_ERROR, "CUDA error '%s' in PmfToQuantizedCdf", cudaGetErrorString(ce));
-    } else if (e.code != kErrNone) {
-      const int bits = (int)e.value;
-      float f;
-      memcpy(&f, &bits, sizeof f);
-      rc = fail(TFCB_INVALID_ARGUMENT,
-                "`pmf` has non-finite or negative element: %g (row %lld, bin %lld). Please check for "
-                "numerical problems in the probability computation.",
-                (double)f, e.stream, e.pos);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&st_dev, sizeof(RowsStatus), s);
+  if (rc == TFCB_OK)
+    rc = launch_rows(pmf, rows, row_stride, n_fixed, lens_dev, out_off_dev, max_n, precision, out, key, age,
+                     g_log2_dev, kLogTab, st_dev, &st, s);
+  if (rc == TFCB_OK && st.first_over_cap) {
+    const unsigned long long at = ~st.first_over_cap;
+    rc = fail(TFCB_INVALID_ARGUMENT,
+              "`pmf` row %lld, bin %lld quantises to %d or more counts; at most %d counts per bin are supported",
+              (long long)(at >> 20), (long long)(at & 0xFFFFF), kMaxLogTab, kMaxLogTab - 1);
+  } else if (rc == TFCB_OK && st.max_count) {
+    // Rows with counts past the shared table were left unadjusted: rerun every row with a table for this
+    // call only (the shared one stays in place for concurrent calls on other streams).
+    const int entries = (int)st.max_count + 1;
+    const std::vector<double> tab = log_table(entries);
+    rc = dev_alloc((void**)&big_lg, (size_t)entries * sizeof(double), s);
+    if (rc == TFCB_OK) {
+      cudaError_t ce = cudaMemcpyAsync(big_lg, tab.data(), (size_t)entries * sizeof(double),
+                                       cudaMemcpyHostToDevice, s);
+      if (ce != cudaSuccess) {
+        (void)cudaGetLastError();
+        rc = fail(TFCB_CUDA_ERROR, "log2 table upload failed: %s", cudaGetErrorString(ce));
+      }
     }
+    if (rc == TFCB_OK)
+      rc = launch_rows(pmf, rows, row_stride, n_fixed, lens_dev, out_off_dev, max_n, precision, out, key, age,
+                       big_lg, entries, st_dev, &st, s);
   }
+  dev_free(big_lg, s);
   dev_free(key, s);
   dev_free(age, s);
-  dev_free(err, s);
+  dev_free(st_dev, s);
   return rc;
 }
 

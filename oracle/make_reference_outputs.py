@@ -14,6 +14,7 @@ import oracle  # noqa: E402
 import test_baseline_configs_gpu  # noqa: E402
 import test_misc_gpu  # noqa: E402
 import test_oracle_pin as pin  # noqa: E402
+import test_pmf_tables_gpu  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden", "reference_outputs.npz")
 
@@ -60,6 +61,9 @@ def main():
       [R.pmf_to_cdf(pmf, 12)[0] for pmf in test_baseline_configs_gpu.tie_row_pmfs()])
   out["pmf_cdf"], out["pmf_cdf_shape"] = flat_rows(
       [R.pmf_to_cdf(test_misc_gpu.pmf_case(n, scale), p) for n, p, scale in test_misc_gpu.PMF_CASES])
+  # stored as counts (the CDF's differences), which compress far better than the CDF itself
+  out["pmf_edge_counts"], out["pmf_edge_counts_shape"] = flat_rows(
+      [np.diff(R.pmf_to_cdf(pmf, p), axis=-1) for p, pmf in test_pmf_tables_gpu.tie_free_reference_rows()])
 
   np.savez_compressed(OUT, **out)
   print(OUT, os.path.getsize(OUT), "bytes")

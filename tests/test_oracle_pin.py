@@ -131,6 +131,18 @@ def test_pmf_to_cdf_invariants_and_tie_rule():
     O.pmf_to_cdf(np.asarray([[0.5, np.nan]], np.float32), 8)
 
 
+def test_pmf_to_cdf_port_equals_compiled_reference_at_the_edges():
+  """The expected values of tests/test_pmf_tables_gpu.py are the port's: on every tie-free edge row there (n up to
+  2^precision, subnormal masses, tens of thousands of steps, counts past 2^16) the port equals the compiled
+  reference's outputs stored in tests/golden/reference_outputs.npz."""
+  import test_pmf_tables_gpu as tables
+  stored = tables.stored_reference_rows()
+  cases = list(tables.tie_free_reference_rows())
+  assert len(cases) == len(stored)
+  for (p, pmf), want in zip(cases, stored):
+    assert np.array_equal(tables.port_cdf(pmf, p), want), (p, pmf.shape)
+
+
 def test_stochastic_round_port_equals_reference_flavour():
   """quantization_kernels.cc:48-95: the C restatement of std::seed_seq + xoshiro256+ against libstdc++'s own
   seed_seq driving the same loop (oracle/ref/ref_driver.cc), and the reference's invariants
