@@ -53,6 +53,8 @@ SIGNATURES = {
     "tfcb_compress_write": (_int, [_vp, _vp, _vp, _vp]),
     "tfcb_compress_ragged": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _p(_vp),
                                     _p(_i64)]),
+    "tfcb_compress_ragged_decoded": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
+                                            _p(_vp), _p(_i64), _vp]),
     "tfcb_decoder_create": (_int, [_vp, _vp, _i64, _vp, _i64, _i64, _vp, _p(_vp)]),
     "tfcb_decode_channel": (_int, [_vp, _vp, _i64, _vp]),
     "tfcb_decode_index": (_int, [_vp, _vp, _vp, _i64, _vp]),

@@ -345,7 +345,8 @@ struct EncDrain {
   }
 };
 
-enum : int { kModeIndex = 1, kModeF32 = 2 };
+// kModeDecoded (encoder only, with kModeF32): the gather warp also writes every symbol's decoded value.
+enum : int { kModeIndex = 1, kModeF32 = 2, kModeDecoded = 4 };
 
 struct EncParams {
   const int32_t* lookup;
@@ -368,6 +369,9 @@ struct EncParams {
   // (multiples of 32).  Null: stream s is symbols [s * n, s * n + n) and words [s * cap, s * cap + cap).
   const long long* sym_off;
   const long long* arena_off;
+  // kModeDecoded: float [n symbols in all], what the f32 decoder returns for each symbol (last: the other fields keep
+  // their parameter offsets)
+  float* decoded;
 };
 
 // Where one stream's symbols (or arena words) are: resolved once per CTA from the offsets array when there is one,
@@ -453,6 +457,14 @@ __device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, 
   }
   int v = f.v;
   if (MODE & kModeF32) v = (int)rintf(f.y - f.loc_or_q) - f.coff;
+  if (MODE & kModeDecoded) {
+    // the resolve warp's dequantisation of the symbol it decodes (v, before the escape mapping): the same integer
+    // and the same float operations, so the value is bit-identical to the decoder's -- including the saturated
+    // conversion of |y - loc| >= 2^31 and NaN -> 0, which recomputing rintf(y - loc) + loc would not reproduce
+    float yv = (float)(v + f.coff);
+    if (P.qoff) yv += f.loc_or_q;
+    P.decoded[at] = yv;
+  }
   const int ncdf = row_ncdf(f.ri.y);
   if (!row_ovf(f.ri.y)) {
     if (v < 0 || v >= ncdf - 1) {
@@ -1895,9 +1907,11 @@ int prepare_ragged(tfcb_encoder* h, const int64_t* sym_off, cudaStream_t s) {
 }
 
 // `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all, laid out by prepare_ragged.
+// `decoded`: the kModeDecoded output.
 template <int MODE>
 int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr) {
+                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr,
+                  float* decoded = nullptr) {
   if (h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
@@ -1929,6 +1943,7 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.err = h->err;
   P.sym_off = sym_off;
   P.arena_off = h->arena_off;
+  P.decoded = decoded;
   if (h->n_streams > 0x7FFFFFFFll) return fail(TFCB_INVALID_ARGUMENT, "too many streams");
   encode_kernel<MODE><<<(unsigned)h->n_streams, 192, 0, s>>>(P);
   TFCB_LAUNCHED();
@@ -2182,20 +2197,31 @@ int checkout_encoder(const int32_t* lookup_host, int64_t lookup_len, int64_t loo
   return TFCB_OK;
 }
 
-// The common part of tfcb_compress and tfcb_compress_ragged: one encode of a checked-out encoder, finalize, and
-// the encoder either handed to the caller or taken back.
+// The common part of tfcb_compress, tfcb_compress_ragged and tfcb_compress_ragged_decoded: one encode of a
+// checked-out encoder, finalize, and the encoder either handed to the caller or taken back.  `decoded` non-null
+// (float values only): the encode also writes the decoded values there.
 int compress_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
                          const float* qoff_dev, const int32_t* cdf_offset_dev, long long n, const long long* sym_off,
-                         int64_t* offsets_dev, cudaStream_t s, tfcb_encoder** out, int64_t* total_bytes_host) {
-  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0);
+                         int64_t* offsets_dev, cudaStream_t s, tfcb_encoder** out, int64_t* total_bytes_host,
+                         float* decoded = nullptr) {
+  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0) | (decoded ? kModeDecoded : 0);
   int rc;
   switch (mode) {
     case 0: rc = launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, s, sym_off); break;
     case kModeIndex: rc = launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, s, sym_off); break;
     case kModeF32: rc = launch_encode<kModeF32>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s, sym_off); break;
-    default:
+    case kModeIndex | kModeF32:
       rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s, sym_off);
       break;
+    case kModeF32 | kModeDecoded:
+      rc = launch_encode<kModeF32 | kModeDecoded>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s, sym_off,
+                                                   decoded);
+      break;
+    case kModeIndex | kModeF32 | kModeDecoded:
+      rc = launch_encode<kModeIndex | kModeF32 | kModeDecoded>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s,
+                                                               sym_off, decoded);
+      break;
+    default: rc = fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values"); break;
   }
   long long total = 0;
   if (rc == TFCB_OK)
@@ -2231,10 +2257,15 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
                               offsets_dev, s, out, total_bytes_host);
 }
 
-int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
-                         const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
-                         int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
-                         int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
+}  // extern "C"
+
+namespace {
+
+// tfcb_compress_ragged, and tfcb_compress_ragged_decoded with `decoded` non-null.
+int compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                    const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                    int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev, int64_t* offsets_dev,
+                    float* decoded, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
   if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
   *out = nullptr;
   *total_bytes_host = 0;
@@ -2264,7 +2295,34 @@ int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t
     return rc;
   }
   return compress_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev,
-                              symbol_offsets_host[n_streams], h->ext, offsets_dev, s, out, total_bytes_host);
+                              symbol_offsets_host[n_streams], h->ext, offsets_dev, s, out, total_bytes_host, decoded);
+}
+
+}  // namespace
+
+extern "C" {
+
+int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                         const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                         int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
+                         int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
+  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev, value_dev,
+                         value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, nullptr, stream, out, total_bytes_host);
+}
+
+int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols,
+                                 int64_t n_streams, const int64_t* symbol_offsets_host, const int32_t* index_dev,
+                                 const void* value_dev, int32_t value_is_f32, const float* qoff_dev,
+                                 const int32_t* cdf_offset_dev, int64_t* offsets_dev, void* stream,
+                                 tfcb_encoder** out, int64_t* total_bytes_host, float* decoded_dev) {
+  if (out) *out = nullptr;
+  if (total_bytes_host) *total_bytes_host = 0;
+  if (!value_is_f32) return fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values (`value_is_f32` is 0)");
+  if (!decoded_dev) return fail(TFCB_INVALID_ARGUMENT, "`decoded` is null");
+  if (!cdf_offset_dev) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev, value_dev,
+                         value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, decoded_dev, stream, out,
+                         total_bytes_host);
 }
 
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {

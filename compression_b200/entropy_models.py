@@ -383,10 +383,14 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     return outputs
 
   # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
-  def compress_ragged(self, bottlenecks):
+  def compress_ragged(self, bottlenecks, return_decoded=False):
     """Compresses a list of coding units of different shapes in one range-coder launch.  Each item has exactly
     `coding_rank` dimensions ending in `prior_shape` (no broadcasting).  Returns a Strings of shape (k,) whose string
-    i equals `compress(bottlenecks[i])`."""
+    i equals `compress(bottlenecks[i])`.
+
+    `return_decoded=True` returns `(strings, items)` with `items` equal, bit for bit, to
+    `decompress_ragged(strings, ...)`: written by the encoder itself for a float32 bottleneck, decoded from the
+    fresh strings otherwise."""
     self._check_compression()
     dev = _cuda()
     items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
@@ -401,13 +405,17 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     coff, qoff = self._flat_tables(dev)
     flat = torch.cat([b.reshape(-1) for b in items])
     if self.bottleneck_dtype == torch.float32:
-      return F.compress_ragged(self._lookup_host(), lengths, flat, qoff, coff)
+      out = F.compress_ragged(self._lookup_host(), lengths, flat, qoff, coff, decoded=return_decoded)
+      return (out[0], _split_items(out[1], [tuple(b.shape) for b in items])) if return_decoded else out
     # compress()'s unfused arithmetic; every item holds whole rows of prior_shape, so the rows line up
     b = flat.to(torch.float32).reshape(-1, coff.numel())
     if qoff is not None:
       b = b - qoff
     symbols = torch.round(b).to(torch.int32) - coff
-    return F.compress_ragged(self._lookup_host(), lengths, symbols.reshape(-1))
+    strings = F.compress_ragged(self._lookup_host(), lengths, symbols.reshape(-1))
+    if not return_decoded:
+      return strings
+    return strings, self.decompress_ragged(strings, [tuple(b.shape[:b.dim() - rank_p]) for b in items])
 
   def decompress_ragged(self, strings, broadcast_shapes):
     """Inverse of compress_ragged: item i has shape `broadcast_shapes[i] + prior_shape` and equals
@@ -598,10 +606,14 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
         raise ValueError(f"each item needs {self.coding_rank} dimensions: received indexes for shape {s}")
     return flat, shapes
 
-  def compress_ragged(self, bottlenecks, indexes, _loc=None):
+  def compress_ragged(self, bottlenecks, indexes, _loc=None, return_decoded=False):
     """Compresses a list of coding units of different shapes (each with exactly `coding_rank` dimensions) in one
     range-coder launch.  Returns a Strings of shape (k,) whose string i equals `compress(bottlenecks[i],
-    indexes[i])`."""
+    indexes[i])`.
+
+    `return_decoded=True` returns `(strings, items)` with `items` equal, bit for bit, to
+    `decompress_ragged(strings, indexes)`: written by the encoder itself for a float32 bottleneck, decoded from the
+    fresh strings otherwise."""
     self._check_compression()
     dev = _cuda()
     items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
@@ -615,11 +627,15 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     coff = self.cdf_offset.to(dev)
     lengths = [b.numel() for b in items]
     if self.bottleneck_dtype == torch.float32:
-      return F.compress_ragged(self._lookup_host(), lengths, b, loc, coff, index=flat)
+      out = F.compress_ragged(self._lookup_host(), lengths, b, loc, coff, index=flat, decoded=return_decoded)
+      return (out[0], _split_items(out[1], shapes)) if return_decoded else out
     if loc is not None:
       b = b - loc
     symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
-    return F.compress_ragged(self._lookup_host(), lengths, symbols, index=flat)
+    strings = F.compress_ragged(self._lookup_host(), lengths, symbols, index=flat)
+    if not return_decoded:
+      return strings
+    return strings, ContinuousIndexedEntropyModel.decompress_ragged(self, strings, indexes, _loc=_loc)
 
   def decompress_ragged(self, strings, indexes, _loc=None):
     """Inverse of compress_ragged: item i has the coding shape of `indexes[i]`.  The items are views into one
@@ -683,9 +699,9 @@ class LocationScaleIndexedEntropyModel(ContinuousIndexedEntropyModel):
   def decompress(self, strings, scale_indexes, loc=None, fused=True):
     return super().decompress(strings, scale_indexes, fused=fused, _loc=loc)
 
-  def compress_ragged(self, bottlenecks, scale_indexes, loc=None):
+  def compress_ragged(self, bottlenecks, scale_indexes, loc=None, return_decoded=False):
     """`loc`: None or a list with one tensor per item."""
-    return super().compress_ragged(bottlenecks, scale_indexes, _loc=loc)
+    return super().compress_ragged(bottlenecks, scale_indexes, _loc=loc, return_decoded=return_decoded)
 
   def decompress_ragged(self, strings, scale_indexes, loc=None):
     return super().decompress_ragged(strings, scale_indexes, _loc=loc)

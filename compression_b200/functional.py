@@ -206,12 +206,16 @@ def _symbol_offsets(lengths):
   return np.ascontiguousarray(np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64))
 
 
-def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, index=None):
+def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, index=None, decoded=False):
   """One compress over streams of different lengths: stream i is the next `lengths[i]` elements of the flat
   `value`.  `value` int32 holds symbols; float32 is quantised in the kernel like compress_f32 (`quant_offset` per
   row in channel mode, the loc tensor in index mode; `cdf_offset` required).  Channel mode (index None) restarts
   at row 0 in every stream.  Returns a Strings of shape (len(lengths),) whose string i equals what compress_f32 /
-  entropy_encode_* give for stream i alone."""
+  entropy_encode_* give for stream i alone.
+
+  `decoded=True` (float values only) returns `(strings, decoded_flat)`: the encoder also writes, per symbol, what
+  decode_ragged with the same `quant_offset` / `cdf_offset` returns for these strings, bit for bit, so an encoder
+  that conditions on its own reconstruction needs no decode."""
   from compression_b200 import gen_ops
   offs = _symbol_offsets(lengths)
   lookup = gen_ops._host_i32(lookup)
@@ -229,17 +233,24 @@ def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, 
   h, total = C.c_void_p(), C.c_int64(0)
   stream = _stream()
   L = _lib.lib()
-  check(L.tfcb_compress_ragged(lookup.ctypes.data_as(C.c_void_p), lookup.size,
-                               0 if lookup.ndim == 1 else lookup.shape[1], k, offs.ctypes.data_as(C.c_void_p),
-                               _p(index), _p(value), int(is_f32), _p(_f32(quant_offset, dev)),
-                               _p(_i32(cdf_offset, dev)), _p(offsets), stream, C.byref(h), C.byref(total)))
+  qoff, coff = _f32(quant_offset, dev), _i32(cdf_offset, dev)  # (kept alive until the call has returned)
+  args = (lookup.ctypes.data_as(C.c_void_p), lookup.size, 0 if lookup.ndim == 1 else lookup.shape[1], k,
+          offs.ctypes.data_as(C.c_void_p), _p(index), _p(value), int(is_f32), _p(qoff), _p(coff), _p(offsets),
+          stream, C.byref(h), C.byref(total))
+  if decoded:
+    buf = torch.empty(max(int(offs[-1]), 1), dtype=torch.float32, device=dev)  # (never null, even with no symbols)
+    dec = buf[:int(offs[-1])]
+    check(L.tfcb_compress_ragged_decoded(*args, _p(buf)))
+  else:
+    check(L.tfcb_compress_ragged(*args))
   try:
     out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
   except BaseException:
     L.tfcb_encoder_destroy(h)
     raise
   check(L.tfcb_compress_write(h, _p(offsets), _p(out), stream))
-  return gen_ops.Strings(out, offsets, (k,))
+  strings = gen_ops.Strings(out, offsets, (k,))
+  return (strings, dec) if decoded else strings
 
 
 def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=None):

@@ -481,6 +481,66 @@ class MS2020Model(_Model):
   def decompress(self, x_shape, y_shape, z_shape, z_string, *y_strings):
     return self.decompress_batch(x_shape, y_shape, z_shape, z_string, *y_strings)[0]
 
+  # -- lists of differently sized images: transforms per image; one range-coder launch for z and one per slice, each
+  # encode handing back the latents it coded, so the encoder decodes nothing --
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element.
+    num_slices + 1 encode launches in all, whatever the number of images, and no decode."""
+    xs = [_as_image(x)[None].to(device=self._device(), dtype=torch.float32) for x in images]
+    if not xs:
+      raise ValueError("`images` is empty")
+    ys = [self.analysis_transform(x) for x in xs]
+    zs = [self.hyper_analysis_transform(y) for y in ys]
+    y_hws = [tuple(y.shape[1:-1]) for y in ys]
+    z_strings, z_hats = self.em_z.compress_ragged([z[0] for z in zs], return_decoded=True)
+    z_strings = z_strings.split()
+    latents = [(self.hyper_synthesis_mean_transform(z_hat[None]), self.hyper_synthesis_scale_transform(z_hat[None]))
+               for z_hat in z_hats]
+    y_hat_slices = [[] for _ in xs]
+    y_strings = []
+    y_slices = [torch.chunk(y, self.num_slices, dim=-1) for y in ys]
+    for i in range(self.num_slices):
+      params = [self._slice_params(i, lm, ls, sl, hw) for (lm, ls), sl, hw in zip(latents, y_hat_slices, y_hws)]
+      strings, y_hats = self.em_y.compress_ragged([s[i][0] for s in y_slices], [p[1][0] for p in params],
+                                                  loc=[p[0][0] for p in params], return_decoded=True)
+      y_strings.append(strings.split())
+      for sl, p, y_hat in zip(y_hat_slices, params, y_hats):
+        sl.append(self._lrp(i, p[2], y_hat[None]))
+    out = []
+    for k, (x, y, z) in enumerate(zip(xs, ys, zs)):
+      shapes = tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+      out.append(shapes + (z_strings[k],) + tuple(s[k] for s in y_strings))
+    return out
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3].  num_slices + 1 decode
+    launches in all, whatever the number of images."""
+    items = list(items)
+    if not items:
+      raise ValueError("`items` is empty")
+    for it in items:
+      if len(it) != 4 + self.num_slices:
+        raise ValueError(f"each item needs 3 shapes and {self.num_slices + 1} strings: received {len(it)} elements")
+    y_hws = [(int(it[1][0]), int(it[1][1])) for it in items]
+    z_hats = self.em_z.decompress_ragged(gen_ops.Strings.concat([it[3] for it in items]),
+                                         [tuple(int(v) for v in it[2]) for it in items])
+    latents = [(self.hyper_synthesis_mean_transform(z_hat[None]), self.hyper_synthesis_scale_transform(z_hat[None]))
+               for z_hat in z_hats]
+    y_hat_slices = [[] for _ in items]
+    for i in range(self.num_slices):
+      params = [self._slice_params(i, lm, ls, sl, hw) for (lm, ls), sl, hw in zip(latents, y_hat_slices, y_hws)]
+      y_hats = self.em_y.decompress_ragged(gen_ops.Strings.concat([it[4 + i] for it in items]),
+                                           [p[1][0] for p in params], loc=[p[0][0] for p in params])
+      for sl, p, y_hat in zip(y_hat_slices, params, y_hats):
+        sl.append(self._lrp(i, p[2], y_hat[None]))
+    out = []
+    for sl, it in zip(y_hat_slices, items):
+      x_hat = self.synthesis_transform(torch.cat(sl, dim=-1))
+      out.append(_to_uint8(x_hat[:, :int(it[0][0]), :int(it[0][1]), :])[0])
+    return out
+
   def compress_to_tfci(self, x):
     packed = PackedTensors()
     packed.pack(self.compress(x))

@@ -122,6 +122,19 @@ int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t
                          const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
                          int32_t value_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev,
                          int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host);
+/* tfcb_compress_ragged that also hands back what decoding the strings would give, without decoding them: on success
+ * `decoded_dev` (float32, one per symbol over all streams, symbol_offsets_host[n_streams] in all) holds exactly
+ * what tfcb_decode_ragged(..., out_is_f32 = 1, the same quant_offset_dev and cdf_offset_dev) returns for these
+ * strings, bit for bit: float(symbol + cdf_offset[row]) + quant_offset (or loc), with the integer the encoder
+ * codes (so |y - loc| >= 2^31 saturates and NaN gives 0, as in the decoder).  An encoder that needs the decoded
+ * values to condition what it codes next (channel-conditional models) saves a decode per step.  Offsets, the one
+ * synchronisation, the returned encoder and the error messages are tfcb_compress_ragged's.  Checked before any
+ * device work (TFCB_INVALID_ARGUMENT): `value_is_f32` nonzero, `decoded_dev` and `cdf_offset_dev` non-null. */
+int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols,
+                                 int64_t n_streams, const int64_t* symbol_offsets_host, const int32_t* index_dev,
+                                 const void* value_dev, int32_t value_is_f32, const float* quant_offset_dev,
+                                 const int32_t* cdf_offset_dev, int64_t* offsets_dev, void* stream,
+                                 tfcb_encoder** out, int64_t* total_bytes_host, float* decoded_dev);
 
 /* ------------------------------------------------------------------------------------------------
  * Range DECODER.  Replaces CreateRangeDecoder / EntropyDecodeChannel / EntropyDecodeIndex /
