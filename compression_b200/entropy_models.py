@@ -31,30 +31,18 @@ def _cuda():
   return torch.device("cuda", torch.cuda.current_device())
 
 
-def _numel(shape):
-  return int(np.prod(shape)) if len(shape) else 1
-
-
-def _split_items(flat, shapes):
-  """Views of a flat tensor holding items of the given shapes back to back."""
-  out, at = [], 0
-  for shape in shapes:
-    n = _numel(shape)
-    out.append(flat[at:at + n].reshape(shape))
-    at += n
-  return out
-
-
-def _ragged_strings(strings, k):
-  if not isinstance(strings, gen_ops.Strings):
-    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
-  if strings.numel() != k:
-    raise ValueError(f"{strings.numel()} strings for {k} items")
-  return strings
-
-
 class ContinuousEntropyModelBase(nn.Module):
-  """continuous_base.py:36-370."""
+  """continuous_base.py:36-370.
+
+  The range-coding plumbing every model's compress / decompress and their ragged forms share lives here (`_encode`,
+  `_decode`, `_encode_ragged`, `_decode_ragged`); a model derives only its batch shape or item shapes, and the
+  table index and offset of every element.  Two coding modes:
+    channel mode (`index` None, ContinuousBatchedEntropyModel): element j of a coding unit uses table row
+      j % rows, where `coff` / `off` hold one value per row (float32 offsets);
+    index mode: element j uses row `index[j]`, and `off` (or None) has the bottleneck's shape.
+  """
+
+  decode_sanity_check = True
 
   def __init__(self, coding_rank=None, compression=False, stateless=False, expected_grads=False,
                tail_mass=2**-8, bottleneck_dtype=None, laplace_tail_mass=0):
@@ -186,7 +174,7 @@ class ContinuousEntropyModelBase(nn.Module):
     samples = torch.arange(max_length, dtype=dtype).reshape([-1] + pmf_length.dim() * [1]) + pmf_start
     pmf = prior.prob(samples.to(prior_dev))
     pmf_shape = tuple(pmf.shape[1:])
-    num_pmfs = int(np.prod(pmf_shape)) if pmf_shape else 1
+    num_pmfs = gen_ops._prod(pmf_shape)
     pmf = pmf.reshape(max_length, num_pmfs).t().contiguous()
     pmf_length = torch.broadcast_to(pmf_length, pmf_shape).reshape(num_pmfs)
     cdf_offset = torch.broadcast_to(minima, pmf_shape).reshape(num_pmfs)
@@ -233,6 +221,99 @@ class ContinuousEntropyModelBase(nn.Module):
       old = getattr(self, n)
       setattr(self, n, torch.as_tensor(w).to(device=old.device, dtype=old.dtype))
     self._cdf_host = None
+
+  # -- range coding --
+  @staticmethod
+  def _strings(strings, k=None):
+    """`strings` as a Strings; with `k`, a list of the k strings of a ragged batch."""
+    if not isinstance(strings, gen_ops.Strings):
+      if k is not None:
+        strings = list(strings)
+      strings = gen_ops.Strings.from_bytes(strings, None if k is None else (len(strings),))
+    if k is not None and strings.numel() != k:
+      raise ValueError(f"{strings.numel()} strings for {k} items")
+    return strings
+
+  def _finish_decode(self, handle):
+    sanity = gen_ops.entropy_decode_finalize(handle)
+    if self.decode_sanity_check and not bool(sanity.all()):
+      raise gen_ops.InvalidArgumentError("Sanity check failed.")
+
+  def _quantize(self, b, off, coff, index=None):
+    """The unfused quantisation to the symbols the coder takes.  Channel mode: rint(float32(b) - off[row]) -> int32 -
+    coff[row], as [elements / rows, rows].  Index mode: rint(b - off) -> int32 - coff[index] in b's dtype, shaped like
+    b.  (continuous_batched.py casts to float32 first, continuous_indexed.py and universal.py do not: the two differ
+    for float16 and float64 bottlenecks.)"""
+    if index is None:
+      b = b.to(torch.float32).reshape(-1, coff.numel())
+      return torch.round(b if off is None else b - off).to(torch.int32) - coff
+    return torch.round(b if off is None else b - off).to(torch.int32) - coff[index.long()]
+
+  def _dequantize(self, symbols, off, coff, index=None):
+    """Inverse of _quantize, in bottleneck_dtype: float(sym + coff[row]) + off[row], as [elements / rows, rows]
+    (channel mode), or float(sym + coff[index]) + off shaped like `symbols` (index mode)."""
+    if index is None:
+      out = (symbols.reshape(-1, coff.numel()) + coff).to(self.bottleneck_dtype)
+      return out if off is None else out + off.to(out.dtype)
+    out = (symbols + coff[index.long()]).to(self.bottleneck_dtype)
+    return out if off is None else out + off
+
+  def _encode(self, batch_shape, b, off, coff, index=None, fused=True):
+    """One string per element of `batch_shape` for `b` (in bottleneck_dtype, coding units innermost).  A float32
+    bottleneck is quantised inside the encoder unless `fused=False`, which issues the reference's op sequence."""
+    if fused and b.dtype == torch.float32:
+      return F.compress_f32(batch_shape, self._lookup_host(), b, off, coff, index=index)
+    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
+    symbols = self._quantize(b, off, coff, index)
+    if index is None:  # the reference's iid_shape + [-1]: every axis left of prior_shape, then the table rows
+      gen_ops.entropy_encode_channel(handle, symbols.reshape(b.shape[:b.dim() - len(self.prior_shape)] + (-1,)))
+    else:
+      gen_ops.entropy_encode_index(handle, index, symbols)
+    return gen_ops.entropy_encode_finalize(handle)
+
+  def _decode(self, strings, shape, off, coff, index=None, fused=True):
+    """Inverse of _encode: a tensor of shape strings.shape + `shape` (the coding unit's) in bottleneck_dtype."""
+    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
+    if fused and self.bottleneck_dtype == torch.float32:
+      if index is None:
+        out = F.decode_channel_f32(handle, strings.shape + shape, off, coff)
+      else:
+        out = F.decode_index_f32(handle, index, off, coff)
+      self._finish_decode(handle)
+      return out
+    if index is None:  # the reference decodes shape[:-rank(prior_shape)] + [rows]
+      lead = shape[:len(shape) - len(self.prior_shape)]
+      handle, symbols = gen_ops.entropy_decode_channel(handle, lead + (gen_ops._prod(self.prior_shape),))
+    else:
+      handle, symbols = gen_ops.entropy_decode_index(handle, index, shape)
+    self._finish_decode(handle)
+    return self._dequantize(symbols, off, coff, index).reshape(strings.shape + shape)
+
+  # ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none)
+  def _encode_ragged(self, shapes, b, off, coff, index=None, return_decoded=False):
+    """Strings of shape (k,) for the k items of the given shapes that `b` (in bottleneck_dtype) holds back to back;
+    with `return_decoded`, also what _decode_ragged makes of them.  A float32 bottleneck is quantised inside the
+    encoder, which then also writes the decoded items."""
+    lengths = [gen_ops._prod(s) for s in shapes]
+    if b.dtype == torch.float32:
+      out = F.compress_ragged(self._lookup_host(), lengths, b, off, coff, index=index, decoded=return_decoded)
+      return (out[0], gen_ops._split_items(out[1], shapes)) if return_decoded else out
+    strings = F.compress_ragged(self._lookup_host(), lengths, self._quantize(b, off, coff, index), index=index)
+    return (strings, self._decode_ragged(strings, shapes, off, coff, index)) if return_decoded else strings
+
+  def _decode_ragged(self, strings, shapes, off, coff, index=None):
+    """Inverse of _encode_ragged: the items, views into one allocation."""
+    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
+    lengths = [gen_ops._prod(s) for s in shapes]
+    fused = self.bottleneck_dtype == torch.float32
+    if fused:
+      out = F.decode_ragged(handle, lengths, index=index, quant_offset=off, cdf_offset=coff)
+    else:
+      out = F.decode_ragged(handle, lengths, index=index)
+    self._finish_decode(handle)
+    if not fused:
+      out = self._dequantize(out, off, coff, index).reshape(-1)
+    return gen_ops._split_items(out, shapes)
 
 
 class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
@@ -343,44 +424,15 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     if rank_p and shape[-rank_p:] != self.prior_shape:
       bottleneck = torch.broadcast_to(bottleneck, shape[:-rank_p] + self.prior_shape)
     coff, qoff = self._flat_tables(bottleneck.device)
-    if fused and bottleneck.dtype == torch.float32:
-      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, qoff, coff)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
-    b = bottleneck.to(torch.float32)
-    if qoff is not None:
-      b = b - qoff.reshape(self.prior_shape)
-    symbols = torch.round(b).to(torch.int32)
-    iid = shape[:len(shape) - rank_p] if rank_p else shape
-    symbols = symbols.reshape(iid + (-1,)) - coff
-    gen_ops.entropy_encode_channel(handle, symbols)
-    return gen_ops.entropy_encode_finalize(handle)
+    return self._encode(batch_shape, bottleneck, qoff, coff, fused=fused)
 
   def decompress(self, strings, broadcast_shape, fused=True):
     """continuous_batched.py:385-422."""
     self._check_compression()
-    if not isinstance(strings, gen_ops.Strings):
-      strings = gen_ops.Strings.from_bytes(strings)
+    strings = self._strings(strings)
     broadcast_shape = tuple(int(d) for d in np.asarray(broadcast_shape).reshape(-1))
-    n_prior = int(np.prod(self.prior_shape)) if self.prior_shape else 1
-    output_shape = tuple(strings.shape) + broadcast_shape + self.prior_shape
-    dev = strings.bytes_dev.device
-    coff, qoff = self._flat_tables(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    if fused and self.bottleneck_dtype == torch.float32:
-      outputs = F.decode_channel_f32(handle, output_shape, qoff, coff)
-      sanity = gen_ops.entropy_decode_finalize(handle)
-      if self.decode_sanity_check and not bool(sanity.all()):
-        raise gen_ops.InvalidArgumentError("Sanity check failed.")
-      return outputs
-    handle, symbols = gen_ops.entropy_decode_channel(handle, broadcast_shape + (n_prior,))
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    symbols = symbols + coff
-    outputs = symbols.reshape(output_shape).to(self.bottleneck_dtype)
-    if qoff is not None:
-      outputs = outputs + qoff.reshape(self.prior_shape).to(outputs.dtype)
-    return outputs
+    coff, qoff = self._flat_tables(strings.bytes_dev.device)
+    return self._decode(strings, broadcast_shape + self.prior_shape, qoff, coff, fused=fused)
 
   # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
   def compress_ragged(self, bottlenecks, return_decoded=False):
@@ -401,45 +453,19 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
                          f"received shape {tuple(b.shape)}")
     if not items:
       raise ValueError("`bottlenecks` is empty")
-    lengths = [b.numel() for b in items]
     coff, qoff = self._flat_tables(dev)
-    flat = torch.cat([b.reshape(-1) for b in items])
-    if self.bottleneck_dtype == torch.float32:
-      out = F.compress_ragged(self._lookup_host(), lengths, flat, qoff, coff, decoded=return_decoded)
-      return (out[0], _split_items(out[1], [tuple(b.shape) for b in items])) if return_decoded else out
-    # compress()'s unfused arithmetic; every item holds whole rows of prior_shape, so the rows line up
-    b = flat.to(torch.float32).reshape(-1, coff.numel())
-    if qoff is not None:
-      b = b - qoff
-    symbols = torch.round(b).to(torch.int32) - coff
-    strings = F.compress_ragged(self._lookup_host(), lengths, symbols.reshape(-1))
-    if not return_decoded:
-      return strings
-    return strings, self.decompress_ragged(strings, [tuple(b.shape[:b.dim() - rank_p]) for b in items])
+    # every item holds whole rows of prior_shape, so channel mode's rows line up across items
+    return self._encode_ragged([tuple(b.shape) for b in items], torch.cat([b.reshape(-1) for b in items]), qoff,
+                               coff, return_decoded=return_decoded)
 
   def decompress_ragged(self, strings, broadcast_shapes):
     """Inverse of compress_ragged: item i has shape `broadcast_shapes[i] + prior_shape` and equals
     `decompress(strings[i:i+1], broadcast_shapes[i])[0]`.  The items are views into one allocation."""
     self._check_compression()
     shapes = [tuple(int(d) for d in np.asarray(s).reshape(-1)) + self.prior_shape for s in broadcast_shapes]
-    strings = _ragged_strings(strings, len(shapes))
-    dev = strings.bytes_dev.device
-    coff, qoff = self._flat_tables(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    lengths = [_numel(s) for s in shapes]
-    if self.bottleneck_dtype == torch.float32:
-      outputs = F.decode_ragged(handle, lengths, quant_offset=qoff, cdf_offset=coff)
-    else:
-      symbols = F.decode_ragged(handle, lengths)
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    if self.bottleneck_dtype != torch.float32:
-      outputs = (symbols.reshape(-1, coff.numel()) + coff).to(self.bottleneck_dtype)
-      if qoff is not None:
-        outputs = outputs + qoff.to(outputs.dtype)
-      outputs = outputs.reshape(-1)
-    return _split_items(outputs, shapes)
+    strings = self._strings(strings, len(shapes))
+    coff, qoff = self._flat_tables(strings.bytes_dev.device)
+    return self._decode_ragged(strings, shapes, qoff, coff)
 
   def get_config(self):
     """continuous_batched.py:424-436."""
@@ -553,40 +579,18 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     indexes = self._normalize_indexes(torch.as_tensor(indexes).to(device=dev, dtype=self.prior_dtype))
     flat = self._flatten_indexes(indexes)
     fshape = tuple(flat.shape)
-    batch_shape = fshape[:len(fshape) - self.coding_rank]
-    coff = self.cdf_offset.to(dev)
-    if fused and bottleneck.dtype == torch.float32:
-      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, _loc, coff, index=flat)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
-    b = bottleneck if _loc is None else bottleneck - _loc
-    symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
-    gen_ops.entropy_encode_index(handle, flat, symbols)
-    return gen_ops.entropy_encode_finalize(handle)
+    return self._encode(fshape[:len(fshape) - self.coding_rank], bottleneck, _loc, self.cdf_offset.to(dev), flat,
+                        fused)
 
   def decompress(self, strings, indexes, fused=True, _loc=None):
     """continuous_indexed.py:388-417."""
     self._check_compression()
-    if not isinstance(strings, gen_ops.Strings):
-      strings = gen_ops.Strings.from_bytes(strings)
+    strings = self._strings(strings)
     dev = strings.bytes_dev.device
     indexes = self._normalize_indexes(torch.as_tensor(indexes).to(device=dev, dtype=self.prior_dtype))
     flat = self._flatten_indexes(indexes)
     fshape = tuple(flat.shape)
-    decode_shape = fshape[len(fshape) - self.coding_rank:] if self.coding_rank else ()
-    coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    if fused and self.bottleneck_dtype == torch.float32:
-      out = F.decode_index_f32(handle, flat, _loc, coff)
-      symbols = None
-    else:
-      handle, symbols = gen_ops.entropy_decode_index(handle, flat, decode_shape)
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    if symbols is None:
-      return out
-    out = (symbols + coff[flat.long()]).to(self.bottleneck_dtype)
-    return out if _loc is None else out + _loc
+    return self._decode(strings, fshape[len(fshape) - self.coding_rank:], _loc, self.cdf_offset.to(dev), flat, fused)
 
   # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
   def _ragged_indexes(self, indexes, dev):
@@ -624,43 +628,17 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     b = torch.cat([b.reshape(-1) for b in items])
     if loc is not None and loc.numel() != b.numel():
       raise ValueError("each `loc` item must have the shape of its bottleneck")
-    coff = self.cdf_offset.to(dev)
-    lengths = [b.numel() for b in items]
-    if self.bottleneck_dtype == torch.float32:
-      out = F.compress_ragged(self._lookup_host(), lengths, b, loc, coff, index=flat, decoded=return_decoded)
-      return (out[0], _split_items(out[1], shapes)) if return_decoded else out
-    if loc is not None:
-      b = b - loc
-    symbols = torch.round(b).to(torch.int32) - coff[flat.long()]
-    strings = F.compress_ragged(self._lookup_host(), lengths, symbols, index=flat)
-    if not return_decoded:
-      return strings
-    return strings, ContinuousIndexedEntropyModel.decompress_ragged(self, strings, indexes, _loc=_loc)
+    return self._encode_ragged(shapes, b, loc, self.cdf_offset.to(dev), flat, return_decoded)
 
   def decompress_ragged(self, strings, indexes, _loc=None):
     """Inverse of compress_ragged: item i has the coding shape of `indexes[i]`.  The items are views into one
     allocation."""
     self._check_compression()
-    strings = _ragged_strings(strings, len(indexes))
+    strings = self._strings(strings, len(indexes))
     dev = strings.bytes_dev.device
     flat, shapes = self._ragged_indexes(indexes, dev)
     loc = None if _loc is None else torch.cat([torch.as_tensor(l).to(dev).reshape(-1) for l in _loc])
-    coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    lengths = [_numel(s) for s in shapes]
-    fused = self.bottleneck_dtype == torch.float32
-    if fused:
-      out = F.decode_ragged(handle, lengths, index=flat, quant_offset=loc, cdf_offset=coff)
-    else:
-      symbols = F.decode_ragged(handle, lengths, index=flat)
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    if not fused:
-      out = (symbols + coff[flat.long()]).to(self.bottleneck_dtype)
-      if loc is not None:
-        out = out + loc
-    return _split_items(out, shapes)
+    return self._decode_ragged(strings, shapes, loc, self.cdf_offset.to(dev), flat)
 
   def get_config(self):
     raise NotImplementedError("Serializing indexed entropy models is not yet implemented.")
@@ -736,9 +714,7 @@ def stateless_uniform_int(shape, seed, maxval, device=None):
   key / counter conventions are not reproduced (there is no TF here to pin them against): strings written with
   universal quantisation decode with THIS implementation, not with the reference's."""
   shape = tuple(int(d) for d in shape)
-  n = 1
-  for d in shape:
-    n *= d
+  n = gen_ops._prod(shape)
   blocks = (n + 3) // 4
   counter = torch.zeros(blocks, 4, dtype=torch.int64, device=device)
   idx = torch.arange(blocks, dtype=torch.int64, device=device)
@@ -794,7 +770,7 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
   def _compute_indexes_and_offset(self, broadcast_shape, device):
     """universal.py:147-170 -> (flat table index, quantisation offset), both of shape broadcast_shape + prior_shape."""
     broadcast_shape = tuple(int(d) for d in broadcast_shape)
-    prior_size = int(np.prod(self.prior_shape)) if self.prior_shape else 1
+    prior_size = gen_ops._prod(self.prior_shape)
     indexes = torch.arange(prior_size, dtype=torch.int32, device=device)
     indexes = torch.broadcast_to(indexes, broadcast_shape + (prior_size,))[..., None]
     indexes = _add_offset_indexes(indexes, self._num_noise_levels)
@@ -828,20 +804,13 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
     broadcast_shape = coding_shape[:self.coding_rank - len(self.prior_shape)]
     indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
     indexes = torch.broadcast_to(indexes, shape).contiguous()
-    coff = self.cdf_offset.to(dev)
-    if fused and bottleneck.dtype == torch.float32:
-      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck,
-                            torch.broadcast_to(offset, shape).contiguous(), coff, index=indexes)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
-    symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[indexes.long()]
-    gen_ops.entropy_encode_index(handle, indexes, symbols)
-    return gen_ops.entropy_encode_finalize(handle)
+    offset = torch.broadcast_to(offset, shape).contiguous()
+    return self._encode(batch_shape, bottleneck, offset, self.cdf_offset.to(dev), indexes, fused)
 
   def decompress(self, strings, broadcast_shape, fused=True):
     """universal.py:253-289."""
     self._check_compression()
-    if not isinstance(strings, gen_ops.Strings):
-      strings = gen_ops.Strings.from_bytes(strings)
+    strings = self._strings(strings)
     dev = strings.bytes_dev.device
     broadcast_shape = tuple(int(d) for d in np.asarray(broadcast_shape).reshape(-1))
     decode_shape = broadcast_shape + self.prior_shape
@@ -849,19 +818,7 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
     indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
     indexes = torch.broadcast_to(indexes, output_shape).contiguous()
     offset = torch.broadcast_to(offset, output_shape).contiguous()
-    coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    if fused and self.bottleneck_dtype == torch.float32:
-      outputs = F.decode_index_f32(handle, indexes, offset, coff)
-      symbols = None
-    else:
-      handle, symbols = gen_ops.entropy_decode_index(handle, indexes, decode_shape)
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    if symbols is None:
-      return outputs
-    return (symbols + coff[indexes.long()]).to(self.bottleneck_dtype) + offset
+    return self._decode(strings, decode_shape, offset, self.cdf_offset.to(dev), indexes, fused)
 
   def get_config(self):
     raise NotImplementedError()
@@ -958,37 +915,18 @@ class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
     bottleneck = torch.as_tensor(bottleneck).to(device=dev, dtype=self.bottleneck_dtype)
     flat, offset = self._coding_tensors(indexes, dev)
     fshape = tuple(flat.shape)
-    batch_shape = fshape[:len(fshape) - self.coding_rank]
-    coff = self.cdf_offset.to(dev)
-    if fused and bottleneck.dtype == torch.float32:
-      return F.compress_f32(batch_shape, self._lookup_host(), bottleneck, offset, coff, index=flat)
-    handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
-    symbols = torch.round(bottleneck - offset).to(torch.int32) - coff[flat.long()]
-    gen_ops.entropy_encode_index(handle, flat, symbols)
-    return gen_ops.entropy_encode_finalize(handle)
+    return self._encode(fshape[:len(fshape) - self.coding_rank], bottleneck, offset, self.cdf_offset.to(dev), flat,
+                        fused)
 
   def decompress(self, strings, indexes, fused=True):
     """universal.py:568-598."""
     self._check_compression()
-    if not isinstance(strings, gen_ops.Strings):
-      strings = gen_ops.Strings.from_bytes(strings)
+    strings = self._strings(strings)
     dev = strings.bytes_dev.device
     flat, offset = self._coding_tensors(indexes, dev)
     fshape = tuple(flat.shape)
-    decode_shape = fshape[len(fshape) - self.coding_rank:]
-    coff = self.cdf_offset.to(dev)
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
-    if fused and self.bottleneck_dtype == torch.float32:
-      outputs = F.decode_index_f32(handle, flat, offset, coff)
-      symbols = None
-    else:
-      handle, symbols = gen_ops.entropy_decode_index(handle, flat, decode_shape)
-    sanity = gen_ops.entropy_decode_finalize(handle)
-    if self.decode_sanity_check and not bool(sanity.all()):
-      raise gen_ops.InvalidArgumentError("Sanity check failed.")
-    if symbols is None:
-      return outputs
-    return (symbols + coff[flat.long()]).to(self.bottleneck_dtype) + offset
+    return self._decode(strings, fshape[len(fshape) - self.coding_rank:], offset, self.cdf_offset.to(dev), flat,
+                        fused)
 
   def get_config(self):
     raise NotImplementedError()

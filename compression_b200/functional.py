@@ -5,7 +5,7 @@ import ctypes as C
 
 import torch
 
-from compression_b200 import _lib
+from compression_b200 import _lib, gen_ops
 from compression_b200._lib import check
 
 GDN_INVERSE = 1
@@ -167,28 +167,25 @@ def encode_index_f32(handle, index, y, loc, cdf_offset):
   return handle
 
 
-def compress_f32(batch_shape, lookup, y, quant_offset, cdf_offset, index=None):
-  """create_range_encoder + encode_channel_f32 (index None) or encode_index_f32 (`quant_offset` is then the loc
-  tensor) + entropy_encode_finalize, as two library calls with one host synchronisation.  The strings are
-  written into tensors this call allocates, so each result owns its memory."""
-  from compression_b200 import gen_ops
-  shape = tuple(int(d) for d in batch_shape)
+def _host_lookup(lookup):
   lookup = gen_ops._host_i32(lookup)
   if lookup.ndim not in (1, 2):
     raise _lib.InvalidArgumentError(f"`lookup` must be rank 1 or 2: {lookup.shape}")
+  return lookup
+
+
+def _compress(entry, lookup, shape, dev, *args, decoded=None):
+  """What compress_f32 and compress_ragged share: calls the library's `entry` with the table, the stream count,
+  `args`, the strings' offsets and (if given) the `decoded` buffer, then allocates the strings' bytes (releasing
+  the encoder if that fails) and writes the strings into them."""
   n_streams = gen_ops._prod(shape)
-  if n_streams == 0:
-    raise _lib.InvalidArgumentError(f"`handle` is empty: handle.shape={shape}")
-  y = _f32(y, y.device)
-  dev = y.device
-  index = _i32(index, dev)
   offsets = torch.empty(n_streams + 1, dtype=torch.int64, device=dev)
   h, total = C.c_void_p(), C.c_int64(0)
   stream = _stream()
+  tail = () if decoded is None else (_p(decoded),)
+  check(entry(lookup.ctypes.data_as(C.c_void_p), lookup.size, 0 if lookup.ndim == 1 else lookup.shape[1], n_streams,
+              *args, _p(offsets), stream, C.byref(h), C.byref(total), *tail))
   L = _lib.lib()
-  check(L.tfcb_compress(lookup.ctypes.data_as(C.c_void_p), lookup.size, 0 if lookup.ndim == 1 else lookup.shape[1],
-                        n_streams, _p(index), _p(y), 1, _p(_f32(quant_offset, dev)), _p(_i32(cdf_offset, dev)),
-                        y.numel() // n_streams, _p(offsets), stream, C.byref(h), C.byref(total)))
   try:
     out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
   except BaseException:
@@ -196,6 +193,22 @@ def compress_f32(batch_shape, lookup, y, quant_offset, cdf_offset, index=None):
     raise
   check(L.tfcb_compress_write(h, _p(offsets), _p(out), stream))
   return gen_ops.Strings(out, offsets, shape)
+
+
+def compress_f32(batch_shape, lookup, y, quant_offset, cdf_offset, index=None):
+  """create_range_encoder + encode_channel_f32 (index None) or encode_index_f32 (`quant_offset` is then the loc
+  tensor) + entropy_encode_finalize, as two library calls with one host synchronisation.  The strings are
+  written into tensors this call allocates, so each result owns its memory."""
+  shape = tuple(int(d) for d in batch_shape)
+  lookup = _host_lookup(lookup)
+  n_streams = gen_ops._prod(shape)
+  if n_streams == 0:
+    raise _lib.InvalidArgumentError(f"`handle` is empty: handle.shape={shape}")
+  y = _f32(y, y.device)
+  dev = y.device
+  index, qoff, coff = _i32(index, dev), _f32(quant_offset, dev), _i32(cdf_offset, dev)
+  return _compress(_lib.lib().tfcb_compress, lookup, shape, dev, _p(index), _p(y), 1, _p(qoff), _p(coff),
+                   y.numel() // n_streams)
 
 
 def _symbol_offsets(lengths):
@@ -216,11 +229,8 @@ def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, 
   `decoded=True` (float values only) returns `(strings, decoded_flat)`: the encoder also writes, per symbol, what
   decode_ragged with the same `quant_offset` / `cdf_offset` returns for these strings, bit for bit, so an encoder
   that conditions on its own reconstruction needs no decode."""
-  from compression_b200 import gen_ops
   offs = _symbol_offsets(lengths)
-  lookup = gen_ops._host_i32(lookup)
-  if lookup.ndim not in (1, 2):
-    raise _lib.InvalidArgumentError(f"`lookup` must be rank 1 or 2: {lookup.shape}")
+  lookup = _host_lookup(lookup)
   k = offs.size - 1
   dev = value.device
   is_f32 = value.dtype != torch.int32
@@ -229,28 +239,13 @@ def compress_ragged(lookup, lengths, value, quant_offset=None, cdf_offset=None, 
   if value.numel() != offs[-1] or (index is not None and index.numel() != offs[-1]):
     raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} symbols, but `value` has {value.numel()}"
                                     + ("" if index is None else f" and `index` {index.numel()}"))
-  offsets = torch.empty(k + 1, dtype=torch.int64, device=dev)
-  h, total = C.c_void_p(), C.c_int64(0)
-  stream = _stream()
-  L = _lib.lib()
   qoff, coff = _f32(quant_offset, dev), _i32(cdf_offset, dev)  # (kept alive until the call has returned)
-  args = (lookup.ctypes.data_as(C.c_void_p), lookup.size, 0 if lookup.ndim == 1 else lookup.shape[1], k,
-          offs.ctypes.data_as(C.c_void_p), _p(index), _p(value), int(is_f32), _p(qoff), _p(coff), _p(offsets),
-          stream, C.byref(h), C.byref(total))
-  if decoded:
-    buf = torch.empty(max(int(offs[-1]), 1), dtype=torch.float32, device=dev)  # (never null, even with no symbols)
-    dec = buf[:int(offs[-1])]
-    check(L.tfcb_compress_ragged_decoded(*args, _p(buf)))
-  else:
-    check(L.tfcb_compress_ragged(*args))
-  try:
-    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
-  except BaseException:
-    L.tfcb_encoder_destroy(h)
-    raise
-  check(L.tfcb_compress_write(h, _p(offsets), _p(out), stream))
-  strings = gen_ops.Strings(out, offsets, (k,))
-  return (strings, dec) if decoded else strings
+  args = (offs.ctypes.data_as(C.c_void_p), _p(index), _p(value), int(is_f32), _p(qoff), _p(coff))
+  if not decoded:
+    return _compress(_lib.lib().tfcb_compress_ragged, lookup, (k,), dev, *args)
+  buf = torch.empty(max(int(offs[-1]), 1), dtype=torch.float32, device=dev)  # (never null, even with no symbols)
+  strings = _compress(_lib.lib().tfcb_compress_ragged_decoded, lookup, (k,), dev, *args, decoded=buf)
+  return strings, buf[:int(offs[-1])]
 
 
 def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=None):
@@ -275,7 +270,6 @@ def run_length_encode_ragged(values, lengths, run_length_code, magnitude_code, u
   """RunLengthEncode of many strings in one launch: string i codes the next `lengths[i]` elements of the flat int32
   `values`.  Returns a Strings of shape (len(lengths),) whose string i equals gen_ops.run_length_encode of those
   elements alone (the empty string for a length of 0)."""
-  from compression_b200 import gen_ops
   offs = _symbol_offsets(lengths)
   k = offs.size - 1
   dev = gen_ops._device()
@@ -302,7 +296,6 @@ def run_length_decode_ragged(strings, lengths, run_length_code, magnitude_code, 
   """Inverse of run_length_encode_ragged, one thread per string in one launch: `strings` (a Strings or a list of
   bytes) holds len(lengths) strings; returns int32 [sum(lengths)], string after string.  A damaged string raises
   InvalidArgumentError naming the lowest-numbered failing string and the message gen_ops.run_length_decode gives."""
-  from compression_b200 import gen_ops
   offs = _symbol_offsets(lengths)
   k = offs.size - 1
   if not isinstance(strings, gen_ops.Strings):

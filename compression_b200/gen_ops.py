@@ -74,6 +74,16 @@ def _prod(shape) -> int:
   return n
 
 
+def _split_items(flat: torch.Tensor, shapes) -> List[torch.Tensor]:
+  """Views of a flat tensor holding items of the given shapes back to back."""
+  out, at = [], 0
+  for shape in shapes:
+    n = _prod(shape)
+    out.append(flat[at:at + n].reshape(shape))
+    at += n
+  return out
+
+
 class Strings:
   """A tensor of byte strings (stand-in for a ``tf.string`` tensor).
 

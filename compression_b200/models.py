@@ -131,6 +131,12 @@ class _Model(nn.Module):
     mse = torch.mean((x - self._last_x_hat)**2)
     return bpp + self.lmbda * mse, bpp, mse
 
+  def compress_to_tfci(self, x):
+    """The .tfci container (bls2017.py:262-282): `compress(x)` packed into one byte string."""
+    packed = PackedTensors()
+    packed.pack(self.compress(x))
+    return packed.string
+
 
 class BLS2017Model(_Model):
   """models/bls2017.py:95-190."""
@@ -161,11 +167,7 @@ class BLS2017Model(_Model):
   # -- one image, the reference's signatures (bls2017.py:163-190) --
   def compress(self, x):
     """x: uint8 [H, W, 3] -> (string [1], x_shape [2], y_shape [2])."""
-    x = torch.as_tensor(x)
-    if x.dim() != 3 or x.shape[-1] != 3:
-      raise ValueError(f"expected one image [H, W, 3], received shape {tuple(x.shape)}")
-    strings, x_shape, y_shape = self.compress_batch(x[None])
-    return strings, x_shape, y_shape
+    return self.compress_batch(_as_image(x)[None])
 
   def decompress(self, string, x_shape, y_shape):
     """-> uint8 [H, W, 3]."""
@@ -212,12 +214,7 @@ class BLS2017Model(_Model):
       out.append(_to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0])
     return out
 
-  # -- .tfci container (bls2017.py:262-282 `compress`, :308-321 `decompress`) --
-  def compress_to_tfci(self, x):
-    packed = PackedTensors()
-    packed.pack(self.compress(x))
-    return packed.string
-
+  # -- .tfci container (bls2017.py:308-321 `decompress`) --
   def decompress_from_tfci(self, data):
     string, x_shape, y_shape = PackedTensors(data).unpack([bytes, torch.int32, torch.int32])
     return self.decompress(string, x_shape, y_shape)
@@ -267,10 +264,7 @@ class BMSHJ2018Model(_Model):
 
   def compress(self, x):
     """bmshj2018.py:225-245: uint8 [H, W, 3] -> (string, side_string, x_shape, y_shape, z_shape)."""
-    x = torch.as_tensor(x)
-    if x.dim() != 3 or x.shape[-1] != 3:
-      raise ValueError(f"expected one image [H, W, 3], received shape {tuple(x.shape)}")
-    return self.compress_batch(x[None])
+    return self.compress_batch(_as_image(x)[None])
 
   def decompress(self, string, side_string, x_shape, y_shape, z_shape):
     """bmshj2018.py:247-264."""
@@ -334,11 +328,6 @@ class BMSHJ2018Model(_Model):
       x_hat = self.synthesis_transform(y_hat[None])
       out.append(_to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0])
     return out
-
-  def compress_to_tfci(self, x):
-    packed = PackedTensors()
-    packed.pack(self.compress(x))
-    return packed.string
 
   def decompress_from_tfci(self, data):
     dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
@@ -473,10 +462,7 @@ class MS2020Model(_Model):
 
   def compress(self, x):
     """One image uint8 [H, W, 3], the reference's signature (ms2020.py:331-389)."""
-    x = torch.as_tensor(x)
-    if x.dim() != 3 or x.shape[-1] != 3:
-      raise ValueError(f"expected one image [H, W, 3], received shape {tuple(x.shape)}")
-    return self.compress_batch(x[None])
+    return self.compress_batch(_as_image(x)[None])
 
   def decompress(self, x_shape, y_shape, z_shape, z_string, *y_strings):
     return self.decompress_batch(x_shape, y_shape, z_shape, z_string, *y_strings)[0]
@@ -540,11 +526,6 @@ class MS2020Model(_Model):
       x_hat = self.synthesis_transform(torch.cat(sl, dim=-1))
       out.append(_to_uint8(x_hat[:, :int(it[0][0]), :int(it[0][1]), :])[0])
     return out
-
-  def compress_to_tfci(self, x):
-    packed = PackedTensors()
-    packed.pack(self.compress(x))
-    return packed.string
 
   def decompress_from_tfci(self, data):
     dtypes = [torch.int32] * 3 + [bytes] * (self.num_slices + 1)

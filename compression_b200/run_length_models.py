@@ -16,13 +16,6 @@ from compression_b200 import gen_ops
 from compression_b200 import math_ops
 
 
-def _prod(shape) -> int:
-  out = 1
-  for d in shape:
-    out *= int(d)
-  return out
-
-
 class _RunLengthEntropyModel(torch.nn.Module):
   """What power_law.py and laplace.py share: quantise with a straight-through round, code every coding unit
   (the innermost ``coding_rank`` axes) as its own string, decode back to ``bottleneck_dtype``."""
@@ -87,8 +80,8 @@ class _RunLengthEntropyModel(torch.nn.Module):
       raise ValueError(f"`bottleneck` must have at least {self.coding_rank} dimensions.")
     shape = tuple(bottleneck.shape)
     strings_shape = shape if self.coding_rank == 0 else shape[:len(shape) - self.coding_rank]
-    unit = _prod(shape[len(strings_shape):])
-    symbols = torch.round(bottleneck).to(torch.int32).reshape(_prod(strings_shape), unit)
+    unit = gen_ops._prod(shape[len(strings_shape):])
+    symbols = torch.round(bottleneck).to(torch.int32).reshape(gen_ops._prod(strings_shape), unit)
     strings = np.empty(symbols.shape[0], dtype=object)
     for i in range(symbols.shape[0]):
       strings[i] = self.encode_fn(symbols[i])
@@ -134,13 +127,9 @@ class _RunLengthEntropyModel(torch.nn.Module):
     for s in shapes:
       if len(s) != self.coding_rank:
         raise ValueError(f"each code shape needs exactly {self.coding_rank} dimensions: received {s}")
-    lengths = [_prod(s) for s in shapes]
+    lengths = [gen_ops._prod(s) for s in shapes]
     flat = functional.run_length_decode_ragged(strings, lengths, *self._code()).to(self.bottleneck_dtype)
-    out, at = [], 0
-    for s, n in zip(shapes, lengths):
-      out.append(flat[at:at + n].reshape(s))
-      at += n
-    return out
+    return gen_ops._split_items(flat, shapes)
 
 
 class PowerLawEntropyModel(_RunLengthEntropyModel):
