@@ -74,4 +74,19 @@ __device__ __forceinline__ void report(DevError* e, int code, long long stream, 
   }
 }
 
+// out[i] = sum over p of part[p * n + i], accumulated in double in the order of p: the fixed-order reduction of
+// per-CTA partials (GDN dgamma / dbeta and exponent gradients, deep-factorized parameter gradients).  A template
+// so that only the translation units that launch it compile it.
+namespace {
+template <typename = void>
+__global__ void reduce_partials_kernel(const float* __restrict__ part, int n_parts, long long n,
+                                       float* __restrict__ out) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double s = 0.0;
+  for (int p = 0; p < n_parts; ++p) s += (double)part[(long long)p * n + i];
+  out[i] = (float)s;
+}
+}  // namespace
+
 }  // namespace tfcb

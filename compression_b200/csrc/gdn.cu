@@ -330,16 +330,6 @@ gdn_bwd_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, 
   if (tid < C) part_b[(long long)blockIdx.x * C + tid] = bsum;
 }
 
-__global__ void reduce_partials_kernel(const float* __restrict__ part, int n_parts, long long n,
-                                       float* __restrict__ out) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  // pairwise-ish: accumulate in double for a stable, order-deterministic result
-  double s = 0.0;
-  for (int p = 0; p < n_parts; ++p) s += (double)part[(long long)p * n + i];
-  out[i] = (float)s;
-}
-
 // Any-C fallback backward: one CTA per launch slice, straightforward loops (small C only).
 __global__ void gdn_bwd_generic_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                                        const float* __restrict__ beta, const float* __restrict__ dy,

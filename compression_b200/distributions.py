@@ -174,6 +174,15 @@ class DeepFactorized(nn.Module):
         logits = logits + torch.tanh(self.factors[i]) * torch.tanh(logits)
     return logits.permute(2, 1, 0).reshape(shape)
 
+  def _packed_parameters(self):
+    """[channels, P]: softplus(matrices), biases, tanh(factors), each flattened row-major per channel, in that
+    order -- the layout of the fused log-likelihood kernels (P = 28 for num_filters (3, 3)).  Built with torch
+    operations, so gradients reach the raw parameters through autograd."""
+    C = self._channels
+    return torch.cat([torch.nn.functional.softplus(m).reshape(C, -1) for m in self.matrices] +
+                     [b.reshape(C, -1) for b in self.biases] + [torch.tanh(f).reshape(C, -1) for f in self.factors],
+                     dim=1)
+
   def log_cdf(self, x):
     return torch.nn.functional.logsigmoid(self._logits_cumulative(x))
 
@@ -335,6 +344,46 @@ def _logsum_expbig_minus_expsmall(big, small):
   return torch.where(torch.isinf(big), big, torch.log1p(-torch.exp(small - big)) + big)
 
 
+_LOC_SCALE_KINDS = {Normal: "normal", Logistic: "logistic", Laplace: "laplace"}
+
+
+def _fused_log_prob_form(base, y):
+  """Which fused kernel computes UniformNoiseAdapter(base).log_prob(y), judged from dtypes and shapes alone:
+  "deep_factorized", "normal", "logistic", "laplace" or None (the graph).
+    * DeepFactorized with num_filters (3, 3): y contiguous with trailing dimensions equal to the batch shape, so the
+      channel of element i is i mod prod(batch_shape);
+    * Normal / Logistic / Laplace: loc and scale each y-shaped and contiguous, or a broadcast scalar (every stride
+      0, as `_LocScale`'s broadcast_tensors hands over a scalar);
+  everything float32."""
+  if not isinstance(y, torch.Tensor) or y.dtype != torch.float32:
+    return None
+  if type(base) is DeepFactorized:
+    k = len(base.batch_shape)
+    params = list(base.matrices) + list(base.biases) + list(base.factors)
+    if (base.num_filters != (3, 3) or any(p.dtype != torch.float32 for p in params) or not y.is_contiguous() or
+        y.dim() < k or tuple(y.shape[y.dim() - k:]) != base.batch_shape):
+      return None
+    return "deep_factorized"
+  kind = _LOC_SCALE_KINDS.get(type(base))
+  if kind is None:
+    return None
+  for t in (base.loc, base.scale):
+    if (t.dtype != torch.float32 or tuple(t.shape) != tuple(y.shape) or
+        not (t.is_contiguous() or all(s == 0 for s in t.stride()))):
+      return None
+  return kind
+
+
+def _fused_log_prob_kind(base, y):
+  """The routing of UniformNoiseAdapter.log_prob: `_fused_log_prob_form` on CUDA tensors of one device, else None."""
+  kind = _fused_log_prob_form(base, y)
+  if kind is None or y.device.type != "cuda":
+    return None
+  tensors = ((base.loc, base.scale) if kind != "deep_factorized" else
+             list(base.matrices) + list(base.biases) + list(base.factors))
+  return kind if all(t.device == y.device for t in tensors) else None
+
+
 class UniformNoiseAdapter(nn.Module):
   """p(y) = c(y + .5) - c(y - .5) of a base density (uniform_noise.py:50-191)."""
 
@@ -355,7 +404,18 @@ class UniformNoiseAdapter(nn.Module):
     return self.base.device
 
   def log_prob(self, y):
-    """uniform_noise.py:128-151 (the log-sf / log-cdf select)."""
+    """uniform_noise.py:128-151.  float32 CUDA priors of the forms `_fused_log_prob_kind` accepts run the fused
+    kernels (forward and backward, `functional.noisy_*_log_prob`); everything else runs the graph."""
+    kind = _fused_log_prob_kind(self.base, y)
+    if kind is None:
+      return self._log_prob_graph(y)
+    from compression_b200 import functional
+    if kind == "deep_factorized":
+      return functional.noisy_deep_factorized_log_prob(y, self.base._packed_parameters())
+    return functional.noisy_loc_scale_log_prob(kind, y, self.base.loc, self.base.scale)
+
+  def _log_prob_graph(self, y):
+    """The log-sf / log-cdf select as a graph of torch operations (any device and dtype)."""
     b = self.base
     logsf_p, logsf_m = b.log_survival_function(y + .5), b.log_survival_function(y - .5)
     logcdf_p, logcdf_m = b.log_cdf(y + .5), b.log_cdf(y - .5)
@@ -508,7 +568,7 @@ class NoisyMixtureSameFamily(nn.Module):
 
   def log_prob(self, y):
     y = torch.as_tensor(y, dtype=self.dtype, device=self.device).unsqueeze(-1)
-    return torch.logsumexp(torch.log(self.mixture_probs) + self.components_distribution.log_prob(y), -1)
+    return torch.logsumexp(torch.log(self.mixture_probs) + self.components_distribution._log_prob_graph(y), -1)
 
   def prob(self, y):
     y = torch.as_tensor(y, dtype=self.dtype, device=self.device).unsqueeze(-1)

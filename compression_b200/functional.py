@@ -136,6 +136,103 @@ def gdn(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon=1.0):
 
 
 # ------------------------------------------------------------------------------------------------
+# Rate term: log p(y) under uniform noise (UniformNoiseAdapter.log_prob, uniform_noise.py:128-151), fused
+# ------------------------------------------------------------------------------------------------
+DEEP_FACTORIZED_PARAMS = 28  # per channel of num_filters (3, 3); layout in include/tfcb200.h
+LOC_SCALE_BASES = {"normal": 0, "logistic": 1, "laplace": 2}
+
+
+def _contiguous_f32(t):
+  assert t.is_cuda and t.dtype == torch.float32, "the fused log-likelihood takes float32 CUDA tensors"
+  return t.contiguous()
+
+
+class _NoisyDeepFactorizedLogProb(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, y, packed):
+    y, packed = _contiguous_f32(y), _contiguous_f32(packed)
+    ctx.save_for_backward(y, packed)
+    out = torch.empty_like(y)
+    check(_lib.lib().tfcb_noisy_deep_factorized_log_prob(_p(y), _p(packed), _p(out), y.numel(), packed.shape[0],
+                                                         _stream()))
+    return out
+
+  @staticmethod
+  @torch.autograd.function.once_differentiable
+  def backward(ctx, dout):
+    y, packed = ctx.saved_tensors
+    dout = dout.to(torch.float32).contiguous()
+    n, C_ = y.numel(), packed.shape[0]
+    dy = torch.empty_like(y)
+    dpacked = torch.empty_like(packed)
+    L = _lib.lib()
+    ws = torch.empty(max(int(L.tfcb_noisy_deep_factorized_workspace_bytes(n, C_)), 1), dtype=torch.uint8,
+                     device=y.device)
+    check(L.tfcb_noisy_deep_factorized_log_prob_backward(_p(y), _p(packed), _p(dout), _p(dy), _p(dpacked), _p(ws), n,
+                                                         C_, _stream()))
+    return dy, dpacked
+
+
+def noisy_deep_factorized_log_prob(y, packed):
+  """log p(y) of NoisyDeepFactorized with num_filters (3, 3), differentiable in `y` and `packed`.  y: float32 CUDA,
+  channel of element i = i mod C (trailing dimensions = the prior's batch shape); packed: float32 [C, 28], the
+  transformed parameters (DeepFactorized._packed_parameters)."""
+  assert packed.dim() == 2 and packed.shape[1] == DEEP_FACTORIZED_PARAMS
+  return _NoisyDeepFactorizedLogProb.apply(y, packed)
+
+
+class _NoisyLocScaleLogProb(torch.autograd.Function):
+  """loc / scale are either y-shaped or 0-d (one value for every element)."""
+
+  @staticmethod
+  def forward(ctx, base, y, loc, scale):
+    y, loc, scale = _contiguous_f32(y), _contiguous_f32(loc), _contiguous_f32(scale)
+    ctx.save_for_backward(y, loc, scale)
+    ctx.base = base
+    out = torch.empty_like(y)
+    check(_lib.lib().tfcb_noisy_loc_scale_log_prob(base, _p(y), _p(loc), int(loc.dim() == 0), _p(scale),
+                                                   int(scale.dim() == 0), _p(out), y.numel(), _stream()))
+    return out
+
+  @staticmethod
+  @torch.autograd.function.once_differentiable
+  def backward(ctx, dout):
+    y, loc, scale = ctx.saved_tensors
+    dout = dout.to(torch.float32).contiguous()
+    dy = torch.empty_like(y)
+    want_loc, want_scale = ctx.needs_input_grad[2], ctx.needs_input_grad[3]
+    dloc = torch.empty_like(y) if want_loc else None
+    dscale = torch.empty_like(y) if want_scale else None
+    check(_lib.lib().tfcb_noisy_loc_scale_log_prob_backward(
+        ctx.base, _p(y), _p(loc), int(loc.dim() == 0), _p(scale), int(scale.dim() == 0), _p(dout), _p(dy), _p(dloc),
+        _p(dscale), y.numel(), _stream()))
+
+    def reduce(d, operand):  # a 0-d operand of a larger y: the elementwise terms summed in double
+      if d is None or operand.dim() == y.dim():
+        return d
+      return d.double().sum().to(torch.float32)
+
+    return None, dy, reduce(dloc, loc), reduce(dscale, scale)
+
+
+def _scalar_or_full(t, shape):
+  """A y-shaped operand as the fused kernel takes it: the 0-d value behind a broadcast scalar (every stride 0; its
+  gradient reaches the original through the indexing), else the tensor itself."""
+  if t.dim() and t.numel() and all(s == 0 for s in t.stride()):
+    return t[(0,) * t.dim()]
+  assert tuple(t.shape) == tuple(shape)
+  return t
+
+
+def noisy_loc_scale_log_prob(base, y, loc, scale):
+  """log p(y) of NoisyNormal / NoisyLogistic / NoisyLaplace (`base` "normal" / "logistic" / "laplace"),
+  differentiable in y, loc and scale.  y float32 CUDA; loc / scale y-shaped, or broadcast scalars."""
+  return _NoisyLocScaleLogProb.apply(LOC_SCALE_BASES[base], y, _scalar_or_full(loc, y.shape),
+                                     _scalar_or_full(scale, y.shape))
+
+
+# ------------------------------------------------------------------------------------------------
 # Fused quantise + encode / decode + dequantise (K3 fused into K4/K5 and K6)
 # ------------------------------------------------------------------------------------------------
 def _f32(t, device):

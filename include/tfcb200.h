@@ -303,6 +303,43 @@ int tfcb_gdn_backward(const float* x_dev, const float* gamma_dev, const float* b
                       void* workspace_dev, int64_t n_pix, int C, int flags, float alpha,
                       float epsilon, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Rate term of training: log p(y) of a prior convolved with U(-1/2, 1/2), forward and backward, fused.
+ * Replaces UniformNoiseAdapter.log_prob (tensorflow_compression/python/distributions/uniform_noise.py:128-151)
+ * and its autograd for the two families the models train with.  Each element is computed in double from float32
+ * inputs and rounded once; the backward is the chain rule of the same expression (NaN and +-inf propagate as in
+ * autograd of the graph).  Zero-size input does nothing (the parameter gradient is zeroed).
+ *
+ * Deep factorized, num_filters (3, 3) (deep_factorized.py:166-193): y float32 [n], element i in channel i mod C.
+ * `packed_dev` float32 [C, 28], already transformed, per channel:
+ *   softplus(matrices[0]) [3,1], softplus(matrices[1]) [3,3], softplus(matrices[2]) [1,3]  (row-major [out][in]),
+ *   biases[0] [3], biases[1] [3], biases[2] [1], tanh(factors[0]) [3], tanh(factors[1]) [3].
+ * The backward writes dy [n] and OVERWRITES dpacked [C, 28] with the gradient summed over all elements, in a fixed
+ * order (bitwise reproducible); `workspace_dev` holds tfcb_noisy_deep_factorized_workspace_bytes(n, C) bytes.
+ * Checked before any device work (TFCB_INVALID_ARGUMENT): C > 0, n >= 0, n mod C == 0, non-null pointers.
+ * ---------------------------------------------------------------------------------------------- */
+int tfcb_noisy_deep_factorized_log_prob(const float* y_dev, const float* packed_dev, float* out_dev, int64_t n,
+                                        int C, void* stream);
+int64_t tfcb_noisy_deep_factorized_workspace_bytes(int64_t n, int C);
+int tfcb_noisy_deep_factorized_log_prob_backward(const float* y_dev, const float* packed_dev, const float* dout_dev,
+                                                 float* dy_dev, float* dpacked_dev, void* workspace_dev, int64_t n,
+                                                 int C, void* stream);
+
+/* Location-scale bases: z = (y +- 1/2 - loc) / scale and the standard log-CDF of `base` (log_ndtr, log-sigmoid, or
+ * the two-branch Laplace form).  y float32 [n]; loc / scale float32 [n], or one value read at [0] for every
+ * element when `loc_scalar` / `scale_scalar` is nonzero.  The backward writes dy [n] and, where the pointer is not
+ * NULL, the elementwise dloc [n] and dscale [n] (the caller sums them for a scalar operand).  Checked before any
+ * device work (TFCB_INVALID_ARGUMENT): a known base, n >= 0, non-null y, loc, scale, out / dout, dy. */
+#define TFCB_NOISY_NORMAL 0
+#define TFCB_NOISY_LOGISTIC 1
+#define TFCB_NOISY_LAPLACE 2
+int tfcb_noisy_loc_scale_log_prob(int base, const float* y_dev, const float* loc_dev, int loc_scalar,
+                                  const float* scale_dev, int scale_scalar, float* out_dev, int64_t n, void* stream);
+int tfcb_noisy_loc_scale_log_prob_backward(int base, const float* y_dev, const float* loc_dev, int loc_scalar,
+                                           const float* scale_dev, int scale_scalar, const float* dout_dev,
+                                           float* dy_dev, float* dloc_dev, float* dscale_dev, int64_t n,
+                                           void* stream);
+
 /* Number of kernel launches issued by this library since load (bench.py's `gpu_launches`). */
 /* Gradients of the loss with respect to the scalar exponents alpha and epsilon (gdn.py:345-367 makes them
  * trainable GDNParameters; TF autodiff differentiates through pow): dalpha_depsilon_dev float32 [2].
