@@ -19,7 +19,11 @@
 // memory (double-buffered, the next chunk is staged while the tensor cores work on the current one) and accumulates
 // one [64 x C] slice of dgamma per warpgroup.
 //
-// Everything outside {C in {128, 192}, alpha in {1, 2}, eps in {1, 0.5}} falls back to the fp32 kernels in gdn.cu.
+// C = 256 and 320 do not fit that layout (shared memory, registers) and split the work over blocks of output columns
+// instead: see "Wide layers" below.
+//
+// Everything outside {C in {128, 192, 256, 320}, alpha in {1, 2}, eps in {1, 0.5}} falls back to the fp32 kernels in
+// gdn.cu.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -492,6 +496,334 @@ gdn_tc_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, f
   }
 }
 
+// ---- Wide layers, C in {256, 320}: the work is split over blocks of NB output columns ----
+//
+// At C > 192 neither gamma's planes (4 C^2 bytes: 256 / 400 KB) nor a warpgroup's A fragments of all K = C plus the
+// accumulators of all C columns fit, so each CTA owns one block of NB channels:
+//   forward / backward pass 1   columns [c0, c0 + NB):  planes of gamma[:, block], acc = pool(x) . gamma[:, block]
+//   backward pass 2             rows J = [j0, j0 + NB):  planes of gamma[J, :],     dp[:, J] = q . gamma[J, :]^T
+//   dgamma                      columns [c0, c0 + NB):  p over all C channels, q over the block's NB
+// Pass 2 exists because with columns split over CTAs no CTA holds all of q, which every entry of dp needs.  A CTA's
+// block is blockIdx.x % kBlocks, so the kBlocks CTAs of one group walk the same pixel tiles side by side: x (and q)
+// come from HBM once and are re-read from L2 by the other blocks.
+template <int C>
+struct WideCfg {
+  static constexpr int kNB = C == 256 ? 128 : 64;  // channels per block; accumulators: NB / 2 registers
+  static constexpr int kBlocks = C / kNB;
+  static constexpr int kKSlices = C == 320 ? 2 : 1;  // A fragments held at once: C / 16 / kKSlices k-steps
+  static constexpr int kWG = 2;
+  static constexpr int kThreads = 128 * kWG;
+  static constexpr int kSmem = 2 * C * kNB * 2;  // hi / lo planes of a C x NB (or NB x C) block of gamma
+  static constexpr int kDgPPlane = C * kTileM * 2;  // dgamma: one bf16 plane of p (all channels) ...
+  static constexpr int kDgQPlane = kNB * kTileM * 2;  // ... and of q (the block's channels)
+  static constexpr int kDgStage = 2 * kDgPPlane + 2 * kDgQPlane;  // p hi, p lo, q hi, q lo
+  static constexpr int kDgSmem = 2 * kDgStage;
+  static_assert(C % kNB == 0 && kNB % 64 == 0, "column blocks of whole wgmma N = 64 tiles");
+  static_assert(kSmem <= 232448 && kDgSmem <= 232448, "shared memory budget");
+};
+
+// gamma rows [j0, j0 + NJ) x columns [i0, i0 + NI) -> hi / lo bf16 planes [j / 8][i][j % 8] (block-local j, i) at
+// smem, smem + NJ * NI * 2: fill_planes restricted to one block.
+template <int C, int NJ, int NI>
+__device__ __forceinline__ void fill_planes_block(const float* __restrict__ gamma, int j0, int i0, uint8_t* smem) {
+  for (int idx = threadIdx.x; idx < (NJ / 8) * NI; idx += blockDim.x) {
+    const int jc = idx / NI, i = idx % NI;
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = __ldg(gamma + (j0 + jc * 8 + e) * C + i0 + i);
+    uint4 hi, lo;
+    split8(v, &hi, &lo);
+    reinterpret_cast<uint4*>(smem)[idx] = hi;
+    reinterpret_cast<uint4*>(smem + NJ * NI * 2)[idx] = lo;
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+}
+
+// A fragments of channels [16 k0, 16 k0 + KA) of a tile of a [n_pix, C] array, at the positions pool_frags uses:
+// pool(x) (POOL) or the values themselves (q).
+template <int C, int KA, bool POOL, bool FAST>
+__device__ __forceinline__ void slice_frags(const float* __restrict__ src, long long r0, long long r1, bool ok0,
+                                            bool ok1, int t, int k0, const TcFlags& f, uint32_t (&ah)[KA / 16][4],
+                                            uint32_t (&al)[KA / 16][4]) {
+#pragma unroll
+  for (int kk = 0; kk < KA / 16; ++kk) {
+    const int c = 16 * (k0 + kk) + 2 * t;
+    const float2 z = make_float2(0.f, 0.f);
+    const float2 v[4] = {ok0 ? ld_pair<0>(src, r0 * C + c) : z, ok1 ? ld_pair<0>(src, r1 * C + c) : z,
+                         ok0 ? ld_pair<0>(src, r0 * C + c + 8) : z, ok1 ? ld_pair<0>(src, r1 * C + c + 8) : z};
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      if (POOL)
+        split2(tc_pool<FAST>(v[r].x, f), tc_pool<FAST>(v[r].y, f), &ah[kk][r], &al[kk][r]);
+      else
+        split2(v[r].x, v[r].y, &ah[kk][r], &al[kk][r]);
+    }
+  }
+}
+
+// acc[64 x NB] = A . B for one 64-pixel tile, K = C, A = split(pool(x)) (POOL) or split(q) from `src`, B = hi + lo
+// planes at bh, bl laid out by fill_planes_block:
+//   TB = 0: B = gamma[:, block]    (k = j, n = i; planes C x NB)
+//   TB = 1: B = gamma[J, :]^T      (k = i, n = j; planes NB x C)
+// K is walked in kKSlices slices, each loaded into registers, multiplied and waited for before the next is loaded:
+// at C = 320 the A fragments of all K (160 registers) next to the accumulators leave ptxas too few registers to
+// avoid spills.  Otherwise gemm3 with the plane extents of one block.
+template <int C, int TB, bool POOL, bool FAST>
+__device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32], const float* __restrict__ src,
+                                          long long r0, long long r1, bool ok0, bool ok1, int t, const TcFlags& f,
+                                          uint32_t bh, uint32_t bl) {
+  constexpr int NB = WideCfg<C>::kNB, KA = C / WideCfg<C>::kKSlices;
+#pragma unroll
+  for (int n = 0; n < NB / 64; ++n)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[n][i] = 0.f;
+  // K-major: core matrix (k / 8, n / 8) at (k / 8) * NB * 16 + (n / 8) * 128 bytes; MN-major: at
+  // (n / 8) * C * 16 + (k / 8) * 128.
+  constexpr uint32_t kLbo = TB ? 128 : NB * 16, kSbo = TB ? C * 16 : 128;
+#pragma unroll
+  for (int s = 0; s < WideCfg<C>::kKSlices; ++s) {
+    uint32_t ah[KA / 16][4], al[KA / 16][4];
+    slice_frags<C, KA, POOL, FAST>(src, r0, r1, ok0, ok1, t, s * KA / 16, f, ah, al);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KA / 16; ++kk)
+#pragma unroll
+      for (int n = 0; n < NB / 64; ++n) {
+        const uint32_t k = s * KA / 16 + kk;
+        const uint32_t off = TB ? (256u * k + (uint32_t)n * C * 128) : (k * NB * 32 + 1024u * n);
+        wgmma_rs<TB>(acc[n], ah[kk], gmma_desc(bh + off, kLbo, kSbo));
+        wgmma_rs<TB>(acc[n], al[kk], gmma_desc(bh + off, kLbo, kSbo));
+        wgmma_rs<TB>(acc[n], ah[kk], gmma_desc(bl + off, kLbo, kSbo));
+      }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_acc(acc);
+  }
+}
+
+template <int C, bool FAST>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                       float* __restrict__ y, long long n_pix, TcFlags f) {
+  using W = WideCfg<C>;
+  constexpr int NB = W::kNB;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int c0 = (int)(blockIdx.x % W::kBlocks) * NB;
+  fill_planes_block<C, C, NB>(gamma, 0, c0, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * NB * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const long long stride = (long long)(gridDim.x / W::kBlocks) * W::kWG;
+  for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    float acc[NB / 64][32];
+    wide_gemm<C, 0, true, FAST>(acc, x, r0, r1, ok0, ok1, t, f, bh, bl);
+    TFCB_FOR_ACC_PAIRS(NB) {
+      const bool ok = h ? ok1 : ok0;
+      const int col = c0 + 64 * n + 8 * jj + 2 * t;
+      const long long idx = (h ? r1 : r0) * C + col;
+      const float2 xv = ok ? ld_pair<0>(x, idx) : make_float2(0.f, 0.f);
+      const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
+      const float y0 = tc_out<FAST>(xv.x, b.x + acc[n][4 * jj + 2 * h], f);
+      const float y1 = tc_out<FAST>(xv.y, b.y + acc[n][4 * jj + 2 * h + 1], f);
+      if (ok) st_pair<0>(y, idx, y0, y1);
+    }
+  }
+}
+
+// Backward, pass 1: n[:, block] = beta + p . gamma[:, block]  ->  q[:, block] (workspace), dx[:, block] = direct term.
+template <int C, bool FAST>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                         const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws,
+                         long long n_pix, TcFlags f) {
+  using W = WideCfg<C>;
+  constexpr int NB = W::kNB;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int c0 = (int)(blockIdx.x % W::kBlocks) * NB;
+  fill_planes_block<C, C, NB>(gamma, 0, c0, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * NB * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const long long stride = (long long)(gridDim.x / W::kBlocks) * W::kWG;
+  for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    float acc[NB / 64][32];
+    wide_gemm<C, 0, true, FAST>(acc, x, r0, r1, ok0, ok1, t, f, bh, bl);
+    TFCB_FOR_ACC_PAIRS(NB) {
+      const bool ok = h ? ok1 : ok0;
+      const int col = c0 + 64 * n + 8 * jj + 2 * t;
+      const long long idx = (h ? r1 : r0) * C + col;
+      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
+      const float2 gv = ok ? __ldg(reinterpret_cast<const float2*>(dy + idx)) : make_float2(0.f, 0.f);
+      const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
+      float2 qv, d;
+      tc_bwd_point<FAST>(xv.x, gv.x, b.x + acc[n][4 * jj + 2 * h], f, &qv.x, &d.x);
+      tc_bwd_point<FAST>(xv.y, gv.y, b.y + acc[n][4 * jj + 2 * h + 1], f, &qv.y, &d.y);
+      if (ok) {
+        *reinterpret_cast<float2*>(q_ws + idx) = qv;
+        *reinterpret_cast<float2*>(dx + idx) = d;
+      }
+    }
+  }
+}
+
+// Backward, pass 2: dp[:, J] = q . gamma[J, :]^T  ->  dx[:, J] += dpool/dx * dp, then the rectifier's mask.
+template <int C, bool FAST>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ q,
+                          float* __restrict__ dx, long long n_pix, TcFlags f) {
+  using W = WideCfg<C>;
+  constexpr int NB = W::kNB;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int j0 = (int)(blockIdx.x % W::kBlocks) * NB;
+  fill_planes_block<C, NB, C>(gamma, j0, 0, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * NB * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const long long stride = (long long)(gridDim.x / W::kBlocks) * W::kWG;
+  for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    float acc[NB / 64][32];
+    wide_gemm<C, 1, false, FAST>(acc, q, r0, r1, ok0, ok1, t, f, bh, bl);
+    TFCB_FOR_ACC_PAIRS(NB) {
+      const bool ok = h ? ok1 : ok0;
+      const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
+      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
+      float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
+      d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
+      d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
+      if (!FAST && f.rectify) {
+        if (!(xv.x > 0.f)) d.x = 0.f;
+        if (!(xv.y > 0.f)) d.y = 0.f;
+      }
+      if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+    }
+  }
+}
+
+// dgamma[:, block] and dbeta[block]: gdn_tc_dgamma_kernel with q staged for the block's NB channels only.  CTA
+// (part, block) adds into columns [c0, c0 + NB) of partial `part`, so the partials keep the [n_parts][C][C] layout.
+// Thread tid stages p channels 8 (tid / 16) .. + 7 of pixels tid % 16 + 16 s, and the same q channels of the block
+// when tid / 16 < NB / 8.
+template <int C, bool FAST>
+__global__ void __launch_bounds__(2 * C, 1)
+gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                          float* __restrict__ part_b, long long n_pix, TcFlags f) {
+  using W = WideCfg<C>;
+  constexpr int NB = W::kNB;
+  constexpr int kP = W::kDgPPlane, kQ = W::kDgQPlane;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int jc = tid >> 4, pl = tid & 15;
+  const bool has_q = jc < NB / 8;
+  const int c0 = (int)(blockIdx.x % W::kBlocks) * NB;
+  const long long part = blockIdx.x / W::kBlocks, n_parts = gridDim.x / W::kBlocks;
+  const long long n_chunks = (n_pix + kTileM - 1) / kTileM;
+  float bsum[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) bsum[e] = 0.f;
+
+  auto stage = [&](long long chunk, int buf) {
+    uint8_t* base = smem + buf * W::kDgStage;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int p = pl + 16 * s;
+      const long long row = chunk * kTileM + p;
+      float v[8], w[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] = w[e] = 0.f;
+      if (row < n_pix) {
+        const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
+        const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1);
+        v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
+        if (has_q) {
+          const float4* qr = reinterpret_cast<const float4*>(q + row * C + c0 + 8 * jc);
+          const float4 q0 = __ldg(qr), q1 = __ldg(qr + 1);
+          w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[e] = tc_pool<FAST>(v[e], f);
+        bsum[e] += w[e];
+      }
+      const int slot = (jc * kTileM + p) * 16;
+      uint4 hi, lo;
+      split8(v, &hi, &lo);
+      *reinterpret_cast<uint4*>(base + slot) = hi;
+      *reinterpret_cast<uint4*>(base + kP + slot) = lo;
+      if (has_q) {
+        split8(w, &hi, &lo);
+        *reinterpret_cast<uint4*>(base + 2 * kP + slot) = hi;
+        *reinterpret_cast<uint4*>(base + 2 * kP + kQ + slot) = lo;
+      }
+    }
+  };
+
+  float acc[NB / 64][32];
+  float* pg = part_g + part * C * C;
+  bool first_flush = true;
+  stage(part, 0);
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+  int k = 0;
+  for (long long chunk = part; chunk < n_chunks; chunk += n_parts, ++k) {
+    if (k % kDgFlush == 0) {
+#pragma unroll
+      for (int n = 0; n < NB / 64; ++n)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[n][i] = 0.f;
+    }
+    // core matrix (channel / 8, pixel / 8) at (channel / 8) * 1024 + (pixel / 8) * 128 bytes of a plane
+    const uint32_t base = smem_u32(smem + (k & 1) * W::kDgStage);
+    const uint32_t pp[3] = {0, kP, 0}, qp[3] = {2 * kP, 2 * kP, 2 * kP + kQ};  // hi.hi, lo.hi, hi.lo
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kTileM / 16; ++kk)
+#pragma unroll
+      for (int pr = 0; pr < 3; ++pr) {
+        const uint64_t a = gmma_desc(base + pp[pr] + wg * 8 * 1024 + 256 * kk, 128, 1024);
+#pragma unroll
+        for (int n = 0; n < NB / 64; ++n)
+          wgmma_ss_mn(acc[n], a, gmma_desc(base + qp[pr] + n * 8 * 1024 + 256 * kk, 128, 1024));
+      }
+    wgmma_commit();
+    const bool last = chunk + n_parts >= n_chunks;
+    if (!last) stage(chunk + n_parts, (k + 1) & 1);
+    wgmma_wait_all();
+    fence_acc(acc);
+    if ((k + 1) % kDgFlush == 0 || last) {
+      TFCB_FOR_ACC_PAIRS(NB) {
+        float2* dst =
+            reinterpret_cast<float2*>(pg + (64 * wg + 16 * warp + g + 8 * h) * C + c0 + 64 * n + 8 * jj + 2 * t);
+        float2 v = make_float2(acc[n][4 * jj + 2 * h], acc[n][4 * jj + 2 * h + 1]);
+        if (!first_flush) {
+          const float2 o = *dst;
+          v.x += o.x;
+          v.y += o.y;
+        }
+        *dst = v;
+      }
+      first_flush = false;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e)
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) bsum[e] += __shfl_xor_sync(0xFFFFFFFFu, bsum[e], o);
+  if (has_q && pl == 0) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) part_b[part * C + c0 + 8 * jc + e] = bsum[e];
+  }
+}
+
 int sm_count_tc() {
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
@@ -538,9 +870,52 @@ int launch_tc_bwd(const float* x, const float* gamma, const float* beta, const f
   return TFCB_OK;
 }
 
+// Wide layers: groups of kBlocks CTAs (one per channel block), as many groups as fill the SMs once.
+template <int C>
+int wide_grid(long long n_tiles_per_group) {
+  using W = WideCfg<C>;
+  const long long groups = std::max(1, std::min(sm_count_tc() / W::kBlocks, kMaxParts));
+  return (int)(std::min<long long>(n_tiles_per_group, groups) * W::kBlocks);
+}
+
+template <int C, bool FAST>
+int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, TcFlags f,
+                       cudaStream_t s) {
+  using W = WideCfg<C>;
+  TFCB_TRY(reserve_smem(gdn_tc_wide_fwd_kernel<C, FAST>, W::kSmem));
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
+  gdn_tc_wide_fwd_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+template <int C, bool FAST>
+int launch_tc_wide_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
+                       float* part_g, float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
+  using W = WideCfg<C>;
+  TFCB_TRY(reserve_smem(gdn_tc_wide_bwd_q_kernel<C, FAST>, W::kSmem));
+  TFCB_TRY(reserve_smem(gdn_tc_wide_bwd_dp_kernel<C, FAST>, W::kSmem));
+  TFCB_TRY(reserve_smem(gdn_tc_wide_dgamma_kernel<C, FAST>, W::kDgSmem));
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
+  gdn_tc_wide_bwd_q_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+  TFCB_LAUNCHED();
+  gdn_tc_wide_bwd_dp_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, q_ws, dx, n_pix, f);
+  TFCB_LAUNCHED();
+  // one partial per group of kBlocks CTAs (at most sms / kBlocks <= kMaxParts): fixed by n_pix, C and the SM count
+  const int grid_g = wide_grid<C>(n_tiles);
+  gdn_tc_wide_dgamma_kernel<C, FAST><<<grid_g, 2 * C, W::kDgSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  *n_parts = grid_g / W::kBlocks;
+  return TFCB_OK;
+}
+
 // Which configurations have a tensor-core kernel; fills *f.
 bool tc_config(int C, int flags, float alpha, float eps, TcFlags* f) {
-  if (!(C == 128 || C == 192)) return false;
+  if (!(C == 128 || C == 192 || C == 256 || C == 320)) return false;
   if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return false;
   if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return false;  // trainable exponents: literal pow
   if (const char* env = getenv("TFCB_GDN_FP32")) {
@@ -568,6 +943,12 @@ int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float*
   if (misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
   const bool fast = tc_fast(f);
+  if (C == 256)
+    return fast ? launch_tc_wide_fwd<256, true>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_wide_fwd<256, false>(x, gamma, beta, y, n_pix, f, s);
+  if (C == 320)
+    return fast ? launch_tc_wide_fwd<320, true>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_wide_fwd<320, false>(x, gamma, beta, y, n_pix, f, s);
   if (C == 128)
     return fast ? launch_tc_fwd<128, true, 0>(x, gamma, beta, y, n_pix, f, s)
                 : launch_tc_fwd<128, false, 0>(x, gamma, beta, y, n_pix, f, s);
@@ -602,6 +983,12 @@ int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const
   if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
   const bool fast = tc_fast(f);
+  if (C == 256)
+    return fast ? launch_tc_wide_bwd<256, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
+                : launch_tc_wide_bwd<256, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
+  if (C == 320)
+    return fast ? launch_tc_wide_bwd<320, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
+                : launch_tc_wide_bwd<320, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
   if (C == 128)
     return fast ? launch_tc_bwd<128, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
                 : launch_tc_bwd<128, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
