@@ -32,7 +32,7 @@ def build(verbose: bool = False) -> str:
 
 
 _p = C.POINTER
-_vp, _i64, _i32, _int, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_int, C.c_float
+_vp, _i64, _i32, _u32, _int, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_int, C.c_float
 
 # name -> (restype, argtypes).  Mirrors include/tfcb200.h one to one; tests/test_abi.py checks that
 # every prototype in the header is listed here and exported by the shared object.
@@ -86,6 +86,9 @@ SIGNATURES = {
     "tfcb_noisy_loc_scale_log_prob": (_int, [_int, _vp, _vp, _int, _vp, _int, _vp, _i64, _vp]),
     "tfcb_noisy_loc_scale_log_prob_backward": (_int, [_int, _vp, _vp, _int, _vp, _int, _vp, _vp, _vp, _vp, _i64,
                                                       _vp]),
+    "tfcb_stateless_uniform_int": (_int, [_vp, _i64, _u32, _u32, _i64, _vp]),
+    "tfcb_universal_coding_tensors": (_int, [_i64, _vp, _u32, _u32, _i64, _i64, _vp, _i32, _vp, _i32, _vp, _vp, _i32,
+                                             _vp]),
 }
 
 _lib = None

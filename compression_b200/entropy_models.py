@@ -712,9 +712,12 @@ def stateless_uniform_int(shape, seed, maxval, device=None):
   element i is word i % 4 of Philox-4x32-10(counter = i // 4, key = seed), reduced modulo `maxval`.  It depends on
   nothing but (seed, i), so sender and receiver -- on any device -- draw the same noise levels.  TensorFlow's own
   key / counter conventions are not reproduced (there is no TF here to pin them against): strings written with
-  universal quantisation decode with THIS implementation, not with the reference's."""
+  universal quantisation decode with THIS implementation, not with the reference's.  On a CUDA device the draw is one
+  kernel (functional.stateless_uniform_int); on the CPU it is the int64 torch arithmetic of _philox4x32."""
   shape = tuple(int(d) for d in shape)
   n = gen_ops._prod(shape)
+  if device is not None and torch.device(device).type == "cuda":
+    return F.stateless_uniform_int(n, seed, maxval, device).reshape(shape)
   blocks = (n + 3) // 4
   counter = torch.zeros(blocks, 4, dtype=torch.int64, device=device)
   idx = torch.arange(blocks, dtype=torch.int64, device=device)
@@ -724,9 +727,12 @@ def stateless_uniform_int(shape, seed, maxval, device=None):
   return (words % int(maxval)).to(torch.int32).reshape(shape)
 
 
+_NOISE_SEED = (1234, 1234)  # universal.py:33-39
+
+
 def _add_offset_indexes(indexes, num_noise_levels):
   """universal.py:30-42: prepends the shared pseudo-random noise-level index to the last axis of `indexes`."""
-  offset_indexes = stateless_uniform_int(indexes.shape[:-1], (1234, 1234), num_noise_levels, indexes.device)
+  offset_indexes = stateless_uniform_int(indexes.shape[:-1], _NOISE_SEED, num_noise_levels, indexes.device)
   return torch.cat((offset_indexes.to(indexes.dtype)[..., None], indexes), dim=-1)
 
 
@@ -739,6 +745,16 @@ def _range_coding_offsets(num_noise_levels, prior_rank, dtype):
   """universal.py:55-62."""
   offset_indexes = torch.arange(num_noise_levels, dtype=dtype).reshape([-1] + [1] * prior_rank)
   return _offset_indexes_to_offset(offset_indexes, num_noise_levels, dtype)
+
+
+def _on_cuda(device):
+  return torch.device(device).type == "cuda"
+
+
+def _kernel_offset_dtype(bottleneck_dtype):
+  """The coding-tensor kernel writes float32 offsets for float32 bottlenecks (the fused coder's type) and float64
+  for every other type, which torch then casts as _offset_indexes_to_offset does."""
+  return torch.float32 if bottleneck_dtype == torch.float32 else torch.float64
 
 
 class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
@@ -767,9 +783,32 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
   def prior_shape_tensor(self):
     return torch.tensor(self.prior_shape, dtype=torch.int32)
 
+  def _item_coding_tensors(self, lengths, device):
+    """Flat table index and offset (in bottleneck_dtype) of items of `lengths` elements, one after the other, from
+    one kernel launch; the noise position restarts in every item, as in a compress of that item alone."""
+    flat, offset = F.universal_coding_tensors(lengths, self._num_noise_levels,
+                                              _kernel_offset_dtype(self.bottleneck_dtype), device,
+                                              prior_size=gen_ops._prod(self.prior_shape), seed=_NOISE_SEED)
+    return flat, offset.to(self.bottleneck_dtype)
+
+  def _unit_coding_tensors(self, units, broadcast_shape, device):
+    """Table index and offset of `units` coding units of shape broadcast_shape + prior_shape, shaped
+    (units,) + that shape.  A CUDA device writes every unit directly; the CPU broadcasts one unit."""
+    full_shape = tuple(broadcast_shape) + self.prior_shape
+    if units > 0 and _on_cuda(device):
+      flat, offset = self._item_coding_tensors([gen_ops._prod(full_shape)] * units, device)
+      return flat.reshape((units,) + full_shape), offset.reshape((units,) + full_shape)
+    indexes, offset = self._compute_indexes_and_offset(broadcast_shape, device)
+    return (torch.broadcast_to(indexes, (units,) + full_shape).contiguous(),
+            torch.broadcast_to(offset, (units,) + full_shape).contiguous())
+
   def _compute_indexes_and_offset(self, broadcast_shape, device):
-    """universal.py:147-170 -> (flat table index, quantisation offset), both of shape broadcast_shape + prior_shape."""
+    """universal.py:147-170 -> (flat table index, quantisation offset), both of shape broadcast_shape + prior_shape.
+    One kernel launch on a CUDA device, torch operations on the CPU."""
     broadcast_shape = tuple(int(d) for d in broadcast_shape)
+    if _on_cuda(device):
+      flat, offset = self._item_coding_tensors([gen_ops._prod(broadcast_shape + self.prior_shape)], device)
+      return flat.reshape(broadcast_shape + self.prior_shape), offset.reshape(broadcast_shape + self.prior_shape)
     prior_size = gen_ops._prod(self.prior_shape)
     indexes = torch.arange(prior_size, dtype=torch.int32, device=device)
     indexes = torch.broadcast_to(indexes, broadcast_shape + (prior_size,))[..., None]
@@ -802,9 +841,13 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
     shape = tuple(bottleneck.shape)
     batch_shape, coding_shape = shape[:len(shape) - self.coding_rank], shape[len(shape) - self.coding_rank:]
     broadcast_shape = coding_shape[:self.coding_rank - len(self.prior_shape)]
-    indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
-    indexes = torch.broadcast_to(indexes, shape).contiguous()
-    offset = torch.broadcast_to(offset, shape).contiguous()
+    if coding_shape == broadcast_shape + self.prior_shape:  # (else prior dimensions of size 1 are broadcast)
+      indexes, offset = self._unit_coding_tensors(gen_ops._prod(batch_shape), broadcast_shape, dev)
+      indexes, offset = indexes.reshape(shape), offset.reshape(shape)
+    else:
+      indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
+      indexes = torch.broadcast_to(indexes, shape).contiguous()
+      offset = torch.broadcast_to(offset, shape).contiguous()
     return self._encode(batch_shape, bottleneck, offset, self.cdf_offset.to(dev), indexes, fused)
 
   def decompress(self, strings, broadcast_shape, fused=True):
@@ -815,10 +858,42 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
     broadcast_shape = tuple(int(d) for d in np.asarray(broadcast_shape).reshape(-1))
     decode_shape = broadcast_shape + self.prior_shape
     output_shape = tuple(strings.shape) + decode_shape
-    indexes, offset = self._compute_indexes_and_offset(broadcast_shape, dev)
-    indexes = torch.broadcast_to(indexes, output_shape).contiguous()
-    offset = torch.broadcast_to(offset, output_shape).contiguous()
+    indexes, offset = self._unit_coding_tensors(gen_ops._prod(strings.shape), broadcast_shape, dev)
+    indexes, offset = indexes.reshape(output_shape), offset.reshape(output_shape)
     return self._decode(strings, decode_shape, offset, self.cdf_offset.to(dev), indexes, fused)
+
+  # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
+  def compress_ragged(self, bottlenecks, return_decoded=False):
+    """Compresses a list of coding units of different shapes in one range-coder launch.  Each item has exactly
+    `coding_rank` dimensions ending in `prior_shape` (no broadcasting).  Returns a Strings of shape (k,) whose string
+    i equals `compress(bottlenecks[i])`: the noise levels of item i are drawn over its own positions.
+
+    `return_decoded=True` returns `(strings, items)` with `items` equal, bit for bit, to
+    `decompress_ragged(strings, ...)`: written by the encoder itself for a float32 bottleneck, decoded from the
+    fresh strings otherwise."""
+    self._check_compression()
+    dev = _cuda()
+    items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
+    rank_p = len(self.prior_shape)
+    for b in items:
+      if b.dim() != self.coding_rank or (rank_p and tuple(b.shape[-rank_p:]) != self.prior_shape):
+        raise ValueError(f"each item needs {self.coding_rank} dimensions ending in {self.prior_shape}: "
+                         f"received shape {tuple(b.shape)}")
+    if not items:
+      raise ValueError("`bottlenecks` is empty")
+    indexes, offset = self._item_coding_tensors([b.numel() for b in items], dev)
+    return self._encode_ragged([tuple(b.shape) for b in items], torch.cat([b.reshape(-1) for b in items]), offset,
+                               self.cdf_offset.to(dev), indexes, return_decoded)
+
+  def decompress_ragged(self, strings, broadcast_shapes):
+    """Inverse of compress_ragged: item i has shape `broadcast_shapes[i] + prior_shape` and equals
+    `decompress(strings[i:i+1], broadcast_shapes[i])[0]`.  The items are views into one allocation."""
+    self._check_compression()
+    shapes = [tuple(int(d) for d in np.asarray(s).reshape(-1)) + self.prior_shape for s in broadcast_shapes]
+    strings = self._strings(strings, len(shapes))
+    dev = strings.bytes_dev.device
+    indexes, offset = self._item_coding_tensors([gen_ops._prod(s) for s in shapes], dev)
+    return self._decode_ragged(strings, shapes, offset, self.cdf_offset.to(dev), indexes)
 
   def get_config(self):
     raise NotImplementedError()
@@ -897,16 +972,64 @@ class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
                                                         expected_grads=self.expected_grads)
     else:
       prior = self._make_prior(indexes)
-      offset = self._offset_from_indexes(_add_offset_indexes(indexes, self._num_noise_levels))
+      if self._kernel_path(indexes.device):
+        offset = self._coding_tensors(indexes.detach(), indexes.device)[1]
+      else:
+        offset = self._offset_from_indexes(_add_offset_indexes(indexes, self._num_noise_levels))
       perturbed = torch.round(bottleneck - offset) + offset
       log_probs = self._log_prob(prior, perturbed)
     axes = tuple(range(-self.coding_rank, 0))
     return perturbed, log_probs.sum(dim=axes) / -math.log(2.)
 
+  def _kernel_path(self, device):
+    """Whether the coding tensors come from the CUDA kernel: on a CUDA device with a float32 / float64 `prior_dtype`.
+    16-bit index types keep the torch operations (whose noise draw is still the kernel's on a CUDA device)."""
+    return _on_cuda(device) and self.prior_dtype in F.UNIVERSAL_INDEX_DTYPES
+
+  def _check_index_shape(self, indexes):
+    num = len(self.index_ranges_without_offsets)
+    if indexes.dim() == 0 or indexes.shape[-1] != num:
+      raise ValueError(f"`indexes` needs a last dimension of {num} (one per index range): received shape "
+                       f"{tuple(indexes.shape)}")
+
+  def _kernel_coding_tensors(self, lengths, indexes, dev):
+    flat, offset = F.universal_coding_tensors(lengths, self._num_noise_levels,
+                                              _kernel_offset_dtype(self.bottleneck_dtype), dev, indexes=indexes,
+                                              index_ranges=self.index_ranges_without_offsets, seed=_NOISE_SEED)
+    return flat, offset.to(self.bottleneck_dtype)
+
   def _coding_tensors(self, indexes, dev):
+    """universal.py:530-598: (flat table index, offset in bottleneck_dtype), both of shape indexes.shape[:-1].  The
+    noise is drawn over every position of that shape, batch dimensions included."""
     indexes = torch.as_tensor(indexes).to(device=dev, dtype=self.prior_dtype)
+    if self._kernel_path(dev):
+      self._check_index_shape(indexes)
+      shape = tuple(indexes.shape[:-1])
+      flat, offset = self._kernel_coding_tensors([gen_ops._prod(shape)], indexes, dev)
+      return flat.reshape(shape), offset.reshape(shape)
     indexes = self._normalize_indexes(_add_offset_indexes(indexes, self._num_noise_levels))
     return self._flatten_indexes(indexes).contiguous(), self._offset_from_indexes(indexes).contiguous()
+
+  def _ragged_coding_tensors(self, indexes, dev):
+    """Flat table indexes and offsets of every item, concatenated (the noise position restarting in every item), and
+    the items' coding shapes."""
+    indexes = [torch.as_tensor(i).to(device=dev, dtype=self.prior_dtype) for i in indexes]
+    if not indexes:
+      raise ValueError("`indexes` is empty")
+    for i in indexes:
+      self._check_index_shape(i)
+    shapes = [tuple(i.shape[:-1]) for i in indexes]
+    for s in shapes:
+      if len(s) != self.coding_rank:
+        raise ValueError(f"each item needs {self.coding_rank} dimensions: received indexes for shape {s}")
+    if self._kernel_path(dev):
+      flat, offset = self._kernel_coding_tensors([gen_ops._prod(s) for s in shapes],
+                                                 torch.cat([i.reshape(-1) for i in indexes]), dev)
+    else:
+      parts = [self._coding_tensors(i, dev) for i in indexes]
+      flat = torch.cat([p[0].reshape(-1) for p in parts])
+      offset = torch.cat([p[1].reshape(-1) for p in parts])
+    return flat, offset, shapes
 
   def compress(self, bottleneck, indexes, fused=True):
     """universal.py:530-566."""
@@ -927,6 +1050,34 @@ class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
     fshape = tuple(flat.shape)
     return self._decode(strings, fshape[len(fshape) - self.coding_rank:], offset, self.cdf_offset.to(dev), flat,
                         fused)
+
+  # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
+  def compress_ragged(self, bottlenecks, indexes, return_decoded=False):
+    """Compresses a list of coding units of different shapes (each with exactly `coding_rank` dimensions) in one
+    range-coder launch.  Returns a Strings of shape (k,) whose string i equals `compress(bottlenecks[i],
+    indexes[i])`.  The noise levels of item i are drawn over its own positions, so the strings differ from those of
+    one `compress` of the items stacked into a batch, which draws them over the batch dimensions too.
+
+    `return_decoded=True` returns `(strings, items)` with `items` equal, bit for bit, to
+    `decompress_ragged(strings, indexes)`: written by the encoder itself for a float32 bottleneck, decoded from the
+    fresh strings otherwise."""
+    self._check_compression()
+    dev = _cuda()
+    items = [torch.as_tensor(b).to(device=dev, dtype=self.bottleneck_dtype) for b in bottlenecks]
+    flat, offset, shapes = self._ragged_coding_tensors(indexes, dev)
+    if len(items) != len(shapes) or any(tuple(b.shape) != s for b, s in zip(items, shapes)):
+      raise ValueError(f"bottleneck shapes {[tuple(b.shape) for b in items]} do not match the indexes' {shapes}")
+    return self._encode_ragged(shapes, torch.cat([b.reshape(-1) for b in items]), offset, self.cdf_offset.to(dev),
+                               flat, return_decoded)
+
+  def decompress_ragged(self, strings, indexes):
+    """Inverse of compress_ragged: item i has the coding shape of `indexes[i]` (without its last dimension).  The
+    items are views into one allocation."""
+    self._check_compression()
+    strings = self._strings(strings, len(indexes))
+    dev = strings.bytes_dev.device
+    flat, offset, shapes = self._ragged_coding_tensors(indexes, dev)
+    return self._decode_ragged(strings, shapes, offset, self.cdf_offset.to(dev), flat)
 
   def get_config(self):
     raise NotImplementedError()

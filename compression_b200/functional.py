@@ -363,6 +363,58 @@ def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=Non
   return out
 
 
+# ------------------------------------------------------------------------------------------------
+# Universal quantisation: shared noise levels and coding tensors (universal.py:30-62,147-170,446-466)
+# ------------------------------------------------------------------------------------------------
+def _seed_words(seed):
+  return int(seed[0]) & 0xFFFFFFFF, int(seed[1]) & 0xFFFFFFFF
+
+
+def stateless_uniform_int(n, seed, maxval, device):
+  """int32 [n]: element i is word i % 4 of Philox-4x32-10(counter = i // 4, key = seed) modulo `maxval`, drawn on
+  the CUDA `device` in one launch (entropy_models.stateless_uniform_int on the CPU gives the same integers)."""
+  maxval = int(maxval)
+  if maxval < 1:
+    raise _lib.InvalidArgumentError(f"`maxval` must be positive: {maxval}")
+  out = torch.empty(int(n), dtype=torch.int32, device=device)
+  check(_lib.lib().tfcb_stateless_uniform_int(_p(out), out.numel(), *_seed_words(seed), min(maxval, 1 << 62),
+                                              _stream()))
+  return out
+
+
+UNIVERSAL_INDEX_DTYPES = (torch.float32, torch.float64)  # index types the coding-tensor kernel reads
+
+
+def universal_coding_tensors(lengths, num_noise_levels, offset_dtype, device, prior_size=None, indexes=None,
+                             index_ranges=None, seed=(1234, 1234)):
+  """Flat int32 table indexes and offsets of items of `lengths` elements, one after the other, in one launch; the
+  noise position restarts in every item.  Batched (`prior_size`): level * prior_size + i % prior_size.  Indexed
+  (`indexes` float32 / float64 [sum(lengths), len(index_ranges)]): the level and the indexes clipped to their ranges
+  and flattened with the strides of (num_noise_levels,) + index_ranges.  The offset (level + 1) / (levels + 1) - 1/2
+  is computed in double and returned as float32 when `offset_dtype` is float32, else as float64."""
+  import numpy as np
+  offs = _symbol_offsets(lengths)
+  n = int(offs[-1])
+  table = torch.empty(n, dtype=torch.int32, device=device)
+  off64 = offset_dtype != torch.float32
+  offset = torch.empty(n, dtype=torch.float64 if off64 else torch.float32, device=device)
+  if indexes is None:
+    idx, is_f64, ranges, n_ranges, prior_size = None, 0, None, 0, int(prior_size)
+  else:
+    if indexes.dtype not in UNIVERSAL_INDEX_DTYPES:
+      raise _lib.InvalidArgumentError(f"indexes of type {indexes.dtype}: the kernel reads float32 or float64")
+    ranges = np.ascontiguousarray(np.asarray(index_ranges, dtype=np.int64).reshape(-1))
+    idx = indexes.to(device).contiguous()
+    if idx.numel() != n * ranges.size:
+      raise _lib.InvalidArgumentError(f"{n} elements of {ranges.size} indexes each, but `indexes` has {idx.numel()}")
+    is_f64, n_ranges, prior_size = int(idx.dtype == torch.float64), ranges.size, 0
+  check(_lib.lib().tfcb_universal_coding_tensors(
+      offs.size - 1, offs.ctypes.data_as(C.c_void_p), *_seed_words(seed), int(num_noise_levels), prior_size, _p(idx),
+      is_f64, None if ranges is None else ranges.ctypes.data_as(C.c_void_p), n_ranges, _p(table), _p(offset),
+      int(off64), _stream()))
+  return table, offset
+
+
 def run_length_encode_ragged(values, lengths, run_length_code, magnitude_code, use_run_length_for_non_zeros):
   """RunLengthEncode of many strings in one launch: string i codes the next `lengths[i]` elements of the flat int32
   `values`.  Returns a Strings of shape (len(lengths),) whose string i equals gen_ops.run_length_encode of those

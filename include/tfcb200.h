@@ -340,6 +340,34 @@ int tfcb_noisy_loc_scale_log_prob_backward(int base, const float* y_dev, const f
                                            float* dy_dev, float* dloc_dev, float* dscale_dev, int64_t n,
                                            void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Universal quantisation (tensorflow_compression/python/entropy_models/universal.py:30-62,147-170,446-466): the
+ * shared noise levels and the coding tensors of UniversalBatchedEntropyModel / UniversalIndexedEntropyModel.
+ * The level of the element at position i of its item is word (i mod 4) of Philox-4x32-10(counter = {lo32(i/4),
+ * hi32(i/4), 0, 0}, key = {seed0, seed1}) mod the number of levels L, the stream entropy_models.stateless_uniform_int
+ * draws on the CPU.  One launch, asynchronous.
+ *
+ * tfcb_stateless_uniform_int: the levels alone, one item of n elements, as int32 (reduced modulo `maxval` only when
+ * maxval <= 2^32; wrapped to int32 like torch's cast).  Checked (TFCB_INVALID_ARGUMENT): n >= 0, maxval >= 1.
+ *
+ * tfcb_universal_coding_tensors: items split by host `item_offsets_host` [n_items + 1] (checked like
+ * tfcb_compress_ragged's symbol offsets, before any device work); the noise position restarts in every item.  Writes
+ * per element the int32 table index and the offset (level + 1) / (L + 1) - 1/2, computed in double and written as
+ * float32, or as float64 when `offset_is_f64` is nonzero.
+ *   batched (indexes_dev NULL, n_ranges 0): index = level * prior_size + i mod prior_size.
+ *   indexed: indexes_dev [elements, n_ranges] float32 (or float64 when `indexes_is_f64`), 1 <= n_ranges <= 8; the
+ *     coordinates (level, indexes...) are read in that type, clipped to [0, range - 1] (max then min; NaN stays NaN)
+ *     and truncated to int32 (NaN gives 0, as torch's cast on the device), and summed with the int32 strides of
+ *     (L,) + index_ranges_host.  The offset uses the clipped level in that type.
+ * Checked (TFCB_INVALID_ARGUMENT): 1 <= L < 2^31, prior_size >= 1 (batched), positive index ranges, non-null
+ * outputs (and indexes) when there are elements. */
+int tfcb_stateless_uniform_int(int32_t* out_dev, int64_t n, uint32_t seed0, uint32_t seed1, int64_t maxval,
+                               void* stream);
+int tfcb_universal_coding_tensors(int64_t n_items, const int64_t* item_offsets_host, uint32_t seed0, uint32_t seed1,
+                                  int64_t num_noise_levels, int64_t prior_size, const void* indexes_dev,
+                                  int32_t indexes_is_f64, const int64_t* index_ranges_host, int32_t n_ranges,
+                                  int32_t* table_index_dev, void* offset_dev, int32_t offset_is_f64, void* stream);
+
 /* Number of kernel launches issued by this library since load (bench.py's `gpu_launches`). */
 /* Gradients of the loss with respect to the scalar exponents alpha and epsilon (gdn.py:345-367 makes them
  * trainable GDNParameters; TF autodiff differentiates through pow): dalpha_depsilon_dev float32 [2].
