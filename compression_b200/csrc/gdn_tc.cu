@@ -23,11 +23,14 @@
 // instead: see "Wide layers" below.
 //
 // Everything outside {C in {128, 192, 256, 320}, alpha in {1, 2}, eps in {1, 0.5}} falls back to the fp32 kernels in
-// gdn.cu.
+// gdn.cu.  At C = 128 / 192 the forward, dx and dgamma kernels also take float16 / bfloat16 activations (IO = 1, 2):
+// each element is widened exactly on load, the arithmetic is the float32 kernels', and the only rounding to 16 bits
+// is the final store, so the result is the float32 result of the widened inputs rounded once.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -177,13 +180,18 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint4* hi, uint4* lo
 
 // Element type of x / y in memory: 0 float32, 1 float16, 2 bfloat16 (the reference's mixed-precision policy keeps the
 // variables in float32 and the activations in 16 bits, gdn_test.py:200-210; arithmetic is float32 here either way).
-// Pairs of consecutive channels of one pixel; idx is the (even) element index.
+// Pairs of consecutive channels of one pixel; idx is the (even) element index.  Widening is exact, so a 16-bit
+// element enters the arithmetic as the float32 value x.float() would give.
+template <int IO>
+__device__ __forceinline__ float2 widen2(uint32_t w) {
+  if (IO == 2) return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
+  return __half22float2(*reinterpret_cast<const __half2*>(&w));
+}
+
 template <int IO>
 __device__ __forceinline__ float2 ld_pair(const void* base, long long idx) {
   if (IO == 0) return __ldg(reinterpret_cast<const float2*>(static_cast<const float*>(base) + idx));
-  const uint32_t w = __ldg(reinterpret_cast<const unsigned int*>(static_cast<const uint16_t*>(base) + idx));
-  if (IO == 2) return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xFFFF0000u));
-  return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  return widen2<IO>(__ldg(reinterpret_cast<const unsigned int*>(static_cast<const uint16_t*>(base) + idx)));
 }
 
 template <int IO>
@@ -311,24 +319,33 @@ gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, c
 }
 
 // Backward, part 1: per 64-pixel tile
-//   n = beta + p . gamma  ->  q = dL/dn (stored for part 2), dx = direct term (stored)
-//   dp = q . gamma^T      ->  dx += dpool/dx * dp (read back from the same thread's stores, L2 resident).
-template <int C, bool FAST>
+//   n = beta + p . gamma  ->  q = dL/dn (stored for part 2), the direct term of dx (stored)
+//   dp = q . gamma^T      ->  dx = direct term + dpool/dx * dp (the direct term read back from the same thread's
+//                             stores, L2 resident).
+// x, dy and dx are float32 (IO = 0) or 16-bit (IO = 1 float16, 2 bfloat16; q stays float32).  With IO = 0 the direct
+// term is stored in dx itself.  A 16-bit dx would round it before the second term is added, so with IO != 0 it goes
+// to the warpgroup's own 64 x C float32 tile of `scratch` instead, and dx is stored once, rounded once: the result is
+// the float32 kernel's on the widened inputs, rounded to the activation type.  No register can hold it through MMA2
+// (the C = 192 FAST variant is at the 255-register limit) and no shared memory is left beside gamma's planes at C = 192.
+template <int C, bool FAST, int IO>
 __global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
-gdn_tc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                     const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                     TcFlags f) {
+gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
+                     TcFlags f, float* __restrict__ scratch) {
   using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   fill_planes<C>(gamma, smem);
   const uint32_t bh = smem_u32(smem), bl = bh + C * C * 2;
   const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  // IO != 0: this thread's row g, columns 2 t, 2 t + 1 of its warp's 16 rows in the warpgroup's scratch tile (the
+  // accumulator pair (n, jj, h) is at + 8 h C + 64 n + 8 jj: immediate offsets)
+  float* const dtile = scratch + ((long long)(blockIdx.x * K::kWG + wg) * kTileM + warp * 16 + g) * C + 2 * t;
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
     uint32_t ah[C / 16][4], al[C / 16][4];
-    pool_frags<C, FAST, 0>(x, r0, r1, ok0, ok1, t, f, ah, al);
+    pool_frags<C, FAST, IO>(x, r0, r1, ok0, ok1, t, f, ah, al);
     float acc[C / 64][32];
     gemm3<C, 0>(acc, ah, al, bh, bl);
     TFCB_FOR_ACC_PAIRS(C) {
@@ -339,14 +356,17 @@ gdn_tc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ gamm
       }
       const int col = 64 * n + 8 * jj + 2 * t;
       const long long idx = (h ? r1 : r0) * C + col;
-      const float2 xv = __ldg(reinterpret_cast<const float2*>(x + idx));
-      const float2 gv = __ldg(reinterpret_cast<const float2*>(dy + idx));
+      const float2 xv = ld_pair<IO>(x, idx);
+      const float2 gv = ld_pair<IO>(dy, idx);
       const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
       float2 q, d;
       tc_bwd_point<FAST>(xv.x, gv.x, b.x + a[0], f, &q.x, &d.x);
       tc_bwd_point<FAST>(xv.y, gv.y, b.y + a[1], f, &q.y, &d.y);
       *reinterpret_cast<float2*>(q_ws + idx) = q;
-      *reinterpret_cast<float2*>(dx + idx) = d;
+      if constexpr (IO == 0)
+        *reinterpret_cast<float2*>(static_cast<float*>(dx) + idx) = d;
+      else
+        *reinterpret_cast<float2*>(dtile + 8 * h * C + 64 * n + 8 * jj) = d;
       a[0] = q.x;
       a[1] = q.y;
     }
@@ -361,15 +381,19 @@ gdn_tc_bwd_dx_kernel(const float* __restrict__ x, const float* __restrict__ gamm
     TFCB_FOR_ACC_PAIRS(C) {
       if (!(h ? ok1 : ok0)) continue;
       const long long idx = (h ? r1 : r0) * C + 64 * n + 8 * jj + 2 * t;
-      const float2 xv = __ldg(reinterpret_cast<const float2*>(x + idx));
-      float2 d = *reinterpret_cast<const float2*>(dx + idx);
+      const float2 xv = ld_pair<IO>(x, idx);
+      float2 d;
+      if constexpr (IO == 0)
+        d = *reinterpret_cast<const float2*>(static_cast<const float*>(dx) + idx);
+      else
+        d = *reinterpret_cast<const float2*>(dtile + 8 * h * C + 64 * n + 8 * jj);
       d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
       d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
       if (!FAST && f.rectify) {
         if (!(xv.x > 0.f)) d.x = 0.f;
         if (!(xv.y > 0.f)) d.y = 0.f;
       }
-      *reinterpret_cast<float2*>(dx + idx) = d;
+      st_pair<IO>(dx, idx, d.x, d.y);
     }
   }
 }
@@ -392,9 +416,13 @@ struct DgCfg {
 // nearest adds, L2 resident) every kDgFlush chunks and restarted.
 constexpr int kDgFlush = 8;
 
-template <int C, bool FAST>
+// x in float32 (IO = 0) or 16 bits (IO = 1, 2: one 16-byte load of the 8 channels, widened exactly); q is float32.
+template <int IO>
+using IoElem = std::conditional_t<IO == 0, float, uint16_t>;
+
+template <int C, bool FAST, int IO>
 __global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
-gdn_tc_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
                      float* __restrict__ part_b, long long n_pix, TcFlags f) {
   using L = DgCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -413,11 +441,20 @@ gdn_tc_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, f
       const long long row = chunk * kTileM + p;
       float v[8], w[8];
       if (row < n_pix) {
-        const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
-        const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
-        const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1), q0 = __ldg(qr), q1 = __ldg(qr + 1);
-        v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
-        w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+        if constexpr (IO == 0) {
+          const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
+          const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
+          const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1), q0 = __ldg(qr), q1 = __ldg(qr + 1);
+          v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
+          w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+        } else {
+          const uint4 x8 = __ldg(reinterpret_cast<const uint4*>(x + row * C + 8 * jc));
+          const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
+          const float4 q0 = __ldg(qr), q1 = __ldg(qr + 1);
+          const float2 x01 = widen2<IO>(x8.x), x23 = widen2<IO>(x8.y), x45 = widen2<IO>(x8.z), x67 = widen2<IO>(x8.w);
+          v[0] = x01.x, v[1] = x01.y, v[2] = x23.x, v[3] = x23.y, v[4] = x45.x, v[5] = x45.y, v[6] = x67.x, v[7] = x67.y;
+          w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+        }
       } else {
 #pragma unroll
         for (int e = 0; e < 8; ++e) v[e] = w[e] = 0.f;
@@ -850,20 +887,34 @@ int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y,
   return TFCB_OK;
 }
 
-template <int C, bool FAST>
-int launch_tc_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                  float* part_g, float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
+// The 16-bit backward's direct-term scratch (gdn_tc_bwd_dx_kernel): one 64 x C float32 tile per warpgroup of a dx
+// grid of at most kMaxParts CTAs.
+template <int C>
+long long bwd16_scratch_floats(long long n_pix) {
+  using K = TcCfg<C>;
+  const long long n_tiles = (std::max(n_pix, 0LL) + kTileM - 1) / kTileM;
+  return std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, kMaxParts) * K::kWG * kTileM * C;
+}
+
+// IO != 0: x, dy, dx in 16 bits and `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.
+template <int C, bool FAST, int IO>
+int launch_tc_bwd(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
+                  float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, TcFlags f,
+                  cudaStream_t s) {
   using K = TcCfg<C>;
   using L = DgCfg<C>;
-  TFCB_TRY(reserve_smem(gdn_tc_bwd_dx_kernel<C, FAST>, K::kSmem));
-  TFCB_TRY(reserve_smem(gdn_tc_dgamma_kernel<C, FAST>, L::kSmem));
+  TFCB_TRY(reserve_smem(gdn_tc_bwd_dx_kernel<C, FAST, IO>, K::kSmem));
+  TFCB_TRY(reserve_smem(gdn_tc_dgamma_kernel<C, FAST, IO>, L::kSmem));
   const int sms = sm_count_tc();
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sms);
-  gdn_tc_bwd_dx_kernel<C, FAST><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+  // dx does not depend on the grid (every tile is computed the same way by whichever CTA takes it)
+  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, IO == 0 ? sms : std::min(sms, kMaxParts));
+  gdn_tc_bwd_dx_kernel<C, FAST, IO><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f,
+                                                                        scratch);
   TFCB_LAUNCHED();
   const int grid_g = (int)std::min<long long>(n_tiles, std::min(sms, kMaxParts));
-  gdn_tc_dgamma_kernel<C, FAST><<<grid_g, L::kThreads, L::kSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
+  gdn_tc_dgamma_kernel<C, FAST, IO><<<grid_g, L::kThreads, L::kSmem, s>>>(static_cast<const IoElem<IO>*>(x), q_ws,
+                                                                          part_g, part_b, n_pix, f);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   *n_parts = grid_g;
@@ -956,21 +1007,61 @@ int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float*
               : launch_tc_fwd<192, false, 0>(x, gamma, beta, y, n_pix, f, s);
 }
 
-// 16-bit activations (float16 / bfloat16 in, same type out; parameters and arithmetic float32): the C = 128 kernel
-// reading and writing the 16-bit elements itself.  *handled = false -> the caller reports the configuration.
+// 16-bit activations (float16 / bfloat16 in, same type out; parameters and arithmetic float32): the C = 128 / 192
+// kernels reading and writing the 16-bit elements themselves.  *handled = false -> the caller reports the
+// configuration.
 int gdn_tc_forward16(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, int C, int flags,
                      float alpha, float eps, int dtype, cudaStream_t s, bool* handled) {
   *handled = false;
   TcFlags f;
-  if (C != 128 || (dtype != 1 && dtype != 2) || misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f))
+  if ((C != 128 && C != 192) || (dtype != 1 && dtype != 2) || misaligned(x, y, beta) ||
+      !tc_config(C, flags, alpha, eps, &f))
     return TFCB_OK;
   *handled = true;
   const bool fast = tc_fast(f);
+  if (C == 128) {
+    if (dtype == 1)
+      return fast ? launch_tc_fwd<128, true, 1>(x, gamma, beta, y, n_pix, f, s)
+                  : launch_tc_fwd<128, false, 1>(x, gamma, beta, y, n_pix, f, s);
+    return fast ? launch_tc_fwd<128, true, 2>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_fwd<128, false, 2>(x, gamma, beta, y, n_pix, f, s);
+  }
   if (dtype == 1)
-    return fast ? launch_tc_fwd<128, true, 1>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_fwd<128, false, 1>(x, gamma, beta, y, n_pix, f, s);
-  return fast ? launch_tc_fwd<128, true, 2>(x, gamma, beta, y, n_pix, f, s)
-              : launch_tc_fwd<128, false, 2>(x, gamma, beta, y, n_pix, f, s);
+    return fast ? launch_tc_fwd<192, true, 1>(x, gamma, beta, y, n_pix, f, s)
+                : launch_tc_fwd<192, false, 1>(x, gamma, beta, y, n_pix, f, s);
+  return fast ? launch_tc_fwd<192, true, 2>(x, gamma, beta, y, n_pix, f, s)
+              : launch_tc_fwd<192, false, 2>(x, gamma, beta, y, n_pix, f, s);
+}
+
+long long gdn_tc_backward16_scratch_floats(long long n_pix, int C) {
+  if (C == 128) return bwd16_scratch_floats<128>(n_pix);
+  if (C == 192) return bwd16_scratch_floats<192>(n_pix);
+  return 0;
+}
+
+// 16-bit backward: x, dy, dx in float16 / bfloat16; q, the partials and `scratch`
+// (gdn_tc_backward16_scratch_floats(n_pix, C) floats) as in gdn_tc_backward.  dx is the float32 backward's dx of the
+// widened inputs rounded once; q and the partials are the float32 backward's, bit for bit.  *handled = false -> the
+// caller reports the configuration.
+int gdn_tc_backward16(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
+                      float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, int C, int flags,
+                      float alpha, float eps, int dtype, cudaStream_t s, bool* handled) {
+  *handled = false;
+  TcFlags f;
+  if ((C != 128 && C != 192) || (dtype != 1 && dtype != 2) || misaligned(x, dy, dx) ||
+      misaligned(q_ws, beta, scratch) || !tc_config(C, flags, alpha, eps, &f))
+    return TFCB_OK;
+  *handled = true;
+#define TFCB_BWD16(C_, FAST_, IO_) \
+  launch_tc_bwd<C_, FAST_, IO_>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f, s)
+  const bool fast = tc_fast(f);
+  if (C == 128) {
+    if (dtype == 1) return fast ? TFCB_BWD16(128, true, 1) : TFCB_BWD16(128, false, 1);
+    return fast ? TFCB_BWD16(128, true, 2) : TFCB_BWD16(128, false, 2);
+  }
+  if (dtype == 1) return fast ? TFCB_BWD16(192, true, 1) : TFCB_BWD16(192, false, 1);
+  return fast ? TFCB_BWD16(192, true, 2) : TFCB_BWD16(192, false, 2);
+#undef TFCB_BWD16
 }
 
 // Tensor-core backward: dx, q (workspace) and the per-CTA partial sums (part_g [n_parts][C][C], part_b [n_parts][C])
@@ -990,10 +1081,11 @@ int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const
     return fast ? launch_tc_wide_bwd<320, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
                 : launch_tc_wide_bwd<320, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
   if (C == 128)
-    return fast ? launch_tc_bwd<128, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
-                : launch_tc_bwd<128, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
-  return fast ? launch_tc_bwd<192, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
-              : launch_tc_bwd<192, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
+    return fast ? launch_tc_bwd<128, true, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s)
+                : launch_tc_bwd<128, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f,
+                                               s);
+  return fast ? launch_tc_bwd<192, true, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s)
+              : launch_tc_bwd<192, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s);
 }
 
 }  // namespace tfcb

@@ -2,6 +2,7 @@
 TF primitives: GDN/IGDN forward + backward (``python/layers/gdn.py:371-421`` + TF autodiff) and the fused
 quantise+encode / decode+dequantise paths of the entropy models."""
 import ctypes as C
+import os
 
 import torch
 
@@ -42,16 +43,28 @@ def _gdn_args(x, gamma, beta):
   return x, gamma, beta, C_, x.numel() // C_
 
 
+def _gdn_native16(x, C_, n_pix, alpha, epsilon, pow_alpha, pow_epsilon, dy=None):
+  """Whether a 16-bit GDN call (forward, or backward with `dy`) runs on the kernels that read and write the 16-bit
+  elements themselves: C = 128 or 192 with the fixed exponents' shortcuts, 16-byte aligned tensors, and for the
+  backward dy in the activations' type.  Everything else, and everything under TFCB_GDN_FP32=1 (which keeps GDN off
+  the tensor cores), converts to float32 and back; both give the same bits."""
+  if os.environ.get("TFCB_GDN_FP32", "").startswith("1"):
+    return False
+  # dy.contiguous() keeps a contiguous dy's pointer and copies any other dy to a fresh (aligned) allocation
+  if dy is not None and (dy.dtype != x.dtype or dy.shape != x.shape or dy.data_ptr() % 16 != 0):
+    return False
+  return (x.dtype in _IO16 and C_ in (128, 192) and not pow_alpha and not pow_epsilon and
+          float(alpha) in (1.0, 2.0) and float(epsilon) in (1.0, 0.5) and n_pix > 0 and x.data_ptr() % 16 == 0)
+
+
 def gdn_forward(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, pow_alpha=False,
                 pow_epsilon=False):
   """x: float32 CUDA [..., C] (channels-last, contiguous) -> y of the same shape."""
   x, gamma, beta, C_, n_pix = _gdn_args(x, gamma, beta)
   if x.dtype in _IO16:
-    # mixed precision (gdn_test.py:200-210): 16-bit activations, float32 parameters and arithmetic.  C = 128 with the
-    # fixed exponents has a kernel that reads and writes 16-bit elements; everything else converts to float32.
-    native = (C_ == 128 and not pow_alpha and not pow_epsilon and float(alpha) in (1.0, 2.0) and
-              float(epsilon) in (1.0, 0.5) and n_pix > 0)
-    if native:
+    # mixed precision (gdn_test.py:200-210): 16-bit activations, float32 parameters and arithmetic.  The result is the
+    # float32 kernel's on the widened x, rounded once, on either path.
+    if _gdn_native16(x, C_, n_pix, alpha, epsilon, pow_alpha, pow_epsilon):
       y = torch.empty_like(x)
       check(_lib.lib().tfcb_gdn_forward_16bit(_p(x), _p(gamma), _p(beta), _p(y), n_pix, C_, _IO16[x.dtype],
                                               _flags(inverse, rectify), float(alpha), float(epsilon), _stream()))
@@ -68,7 +81,19 @@ def gdn_backward(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1.0, ep
                  pow_epsilon=False):
   """Returns (dx, dgamma, dbeta) for upstream gradient dy."""
   x, gamma, beta, C_, n_pix = _gdn_args(x, gamma, beta)
-  if x.dtype in _IO16:  # the backward kernels are float32: convert, run, hand dx back in the activations' type
+  if x.dtype in _IO16:
+    # dx in the activations' type: the float32 backward's dx of the widened x and dy, rounded once, on either path
+    if _gdn_native16(x, C_, n_pix, alpha, epsilon, pow_alpha, pow_epsilon, dy):
+      dy = dy.contiguous()
+      dx = torch.empty_like(x)
+      dgamma = torch.empty_like(gamma)
+      dbeta = torch.empty_like(beta)
+      L = _lib.lib()
+      ws = torch.empty(int(L.tfcb_gdn_backward_16bit_workspace_bytes(n_pix, C_)), dtype=torch.uint8, device=x.device)
+      check(L.tfcb_gdn_backward_16bit(_p(x), _p(gamma), _p(beta), _p(dy), _p(dx), _p(dgamma), _p(dbeta), _p(ws), n_pix,
+                                      C_, _IO16[x.dtype], _flags(inverse, rectify), float(alpha), float(epsilon),
+                                      _stream()))
+      return dx, dgamma, dbeta
     dx, dgamma, dbeta = gdn_backward(x.float(), gamma, beta, dy, inverse, rectify, alpha, epsilon, pow_alpha, pow_epsilon)
     return dx.to(x.dtype), dgamma, dbeta
   dy = dy.to(dtype=torch.float32).contiguous()

@@ -292,8 +292,8 @@ int tfcb_gdn_forward(const float* x_dev, const float* gamma_dev, const float* be
  * tfcb_gdn_backward_workspace_bytes(n_pix, C) bytes. */
 /* Mixed-precision variant (gdn_test.py:200-210: float32 variables, float16 / bfloat16 activations): x and y in
  * 16 bits (dtype 1 float16, 2 bfloat16), arithmetic in float32 -- 4 bytes of HBM traffic per element instead of 8.
- * Native kernel for C = 128 with alpha in {1, 2}, epsilon in {1, 1/2}; TFCB_INVALID_ARGUMENT otherwise (the caller
- * converts to float32). */
+ * Native kernel for C = 128 or 192 with alpha in {1, 2}, epsilon in {1, 1/2}; TFCB_INVALID_ARGUMENT otherwise (the
+ * caller converts to float32).  y is exactly the float32 result for the widened x, rounded once to dtype. */
 int tfcb_gdn_forward_16bit(const void* x_dev, const float* gamma_dev, const float* beta_dev, void* y_dev,
                            int64_t n_pix, int C, int dtype, int flags, float alpha, float epsilon, void* stream);
 
@@ -302,6 +302,18 @@ int tfcb_gdn_backward(const float* x_dev, const float* gamma_dev, const float* b
                       const float* dy_dev, float* dx_dev, float* dgamma_dev, float* dbeta_dev,
                       void* workspace_dev, int64_t n_pix, int C, int flags, float alpha,
                       float epsilon, void* stream);
+
+/* Mixed-precision backward: x, dy and dx in 16 bits (dtype 1 float16, 2 bfloat16), dgamma / dbeta and the arithmetic
+ * in float32 -- 6 bytes of algorithmic HBM traffic per element instead of 12.  dx is exactly the float32 backward's dx
+ * for the widened x and dy, rounded once to dtype; dgamma / dbeta are the float32 backward's, bit for bit.  Native
+ * kernels for C = 128 or 192 with alpha in {1, 2}, epsilon in {1, 1/2} and 16-byte aligned pointers;
+ * TFCB_INVALID_ARGUMENT otherwise (the caller converts to float32), and under TFCB_GDN_FP32=1.  n_pix = 0 launches
+ * nothing and sets dgamma / dbeta to zero, as tfcb_gdn_backward does.  `workspace_dev` must hold
+ * tfcb_gdn_backward_16bit_workspace_bytes(n_pix, C) bytes. */
+int64_t tfcb_gdn_backward_16bit_workspace_bytes(int64_t n_pix, int C);
+int tfcb_gdn_backward_16bit(const void* x_dev, const float* gamma_dev, const float* beta_dev, const void* dy_dev,
+                            void* dx_dev, float* dgamma_dev, float* dbeta_dev, void* workspace_dev, int64_t n_pix,
+                            int C, int dtype, int flags, float alpha, float epsilon, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Rate term of training: log p(y) of a prior convolved with U(-1/2, 1/2), forward and backward, fused.
