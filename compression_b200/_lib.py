@@ -80,6 +80,9 @@ SIGNATURES = {
     "tfcb_gdn_exponent_grads_workspace_bytes": (_i64, []),
     "tfcb_gdn_exponent_grads": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _f32, _f32, _vp]),
     "tfcb_gdn_backward": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _f32, _f32, _vp]),
+    "tfcb_gdn_backward_exponents_workspace_bytes": (_i64, [_i64, _int]),
+    "tfcb_gdn_backward_exponents": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _f32, _f32,
+                                           _vp]),
     "tfcb_gdn_backward_16bit_workspace_bytes": (_i64, [_i64, _int]),
     "tfcb_gdn_backward_16bit": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _f32, _f32,
                                        _vp]),

@@ -456,6 +456,11 @@ int sm_count() {
 
 bool fast_c(int C) { return C % 32 == 0 && C >= 32 && C <= 192; }
 
+// The tiled kernels read x (and q) with 16-byte loads: other pointers take the generic kernels.
+bool aligned16(const void* a, const void* b, const void* c) {
+  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
+}
+
 size_t fast_smem(int C) { return ((size_t)C * C + (size_t)kTM * (C + 4)) * sizeof(float); }
 
 template <typename K>
@@ -475,6 +480,10 @@ int gdn_tc_forward16(const void* x, const float* gamma, const float* beta, void*
 int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
                     float* part_g, float* part_b, int* n_parts, long long n_pix, int C, int flags, float alpha,
                     float eps, cudaStream_t s, bool* handled);
+int gdn_tc_backward_exponents(const float* x, const float* gamma, const float* beta, const float* dy, float* dx,
+                              float* q_ws, float* part_g, float* part_b, float* part_e, int* n_parts, int* n_parts_e,
+                              long long n_pix, int C, int flags, float alpha, float eps, cudaStream_t s,
+                              bool* handled);
 long long gdn_tc_backward16_scratch_floats(long long n_pix, int C);
 int gdn_tc_backward16(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
                       float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, int C, int flags,
@@ -522,7 +531,7 @@ int tfcb_gdn_forward(const float* x_dev, const float* gamma_dev, const float* be
   bool handled = false;
   TFCB_TRY(gdn_tc_forward(x_dev, gamma_dev, beta_dev, y_dev, n_pix, C, flags, alpha, epsilon, s, &handled));
   if (handled) return TFCB_OK;
-  if (fast_c(C)) {
+  if (fast_c(C) && aligned16(x_dev, y_dev, nullptr)) {
     const size_t smem = fast_smem(C);
     const long long n_tiles = (n_pix + kTM - 1) / kTM;
     const int grid = (int)std::min<long long>(n_tiles, sm_count());
@@ -583,7 +592,7 @@ int tfcb_gdn_backward(const float* x_dev, const float* gamma_dev, const float* b
                            alpha, epsilon, s, &handled));
   if (handled) {
     reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
-  } else if (fast_c(C)) {
+  } else if (fast_c(C) && aligned16(x_dev, dy_dev, dx_dev)) {
     const size_t smem = fast_smem(C);
     const long long n_tiles = (n_pix + kTM - 1) / kTM;
     const int grid = (int)std::min<long long>(n_tiles, sm_count());
@@ -677,6 +686,50 @@ int tfcb_gdn_exponent_grads(const float* x_dev, const float* gamma_dev, const fl
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
+}
+
+// tfcb_gdn_backward's workspace, then the exponent partials [kExpGrid][2] (the exponent kernel's grid bounds the
+// tensor-core kernels' CTA count too).
+int64_t tfcb_gdn_backward_exponents_workspace_bytes(int64_t n_pix, int C) {
+  return tfcb_gdn_backward_workspace_bytes(n_pix, C) + tfcb_gdn_exponent_grads_workspace_bytes();
+}
+
+int tfcb_gdn_backward_exponents(const float* x_dev, const float* gamma_dev, const float* beta_dev, const float* dy_dev,
+                                float* dx_dev, float* dgamma_dev, float* dbeta_dev, float* dalpha_depsilon_dev,
+                                void* workspace_dev, int64_t n_pix, int C, int flags, float alpha, float epsilon,
+                                void* stream) {
+  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
+  if (!x_dev || !gamma_dev || !beta_dev || !dy_dev || !dx_dev || !dgamma_dev || !dbeta_dev || !dalpha_depsilon_dev ||
+      !workspace_dev)
+    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  if ((size_t)C * 4 * sizeof(float) > 48 * 1024) return fail(TFCB_INVALID_ARGUMENT, "GDN exponent gradients: C too large");
+  cudaStream_t s = as_stream(stream);
+  if (n_pix == 0) {  // the empty sums, no kernel
+    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
+    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
+    TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon_dev, 0, 2 * sizeof(float), s));
+    return TFCB_OK;
+  }
+  float* q = reinterpret_cast<float*>(workspace_dev);
+  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
+  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
+  void* exp_ws = static_cast<uint8_t*>(workspace_dev) + tfcb_gdn_backward_workspace_bytes(n_pix, C);
+  bool handled = false;
+  int n_parts = 0, n_parts_e = 0;
+  TFCB_TRY(gdn_tc_backward_exponents(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b,
+                                     static_cast<float*>(exp_ws), &n_parts, &n_parts_e, n_pix, C, flags, alpha, epsilon,
+                                     s, &handled));
+  if (handled) {
+    reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
+    reduce_partials_kernel<<<1, 32, 0, s>>>(static_cast<const float*>(exp_ws), n_parts_e, 2, dalpha_depsilon_dev);
+    TFCB_LAUNCHED();
+    TFCB_CUDA_TRY(cudaGetLastError());
+    return TFCB_OK;
+  }
+  TFCB_TRY(tfcb_gdn_backward(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, workspace_dev, n_pix, C,
+                             flags, alpha, epsilon, stream));
+  return tfcb_gdn_exponent_grads(x_dev, gamma_dev, beta_dev, dy_dev, dalpha_depsilon_dev, exp_ws, n_pix, C, flags,
+                                 alpha, epsilon, stream);
 }
 
 }  // extern "C"

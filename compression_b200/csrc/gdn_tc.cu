@@ -22,7 +22,9 @@
 // C = 256 and 320 do not fit that layout (shared memory, registers) and split the work over blocks of output columns
 // instead: see "Wide layers" below.
 //
-// Everything outside {C in {128, 192, 256, 320}, alpha in {1, 2}, eps in {1, 0.5}} falls back to the fp32 kernels in
+// At C in {128, 192, 256, 320}, trainable exponents and fixed ones outside alpha in {1, 2}, eps in {1, 0.5} run the
+// literal-pow variant of every kernel (gdn_tc_pow_*, float32 only: powf / logf in the element functions, and the
+// backward sums dL/dalpha and dL/depsilon in its epilogues).  Every other width falls back to the fp32 kernels in
 // gdn.cu.  At C = 128 / 192 the forward, dx and dgamma kernels also take float16 / bfloat16 activations (IO = 1, 2):
 // each element is widened exactly on load, the arithmetic is the float32 kernels', and the only rounding to 16 bits
 // is the final store, so the result is the float32 result of the widened inputs rounded once.
@@ -157,6 +159,107 @@ __device__ __forceinline__ float tc_dpool(float x, const TcFlags& f) {
   return (u > 0.f) ? 1.f : ((u < 0.f) ? -1.f : 0.f);
 }
 
+// Literal-pow variant: trainable exponents (TFCB_GDN_POW_*) and fixed exponents outside {1, 2} / {1, 1/2}.  Its own
+// flags type selects the overloads below, so the kernels instantiated with TcFlags keep their code.  The element
+// functions are the fp32 kernels' pool_of / norm_of / dpool_du / dl_dn (gdn.cu) with IEEE divides: a mode of 0 is
+// powf, and a fixed exponent of a mixed configuration keeps its |u|, u^2 or sqrt shortcut.
+struct TcPowFlags {
+  int inverse, rectify, alpha_mode, eps_mode;  // alpha_mode: 0 powf(u, alpha), 1 |u|, 2 u^2; eps_mode: 0 powf, 1, 2 sqrt
+  float alpha, eps;
+  float* part_e;  // backward: per-CTA partials (dL/dalpha, dL/depsilon) [grid][2], or null
+};
+
+template <class F>
+constexpr bool kPow = std::is_same_v<F, TcPowFlags>;
+
+template <bool FAST>
+__device__ __forceinline__ float tc_pool(float x, const TcPowFlags& f) {
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  if (f.alpha_mode == 1) return f.rectify ? u : fabsf(u);
+  if (f.alpha_mode == 2) return u * u;
+  return powf(u, f.alpha);
+}
+
+__device__ __forceinline__ float tc_norm(float n, const TcPowFlags& f) {
+  if (f.eps_mode == 1) return n;
+  if (f.eps_mode == 2) return sqrtf(n);
+  return powf(n, f.eps);
+}
+
+template <bool FAST>
+__device__ __forceinline__ float tc_out(float x, float n, const TcPowFlags& f) {
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  const float m = tc_norm(n, f);
+  return f.inverse ? u * m : u / m;
+}
+
+template <bool FAST>
+__device__ __forceinline__ void tc_bwd_point(float x, float g, float n, const TcPowFlags& f, float* q, float* d) {
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  const float m = tc_norm(n, f);
+  *d = f.inverse ? g * m : g / m;
+  if (!f.inverse) {
+    if (f.eps_mode == 1)
+      *q = -g * u / (n * n);
+    else if (f.eps_mode == 2)
+      *q = -0.5f * g * u / (n * sqrtf(n));
+    else
+      *q = -f.eps * g * u * powf(n, -f.eps - 1.f);
+  } else {
+    if (f.eps_mode == 1)
+      *q = g * u;
+    else if (f.eps_mode == 2)
+      *q = 0.5f * g * u / sqrtf(n);
+    else
+      *q = f.eps * g * u * powf(n, f.eps - 1.f);
+  }
+}
+
+template <bool FAST>
+__device__ __forceinline__ float tc_dpool(float x, const TcPowFlags& f) {
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  if (f.alpha_mode == 1) {
+    if (f.rectify) return 1.f;
+    return (u > 0.f) ? 1.f : ((u < 0.f) ? -1.f : 0.f);
+  }
+  if (f.alpha_mode == 2) return 2.f * u;
+  return f.alpha * powf(u, f.alpha - 1.f);
+}
+
+// The exponent gradients' terms of one element (gdn.cu gdn_bwd_exponents_kernel):
+//   dL/depsilon += q n ln(n) / epsilon          from the epilogue that forms q
+//   dL/dalpha   += dp p ln(u)   (u > 0)          from the epilogue that adds dpool/dx . dp
+__device__ __forceinline__ float tc_deps_term(float q, float n, const TcPowFlags& f) { return q * n * logf(n) / f.eps; }
+
+__device__ __forceinline__ float tc_dalpha_term(float x, float dp, const TcPowFlags& f) {
+  const float u = f.rectify ? fmaxf(x, 0.f) : x;
+  return (u > 0.f) ? dp * tc_pool<false>(x, f) * logf(u) : 0.f;
+}
+
+// Sums the CTA's (dL/dalpha, dL/depsilon) in a fixed order and writes them to part[0], part[1] (either may be
+// skipped with WRITE_A / WRITE_E).  Called by every thread after its last MMA: reuses the start of `smem`.
+template <bool WRITE_A, bool WRITE_E>
+__device__ __forceinline__ void cta_exponent_partial(float dal, float dep, uint8_t* smem, float* part) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    dal += __shfl_xor_sync(0xFFFFFFFFu, dal, o);
+    dep += __shfl_xor_sync(0xFFFFFFFFu, dep, o);
+  }
+  float* red = reinterpret_cast<float*>(smem);
+  const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) {
+    red[2 * warp] = dal;
+    red[2 * warp + 1] = dep;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2 && (threadIdx.x == 0 ? WRITE_A : WRITE_E)) {
+    float s = 0.f;
+    for (int w = 0; w < n_warps; ++w) s += red[2 * w + threadIdx.x];
+    part[threadIdx.x] = s;
+  }
+}
+
 // Two floats -> bf16x2, the first in the low half (the lower column of a fragment).
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
   uint32_t r;
@@ -238,9 +341,9 @@ __device__ __forceinline__ void fill_planes(const float* __restrict__ gamma, uin
 
 // A fragments of pool(x) for one tile: k-step kk covers channels 16 kk .. 16 kk + 15; register r of a step holds
 // (row g, cols c, c+1), (row g+8, c, c+1), (row g, c+8, c+9), (row g+8, c+8, c+9), c = 16 kk + 2 t.
-template <int C, bool FAST, int IO>
+template <int C, bool FAST, int IO, class F>
 __device__ __forceinline__ void pool_frags(const void* __restrict__ x, long long r0, long long r1, bool ok0, bool ok1,
-                                           int t, const TcFlags& f, uint32_t (&ah)[C / 16][4],
+                                           int t, const F& f, uint32_t (&ah)[C / 16][4],
                                            uint32_t (&al)[C / 16][4]) {
 #pragma unroll
   for (int kk = 0; kk < C / 16; ++kk) {
@@ -286,10 +389,12 @@ __device__ __forceinline__ void gemm3(float (&acc)[C / 64][32], const uint32_t (
   _Pragma("unroll") for (int jj = 0; jj < 8; ++jj)     \
   _Pragma("unroll") for (int h = 0; h < 2; ++h)
 
-template <int C, bool FAST, int IO>
-__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
-gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                  void* __restrict__ y, long long n_pix, TcFlags f) {
+// The kernels' bodies take the flags type F: TcFlags for the fixed-exponent kernels, TcPowFlags for the literal-pow
+// kernels (float32 I/O, FAST = false), which are named gdn_tc_pow_*.
+template <int C, bool FAST, int IO, class F>
+__device__ __forceinline__ void tc_fwd_body(const void* __restrict__ x, const float* __restrict__ gamma,
+                                            const float* __restrict__ beta, void* __restrict__ y, long long n_pix,
+                                            const F& f) {
   using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   fill_planes<C>(gamma, smem);
@@ -318,6 +423,20 @@ gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, c
   }
 }
 
+template <int C, bool FAST, int IO>
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                  void* __restrict__ y, long long n_pix, TcFlags f) {
+  tc_fwd_body<C, FAST, IO>(x, gamma, beta, y, n_pix, f);
+}
+
+template <int C>
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_pow_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                      void* __restrict__ y, long long n_pix, TcPowFlags f) {
+  tc_fwd_body<C, false, 0>(x, gamma, beta, y, n_pix, f);
+}
+
 // Backward, part 1: per 64-pixel tile
 //   n = beta + p . gamma  ->  q = dL/dn (stored for part 2), the direct term of dx (stored)
 //   dp = q . gamma^T      ->  dx = direct term + dpool/dx * dp (the direct term read back from the same thread's
@@ -327,11 +446,12 @@ gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, c
 // to the warpgroup's own 64 x C float32 tile of `scratch` instead, and dx is stored once, rounded once: the result is
 // the float32 kernel's on the widened inputs, rounded to the activation type.  No register can hold it through MMA2
 // (the C = 192 FAST variant is at the 255-register limit) and no shared memory is left beside gamma's planes at C = 192.
-template <int C, bool FAST, int IO>
-__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
-gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                     const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                     TcFlags f, float* __restrict__ scratch) {
+// The literal-pow variant also sums dL/depsilon in the first epilogue and dL/dalpha in the second, one partial per CTA.
+template <int C, bool FAST, int IO, class F>
+__device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const float* __restrict__ gamma,
+                                               const float* __restrict__ beta, const void* __restrict__ dy,
+                                               void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
+                                               const F& f, float* __restrict__ scratch) {
   using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   fill_planes<C>(gamma, smem);
@@ -341,6 +461,7 @@ gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma
   // accumulator pair (n, jj, h) is at + 8 h C + 64 n + 8 jj: immediate offsets)
   float* const dtile = scratch + ((long long)(blockIdx.x * K::kWG + wg) * kTileM + warp * 16 + g) * C + 2 * t;
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  float dal = 0.f, dep = 0.f;  // literal-pow variant: this thread's exponent-gradient sums
   for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
@@ -362,6 +483,7 @@ gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma
       float2 q, d;
       tc_bwd_point<FAST>(xv.x, gv.x, b.x + a[0], f, &q.x, &d.x);
       tc_bwd_point<FAST>(xv.y, gv.y, b.y + a[1], f, &q.y, &d.y);
+      if constexpr (kPow<F>) dep += tc_deps_term(q.x, b.x + a[0], f) + tc_deps_term(q.y, b.y + a[1], f);
       *reinterpret_cast<float2*>(q_ws + idx) = q;
       if constexpr (IO == 0)
         *reinterpret_cast<float2*>(static_cast<float*>(dx) + idx) = d;
@@ -389,6 +511,8 @@ gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma
         d = *reinterpret_cast<const float2*>(dtile + 8 * h * C + 64 * n + 8 * jj);
       d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
       d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
+      if constexpr (kPow<F>)
+        dal += tc_dalpha_term(xv.x, acc[n][4 * jj + 2 * h], f) + tc_dalpha_term(xv.y, acc[n][4 * jj + 2 * h + 1], f);
       if (!FAST && f.rectify) {
         if (!(xv.x > 0.f)) d.x = 0.f;
         if (!(xv.y > 0.f)) d.y = 0.f;
@@ -396,6 +520,25 @@ gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma
       st_pair<IO>(dx, idx, d.x, d.y);
     }
   }
+  if constexpr (kPow<F>) {
+    if (f.part_e != nullptr) cta_exponent_partial<true, true>(dal, dep, smem, f.part_e + 2 * blockIdx.x);
+  }
+}
+
+template <int C, bool FAST, int IO>
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
+                     TcFlags f, float* __restrict__ scratch) {
+  tc_bwd_dx_body<C, FAST, IO>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
+}
+
+template <int C>
+__global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
+gdn_tc_pow_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                         const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
+                         TcPowFlags f, float* __restrict__ scratch) {
+  tc_bwd_dx_body<C, false, 0>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
 }
 
 // Backward, part 2: per-CTA partials dgamma[j, i] = sum_pix p[pix, j] q[pix, i] and dbeta[i] = sum_pix q[pix, i].
@@ -420,10 +563,10 @@ constexpr int kDgFlush = 8;
 template <int IO>
 using IoElem = std::conditional_t<IO == 0, float, uint16_t>;
 
-template <int C, bool FAST, int IO>
-__global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
-gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                     float* __restrict__ part_b, long long n_pix, TcFlags f) {
+template <int C, bool FAST, int IO, class F>
+__device__ __forceinline__ void tc_dgamma_body(const IoElem<IO>* __restrict__ x, const float* __restrict__ q,
+                                               float* __restrict__ part_g, float* __restrict__ part_b, long long n_pix,
+                                               const F& f) {
   using L = DgCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
@@ -461,7 +604,11 @@ gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__
       }
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        v[e] = tc_pool<FAST>(v[e], f);
+        // pow(0, alpha) is inf for alpha < 0: rows past the end must stay 0
+        if constexpr (kPow<F>)
+          v[e] = row < n_pix ? tc_pool<FAST>(v[e], f) : 0.f;
+        else
+          v[e] = tc_pool<FAST>(v[e], f);
         bsum[e] += w[e];
       }
       const int slot = (jc * kTileM + p) * 16;
@@ -533,6 +680,20 @@ gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__
   }
 }
 
+template <int C, bool FAST, int IO>
+__global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
+gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                     float* __restrict__ part_b, long long n_pix, TcFlags f) {
+  tc_dgamma_body<C, FAST, IO>(x, q, part_g, part_b, n_pix, f);
+}
+
+template <int C>
+__global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
+gdn_tc_pow_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                         float* __restrict__ part_b, long long n_pix, TcPowFlags f) {
+  tc_dgamma_body<C, false, 0>(x, q, part_g, part_b, n_pix, f);
+}
+
 // ---- Wide layers, C in {256, 320}: the work is split over blocks of NB output columns ----
 //
 // At C > 192 neither gamma's planes (4 C^2 bytes: 256 / 400 KB) nor a warpgroup's A fragments of all K = C plus the
@@ -579,9 +740,9 @@ __device__ __forceinline__ void fill_planes_block(const float* __restrict__ gamm
 
 // A fragments of channels [16 k0, 16 k0 + KA) of a tile of a [n_pix, C] array, at the positions pool_frags uses:
 // pool(x) (POOL) or the values themselves (q).
-template <int C, int KA, bool POOL, bool FAST>
+template <int C, int KA, bool POOL, bool FAST, class F>
 __device__ __forceinline__ void slice_frags(const float* __restrict__ src, long long r0, long long r1, bool ok0,
-                                            bool ok1, int t, int k0, const TcFlags& f, uint32_t (&ah)[KA / 16][4],
+                                            bool ok1, int t, int k0, const F& f, uint32_t (&ah)[KA / 16][4],
                                             uint32_t (&al)[KA / 16][4]) {
 #pragma unroll
   for (int kk = 0; kk < KA / 16; ++kk) {
@@ -606,9 +767,9 @@ __device__ __forceinline__ void slice_frags(const float* __restrict__ src, long 
 // K is walked in kKSlices slices, each loaded into registers, multiplied and waited for before the next is loaded:
 // at C = 320 the A fragments of all K (160 registers) next to the accumulators leave ptxas too few registers to
 // avoid spills.  Otherwise gemm3 with the plane extents of one block.
-template <int C, int TB, bool POOL, bool FAST>
+template <int C, int TB, bool POOL, bool FAST, class F>
 __device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32], const float* __restrict__ src,
-                                          long long r0, long long r1, bool ok0, bool ok1, int t, const TcFlags& f,
+                                          long long r0, long long r1, bool ok0, bool ok1, int t, const F& f,
                                           uint32_t bh, uint32_t bl) {
   constexpr int NB = WideCfg<C>::kNB, KA = C / WideCfg<C>::kKSlices;
 #pragma unroll
@@ -639,10 +800,10 @@ __device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32]
   }
 }
 
-template <int C, bool FAST>
-__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
-gdn_tc_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                       float* __restrict__ y, long long n_pix, TcFlags f) {
+template <int C, bool FAST, class F>
+__device__ __forceinline__ void tc_wide_fwd_body(const float* __restrict__ x, const float* __restrict__ gamma,
+                                                 const float* __restrict__ beta, float* __restrict__ y,
+                                                 long long n_pix, const F& f) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -670,12 +831,27 @@ gdn_tc_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ ga
   }
 }
 
-// Backward, pass 1: n[:, block] = beta + p . gamma[:, block]  ->  q[:, block] (workspace), dx[:, block] = direct term.
 template <int C, bool FAST>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
-gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                         const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws,
-                         long long n_pix, TcFlags f) {
+gdn_tc_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                       float* __restrict__ y, long long n_pix, TcFlags f) {
+  tc_wide_fwd_body<C, FAST>(x, gamma, beta, y, n_pix, f);
+}
+
+template <int C>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_pow_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
+                           const float* __restrict__ beta, float* __restrict__ y, long long n_pix, TcPowFlags f) {
+  tc_wide_fwd_body<C, false>(x, gamma, beta, y, n_pix, f);
+}
+
+// Backward, pass 1: n[:, block] = beta + p . gamma[:, block]  ->  q[:, block] (workspace), dx[:, block] = direct term.
+// The literal-pow variant also sums dL/depsilon over the block's columns: partial [blockIdx.x][1].
+template <int C, bool FAST, class F>
+__device__ __forceinline__ void tc_wide_bwd_q_body(const float* __restrict__ x, const float* __restrict__ gamma,
+                                                   const float* __restrict__ beta, const float* __restrict__ dy,
+                                                   float* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
+                                                   const F& f) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -685,6 +861,7 @@ gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ 
   const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const long long stride = (long long)(gridDim.x / W::kBlocks) * W::kWG;
+  float dep = 0.f;
   for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
@@ -700,12 +877,36 @@ gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ 
       float2 qv, d;
       tc_bwd_point<FAST>(xv.x, gv.x, b.x + acc[n][4 * jj + 2 * h], f, &qv.x, &d.x);
       tc_bwd_point<FAST>(xv.y, gv.y, b.y + acc[n][4 * jj + 2 * h + 1], f, &qv.y, &d.y);
+      if constexpr (kPow<F>) {
+        const float e = tc_deps_term(qv.x, b.x + acc[n][4 * jj + 2 * h], f) +
+                        tc_deps_term(qv.y, b.y + acc[n][4 * jj + 2 * h + 1], f);
+        if (ok) dep += e;
+      }
       if (ok) {
         *reinterpret_cast<float2*>(q_ws + idx) = qv;
         *reinterpret_cast<float2*>(dx + idx) = d;
       }
     }
   }
+  if constexpr (kPow<F>) {
+    if (f.part_e != nullptr) cta_exponent_partial<false, true>(0.f, dep, smem, f.part_e + 2 * blockIdx.x);
+  }
+}
+
+template <int C, bool FAST>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
+                         const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws,
+                         long long n_pix, TcFlags f) {
+  tc_wide_bwd_q_body<C, FAST>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+}
+
+template <int C>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_pow_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
+                             const float* __restrict__ beta, const float* __restrict__ dy, float* __restrict__ dx,
+                             float* __restrict__ q_ws, long long n_pix, TcPowFlags f) {
+  tc_wide_bwd_q_body<C, false>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
 }
 
 // Backward, pass 2: dp[:, J] = q . gamma[J, :]^T  ->  dx[:, J] += dpool/dx * dp, then the rectifier's mask.
@@ -743,14 +944,56 @@ gdn_tc_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__
   }
 }
 
+// The literal-pow pass 2 also sums dL/dalpha over the block's rows: partial [blockIdx.x][0].  It is a copy of
+// gdn_tc_wide_bwd_dp_kernel rather than a shared inline body: routed through one, the fixed-exponent kernel's
+// instruction schedule changed.
+template <int C>
+__global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
+gdn_tc_pow_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
+                              const float* __restrict__ q, float* __restrict__ dx, long long n_pix, TcPowFlags f) {
+  using W = WideCfg<C>;
+  constexpr int NB = W::kNB;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int j0 = (int)(blockIdx.x % W::kBlocks) * NB;
+  fill_planes_block<C, NB, C>(gamma, j0, 0, smem);
+  const uint32_t bh = smem_u32(smem), bl = bh + C * NB * 2;
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
+  const long long stride = (long long)(gridDim.x / W::kBlocks) * W::kWG;
+  float dal = 0.f;
+  for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
+    const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
+    const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    float acc[NB / 64][32];
+    wide_gemm<C, 1, false, false>(acc, q, r0, r1, ok0, ok1, t, f, bh, bl);
+    TFCB_FOR_ACC_PAIRS(NB) {
+      const bool ok = h ? ok1 : ok0;
+      const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
+      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
+      float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
+      const float dp0 = acc[n][4 * jj + 2 * h], dp1 = acc[n][4 * jj + 2 * h + 1];
+      d.x += tc_dpool<false>(xv.x, f) * dp0;
+      d.y += tc_dpool<false>(xv.y, f) * dp1;
+      const float e = tc_dalpha_term(xv.x, dp0, f) + tc_dalpha_term(xv.y, dp1, f);
+      if (ok) dal += e;
+      if (f.rectify) {
+        if (!(xv.x > 0.f)) d.x = 0.f;
+        if (!(xv.y > 0.f)) d.y = 0.f;
+      }
+      if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+    }
+  }
+  if (f.part_e != nullptr) cta_exponent_partial<true, false>(dal, 0.f, smem, f.part_e + 2 * blockIdx.x);
+}
+
 // dgamma[:, block] and dbeta[block]: gdn_tc_dgamma_kernel with q staged for the block's NB channels only.  CTA
 // (part, block) adds into columns [c0, c0 + NB) of partial `part`, so the partials keep the [n_parts][C][C] layout.
 // Thread tid stages p channels 8 (tid / 16) .. + 7 of pixels tid % 16 + 16 s, and the same q channels of the block
 // when tid / 16 < NB / 8.
-template <int C, bool FAST>
-__global__ void __launch_bounds__(2 * C, 1)
-gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                          float* __restrict__ part_b, long long n_pix, TcFlags f) {
+template <int C, bool FAST, class F>
+__device__ __forceinline__ void tc_wide_dgamma_body(const float* __restrict__ x, const float* __restrict__ q,
+                                                    float* __restrict__ part_g, float* __restrict__ part_b,
+                                                    long long n_pix, const F& f) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   constexpr int kP = W::kDgPPlane, kQ = W::kDgQPlane;
@@ -786,7 +1029,11 @@ gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__
       }
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        v[e] = tc_pool<FAST>(v[e], f);
+        // pow(0, alpha) is inf for alpha < 0: rows past the end must stay 0
+        if constexpr (kPow<F>)
+          v[e] = row < n_pix ? tc_pool<FAST>(v[e], f) : 0.f;
+        else
+          v[e] = tc_pool<FAST>(v[e], f);
         bsum[e] += w[e];
       }
       const int slot = (jc * kTileM + p) * 16;
@@ -861,6 +1108,20 @@ gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__
   }
 }
 
+template <int C, bool FAST>
+__global__ void __launch_bounds__(2 * C, 1)
+gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                          float* __restrict__ part_b, long long n_pix, TcFlags f) {
+  tc_wide_dgamma_body<C, FAST>(x, q, part_g, part_b, n_pix, f);
+}
+
+template <int C>
+__global__ void __launch_bounds__(2 * C, 1)
+gdn_tc_pow_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
+                              float* __restrict__ part_b, long long n_pix, TcPowFlags f) {
+  tc_wide_dgamma_body<C, false>(x, q, part_g, part_b, n_pix, f);
+}
+
 int sm_count_tc() {
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
@@ -874,14 +1135,52 @@ int reserve_smem(Kern kernel, int bytes) {
   return TFCB_OK;
 }
 
-template <int C, bool FAST, int IO>
-int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, TcFlags f,
+// The kernels of a configuration: gdn_tc_* for TcFlags, gdn_tc_pow_* (float32, FAST = false) for TcPowFlags.
+template <int C, bool FAST, int IO, class F>
+auto fwd_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_fwd_kernel<C>;
+  else return gdn_tc_fwd_kernel<C, FAST, IO>;
+}
+template <int C, bool FAST, int IO, class F>
+auto bwd_dx_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_bwd_dx_kernel<C>;
+  else return gdn_tc_bwd_dx_kernel<C, FAST, IO>;
+}
+template <int C, bool FAST, int IO, class F>
+auto dgamma_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_dgamma_kernel<C>;
+  else return gdn_tc_dgamma_kernel<C, FAST, IO>;
+}
+template <int C, bool FAST, class F>
+auto wide_fwd_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_fwd_kernel<C>;
+  else return gdn_tc_wide_fwd_kernel<C, FAST>;
+}
+template <int C, bool FAST, class F>
+auto wide_bwd_q_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_q_kernel<C>;
+  else return gdn_tc_wide_bwd_q_kernel<C, FAST>;
+}
+template <int C, bool FAST, class F>
+auto wide_bwd_dp_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_dp_kernel<C>;
+  else return gdn_tc_wide_bwd_dp_kernel<C, FAST>;
+}
+template <int C, bool FAST, class F>
+auto wide_dgamma_kernel() {
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_dgamma_kernel<C>;
+  else return gdn_tc_wide_dgamma_kernel<C, FAST>;
+}
+
+template <int C, bool FAST, int IO, class F>
+int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, F f,
                   cudaStream_t s) {
   using K = TcCfg<C>;
-  TFCB_TRY(reserve_smem(gdn_tc_fwd_kernel<C, FAST, IO>, K::kSmem));
+  const auto kern = fwd_kernel<C, FAST, IO, F>();
+  TFCB_TRY(reserve_smem(kern, K::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sm_count_tc());
-  gdn_tc_fwd_kernel<C, FAST, IO><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
+  kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
@@ -896,28 +1195,31 @@ long long bwd16_scratch_floats(long long n_pix) {
   return std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, kMaxParts) * K::kWG * kTileM * C;
 }
 
-// IO != 0: x, dy, dx in 16 bits and `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.
-template <int C, bool FAST, int IO>
+// IO != 0: x, dy, dx in 16 bits and `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.  TcPowFlags: the dx
+// kernel's CTAs write f.part_e[CTA][2] (when not null), *n_parts_e of them (at most kMaxParts).
+template <int C, bool FAST, int IO, class F>
 int launch_tc_bwd(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
-                  float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, TcFlags f,
-                  cudaStream_t s) {
+                  float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, F f,
+                  cudaStream_t s, int* n_parts_e = nullptr) {
   using K = TcCfg<C>;
   using L = DgCfg<C>;
-  TFCB_TRY(reserve_smem(gdn_tc_bwd_dx_kernel<C, FAST, IO>, K::kSmem));
-  TFCB_TRY(reserve_smem(gdn_tc_dgamma_kernel<C, FAST, IO>, L::kSmem));
+  const auto dx_kern = bwd_dx_kernel<C, FAST, IO, F>();
+  const auto dg_kern = dgamma_kernel<C, FAST, IO, F>();
+  TFCB_TRY(reserve_smem(dx_kern, K::kSmem));
+  TFCB_TRY(reserve_smem(dg_kern, L::kSmem));
   const int sms = sm_count_tc();
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   // dx does not depend on the grid (every tile is computed the same way by whichever CTA takes it)
-  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, IO == 0 ? sms : std::min(sms, kMaxParts));
-  gdn_tc_bwd_dx_kernel<C, FAST, IO><<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f,
-                                                                        scratch);
+  const bool capped = IO != 0 || kPow<F>;
+  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, capped ? std::min(sms, kMaxParts) : sms);
+  dx_kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
   TFCB_LAUNCHED();
   const int grid_g = (int)std::min<long long>(n_tiles, std::min(sms, kMaxParts));
-  gdn_tc_dgamma_kernel<C, FAST, IO><<<grid_g, L::kThreads, L::kSmem, s>>>(static_cast<const IoElem<IO>*>(x), q_ws,
-                                                                          part_g, part_b, n_pix, f);
+  dg_kern<<<grid_g, L::kThreads, L::kSmem, s>>>(static_cast<const IoElem<IO>*>(x), q_ws, part_g, part_b, n_pix, f);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   *n_parts = grid_g;
+  if (n_parts_e) *n_parts_e = grid;
   return TFCB_OK;
 }
 
@@ -929,38 +1231,46 @@ int wide_grid(long long n_tiles_per_group) {
   return (int)(std::min<long long>(n_tiles_per_group, groups) * W::kBlocks);
 }
 
-template <int C, bool FAST>
-int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, TcFlags f,
+template <int C, bool FAST, class F>
+int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, F f,
                        cudaStream_t s) {
   using W = WideCfg<C>;
-  TFCB_TRY(reserve_smem(gdn_tc_wide_fwd_kernel<C, FAST>, W::kSmem));
+  const auto kern = wide_fwd_kernel<C, FAST, F>();
+  TFCB_TRY(reserve_smem(kern, W::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
-  gdn_tc_wide_fwd_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
+  kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
 }
 
-template <int C, bool FAST>
+// TcPowFlags: CTA b of pass 1 writes f.part_e[b][1] and CTA b of pass 2 f.part_e[b][0] (when not null), *n_parts_e
+// partials (at most kMaxParts * kBlocks).
+template <int C, bool FAST, class F>
 int launch_tc_wide_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                       float* part_g, float* part_b, int* n_parts, long long n_pix, TcFlags f, cudaStream_t s) {
+                       float* part_g, float* part_b, int* n_parts, long long n_pix, F f, cudaStream_t s,
+                       int* n_parts_e = nullptr) {
   using W = WideCfg<C>;
-  TFCB_TRY(reserve_smem(gdn_tc_wide_bwd_q_kernel<C, FAST>, W::kSmem));
-  TFCB_TRY(reserve_smem(gdn_tc_wide_bwd_dp_kernel<C, FAST>, W::kSmem));
-  TFCB_TRY(reserve_smem(gdn_tc_wide_dgamma_kernel<C, FAST>, W::kDgSmem));
+  const auto q_kern = wide_bwd_q_kernel<C, FAST, F>();
+  const auto dp_kern = wide_bwd_dp_kernel<C, FAST, F>();
+  const auto dg_kern = wide_dgamma_kernel<C, FAST, F>();
+  TFCB_TRY(reserve_smem(q_kern, W::kSmem));
+  TFCB_TRY(reserve_smem(dp_kern, W::kSmem));
+  TFCB_TRY(reserve_smem(dg_kern, W::kDgSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
-  gdn_tc_wide_bwd_q_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+  q_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
   TFCB_LAUNCHED();
-  gdn_tc_wide_bwd_dp_kernel<C, FAST><<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, q_ws, dx, n_pix, f);
+  dp_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, q_ws, dx, n_pix, f);
   TFCB_LAUNCHED();
   // one partial per group of kBlocks CTAs (at most sms / kBlocks <= kMaxParts): fixed by n_pix, C and the SM count
   const int grid_g = wide_grid<C>(n_tiles);
-  gdn_tc_wide_dgamma_kernel<C, FAST><<<grid_g, 2 * C, W::kDgSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
+  dg_kern<<<grid_g, 2 * C, W::kDgSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   *n_parts = grid_g / W::kBlocks;
+  if (n_parts_e) *n_parts_e = grid;
   return TFCB_OK;
 }
 
@@ -981,8 +1291,51 @@ bool tc_config(int C, int flags, float alpha, float eps, TcFlags* f) {
 
 bool tc_fast(const TcFlags& f) { return f.alpha_mode == 1 && f.eps_mode == 1 && !f.rectify; }
 
+// The configurations of the four widths that tc_config leaves out (a trainable exponent, or a fixed one outside
+// {1, 2} / {1, 1/2}) run the literal-pow kernels; fills *f as gdn.cu's parse_flags does, part_e null.
+bool tc_pow_config(int C, int flags, float alpha, float eps, TcPowFlags* f) {
+  if (!(C == 128 || C == 192 || C == 256 || C == 320)) return false;
+  if (const char* env = getenv("TFCB_GDN_FP32")) {
+    if (env[0] == '1') return false;
+  }
+  TcFlags fixed;
+  if (tc_config(C, flags, alpha, eps, &fixed)) return false;
+  f->inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
+  f->rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
+  f->alpha_mode = (flags & TFCB_GDN_POW_ALPHA) ? 0 : (alpha == 1.f ? 1 : (alpha == 2.f ? 2 : 0));
+  f->eps_mode = (flags & TFCB_GDN_POW_EPSILON) ? 0 : (eps == 1.f ? 1 : (eps == 0.5f ? 2 : 0));
+  f->alpha = alpha;
+  f->eps = eps;
+  f->part_e = nullptr;
+  return true;
+}
+
 bool misaligned(const void* a, const void* b, const void* c) {
   return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) != 0;
+}
+
+int launch_pow_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
+                   const TcPowFlags& f, cudaStream_t s) {
+  if (C == 128) return launch_tc_fwd<128, false, 0>(x, gamma, beta, y, n_pix, f, s);
+  if (C == 192) return launch_tc_fwd<192, false, 0>(x, gamma, beta, y, n_pix, f, s);
+  if (C == 256) return launch_tc_wide_fwd<256, false>(x, gamma, beta, y, n_pix, f, s);
+  return launch_tc_wide_fwd<320, false>(x, gamma, beta, y, n_pix, f, s);
+}
+
+int launch_pow_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
+                   float* part_g, float* part_b, int* n_parts, int* n_parts_e, long long n_pix, int C,
+                   const TcPowFlags& f, cudaStream_t s) {
+  if (C == 128)
+    return launch_tc_bwd<128, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s,
+                                        n_parts_e);
+  if (C == 192)
+    return launch_tc_bwd<192, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s,
+                                        n_parts_e);
+  if (C == 256)
+    return launch_tc_wide_bwd<256, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
+                                          n_parts_e);
+  return launch_tc_wide_bwd<320, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
+                                        n_parts_e);
 }
 
 }  // namespace
@@ -990,6 +1343,11 @@ bool misaligned(const void* a, const void* b, const void* c) {
 int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
                    int flags, float alpha, float eps, cudaStream_t s, bool* handled) {
   *handled = false;
+  TcPowFlags pf;
+  if (!misaligned(x, y, beta) && tc_pow_config(C, flags, alpha, eps, &pf)) {
+    *handled = true;
+    return launch_pow_fwd(x, gamma, beta, y, n_pix, C, pf, s);
+  }
   TcFlags f;
   if (misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
@@ -1070,6 +1428,12 @@ int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const
                     float* part_g, float* part_b, int* n_parts, long long n_pix, int C, int flags, float alpha,
                     float eps, cudaStream_t s, bool* handled) {
   *handled = false;
+  TcPowFlags pf;
+  if (!misaligned(x, dy, dx) && !misaligned(q_ws, beta, nullptr) && tc_pow_config(C, flags, alpha, eps, &pf)) {
+    *handled = true;
+    int n_parts_e = 0;
+    return launch_pow_bwd(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, &n_parts_e, n_pix, C, pf, s);
+  }
   TcFlags f;
   if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
   *handled = true;
@@ -1086,6 +1450,22 @@ int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const
                                                s);
   return fast ? launch_tc_bwd<192, true, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s)
               : launch_tc_bwd<192, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s);
+}
+
+// gdn_tc_backward with dL/dalpha and dL/depsilon fused in, for the literal-pow configurations: part_e receives
+// *n_parts_e partials [2] (at most kMaxParts * 5), reduced by the caller.  *handled = false (every other
+// configuration) -> the caller runs the fp32 kernels and the exponent kernel.
+int gdn_tc_backward_exponents(const float* x, const float* gamma, const float* beta, const float* dy, float* dx,
+                              float* q_ws, float* part_g, float* part_b, float* part_e, int* n_parts, int* n_parts_e,
+                              long long n_pix, int C, int flags, float alpha, float eps, cudaStream_t s,
+                              bool* handled) {
+  *handled = false;
+  TcPowFlags pf;
+  if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_pow_config(C, flags, alpha, eps, &pf))
+    return TFCB_OK;
+  *handled = true;
+  pf.part_e = part_e;
+  return launch_pow_bwd(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_parts_e, n_pix, C, pf, s);
 }
 
 }  // namespace tfcb

@@ -122,6 +122,29 @@ def gdn_exponent_grads(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1
   return out
 
 
+def gdn_backward_exponents(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, pow_alpha=True,
+                           pow_epsilon=True):
+  """(dx, dgamma, dbeta, dalpha_depsilon) in one library call: gdn_backward's three gradients and gdn_exponent_grads'
+  [2] tensor.  With a trainable exponent at C = 128, 192, 256 or 320 the exponent sums are fused into the tensor-core
+  backward.  16-bit activations go through float32 (dx is rounded once to their type)."""
+  if x.dtype in _IO16:
+    dx, dgamma, dbeta, dae = gdn_backward_exponents(x.float(), gamma, beta, dy, inverse, rectify, alpha, epsilon,
+                                                    pow_alpha, pow_epsilon)
+    return dx.to(x.dtype), dgamma, dbeta, dae
+  x, gamma, beta, C_, n_pix = _gdn_args(x, gamma, beta)
+  dy = dy.to(dtype=torch.float32).contiguous()
+  dx = torch.empty_like(x)
+  dgamma = torch.empty_like(gamma)
+  dbeta = torch.empty_like(beta)
+  dae = torch.empty(2, dtype=torch.float32, device=x.device)
+  L = _lib.lib()
+  ws = torch.empty(int(L.tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C_)), dtype=torch.uint8, device=x.device)
+  check(L.tfcb_gdn_backward_exponents(_p(x), _p(gamma), _p(beta), _p(dy), _p(dx), _p(dgamma), _p(dbeta), _p(dae),
+                                      _p(ws), n_pix, C_, _flags(inverse, rectify, pow_alpha, pow_epsilon),
+                                      float(alpha), float(epsilon), _stream()))
+  return dx, dgamma, dbeta, dae
+
+
 class _GDNFunction(torch.autograd.Function):
   """alpha_t / epsilon_t: 0-d tensors when the exponent is trainable (their value is read on the host: the kernels
   take the exponents as scalars), else None and the fixed value travels in `alpha` / `epsilon`."""
@@ -141,12 +164,13 @@ class _GDNFunction(torch.autograd.Function):
   def backward(ctx, dy):
     x, gamma, beta = ctx.saved_tensors
     inverse, rectify, alpha, epsilon, pa, pe = ctx.cfg
-    dx, dgamma, dbeta = gdn_backward(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
     dalpha = depsilon = None
     if (pa and ctx.needs_input_grad[3]) or (pe and ctx.needs_input_grad[4]):
-      g2 = gdn_exponent_grads(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
+      dx, dgamma, dbeta, g2 = gdn_backward_exponents(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
       dalpha = g2[0] if pa else None
       depsilon = g2[1] if pe else None
+    else:
+      dx, dgamma, dbeta = gdn_backward(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
     return dx, dgamma, dbeta, dalpha, depsilon, None, None, None, None
 
 

@@ -271,9 +271,10 @@ int tfcb_stochastic_round(const void* inputs_dev, int dtype, int64_t n, float st
  *   y_i = u_i / n_i^eps  (GDN)   or   u_i * n_i^eps  (IGDN)
  * x, y: float32 [n_pix, C] row-major;  gamma float32 [C, C] (row j, column i);  beta float32 [C].
  * alpha in {1, 2} and eps in {1, 0.5} take the reference's fast paths; other values use powf.
- * C in {128, 192} with those alpha / eps and 16-byte aligned pointers run on the tensor cores (bf16 split with
- * fp32 accumulation: <= 1e-5 relative forward, <= 2e-5 of the largest gradient backward); every other shape
- * runs the fp32 kernels.  TFCB_GDN_FP32=1 in the environment forces the fp32 kernels.
+ * C in {128, 192, 256, 320} with 16-byte aligned pointers run on the tensor cores (bf16 split with fp32
+ * accumulation: <= 1e-5 relative forward, <= 2e-5 of the largest gradient backward), with literal powf kernels for
+ * trainable exponents and fixed ones outside those values; every other shape runs the fp32 kernels.
+ * TFCB_GDN_FP32=1 in the environment forces the fp32 kernels.
  * The reference has no native GDN code (TF graph of abs / conv1x1 / bias_add / div); the backward
  * pass replaces TF autodiff of that graph.
  * ---------------------------------------------------------------------------------------------- */
@@ -388,6 +389,20 @@ int64_t tfcb_gdn_exponent_grads_workspace_bytes(void);
 int tfcb_gdn_exponent_grads(const float* x_dev, const float* gamma_dev, const float* beta_dev,
                             const float* dy_dev, float* dalpha_depsilon_dev, void* workspace_dev,
                             int64_t n_pix, int C, int flags, float alpha, float epsilon, void* stream);
+
+/* All five gradients in one call: dx, dgamma, dbeta as tfcb_gdn_backward and dalpha_depsilon_dev float32 [2] as
+ * tfcb_gdn_exponent_grads, for any configuration.  C in {128, 192, 256, 320} with a trainable exponent (or a fixed one
+ * outside {1, 2} / {1, 1/2}) and 16-byte aligned pointers runs the tensor-core backward with both exponent sums fused
+ * into its epilogues (bitwise reproducible from call to call); everything else, and TFCB_GDN_FP32=1, runs
+ * tfcb_gdn_backward's kernels followed by tfcb_gdn_exponent_grads' and gives their results.  `workspace_dev` holds
+ * tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C) bytes: tfcb_gdn_backward's workspace followed by
+ * tfcb_gdn_exponent_grads_workspace_bytes() bytes.  Shapes, pointers and C <= 3072 are checked before any device work
+ * (TFCB_INVALID_ARGUMENT); n_pix = 0 launches nothing and sets dgamma, dbeta, dalpha and depsilon to zero. */
+int64_t tfcb_gdn_backward_exponents_workspace_bytes(int64_t n_pix, int C);
+int tfcb_gdn_backward_exponents(const float* x_dev, const float* gamma_dev, const float* beta_dev, const float* dy_dev,
+                                float* dx_dev, float* dgamma_dev, float* dbeta_dev, float* dalpha_depsilon_dev,
+                                void* workspace_dev, int64_t n_pix, int C, int flags, float alpha, float epsilon,
+                                void* stream);
 
 int64_t tfcb_launch_count(void);
 
