@@ -86,6 +86,10 @@ SIGNATURES = {
     "tfcb_gdn_backward_16bit_workspace_bytes": (_i64, [_i64, _int]),
     "tfcb_gdn_backward_16bit": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _f32, _f32,
                                        _vp]),
+    "tfcb_gdn_forward_cf": (_int, [_vp, _vp, _vp, _vp, _i64, _i64, _int, _int, _int, _f32, _f32, _vp]),
+    "tfcb_gdn_backward_cf_workspace_bytes": (_i64, [_i64, _i64, _int, _int]),
+    "tfcb_gdn_backward_cf": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _int, _int, _int, _f32,
+                                    _f32, _vp]),
     "tfcb_noisy_deep_factorized_log_prob": (_int, [_vp, _vp, _vp, _i64, _int, _vp]),
     "tfcb_noisy_deep_factorized_workspace_bytes": (_i64, [_i64, _int]),
     "tfcb_noisy_deep_factorized_log_prob_backward": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _int, _vp]),

@@ -488,6 +488,40 @@ long long gdn_tc_backward16_scratch_floats(long long n_pix, int C);
 int gdn_tc_backward16(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
                       float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, int C, int flags,
                       float alpha, float eps, int dtype, cudaStream_t s, bool* handled);
+bool gdn_tc_cf_config(int C, int dtype, int flags, float alpha, float eps, bool* pow);
+int gdn_tc_forward_cf(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, long long S,
+                      int C, int flags, float alpha, float eps, int dtype, cudaStream_t s);
+int gdn_tc_backward_cf(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
+                       float* part_g, float* part_b, float* scratch, float* part_e, int* n_parts, int* n_parts_e,
+                       long long n_pix, long long S, int C, int flags, float alpha, float eps, int dtype,
+                       cudaStream_t s);
+
+namespace {
+
+// The host-side checks of the channels-first entries, before any device work: sizes (*n_pix = n_items * spatial
+// without overflow, nor of n_pix * C), dtype and a configuration with kernels (*pow: the literal-pow ones).
+int cf_check(int64_t n_items, int64_t spatial, int C, int dtype, int flags, float alpha, float eps, int64_t* n_pix,
+             bool* pow) {
+  int64_t n = 0, elems = 0;
+  if (n_items < 0 || spatial < 0 || C <= 0)
+    return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_items=%lld spatial=%lld C=%d", (long long)n_items,
+                (long long)spatial, C);
+  if (__builtin_mul_overflow(n_items, spatial, &n) || __builtin_mul_overflow(n, (int64_t)C, &elems))
+    return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_items * spatial * C overflows (n_items=%lld spatial=%lld C=%d)",
+                (long long)n_items, (long long)spatial, C);
+  if (dtype < 0 || dtype > 2) return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: dtype must be 0, 1 or 2, got %d", dtype);
+  if (!gdn_tc_cf_config(C, dtype, flags, alpha, eps, pow))
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for C=%d dtype=%d flags=%d alpha=%g epsilon=%g "
+                "(float32 at C = 128, 192, 256, 320; 16 bits at C = 128, 192 with alpha in {1, 2}, epsilon in {1, 1/2}; "
+                "not under TFCB_GDN_FP32=1): transpose to channels-last for this configuration",
+                C, dtype, flags, (double)alpha, (double)eps);
+  *n_pix = n;
+  return TFCB_OK;
+}
+
+bool unaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+}  // namespace
 
 namespace {
 
@@ -730,6 +764,80 @@ int tfcb_gdn_backward_exponents(const float* x_dev, const float* gamma_dev, cons
                              flags, alpha, epsilon, stream));
   return tfcb_gdn_exponent_grads(x_dev, gamma_dev, beta_dev, dy_dev, dalpha_depsilon_dev, exp_ws, n_pix, C, flags,
                                  alpha, epsilon, stream);
+}
+
+int tfcb_gdn_forward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, void* y_dev, int64_t n_items,
+                        int64_t spatial, int C, int dtype, int flags, float alpha, float epsilon, void* stream) {
+  int64_t n_pix = 0;
+  bool pow = false;
+  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &pow));
+  if (!gamma_dev || !beta_dev || (n_pix > 0 && (!x_dev || !y_dev))) return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  if (unaligned16(x_dev) || unaligned16(y_dev) || unaligned16(beta_dev))
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: x, y and beta must be 16-byte aligned");
+  if (n_pix == 0) return TFCB_OK;
+  TFCB_TRY(gdn_tc_forward_cf(x_dev, gamma_dev, beta_dev, y_dev, n_pix, spatial, C, flags, alpha, epsilon, dtype,
+                             as_stream(stream)));
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+// 16 bits: tfcb_gdn_backward_16bit's workspace (q, the partials, the dx kernel's direct-term scratch); float32:
+// tfcb_gdn_backward_exponents' (q, the partials, the exponent partials) followed by the same scratch, which the
+// channels-first float32 dx kernel uses too.  -1 for arguments the entries reject.
+int64_t tfcb_gdn_backward_cf_workspace_bytes(int64_t n_items, int64_t spatial, int C, int dtype) {
+  int64_t n_pix = 0, elems = 0;
+  if (n_items < 0 || spatial < 0 || C <= 0 || dtype < 0 || dtype > 2 ||
+      __builtin_mul_overflow(n_items, spatial, &n_pix) || __builtin_mul_overflow(n_pix, (int64_t)C, &elems))
+    return -1;
+  return dtype == 0 ? tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C) +
+                          (int64_t)gdn_tc_backward16_scratch_floats(n_pix, C) * (int64_t)sizeof(float)
+                    : tfcb_gdn_backward_16bit_workspace_bytes(n_pix, C);
+}
+
+int tfcb_gdn_backward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, const void* dy_dev,
+                         void* dx_dev, float* dgamma_dev, float* dbeta_dev, float* dalpha_depsilon_dev,
+                         void* workspace_dev, int64_t n_items, int64_t spatial, int C, int dtype, int flags,
+                         float alpha, float epsilon, void* stream) {
+  int64_t n_pix = 0;
+  bool pow = false;
+  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &pow));
+  const bool want_e = (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) != 0;
+  if (!gamma_dev || !beta_dev || !dgamma_dev || !dbeta_dev || !workspace_dev || (want_e && !dalpha_depsilon_dev) ||
+      (n_pix > 0 && (!x_dev || !dy_dev || !dx_dev)))
+    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  if (dalpha_depsilon_dev && !pow)
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: dalpha_depsilon_dev must be NULL when alpha and epsilon are "
+                "fixed at the shortcut values (alpha in {1, 2}, epsilon in {1, 1/2})");
+  if (unaligned16(x_dev) || unaligned16(dy_dev) || unaligned16(dx_dev) || unaligned16(beta_dev) ||
+      unaligned16(workspace_dev))
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: x, dy, dx, beta and the workspace must be 16-byte aligned");
+  cudaStream_t s = as_stream(stream);
+  if (n_pix == 0) {  // as tfcb_gdn_backward: no kernel, the gradients are the empty sums
+    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
+    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
+    if (dalpha_depsilon_dev) TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon_dev, 0, 2 * sizeof(float), s));
+    return TFCB_OK;
+  }
+  // the channels-last entries' workspace layouts: q, the partials, then the 16-bit dx kernel's scratch (16 bits) or
+  // the exponent partials and the scratch (float32)
+  uint8_t* ws = static_cast<uint8_t*>(workspace_dev);
+  float* q = reinterpret_cast<float*>(ws);
+  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
+  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
+  float* part_e = reinterpret_cast<float*>(ws + tfcb_gdn_backward_workspace_bytes(n_pix, C));
+  float* scratch = dtype == 0 ? reinterpret_cast<float*>(ws + tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C))
+                              : part_b + (size_t)kDgammaGrid * C;
+  int n_parts = 0, n_parts_e = 0;
+  TFCB_TRY(gdn_tc_backward_cf(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b, scratch,
+                              dalpha_depsilon_dev ? part_e : nullptr, &n_parts, &n_parts_e, n_pix, spatial, C, flags,
+                              alpha, epsilon, dtype, s));
+  reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
+  if (dalpha_depsilon_dev) {
+    reduce_partials_kernel<<<1, 32, 0, s>>>(part_e, n_parts_e, 2, dalpha_depsilon_dev);
+    TFCB_LAUNCHED();
+  }
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
 }
 
 }  // extern "C"

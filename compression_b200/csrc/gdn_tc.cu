@@ -313,6 +313,89 @@ __device__ __forceinline__ void st_pair(void* base, long long idx, float a, floa
   *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(base) + idx) = w;
 }
 
+// Layout of the activations x, y, dy and dx.  Channels-last (CF = false): element (pixel r, channel c) at r * C + c.
+// Channels-first (CF = true, [N, C, S] with S the product of the spatial dimensions): pixel r of the flattened
+// [N * S] order is position r % S of item r / S, and its channel c lives at (r / S) * C * S + c * S + r % S.  A row's
+// base (its channel 0) takes the one division; channel c is then at base + ch_off(c).  Tiles run over the flattened
+// pixel order either way (a tile may span two items), and q, the 16-bit scratch and the partials stay channels-last,
+// so the channels-first kernels compute every value exactly as the channels-last kernels do on the transposed tensor.
+template <bool CF>
+__device__ __forceinline__ long long row_base(long long r, int C, long long S) {
+  if constexpr (CF) {
+    const long long item = r / S;
+    return item * C * S + (r - item * S);
+  } else {
+    return r * C;
+  }
+}
+
+template <bool CF>
+__device__ __forceinline__ long long ch_off(int c, long long S) {
+  if constexpr (CF) return (long long)c * S;
+  else return c;
+}
+
+// The index of channel c of the row at `base` in layout CF, given the channels-last index `cl` of the same element:
+// channels-last code keeps its own index expressions (and its instructions).
+template <bool CF>
+__device__ __forceinline__ long long cf_idx(long long cl, long long base, int c, long long S) {
+  if constexpr (CF) return base + (long long)c * S;
+  else return cl;
+}
+
+template <int IO>
+__device__ __forceinline__ float ld_one(const void* base, long long idx) {
+  if (IO == 0) return __ldg(static_cast<const float*>(base) + idx);
+  const unsigned short w = __ldg(static_cast<const unsigned short*>(base) + idx);
+  if (IO == 2) return __uint_as_float((uint32_t)w << 16);
+  return __half2float(__ushort_as_half(w));
+}
+
+// One element, rounded to nearest as st_pair's paired conversions round each of theirs.
+template <int IO>
+__device__ __forceinline__ void st_one(void* base, long long idx, float v) {
+  if (IO == 0) {
+    static_cast<float*>(base)[idx] = v;
+    return;
+  }
+  static_cast<unsigned short*>(base)[idx] =
+      IO == 2 ? __bfloat16_as_ushort(__float2bfloat16_rn(v)) : __half_as_ushort(__float2half_rn(v));
+}
+
+// Channels c, c + 1 of one pixel at idx = row_base + ch_off(c): one access channels-last, two channels-first.
+template <int IO, bool CF>
+__device__ __forceinline__ float2 ld_px(const void* base, long long idx, long long S) {
+  if constexpr (CF) return make_float2(ld_one<IO>(base, idx), ld_one<IO>(base, idx + S));
+  else return ld_pair<IO>(base, idx);
+}
+
+template <int IO, bool CF>
+__device__ __forceinline__ void st_px(void* base, long long idx, long long S, float a, float b) {
+  if constexpr (CF) {
+    st_one<IO>(base, idx, a);
+    st_one<IO>(base, idx + S, b);
+  } else {
+    st_pair<IO>(base, idx, a, b);
+  }
+}
+
+// float32 dx written, and read back in the kernel that wrote it (no read-only cache).
+template <bool CF>
+__device__ __forceinline__ float2 ld_px_rw(const float* base, long long idx, long long S) {
+  if constexpr (CF) return make_float2(base[idx], base[idx + S]);
+  else return *reinterpret_cast<const float2*>(base + idx);
+}
+
+template <bool CF>
+__device__ __forceinline__ void st_px_f2(float* base, long long idx, long long S, float2 v) {
+  if constexpr (CF) {
+    base[idx] = v.x;
+    base[idx + S] = v.y;
+  } else {
+    *reinterpret_cast<float2*>(base + idx) = v;
+  }
+}
+
 template <int C>
 struct TcCfg {
   static constexpr int kWG = C == 128 ? 3 : 2;  // warpgroups per CTA: as many as the registers allow
@@ -340,17 +423,20 @@ __device__ __forceinline__ void fill_planes(const float* __restrict__ gamma, uin
 }
 
 // A fragments of pool(x) for one tile: k-step kk covers channels 16 kk .. 16 kk + 15; register r of a step holds
-// (row g, cols c, c+1), (row g+8, c, c+1), (row g, c+8, c+9), (row g+8, c+8, c+9), c = 16 kk + 2 t.
-template <int C, bool FAST, int IO, class F>
-__device__ __forceinline__ void pool_frags(const void* __restrict__ x, long long r0, long long r1, bool ok0, bool ok1,
-                                           int t, const F& f, uint32_t (&ah)[C / 16][4],
-                                           uint32_t (&al)[C / 16][4]) {
+// (row g, cols c, c+1), (row g+8, c, c+1), (row g, c+8, c+9), (row g+8, c+8, c+9), c = 16 kk + 2 t.  b0, b1: the
+// row bases (row_base) of rows r0, r1 in layout CF.
+template <int C, bool FAST, int IO, bool CF, class F>
+__device__ __forceinline__ void pool_frags(const void* __restrict__ x, long long r0, long long r1, long long b0,
+                                           long long b1, long long S, bool ok0, bool ok1, int t, const F& f,
+                                           uint32_t (&ah)[C / 16][4], uint32_t (&al)[C / 16][4]) {
 #pragma unroll
   for (int kk = 0; kk < C / 16; ++kk) {
     const int c = 16 * kk + 2 * t;
     const float2 z = make_float2(0.f, 0.f);
-    const float2 v[4] = {ok0 ? ld_pair<IO>(x, r0 * C + c) : z, ok1 ? ld_pair<IO>(x, r1 * C + c) : z,
-                         ok0 ? ld_pair<IO>(x, r0 * C + c + 8) : z, ok1 ? ld_pair<IO>(x, r1 * C + c + 8) : z};
+    const float2 v[4] = {ok0 ? ld_px<IO, CF>(x, cf_idx<CF>(r0 * C + c, b0, c, S), S) : z,
+                         ok1 ? ld_px<IO, CF>(x, cf_idx<CF>(r1 * C + c, b1, c, S), S) : z,
+                         ok0 ? ld_px<IO, CF>(x, cf_idx<CF>(r0 * C + c + 8, b0, c + 8, S), S) : z,
+                         ok1 ? ld_px<IO, CF>(x, cf_idx<CF>(r1 * C + c + 8, b1, c + 8, S), S) : z};
 #pragma unroll
     for (int r = 0; r < 4; ++r) split2(tc_pool<FAST>(v[r].x, f), tc_pool<FAST>(v[r].y, f), &ah[kk][r], &al[kk][r]);
   }
@@ -391,10 +477,12 @@ __device__ __forceinline__ void gemm3(float (&acc)[C / 64][32], const uint32_t (
 
 // The kernels' bodies take the flags type F: TcFlags for the fixed-exponent kernels, TcPowFlags for the literal-pow
 // kernels (float32 I/O, FAST = false), which are named gdn_tc_pow_*.
-template <int C, bool FAST, int IO, class F>
+// The kernels take the activations' layout CF (row_base) and S, the item size of the channels-first layout (unused
+// channels-last).
+template <int C, bool FAST, int IO, bool CF, class F>
 __device__ __forceinline__ void tc_fwd_body(const void* __restrict__ x, const float* __restrict__ gamma,
                                             const float* __restrict__ beta, void* __restrict__ y, long long n_pix,
-                                            const F& f) {
+                                            const F& f, long long S) {
   using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   fill_planes<C>(gamma, smem);
@@ -404,8 +492,9 @@ __device__ __forceinline__ void tc_fwd_body(const void* __restrict__ x, const fl
   for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     uint32_t ah[C / 16][4], al[C / 16][4];
-    pool_frags<C, FAST, IO>(x, r0, r1, ok0, ok1, t, f, ah, al);
+    pool_frags<C, FAST, IO, CF>(x, r0, r1, b0, b1, S, ok0, ok1, t, f, ah, al);
     float acc[C / 64][32];
     gemm3<C, 0>(acc, ah, al, bh, bl);
     // accumulators are read on every thread (only the memory accesses are predicated): a read inside a divergent
@@ -413,28 +502,28 @@ __device__ __forceinline__ void tc_fwd_body(const void* __restrict__ x, const fl
     TFCB_FOR_ACC_PAIRS(C) {
       const bool ok = h ? ok1 : ok0;
       const int col = 64 * n + 8 * jj + 2 * t;
-      const long long idx = (h ? r1 : r0) * C + col;
-      const float2 xv = ok ? ld_pair<IO>(x, idx) : make_float2(0.f, 0.f);
+      const long long idx = cf_idx<CF>((h ? r1 : r0) * C + col, h ? b1 : b0, col, S);
+      const float2 xv = ok ? ld_px<IO, CF>(x, idx, S) : make_float2(0.f, 0.f);
       const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
       const float y0 = tc_out<FAST>(xv.x, b.x + acc[n][4 * jj + 2 * h], f);
       const float y1 = tc_out<FAST>(xv.y, b.y + acc[n][4 * jj + 2 * h + 1], f);
-      if (ok) st_pair<IO>(y, idx, y0, y1);
+      if (ok) st_px<IO, CF>(y, idx, S, y0, y1);
     }
   }
 }
 
-template <int C, bool FAST, int IO>
+template <int C, bool FAST, int IO, bool CF>
 __global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
 gdn_tc_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                  void* __restrict__ y, long long n_pix, TcFlags f) {
-  tc_fwd_body<C, FAST, IO>(x, gamma, beta, y, n_pix, f);
+                  void* __restrict__ y, long long n_pix, TcFlags f, long long S) {
+  tc_fwd_body<C, FAST, IO, CF>(x, gamma, beta, y, n_pix, f, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
 gdn_tc_pow_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                      void* __restrict__ y, long long n_pix, TcPowFlags f) {
-  tc_fwd_body<C, false, 0>(x, gamma, beta, y, n_pix, f);
+                      void* __restrict__ y, long long n_pix, TcPowFlags f, long long S) {
+  tc_fwd_body<C, false, 0, CF>(x, gamma, beta, y, n_pix, f, S);
 }
 
 // Backward, part 1: per 64-pixel tile
@@ -446,12 +535,14 @@ gdn_tc_pow_fwd_kernel(const void* __restrict__ x, const float* __restrict__ gamm
 // to the warpgroup's own 64 x C float32 tile of `scratch` instead, and dx is stored once, rounded once: the result is
 // the float32 kernel's on the widened inputs, rounded to the activation type.  No register can hold it through MMA2
 // (the C = 192 FAST variant is at the 255-register limit) and no shared memory is left beside gamma's planes at C = 192.
+// Channels-first (CF) float32 keeps the direct term in the scratch as well, so dx is only written: storing it in dx
+// and reading it back would keep a second strided address per pair alive across MMA2, and those kernels spilled.
 // The literal-pow variant also sums dL/depsilon in the first epilogue and dL/dalpha in the second, one partial per CTA.
-template <int C, bool FAST, int IO, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const float* __restrict__ gamma,
                                                const float* __restrict__ beta, const void* __restrict__ dy,
                                                void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                                               const F& f, float* __restrict__ scratch) {
+                                               const F& f, float* __restrict__ scratch, long long S) {
   using K = TcCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   fill_planes<C>(gamma, smem);
@@ -465,8 +556,9 @@ __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const
   for (long long tile = (long long)blockIdx.x * K::kWG + wg; tile < n_tiles; tile += (long long)gridDim.x * K::kWG) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     uint32_t ah[C / 16][4], al[C / 16][4];
-    pool_frags<C, FAST, IO>(x, r0, r1, ok0, ok1, t, f, ah, al);
+    pool_frags<C, FAST, IO, CF>(x, r0, r1, b0, b1, S, ok0, ok1, t, f, ah, al);
     float acc[C / 64][32];
     gemm3<C, 0>(acc, ah, al, bh, bl);
     TFCB_FOR_ACC_PAIRS(C) {
@@ -476,16 +568,17 @@ __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const
         continue;
       }
       const int col = 64 * n + 8 * jj + 2 * t;
-      const long long idx = (h ? r1 : r0) * C + col;
-      const float2 xv = ld_pair<IO>(x, idx);
-      const float2 gv = ld_pair<IO>(dy, idx);
+      const long long idx = (h ? r1 : r0) * C + col;                // q (channels-last)
+      const long long gi = cf_idx<CF>(idx, h ? b1 : b0, col, S);  // x, dy, dx
+      const float2 xv = ld_px<IO, CF>(x, gi, S);
+      const float2 gv = ld_px<IO, CF>(dy, gi, S);
       const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
       float2 q, d;
       tc_bwd_point<FAST>(xv.x, gv.x, b.x + a[0], f, &q.x, &d.x);
       tc_bwd_point<FAST>(xv.y, gv.y, b.y + a[1], f, &q.y, &d.y);
       if constexpr (kPow<F>) dep += tc_deps_term(q.x, b.x + a[0], f) + tc_deps_term(q.y, b.y + a[1], f);
       *reinterpret_cast<float2*>(q_ws + idx) = q;
-      if constexpr (IO == 0)
+      if constexpr (IO == 0 && !CF)
         *reinterpret_cast<float2*>(static_cast<float*>(dx) + idx) = d;
       else
         *reinterpret_cast<float2*>(dtile + 8 * h * C + 64 * n + 8 * jj) = d;
@@ -502,10 +595,11 @@ __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const
     gemm3<C, 1>(acc, ah, al, bh, bl);
     TFCB_FOR_ACC_PAIRS(C) {
       if (!(h ? ok1 : ok0)) continue;
-      const long long idx = (h ? r1 : r0) * C + 64 * n + 8 * jj + 2 * t;
-      const float2 xv = ld_pair<IO>(x, idx);
+      const long long idx = cf_idx<CF>((h ? r1 : r0) * C + 64 * n + 8 * jj + 2 * t, h ? b1 : b0,
+                                       64 * n + 8 * jj + 2 * t, S);
+      const float2 xv = ld_px<IO, CF>(x, idx, S);
       float2 d;
-      if constexpr (IO == 0)
+      if constexpr (IO == 0 && !CF)
         d = *reinterpret_cast<const float2*>(static_cast<const float*>(dx) + idx);
       else
         d = *reinterpret_cast<const float2*>(dtile + 8 * h * C + 64 * n + 8 * jj);
@@ -517,7 +611,7 @@ __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const
         if (!(xv.x > 0.f)) d.x = 0.f;
         if (!(xv.y > 0.f)) d.y = 0.f;
       }
-      st_pair<IO>(dx, idx, d.x, d.y);
+      st_px<IO, CF>(dx, idx, S, d.x, d.y);
     }
   }
   if constexpr (kPow<F>) {
@@ -525,20 +619,20 @@ __device__ __forceinline__ void tc_bwd_dx_body(const void* __restrict__ x, const
   }
 }
 
-template <int C, bool FAST, int IO>
+template <int C, bool FAST, int IO, bool CF>
 __global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
 gdn_tc_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                      const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                     TcFlags f, float* __restrict__ scratch) {
-  tc_bwd_dx_body<C, FAST, IO>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
+                     TcFlags f, float* __restrict__ scratch, long long S) {
+  tc_bwd_dx_body<C, FAST, IO, CF>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(TcCfg<C>::kThreads, 1)
 gdn_tc_pow_bwd_dx_kernel(const void* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                          const void* __restrict__ dy, void* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                         TcPowFlags f, float* __restrict__ scratch) {
-  tc_bwd_dx_body<C, false, 0>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
+                         TcPowFlags f, float* __restrict__ scratch, long long S) {
+  tc_bwd_dx_body<C, false, 0, CF>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch, S);
 }
 
 // Backward, part 2: per-CTA partials dgamma[j, i] = sum_pix p[pix, j] q[pix, i] and dbeta[i] = sum_pix q[pix, i].
@@ -563,10 +657,10 @@ constexpr int kDgFlush = 8;
 template <int IO>
 using IoElem = std::conditional_t<IO == 0, float, uint16_t>;
 
-template <int C, bool FAST, int IO, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 __device__ __forceinline__ void tc_dgamma_body(const IoElem<IO>* __restrict__ x, const float* __restrict__ q,
                                                float* __restrict__ part_g, float* __restrict__ part_b, long long n_pix,
-                                               const F& f) {
+                                               const F& f, long long S) {
   using L = DgCfg<C>;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
@@ -584,7 +678,14 @@ __device__ __forceinline__ void tc_dgamma_body(const IoElem<IO>* __restrict__ x,
       const long long row = chunk * kTileM + p;
       float v[8], w[8];
       if (row < n_pix) {
-        if constexpr (IO == 0) {
+        if constexpr (CF) {  // 8 element loads, one per channel; 16 lanes read 16 consecutive pixels of each
+          const long long xb = row_base<true>(row, C, S) + ch_off<true>(8 * jc, S);
+          const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
+          const float4 q0 = __ldg(qr), q1 = __ldg(qr + 1);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = ld_one<IO>(x, xb + e * S);
+          w[0] = q0.x, w[1] = q0.y, w[2] = q0.z, w[3] = q0.w, w[4] = q1.x, w[5] = q1.y, w[6] = q1.z, w[7] = q1.w;
+        } else if constexpr (IO == 0) {
           const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
           const float4* qr = reinterpret_cast<const float4*>(q + row * C + 8 * jc);
           const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1), q0 = __ldg(qr), q1 = __ldg(qr + 1);
@@ -680,18 +781,18 @@ __device__ __forceinline__ void tc_dgamma_body(const IoElem<IO>* __restrict__ x,
   }
 }
 
-template <int C, bool FAST, int IO>
+template <int C, bool FAST, int IO, bool CF>
 __global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
 gdn_tc_dgamma_kernel(const IoElem<IO>* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                     float* __restrict__ part_b, long long n_pix, TcFlags f) {
-  tc_dgamma_body<C, FAST, IO>(x, q, part_g, part_b, n_pix, f);
+                     float* __restrict__ part_b, long long n_pix, TcFlags f, long long S) {
+  tc_dgamma_body<C, FAST, IO, CF>(x, q, part_g, part_b, n_pix, f, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(DgCfg<C>::kThreads, 1)
 gdn_tc_pow_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                         float* __restrict__ part_b, long long n_pix, TcPowFlags f) {
-  tc_dgamma_body<C, false, 0>(x, q, part_g, part_b, n_pix, f);
+                         float* __restrict__ part_b, long long n_pix, TcPowFlags f, long long S) {
+  tc_dgamma_body<C, false, 0, CF>(x, q, part_g, part_b, n_pix, f, S);
 }
 
 // ---- Wide layers, C in {256, 320}: the work is split over blocks of NB output columns ----
@@ -738,18 +839,20 @@ __device__ __forceinline__ void fill_planes_block(const float* __restrict__ gamm
   __syncthreads();
 }
 
-// A fragments of channels [16 k0, 16 k0 + KA) of a tile of a [n_pix, C] array, at the positions pool_frags uses:
-// pool(x) (POOL) or the values themselves (q).
-template <int C, int KA, bool POOL, bool FAST, class F>
-__device__ __forceinline__ void slice_frags(const float* __restrict__ src, long long r0, long long r1, bool ok0,
-                                            bool ok1, int t, int k0, const F& f, uint32_t (&ah)[KA / 16][4],
-                                            uint32_t (&al)[KA / 16][4]) {
+// A fragments of channels [16 k0, 16 k0 + KA) of a tile of a [n_pix, C] array in layout CF (row bases b0, b1), at
+// the positions pool_frags uses: pool(x) (POOL) or the values themselves (q, always channels-last).
+template <int C, int KA, bool POOL, bool FAST, bool CF, class F>
+__device__ __forceinline__ void slice_frags(const float* __restrict__ src, long long r0, long long r1, long long b0,
+                                            long long b1, long long S, bool ok0, bool ok1, int t, int k0, const F& f,
+                                            uint32_t (&ah)[KA / 16][4], uint32_t (&al)[KA / 16][4]) {
 #pragma unroll
   for (int kk = 0; kk < KA / 16; ++kk) {
     const int c = 16 * (k0 + kk) + 2 * t;
     const float2 z = make_float2(0.f, 0.f);
-    const float2 v[4] = {ok0 ? ld_pair<0>(src, r0 * C + c) : z, ok1 ? ld_pair<0>(src, r1 * C + c) : z,
-                         ok0 ? ld_pair<0>(src, r0 * C + c + 8) : z, ok1 ? ld_pair<0>(src, r1 * C + c + 8) : z};
+    const float2 v[4] = {ok0 ? ld_px<0, CF>(src, cf_idx<CF>(r0 * C + c, b0, c, S), S) : z,
+                         ok1 ? ld_px<0, CF>(src, cf_idx<CF>(r1 * C + c, b1, c, S), S) : z,
+                         ok0 ? ld_px<0, CF>(src, cf_idx<CF>(r0 * C + c + 8, b0, c + 8, S), S) : z,
+                         ok1 ? ld_px<0, CF>(src, cf_idx<CF>(r1 * C + c + 8, b1, c + 8, S), S) : z};
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
       if (POOL)
@@ -767,10 +870,10 @@ __device__ __forceinline__ void slice_frags(const float* __restrict__ src, long 
 // K is walked in kKSlices slices, each loaded into registers, multiplied and waited for before the next is loaded:
 // at C = 320 the A fragments of all K (160 registers) next to the accumulators leave ptxas too few registers to
 // avoid spills.  Otherwise gemm3 with the plane extents of one block.
-template <int C, int TB, bool POOL, bool FAST, class F>
+template <int C, int TB, bool POOL, bool FAST, bool CF, class F>
 __device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32], const float* __restrict__ src,
-                                          long long r0, long long r1, bool ok0, bool ok1, int t, const F& f,
-                                          uint32_t bh, uint32_t bl) {
+                                          long long r0, long long r1, long long b0, long long b1, long long S,
+                                          bool ok0, bool ok1, int t, const F& f, uint32_t bh, uint32_t bl) {
   constexpr int NB = WideCfg<C>::kNB, KA = C / WideCfg<C>::kKSlices;
 #pragma unroll
   for (int n = 0; n < NB / 64; ++n)
@@ -782,7 +885,7 @@ __device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32]
 #pragma unroll
   for (int s = 0; s < WideCfg<C>::kKSlices; ++s) {
     uint32_t ah[KA / 16][4], al[KA / 16][4];
-    slice_frags<C, KA, POOL, FAST>(src, r0, r1, ok0, ok1, t, s * KA / 16, f, ah, al);
+    slice_frags<C, KA, POOL, FAST, CF>(src, r0, r1, b0, b1, S, ok0, ok1, t, s * KA / 16, f, ah, al);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < KA / 16; ++kk)
@@ -800,10 +903,10 @@ __device__ __forceinline__ void wide_gemm(float (&acc)[WideCfg<C>::kNB / 64][32]
   }
 }
 
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 __device__ __forceinline__ void tc_wide_fwd_body(const float* __restrict__ x, const float* __restrict__ gamma,
                                                  const float* __restrict__ beta, float* __restrict__ y,
-                                                 long long n_pix, const F& f) {
+                                                 long long n_pix, const F& f, long long S) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -816,42 +919,44 @@ __device__ __forceinline__ void tc_wide_fwd_body(const float* __restrict__ x, co
   for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     float acc[NB / 64][32];
-    wide_gemm<C, 0, true, FAST>(acc, x, r0, r1, ok0, ok1, t, f, bh, bl);
+    wide_gemm<C, 0, true, FAST, CF>(acc, x, r0, r1, b0, b1, S, ok0, ok1, t, f, bh, bl);
     TFCB_FOR_ACC_PAIRS(NB) {
       const bool ok = h ? ok1 : ok0;
       const int col = c0 + 64 * n + 8 * jj + 2 * t;
-      const long long idx = (h ? r1 : r0) * C + col;
-      const float2 xv = ok ? ld_pair<0>(x, idx) : make_float2(0.f, 0.f);
+      const long long idx = cf_idx<CF>((h ? r1 : r0) * C + col, h ? b1 : b0, col, S);
+      const float2 xv = ok ? ld_px<0, CF>(x, idx, S) : make_float2(0.f, 0.f);
       const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
       const float y0 = tc_out<FAST>(xv.x, b.x + acc[n][4 * jj + 2 * h], f);
       const float y1 = tc_out<FAST>(xv.y, b.y + acc[n][4 * jj + 2 * h + 1], f);
-      if (ok) st_pair<0>(y, idx, y0, y1);
+      if (ok) st_px<0, CF>(y, idx, S, y0, y1);
     }
   }
 }
 
-template <int C, bool FAST>
+template <int C, bool FAST, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                       float* __restrict__ y, long long n_pix, TcFlags f) {
-  tc_wide_fwd_body<C, FAST>(x, gamma, beta, y, n_pix, f);
+                       float* __restrict__ y, long long n_pix, TcFlags f, long long S) {
+  tc_wide_fwd_body<C, FAST, CF>(x, gamma, beta, y, n_pix, f, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_pow_wide_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
-                           const float* __restrict__ beta, float* __restrict__ y, long long n_pix, TcPowFlags f) {
-  tc_wide_fwd_body<C, false>(x, gamma, beta, y, n_pix, f);
+                           const float* __restrict__ beta, float* __restrict__ y, long long n_pix, TcPowFlags f,
+                           long long S) {
+  tc_wide_fwd_body<C, false, CF>(x, gamma, beta, y, n_pix, f, S);
 }
 
 // Backward, pass 1: n[:, block] = beta + p . gamma[:, block]  ->  q[:, block] (workspace), dx[:, block] = direct term.
 // The literal-pow variant also sums dL/depsilon over the block's columns: partial [blockIdx.x][1].
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 __device__ __forceinline__ void tc_wide_bwd_q_body(const float* __restrict__ x, const float* __restrict__ gamma,
                                                    const float* __restrict__ beta, const float* __restrict__ dy,
                                                    float* __restrict__ dx, float* __restrict__ q_ws, long long n_pix,
-                                                   const F& f) {
+                                                   const F& f, long long S) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -865,14 +970,16 @@ __device__ __forceinline__ void tc_wide_bwd_q_body(const float* __restrict__ x, 
   for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     float acc[NB / 64][32];
-    wide_gemm<C, 0, true, FAST>(acc, x, r0, r1, ok0, ok1, t, f, bh, bl);
+    wide_gemm<C, 0, true, FAST, CF>(acc, x, r0, r1, b0, b1, S, ok0, ok1, t, f, bh, bl);
     TFCB_FOR_ACC_PAIRS(NB) {
       const bool ok = h ? ok1 : ok0;
       const int col = c0 + 64 * n + 8 * jj + 2 * t;
-      const long long idx = (h ? r1 : r0) * C + col;
-      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
-      const float2 gv = ok ? __ldg(reinterpret_cast<const float2*>(dy + idx)) : make_float2(0.f, 0.f);
+      const long long idx = (h ? r1 : r0) * C + col;                // q (channels-last)
+      const long long gi = cf_idx<CF>(idx, h ? b1 : b0, col, S);  // x, dy, dx
+      const float2 xv = ok ? ld_px<0, CF>(x, gi, S) : make_float2(0.f, 0.f);
+      const float2 gv = ok ? ld_px<0, CF>(dy, gi, S) : make_float2(0.f, 0.f);
       const float2 b = __ldg(reinterpret_cast<const float2*>(beta + col));
       float2 qv, d;
       tc_bwd_point<FAST>(xv.x, gv.x, b.x + acc[n][4 * jj + 2 * h], f, &qv.x, &d.x);
@@ -884,7 +991,7 @@ __device__ __forceinline__ void tc_wide_bwd_q_body(const float* __restrict__ x, 
       }
       if (ok) {
         *reinterpret_cast<float2*>(q_ws + idx) = qv;
-        *reinterpret_cast<float2*>(dx + idx) = d;
+        st_px_f2<CF>(dx, gi, S, d);
       }
     }
   }
@@ -893,27 +1000,41 @@ __device__ __forceinline__ void tc_wide_bwd_q_body(const float* __restrict__ x, 
   }
 }
 
-template <int C, bool FAST>
+template <int C, bool FAST, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                          const float* __restrict__ dy, float* __restrict__ dx, float* __restrict__ q_ws,
-                         long long n_pix, TcFlags f) {
-  tc_wide_bwd_q_body<C, FAST>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+                         long long n_pix, TcFlags f, long long S) {
+  tc_wide_bwd_q_body<C, FAST, CF>(x, gamma, beta, dy, dx, q_ws, n_pix, f, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_pow_wide_bwd_q_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                              const float* __restrict__ beta, const float* __restrict__ dy, float* __restrict__ dx,
-                             float* __restrict__ q_ws, long long n_pix, TcPowFlags f) {
-  tc_wide_bwd_q_body<C, false>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+                             float* __restrict__ q_ws, long long n_pix, TcPowFlags f, long long S) {
+  tc_wide_bwd_q_body<C, false, CF>(x, gamma, beta, dy, dx, q_ws, n_pix, f, S);
 }
 
-// Backward, pass 2: dp[:, J] = q . gamma[J, :]^T  ->  dx[:, J] += dpool/dx * dp, then the rectifier's mask.
-template <int C, bool FAST>
+// Channels-first pass 2: pass 1's direct term in dx for columns c + 8 jj of rows r0, r1 (bases b0, b1), one 64-column
+// block, all loaded before the block's stores.  With runtime strides the compiler cannot move a load above an earlier
+// pair's store, and one memory round trip per pair made the kernel latency bound (2.8x the channels-last time).
+__device__ __forceinline__ void wide_dx_prefetch(const float* dx, long long b0, long long b1, long long S, bool ok0,
+                                                 bool ok1, int c, float2 (&dv)[8][2]) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      dv[jj][h] = (h ? ok1 : ok0) ? ld_px_rw<true>(dx, (h ? b1 : b0) + ch_off<true>(c + 8 * jj, S), S)
+                                  : make_float2(0.f, 0.f);
+}
+
+// Backward, pass 2: dp[:, J] = q . gamma[J, :]^T  ->  dx[:, J] += dpool/dx * dp, then the rectifier's mask.  q is
+// channels-last in either layout; x and dx are in layout CF.
+template <int C, bool FAST, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ q,
-                          float* __restrict__ dx, long long n_pix, TcFlags f) {
+                          float* __restrict__ dx, long long n_pix, TcFlags f, long long S) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -926,20 +1047,45 @@ gdn_tc_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__
   for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     float acc[NB / 64][32];
-    wide_gemm<C, 1, false, FAST>(acc, q, r0, r1, ok0, ok1, t, f, bh, bl);
-    TFCB_FOR_ACC_PAIRS(NB) {
-      const bool ok = h ? ok1 : ok0;
-      const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
-      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
-      float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
-      d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
-      d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
-      if (!FAST && f.rectify) {
-        if (!(xv.x > 0.f)) d.x = 0.f;
-        if (!(xv.y > 0.f)) d.y = 0.f;
+    wide_gemm<C, 1, false, FAST, false>(acc, q, r0, r1, r0 * C, r1 * C, S, ok0, ok1, t, f, bh, bl);
+    if constexpr (CF) {
+#pragma unroll
+      for (int n = 0; n < NB / 64; ++n) {
+        float2 dv[8][2];
+        wide_dx_prefetch(dx, b0, b1, S, ok0, ok1, j0 + 64 * n + 2 * t, dv);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const bool ok = h ? ok1 : ok0;
+            const long long idx = (h ? b1 : b0) + ch_off<true>(j0 + 64 * n + 8 * jj + 2 * t, S);
+            const float2 xv = ok ? ld_px<0, true>(x, idx, S) : make_float2(0.f, 0.f);
+            float2 d = dv[jj][h];
+            d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
+            d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
+            if (!FAST && f.rectify) {
+              if (!(xv.x > 0.f)) d.x = 0.f;
+              if (!(xv.y > 0.f)) d.y = 0.f;
+            }
+            if (ok) st_px_f2<true>(dx, idx, S, d);
+          }
       }
-      if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+    } else {
+      TFCB_FOR_ACC_PAIRS(NB) {
+        const bool ok = h ? ok1 : ok0;
+        const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
+        const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
+        float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
+        d.x += tc_dpool<FAST>(xv.x, f) * acc[n][4 * jj + 2 * h];
+        d.y += tc_dpool<FAST>(xv.y, f) * acc[n][4 * jj + 2 * h + 1];
+        if (!FAST && f.rectify) {
+          if (!(xv.x > 0.f)) d.x = 0.f;
+          if (!(xv.y > 0.f)) d.y = 0.f;
+        }
+        if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+      }
     }
   }
 }
@@ -947,10 +1093,11 @@ gdn_tc_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__
 // The literal-pow pass 2 also sums dL/dalpha over the block's rows: partial [blockIdx.x][0].  It is a copy of
 // gdn_tc_wide_bwd_dp_kernel rather than a shared inline body: routed through one, the fixed-exponent kernel's
 // instruction schedule changed.
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(WideCfg<C>::kThreads, 1)
 gdn_tc_pow_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
-                              const float* __restrict__ q, float* __restrict__ dx, long long n_pix, TcPowFlags f) {
+                              const float* __restrict__ q, float* __restrict__ dx, long long n_pix, TcPowFlags f,
+                              long long S) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -964,23 +1111,51 @@ gdn_tc_pow_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restri
   for (long long tile = (long long)(blockIdx.x / W::kBlocks) * W::kWG + wg; tile < n_tiles; tile += stride) {
     const long long r0 = tile * kTileM + warp * 16 + g, r1 = r0 + 8;
     const bool ok0 = r0 < n_pix, ok1 = r1 < n_pix;
+    const long long b0 = row_base<CF>(r0, C, S), b1 = row_base<CF>(r1, C, S);
     float acc[NB / 64][32];
-    wide_gemm<C, 1, false, false>(acc, q, r0, r1, ok0, ok1, t, f, bh, bl);
-    TFCB_FOR_ACC_PAIRS(NB) {
-      const bool ok = h ? ok1 : ok0;
-      const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
-      const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
-      float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
-      const float dp0 = acc[n][4 * jj + 2 * h], dp1 = acc[n][4 * jj + 2 * h + 1];
-      d.x += tc_dpool<false>(xv.x, f) * dp0;
-      d.y += tc_dpool<false>(xv.y, f) * dp1;
-      const float e = tc_dalpha_term(xv.x, dp0, f) + tc_dalpha_term(xv.y, dp1, f);
-      if (ok) dal += e;
-      if (f.rectify) {
-        if (!(xv.x > 0.f)) d.x = 0.f;
-        if (!(xv.y > 0.f)) d.y = 0.f;
+    wide_gemm<C, 1, false, false, false>(acc, q, r0, r1, r0 * C, r1 * C, S, ok0, ok1, t, f, bh, bl);
+    if constexpr (CF) {  // the dx read-backs of a 64-column block first, as in gdn_tc_wide_bwd_dp_kernel
+#pragma unroll
+      for (int n = 0; n < NB / 64; ++n) {
+        float2 dv[8][2];
+        wide_dx_prefetch(dx, b0, b1, S, ok0, ok1, j0 + 64 * n + 2 * t, dv);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const bool ok = h ? ok1 : ok0;
+            const long long idx = (h ? b1 : b0) + ch_off<true>(j0 + 64 * n + 8 * jj + 2 * t, S);
+            const float2 xv = ok ? ld_px<0, true>(x, idx, S) : make_float2(0.f, 0.f);
+            float2 d = dv[jj][h];
+            const float dp0 = acc[n][4 * jj + 2 * h], dp1 = acc[n][4 * jj + 2 * h + 1];
+            d.x += tc_dpool<false>(xv.x, f) * dp0;
+            d.y += tc_dpool<false>(xv.y, f) * dp1;
+            const float e = tc_dalpha_term(xv.x, dp0, f) + tc_dalpha_term(xv.y, dp1, f);
+            if (ok) dal += e;
+            if (f.rectify) {
+              if (!(xv.x > 0.f)) d.x = 0.f;
+              if (!(xv.y > 0.f)) d.y = 0.f;
+            }
+            if (ok) st_px_f2<true>(dx, idx, S, d);
+          }
       }
-      if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+    } else {
+      TFCB_FOR_ACC_PAIRS(NB) {
+        const bool ok = h ? ok1 : ok0;
+        const long long idx = (h ? r1 : r0) * C + j0 + 64 * n + 8 * jj + 2 * t;
+        const float2 xv = ok ? __ldg(reinterpret_cast<const float2*>(x + idx)) : make_float2(0.f, 0.f);
+        float2 d = ok ? *reinterpret_cast<const float2*>(dx + idx) : make_float2(0.f, 0.f);
+        const float dp0 = acc[n][4 * jj + 2 * h], dp1 = acc[n][4 * jj + 2 * h + 1];
+        d.x += tc_dpool<false>(xv.x, f) * dp0;
+        d.y += tc_dpool<false>(xv.y, f) * dp1;
+        const float e = tc_dalpha_term(xv.x, dp0, f) + tc_dalpha_term(xv.y, dp1, f);
+        if (ok) dal += e;
+        if (f.rectify) {
+          if (!(xv.x > 0.f)) d.x = 0.f;
+          if (!(xv.y > 0.f)) d.y = 0.f;
+        }
+        if (ok) *reinterpret_cast<float2*>(dx + idx) = d;
+      }
     }
   }
   if (f.part_e != nullptr) cta_exponent_partial<true, false>(dal, 0.f, smem, f.part_e + 2 * blockIdx.x);
@@ -990,10 +1165,10 @@ gdn_tc_pow_wide_bwd_dp_kernel(const float* __restrict__ x, const float* __restri
 // (part, block) adds into columns [c0, c0 + NB) of partial `part`, so the partials keep the [n_parts][C][C] layout.
 // Thread tid stages p channels 8 (tid / 16) .. + 7 of pixels tid % 16 + 16 s, and the same q channels of the block
 // when tid / 16 < NB / 8.
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 __device__ __forceinline__ void tc_wide_dgamma_body(const float* __restrict__ x, const float* __restrict__ q,
                                                     float* __restrict__ part_g, float* __restrict__ part_b,
-                                                    long long n_pix, const F& f) {
+                                                    long long n_pix, const F& f, long long S) {
   using W = WideCfg<C>;
   constexpr int NB = W::kNB;
   constexpr int kP = W::kDgPPlane, kQ = W::kDgQPlane;
@@ -1018,9 +1193,15 @@ __device__ __forceinline__ void tc_wide_dgamma_body(const float* __restrict__ x,
 #pragma unroll
       for (int e = 0; e < 8; ++e) v[e] = w[e] = 0.f;
       if (row < n_pix) {
-        const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
-        const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1);
-        v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
+        if constexpr (CF) {
+          const long long xb = row_base<true>(row, C, S) + ch_off<true>(8 * jc, S);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) v[e] = ld_one<0>(x, xb + e * S);
+        } else {
+          const float4* xr = reinterpret_cast<const float4*>(x + row * C + 8 * jc);
+          const float4 x0 = __ldg(xr), x1 = __ldg(xr + 1);
+          v[0] = x0.x, v[1] = x0.y, v[2] = x0.z, v[3] = x0.w, v[4] = x1.x, v[5] = x1.y, v[6] = x1.z, v[7] = x1.w;
+        }
         if (has_q) {
           const float4* qr = reinterpret_cast<const float4*>(q + row * C + c0 + 8 * jc);
           const float4 q0 = __ldg(qr), q1 = __ldg(qr + 1);
@@ -1108,18 +1289,18 @@ __device__ __forceinline__ void tc_wide_dgamma_body(const float* __restrict__ x,
   }
 }
 
-template <int C, bool FAST>
+template <int C, bool FAST, bool CF>
 __global__ void __launch_bounds__(2 * C, 1)
 gdn_tc_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                          float* __restrict__ part_b, long long n_pix, TcFlags f) {
-  tc_wide_dgamma_body<C, FAST>(x, q, part_g, part_b, n_pix, f);
+                          float* __restrict__ part_b, long long n_pix, TcFlags f, long long S) {
+  tc_wide_dgamma_body<C, FAST, CF>(x, q, part_g, part_b, n_pix, f, S);
 }
 
-template <int C>
+template <int C, bool CF>
 __global__ void __launch_bounds__(2 * C, 1)
 gdn_tc_pow_wide_dgamma_kernel(const float* __restrict__ x, const float* __restrict__ q, float* __restrict__ part_g,
-                              float* __restrict__ part_b, long long n_pix, TcPowFlags f) {
-  tc_wide_dgamma_body<C, false>(x, q, part_g, part_b, n_pix, f);
+                              float* __restrict__ part_b, long long n_pix, TcPowFlags f, long long S) {
+  tc_wide_dgamma_body<C, false, CF>(x, q, part_g, part_b, n_pix, f, S);
 }
 
 int sm_count_tc() {
@@ -1135,52 +1316,55 @@ int reserve_smem(Kern kernel, int bytes) {
   return TFCB_OK;
 }
 
-// The kernels of a configuration: gdn_tc_* for TcFlags, gdn_tc_pow_* (float32, FAST = false) for TcPowFlags.
-template <int C, bool FAST, int IO, class F>
+// The kernels of a configuration: gdn_tc_* for TcFlags, gdn_tc_pow_* (float32, FAST = false) for TcPowFlags, in the
+// activation layout CF.
+template <int C, bool FAST, int IO, bool CF, class F>
 auto fwd_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_fwd_kernel<C>;
-  else return gdn_tc_fwd_kernel<C, FAST, IO>;
+  if constexpr (kPow<F>) return gdn_tc_pow_fwd_kernel<C, CF>;
+  else return gdn_tc_fwd_kernel<C, FAST, IO, CF>;
 }
-template <int C, bool FAST, int IO, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 auto bwd_dx_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_bwd_dx_kernel<C>;
-  else return gdn_tc_bwd_dx_kernel<C, FAST, IO>;
+  if constexpr (kPow<F>) return gdn_tc_pow_bwd_dx_kernel<C, CF>;
+  else return gdn_tc_bwd_dx_kernel<C, FAST, IO, CF>;
 }
-template <int C, bool FAST, int IO, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 auto dgamma_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_dgamma_kernel<C>;
-  else return gdn_tc_dgamma_kernel<C, FAST, IO>;
+  if constexpr (kPow<F>) return gdn_tc_pow_dgamma_kernel<C, CF>;
+  else return gdn_tc_dgamma_kernel<C, FAST, IO, CF>;
 }
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 auto wide_fwd_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_wide_fwd_kernel<C>;
-  else return gdn_tc_wide_fwd_kernel<C, FAST>;
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_fwd_kernel<C, CF>;
+  else return gdn_tc_wide_fwd_kernel<C, FAST, CF>;
 }
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 auto wide_bwd_q_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_q_kernel<C>;
-  else return gdn_tc_wide_bwd_q_kernel<C, FAST>;
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_q_kernel<C, CF>;
+  else return gdn_tc_wide_bwd_q_kernel<C, FAST, CF>;
 }
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 auto wide_bwd_dp_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_dp_kernel<C>;
-  else return gdn_tc_wide_bwd_dp_kernel<C, FAST>;
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_bwd_dp_kernel<C, CF>;
+  else return gdn_tc_wide_bwd_dp_kernel<C, FAST, CF>;
 }
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF, class F>
 auto wide_dgamma_kernel() {
-  if constexpr (kPow<F>) return gdn_tc_pow_wide_dgamma_kernel<C>;
-  else return gdn_tc_wide_dgamma_kernel<C, FAST>;
+  if constexpr (kPow<F>) return gdn_tc_pow_wide_dgamma_kernel<C, CF>;
+  else return gdn_tc_wide_dgamma_kernel<C, FAST, CF>;
 }
 
-template <int C, bool FAST, int IO, class F>
+// The launchers take the layout CF and the channels-first item size S (1 channels-last); grids, partial counts and
+// everything else depend on n_pix only, so both layouts run the same CTAs over the same tiles.
+template <int C, bool FAST, int IO, bool CF = false, class F>
 int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, F f,
-                  cudaStream_t s) {
+                  cudaStream_t s, long long S = 1) {
   using K = TcCfg<C>;
-  const auto kern = fwd_kernel<C, FAST, IO, F>();
+  const auto kern = fwd_kernel<C, FAST, IO, CF, F>();
   TFCB_TRY(reserve_smem(kern, K::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sm_count_tc());
-  kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
+  kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f, S);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
@@ -1195,27 +1379,28 @@ long long bwd16_scratch_floats(long long n_pix) {
   return std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, kMaxParts) * K::kWG * kTileM * C;
 }
 
-// IO != 0: x, dy, dx in 16 bits and `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.  TcPowFlags: the dx
-// kernel's CTAs write f.part_e[CTA][2] (when not null), *n_parts_e of them (at most kMaxParts).
-template <int C, bool FAST, int IO, class F>
+// IO != 0: x, dy, dx in 16 bits.  IO != 0 or CF: `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.
+// TcPowFlags: the dx kernel's CTAs write f.part_e[CTA][2] (when not null), *n_parts_e of them (at most kMaxParts).
+template <int C, bool FAST, int IO, bool CF = false, class F>
 int launch_tc_bwd(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
                   float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, F f,
-                  cudaStream_t s, int* n_parts_e = nullptr) {
+                  cudaStream_t s, int* n_parts_e = nullptr, long long S = 1) {
   using K = TcCfg<C>;
   using L = DgCfg<C>;
-  const auto dx_kern = bwd_dx_kernel<C, FAST, IO, F>();
-  const auto dg_kern = dgamma_kernel<C, FAST, IO, F>();
+  const auto dx_kern = bwd_dx_kernel<C, FAST, IO, CF, F>();
+  const auto dg_kern = dgamma_kernel<C, FAST, IO, CF, F>();
   TFCB_TRY(reserve_smem(dx_kern, K::kSmem));
   TFCB_TRY(reserve_smem(dg_kern, L::kSmem));
   const int sms = sm_count_tc();
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   // dx does not depend on the grid (every tile is computed the same way by whichever CTA takes it)
-  const bool capped = IO != 0 || kPow<F>;
+  const bool capped = IO != 0 || CF || kPow<F>;
   const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, capped ? std::min(sms, kMaxParts) : sms);
-  dx_kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch);
+  dx_kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f, scratch, S);
   TFCB_LAUNCHED();
   const int grid_g = (int)std::min<long long>(n_tiles, std::min(sms, kMaxParts));
-  dg_kern<<<grid_g, L::kThreads, L::kSmem, s>>>(static_cast<const IoElem<IO>*>(x), q_ws, part_g, part_b, n_pix, f);
+  dg_kern<<<grid_g, L::kThreads, L::kSmem, s>>>(static_cast<const IoElem<IO>*>(x), q_ws, part_g, part_b, n_pix, f,
+                                                S);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   *n_parts = grid_g;
@@ -1231,15 +1416,15 @@ int wide_grid(long long n_tiles_per_group) {
   return (int)(std::min<long long>(n_tiles_per_group, groups) * W::kBlocks);
 }
 
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF = false, class F>
 int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, F f,
-                       cudaStream_t s) {
+                       cudaStream_t s, long long S = 1) {
   using W = WideCfg<C>;
-  const auto kern = wide_fwd_kernel<C, FAST, F>();
+  const auto kern = wide_fwd_kernel<C, FAST, CF, F>();
   TFCB_TRY(reserve_smem(kern, W::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
-  kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f);
+  kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f, S);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
@@ -1247,26 +1432,26 @@ int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, fl
 
 // TcPowFlags: CTA b of pass 1 writes f.part_e[b][1] and CTA b of pass 2 f.part_e[b][0] (when not null), *n_parts_e
 // partials (at most kMaxParts * kBlocks).
-template <int C, bool FAST, class F>
+template <int C, bool FAST, bool CF = false, class F>
 int launch_tc_wide_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
                        float* part_g, float* part_b, int* n_parts, long long n_pix, F f, cudaStream_t s,
-                       int* n_parts_e = nullptr) {
+                       int* n_parts_e = nullptr, long long S = 1) {
   using W = WideCfg<C>;
-  const auto q_kern = wide_bwd_q_kernel<C, FAST, F>();
-  const auto dp_kern = wide_bwd_dp_kernel<C, FAST, F>();
-  const auto dg_kern = wide_dgamma_kernel<C, FAST, F>();
+  const auto q_kern = wide_bwd_q_kernel<C, FAST, CF, F>();
+  const auto dp_kern = wide_bwd_dp_kernel<C, FAST, CF, F>();
+  const auto dg_kern = wide_dgamma_kernel<C, FAST, CF, F>();
   TFCB_TRY(reserve_smem(q_kern, W::kSmem));
   TFCB_TRY(reserve_smem(dp_kern, W::kSmem));
   TFCB_TRY(reserve_smem(dg_kern, W::kDgSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
-  q_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f);
+  q_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f, S);
   TFCB_LAUNCHED();
-  dp_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, q_ws, dx, n_pix, f);
+  dp_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, q_ws, dx, n_pix, f, S);
   TFCB_LAUNCHED();
   // one partial per group of kBlocks CTAs (at most sms / kBlocks <= kMaxParts): fixed by n_pix, C and the SM count
   const int grid_g = wide_grid<C>(n_tiles);
-  dg_kern<<<grid_g, 2 * C, W::kDgSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f);
+  dg_kern<<<grid_g, 2 * C, W::kDgSmem, s>>>(x, q_ws, part_g, part_b, n_pix, f, S);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   *n_parts = grid_g / W::kBlocks;
@@ -1314,28 +1499,31 @@ bool misaligned(const void* a, const void* b, const void* c) {
   return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) != 0;
 }
 
+template <bool CF = false>
 int launch_pow_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
-                   const TcPowFlags& f, cudaStream_t s) {
-  if (C == 128) return launch_tc_fwd<128, false, 0>(x, gamma, beta, y, n_pix, f, s);
-  if (C == 192) return launch_tc_fwd<192, false, 0>(x, gamma, beta, y, n_pix, f, s);
-  if (C == 256) return launch_tc_wide_fwd<256, false>(x, gamma, beta, y, n_pix, f, s);
-  return launch_tc_wide_fwd<320, false>(x, gamma, beta, y, n_pix, f, s);
+                   const TcPowFlags& f, cudaStream_t s, long long S = 1) {
+  if (C == 128) return launch_tc_fwd<128, false, 0, CF>(x, gamma, beta, y, n_pix, f, s, S);
+  if (C == 192) return launch_tc_fwd<192, false, 0, CF>(x, gamma, beta, y, n_pix, f, s, S);
+  if (C == 256) return launch_tc_wide_fwd<256, false, CF>(x, gamma, beta, y, n_pix, f, s, S);
+  return launch_tc_wide_fwd<320, false, CF>(x, gamma, beta, y, n_pix, f, s, S);
 }
 
+// CF: `scratch` as launch_tc_bwd takes it at C = 128 / 192.
+template <bool CF = false>
 int launch_pow_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
                    float* part_g, float* part_b, int* n_parts, int* n_parts_e, long long n_pix, int C,
-                   const TcPowFlags& f, cudaStream_t s) {
+                   const TcPowFlags& f, cudaStream_t s, long long S = 1, float* scratch = nullptr) {
   if (C == 128)
-    return launch_tc_bwd<128, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s,
-                                        n_parts_e);
+    return launch_tc_bwd<128, false, 0, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f,
+                                            s, n_parts_e, S);
   if (C == 192)
-    return launch_tc_bwd<192, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s,
-                                        n_parts_e);
+    return launch_tc_bwd<192, false, 0, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f,
+                                            s, n_parts_e, S);
   if (C == 256)
-    return launch_tc_wide_bwd<256, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
-                                          n_parts_e);
-  return launch_tc_wide_bwd<320, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
-                                        n_parts_e);
+    return launch_tc_wide_bwd<256, false, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
+                                              n_parts_e, S);
+  return launch_tc_wide_bwd<320, false, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
+                                            n_parts_e, S);
 }
 
 }  // namespace
@@ -1466,6 +1654,92 @@ int gdn_tc_backward_exponents(const float* x, const float* gamma, const float* b
   *handled = true;
   pf.part_e = part_e;
   return launch_pow_bwd(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_parts_e, n_pix, C, pf, s);
+}
+
+// ---- Channels-first activations: x, y, dy, dx [n_pix / S, C, S] ----
+//
+// Covered exactly where the channels-last tensor-core kernels run: float32 (dtype 0) at C in {128, 192, 256, 320}
+// with any exponents (*pow: on the literal-pow kernels), float16 / bfloat16 (dtype 1, 2) at C = 128 / 192 with the
+// fixed exponents' shortcuts; nothing under TFCB_GDN_FP32=1.  The caller checks this before any device work.
+bool gdn_tc_cf_config(int C, int dtype, int flags, float alpha, float eps, bool* pow) {
+  TcPowFlags pf;
+  TcFlags f;
+  *pow = dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf);
+  if (*pow) return true;
+  if (dtype != 0 && !((dtype == 1 || dtype == 2) && (C == 128 || C == 192))) return false;
+  return tc_config(C, flags, alpha, eps, &f);
+}
+
+// A configuration gdn_tc_cf_config accepts, n_pix > 0.  The kernels and grids of the channels-last entries with the
+// channels-first accesses: y is, bit for bit, what they write for the transposed x.
+int gdn_tc_forward_cf(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, long long S,
+                      int C, int flags, float alpha, float eps, int dtype, cudaStream_t s) {
+  const float* xf = static_cast<const float*>(x);
+  float* yf = static_cast<float*>(y);
+  TcPowFlags pf;
+  if (dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf))
+    return launch_pow_fwd<true>(xf, gamma, beta, yf, n_pix, C, pf, s, S);
+  TcFlags f;
+  if (!tc_config(C, flags, alpha, eps, &f))
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for this configuration");
+  const bool fast = tc_fast(f);
+#define TFCB_FWD_CF(C_, IO_)                                                 \
+  (fast ? launch_tc_fwd<C_, true, IO_, true>(x, gamma, beta, y, n_pix, f, s, S) \
+        : launch_tc_fwd<C_, false, IO_, true>(x, gamma, beta, y, n_pix, f, s, S))
+  if (dtype == 0) {
+    if (C == 256)
+      return fast ? launch_tc_wide_fwd<256, true, true>(xf, gamma, beta, yf, n_pix, f, s, S)
+                  : launch_tc_wide_fwd<256, false, true>(xf, gamma, beta, yf, n_pix, f, s, S);
+    if (C == 320)
+      return fast ? launch_tc_wide_fwd<320, true, true>(xf, gamma, beta, yf, n_pix, f, s, S)
+                  : launch_tc_wide_fwd<320, false, true>(xf, gamma, beta, yf, n_pix, f, s, S);
+    return C == 128 ? TFCB_FWD_CF(128, 0) : TFCB_FWD_CF(192, 0);
+  }
+  if (C == 128) return dtype == 1 ? TFCB_FWD_CF(128, 1) : TFCB_FWD_CF(128, 2);
+  return dtype == 1 ? TFCB_FWD_CF(192, 1) : TFCB_FWD_CF(192, 2);
+#undef TFCB_FWD_CF
+}
+
+// dx, q and the partials as gdn_tc_backward (float32) / gdn_tc_backward16 (16-bit) write them, for channels-first x,
+// dy, dx; at C = 128 / 192 `scratch` holds gdn_tc_backward16_scratch_floats(n_pix, C) floats in either type.  On the
+// literal-pow kernels part_e, when not null, receives the exponent partials as gdn_tc_backward_exponents writes them
+// (*n_parts_e).
+int gdn_tc_backward_cf(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
+                       float* part_g, float* part_b, float* scratch, float* part_e, int* n_parts, int* n_parts_e,
+                       long long n_pix, long long S, int C, int flags, float alpha, float eps, int dtype,
+                       cudaStream_t s) {
+  const float* xf = static_cast<const float*>(x);
+  const float* dyf = static_cast<const float*>(dy);
+  float* dxf = static_cast<float*>(dx);
+  TcPowFlags pf;
+  if (dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf)) {
+    pf.part_e = part_e;
+    return launch_pow_bwd<true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_parts_e, n_pix, C, pf, s,
+                                S, scratch);
+  }
+  TcFlags f;
+  if (!tc_config(C, flags, alpha, eps, &f))
+    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for this configuration");
+  const bool fast = tc_fast(f);
+#define TFCB_BWD_CF(C_, IO_, SCRATCH_)                                                                              \
+  (fast ? launch_tc_bwd<C_, true, IO_, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, SCRATCH_, n_parts, n_pix, \
+                                             f, s, nullptr, S)                                                     \
+        : launch_tc_bwd<C_, false, IO_, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, SCRATCH_, n_parts,      \
+                                              n_pix, f, s, nullptr, S))
+#define TFCB_WIDE_BWD_CF(C_)                                                                                         \
+  (fast ? launch_tc_wide_bwd<C_, true, true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_pix, f, s, \
+                                             nullptr, S)                                                            \
+        : launch_tc_wide_bwd<C_, false, true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_pix, f, s, \
+                                              nullptr, S))
+  if (dtype == 0) {
+    if (C == 256) return TFCB_WIDE_BWD_CF(256);
+    if (C == 320) return TFCB_WIDE_BWD_CF(320);
+    return C == 128 ? TFCB_BWD_CF(128, 0, scratch) : TFCB_BWD_CF(192, 0, scratch);
+  }
+  if (C == 128) return dtype == 1 ? TFCB_BWD_CF(128, 1, scratch) : TFCB_BWD_CF(128, 2, scratch);
+  return dtype == 1 ? TFCB_BWD_CF(192, 1, scratch) : TFCB_BWD_CF(192, 2, scratch);
+#undef TFCB_BWD_CF
+#undef TFCB_WIDE_BWD_CF
 }
 
 }  // namespace tfcb

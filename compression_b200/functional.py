@@ -2,6 +2,7 @@
 TF primitives: GDN/IGDN forward + backward (``python/layers/gdn.py:371-421`` + TF autodiff) and the fused
 quantise+encode / decode+dequantise paths of the entropy models."""
 import ctypes as C
+import math
 import os
 
 import torch
@@ -57,9 +58,88 @@ def _gdn_native16(x, C_, n_pix, alpha, epsilon, pow_alpha, pow_epsilon, dy=None)
           float(alpha) in (1.0, 2.0) and float(epsilon) in (1.0, 0.5) and n_pix > 0 and x.data_ptr() % 16 == 0)
 
 
+_CF_DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+def _gdn_native_cf(x, alpha, epsilon, pow_alpha, pow_epsilon, dy=None, exponent_grads=False):
+  """Whether a channels-first GDN call (x [N, C, *spatial]; the backward with `dy`, and with `exponent_grads` the
+  one that also returns dalpha / depsilon) runs on the kernels that read and write that layout in place
+  (tfcb_gdn_*_cf).  That is exactly where the channels-last path runs on the tensor cores: float32 at C in
+  {128, 192, 256, 320} with any exponents, float16 / bfloat16 at C in {128, 192} with alpha in {1, 2}, epsilon in
+  {1, 1/2} and neither exponent trainable.  x has rank >= 3, is contiguous in the default memory format and 16-byte
+  aligned; dy has x's type, shape and layout and is 16-byte aligned; the exponent gradients need the float32 literal-pow
+  kernels (a trainable exponent, or a fixed one outside the shortcuts).  Never under TFCB_GDN_FP32=1.  Every other
+  call takes the channels-last path on x.movedim(1, -1), which gives the same values; in particular a
+  torch.channels_last tensor, whose movedim(1, -1) is already contiguous.  The device is not looked at here: every
+  channels-first call checks it first (_check_cf_devices), so a host tensor is refused on either path."""
+  if os.environ.get("TFCB_GDN_FP32", "").startswith("1"):
+    return False
+  if x.dim() < 3 or x.dtype not in _CF_DTYPES or not x.is_contiguous() or x.data_ptr() % 16 != 0:
+    return False
+  if dy is not None and (dy.dtype != x.dtype or dy.shape != x.shape or not dy.is_contiguous() or
+                         dy.data_ptr() % 16 != 0):
+    return False
+  C_ = x.shape[1]
+  shortcuts = (not pow_alpha and not pow_epsilon and float(alpha) in (1.0, 2.0) and float(epsilon) in (1.0, 0.5))
+  if x.dtype == torch.float32:
+    return C_ in (128, 192, 256, 320) and not (exponent_grads and shortcuts)
+  return C_ in (128, 192) and shortcuts and not exponent_grads
+
+
+def _check_cf_devices(x, dy=None):
+  """Channels-first calls take CUDA tensors, dy on x's device: anything else is refused before it can reach the
+  library (whose kernels would be handed host pointers), on the native and the movedim path alike."""
+  if not x.is_cuda:
+    raise _lib.InvalidArgumentError(f"GDN takes CUDA tensors, got x on {x.device}")
+  if dy is not None and dy.device != x.device:
+    raise _lib.InvalidArgumentError(f"GDN: dy is on {dy.device}, x on {x.device}")
+
+
+def _gdn_cf_args(x, gamma, beta, dy=None):
+  _check_cf_devices(x, dy)
+  C_ = x.shape[1]
+  gamma = gamma.to(device=x.device, dtype=torch.float32).contiguous()
+  beta = beta.to(device=x.device, dtype=torch.float32).contiguous()
+  assert gamma.shape == (C_, C_) and beta.shape == (C_,)
+  if beta.data_ptr() % 16 != 0:  # the kernels read beta in pairs and the library checks its alignment
+    beta = beta.clone()
+  return gamma, beta, C_, x.shape[0], math.prod(x.shape[2:])
+
+
+def _gdn_backward_cf(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pow_alpha, pow_epsilon, exponent_grads):
+  """One tfcb_gdn_backward_cf call for inputs _gdn_native_cf accepts: (dx, dgamma, dbeta, dalpha_depsilon or None)."""
+  gamma, beta, C_, n_items, spatial = _gdn_cf_args(x, gamma, beta, dy)
+  dx = torch.empty_like(x)
+  dgamma = torch.empty_like(gamma)
+  dbeta = torch.empty_like(beta)
+  # the library fills the exponent gradients whenever an exponent is trainable
+  dae = torch.empty(2, dtype=torch.float32, device=x.device) if exponent_grads or pow_alpha or pow_epsilon else None
+  L = _lib.lib()
+  dtype = _CF_DTYPES[x.dtype]
+  ws = torch.empty(int(L.tfcb_gdn_backward_cf_workspace_bytes(n_items, spatial, C_, dtype)), dtype=torch.uint8,
+                   device=x.device)
+  check(L.tfcb_gdn_backward_cf(_p(x), _p(gamma), _p(beta), _p(dy), _p(dx), _p(dgamma), _p(dbeta), _p(dae), _p(ws),
+                               n_items, spatial, C_, dtype, _flags(inverse, rectify, pow_alpha, pow_epsilon),
+                               float(alpha), float(epsilon), _stream()))
+  return dx, dgamma, dbeta, dae
+
+
 def gdn_forward(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, pow_alpha=False,
-                pow_epsilon=False):
-  """x: float32 CUDA [..., C] (channels-last, contiguous) -> y of the same shape."""
+                pow_epsilon=False, channels_first=False):
+  """x: float32 CUDA [..., C] (channels-last, contiguous) -> y of the same shape.  With `channels_first`, x is
+  [N, C, *spatial]: inputs _gdn_native_cf accepts give a contiguous y from one library call, any other the
+  movedim(-1, 1) view of the channels-last result on x.movedim(1, -1); the values are the same."""
+  if channels_first:
+    _check_cf_devices(x)
+    if not _gdn_native_cf(x, alpha, epsilon, pow_alpha, pow_epsilon):
+      return gdn_forward(x.movedim(1, -1), gamma, beta, inverse, rectify, alpha, epsilon, pow_alpha,
+                         pow_epsilon).movedim(-1, 1)
+    gamma, beta, C_, n_items, spatial = _gdn_cf_args(x, gamma, beta)
+    y = torch.empty_like(x)
+    check(_lib.lib().tfcb_gdn_forward_cf(_p(x), _p(gamma), _p(beta), _p(y), n_items, spatial, C_,
+                                         _CF_DTYPES[x.dtype], _flags(inverse, rectify, pow_alpha, pow_epsilon),
+                                         float(alpha), float(epsilon), _stream()))
+    return y
   x, gamma, beta, C_, n_pix = _gdn_args(x, gamma, beta)
   if x.dtype in _IO16:
     # mixed precision (gdn_test.py:200-210): 16-bit activations, float32 parameters and arithmetic.  The result is the
@@ -78,8 +158,16 @@ def gdn_forward(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon
 
 
 def gdn_backward(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, pow_alpha=False,
-                 pow_epsilon=False):
-  """Returns (dx, dgamma, dbeta) for upstream gradient dy."""
+                 pow_epsilon=False, channels_first=False):
+  """Returns (dx, dgamma, dbeta) for upstream gradient dy.  With `channels_first` (x, dy [N, C, *spatial]) dx is
+  contiguous when _gdn_native_cf accepts x and dy, else the movedim(-1, 1) view of the channels-last dx."""
+  if channels_first:
+    _check_cf_devices(x, dy)
+    if not _gdn_native_cf(x, alpha, epsilon, pow_alpha, pow_epsilon, dy):
+      dx, dgamma, dbeta = gdn_backward(x.movedim(1, -1), gamma, beta, dy.movedim(1, -1), inverse, rectify, alpha,
+                                       epsilon, pow_alpha, pow_epsilon)
+      return dx.movedim(-1, 1), dgamma, dbeta
+    return _gdn_backward_cf(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pow_alpha, pow_epsilon, False)[:3]
   x, gamma, beta, C_, n_pix = _gdn_args(x, gamma, beta)
   if x.dtype in _IO16:
     # dx in the activations' type: the float32 backward's dx of the widened x and dy, rounded once, on either path
@@ -123,10 +211,18 @@ def gdn_exponent_grads(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1
 
 
 def gdn_backward_exponents(x, gamma, beta, dy, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, pow_alpha=True,
-                           pow_epsilon=True):
+                           pow_epsilon=True, channels_first=False):
   """(dx, dgamma, dbeta, dalpha_depsilon) in one library call: gdn_backward's three gradients and gdn_exponent_grads'
   [2] tensor.  With a trainable exponent at C = 128, 192, 256 or 320 the exponent sums are fused into the tensor-core
-  backward.  16-bit activations go through float32 (dx is rounded once to their type)."""
+  backward.  16-bit activations go through float32 (dx is rounded once to their type).  `channels_first` as for
+  gdn_backward."""
+  if channels_first:
+    _check_cf_devices(x, dy)
+    if not _gdn_native_cf(x, alpha, epsilon, pow_alpha, pow_epsilon, dy, exponent_grads=True):
+      dx, dgamma, dbeta, dae = gdn_backward_exponents(x.movedim(1, -1), gamma, beta, dy.movedim(1, -1), inverse,
+                                                      rectify, alpha, epsilon, pow_alpha, pow_epsilon)
+      return dx.movedim(-1, 1), dgamma, dbeta, dae
+    return _gdn_backward_cf(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pow_alpha, pow_epsilon, True)
   if x.dtype in _IO16:
     dx, dgamma, dbeta, dae = gdn_backward_exponents(x.float(), gamma, beta, dy, inverse, rectify, alpha, epsilon,
                                                     pow_alpha, pow_epsilon)
@@ -150,38 +246,40 @@ class _GDNFunction(torch.autograd.Function):
   take the exponents as scalars), else None and the fixed value travels in `alpha` / `epsilon`."""
 
   @staticmethod
-  def forward(ctx, x, gamma, beta, alpha_t, epsilon_t, inverse, rectify, alpha, epsilon):
+  def forward(ctx, x, gamma, beta, alpha_t, epsilon_t, inverse, rectify, alpha, epsilon, channels_first):
     pa, pe = alpha_t is not None, epsilon_t is not None
     if pa:
       alpha = float(alpha_t)
     if pe:
       epsilon = float(epsilon_t)
     ctx.save_for_backward(x, gamma, beta)
-    ctx.cfg = (inverse, rectify, alpha, epsilon, pa, pe)
-    return gdn_forward(x, gamma, beta, inverse, rectify, alpha, epsilon, pa, pe)
+    ctx.cfg = (inverse, rectify, alpha, epsilon, pa, pe, channels_first)
+    return gdn_forward(x, gamma, beta, inverse, rectify, alpha, epsilon, pa, pe, channels_first=channels_first)
 
   @staticmethod
   def backward(ctx, dy):
     x, gamma, beta = ctx.saved_tensors
-    inverse, rectify, alpha, epsilon, pa, pe = ctx.cfg
+    inverse, rectify, alpha, epsilon, pa, pe, cf = ctx.cfg
     dalpha = depsilon = None
     if (pa and ctx.needs_input_grad[3]) or (pe and ctx.needs_input_grad[4]):
-      dx, dgamma, dbeta, g2 = gdn_backward_exponents(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
+      dx, dgamma, dbeta, g2 = gdn_backward_exponents(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe,
+                                                     channels_first=cf)
       dalpha = g2[0] if pa else None
       depsilon = g2[1] if pe else None
     else:
-      dx, dgamma, dbeta = gdn_backward(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe)
-    return dx, dgamma, dbeta, dalpha, depsilon, None, None, None, None
+      dx, dgamma, dbeta = gdn_backward(x, gamma, beta, dy, inverse, rectify, alpha, epsilon, pa, pe, channels_first=cf)
+    return dx, dgamma, dbeta, dalpha, depsilon, None, None, None, None, None
 
 
-def gdn(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon=1.0):
+def gdn(x, gamma, beta, inverse=False, rectify=False, alpha=1.0, epsilon=1.0, channels_first=False):
   """Differentiable GDN/IGDN on channels-last float32 / float16 / bfloat16 CUDA tensors (float32 parameters).  `alpha` / `epsilon`: Python numbers (fixed
   exponents: |u|, u^2, sqrt shortcuts and the tensor-core kernels apply) or 0-d tensors (trainable: literal pow, with
-  gradients)."""
+  gradients).  `channels_first`: x is [N, C, *spatial] (gdn_forward / gdn_backward describe the layouts returned)."""
   at = alpha if isinstance(alpha, torch.Tensor) else None
   et = epsilon if isinstance(epsilon, torch.Tensor) else None
   return _GDNFunction.apply(x, gamma, beta, at, et, bool(inverse), bool(rectify),
-                            1.0 if at is not None else float(alpha), 1.0 if et is not None else float(epsilon))
+                            1.0 if at is not None else float(alpha), 1.0 if et is not None else float(epsilon),
+                            bool(channels_first))
 
 
 # ------------------------------------------------------------------------------------------------

@@ -141,15 +141,19 @@ class GDN(nn.Module):
     if not self.built:
       self.build(inputs.shape, device=inputs.device)
     dev = inputs.device
-    x = inputs.movedim(1, -1) if self.data_format == "channels_first" else inputs
-    out_dtype = x.dtype
-    # float16 / bfloat16 activations go to the kernels as they are (mixed precision, gdn_test.py:200-210)
-    x32 = (x if x.dtype in (torch.float32, torch.float16, torch.bfloat16) else x.to(torch.float32)).contiguous()
     alpha, epsilon = self.alpha_parameter, self.epsilon_parameter
     # trainable exponents travel as 0-d tensors: literal pow in the kernels plus the two scalar gradients
     # (gdn.py:345-367,388,411); fixed ones as Python numbers (|u| / u^2 / sqrt shortcuts, tensor-core kernels)
     a = self._param("alpha", device=dev) if callable(alpha) else float(alpha)
     e = self._param("epsilon", device=dev) if callable(epsilon) else float(epsilon)
+    if self.data_format == "channels_first" and F._gdn_native_cf(inputs, a, e, callable(alpha), callable(epsilon)):
+      # contiguous [N, C, *spatial] read and written in place: y and, in the backward, dx come back contiguous
+      return F.gdn(inputs, self._param("gamma", device=dev), self._param("beta", device=dev), self.inverse,
+                   self.rectify, a, e, channels_first=True)
+    x = inputs.movedim(1, -1) if self.data_format == "channels_first" else inputs
+    out_dtype = x.dtype
+    # float16 / bfloat16 activations go to the kernels as they are (mixed precision, gdn_test.py:200-210)
+    x32 = (x if x.dtype in (torch.float32, torch.float16, torch.bfloat16) else x.to(torch.float32)).contiguous()
     y = F.gdn(x32, self._param("gamma", device=dev), self._param("beta", device=dev), self.inverse, self.rectify, a, e)
     y = y.to(out_dtype)
     return y.movedim(-1, 1) if self.data_format == "channels_first" else y

@@ -404,6 +404,30 @@ int tfcb_gdn_backward_exponents(const float* x_dev, const float* gamma_dev, cons
                                 void* workspace_dev, int64_t n_pix, int C, int flags, float alpha, float epsilon,
                                 void* stream);
 
+/* Channels-first GDN / IGDN (the reference's data_format="channels_first", gdn.py:127-175): x, y, dy, dx are
+ * [n_items, C, spatial] contiguous, spatial the product of the spatial dimensions, so element (item b, channel c,
+ * position s) is at (b * C + c) * spatial + s.  `dtype` 0 float32, 1 float16, 2 bfloat16 (parameters, dgamma, dbeta
+ * and the arithmetic float32).  The same kernels as the channels-last entries read and write this layout in place:
+ * every output (y, dx, dgamma, dbeta, dalpha / depsilon) is bit for bit what tfcb_gdn_forward / tfcb_gdn_backward /
+ * tfcb_gdn_backward_exponents (float32) or the _16bit entries (16 bits) give for the same tensors transposed to
+ * [n_items * spatial, C], so the channels-last accuracy bounds above hold as they are.
+ * Covered exactly where the channels-last tensor-core kernels run: float32 at C in {128, 192, 256, 320} with any
+ * exponents, float16 / bfloat16 at C in {128, 192} with alpha in {1, 2} and epsilon in {1, 1/2} and no POW flag.
+ * Checked before any device work (TFCB_INVALID_ARGUMENT): n_items, spatial >= 0, C > 0, n_items * spatial * C within
+ * int64; a covered configuration (never under TFCB_GDN_FP32=1: transpose to channels-last there); non-null pointers
+ * (x, y, dy, dx may be NULL when n_items * spatial = 0); x, y, dy, dx, beta and the workspace 16-byte aligned.
+ * An empty tensor launches nothing; the backward then sets dgamma, dbeta (and dalpha / depsilon) to zero.
+ * Backward: dalpha_depsilon_dev float32 [2] receives (dL/dalpha, dL/depsilon) and is required with a POW flag; it may
+ * be NULL without one, and must be NULL when both exponents take the shortcuts.  `workspace_dev` holds
+ * tfcb_gdn_backward_cf_workspace_bytes(n_items, spatial, C, dtype) bytes (-1 for arguments the entries reject). */
+int tfcb_gdn_forward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, void* y_dev, int64_t n_items,
+                        int64_t spatial, int C, int dtype, int flags, float alpha, float epsilon, void* stream);
+int64_t tfcb_gdn_backward_cf_workspace_bytes(int64_t n_items, int64_t spatial, int C, int dtype);
+int tfcb_gdn_backward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, const void* dy_dev,
+                         void* dx_dev, float* dgamma_dev, float* dbeta_dev, float* dalpha_depsilon_dev,
+                         void* workspace_dev, int64_t n_items, int64_t spatial, int C, int dtype, int flags,
+                         float alpha, float epsilon, void* stream);
+
 int64_t tfcb_launch_count(void);
 
 #ifdef __cplusplus
