@@ -8,6 +8,7 @@
 //   cc/ops/quantization_ops.cc:28-53   StochasticRound
 //   cc/ops/run_length_ops.cc:28-84, run_length_gamma_ops.cc:26-58   RunLength{,Gamma}{Encode,Decode}
 //   cc/ops/range_coding_ops.cc:30-124  RangeEncode, RangeDecode (legacy single-stream ops)
+//   cc/ops/range_coding_ops.cc:126-247 UnboundedIndexRangeEncode, UnboundedIndexRangeDecode
 // and their CPU kernels stay registered (cc/kernels/range_coder_kernels.cc:505-700 etc.); TensorFlow's placer picks
 // the GPU kernel when the data tensors live on the GPU, so python/ops/gen_ops.py and models/*.py are unchanged.
 // GDN has no op in the reference (python/layers/gdn.py:371-421 composes TF ops): GdnForward / GdnBackward are
@@ -478,6 +479,112 @@ class RangeDecodeGpuOp : public tf::OpKernel {
 };
 REGISTER_KERNEL_BUILDER(Name("RangeDecode").Device(tf::DEVICE_GPU).HostMemory("encoded").HostMemory("shape"),
                         RangeDecodeGpuOp);
+
+// ---- UnboundedIndexRangeEncode / Decode (unbounded_index_range_coding_kernels.cc): the one-item case of the
+// library's ragged entries; `encoded` lives in host memory as for RangeEncode ----
+class UnboundedIndexRangeGpuOpBase : public tf::OpKernel {
+ public:
+  explicit UnboundedIndexRangeGpuOpBase(tf::OpKernelConstruction* c) : tf::OpKernel(c) {
+    OP_REQUIRES_OK(c, c->GetAttr("precision", &precision_));
+    OP_REQUIRES_OK(c, c->GetAttr("overflow_width", &overflow_width_));
+    OP_REQUIRES_OK(c, c->GetAttr("debug_level", &debug_level_));
+  }
+ protected:
+  // cdf_size and offset must be vectors (the library sees their lengths only).
+  tf::Status TableShapes(tf::OpKernelContext* ctx, int first, std::vector<int64_t>* cs) {
+    const tf::Tensor& cdf = ctx->input(first);
+    if (!tf::TensorShapeUtils::IsVector(ctx->input(first + 1).shape()))
+      return InvalidArgument("'cdf_size' should be 1-D and its length should match the number of rows in 'cdf': ",
+                             ctx->input(first + 1).shape().DebugString());
+    if (!tf::TensorShapeUtils::IsVector(ctx->input(first + 2).shape()))
+      return InvalidArgument("'offset' should be 1-D and its length should match the number of rows in 'cdf': "
+                             "offset.shape=", ctx->input(first + 2).shape().DebugString());
+    *cs = Dims(cdf.shape());
+    return tf::OkStatus();
+  }
+  int precision_, overflow_width_, debug_level_;
+};
+
+class UnboundedIndexRangeEncodeGpuOp : public UnboundedIndexRangeGpuOpBase {
+ public:
+  using UnboundedIndexRangeGpuOpBase::UnboundedIndexRangeGpuOpBase;
+  void Compute(tf::OpKernelContext* ctx) override {
+    const tf::Tensor& data = ctx->input(0);
+    const tf::Tensor& index = ctx->input(1);
+    OP_REQUIRES(ctx, data.shape() == index.shape(),
+                InvalidArgument("`data` and `index` should have the same shape: data.shape=",
+                                data.shape().DebugString(), ", index.shape=", index.shape().DebugString()));
+    std::vector<int64_t> cs;
+    OP_REQUIRES_OK(ctx, TableShapes(ctx, 2, &cs));
+    const int64_t items[2] = {0, data.NumElements()};
+    tf::Tensor offsets;
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(tf::DT_INT64, tf::TensorShape({2}), &offsets));
+    tfcb_ubi_encoder* h = nullptr;
+    int64_t total = 0;
+    OP_REQUIRES_OK(ctx, FromRc(tfcb_unbounded_index_range_encode_ragged(
+                            data.flat<int32_t>().data(), index.flat<int32_t>().data(), 1, items,
+                            ctx->input(2).flat<int32_t>().data(), cs.data(), ctx->input(2).dims(),
+                            ctx->input(3).flat<int32_t>().data(), ctx->input(3).NumElements(),
+                            ctx->input(4).flat<int32_t>().data(), ctx->input(4).NumElements(), precision_,
+                            overflow_width_, debug_level_, offsets.flat<int64_t>().data(), CudaStream(ctx), &h,
+                            &total)));
+    tf::Tensor bytes;
+    tf::Status st = ctx->allocate_temp(tf::DT_UINT8, tf::TensorShape({std::max<int64_t>(total, 1)}), &bytes);
+    if (!st.ok()) {
+      tfcb_unbounded_index_range_encoder_destroy(h);
+      ctx->SetStatus(st);
+      return;
+    }
+    OP_REQUIRES_OK(ctx, FromRc(tfcb_unbounded_index_range_write(h, bytes.flat<uint8_t>().data(), CudaStream(ctx))));
+    std::string host(static_cast<size_t>(total), '\0');
+    if (total > 0) {
+      auto* stream = ctx->op_device_context()->stream();
+      stream_executor::DeviceMemoryBase src(bytes.flat<uint8_t>().data(), static_cast<uint64_t>(total));
+      OP_REQUIRES_OK(ctx, stream->Memcpy(&host[0], src, static_cast<uint64_t>(total)));
+      OP_REQUIRES_OK(ctx, stream->BlockHostUntilDone());
+    }
+    tf::Tensor* out;
+    OP_REQUIRES_OK(ctx, ctx->allocate_output(0, tf::TensorShape({}), &out));
+    out->scalar<tf::tstring>()() = std::move(host);
+  }
+};
+REGISTER_KERNEL_BUILDER(Name("UnboundedIndexRangeEncode").Device(tf::DEVICE_GPU).HostMemory("encoded"),
+                        UnboundedIndexRangeEncodeGpuOp);
+
+class UnboundedIndexRangeDecodeGpuOp : public UnboundedIndexRangeGpuOpBase {
+ public:
+  using UnboundedIndexRangeGpuOpBase::UnboundedIndexRangeGpuOpBase;
+  void Compute(tf::OpKernelContext* ctx) override {
+    const tf::Tensor& encoded = ctx->input(0);  // host memory
+    const tf::Tensor& index = ctx->input(1);
+    OP_REQUIRES(ctx, tf::TensorShapeUtils::IsScalar(encoded.shape()),
+                InvalidArgument("`encoded` should be a scalar: ", encoded.shape().DebugString()));
+    std::vector<int64_t> cs;
+    OP_REQUIRES_OK(ctx, TableShapes(ctx, 2, &cs));
+    const tf::tstring& src = encoded.scalar<tf::tstring>()();
+    const int64_t n_bytes = static_cast<int64_t>(src.size());
+    tf::Tensor bytes, offsets;
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(tf::DT_UINT8, tf::TensorShape({std::max<int64_t>(n_bytes, 1)}), &bytes));
+    OP_REQUIRES_OK(ctx, ctx->allocate_temp(tf::DT_INT64, tf::TensorShape({2}), &offsets));
+    auto* stream = ctx->op_device_context()->stream();
+    const int64_t host_offsets[2] = {0, n_bytes};
+    stream_executor::DeviceMemoryBase d_bytes(bytes.flat<uint8_t>().data(), static_cast<uint64_t>(n_bytes));
+    stream_executor::DeviceMemoryBase d_offsets(offsets.flat<int64_t>().data(), 16);
+    if (n_bytes > 0) OP_REQUIRES_OK(ctx, stream->Memcpy(&d_bytes, src.data(), static_cast<uint64_t>(n_bytes)));
+    OP_REQUIRES_OK(ctx, stream->Memcpy(&d_offsets, host_offsets, 16));
+    tf::Tensor* out;
+    OP_REQUIRES_OK(ctx, ctx->allocate_output(0, index.shape(), &out));
+    const int64_t items[2] = {0, index.NumElements()};
+    OP_REQUIRES_OK(ctx, FromRc(tfcb_unbounded_index_range_decode_ragged(
+                            bytes.flat<uint8_t>().data(), offsets.flat<int64_t>().data(), 1, items,
+                            index.flat<int32_t>().data(), ctx->input(2).flat<int32_t>().data(), cs.data(),
+                            ctx->input(2).dims(), ctx->input(3).flat<int32_t>().data(), ctx->input(3).NumElements(),
+                            ctx->input(4).flat<int32_t>().data(), ctx->input(4).NumElements(), precision_,
+                            overflow_width_, debug_level_, out->flat<int32_t>().data(), CudaStream(ctx))));
+  }
+};
+REGISTER_KERNEL_BUILDER(Name("UnboundedIndexRangeDecode").Device(tf::DEVICE_GPU).HostMemory("encoded"),
+                        UnboundedIndexRangeDecodeGpuOp);
 
 // ---- GDN: two new ops (the reference has none); see gdn_custom_gradient.py in this directory ----
 REGISTER_OP("GdnForward")

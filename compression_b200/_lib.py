@@ -65,6 +65,12 @@ SIGNATURES = {
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_range_decode": (_int, [_vp, _i64, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),
+    "tfcb_unbounded_index_range_encode_ragged": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _int, _vp, _i64, _vp, _i64,
+                                                        _int, _int, _int, _vp, _vp, _p(_vp), _p(_i64)]),
+    "tfcb_unbounded_index_range_write": (_int, [_vp, _vp, _vp]),
+    "tfcb_unbounded_index_range_encoder_destroy": (None, [_vp]),
+    "tfcb_unbounded_index_range_decode_ragged": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _int, _vp, _i64, _vp,
+                                                        _i64, _int, _int, _int, _vp, _vp]),
     "tfcb_pmf_to_quantized_cdf": (_int, [_vp, _i64, _i64, _int, _vp, _vp]),
     "tfcb_build_lookup": (_int, [_vp, _i64, _i64, _vp, _int, _vp, _vp]),
     "tfcb_run_length_encode": (_int, [_vp, _i64, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),

@@ -1971,9 +1971,10 @@ EncResult* mapped_result(EncResult** dev) {
 }
 
 // Lengths, offsets (into `offsets`), the one host round trip, then the deferred argument errors (`what` selects their
-// wording, see decode_error) and the total.
+// wording, see decode_error) and the total.  `err_out`, when given, receives the raw error record instead and no
+// wording is applied (callers that keep their own error keys in it).
 int enc_offsets(const EncArena& a, long long* offsets, bool reset_err, const char* what, cudaStream_t s,
-                long long* total) {
+                long long* total, DevError* err_out = nullptr) {
   EncResult* dres = nullptr;
   EncResult* res = mapped_result(&dres);
   if (!res) return fail(TFCB_CUDA_ERROR, "could not allocate host-mapped memory for the finalize result");
@@ -1985,6 +1986,10 @@ int enc_offsets(const EncArena& a, long long* offsets, bool reset_err, const cha
   EncResult r;
   std::memcpy(&r, res, sizeof r);
   *total = r.total;
+  if (err_out) {
+    *err_out = r.err;
+    return TFCB_OK;
+  }
   return decode_error(r.err, what);
 }
 
@@ -2668,6 +2673,576 @@ int tfcb_range_decode(const uint8_t* encoded_host, int64_t n_bytes, const int64_
   cleanup();
   if (e != cudaSuccess) return fail(TFCB_CUDA_ERROR, "CUDA error '%s' in tfcb_range_decode", cudaGetErrorString(e));
   return TFCB_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------
+// UnboundedIndexRangeEncode / UnboundedIndexRangeDecode (range_coding_ops.cc:126-247,
+// unbounded_index_range_coding_kernels.cc), one warp per string over a ragged batch of strings.
+//
+// Element i of a string codes d = data[i] - offset[r] (r = index[i], m = cdf_size[r] - 2) with row r when
+// 0 <= d < m, else the escape bin m followed by u = -2d - 1 (d < 0) or 2(d - m) (d >= m) as a run of
+// widths = ceil(bitlen(u) / w) in w-bit symbols (runs of M = 2^w - 1, then the remainder) and the widths w-bit digits
+// of u, least significant first.  The reference computes d, u and widths in signed 32-bit arithmetic and is undefined
+// for d <= -2^30, d - m >= 2^30 and u >= 2^(w * floor(31 / w)); here d and u wrap as uint32 and widths comes from
+// clz, which equals the reference wherever it is defined and extends the op to every int32 (DESIGN.md §3.8).
+// ---------------------------------------------------------------------------------------------
+namespace tfcb {
+namespace {
+
+// Error keys kept in a DevError with atomicMin, so that the lowest one wins whatever the schedule:
+//   .stream  element key  g << 3 | kind   (g = element index over the whole batch: ordered by string, then element)
+//   .pos     row key      r (cdf_size out of [3, W]), or 2^62 | r << 1 | (0: start / end, 1: not monotonic)
+//   .value   the lowest element whose index is outside [0, R) (debug check only)
+// All three start at ~0.  .code stays 0 unless the arena bound were ever exceeded (kErrCapacity).
+enum : int { kUbiIndex = 1, kUbiCdfSize = 2, kUbiInterval = 3, kUbiPrefix = 4 };
+constexpr unsigned long long kUbiNone = ~0ull;
+constexpr unsigned long long kUbiCdfKey = 1ull << 62;
+
+__device__ __forceinline__ void ubi_key(long long* field, unsigned long long key) {
+  atomicMin(reinterpret_cast<unsigned long long*>(field), key);
+}
+
+struct UbiParams {
+  const int32_t* data;      // encoder: [elements]
+  int32_t* out;             // decoder: [elements]
+  const int32_t* index;     // [elements]
+  const int32_t* cdf;       // [R, W]
+  const int32_t* cdf_size;  // [R]
+  const int32_t* offset;    // [R]
+  long long R, W;
+  int precision, width;
+  const long long* elem_off;   // [strings + 1]: string s is elements [elem_off[s], elem_off[s + 1])
+  const long long* arena_off;  // encoder: [strings + 1], words of string s (multiples of 32)
+  EncState* state;
+  uint16_t* words;
+  uint32_t* cbits;
+  const uint8_t* bytes;        // decoder: string s is bytes [str_off[s], str_off[s + 1])
+  const long long* str_off;
+  DevError* err;
+};
+
+// Row of element g, or -1 after recording why it cannot be coded.  Checked whatever debug_level is: an index or a
+// cdf_size outside its range would make the kernels read outside `cdf`.
+__device__ __forceinline__ int ubi_row(const UbiParams& P, long long g) {
+  const int r = P.index[g];
+  if (r < 0 || r >= P.R) {
+    ubi_key(&P.err->stream, ((unsigned long long)g << 3) | kUbiIndex);
+    return -1;
+  }
+  const int sz = P.cdf_size[r];
+  if (sz < 3 || sz > P.W) {
+    ubi_key(&P.err->stream, ((unsigned long long)g << 3) | kUbiCdfSize);
+    return -1;
+  }
+  return r;
+}
+
+// debug_level 1: CheckIndex, CheckCdfSize and CheckCdf of the reference over the whole tensors, each row against its
+// own cdf_size prefix; the keys order the failures the way the reference's sequential checks would meet them.
+__global__ void ubi_check_kernel(const int32_t* index, long long n, const int32_t* cdf, const int32_t* cdf_size,
+                                 long long R, long long W, int precision, DevError* err) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  for (long long i = t; i < n; i += stride) {
+    const int r = index[i];
+    if (r < 0 || r >= R) ubi_key(&err->value, (unsigned long long)i);
+  }
+  const int32_t top = 1 << precision;
+  for (long long r = t; r < R; r += stride) {
+    const int sz = cdf_size[r];
+    if (sz < 3 || sz > W) {
+      ubi_key(&err->pos, (unsigned long long)r);
+      continue;
+    }
+    const int32_t* row = cdf + r * W;
+    if (row[0] != 0 || row[sz - 1] != top) {
+      ubi_key(&err->pos, kUbiCdfKey | ((unsigned long long)r << 1));
+      continue;
+    }
+    for (int j = 0; j + 1 < sz; ++j) {
+      if (row[j + 1] <= row[j]) {
+        ubi_key(&err->pos, kUbiCdfKey | ((unsigned long long)r << 1) | 1ull);
+        break;
+      }
+    }
+  }
+}
+
+// One warp per string.  Lanes map 32 elements at a time; then every lane runs the same recurrence over the
+// elements' records in order (main symbol at precision p, width prefix and digits at precision w), lane j keeping
+// entry j of the current 32, and EncDrain turns each full set of 32 entries into words, as legacy_encode_kernel does.
+__global__ void __launch_bounds__(32) ubi_encode_kernel(const UbiParams P) {
+  __shared__ __align__(8) uint2 s_ent[32];
+  const int lane = threadIdx.x;
+  const long long s = blockIdx.x;
+  const Extent e = stream_extent(P.elem_off, s, 0);
+  const Extent a = stream_extent(P.arena_off, s, 0);
+  const EncState st0 = enc_initial_state();
+  EncChain c;
+  c.s = st0.raw;
+  EncDrain d;
+  d.begin(st0, P.words + a.base, P.cbits + (a.base >> 5), (uint32_t)a.len, lane);
+  const uint32_t p = (uint32_t)P.precision, w = (uint32_t)P.width, M = (1u << w) - 1u;
+  uint2 mine = make_uint2(0u, 0u);
+  int fill = 0;
+  auto push = [&](uint32_t lo, uint32_t hi, uint32_t prec) {
+    const uint2 ent = c.step(enc_operands(lo, hi, prec));
+    if (lane == fill) mine = ent;
+    if (++fill == 32) {
+      s_ent[lane] = mine;
+      __syncwarp();
+      d.drain<1>(s_ent, 32);
+      __syncwarp();
+      fill = 0;
+    }
+  };
+  for (long long g0 = 0; g0 < e.len; g0 += 32) {
+    const int count = (int)min(32ll, e.len - g0);
+    uint32_t lower = 0, upper = 1, u = 0;
+    int esc = 0;
+    bool bad = false;
+    if (lane < count) {
+      const long long g = e.base + g0 + lane;
+      const int r = ubi_row(P, g);
+      if (r < 0) {
+        bad = true;
+      } else {
+        const uint32_t m = (uint32_t)(P.cdf_size[r] - 2);
+        const uint32_t du = (uint32_t)P.data[g] - (uint32_t)P.offset[r];
+        const int32_t dd = (int32_t)du;
+        uint32_t v = du;
+        if (dd < 0) {
+          u = 0u - 2u * du - 1u;
+          v = m;
+        } else if (du >= m) {
+          u = 2u * (du - m);
+          v = m;
+        }
+        esc = v == m;
+        const int32_t* row = P.cdf + r * P.W;
+        lower = (uint32_t)row[v];
+        upper = (uint32_t)row[v + 1];
+        if (!(lower < upper) || upper > (1u << p)) {  // an empty interval: the reference's output is garbage
+          ubi_key(&P.err->stream, ((unsigned long long)g << 3) | kUbiInterval);
+          bad = true;
+        }
+      }
+    }
+    if (__ballot_sync(kFull, bad)) break;
+    for (int k = 0; k < count; ++k) {
+      push(__shfl_sync(kFull, lower, k), __shfl_sync(kFull, upper, k), p);
+      if (__shfl_sync(kFull, esc, k)) {
+        const uint32_t uk = __shfl_sync(kFull, u, k);
+        const uint32_t widths = (32u - __clz(uk) + w - 1u) / w;  // __clz(0) = 32: no digits
+        uint32_t val = widths;
+        for (; val >= M; val -= M) push(M, M + 1u, w);
+        push(val, val + 1u, w);
+        for (uint32_t j = 0; j < widths; ++j) {  // j * w < bitlen(u) <= 32
+          const uint32_t digit = (uk >> (j * w)) & M;
+          push(digit, digit + 1u, w);
+        }
+      }
+    }
+  }
+  if (fill) {
+    s_ent[lane] = mine;
+    __syncwarp();
+    d.drain<1>(s_ent, fill);
+    __syncwarp();
+  }
+  d.end(P.err, s);
+  if (lane == 0) {
+    EncState st;
+    st.base = d.dbase;
+    st.span = (c.s < 65536u) ? ((c.s << 16) | 0xFFFFu) : c.s;
+    st.cnt = d.cnt;
+    st.raw = c.s;
+    P.state[s] = st;
+  }
+}
+
+// RangeDecoder::Decode over the uniform table 0, 1, ..., 2^w at precision w, computed instead of searched: the
+// smallest i in [1, 2^w] with (value - base + 1) * 2^w <= size * i, which is what the reference's binary search finds.
+__device__ __forceinline__ uint32_t ubi_dec_uniform(DecChain& c, ByteWindow& win, uint32_t w, int lane) {
+  const unsigned long long size = (unsigned long long)c.span + 1ull;
+  const unsigned long long want = ((unsigned long long)(c.value - c.base) + 1ull) << w;
+  unsigned long long i = (want + size - 1ull) / size;
+  if (i > (1ull << w)) i = 1ull << w;  // only on damaged strings; the reference reads past its table there
+  const uint32_t sym = (uint32_t)i;
+  dec_update(c, win, scale_cum(c.span, sym - 1u, w), scale_cum(c.span, sym, w), lane);
+  return sym - 1u;
+}
+
+// One warp per string, legacy_decode_kernel's chain.  The width prefix stops once its running total exceeds
+// K = ceil(32 / w), the most any encoder writes: every symbol then takes at most 2K + 2 decode steps, on any bytes.
+__global__ void __launch_bounds__(32) ubi_decode_kernel(const UbiParams P) {
+  const int lane = threadIdx.x;
+  const long long s = blockIdx.x;
+  const Extent e = stream_extent(P.elem_off, s, 0);
+  const Extent b = stream_extent(P.str_off, s, 0);
+  DecChain c;
+  c.base = 0;
+  c.span = 0xFFFFFFFFu;
+  ByteWindow win;
+  win.p = P.bytes + b.base;
+  win.len = b.len;
+  c.value = (bw_fetch(win, 0) << 16) | bw_fetch(win, 1);
+  c.pos = 2;
+  bw_seek(win, c.pos, lane);
+  const uint32_t p = (uint32_t)P.precision, w = (uint32_t)P.width, M = (1u << w) - 1u;
+  const uint32_t K = (32u + w - 1u) / w;
+  for (long long g0 = 0; g0 < e.len; g0 += 32) {
+    const int count = (int)min(32ll, e.len - g0);
+    int r = 0, m = 0, off = 0;
+    bool bad = false;
+    if (lane < count) {
+      r = ubi_row(P, e.base + g0 + lane);
+      if (r < 0) {
+        bad = true;
+      } else {
+        m = P.cdf_size[r] - 2;
+        off = P.offset[r];
+      }
+    }
+    if (__ballot_sync(kFull, bad)) return;
+    int32_t my_val = 0;
+    int done = count;
+    for (int k = 0; k < count; ++k) {
+      const int rk = __shfl_sync(kFull, r, k);
+      const int mk = __shfl_sync(kFull, m, k);
+      const int sym = dec_symbol(c, win, P.cdf + rk * P.W, mk + 2, p, lane);
+      uint32_t v = (uint32_t)sym;
+      if (sym == mk) {
+        uint32_t widths = 0, val;
+        bool over = false;
+        do {
+          val = ubi_dec_uniform(c, win, w, lane);
+          widths += val;
+          if (widths > K) {
+            over = true;
+            break;
+          }
+        } while (val == M);
+        if (over) {
+          if (lane == 0) ubi_key(&P.err->stream, ((unsigned long long)(e.base + g0 + k) << 3) | kUbiPrefix);
+          done = k;
+          break;
+        }
+        uint32_t u = 0;
+        for (uint32_t j = 0; j < widths; ++j) u |= ubi_dec_uniform(c, win, w, lane) << (j * w);
+        v = u >> 1;
+        v = (u & 1u) ? 0u - v - 1u : v + (uint32_t)mk;
+      }
+      v += (uint32_t)__shfl_sync(kFull, off, k);
+      if (lane == k) my_val = (int32_t)v;
+    }
+    if (lane < done) P.out[e.base + g0 + lane] = my_val;
+    if (done < count) return;
+  }
+}
+
+// ---- host side ----
+int ubi_check_attrs(int precision, int overflow_width, int debug_level) {
+  if (!(0 < precision && precision <= 16))
+    return fail(TFCB_INVALID_ARGUMENT, "`precision` must be in [1, 16]: %d", precision);
+  if (!(0 < overflow_width && overflow_width <= 16))
+    return fail(TFCB_INVALID_ARGUMENT, "`overflow_width` must be in [1, 16]: %d", overflow_width);
+  if (!(debug_level == 0 || debug_level == 1))
+    return fail(TFCB_INVALID_ARGUMENT, "`debug_level` must be 0 or 1: %d", debug_level);
+  return TFCB_OK;
+}
+
+// CheckArgumentShapes of the reference on the host shapes, then the batch offsets and pointers.
+int ubi_check_args(const int64_t* cdf_shape, int cdf_rank, int64_t cdf_size_len, int64_t offset_len,
+                   int64_t n_items, const int64_t* item_offsets, const void* index, const void* cdf,
+                   const void* cdf_size, const void* offset) {
+  if (cdf_rank != 2 || !cdf_shape || cdf_shape[1] < 3 || cdf_shape[0] < 0)
+    return fail(TFCB_INVALID_ARGUMENT, "'cdf' should be 2-D and cdf.dim_size(1) >= 3: rank %d", cdf_rank);
+  if (cdf_size_len != cdf_shape[0])
+    return fail(TFCB_INVALID_ARGUMENT,
+                "'cdf_size' should be 1-D and its length should match the number of rows in 'cdf': [%lld]",
+                (long long)cdf_size_len);
+  if (offset_len != cdf_shape[0])
+    return fail(TFCB_INVALID_ARGUMENT,
+                "'offset' should be 1-D and its length should match the number of rows in 'cdf': offset.shape=[%lld], "
+                "cdf.shape=[%lld,%lld]",
+                (long long)offset_len, (long long)cdf_shape[0], (long long)cdf_shape[1]);
+  if (cdf_shape[0] >= (1ll << 31) || cdf_shape[0] * cdf_shape[1] >= (1ll << 40))
+    return fail(TFCB_INVALID_ARGUMENT, "'cdf' too large");
+  if (n_items >= (1ll << 31)) return fail(TFCB_INVALID_ARGUMENT, "too many strings: %lld", (long long)n_items);
+  TFCB_TRY(check_symbol_offsets(item_offsets, n_items));
+  // (debug_level 1 reads every row even when there are no elements)
+  if ((item_offsets[n_items] > 0 && !index) || (cdf_shape[0] > 0 && (!cdf || !cdf_size || !offset)))
+    return fail(TFCB_INVALID_ARGUMENT, "null pointer argument");
+  return TFCB_OK;
+}
+
+// Worst-case bits per element: p for the main symbol, and for an escape floor(K / M) + 1 prefix symbols and K digits
+// of w bits each (K = ceil(32 / w)): 65 + p at w = 1, 33 + p at w = 16.  Every Encode at precision q consumes at most
+// q bits (see bits_bound).
+long long ubi_bits_bound(int precision, int w) {
+  const long long K = (32 + w - 1) / w, M = (1ll << w) - 1;
+  return precision + (long long)w * (K / M + 1 + K);
+}
+
+// Reads what the messages name from the device (error path only) and returns the first failure in the order the
+// reference would meet it.
+int ubi_error(const DevError& e, int debug_level, const int64_t* item_offsets, int64_t n_items, const int32_t* index,
+              const int32_t* cdf, const int32_t* cdf_size, long long R, long long W, int precision, int overflow_width,
+              cudaStream_t s) {
+  if (e.code == kErrCapacity)
+    return fail(TFCB_CUDA_ERROR, "internal: output arena too small (string %lld needs > %lld words)", e.stream,
+                e.limit);
+  const unsigned long long ekey = (unsigned long long)e.stream, rkey = (unsigned long long)e.pos,
+                           ikey = (unsigned long long)e.value;
+  if (ekey == kUbiNone && rkey == kUbiNone && ikey == kUbiNone) return TFCB_OK;
+  auto at = [&](const int32_t* p, long long i) {
+    int32_t v = 0;
+    if (cudaMemcpyAsync(&v, p + i, sizeof v, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+        cudaStreamSynchronize(s) != cudaSuccess)
+      (void)cudaGetLastError();
+    return v;
+  };
+  auto where = [&](long long g, long long* item, long long* elem) {
+    const int64_t* hi = std::upper_bound(item_offsets, item_offsets + n_items + 1, (int64_t)g);
+    *item = (long long)(hi - item_offsets) - 1;
+    *elem = g - item_offsets[*item];
+  };
+  long long item, elem;
+  if (debug_level > 0 && ikey != kUbiNone) {
+    where((long long)ikey, &item, &elem);
+    return fail(TFCB_INVALID_ARGUMENT, "'index' has a value not in [0, %lld): value=%d (string %lld, element %lld)", R,
+                at(index, (long long)ikey), item, elem);
+  }
+  if (debug_level > 0 && rkey != kUbiNone) {
+    if (!(rkey & kUbiCdfKey))
+      return fail(TFCB_INVALID_ARGUMENT, "'cdf_size' has a value not in [3, %lld]: value=%d", W,
+                  at(cdf_size, (long long)rkey));
+    const long long r = (long long)((rkey & ~kUbiCdfKey) >> 1);
+    if (rkey & 1ull) return fail(TFCB_INVALID_ARGUMENT, "CDF is not monotonic");
+    const int sz = at(cdf_size, r);
+    return fail(TFCB_INVALID_ARGUMENT, "Each cdf should start from 0 and end at %d: cdf[0]=%d, cdf[^1]=%d",
+                1 << precision, at(cdf, r * W), at(cdf, r * W + sz - 1));
+  }
+  const long long g = (long long)(ekey >> 3);
+  where(g, &item, &elem);
+  switch ((int)(ekey & 7ull)) {
+    case kUbiIndex:
+      return fail(TFCB_INVALID_ARGUMENT, "'index' has a value not in [0, %lld): value=%d (string %lld, element %lld)",
+                  R, at(index, g), item, elem);
+    case kUbiCdfSize:
+      return fail(TFCB_INVALID_ARGUMENT, "'cdf_size' has a value not in [3, %lld]: value=%d (string %lld, element %lld)",
+                  W, at(cdf_size, at(index, g)), item, elem);
+    case kUbiInterval:
+      return fail(TFCB_INVALID_ARGUMENT,
+                  "symbol with zero probability or a CDF row beyond 2^precision (string %lld, element %lld)", item,
+                  elem);
+    case kUbiPrefix:
+      return fail(TFCB_INVALID_ARGUMENT,
+                  "damaged string: overflow width prefix exceeds %d digits of %d bits (string %lld, element %lld)",
+                  (32 + overflow_width - 1) / overflow_width, overflow_width, item, elem);
+  }
+  return fail(TFCB_CUDA_ERROR, "internal: unknown error key %llx", ekey);
+}
+
+// The error record with every key at "none".
+int ubi_reset_error(DevError* err, cudaStream_t s) {
+  TFCB_CUDA_TRY(cudaMemsetAsync(err, 0, sizeof(DevError), s));
+  TFCB_CUDA_TRY(cudaMemsetAsync(&err->stream, 0xFF, 3 * sizeof(long long), s));
+  return TFCB_OK;
+}
+
+void ubi_launch_check(const UbiParams& P, long long n, cudaStream_t s) {
+  const long long work = std::max<long long>(n, P.R);
+  const unsigned blocks = (unsigned)std::min<long long>(std::max<long long>((work + 255) / 256, 1), 1024);
+  ubi_check_kernel<<<blocks, 256, 0, s>>>(P.index, n, P.cdf, P.cdf_size, P.R, P.W, P.precision, P.err);
+  TFCB_LAUNCHED();
+}
+
+}  // namespace
+}  // namespace tfcb
+
+struct tfcb_ubi_encoder : tfcb::EncArena {
+  long long* ext = nullptr;  // device [2 * (n_streams + 1)]: element offsets, then arena offsets
+  long long* offsets = nullptr;  // the caller's string offsets
+  cudaStream_t s = nullptr;
+};
+
+namespace {
+void ubi_release(tfcb_ubi_encoder* h, cudaStream_t s) {
+  dev_free(h->state, s);
+  dev_free(h->words, s);
+  dev_free(h->cbits, s);
+  dev_free(h->err, s);
+  dev_free(h->ext, s);
+  delete h;
+}
+}  // namespace
+
+extern "C" {
+
+int tfcb_unbounded_index_range_encode_ragged(const int32_t* data_dev, const int32_t* index_dev, int64_t n_items,
+                                             const int64_t* item_offsets_host, const int32_t* cdf_dev,
+                                             const int64_t* cdf_shape_host, int cdf_rank, const int32_t* cdf_size_dev,
+                                             int64_t cdf_size_len, const int32_t* offset_dev, int64_t offset_len,
+                                             int precision, int overflow_width, int debug_level, int64_t* offsets_dev,
+                                             void* stream, tfcb_ubi_encoder** out, int64_t* total_bytes_host) {
+  TFCB_TRY(ubi_check_attrs(precision, overflow_width, debug_level));
+  TFCB_TRY(ubi_check_args(cdf_shape_host, cdf_rank, cdf_size_len, offset_len, n_items, item_offsets_host, index_dev,
+                          cdf_dev, cdf_size_dev, offset_dev));
+  if (!out || !total_bytes_host || !offsets_dev || (!data_dev && item_offsets_host[n_items] > 0))
+    return fail(TFCB_INVALID_ARGUMENT, "null pointer argument");
+  const long long S = n_items, bits = ubi_bits_bound(precision, overflow_width);
+  std::vector<long long> off(2 * (S + 1));
+  long long* arena = off.data() + S + 1;
+  long long total = 0;
+  for (long long i = 0; i <= S; ++i) {
+    off[i] = item_offsets_host[i];
+    arena[i] = total;
+    if (i == S) break;
+    const long long n = item_offsets_host[i + 1] - item_offsets_host[i];
+    if (n > ((kMaxStreamWords - 96) * 16) / bits)
+      return fail(TFCB_INVALID_ARGUMENT, "string %lld: %lld elements may not fit one code stream (2^31 16-bit words)",
+                  i, n);
+    total += (words_for(bits, n) + 32 + 31) & ~31ll;
+  }
+  *out = nullptr;
+  *total_bytes_host = 0;
+  cudaStream_t s = as_stream(stream);
+  auto* h = new tfcb_ubi_encoder;
+  h->n_streams = S;
+  h->s = s;
+  h->offsets = reinterpret_cast<long long*>(offsets_dev);
+  int rc = dev_alloc((void**)&h->state, (size_t)S * sizeof(EncState), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&h->words, (size_t)total * sizeof(uint16_t), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&h->cbits, (size_t)(total >> 5) * sizeof(uint32_t), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&h->err, sizeof(DevError), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&h->ext, off.size() * sizeof(long long), s);
+  if (rc == TFCB_OK) rc = ubi_reset_error(h->err, s);
+  if (rc == TFCB_OK) {
+    // (pageable source: staged before the call returns)
+    const cudaError_t e = cudaMemcpyAsync(h->ext, off.data(), off.size() * sizeof(long long), cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      rc = fail(TFCB_CUDA_ERROR, "UnboundedIndexRangeEncode: %s", cudaGetErrorString(e));
+    }
+  }
+  if (rc != TFCB_OK) {
+    ubi_release(h, s);
+    return rc;
+  }
+  h->arena_off = h->ext + S + 1;
+  UbiParams P{};
+  P.data = data_dev;
+  P.index = index_dev;
+  P.cdf = cdf_dev;
+  P.cdf_size = cdf_size_dev;
+  P.offset = offset_dev;
+  P.R = cdf_shape_host[0];
+  P.W = cdf_shape_host[1];
+  P.precision = precision;
+  P.width = overflow_width;
+  P.elem_off = h->ext;
+  P.arena_off = h->arena_off;
+  P.state = h->state;
+  P.words = h->words;
+  P.cbits = h->cbits;
+  P.err = h->err;
+  if (debug_level > 0) ubi_launch_check(P, item_offsets_host[S], s);
+  ubi_encode_kernel<<<(unsigned)S, 32, 0, s>>>(P);
+  TFCB_LAUNCHED();
+  long long bytes = 0;
+  DevError e{};
+  rc = enc_offsets(*h, h->offsets, false, "unbounded", s, &bytes, &e);
+  if (rc == TFCB_OK)
+    rc = ubi_error(e, debug_level, item_offsets_host, n_items, index_dev, cdf_dev, cdf_size_dev, P.R, P.W, precision,
+                   overflow_width, s);
+  if (rc != TFCB_OK) {
+    ubi_release(h, s);
+    return rc;
+  }
+  *total_bytes_host = bytes;
+  *out = h;
+  return TFCB_OK;
+}
+
+int tfcb_unbounded_index_range_write(tfcb_ubi_encoder* h, uint8_t* bytes_dev, void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "UnboundedIndexRangeEncode: not an encoder handle");
+  cudaStream_t s = as_stream(stream);
+  int rc = TFCB_OK;
+  if (!bytes_dev) {
+    rc = fail(TFCB_INVALID_ARGUMENT, "UnboundedIndexRangeEncode: null output buffer");
+  } else {
+    enc_write(*h, h->offsets, bytes_dev, s);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = fail(TFCB_CUDA_ERROR, "UnboundedIndexRangeEncode: %s", cudaGetErrorString(e));
+  }
+  ubi_release(h, s);
+  return rc;
+}
+
+void tfcb_unbounded_index_range_encoder_destroy(tfcb_ubi_encoder* h) {
+  if (h) ubi_release(h, h->s);
+}
+
+int tfcb_unbounded_index_range_decode_ragged(const uint8_t* bytes_dev, const int64_t* offsets_dev, int64_t n_items,
+                                             const int64_t* item_offsets_host, const int32_t* index_dev,
+                                             const int32_t* cdf_dev, const int64_t* cdf_shape_host, int cdf_rank,
+                                             const int32_t* cdf_size_dev, int64_t cdf_size_len,
+                                             const int32_t* offset_dev, int64_t offset_len, int precision,
+                                             int overflow_width, int debug_level, int32_t* out_dev, void* stream) {
+  TFCB_TRY(ubi_check_attrs(precision, overflow_width, debug_level));
+  TFCB_TRY(ubi_check_args(cdf_shape_host, cdf_rank, cdf_size_len, offset_len, n_items, item_offsets_host, index_dev,
+                          cdf_dev, cdf_size_dev, offset_dev));
+  if (!bytes_dev || !offsets_dev || (!out_dev && item_offsets_host[n_items] > 0))
+    return fail(TFCB_INVALID_ARGUMENT, "null pointer argument");
+  cudaStream_t s = as_stream(stream);
+  const long long S = n_items;
+  DevError* err = nullptr;
+  long long* elem_off = nullptr;
+  int rc = dev_alloc((void**)&err, sizeof(DevError), s);
+  if (rc == TFCB_OK) rc = dev_alloc((void**)&elem_off, (size_t)(S + 1) * sizeof(long long), s);
+  if (rc == TFCB_OK) rc = ubi_reset_error(err, s);
+  if (rc == TFCB_OK &&
+      cudaMemcpyAsync(elem_off, item_offsets_host, (size_t)(S + 1) * sizeof(long long), cudaMemcpyHostToDevice, s) !=
+          cudaSuccess) {
+    (void)cudaGetLastError();
+    rc = fail(TFCB_CUDA_ERROR, "UnboundedIndexRangeDecode: could not upload the item offsets");
+  }
+  DevError e{};
+  if (rc == TFCB_OK) {
+    UbiParams P{};
+    P.out = out_dev;
+    P.index = index_dev;
+    P.cdf = cdf_dev;
+    P.cdf_size = cdf_size_dev;
+    P.offset = offset_dev;
+    P.R = cdf_shape_host[0];
+    P.W = cdf_shape_host[1];
+    P.precision = precision;
+    P.width = overflow_width;
+    P.elem_off = elem_off;
+    P.bytes = bytes_dev;
+    P.str_off = reinterpret_cast<const long long*>(offsets_dev);
+    P.err = err;
+    if (debug_level > 0) ubi_launch_check(P, item_offsets_host[S], s);
+    ubi_decode_kernel<<<(unsigned)S, 32, 0, s>>>(P);
+    TFCB_LAUNCHED();
+    cudaError_t ce = cudaMemcpyAsync(&e, err, sizeof e, cudaMemcpyDeviceToHost, s);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(s);
+    if (ce != cudaSuccess) {
+      (void)cudaGetLastError();
+      rc = fail(TFCB_CUDA_ERROR, "CUDA error '%s' in UnboundedIndexRangeDecode", cudaGetErrorString(ce));
+    }
+  }
+  if (rc == TFCB_OK)
+    rc = ubi_error(e, debug_level, item_offsets_host, n_items, index_dev, cdf_dev, cdf_size_dev, cdf_shape_host[0],
+                   cdf_shape_host[1], precision, overflow_width, s);
+  dev_free(err, s);
+  dev_free(elem_off, s);
+  return rc;
 }
 
 }  // extern "C"

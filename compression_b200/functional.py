@@ -5,6 +5,7 @@ import ctypes as C
 import math
 import os
 
+import numpy as np
 import torch
 
 from compression_b200 import _lib, gen_ops
@@ -641,3 +642,35 @@ def build_lookup(pmf, pmf_length, precision):
   check(_lib.lib().tfcb_build_lookup(_p(pmf), pmf.shape[0], pmf.shape[1], lens.ctypes.data_as(C.c_void_p),
                                      int(precision), _p(lookup), _stream()))
   return lookup
+
+
+def unbounded_index_range_encode_ragged(data, index, lengths, cdf, cdf_size, offset, precision, overflow_width,
+                                        debug_level=1):
+  """UnboundedIndexRangeEncode of many strings in one launch, one warp per string: string i codes the next
+  `lengths[i]` elements of the flat int32 `data` with the same elements of `index`.  Returns a Strings of shape
+  (len(lengths),) whose string i equals gen_ops.unbounded_index_range_encode of those elements alone (the empty
+  string for a length of 0).  Errors name the lowest failing string and element."""
+  offs = _symbol_offsets(lengths)
+  gen_ops._ubi_check(precision, overflow_width, debug_level, (int(offs[-1]),), cdf, cdf_size, offset)
+  n_data, n_index = (int(np.prod(gen_ops._shape_of(x))) for x in (data, index))
+  if n_data != offs[-1] or n_index != offs[-1]:
+    raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} elements, but `data` has {n_data} and "
+                                    f"`index` {n_index}")
+  return gen_ops._ubi_encode(data, index, offs, cdf, cdf_size, offset, precision, overflow_width, debug_level)
+
+
+def unbounded_index_range_decode_ragged(strings, index, lengths, cdf, cdf_size, offset, precision, overflow_width,
+                                        debug_level=1):
+  """Inverse of unbounded_index_range_encode_ragged: `strings` (a Strings or a list of bytes) holds len(lengths)
+  strings; returns int32 [sum(lengths)], string after string.  A width prefix longer than any encoder writes raises
+  InvalidArgumentError naming the lowest failing string and element."""
+  offs = _symbol_offsets(lengths)
+  gen_ops._ubi_check(precision, overflow_width, debug_level, (int(offs[-1]),), cdf, cdf_size, offset)
+  if not isinstance(strings, gen_ops.Strings):
+    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+  if strings.numel() != offs.size - 1:
+    raise _lib.InvalidArgumentError(f"{strings.numel()} strings for {offs.size - 1} lengths")
+  n_index = int(np.prod(gen_ops._shape_of(index)))
+  if n_index != offs[-1]:
+    raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} elements, but `index` has {n_index}")
+  return gen_ops._ubi_decode(strings, index, offs, cdf, cdf_size, offset, precision, overflow_width, debug_level)

@@ -35,6 +35,8 @@ __all__ = [
     "pmf_to_quantized_cdf",
     "range_encode",
     "range_decode",
+    "unbounded_index_range_encode",
+    "unbounded_index_range_decode",
     "Strings",
     "InvalidArgumentError",
 ]
@@ -472,3 +474,99 @@ def run_length_gamma_encode(data) -> bytes:
 
 def run_length_gamma_decode(code, shape):
   return run_length_decode(code, shape, -1, -1, False)
+
+
+# ------------------------------------------------------------------------------------------------
+# UnboundedIndexRangeEncode / UnboundedIndexRangeDecode (cc/ops/range_coding_ops.cc:126-247)
+# ------------------------------------------------------------------------------------------------
+def _shape_of(x):
+  return tuple(int(d) for d in (x.shape if hasattr(x, "shape") else np.shape(x)))
+
+
+def _ubi_check(precision, overflow_width, debug_level, index_shape, cdf, cdf_size, offset, data_shape=None):
+  """The op's attribute and shape checks, in the reference's order, before anything reaches the device."""
+  if not 0 < int(precision) <= 16:
+    raise InvalidArgumentError(f"`precision` must be in [1, 16]: {precision}")
+  if not 0 < int(overflow_width) <= 16:
+    raise InvalidArgumentError(f"`overflow_width` must be in [1, 16]: {overflow_width}")
+  if int(debug_level) not in (0, 1):
+    raise InvalidArgumentError(f"`debug_level` must be 0 or 1: {debug_level}")
+  if data_shape is not None and tuple(data_shape) != tuple(index_shape):
+    raise InvalidArgumentError(f"`data` and `index` should have the same shape: data.shape={list(data_shape)}, "
+                               f"index.shape={list(index_shape)}")
+  cs, ss, os_ = _shape_of(cdf), _shape_of(cdf_size), _shape_of(offset)
+  if len(cs) != 2 or cs[1] < 3:
+    raise InvalidArgumentError(f"'cdf' should be 2-D and cdf.dim_size(1) >= 3: {list(cs)}")
+  if len(ss) != 1 or ss[0] != cs[0]:
+    raise InvalidArgumentError("'cdf_size' should be 1-D and its length should match the number of rows in "
+                               f"'cdf': {list(ss)}")
+  if len(os_) != 1 or os_[0] != cs[0]:
+    raise InvalidArgumentError("'offset' should be 1-D and its length should match the number of rows in 'cdf': "
+                               f"offset.shape={list(os_)}, cdf.shape={list(cs)}")
+
+
+def _ubi_encode(data, index, item_offsets, cdf, cdf_size, offset, precision, overflow_width, debug_level) -> Strings:
+  """Strings [k]: item u is data[item_offsets[u]:item_offsets[u + 1]] (flat int32 on the device)."""
+  dev = _device()
+  data, index = _dev(data, torch.int32).reshape(-1), _dev(index, torch.int32).reshape(-1)
+  cdf, cdf_size, offset = _dev(cdf, torch.int32), _dev(cdf_size, torch.int32), _dev(offset, torch.int32)
+  k = item_offsets.size - 1
+  cs = _shape_arr(cdf.shape)
+  offsets = torch.empty(k + 1, dtype=torch.int64, device=dev)
+  h, total = C.c_void_p(), C.c_int64(0)
+  L = _lib.lib()
+  check(L.tfcb_unbounded_index_range_encode_ragged(
+      _ptr(data), _ptr(index), k, item_offsets.ctypes.data_as(C.c_void_p), _ptr(cdf), cs.ctypes.data_as(C.c_void_p),
+      cdf.dim(), _ptr(cdf_size), cdf_size.numel(), _ptr(offset), offset.numel(), int(precision), int(overflow_width),
+      int(debug_level), _ptr(offsets), _stream(), C.byref(h), C.byref(total)))
+  try:
+    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=dev)
+  except BaseException:
+    L.tfcb_unbounded_index_range_encoder_destroy(h)
+    raise
+  check(L.tfcb_unbounded_index_range_write(h, _ptr(out), _stream()))
+  return Strings(out, offsets, (k,))
+
+
+def _ubi_decode(strings: Strings, index, item_offsets, cdf, cdf_size, offset, precision, overflow_width,
+                debug_level) -> torch.Tensor:
+  """Flat int32 [item_offsets[-1]]: string u decoded into elements item_offsets[u]:item_offsets[u + 1]."""
+  index = _dev(index, torch.int32).reshape(-1)
+  cdf, cdf_size, offset = _dev(cdf, torch.int32), _dev(cdf_size, torch.int32), _dev(offset, torch.int32)
+  k = item_offsets.size - 1
+  cs = _shape_arr(cdf.shape)
+  out = torch.empty(int(item_offsets[-1]), dtype=torch.int32, device=index.device)
+  check(_lib.lib().tfcb_unbounded_index_range_decode_ragged(
+      _ptr(strings.bytes_dev), _ptr(strings.offsets_dev), k, item_offsets.ctypes.data_as(C.c_void_p), _ptr(index),
+      _ptr(cdf), cs.ctypes.data_as(C.c_void_p), cdf.dim(), _ptr(cdf_size), cdf_size.numel(), _ptr(offset),
+      offset.numel(), int(precision), int(overflow_width), int(debug_level), _ptr(out), _stream()))
+  return out
+
+
+def unbounded_index_range_encode(data, index, cdf, cdf_size, offset, precision: int, overflow_width: int,
+                                 debug_level: int = 1) -> bytes:
+  """UnboundedIndexRangeEncode: int32 `data` coded with row index[i] of `cdf` (first cdf_size[r] entries, the last
+  bin the escape) into one byte string; values outside [offset[r], offset[r] + cdf_size[r] - 2) escape into
+  overflow_width-bit digits."""
+  _ubi_check(precision, overflow_width, debug_level, _shape_of(index), cdf, cdf_size, offset, _shape_of(data))
+  n = _prod(_shape_of(data))
+  s = _ubi_encode(data, index, np.array([0, n], np.int64), cdf, cdf_size, offset, precision, overflow_width,
+                  debug_level)
+  return s.tolist()[0]
+
+
+def unbounded_index_range_decode(encoded, index, cdf, cdf_size, offset, precision: int, overflow_width: int,
+                                 debug_level: int = 1) -> torch.Tensor:
+  """UnboundedIndexRangeDecode: the inverse; returns int32 shaped like `index`."""
+  if isinstance(encoded, Strings):
+    if encoded.shape != ():
+      raise InvalidArgumentError(f"`encoded` should be a scalar: {list(encoded.shape)}")
+  elif not isinstance(encoded, (bytes, bytearray)):
+    raise InvalidArgumentError(f"`encoded` should be a scalar: {list(np.shape(encoded))}")
+  shape = _shape_of(index)
+  _ubi_check(precision, overflow_width, debug_level, shape, cdf, cdf_size, offset)
+  if not isinstance(encoded, Strings):
+    encoded = Strings.from_bytes(bytes(encoded))
+  out = _ubi_decode(encoded, index, np.array([0, _prod(shape)], np.int64), cdf, cdf_size, offset, precision,
+                    overflow_width, debug_level)
+  return out.reshape(shape)

@@ -195,6 +195,45 @@ int tfcb_range_decode(const uint8_t* encoded_host, int64_t n_bytes, const int64_
                       int precision, int debug_level, int16_t* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * UnboundedIndexRangeEncode / UnboundedIndexRangeDecode over a ragged batch, one warp per string:
+ *   op contract   tensorflow_compression/cc/ops/range_coding_ops.cc:126-247
+ *   CPU kernels   tensorflow_compression/cc/kernels/unbounded_index_range_coding_kernels.cc
+ * Item u is elements [item_offsets_host[u], item_offsets_host[u+1]) of data_dev / index_dev (int32, flat); string u is
+ * byte-identical to the reference op on item u alone wherever the reference is defined, and an empty item gives the
+ * empty string.  cdf_dev int32 [cdf_shape_host[0], cdf_shape_host[1]] (cdf_rank 2, at least 3 columns), cdf_size_dev
+ * and offset_dev int32 [rows].  Outside the reference's defined domain (DESIGN.md §3.8) d and u wrap as uint32, so
+ * decoding what the encoder wrote gives back every int32 input.
+ * Checked before any device work (TFCB_INVALID_ARGUMENT, with the reference's messages): precision and
+ * overflow_width in [1, 16], debug_level 0 or 1, the shapes, null pointers, and the item offsets as for
+ * tfcb_compress_ragged.  On the device, whatever debug_level is: index in [0, rows), cdf_size in [3, cols], and a
+ * non-empty interval for every coded bin; debug_level 1 also checks every index and, per row, the start, end and
+ * monotonicity of its cdf_size prefix.  Failures name the lowest failing string and element.
+ * tfcb_unbounded_index_range_encode_ragged writes where each string starts to `offsets_dev` int64 [n_items + 1],
+ * synchronises once and returns the total size and a handle; tfcb_unbounded_index_range_write writes the strings
+ * back to back into `bytes_dev` [total] (asynchronous) and takes the handle back, also when it fails;
+ * tfcb_unbounded_index_range_encoder_destroy releases a handle that is never written.
+ * tfcb_unbounded_index_range_decode_ragged decodes string u (bytes_dev[offsets_dev[u] .. offsets_dev[u+1]), device
+ * offsets) into out_dev[item_offsets_host[u] ..) and synchronises once.  Damaged strings decode to what the
+ * reference decoder gives, except that a width prefix longer than ceil(32 / overflow_width) digits (undefined in the
+ * reference) is reported as TFCB_INVALID_ARGUMENT naming the lowest failing string and element.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct tfcb_ubi_encoder tfcb_ubi_encoder;
+int tfcb_unbounded_index_range_encode_ragged(const int32_t* data_dev, const int32_t* index_dev, int64_t n_items,
+                                             const int64_t* item_offsets_host, const int32_t* cdf_dev,
+                                             const int64_t* cdf_shape_host, int cdf_rank, const int32_t* cdf_size_dev,
+                                             int64_t cdf_size_len, const int32_t* offset_dev, int64_t offset_len,
+                                             int precision, int overflow_width, int debug_level, int64_t* offsets_dev,
+                                             void* stream, tfcb_ubi_encoder** out, int64_t* total_bytes_host);
+int tfcb_unbounded_index_range_write(tfcb_ubi_encoder* h, uint8_t* bytes_dev, void* stream);
+void tfcb_unbounded_index_range_encoder_destroy(tfcb_ubi_encoder* h);
+int tfcb_unbounded_index_range_decode_ragged(const uint8_t* bytes_dev, const int64_t* offsets_dev, int64_t n_items,
+                                             const int64_t* item_offsets_host, const int32_t* index_dev,
+                                             const int32_t* cdf_dev, const int64_t* cdf_shape_host, int cdf_rank,
+                                             const int32_t* cdf_size_dev, int64_t cdf_size_len,
+                                             const int32_t* offset_dev, int64_t offset_len, int precision,
+                                             int overflow_width, int debug_level, int32_t* out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * PmfToQuantizedCdf:
  *   op contract   tensorflow_compression/cc/ops/pmf_to_cdf_ops.cc:28-57
  *   CPU kernel    tensorflow_compression/cc/kernels/pmf_to_cdf_kernels.cc:58-208
