@@ -55,12 +55,18 @@ SIGNATURES = {
                                     _p(_i64)]),
     "tfcb_compress_ragged_decoded": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
                                             _p(_vp), _p(_i64), _vp]),
+    "tfcb_compress_16bit": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _int, _vp, _int, _vp, _i64, _vp, _vp, _p(_vp),
+                                   _p(_i64)]),
+    "tfcb_compress_ragged_16bit": (_int, [_vp, _i64, _i64, _i64, _vp, _vp, _vp, _int, _vp, _int, _vp, _vp, _vp, _vp,
+                                          _p(_vp), _p(_i64)]),
     "tfcb_decoder_create": (_int, [_vp, _vp, _i64, _vp, _i64, _i64, _vp, _p(_vp)]),
     "tfcb_decode_channel": (_int, [_vp, _vp, _i64, _vp]),
     "tfcb_decode_index": (_int, [_vp, _vp, _vp, _i64, _vp]),
     "tfcb_decode_channel_f32": (_int, [_vp, _vp, _vp, _vp, _i64, _vp]),
     "tfcb_decode_index_f32": (_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "tfcb_decode_ragged": (_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "tfcb_decode_16bit": (_int, [_vp, _vp, _vp, _int, _vp, _int, _vp, _i64, _vp]),
+    "tfcb_decode_ragged_16bit": (_int, [_vp, _vp, _vp, _vp, _int, _vp, _int, _vp, _vp]),
     "tfcb_decode_finalize": (_int, [_vp, _vp, _vp]),
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),

@@ -28,6 +28,9 @@
 #include <mutex>
 #include <vector>
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace tfcb {
@@ -345,8 +348,13 @@ struct EncDrain {
   }
 };
 
-// kModeDecoded (encoder only, with kModeF32): the gather warp also writes every symbol's decoded value.
-enum : int { kModeIndex = 1, kModeF32 = 2, kModeDecoded = 4 };
+// kModeDecoded (encoder only, with kModeF32 or a 16-bit mode): the gather warp also writes every symbol's decoded
+// value.  kModeH16 / kModeB16: the value is float16 / bfloat16, quantised and dequantised with the arithmetic of the
+// entropy models' unfused 16-bit path (enc_gather, dequantise16).  kModeLocF32 (index mode with a 16-bit value): the
+// loc is float32, and so is the decoded value (torch's type promotion); without it the loc is in the value's type.
+enum : int { kModeIndex = 1, kModeF32 = 2, kModeDecoded = 4, kModeH16 = 8, kModeB16 = 16, kModeLocF32 = 32 };
+constexpr int kMode16 = kModeH16 | kModeB16;
+constexpr int kModeFloat = kModeF32 | kMode16;  // float values: quantised in the kernel, cdf_offset is read
 
 struct EncParams {
   const int32_t* lookup;
@@ -370,9 +378,36 @@ struct EncParams {
   const long long* sym_off;
   const long long* arena_off;
   // kModeDecoded: float [n symbols in all], what the f32 decoder returns for each symbol (last: the other fields keep
-  // their parameter offsets)
+  // their parameter offsets); in 16-bit modes only under kModeLocF32
   float* decoded;
+  // 16-bit modes (after `decoded`, for the same reason): loc [S, n] in the value's type (index mode without
+  // kModeLocF32; may be null), and kModeDecoded's output in the value's type (without kModeLocF32)
+  const uint16_t* loc16;
+  uint16_t* decoded16;
 };
+
+// 16-bit values as float32 (exact) and float32 rounded to the nearest 16-bit value (ties to even; overflow to inf,
+// NaN stays NaN): the conversions torch's elementwise kernels make on the device.
+template <int MODE>
+__device__ __forceinline__ float widen16(uint32_t bits) {
+  if (MODE & kModeH16) return __half2float(__ushort_as_half((unsigned short)bits));
+  return __bfloat162float(__ushort_as_bfloat16((unsigned short)bits));
+}
+template <int MODE>
+__device__ __forceinline__ uint16_t narrow16(float x) {
+  if (MODE & kModeH16) return __half_as_ushort(__float2half_rn(x));
+  return __bfloat16_as_ushort(__float2bfloat16_rn(x));
+}
+
+// The 16-bit dequantisation of entropy_models._dequantize: the int32 sum `sc` = symbol + cdf_offset cast to the
+// value's type as torch casts int32 (to float, then to 16 bits: two roundings), then plus the offset `off` (widened
+// to float32) in float32.  The caller rounds the result once to the value's type, or stores it as float32 under
+// kModeLocF32, where torch promotes the sum with a float32 loc.
+template <int MODE>
+__device__ __forceinline__ float dequantise16(int sc, bool has_off, float off) {
+  const float h = widen16<MODE>(narrow16<MODE>((float)sc));
+  return has_off ? h + off : h;
+}
 
 // Where one stream's symbols (or arena words) are: resolved once per CTA from the offsets array when there is one,
 // else from the uniform stride.
@@ -398,6 +433,9 @@ struct Fetched {
   int row;
   int2 ri;
   bool valid;
+  // 16-bit modes: the value's (and a 16-bit loc's) bits as loaded, widened in stage B -- a conversion in stage A
+  // would wait for the load there
+  uint32_t y16, loc16;
 };
 
 struct Gathered {
@@ -417,19 +455,29 @@ __device__ __forceinline__ Fetched enc_fetch(const EncParams& P, long long end, 
   f.coff = 0;
   f.row = (int)chan_row;
   f.ri = make_int2(0, 0);
+  if (MODE & kMode16) {
+    f.y16 = 0;
+    f.loc16 = 0;
+  }
   f.valid = at < end;
   if (!f.valid) return f;
   if (MODE & kModeF32) {
     f.y = __ldg(reinterpret_cast<const float*>(P.value) + at);
+  } else if (MODE & kMode16) {
+    f.y16 = __ldg(reinterpret_cast<const unsigned short*>(P.value) + at);
   } else {
     f.v = __ldg(reinterpret_cast<const int32_t*>(P.value) + at);
   }
   if (MODE & kModeIndex) {
     f.row = __ldg(P.index + at);
-    if ((MODE & kModeF32) && P.qoff) f.loc_or_q = __ldg(P.qoff + at);
+    if ((MODE & kMode16) && !(MODE & kModeLocF32)) {
+      if (P.loc16) f.loc16 = __ldg(P.loc16 + at);
+    } else if ((MODE & kModeFloat) && P.qoff) {
+      f.loc_or_q = __ldg(P.qoff + at);
+    }
   } else {
     f.ri = __ldg(P.rows + f.row);
-    if (MODE & kModeF32) {
+    if (MODE & kModeFloat) {
       if (P.qoff) f.loc_or_q = __ldg(P.qoff + f.row);
       f.coff = __ldg(P.coff + f.row);
     }
@@ -453,17 +501,38 @@ __device__ __forceinline__ Gathered enc_gather(const EncParams& P, long long s, 
       return g;
     }
     f.ri = __ldg(P.rows + f.row);
-    if (MODE & kModeF32) f.coff = __ldg(P.coff + f.row);
+    if (MODE & kModeFloat) f.coff = __ldg(P.coff + f.row);
+  }
+  if (MODE & kMode16) {
+    f.y = widen16<MODE>(f.y16);
+    if ((MODE & kModeIndex) && !(MODE & kModeLocF32)) f.loc_or_q = widen16<MODE>(f.loc16);  // (+0 without a loc)
   }
   int v = f.v;
-  if (MODE & kModeF32) v = (int)rintf(f.y - f.loc_or_q) - f.coff;
+  if (MODE & kModeFloat) {
+    // 16-bit values: channel mode quantises the value widened to float32 against the float32 quantisation offset,
+    // as does index mode with a float32 loc (torch promotes the difference to float32); with a loc in the value's
+    // type (or none) index mode rounds the difference to that type first, as the unfused path's 16-bit subtraction
+    float d = f.y - f.loc_or_q;
+    if ((MODE & kMode16) && (MODE & kModeIndex) && !(MODE & kModeLocF32)) d = widen16<MODE>(narrow16<MODE>(d));
+    v = (int)rintf(d) - f.coff;
+  }
   if (MODE & kModeDecoded) {
     // the resolve warp's dequantisation of the symbol it decodes (v, before the escape mapping): the same integer
     // and the same float operations, so the value is bit-identical to the decoder's -- including the saturated
     // conversion of |y - loc| >= 2^31 and NaN -> 0, which recomputing rintf(y - loc) + loc would not reproduce
-    float yv = (float)(v + f.coff);
-    if (P.qoff) yv += f.loc_or_q;
-    P.decoded[at] = yv;
+    if (MODE & kMode16) {
+      const bool loc16 = (MODE & kModeIndex) && !(MODE & kModeLocF32);
+      const bool has_off = loc16 ? P.loc16 != nullptr : P.qoff != nullptr;
+      // channel mode adds the quantisation offset rounded to the value's type (_dequantize's off.to(out.dtype))
+      const float off = (MODE & kModeIndex) ? f.loc_or_q : widen16<MODE>(narrow16<MODE>(f.loc_or_q));
+      const float r = dequantise16<MODE>(v + f.coff, has_off, off);
+      if (MODE & kModeLocF32) P.decoded[at] = r;
+      else P.decoded16[at] = narrow16<MODE>(r);
+    } else {
+      float yv = (float)(v + f.coff);
+      if (P.qoff) yv += f.loc_or_q;
+      P.decoded[at] = yv;
+    }
   }
   const int ncdf = row_ncdf(f.ri.y);
   if (!row_ovf(f.ri.y)) {
@@ -974,6 +1043,9 @@ struct DecParams {
   DecState* state;
   DevError* err;
   const long long* sym_off;  // ragged batches: stream s is symbols [sym_off[s], sym_off[s+1]); null: [s * n, s * n + n)
+  // 16-bit index modes without kModeLocF32: loc [S, n] in the output's type, or null (last: the other fields keep
+  // their parameter offsets).  `out` is in the value's type, float under kModeLocF32; `qoff` is float32 otherwise.
+  const uint16_t* loc16;
 };
 
 struct ByteWindow {
@@ -1312,7 +1384,24 @@ __global__ void __launch_bounds__(96) decode_kernel(const DecParams P) {
             }
             sym = hi - 1;
           }
-          if (MODE & kModeF32) {
+          if (MODE & kMode16) {
+            const int sc = sym + __ldg(P.coff + row);
+            float off = 0.f;
+            bool has_off;
+            if (!(MODE & kModeIndex)) {  // the quantisation offset rounded to the value's type, as in enc_gather
+              has_off = P.qoff != nullptr;
+              if (has_off) off = widen16<MODE>(narrow16<MODE>(__ldg(P.qoff + row)));
+            } else if (MODE & kModeLocF32) {
+              has_off = true;
+              off = __ldg(P.qoff + at);
+            } else {
+              has_off = P.loc16 != nullptr;
+              if (has_off) off = widen16<MODE>(__ldg(P.loc16 + at));
+            }
+            const float r = dequantise16<MODE>(sc, has_off, off);
+            if (MODE & kModeLocF32) reinterpret_cast<float*>(P.out)[at] = r;
+            else reinterpret_cast<uint16_t*>(P.out)[at] = narrow16<MODE>(r);
+          } else if (MODE & kModeF32) {
             float yv = (float)(sym + __ldg(P.coff + row));
             if (P.qoff) yv += (MODE & kModeIndex) ? __ldg(P.qoff + at) : __ldg(P.qoff + row);
             reinterpret_cast<float*>(P.out)[at] = yv;
@@ -1907,18 +1996,18 @@ int prepare_ragged(tfcb_encoder* h, const int64_t* sym_off, cudaStream_t s) {
 }
 
 // `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all, laid out by prepare_ragged.
-// `decoded`: the kModeDecoded output.
+// `decoded` / `decoded16`: the kModeDecoded output; `loc16`: the 16-bit loc (EncParams).
 template <int MODE>
 int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, const float* qoff,
                   const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr,
-                  float* decoded = nullptr) {
+                  float* decoded = nullptr, const uint16_t* loc16 = nullptr, uint16_t* decoded16 = nullptr) {
   if (h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
   if (h->lut.n_rows == 0) return fail(TFCB_INVALID_ARGUMENT, "index=0 not in range [0, 0)");
   if (value == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`value` is null");
   if ((MODE & kModeIndex) && index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
-  if ((MODE & kModeF32) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  if ((MODE & kModeFloat) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
   if (!sym_off) {
     const long long extra = words_bound(h, n);
     TFCB_TRY(ensure_capacity(h, extra, s));
@@ -1944,6 +2033,8 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.sym_off = sym_off;
   P.arena_off = h->arena_off;
   P.decoded = decoded;
+  P.loc16 = loc16;
+  P.decoded16 = decoded16;
   if (h->n_streams > 0x7FFFFFFFll) return fail(TFCB_INVALID_ARGUMENT, "too many streams");
   encode_kernel<MODE><<<(unsigned)h->n_streams, 192, 0, s>>>(P);
   TFCB_LAUNCHED();
@@ -2202,13 +2293,29 @@ int checkout_encoder(const int32_t* lookup_host, int64_t lookup_len, int64_t loo
   return TFCB_OK;
 }
 
-// The common part of tfcb_compress, tfcb_compress_ragged and tfcb_compress_ragged_decoded: one encode of a
-// checked-out encoder, finalize, and the encoder either handed to the caller or taken back.  `decoded` non-null
-// (float values only): the encode also writes the decoded values there.
-int compress_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
-                         const float* qoff_dev, const int32_t* cdf_offset_dev, long long n, const long long* sym_off,
-                         int64_t* offsets_dev, cudaStream_t s, tfcb_encoder** out, int64_t* total_bytes_host,
-                         float* decoded = nullptr) {
+// After the encode of a checked-out encoder (`rc` its result): finalize, and the encoder either handed to the caller
+// or taken back.
+int finish_compress(tfcb_encoder* h, int rc, int64_t* offsets_dev, cudaStream_t s, tfcb_encoder** out,
+                    int64_t* total_bytes_host) {
+  long long total = 0;
+  if (rc == TFCB_OK)
+    rc = finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
+  if (rc != TFCB_OK) {
+    // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
+    if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
+    else tfcb_encoder_destroy(h);
+    return rc;
+  }
+  *out = h;
+  *total_bytes_host = total;
+  return TFCB_OK;
+}
+
+// The encode of tfcb_compress, tfcb_compress_ragged and tfcb_compress_ragged_decoded on a checked-out encoder.
+// `decoded` non-null (float values only): the encode also writes the decoded values there.
+int encode_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
+                       const float* qoff_dev, const int32_t* cdf_offset_dev, long long n, const long long* sym_off,
+                       cudaStream_t s, float* decoded = nullptr) {
   const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0) | (decoded ? kModeDecoded : 0);
   int rc;
   switch (mode) {
@@ -2228,18 +2335,63 @@ int compress_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* 
       break;
     default: rc = fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values"); break;
   }
-  long long total = 0;
-  if (rc == TFCB_OK)
-    rc = finalize_encoder(h, reinterpret_cast<long long*>(offsets_dev), /*reset_err=*/true, s, &total);
-  if (rc != TFCB_OK) {
-    // argument errors leave the encoder clean (the finalize kernel cleared the error record): keep it
-    if (rc == TFCB_INVALID_ARGUMENT) encoder_pool().give(h);
-    else tfcb_encoder_destroy(h);
-    return rc;
-  }
-  *out = h;
-  *total_bytes_host = total;
+  return rc;
+}
+
+// The 16-bit value types' host-side arguments, checked before any device work: `dtype` 1 float16 or 2 bfloat16;
+// `loc_dtype` 0 (float32), or in index mode also `dtype`; cdf_offset always, and the value (or output) whenever
+// there are symbols.
+int check16(int dtype, bool index_mode, int loc_dtype, const void* data, const char* data_name,
+            const int32_t* cdf_offset_dev, long long n_symbols) {
+  if (dtype != 1 && dtype != 2)
+    return fail(TFCB_INVALID_ARGUMENT, "`dtype` must be 1 (float16) or 2 (bfloat16): %d", dtype);
+  if (loc_dtype != 0 && !(index_mode && loc_dtype == dtype))
+    return fail(TFCB_INVALID_ARGUMENT, "`loc_dtype` must be 0 (float32)%s: %d",
+                index_mode ? " or the value's `dtype`" : " in channel mode", loc_dtype);
+  if (!cdf_offset_dev) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  if (n_symbols > 0 && !data) return fail(TFCB_INVALID_ARGUMENT, "`%s` is null", data_name);
   return TFCB_OK;
+}
+
+// The modes of a 16-bit call: the value's type, index mode, and a float32 loc in index mode (kModeLocF32, which
+// also makes the decoded values float32).  The loc is float32 in channel mode (the quantisation offsets).
+int mode16(int dtype, const int32_t* index, const void* loc, int loc_dtype) {
+  return (dtype == 1 ? kModeH16 : kModeB16) | (index ? kModeIndex : 0) | (index && loc && loc_dtype == 0 ? kModeLocF32 : 0);
+}
+
+template <int MODE>
+int encode16(tfcb_encoder* h, const void* value, const int32_t* index, const void* loc, const int32_t* coff,
+             long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
+  constexpr bool loc16 = (MODE & kModeIndex) && !(MODE & kModeLocF32);
+  return launch_encode<MODE>(h, value, index, loc16 ? nullptr : static_cast<const float*>(loc), coff, n, s, sym_off,
+                             (MODE & kModeLocF32) ? static_cast<float*>(decoded) : nullptr,
+                             loc16 ? static_cast<const uint16_t*>(loc) : nullptr,
+                             (MODE & kModeLocF32) ? nullptr : static_cast<uint16_t*>(decoded));
+}
+
+// One encode of a 16-bit value (`decoded` non-null: kModeDecoded) with the mode mode16 selects.
+template <int DT>
+int encode16_of(int mode, tfcb_encoder* h, const void* value, const int32_t* index, const void* loc,
+                const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
+  switch ((mode & ~kMode16) | (decoded ? kModeDecoded : 0)) {
+    case 0: return encode16<DT>(h, value, index, loc, coff, n, s, sym_off, decoded);
+    case kModeDecoded: return encode16<DT | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off, decoded);
+    case kModeIndex: return encode16<DT | kModeIndex>(h, value, index, loc, coff, n, s, sym_off, decoded);
+    case kModeIndex | kModeDecoded:
+      return encode16<DT | kModeIndex | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off, decoded);
+    case kModeIndex | kModeLocF32:
+      return encode16<DT | kModeIndex | kModeLocF32>(h, value, index, loc, coff, n, s, sym_off, decoded);
+    default:
+      return encode16<DT | kModeIndex | kModeLocF32 | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off,
+                                                                     decoded);
+  }
+}
+
+int encode16_any(int dtype, tfcb_encoder* h, const void* value, const int32_t* index, const void* loc, int loc_dtype,
+                 const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
+  const int mode = mode16(dtype, index, loc, loc_dtype);
+  if (mode & kModeH16) return encode16_of<kModeH16>(mode, h, value, index, loc, coff, n, s, sym_off, decoded);
+  return encode16_of<kModeB16>(mode, h, value, index, loc, coff, n, s, sym_off, decoded);
 }
 
 }  // namespace
@@ -2258,19 +2410,40 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
   cudaStream_t s = as_stream(stream);
   tfcb_encoder* h = nullptr;
   TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
-  return compress_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev, n, nullptr,
-                              offsets_dev, s, out, total_bytes_host);
+  return finish_compress(h, encode_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev, n,
+                                               nullptr, s),
+                         offsets_dev, s, out, total_bytes_host);
+}
+
+int tfcb_compress_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                        const int32_t* index_dev, const void* value_dev, int dtype, const void* loc_dev, int loc_dtype,
+                        const int32_t* cdf_offset_dev, int64_t n, int64_t* offsets_dev, void* stream,
+                        tfcb_encoder** out, int64_t* total_bytes_host) {
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  *out = nullptr;
+  *total_bytes_host = 0;
+  if (n_streams < 0) return fail(TFCB_INVALID_ARGUMENT, "negative stream count");
+  if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, value_dev, "value", cdf_offset_dev, n_streams * n));
+  cudaStream_t s = as_stream(stream);
+  tfcb_encoder* h = nullptr;
+  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
+  return finish_compress(h, encode16_any(dtype, h, value_dev, index_dev, loc_dev, loc_dtype, cdf_offset_dev, n, s,
+                                         nullptr, nullptr),
+                         offsets_dev, s, out, total_bytes_host);
 }
 
 }  // extern "C"
 
 namespace {
 
-// tfcb_compress_ragged, and tfcb_compress_ragged_decoded with `decoded` non-null.
+// What the ragged compress entries share: the host-side checks, an encoder laid out for the batch, then
+// `encode(h, n_symbols, device symbol offsets, stream)` and finish_compress.
+template <typename Encode>
 int compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
-                    const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
-                    int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev, int64_t* offsets_dev,
-                    float* decoded, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
+                    const int64_t* symbol_offsets_host, int64_t* offsets_dev, void* stream, tfcb_encoder** out,
+                    int64_t* total_bytes_host, Encode encode) {
   if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
   *out = nullptr;
   *total_bytes_host = 0;
@@ -2299,8 +2472,22 @@ int compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t look
     tfcb_encoder_destroy(h);
     return rc;
   }
-  return compress_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev,
-                              symbol_offsets_host[n_streams], h->ext, offsets_dev, s, out, total_bytes_host, decoded);
+  return finish_compress(h, encode(h, (long long)symbol_offsets_host[n_streams], h->ext, s), offsets_dev, s, out,
+                         total_bytes_host);
+}
+
+// tfcb_compress_ragged, and tfcb_compress_ragged_decoded with `decoded` non-null.
+int compress_ragged_f32(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                        const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                        int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
+                        int64_t* offsets_dev, float* decoded, void* stream, tfcb_encoder** out,
+                        int64_t* total_bytes_host) {
+  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, offsets_dev, stream,
+                         out, total_bytes_host,
+                         [&](tfcb_encoder* h, long long n, const long long* sym_off, cudaStream_t s) {
+                           return encode_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev,
+                                                     n, sym_off, s, decoded);
+                         });
 }
 
 }  // namespace
@@ -2311,8 +2498,9 @@ int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t
                          const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
                          int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
                          int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
-  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev, value_dev,
-                         value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, nullptr, stream, out, total_bytes_host);
+  return compress_ragged_f32(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev,
+                             value_dev, value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, nullptr, stream, out,
+                             total_bytes_host);
 }
 
 int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols,
@@ -2325,9 +2513,27 @@ int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len,
   if (!value_is_f32) return fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values (`value_is_f32` is 0)");
   if (!decoded_dev) return fail(TFCB_INVALID_ARGUMENT, "`decoded` is null");
   if (!cdf_offset_dev) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
-  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev, value_dev,
-                         value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, decoded_dev, stream, out,
-                         total_bytes_host);
+  return compress_ragged_f32(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev,
+                             value_dev, value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, decoded_dev, stream, out,
+                             total_bytes_host);
+}
+
+int tfcb_compress_ragged_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                               const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                               int dtype, const void* loc_dev, int loc_dtype, const int32_t* cdf_offset_dev,
+                               void* decoded_dev, int64_t* offsets_dev, void* stream, tfcb_encoder** out,
+                               int64_t* total_bytes_host) {
+  if (out) *out = nullptr;
+  if (total_bytes_host) *total_bytes_host = 0;
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
+  TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, value_dev, "value", cdf_offset_dev,
+                   symbol_offsets_host[n_streams]));
+  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, offsets_dev, stream,
+                         out, total_bytes_host,
+                         [&](tfcb_encoder* h, long long n, const long long* sym_off, cudaStream_t s) {
+                           return encode16_any(dtype, h, value_dev, index_dev, loc_dev, loc_dtype, cdf_offset_dev, n,
+                                               s, sym_off, decoded_dev);
+                         });
 }
 
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
@@ -2361,16 +2567,17 @@ struct tfcb_decoder {
 
 namespace {
 
-// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all.
+// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all.  `loc16`: DecParams.
 template <int MODE>
 int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr) {
+                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr,
+                  const uint16_t* loc16 = nullptr) {
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
   if (h->lut.n_rows == 0) return fail(TFCB_INVALID_ARGUMENT, "index=0 not in range [0, 0)");
   if (out == nullptr) return fail(TFCB_INVALID_ARGUMENT, "output is null");
   if ((MODE & kModeIndex) && index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
-  if ((MODE & kModeF32) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  if ((MODE & kModeFloat) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
   DecParams P;
   P.lookup = h->lut.lookup;
   P.rows = h->lut.rows;
@@ -2391,6 +2598,7 @@ int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float*
   P.state = h->state;
   P.err = h->err;
   P.sym_off = sym_off;
+  P.loc16 = loc16;
   // Search keys live in shared memory whenever they fit beside the kernel's static 16 KB: up to 96 KB two CTAs
   // (streams) still share an SM; up to 200 KB one CTA per SM (cfg3's 64 NoisyNormal tables up to sigma = 256 take
   // 118 KB: from L1/L2 every slow-path search round cost a global-memory latency on the chain warp).
@@ -2404,6 +2612,45 @@ int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float*
   }
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+template <int MODE>
+int decode16(tfcb_decoder* h, const int32_t* index, void* out, const void* loc, const int32_t* coff, long long n,
+             cudaStream_t s, const long long* sym_off) {
+  constexpr bool loc16 = (MODE & kModeIndex) && !(MODE & kModeLocF32);
+  return launch_decode<MODE>(h, index, out, loc16 ? nullptr : static_cast<const float*>(loc), coff, n, s, sym_off,
+                             loc16 ? static_cast<const uint16_t*>(loc) : nullptr);
+}
+
+template <int DT>
+int decode16_of(int mode, tfcb_decoder* h, const int32_t* index, void* out, const void* loc, const int32_t* coff,
+                long long n, cudaStream_t s, const long long* sym_off) {
+  switch (mode & ~kMode16) {
+    case 0: return decode16<DT>(h, index, out, loc, coff, n, s, sym_off);
+    case kModeIndex: return decode16<DT | kModeIndex>(h, index, out, loc, coff, n, s, sym_off);
+    default: return decode16<DT | kModeIndex | kModeLocF32>(h, index, out, loc, coff, n, s, sym_off);
+  }
+}
+
+// One decode of 16-bit values with the mode mode16 selects.
+int decode16_any(int dtype, tfcb_decoder* h, const int32_t* index, void* out, const void* loc, int loc_dtype,
+                 const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off) {
+  const int mode = mode16(dtype, index, loc, loc_dtype);
+  if (mode & kModeH16) return decode16_of<kModeH16>(mode, h, index, out, loc, coff, n, s, sym_off);
+  return decode16_of<kModeB16>(mode, h, index, out, loc, coff, n, s, sym_off);
+}
+
+// A ragged decode's symbol offsets, checked and copied to the decoder (`*n`: the symbols in all; nothing is copied
+// when there are none).
+int upload_symbol_offsets(tfcb_decoder* h, const int64_t* symbol_offsets_host, cudaStream_t s, long long* n) {
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, h->n_streams));
+  *n = symbol_offsets_host[h->n_streams];
+  if (*n == 0) return TFCB_OK;
+  if (!h->sym_off) TFCB_TRY(dev_alloc((void**)&h->sym_off, (h->n_streams + 1) * sizeof(long long), s));
+  // (pageable source: staged before the call returns; an earlier decode on this stream has read the old offsets)
+  TFCB_CUDA_TRY(cudaMemcpyAsync(h->sym_off, symbol_offsets_host, (h->n_streams + 1) * sizeof(long long),
+                                cudaMemcpyHostToDevice, s));
   return TFCB_OK;
 }
 
@@ -2470,14 +2717,10 @@ int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, cons
                        int32_t out_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev,
                        void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, h->n_streams));
-  const long long n = symbol_offsets_host[h->n_streams];
-  if (n == 0) return TFCB_OK;
   cudaStream_t s = as_stream(stream);
-  if (!h->sym_off) TFCB_TRY(dev_alloc((void**)&h->sym_off, (h->n_streams + 1) * sizeof(long long), s));
-  // (pageable source: staged before the call returns; an earlier decode on this stream has read the old offsets)
-  TFCB_CUDA_TRY(cudaMemcpyAsync(h->sym_off, symbol_offsets_host, (h->n_streams + 1) * sizeof(long long),
-                                cudaMemcpyHostToDevice, s));
+  long long n = 0;
+  TFCB_TRY(upload_symbol_offsets(h, symbol_offsets_host, s, &n));
+  if (n == 0) return TFCB_OK;
   const float* q = quant_offset_dev;
   const int32_t* c = cdf_offset_dev;
   switch ((index_dev ? kModeIndex : 0) | (out_is_f32 ? kModeF32 : 0)) {
@@ -2486,6 +2729,28 @@ int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, cons
     case kModeF32: return launch_decode<kModeF32>(h, nullptr, out_dev, q, c, n, s, h->sym_off);
     default: return launch_decode<kModeIndex | kModeF32>(h, index_dev, out_dev, q, c, n, s, h->sym_off);
   }
+}
+
+int tfcb_decode_16bit(tfcb_decoder* h, const int32_t* index_dev, void* out_dev, int dtype, const void* loc_dev,
+                      int loc_dtype, const int32_t* cdf_offset_dev, int64_t n_per_stream, void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
+  if (n_per_stream < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
+  TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, out_dev, "out", cdf_offset_dev, h->n_streams * n_per_stream));
+  return decode16_any(dtype, h, index_dev, out_dev, loc_dev, loc_dtype, cdf_offset_dev, n_per_stream,
+                      as_stream(stream), nullptr);
+}
+
+int tfcb_decode_ragged_16bit(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev,
+                             void* out_dev, int dtype, const void* loc_dev, int loc_dtype,
+                             const int32_t* cdf_offset_dev, void* stream) {
+  if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, h->n_streams));
+  TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, out_dev, "out", cdf_offset_dev,
+                   symbol_offsets_host[h->n_streams]));
+  cudaStream_t s = as_stream(stream);
+  long long n = 0;
+  TFCB_TRY(upload_symbol_offsets(h, symbol_offsets_host, s, &n));
+  return decode16_any(dtype, h, index_dev, out_dev, loc_dev, loc_dtype, cdf_offset_dev, n, s, h->sym_off);
 }
 
 int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream) {

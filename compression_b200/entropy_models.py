@@ -258,11 +258,21 @@ class ContinuousEntropyModelBase(nn.Module):
     out = (symbols + coff[index.long()]).to(self.bottleneck_dtype)
     return out if off is None else out + off
 
+  # float16 / bfloat16 bottlenecks are quantised in the encoder and dequantised in the decoder where
+  # functional._coder16 accepts the operands; the universal models keep the unfused path
+  _coder16_models = True
+
+  def _coder16(self, dtype, device, off, index, shape):
+    return self._coder16_models and F._coder16(dtype, device, off, index, shape)
+
   def _encode(self, batch_shape, b, off, coff, index=None, fused=True):
     """One string per element of `batch_shape` for `b` (in bottleneck_dtype, coding units innermost).  A float32
-    bottleneck is quantised inside the encoder unless `fused=False`, which issues the reference's op sequence."""
+    bottleneck, and a 16-bit one with the operands _coder16 accepts, is quantised inside the encoder unless
+    `fused=False`, which issues the reference's op sequence."""
     if fused and b.dtype == torch.float32:
       return F.compress_f32(batch_shape, self._lookup_host(), b, off, coff, index=index)
+    if fused and self._coder16(b.dtype, b.device, off, index, b.shape):
+      return F.compress_16bit(batch_shape, self._lookup_host(), b, off, coff, index=index)
     handle = gen_ops.create_range_encoder(batch_shape, self._lookup_host())
     symbols = self._quantize(b, off, coff, index)
     if index is None:  # the reference's iid_shape + [-1]: every axis left of prior_shape, then the table rows
@@ -281,6 +291,11 @@ class ContinuousEntropyModelBase(nn.Module):
         out = F.decode_index_f32(handle, index, off, coff)
       self._finish_decode(handle)
       return out
+    dev = strings.bytes_dev.device
+    if fused and self._coder16(self.bottleneck_dtype, dev, off, index, None if index is None else index.shape):
+      out = F.decode_16bit(handle, strings.shape + shape, self.bottleneck_dtype, off, coff, index=index)
+      self._finish_decode(handle)
+      return out
     if index is None:  # the reference decodes shape[:-rank(prior_shape)] + [rows]
       lead = shape[:len(shape) - len(self.prior_shape)]
       handle, symbols = gen_ops.entropy_decode_channel(handle, lead + (gen_ops._prod(self.prior_shape),))
@@ -292,11 +307,14 @@ class ContinuousEntropyModelBase(nn.Module):
   # ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none)
   def _encode_ragged(self, shapes, b, off, coff, index=None, return_decoded=False):
     """Strings of shape (k,) for the k items of the given shapes that `b` (in bottleneck_dtype) holds back to back;
-    with `return_decoded`, also what _decode_ragged makes of them.  A float32 bottleneck is quantised inside the
-    encoder, which then also writes the decoded items."""
+    with `return_decoded`, also what _decode_ragged makes of them.  A float32 bottleneck, and a 16-bit one with the
+    operands _coder16 accepts, is quantised inside the encoder, which then also writes the decoded items."""
     lengths = [gen_ops._prod(s) for s in shapes]
     if b.dtype == torch.float32:
       out = F.compress_ragged(self._lookup_host(), lengths, b, off, coff, index=index, decoded=return_decoded)
+      return (out[0], gen_ops._split_items(out[1], shapes)) if return_decoded else out
+    if self._coder16(b.dtype, b.device, off, index, b.shape):
+      out = F.compress_ragged_16bit(self._lookup_host(), lengths, b, off, coff, index=index, decoded=return_decoded)
       return (out[0], gen_ops._split_items(out[1], shapes)) if return_decoded else out
     strings = F.compress_ragged(self._lookup_host(), lengths, self._quantize(b, off, coff, index), index=index)
     return (strings, self._decode_ragged(strings, shapes, off, coff, index)) if return_decoded else strings
@@ -305,13 +323,17 @@ class ContinuousEntropyModelBase(nn.Module):
     """Inverse of _encode_ragged: the items, views into one allocation."""
     handle = gen_ops.create_range_decoder(strings, self._lookup_host())
     lengths = [gen_ops._prod(s) for s in shapes]
-    fused = self.bottleneck_dtype == torch.float32
-    if fused:
+    dtype, dev = self.bottleneck_dtype, strings.bytes_dev.device
+    unfused = False
+    if dtype == torch.float32:
       out = F.decode_ragged(handle, lengths, index=index, quant_offset=off, cdf_offset=coff)
+    elif self._coder16(dtype, dev, off, index, None if index is None else index.shape):
+      out = F.decode_ragged_16bit(handle, lengths, dtype, off, coff, index=index)
     else:
       out = F.decode_ragged(handle, lengths, index=index)
+      unfused = True
     self._finish_decode(handle)
-    if not fused:
+    if unfused:
       out = self._dequantize(out, off, coff, index).reshape(-1)
     return gen_ops._split_items(out, shapes)
 
@@ -760,6 +782,8 @@ def _kernel_offset_dtype(bottleneck_dtype):
 class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
   """universal.py:65-330."""
 
+  _coder16_models = False  # (offsets follow a float64 rule, see _kernel_offset_dtype)
+
   def __init__(self, prior, coding_rank, compression=False, laplace_tail_mass=0.0, expected_grads=False,
                tail_mass=2**-8, range_coder_precision=12, bottleneck_dtype=None, num_noise_levels=15, stateless=False,
                decode_sanity_check=True):
@@ -901,6 +925,8 @@ class UniversalBatchedEntropyModel(ContinuousEntropyModelBase):
 
 class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
   """universal.py:292-603."""
+
+  _coder16_models = False  # (offsets follow a float64 rule, see _kernel_offset_dtype)
 
   def __init__(self, prior_fn, index_ranges, parameter_fns, coding_rank, compression=False, laplace_tail_mass=0.0,
                expected_grads=False, tail_mass=2**-8, range_coder_precision=12, bottleneck_dtype=None,

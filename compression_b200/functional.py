@@ -628,6 +628,127 @@ def decode_index_f32(handle, index, loc, cdf_offset):
   return out
 
 
+# ------------------------------------------------------------------------------------------------
+# 16-bit bottlenecks: quantised in the encoder, dequantised in the decoder (tfcb_*_16bit), with the arithmetic of
+# the entropy models' unfused path (ContinuousEntropyModelBase._quantize / _dequantize)
+# ------------------------------------------------------------------------------------------------
+_LOC_DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+
+
+def _coder16(dtype, device, off=None, index=None, shape=None):
+  """Whether range coding of a `dtype` bottleneck on `device` runs on the 16-bit entries below, which give the bytes
+  and bits of the unfused path: `dtype` float16 or bfloat16 on a CUDA device; channel mode (`index` None): `off` None
+  or float32 with one value per table row (the models' quantisation offsets); index mode: `index` of shape `shape`,
+  and `off` None or of that shape in `dtype` or float32.  Every operand is on `device`.  Reads dtypes, shapes and
+  devices only.  Everything else (e.g. a float64 loc, or a loc broadcast from another shape) keeps the unfused
+  path."""
+  device = torch.device(device)
+  if dtype not in _IO16 or device.type != "cuda":
+    return False
+  if any(t is not None and t.device != device for t in (off, index)):
+    return False
+  if index is None:
+    return off is None or (off.dtype == torch.float32 and len(off.shape) == 1)
+  shape = tuple(shape)
+  return tuple(index.shape) == shape and (off is None or (off.dtype in (dtype, torch.float32) and
+                                                          tuple(off.shape) == shape))
+
+
+def _loc16(loc, dev):
+  """A 16-bit call's loc operand as the library takes it: (contiguous flat tensor or None, loc_dtype code)."""
+  if loc is None:
+    return None, 0
+  loc = loc.to(dev).contiguous().reshape(-1)
+  return loc, _LOC_DTYPES.get(loc.dtype, -1)
+
+
+def _out16_dtype(dtype, loc, index):
+  """The decoded values' type: the bottleneck's, or float32 in index mode with a float32 loc (torch's promotion of
+  the unfused path's `out + loc`)."""
+  return torch.float32 if index is not None and loc is not None and loc.dtype == torch.float32 else dtype
+
+
+def _check16_lengths(n, loc, index, cdf_offset, value=None):
+  """A 16-bit call's operands against its `n` symbols, before the library is called: value and index have n
+  elements, loc n (index mode) or one per cdf_offset row (channel mode)."""
+  if value is not None and value.numel() != n:
+    raise _lib.InvalidArgumentError(f"{n} symbols, but `value` has {value.numel()}")
+  if index is not None and index.numel() != n:
+    raise _lib.InvalidArgumentError(f"{n} symbols, but `index` has {index.numel()}")
+  if loc is not None:
+    want = n if index is not None else (loc.numel() if cdf_offset is None else cdf_offset.numel())
+    if loc.numel() != want:
+      raise _lib.InvalidArgumentError(f"`loc` has {loc.numel()} elements, expected {want}")
+
+
+def compress_16bit(batch_shape, lookup, value, loc, cdf_offset, index=None):
+  """compress_f32 for a float16 / bfloat16 `value`, quantised in the encoder as the entropy models' unfused path
+  does: channel mode (index None) rint(float32(value) - loc[row]) with `loc` the float32 quantisation offsets (or
+  None); index mode rint(value - loc) in torch's promoted type (`loc` None, in value's dtype, or float32).  The
+  strings are those of the unfused path, byte for byte."""
+  shape = tuple(int(d) for d in batch_shape)
+  lookup = _host_lookup(lookup)
+  n_streams = gen_ops._prod(shape)
+  if n_streams == 0:
+    raise _lib.InvalidArgumentError(f"`handle` is empty: handle.shape={shape}")
+  dev = value.device
+  value = value.contiguous()
+  index, coff = _i32(index, dev), _i32(cdf_offset, dev)
+  loc, loc_dtype = _loc16(loc, dev)
+  _check16_lengths(value.numel(), loc, index, coff)
+  return _compress(_lib.lib().tfcb_compress_16bit, lookup, shape, dev, _p(index), _p(value), _IO16.get(value.dtype, 0),
+                   _p(loc), loc_dtype, _p(coff), value.numel() // n_streams)
+
+
+def compress_ragged_16bit(lookup, lengths, value, loc=None, cdf_offset=None, index=None, decoded=False):
+  """compress_ragged for a float16 / bfloat16 `value` (quantised as compress_16bit).  `decoded=True` returns
+  `(strings, decoded_flat)`: per symbol, exactly what decode_ragged_16bit returns for these strings, written by the
+  encoder (in value's dtype, or float32 in index mode with a float32 loc)."""
+  offs = _symbol_offsets(lengths)
+  lookup = _host_lookup(lookup)
+  k, n = offs.size - 1, int(offs[-1])
+  dev = value.device
+  value = value.contiguous().reshape(-1)
+  index, coff = _i32(index, dev), _i32(cdf_offset, dev)
+  loc, loc_dtype = _loc16(loc, dev)
+  _check16_lengths(n, loc, index, coff, value)
+  buf = torch.empty(max(n, 1), dtype=_out16_dtype(value.dtype, loc, index), device=dev) if decoded else None
+  strings = _compress(_lib.lib().tfcb_compress_ragged_16bit, lookup, (k,), dev, offs.ctypes.data_as(C.c_void_p),
+                      _p(index), _p(value), _IO16.get(value.dtype, 0), _p(loc), loc_dtype, _p(coff), _p(buf))
+  return (strings, buf[:n]) if decoded else strings
+
+
+def decode_16bit(handle, out_shape, dtype, loc, cdf_offset, index=None):
+  """Decodes and dequantises float16 / bfloat16 values as the entropy models' unfused path: h = dtype(float(sym +
+  cdf_offset[row])), then h + loc computed in float32 and rounded to dtype -- or returned as float32 in index mode
+  with a float32 loc.  Shape `out_shape` in channel mode, index's shape in index mode."""
+  dev = handle._encoded.bytes_dev.device
+  index, coff = _i32(index, dev), _i32(cdf_offset, dev)
+  loc, loc_dtype = _loc16(loc, dev)
+  shape = tuple(out_shape) if index is None else tuple(index.shape)
+  out = torch.empty(shape, dtype=_out16_dtype(dtype, loc, index), device=dev)
+  _check16_lengths(out.numel(), loc, index, coff)
+  check(_lib.lib().tfcb_decode_16bit(handle._h, _p(index), _p(out), _IO16.get(dtype, 0), _p(loc), loc_dtype, _p(coff),
+                                     out.numel() // handle.n_streams, _stream()))
+  return out
+
+
+def decode_ragged_16bit(handle, lengths, dtype, loc=None, cdf_offset=None, index=None):
+  """decode_ragged of float16 / bfloat16 values, dequantised as decode_16bit: one flat tensor, stream after
+  stream."""
+  offs = _symbol_offsets(lengths)
+  if offs.size - 1 != handle.n_streams:
+    raise _lib.InvalidArgumentError(f"{offs.size - 1} lengths for {handle.n_streams} strings")
+  dev = handle._encoded.bytes_dev.device
+  index, coff = _i32(index, dev), _i32(cdf_offset, dev)
+  loc, loc_dtype = _loc16(loc, dev)
+  _check16_lengths(int(offs[-1]), loc, index, coff)
+  out = torch.empty(int(offs[-1]), dtype=_out16_dtype(dtype, loc, index), device=dev)
+  check(_lib.lib().tfcb_decode_ragged_16bit(handle._h, offs.ctypes.data_as(C.c_void_p), _p(index), _p(out),
+                                            _IO16.get(dtype, 0), _p(loc), loc_dtype, _p(coff), _stream()))
+  return out
+
+
 def build_lookup(pmf, pmf_length, precision):
   """The per-row PMF -> CDF loop of _build_tables in one launch (continuous_base.py:282-294):
   pmf float32 [rows, max_len] (CUDA), pmf_length int [rows] -> 1-D int32 lookup [-p, cdf...]*rows."""

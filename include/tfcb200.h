@@ -135,6 +135,29 @@ int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len,
                                  const void* value_dev, int32_t value_is_f32, const float* quant_offset_dev,
                                  const int32_t* cdf_offset_dev, int64_t* offsets_dev, void* stream,
                                  tfcb_encoder** out, int64_t* total_bytes_host, float* decoded_dev);
+/* float16 / bfloat16 values (`dtype` 1 / 2), quantised in the encoder with the arithmetic of the entropy models'
+ * unfused 16-bit path, so the strings are those of tfcb_compress on the int32 symbols that path computes:
+ *   channel mode (index_dev NULL): int(rint(float(value) - loc[row])) - cdf_offset[row], `loc_dev` NULL or float32
+ *     [rows] (the quantisation offsets; `loc_dtype` 0);
+ *   index mode: `loc_dev` NULL, or shaped like the value in float32 (`loc_dtype` 0: the difference is taken in
+ *     float32) or in the value's type (`loc_dtype` == dtype: the difference is rounded to that type first).
+ * float -> int32 saturates and NaN gives 0, as in the *_f32 calls.  Otherwise exactly tfcb_compress (checks, offsets,
+ * one synchronisation, the encoder tfcb_compress_write packs).  Checked before any device work
+ * (TFCB_INVALID_ARGUMENT): `dtype` 1 or 2, `loc_dtype` 0 or (index mode) `dtype`, `cdf_offset_dev` non-null, and
+ * `value_dev` non-null whenever there are symbols. */
+int tfcb_compress_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                        const int32_t* index_dev, const void* value_dev, int dtype, const void* loc_dev, int loc_dtype,
+                        const int32_t* cdf_offset_dev, int64_t n_per_stream, int64_t* offsets_dev, void* stream,
+                        tfcb_encoder** out, int64_t* total_bytes_host);
+/* tfcb_compress_16bit over a ragged batch, laid out and checked like tfcb_compress_ragged.  `decoded_dev` non-null:
+ * the encoder also writes, per symbol, exactly what tfcb_decode_ragged_16bit with the same dtype, loc and cdf_offset
+ * returns for these strings (as tfcb_compress_ragged_decoded does for float32): in the value's type, or float32 in
+ * index mode with a float32 loc. */
+int tfcb_compress_ragged_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
+                               const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
+                               int dtype, const void* loc_dev, int loc_dtype, const int32_t* cdf_offset_dev,
+                               void* decoded_dev, int64_t* offsets_dev, void* stream, tfcb_encoder** out,
+                               int64_t* total_bytes_host);
 
 /* ------------------------------------------------------------------------------------------------
  * Range DECODER.  Replaces CreateRangeDecoder / EntropyDecodeChannel / EntropyDecodeIndex /
@@ -172,6 +195,20 @@ int tfcb_decode_index_f32(tfcb_decoder* h, const int32_t* index_dev, float* out_
  * reports. */
 int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev, void* out_dev,
                        int32_t out_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev, void* stream);
+/* Fused decode + dequantise of float16 / bfloat16 values (`dtype` 1 / 2; `index_dev` NULL: channel mode), the
+ * inverse of tfcb_compress_16bit with the same loc operand and the arithmetic of the entropy models' unfused path:
+ * h = to16(float(sym + cdf_offset[row])) (int32 -> float -> 16 bits, two roundings), then
+ *   channel mode: out = to16(float(h) + float(to16(loc[row]))) (loc float32 [rows] or NULL: out = h);
+ *   index mode, loc in the value's type (or NULL): out = to16(float(h) + float(loc));
+ *   index mode, float32 loc: out = float(h) + loc, written as FLOAT32.
+ * `out_dev` holds n_streams * n_per_stream outputs of that type.  Checked before any device work like
+ * tfcb_compress_16bit (`out_dev` in place of `value_dev`). */
+int tfcb_decode_16bit(tfcb_decoder* h, const int32_t* index_dev, void* out_dev, int dtype, const void* loc_dev,
+                      int loc_dtype, const int32_t* cdf_offset_dev, int64_t n_per_stream, void* stream);
+/* tfcb_decode_16bit over a ragged batch, with tfcb_decode_ragged's offsets and layout. */
+int tfcb_decode_ragged_16bit(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev,
+                             void* out_dev, int dtype, const void* loc_dev, int loc_dtype,
+                             const int32_t* cdf_offset_dev, void* stream);
 /* EntropyDecodeFinalize: ok_host[s] = RangeDecoder::Finalize() of stream s (range_coder.h:144-169).
  * Synchronises; also reports a pending out-of-range index as TFCB_INVALID_ARGUMENT. */
 int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream);
