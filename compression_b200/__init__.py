@@ -11,7 +11,7 @@ from compression_b200._lib import InvalidArgumentError
 def __getattr__(name):  # lazy: importing the package must not require torch / the built library
   import importlib
   modules = ("gen_ops", "functional", "math_ops", "distributions", "entropy_models", "gdn", "packed_tensors",
-             "signal_conv", "models", "sharding", "run_length_models", "soft_round_layers", "layers", "ops", "parameters", "y4m_dataset")
+             "signal_conv", "models", "sharding", "run_length_models", "soft_round_layers", "layers", "ops", "parameters", "y4m_dataset", "image")
   if name in modules:
     return importlib.import_module("compression_b200." + name)
   exported = {

@@ -108,6 +108,11 @@ SIGNATURES = {
     "tfcb_noisy_loc_scale_log_prob": (_int, [_int, _vp, _vp, _int, _vp, _int, _vp, _i64, _vp]),
     "tfcb_noisy_loc_scale_log_prob_backward": (_int, [_int, _vp, _vp, _int, _vp, _int, _vp, _vp, _vp, _vp, _i64,
                                                       _vp]),
+    "tfcb_ssim_workspace_bytes": (_i64, [_int, _i64, _i64, _i64, _i64, _int, _int]),
+    "tfcb_ssim_stats": (_int, [_vp, _vp, _int, _i64, _i64, _i64, _i64, _f32, _int, _int, _f32, _f32, _f32, _vp, _vp,
+                               _vp]),
+    "tfcb_ssim_stats_backward": (_int, [_vp, _vp, _int, _i64, _i64, _i64, _i64, _f32, _int, _int, _f32, _f32, _f32,
+                                        _vp, _vp, _vp, _vp, _vp]),
     "tfcb_stateless_uniform_int": (_int, [_vp, _i64, _u32, _u32, _i64, _vp]),
     "tfcb_universal_coding_tensors": (_int, [_i64, _vp, _u32, _u32, _i64, _i64, _vp, _i32, _vp, _i32, _vp, _vp, _i32,
                                              _vp]),

@@ -131,6 +131,25 @@ class _Model(nn.Module):
     mse = torch.mean((x - self._last_x_hat)**2)
     return bpp + self.lmbda * mse, bpp, mse
 
+  @torch.no_grad()
+  def evaluate(self, x):
+    """The verbose block of the reference's `compress` (bls2017.py:287-305) for one uint8 image [H, W, 3]: codes it
+    to `.tfci`, decodes that, and returns the metrics of the float32 pair as Python floats: `mse`, `psnr` and `msssim`
+    (tf.image's, max_val 255), `msssim_db` = -10 log10(1 - msssim), and `bpp`, the container's bits per pixel."""
+    from compression_b200 import image
+    x = _as_image(x)
+    tfci = self.compress_to_tfci(x)
+    x_hat = self.decompress_from_tfci(tfci)
+    x = x.to(device=x_hat.device, dtype=torch.float32)
+    x_hat = x_hat.to(torch.float32)
+    mse = torch.mean((x - x_hat)**2)
+    psnr = image.psnr(x, x_hat, 255)
+    msssim = image.ssim_multiscale(x, x_hat, 255)
+    msssim_db = -10. * torch.log(1 - msssim) / math.log(10.)
+    bpp = len(tfci) * 8 / (x.shape[0] * x.shape[1])
+    return {"mse": float(mse), "psnr": float(psnr), "msssim": float(msssim), "msssim_db": float(msssim_db),
+            "bpp": float(bpp)}
+
   def compress_to_tfci(self, x):
     """The .tfci container (bls2017.py:262-282): `compress(x)` packed into one byte string."""
     packed = PackedTensors()

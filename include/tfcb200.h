@@ -504,6 +504,43 @@ int tfcb_gdn_backward_cf(const void* x_dev, const float* gamma_dev, const float*
                          void* workspace_dev, int64_t n_items, int64_t spatial, int C, int dtype, int flags,
                          float alpha, float epsilon, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Image quality: the statistics behind tf.image.ssim and tf.image.ssim_multiscale
+ * (tensorflow/python/ops/image_ops_impl.py), which the model scripts print after compressing an image
+ * (models/bls2017.py:294-295, bmshj2018.py:370-371, ms2020.py:540-541).  The host combines them into the metrics:
+ *   ssim            = mean over channels of stats[..., 0, 1]
+ *   ssim_multiscale = mean over channels of prod_k v_k ** power_factors[k], v_k = relu(stats[..., k, 0]) for
+ *                     k < n_scales - 1 and relu(stats[..., n_scales - 1, 1]) for the last scale.
+ * img1_dev, img2_dev: [n_images, H, W, C] channels-last, `dtype` 0 float32, 1 float16, 2 bfloat16, 3 uint8 (widened to
+ * float32(u) * float32(1/255) like convert_image_dtype; `max_val` is given after that conversion, 1.0 for 255).
+ * Window: filter_size x filter_size, the softmax of -(i^2 + j^2) / (2 filter_sigma^2) around (filter_size - 1) / 2,
+ * VALID, per channel.  With c1 = (k1 max_val)^2, c2 = (k2 max_val)^2 and mx, my, S(.) the windowed means and moments:
+ *   l = (2 mx my + c1) / (mx^2 + my^2 + c1),  cs = (2 (Sxy - mx my) + c2) / (S(x^2 + y^2) - mx^2 - my^2 + c2).
+ * Scale s + 1 is scale s padded at its end by one repeated row / column where odd, then 2x2 average pooled.
+ * stats_dev float32 [n_images, C, n_scales, 2] receives (mean(cs), mean(l * cs)) over each scale's valid positions,
+ * summed in double in a fixed order and rounded once: bitwise reproducible, and an image's values do not depend on the
+ * batch it is in.  The launch count depends on n_scales only.
+ *
+ * The backward takes g_stats_dev float32 [n_images, C, n_scales, 2] (the loss gradient of stats) and writes dimg1 /
+ * dimg2 in the image dtype (computed in float32, rounded once); either may be NULL, and with both NULL nothing runs.
+ * uint8 images have no gradient (TFCB_INVALID_ARGUMENT).
+ *
+ * `workspace_dev` holds tfcb_ssim_workspace_bytes(dtype, n_images, H, W, C, n_scales, filter_size) bytes (the same
+ * size serves both directions; -1 for arguments the entries reject).  Checked before any device work
+ * (TFCB_INVALID_ARGUMENT): a known dtype; n_images >= 0, H, W, C >= 1, n_images * H * W * C within int64 and
+ * n_images * C < 2^31; 1 <= filter_size <= 32; 1 <= n_scales <= 16; every scale at least filter_size in H and W (as
+ * TF asserts: with the defaults 161 passes and 160 fails); filter_sigma > 0 and finite; finite max_val, k1, k2; non-null
+ * pointers.  n_images = 0 launches nothing. */
+int64_t tfcb_ssim_workspace_bytes(int dtype, int64_t n_images, int64_t H, int64_t W, int64_t C, int n_scales,
+                                  int filter_size);
+int tfcb_ssim_stats(const void* img1_dev, const void* img2_dev, int dtype, int64_t n_images, int64_t H, int64_t W,
+                    int64_t C, float max_val, int n_scales, int filter_size, float filter_sigma, float k1, float k2,
+                    float* stats_dev, void* workspace_dev, void* stream);
+int tfcb_ssim_stats_backward(const void* img1_dev, const void* img2_dev, int dtype, int64_t n_images, int64_t H,
+                             int64_t W, int64_t C, float max_val, int n_scales, int filter_size, float filter_sigma,
+                             float k1, float k2, const float* g_stats_dev, void* dimg1_dev, void* dimg2_dev,
+                             void* workspace_dev, void* stream);
+
 int64_t tfcb_launch_count(void);
 
 #ifdef __cplusplus
