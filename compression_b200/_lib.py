@@ -113,6 +113,9 @@ SIGNATURES = {
                                _vp]),
     "tfcb_ssim_stats_backward": (_int, [_vp, _vp, _int, _i64, _i64, _i64, _i64, _f32, _int, _int, _f32, _f32, _f32,
                                         _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_image_metrics_ragged_workspace_bytes": (_i64, [_int, _i64, _vp, _vp, _i64, _int, _int, _int]),
+    "tfcb_image_metrics_ragged": (_int, [_vp, _vp, _int, _i64, _vp, _vp, _vp, _i64, _int, _f32, _int, _int, _f32,
+                                         _f32, _f32, _vp, _vp, _vp, _vp]),
     "tfcb_stateless_uniform_int": (_int, [_vp, _i64, _u32, _u32, _i64, _vp]),
     "tfcb_universal_coding_tensors": (_int, [_i64, _vp, _u32, _u32, _i64, _i64, _vp, _i32, _vp, _i32, _vp, _vp, _i32,
                                              _vp]),

@@ -28,7 +28,7 @@ from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
 __all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
-           "HyperSynthesisTransform", "bench_model_paths"]
+           "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
 class _Scale(nn.Module):
@@ -113,6 +113,15 @@ def _as_image(x):
   return x
 
 
+def mean_metrics(per_image):
+  """The mean of each key over a list of `evaluate` / `evaluate_images` dicts: a rate-distortion point as the
+  reference's results report it, per-image values averaged at one lambda."""
+  per_image = list(per_image)
+  if not per_image:
+    raise ValueError("no metrics to average")
+  return {k: math.fsum(d[k] for d in per_image) / len(per_image) for k in per_image[0]}
+
+
 class _Model(nn.Module):
 
   def _device(self):
@@ -149,6 +158,35 @@ class _Model(nn.Module):
     bpp = len(tfci) * 8 / (x.shape[0] * x.shape[1])
     return {"mse": float(mse), "psnr": float(psnr), "msssim": float(msssim), "msssim_db": float(msssim_db),
             "bpp": float(bpp)}
+
+  @torch.no_grad()
+  def evaluate_images(self, images):
+    """`evaluate` for a list of uint8 images [H_i, W_i, 3] of their own sizes, one dict of Python floats per image.
+
+    Runs `compress_images` once, packs each image's items into its own `.tfci` (for `bpp`), runs `decompress_images`
+    once, then one `image.metrics_ragged` call per colour space on the float32 pairs (max_val 255).  The keys of
+    `evaluate` have its meaning, with the same `bpp` and `msssim` bit for bit (`mse` and `psnr` are summed in another
+    order).  Added: `psnr_y`, `msssim_y`, `msssim_db_y` on Y', and `psnr_ycbcr`, `msssim_ycbcr`, `msssim_db_ycbcr`, the
+    6:1:1 average over Y'CbCr that the reference's results recommend.  `mean_metrics` averages the list."""
+    from compression_b200 import image
+    images = [_as_image(x) for x in images]
+    if not images:
+      return []
+    items = self.compress_images(images)
+    n_bytes = []
+    for item in items:
+      packed = PackedTensors()
+      packed.pack(item)
+      n_bytes.append(len(packed.string))
+    x_hats = [x.to(torch.float32) for x in self.decompress_images(items)]
+    xs = [x.to(device=x_hat.device, dtype=torch.float32) for x, x_hat in zip(images, x_hats)]
+    out = [{"bpp": n * 8 / (x.shape[0] * x.shape[1])} for n, x in zip(n_bytes, images)]
+    for color, suffix in (("rgb", ""), ("y", "_y"), ("ycbcr", "_ycbcr")):
+      metrics = image.metrics_ragged(xs, x_hats, 255, color)
+      for key in ("mse", "psnr", "msssim", "msssim_db") if color == "rgb" else ("psnr", "msssim", "msssim_db"):
+        for d, v in zip(out, metrics[key].tolist()):
+          d[key + suffix] = v
+    return out
 
   def compress_to_tfci(self, x):
     """The .tfci container (bls2017.py:262-282): `compress(x)` packed into one byte string."""

@@ -541,6 +541,41 @@ int tfcb_ssim_stats_backward(const void* img1_dev, const void* img2_dev, int dty
                              float k1, float k2, const float* g_stats_dev, void* dimg1_dev, void* dimg2_dev,
                              void* workspace_dev, void* stream);
 
+/* Rate-distortion evaluation of a list of image pairs of their own sizes: the forward statistics above and the mean
+ * squared error of every image and plane, with one launch per kernel per scale whatever the number of images (at most
+ * 2 n_scales launches).  Pair i is img1_dev / img2_dev [item_offsets_host[i] .. item_offsets_host[i + 1]), channels-last
+ * [heights_host[i], widths_host[i], C] in `dtype` (as tfcb_ssim_stats; uint8 is widened the same way).  The offsets and
+ * sizes are host arrays [n_items + 1] and [n_items].  `mode` selects the planes:
+ *   TFCB_COLOR_RGB    the C channels;
+ *   TFCB_COLOR_Y      one Y' plane from C = 3;
+ *   TFCB_COLOR_YCBCR  three Y'CbCr planes from C = 3.
+ * Y'CbCr is BT.601 full range (JFIF) in the images' units after the dtype conversion, m = max_val, evaluated in float32
+ * left to right with every product and sum rounded:
+ *   Y' = 0.299 R + 0.587 G + 0.114 B
+ *   Cb = float32(128/255) m + (-0.168736 R - 0.331264 G + 0.5 B)
+ *   Cr = float32(128/255) m + (0.5 R - 0.418688 G - 0.081312 B)
+ * It is applied as scale 0 is read; nothing converted is written to memory.
+ * stats_dev float32 [n_items, planes, n_scales, 2] receives what tfcb_ssim_stats gives for the planes (for RGB, bit
+ * for bit what it gives for each image alone).  mse_dev float32 [n_items, planes] receives mean((x - y)^2) over each
+ * plane, summed in double in a fixed order and rounded once.  Results are bitwise reproducible, and an image's values
+ * do not depend on the list it is in.  There is no backward.
+ * `workspace_dev` holds tfcb_image_metrics_ragged_workspace_bytes(...) bytes (-1 for arguments the entry rejects).
+ * Checked before any device work (TFCB_INVALID_ARGUMENT): a known dtype and mode; C >= 1, and C = 3 for Y' and Y'CbCr;
+ * n_items >= 0; every size at least 1 and, at every scale, at least filter_size (the message names the image);
+ * item_offsets_host[0] = 0 and each item spanning H W C elements; the other arguments as tfcb_ssim_stats; non-null
+ * pointers.  n_items = 0 launches nothing.  The offsets and sizes are staged into the workspace (pageable copies). */
+#define TFCB_COLOR_RGB 0
+#define TFCB_COLOR_Y 1
+#define TFCB_COLOR_YCBCR 2
+int64_t tfcb_image_metrics_ragged_workspace_bytes(int dtype, int64_t n_items, const int64_t* heights_host,
+                                                  const int64_t* widths_host, int64_t C, int mode, int n_scales,
+                                                  int filter_size);
+int tfcb_image_metrics_ragged(const void* img1_dev, const void* img2_dev, int dtype, int64_t n_items,
+                              const int64_t* item_offsets_host, const int64_t* heights_host,
+                              const int64_t* widths_host, int64_t C, int mode, float max_val, int n_scales,
+                              int filter_size, float filter_sigma, float k1, float k2, float* stats_dev,
+                              float* mse_dev, void* workspace_dev, void* stream);
+
 int64_t tfcb_launch_count(void);
 
 #ifdef __cplusplus
