@@ -68,6 +68,11 @@ SIGNATURES = {
     "tfcb_decode_16bit": (_int, [_vp, _vp, _vp, _int, _vp, _int, _vp, _i64, _vp]),
     "tfcb_decode_ragged_16bit": (_int, [_vp, _vp, _vp, _vp, _int, _vp, _int, _vp, _vp]),
     "tfcb_decode_finalize": (_int, [_vp, _vp, _vp]),
+    "tfcb_ar_packed_floats": (_i64, [_int]),
+    "tfcb_ar_pack_weights": (_int, [_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "tfcb_ar_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp]),
+    "tfcb_ar_encode": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_ar_decode": (_int, [_vp, _vp, _i64, _int, _vp, _i64, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp]),
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_range_decode": (_int, [_vp, _i64, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),

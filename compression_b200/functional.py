@@ -795,3 +795,149 @@ def unbounded_index_range_decode_ragged(strings, index, lengths, cdf, cdf_size, 
   if n_index != offs[-1]:
     raise _lib.InvalidArgumentError(f"ragged batch of {int(offs[-1])} elements, but `index` has {n_index}")
   return gen_ops._ubi_decode(strings, index, offs, cdf, cdf_size, offset, precision, overflow_width, debug_level)
+
+
+# ------------------------------------------------------------------------------------------------
+# Joint autoregressive + hierarchical prior (Minnen 2018): the packed parameter network and the parameter, encoder and
+# decoder steps over latent positions in raster order (tfcb_ar_*).  Latents are float32 CUDA [B, H, W, M], the hyper
+# feature psi [B, H, W, 2M].
+# ------------------------------------------------------------------------------------------------
+def ar_packed_floats(M):
+  """Floats of the packed parameter buffer for latent depth M (a multiple of 6 in [6, 384])."""
+  n = int(_lib.lib().tfcb_ar_packed_floats(int(M)))
+  if n < 0:
+    raise _lib.InvalidArgumentError(f"latent depth M={M} must be a positive multiple of 6 and at most 384")
+  return n
+
+
+def ar_pack_weights(ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
+  """The device layout the parameter kernel reads: the context kernel [5, 5, M, 2M] (masked or not: only its 12
+  causal taps are read), then each 1x1 layer as [inputs, outputs] and its bias.  Returns float32 [packed floats] on
+  the context kernel's device; the values are copied unchanged."""
+  ctx_kernel = ctx_kernel.detach()
+  if ctx_kernel.dim() != 4 or ctx_kernel.shape[:2] != (5, 5) or ctx_kernel.shape[3] != 2 * ctx_kernel.shape[2]:
+    raise _lib.InvalidArgumentError(f"context kernel must be [5, 5, M, 2M]: {tuple(ctx_kernel.shape)}")
+  M = int(ctx_kernel.shape[2])
+  n = ar_packed_floats(M)
+  n3, n4 = 10 * M // 3, 8 * M // 3
+  dev = ctx_kernel.device
+  if dev.type != "cuda":
+    raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
+  want = ((ctx_bias, (2 * M,)), (w1, (4 * M, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, 2 * M)),
+          (b3, (2 * M,)))
+  ops = [_f32(ctx_kernel, dev)]
+  for t, shape in want:
+    t = t.detach()
+    if tuple(t.shape) != shape:
+      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where M={M} needs {shape}")
+    ops.append(_f32(t, dev))
+  packed = torch.empty(n, dtype=torch.float32, device=dev)
+  check(_lib.lib().tfcb_ar_pack_weights(M, *[_p(t) for t in ops], _p(packed), n, _stream()))
+  return packed
+
+
+def _ar_tensor(t, name, shape, dev, dtype=torch.float32):
+  if not isinstance(t, torch.Tensor) or t.device != dev or t.dtype != dtype:
+    raise _lib.InvalidArgumentError(f"`{name}` must be a {dtype} tensor on {dev}")
+  if tuple(t.shape) != tuple(shape):
+    raise _lib.InvalidArgumentError(f"`{name}` has shape {tuple(t.shape)}, expected {tuple(shape)}")
+  return t.contiguous()
+
+
+def _ar_dims(packed, psi):
+  """(B, H, W, M, packed floats) from psi [B, H, W, 2M], checked against the packed buffer."""
+  if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
+    raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
+  B, H, W, M = int(psi.shape[0]), int(psi.shape[1]), int(psi.shape[2]), int(psi.shape[3]) // 2
+  if B == 0 or H == 0 or W == 0:
+    raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from ar_pack_weights")
+  n = ar_packed_floats(M)
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, M={M} needs {n}")
+  if packed.device.type != "cuda" or psi.device != packed.device:
+    raise _lib.InvalidArgumentError(f"`packed` ({packed.device}) and `psi` ({psi.device}) must share a CUDA device")
+  return B, H, W, M, n
+
+
+def ar_params(packed, y_hat, psi, p, num_scales):
+  """The parameter step at position p (0 <= p < H * W) of every image: (loc, scale_index, index) [B, M], float32,
+  float32 and int32, from y_hat [B, H, W, M] at earlier positions.  Row b depends only on image b."""
+  B, H, W, M, n = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  if not 0 <= int(p) < H * W:
+    raise _lib.InvalidArgumentError(f"position {p} outside [0, {H * W})")
+  loc = torch.empty((B, M), dtype=torch.float32, device=dev)
+  scale = torch.empty_like(loc)
+  index = torch.empty((B, M), dtype=torch.int32, device=dev)
+  check(_lib.lib().tfcb_ar_params(_p(packed), n, M, _p(y_hat), _p(psi), B, H, W, int(p), int(num_scales), _p(loc),
+                                  _p(scale), _p(index), _stream()))
+  return loc, scale, index
+
+
+def _ar_range(p_begin, p_end, H, W):
+  p_end = H * W if p_end is None else int(p_end)
+  if not 0 <= int(p_begin) <= p_end <= H * W:
+    raise _lib.InvalidArgumentError(f"positions [{p_begin}, {p_end}) outside [0, {H * W})")
+  return int(p_begin), p_end
+
+
+def ar_encode(packed, y, psi, num_scales, y_hat=None, p_begin=0, p_end=None, scale_index=False):
+  """Encoder steps p_begin <= p < p_end (default: all) in one launch: returns (y_hat, loc, index) [B, H, W, M], and
+  scale_index last with `scale_index=True`.  y_hat = float(int32(rint(y - loc))) + loc; a given `y_hat` holds the
+  earlier positions and is written in place.  The strings are one index-mode encode of y with `index` and `loc`."""
+  B, H, W, M, n = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  p_begin, p_end = _ar_range(p_begin, p_end, H, W)
+  if y_hat is None:
+    y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  elif not (isinstance(y_hat, torch.Tensor) and y_hat.is_contiguous()):
+    raise _lib.InvalidArgumentError("`y_hat` must be a contiguous tensor (it is written in place)")
+  y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  loc = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  index = torch.zeros((B, H, W, M), dtype=torch.int32, device=dev)
+  scale = torch.zeros_like(loc) if scale_index else None
+  check(_lib.lib().tfcb_ar_encode(_p(packed), n, M, _p(y), _p(psi), B, H, W, p_begin, p_end, int(num_scales),
+                                  _p(y_hat), _p(loc), _p(index), _p(scale), _stream()))
+  return (y_hat, loc, index) + ((scale,) if scale_index else ())
+
+
+def ar_decode(handle, packed, psi, num_scales, cdf_offset, y_hat=None, p_begin=0, p_end=None):
+  """Decoder steps p_begin <= p < p_end (default: all) in one launch, continuing `handle` (a DecoderHandle of B
+  index-mode strings): returns y_hat [B, H, W, M], written in place into a given `y_hat` that holds the earlier
+  positions.  Stream errors surface at entropy_decode_finalize, as for the other decode calls."""
+  B, H, W, M, n = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  if handle.n_streams != B:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a batch of {B}")
+  p_begin, p_end = _ar_range(p_begin, p_end, H, W)
+  if y_hat is None:
+    y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  elif not (isinstance(y_hat, torch.Tensor) and y_hat.is_contiguous()):
+    raise _lib.InvalidArgumentError("`y_hat` must be a contiguous tensor (it is written in place)")
+  y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  coff = _i32(cdf_offset, dev)
+  check(_lib.lib().tfcb_ar_decode(handle._h, _p(packed), n, M, _p(psi), B, H, W, p_begin, p_end, int(num_scales),
+                                  _p(coff), _p(y_hat), _stream()))
+  return y_hat
+
+
+def ar_decode_naive(handle, packed, psi, num_scales, cdf_offset):
+  """The decoder as a host loop, for comparison: per position one tfcb_ar_params launch and one
+  tfcb_decode_index_f32 of M symbols per stream, written into y_hat by torch.  Gives ar_decode's y_hat bit for bit;
+  2 H W library launches and H W torch copies."""
+  B, H, W, M, _ = _ar_dims(packed, psi)
+  dev = packed.device
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  flat = y_hat.view(B, H * W, M)
+  coff = _i32(cdf_offset, dev)
+  for p in range(H * W):
+    loc, _, index = ar_params(packed, y_hat, psi, p, num_scales)
+    flat[:, p] = decode_index_f32(handle, index, loc, coff)
+  return y_hat

@@ -22,12 +22,13 @@ from torch import nn
 
 from compression_b200 import distributions as D
 from compression_b200 import entropy_models as E
+from compression_b200 import functional as F
 from compression_b200 import gen_ops
 from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -586,6 +587,217 @@ class MS2020Model(_Model):
 
   def decompress_from_tfci(self, data):
     dtypes = [torch.int32] * 3 + [bytes] * (self.num_slices + 1)
+    return self.decompress(*PackedTensors(data).unpack(dtypes))
+
+
+def _leaky(x):
+  """The LeakyReLU of the joint-prior model's hyper transforms and entropy-parameter layers (slope 0.01, as in the
+  parameter kernel: x > 0 ? x : 0.01 x)."""
+  return torch.nn.functional.leaky_relu(x, 0.01)
+
+
+def causal_mask(kernel_size=5):
+  """Type-A mask [k, k]: 1 at the taps strictly before the centre in raster order (12 for k = 5), 0 elsewhere."""
+  m = torch.zeros(kernel_size * kernel_size)
+  m[:kernel_size * kernel_size // 2] = 1
+  return m.reshape(kernel_size, kernel_size)
+
+
+class MaskedConv2D(nn.Module):
+  """The context model of Minnen et al. 2018: a 5x5 correlation with a type-A mask, channels-last, zero padded to
+  the input's size.  `kernel` is [5, 5, in, out] like SignalConv2D's; the training path multiplies it by the fixed
+  mask and runs one conv2d, the coding path reads the 12 causal taps from the packed parameters."""
+
+  def __init__(self, in_channels, filters):
+    super().__init__()
+    std = math.sqrt(1.0 / (12 * in_channels))
+    self.kernel = nn.Parameter(torch.randn(5, 5, in_channels, filters) * std)
+    self.bias = nn.Parameter(torch.zeros(filters))
+    self.register_buffer("mask", causal_mask(5)[:, :, None, None], persistent=False)
+
+  def forward(self, x):
+    w = (self.kernel * self.mask).permute(3, 2, 0, 1)
+    y = torch.nn.functional.conv2d(x.permute(0, 3, 1, 2), w.to(x.dtype), self.bias.to(x.dtype), padding=2)
+    return y.permute(0, 2, 3, 1).contiguous()
+
+
+class MBT2018Model(_Model):
+  """Joint autoregressive and hierarchical priors (Minnen, Ballé & Toderici, NeurIPS 2018, Fig. 4 / Table 1).
+  N = num_filters, M = latent_depth (a multiple of 6).  bmshj2018's analysis / synthesis with GDN; hyper analysis
+  of y (3x3 N, 5x5/2 N, 5x5/2 N); hyper synthesis to psi (5x5 x2 M, 5x5 x2 3M/2, 3x3 2M); a 5x5 type-A masked
+  context model M -> 2M; entropy parameters 1x1 4M -> 10M/3 -> 8M/3 -> 2M on [psi, ctx] = [loc, scale_index], with
+  LeakyReLU between layers.  z is coded with a NoisyDeepFactorized prior, y by a LocationScaleIndexedEntropyModel
+  (NoisyNormal, 64 scales from 0.11 to 256) with `loc`.
+
+  Coding runs on the parameter kernel (functional.ar_*): the encoder visits positions in raster order, then ONE
+  index-mode encode of y with the kernel's table indexes and loc makes the strings (the bytes of
+  `LocationScaleIndexedEntropyModel.compress(y, scale_index, loc)`); the decoder runs the parameter step and the
+  M symbols of each position in one launch.  The hyper synthesis runs per image, so psi, and with it the decoded
+  latents, do not depend on how images were batched."""
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.):
+    super().__init__()
+    N, M = int(num_filters), int(latent_depth)
+    if M <= 0 or M % 6:
+      raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
+    self.lmbda = lmbda
+    self.num_filters, self.latent_depth, self.num_scales = N, M, int(num_scales)
+    offset = math.log(scale_min)
+    factor = (math.log(scale_max) - math.log(scale_min)) / (num_scales - 1.)
+    self.scale_fn = lambda i: torch.exp(offset + factor * i)
+    self.analysis_transform = nn.Sequential(
+        _Scale(1 / 255.), *[_conv(N, 5, f"layer_{i}", down=2, activation=GDN(name=f"gdn_{i}")) for i in range(3)],
+        _conv(M, 5, "layer_3", down=2))
+    self.synthesis_transform = SynthesisTransform(N, hyperprior=True)
+    self.hyper_analysis_transform = nn.Sequential(
+        _conv(N, 3, "layer_0", activation=_leaky), _conv(N, 5, "layer_1", down=2, activation=_leaky),
+        _conv(N, 5, "layer_2", down=2, use_bias=False))
+    hs = lambda f, k, name, up, act: _conv(f, k, name, up=up, corr=False, kernel_parameter="variable", activation=act)
+    self.hyper_synthesis_transform = nn.Sequential(
+        hs(M, 5, "layer_0", 2, _leaky), hs(3 * M // 2, 5, "layer_1", 2, _leaky), hs(2 * M, 3, "layer_2", 1, None))
+    self.context_model = MaskedConv2D(M, 2 * M)
+    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
+    self.entropy_parameters = nn.Sequential(
+        ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(2 * M, "layer_2", None))
+    self.hyperprior = D.NoisyDeepFactorized(batch_shape=(N,))
+    self.entropy_model = None
+    self.side_entropy_model = None
+    self._packed = None
+
+  def _psi(self, z_hat, y_hw):
+    """The hyper feature of each image, computed one image at a time, cropped to y's size: [B, H, W, 2M]."""
+    return torch.cat([self.hyper_synthesis_transform(z_hat[i:i + 1])[:, :y_hw[0], :y_hw[1], :]
+                      for i in range(z_hat.shape[0])]).contiguous()
+
+  def entropy_parameters_of(self, y_ctx, psi):
+    """The parallel (training) form of the parameter network: (loc, scale_index) of every position from the latents
+    the context model sees and psi."""
+    ctx = self.context_model(y_ctx)
+    params = self.entropy_parameters(torch.cat([psi, ctx], dim=-1))
+    return params[..., :self.latent_depth], params[..., self.latent_depth:]
+
+  def forward(self, x, training=True):
+    """-> (loss, bpp, mse).  The context model sees y plus uniform noise when training, round(y) otherwise."""
+    entropy_model = E.LocationScaleIndexedEntropyModel(D.NoisyNormal, self.num_scales, self.scale_fn, coding_rank=3,
+                                                       compression=False)
+    side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3, compression=False)
+    x = x.to(torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    z_hat, side_bits = side_entropy_model(z, training=training)
+    psi = self.hyper_synthesis_transform(z_hat)[:, :y.shape[1], :y.shape[2], :]
+    y_ctx = y + torch.empty_like(y).uniform_(-.5, .5) if training else torch.round(y)
+    loc, scale_index = self.entropy_parameters_of(y_ctx, psi)
+    y_hat, bits = entropy_model(y, scale_index, loc=loc, training=training)
+    self._last_x_hat = self.synthesis_transform(y_hat)[:, :x.shape[1], :x.shape[2], :]
+    return self.rate_distortion(x, bits.sum() + side_bits.sum())
+
+  def fix_tables(self):
+    """Builds the coding tables and packs the parameter network for the coding kernels (call again after the
+    weights change)."""
+    dev = self._device()
+    self.entropy_model = E.LocationScaleIndexedEntropyModel(D.NoisyNormal, self.num_scales, self.scale_fn,
+                                                            coding_rank=3, compression=True).to(dev)
+    self.side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3, compression=True).to(dev)
+    layers = list(self.entropy_parameters)
+    if any(not layer.built for layer in layers):
+      raise RuntimeError("the entropy-parameter layers are not built: call build() first")
+    w = [t for layer in layers for t in (layer.kernel.reshape(layer.kernel.shape[-2:]), layer.bias)]
+    self._packed = F.ar_pack_weights(self.context_model.kernel, self.context_model.bias, *w)
+    return self
+
+  # -- coding: one latent shape per call --
+  def _encode_latents(self, y, psi):
+    """(strings, y_hat, loc, index) of latents y [B, H, W, M] with hyper feature psi."""
+    em = self.entropy_model
+    y = y.contiguous()
+    y_hat, loc, index = F.ar_encode(self._packed, y, psi, self.num_scales)
+    strings = F.compress_f32((y.shape[0],), em._lookup_host(), y, loc, em.cdf_offset.to(y.device), index=index)
+    return strings, y_hat, loc, index
+
+  def _decode_latents(self, strings, psi):
+    em = self.entropy_model
+    handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
+    y_hat = F.ar_decode(handle, self._packed, psi, self.num_scales, em.cdf_offset.to(psi.device))
+    em._finish_decode(handle)
+    return y_hat
+
+  def compress(self, x):
+    """uint8 [H, W, 3] -> (string, side_string, x_shape, y_shape, z_shape), bmshj2018's signature."""
+    return self.compress_batch(_as_image(x)[None])
+
+  def decompress(self, string, side_string, x_shape, y_shape, z_shape):
+    return self.decompress_batch(string, side_string, x_shape, y_shape, z_shape)[0]
+
+  @torch.no_grad()
+  def compress_batch(self, x):
+    x = _as_batch(x).to(device=self._device(), dtype=torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    shapes = tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+    side_string = self.side_entropy_model.compress(z)
+    psi = self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))
+    string = self._encode_latents(y, psi)[0]
+    return (string, side_string) + shapes
+
+  @torch.no_grad()
+  def decompress_batch(self, string, side_string, x_shape, y_shape, z_shape):
+    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape))
+    psi = self._psi(z_hat, (int(y_shape[0]), int(y_shape[1])))
+    y_hat = self._decode_latents(string, psi)
+    x_hat = self.synthesis_transform(y_hat)
+    return _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])
+
+  # -- lists of differently sized images: transforms per image, coding grouped by latent shape --
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element.
+    The transforms run per image; images of one latent shape share one encoder launch and one range encode."""
+    xs = [_as_image(x)[None].to(device=self._device(), dtype=torch.float32) for x in images]
+    if not xs:
+      raise ValueError("`images` is empty")
+    ys = [self.analysis_transform(x) for x in xs]
+    zs = [self.hyper_analysis_transform(y) for y in ys]
+    side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs]).split()
+    psis = [self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1])) for y, z in zip(ys, zs)]
+    strings = [None] * len(xs)
+    for members in self._groups([tuple(y.shape[1:-1]) for y in ys]):
+      group = self._encode_latents(torch.cat([ys[i] for i in members]), torch.cat([psis[i] for i in members]))[0]
+      for i, s in zip(members, group.split()):
+        strings[i] = s
+    return [(strings[i], side_strings[i]) + tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+            for i, (x, y, z) in enumerate(zip(xs, ys, zs))]
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
+    items = list(items)
+    if not items:
+      raise ValueError("`items` is empty")
+    z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
+                                                       [tuple(int(v) for v in it[4]) for it in items])
+    y_hws = [(int(it[3][0]), int(it[3][1])) for it in items]
+    psis = [self._psi(z_hat[None], hw) for z_hat, hw in zip(z_hats, y_hws)]
+    out = [None] * len(items)
+    for members in self._groups(y_hws):
+      y_hat = self._decode_latents(gen_ops.Strings.concat([items[i][0] for i in members]),
+                                   torch.cat([psis[i] for i in members]))
+      for k, i in enumerate(members):
+        x_shape = items[i][2]
+        x_hat = self.synthesis_transform(y_hat[k:k + 1])
+        out[i] = _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0]
+    return out
+
+  @staticmethod
+  def _groups(shapes):
+    """Indexes of the items of each distinct shape, in order of first appearance."""
+    groups = {}
+    for i, s in enumerate(shapes):
+      groups.setdefault(tuple(s), []).append(i)
+    return list(groups.values())
+
+  def decompress_from_tfci(self, data):
+    dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
     return self.decompress(*PackedTensors(data).unpack(dtypes))
 
 

@@ -215,6 +215,47 @@ int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream);
 void tfcb_decoder_destroy(tfcb_decoder* h);
 
 /* ------------------------------------------------------------------------------------------------
+ * Joint autoregressive + hierarchical prior (Minnen, Ballé & Toderici 2018): the entropy parameters of a latent
+ * position from its 12 causal neighbours (5x5 type-A mask) and the hyper feature psi, and the serial encoder /
+ * decoder over positions.  M = latent depth, a multiple of 6 in [6, 384]; latents are channels-last float32
+ * [B, H, W, M], psi [B, H, W, 2M]; positions p = y * W + x run in raster order.  Per position and image:
+ *   ctx = Wc * taps + bc (2M); h1 = leaky(W1 * [psi_p, ctx] + b1) (10M/3); h2 = leaky(W2 * h1 + b2) (8M/3);
+ *   [loc, scale_index] = W3 * h2 + b3 (M each); index = int32(min(max(scale_index, 0), num_scales - 1)),
+ * leaky(x) = x > 0 ? x : 0.01 x.  Each output is one fixed sequence of float32 operations that depends only on
+ * that image's inputs: results do not depend on B, an image's place in the batch, or the device's SM count.
+ * Every call checks M, the packed size, shapes, the position range and null pointers before any device work.
+ * ---------------------------------------------------------------------------------------------- */
+/* Floats of the packed parameter buffer for latent depth M, or -1 if M is not supported. */
+int64_t tfcb_ar_packed_floats(int M);
+/* Packs the parameters into `packed_dev` (tfcb_ar_packed_floats(M) floats), stream-ordered device copies of the
+ * values unchanged: the context kernel [5, 5, M, 2M] (its first 12 taps in raster order are the causal ones), its
+ * bias [2M], then W1 [4M, 10M/3], b1, W2 [10M/3, 8M/3], b2, W3 [8M/3, 2M], b3 (inputs x outputs, row major). */
+int tfcb_ar_pack_weights(int M, const float* ctx_kernel_dev, const float* ctx_bias_dev, const float* w1_dev,
+                         const float* b1_dev, const float* w2_dev, const float* b2_dev, const float* w3_dev,
+                         const float* b3_dev, float* packed_dev, int64_t packed_floats, void* stream);
+/* Parameter step: loc, scale_index and the table index [B, M] of position p for every image, from the decoded
+ * latents `yhat_dev` at earlier positions (later positions are not read).  Each output may be NULL.  One launch. */
+int tfcb_ar_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,
+                   int64_t B, int64_t H, int64_t W, int64_t p, int num_scales, float* loc_dev, float* scale_index_dev,
+                   int32_t* index_dev, void* stream);
+/* Encoder steps p_begin <= p < p_end: per position the parameter step, then yhat = float(int32(rint(y - loc))) +
+ * loc, the value tfcb_decode_index_f32 returns for the symbol an index-mode encode with this loc codes.  Writes
+ * yhat, loc and index [B, H, W, M] (and scale_index, if not NULL) at those positions; yhat must hold the earlier
+ * positions.  The strings are made afterwards by one index-mode encode (tfcb_compress) of y with index and loc.
+ * One launch, no host synchronisation. */
+int tfcb_ar_encode(const float* packed_dev, int64_t packed_floats, int M, const float* y_dev, const float* psi_dev,
+                   int64_t B, int64_t H, int64_t W, int64_t p_begin, int64_t p_end, int num_scales, float* yhat_dev,
+                   float* loc_dev, int32_t* index_dev, float* scale_index_dev, void* stream);
+/* Decoder steps p_begin <= p < p_end: per position the parameter step, then the M symbols of each of the B streams
+ * of `h` (which must hold B strings, made with index-mode tables of at least num_scales rows) are decoded from the
+ * handle's state and dequantised like tfcb_decode_index_f32: yhat[b, p, c] = float(sym + cdf_offset[index]) + loc.
+ * The handle's state advances as with the other decode calls, so steps may be mixed with them and
+ * tfcb_decode_finalize reports each stream.  One launch, no host synchronisation. */
+int tfcb_ar_decode(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
+                   int64_t B, int64_t H, int64_t W, int64_t p_begin, int64_t p_end, int num_scales,
+                   const int32_t* cdf_offset_dev, float* yhat_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Legacy single-stream ops RangeEncode / RangeDecode (int16 data, broadcastable N-D int32 CDF):
  *   op contract   tensorflow_compression/cc/ops/range_coding_ops.cc:30-124
  *   CPU kernels   tensorflow_compression/cc/kernels/range_coding_kernels.cc:60-379
