@@ -14,6 +14,7 @@ from compression_b200 import entropy_models as E
 from compression_b200 import functional as F
 from compression_b200 import gen_ops
 from compression_b200 import models
+from oracle import ar_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -186,13 +187,16 @@ def test_params_match_a_float64_restatement(M):
   y_hat = torch.round(y_hat)
   ws = _weights(M, 0)
   packed = _packed(M)
-  for p in (0, 1, 10, 30, 53):
+  positions = (0, 1, 10, 30, 53)
+  bounds = ar_oracle.bound64(ws, y_hat, psi, positions)  # per element: the kernel order's derived error bound
+  for i, p in enumerate(positions):
     loc, scale, _ = F.ar_params(packed, y_hat, psi, p, NUM_SCALES)
     rloc, rscale = _reference64(ws, y_hat, psi, p)
-    # float32 with fixed-order sums of up to 12M terms: within 2e-5 of the output's scale
-    for got, want in ((loc, rloc), (scale, rscale)):
-      err = (got.double().cpu() - want).abs().max().item()
-      assert err <= 2e-5 * (1 + want.abs().max().item()), (p, err)
+    # float32 with fixed-order sums of up to 12M terms: within 2e-5 of the output's scale, and within the bound
+    for got, want, bound in ((loc, rloc, bounds[0]), (scale, rscale, bounds[1])):
+      err = (got.double().cpu() - want).abs()
+      assert err.max().item() <= 2e-5 * (1 + want.abs().max().item()), (p, err.max().item())
+      assert bool((err <= torch.from_numpy(bound[:, i])).all()), p
 
 
 @pytest.fixture(scope="module")
