@@ -11,9 +11,13 @@
 // CTA walks 64-pixel tiles; warp w owns 8 pixels, lane l owns output channels {l + 32 m}; the pool
 // tile is read with 128-bit broadcast loads (4 input channels at a time), gamma rows with
 // conflict-free scalar loads.  The wgmma tensor-core path lives in gdn_tc.cu.
+//
+// The C entry points at the end check their own arguments, ask gdn_tc_route (gdn_tc.cuh) which tensor-core kernels
+// take the configuration, and call the one internal forward or backward; only float32 channels-last calls fall back to
+// the kernels above.  bwd_workspace is the one description of the backward workspace.
 #include <algorithm>
 
-#include "common.cuh"
+#include "gdn_tc.cuh"
 
 namespace tfcb {
 namespace {
@@ -429,79 +433,63 @@ __global__ void __launch_bounds__(128) gdn_bwd_exponents_kernel(const float* __r
 
 constexpr int kExpGrid = 1184;  // blocks of the exponent-gradient kernel (fixed: the reduction order does not depend on the GPU)
 
-int parse_flags(int flags, float alpha, float eps, GdnFlags* f) {
-  f->inverse = (flags & TFCB_GDN_INVERSE) != 0;
-  f->rectify = (flags & TFCB_GDN_RECTIFY) != 0;
-  f->alpha = alpha;
-  f->eps = eps;
-  f->alpha_mode = (alpha == 1.f) ? 1 : ((alpha == 2.f) ? 2 : 0);
-  f->eps_mode = (eps == 1.f) ? 1 : ((eps == 0.5f) ? 2 : 0);
+GdnFlags parse_flags(int flags, float alpha, float eps) {
+  GdnFlags f;
+  f.inverse = (flags & TFCB_GDN_INVERSE) != 0;
+  f.rectify = (flags & TFCB_GDN_RECTIFY) != 0;
+  f.alpha = alpha;
+  f.eps = eps;
+  f.alpha_mode = (alpha == 1.f) ? 1 : ((alpha == 2.f) ? 2 : 0);
+  f.eps_mode = (eps == 1.f) ? 1 : ((eps == 0.5f) ? 2 : 0);
   // trainable exponents: the reference takes `inputs ** alpha` / `norm_pool ** epsilon` whatever the current value
   // (gdn.py:380-388,406-411: the fixed-exponent shortcuts apply only when the parameter is not callable)
-  if (flags & TFCB_GDN_POW_ALPHA) f->alpha_mode = 0;
-  if (flags & TFCB_GDN_POW_EPSILON) f->eps_mode = 0;
-  return TFCB_OK;
-}
-
-int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
+  if (flags & TFCB_GDN_POW_ALPHA) f.alpha_mode = 0;
+  if (flags & TFCB_GDN_POW_EPSILON) f.eps_mode = 0;
+  return f;
 }
 
 bool fast_c(int C) { return C % 32 == 0 && C >= 32 && C <= 192; }
 
-// The tiled kernels read x (and q) with 16-byte loads: other pointers take the generic kernels.
-bool aligned16(const void* a, const void* b, const void* c) {
-  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
-}
-
 size_t fast_smem(int C) { return ((size_t)C * C + (size_t)kTM * (C + 4)) * sizeof(float); }
 
-template <typename K>
-int set_smem(K kernel, size_t bytes) {
-  TFCB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+// The backward workspace, as byte offsets from its start and its size.  q comes first, for whole 128-pixel tiles (the
+// C = 192 tensor-core pair hands q over tile by tile), then the per-CTA partials part_g [kMaxParts][C][C] and part_b
+// [kMaxParts][C].  The 16-bit layout puts the tensor-core dx scratch right after them.  The float32 ones leave 256
+// bytes, then hold the exponent partials [kExpGrid][2] when `exponents`, and the scratch after those when `scratch`.
+// Every offset is a multiple of 16 bytes.
+struct BwdWorkspace {
+  int64_t part_g, part_b, part_e, scratch, bytes;
+};
+
+BwdWorkspace bwd_workspace(int64_t n_pix, int C, bool exponents, bool scratch) {
+  const int64_t f = sizeof(float);
+  BwdWorkspace w;
+  w.part_g = (n_pix + 127) / 128 * 128 * C * f;
+  w.part_b = w.part_g + (int64_t)kMaxParts * C * C * f;
+  const int64_t parts_end = w.part_b + (int64_t)kMaxParts * C * f;
+  w.part_e = parts_end + 256;
+  const int64_t exp_end = w.part_e + (exponents ? kExpGrid * 2 * f : 0);
+  w.scratch = exponents ? exp_end : parts_end;
+  w.bytes = exp_end + (scratch ? gdn_tc_scratch_floats(n_pix, C) * f : 0);
+  return w;
+}
+
+float* at(void* ws, int64_t offset) { return reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + offset); }
+
+int check_shape(int64_t n_pix, int C) {
+  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
   return TFCB_OK;
 }
 
-constexpr int kDgammaGrid = 148;
-
-}  // namespace
-
-int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
-                   int flags, float alpha, float eps, cudaStream_t s, bool* handled);
-int gdn_tc_forward16(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, int C, int flags,
-                     float alpha, float eps, int dtype, cudaStream_t s, bool* handled);
-int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                    float* part_g, float* part_b, int* n_parts, long long n_pix, int C, int flags, float alpha,
-                    float eps, cudaStream_t s, bool* handled);
-int gdn_tc_backward_exponents(const float* x, const float* gamma, const float* beta, const float* dy, float* dx,
-                              float* q_ws, float* part_g, float* part_b, float* part_e, int* n_parts, int* n_parts_e,
-                              long long n_pix, int C, int flags, float alpha, float eps, cudaStream_t s,
-                              bool* handled);
-long long gdn_tc_backward16_scratch_floats(long long n_pix, int C);
-int gdn_tc_backward16(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
-                      float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, int C, int flags,
-                      float alpha, float eps, int dtype, cudaStream_t s, bool* handled);
-bool gdn_tc_cf_config(int C, int dtype, int flags, float alpha, float eps, bool* pow);
-int gdn_tc_forward_cf(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, long long S,
-                      int C, int flags, float alpha, float eps, int dtype, cudaStream_t s);
-int gdn_tc_backward_cf(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
-                       float* part_g, float* part_b, float* scratch, float* part_e, int* n_parts, int* n_parts_e,
-                       long long n_pix, long long S, int C, int flags, float alpha, float eps, int dtype,
-                       cudaStream_t s);
-
-namespace {
+template <class... P>
+int check_pointers(P... p) {
+  return (!p || ...) ? fail(TFCB_INVALID_ARGUMENT, "null pointer") : TFCB_OK;
+}
 
 // The host-side checks of the channels-first entries, before any device work: sizes (*n_pix = n_items * spatial
-// without overflow, nor of n_pix * C), dtype and a configuration with kernels (*pow: the literal-pow ones).
+// without overflow, nor of n_pix * C), dtype and a configuration with kernels (*r).
 int cf_check(int64_t n_items, int64_t spatial, int C, int dtype, int flags, float alpha, float eps, int64_t* n_pix,
-             bool* pow) {
+             TcRoute* r) {
   int64_t n = 0, elems = 0;
   if (n_items < 0 || spatial < 0 || C <= 0)
     return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_items=%lld spatial=%lld C=%d", (long long)n_items,
@@ -510,7 +498,8 @@ int cf_check(int64_t n_items, int64_t spatial, int C, int dtype, int flags, floa
     return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_items * spatial * C overflows (n_items=%lld spatial=%lld C=%d)",
                 (long long)n_items, (long long)spatial, C);
   if (dtype < 0 || dtype > 2) return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: dtype must be 0, 1 or 2, got %d", dtype);
-  if (!gdn_tc_cf_config(C, dtype, flags, alpha, eps, pow))
+  *r = gdn_tc_route(C, dtype, flags, alpha, eps);
+  if (r->family == TcRoute::kNone)
     return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for C=%d dtype=%d flags=%d alpha=%g epsilon=%g "
                 "(float32 at C = 128, 192, 256, 320; 16 bits at C = 128, 192 with alpha in {1, 2}, epsilon in {1, 1/2}; "
                 "not under TFCB_GDN_FP32=1): transpose to channels-last for this configuration",
@@ -519,15 +508,17 @@ int cf_check(int64_t n_items, int64_t spatial, int C, int dtype, int flags, floa
   return TFCB_OK;
 }
 
-bool unaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+// n_pix = 0: no kernel, the gradients are the empty sums.
+int zero_grads(float* dgamma, float* dbeta, float* dalpha_depsilon, int C, cudaStream_t s) {
+  if (dgamma) TFCB_CUDA_TRY(cudaMemsetAsync(dgamma, 0, (size_t)C * C * sizeof(float), s));
+  if (dbeta) TFCB_CUDA_TRY(cudaMemsetAsync(dbeta, 0, (size_t)C * sizeof(float), s));
+  if (dalpha_depsilon) TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon, 0, 2 * sizeof(float), s));
+  return TFCB_OK;
+}
 
-}  // namespace
-
-namespace {
-
-// dgamma, dbeta from the per-CTA partials of the tensor-core backward, summed in a fixed order.
-void reduce_tc_partials(const float* part_g, const float* part_b, int n_parts, int C, float* dgamma, float* dbeta,
-                        cudaStream_t s) {
+// dgamma, dbeta from per-CTA partials, summed in a fixed order.
+void reduce_dgamma(const float* part_g, const float* part_b, int n_parts, int C, float* dgamma, float* dbeta,
+                   cudaStream_t s) {
   const long long ng = (long long)C * C;
   reduce_partials_kernel<<<(unsigned)((ng + 255) / 256), 256, 0, s>>>(part_g, n_parts, ng, dgamma);
   reduce_partials_kernel<<<(unsigned)((C + 255) / 256), 256, 0, s>>>(part_b, n_parts, C, dbeta);
@@ -535,11 +526,17 @@ void reduce_tc_partials(const float* part_g, const float* part_b, int n_parts, i
   TFCB_LAUNCHED();
 }
 
-}  // namespace
-
-}  // namespace tfcb
-
-using namespace tfcb;
+// dL/dalpha, dL/depsilon from the exponent kernel's partials `part` [kExpGrid][2], n_pix > 0.
+int exponent_grads(const float* x, const float* gamma, const float* beta, const float* dy, float* dalpha_depsilon,
+                   float* part, int64_t n_pix, int C, const GdnFlags& f, cudaStream_t s) {
+  const int grid = (int)std::min<long long>((n_pix + 3) / 4, kExpGrid);
+  gdn_bwd_exponents_kernel<<<grid, 128, (size_t)C * 4 * sizeof(float), s>>>(x, gamma, beta, dy, part, n_pix, C, f);
+  reduce_partials_kernel<<<1, 32, 0, s>>>(part, grid, 2, dalpha_depsilon);
+  TFCB_LAUNCHED();
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
 
 #define DISPATCH_CPL(C, ...)                                   \
   switch ((C) / 32) {                                          \
@@ -552,148 +549,155 @@ using namespace tfcb;
     default: return fail(TFCB_INVALID_ARGUMENT, "unsupported channel count %d", (C)); \
   }
 
+// Every forward entry after its checks, n_pix > 0: the route's tensor-core kernels, or for kNone (float32
+// channels-last only) the CUDA-core ones, tiled where x and y allow 16-byte loads.
+int forward(const TcRoute& r, bool channels_first, const void* x, const float* gamma, const float* beta, void* y,
+            int64_t n_pix, int64_t S, cudaStream_t s) {
+  if (r.family != TcRoute::kNone) {
+    TFCB_TRY(gdn_tc_forward(r, channels_first, x, gamma, beta, y, n_pix, S, s));
+  } else {
+    const int C = r.C;
+    const GdnFlags f = parse_flags(r.flags, r.alpha, r.eps);
+    const float* xf = static_cast<const float*>(x);
+    float* yf = static_cast<float*>(y);
+    if (fast_c(C) && aligned16(x, y)) {
+      const size_t smem = fast_smem(C);
+      const long long n_tiles = (n_pix + kTM - 1) / kTM;
+      const int grid = (int)std::min<long long>(n_tiles, sm_count());
+      DISPATCH_CPL(C, {
+        TFCB_TRY(set_smem(gdn_fwd_kernel<CPL>, smem));
+        gdn_fwd_kernel<CPL><<<grid, kThreads, smem, s>>>(xf, gamma, beta, yf, n_pix, f);
+      });
+    } else {
+      const long long blocks = (n_pix + 3) / 4;
+      gdn_fwd_generic_kernel<<<(unsigned)blocks, 128, 0, s>>>(xf, gamma, beta, yf, n_pix, C, f);
+    }
+    TFCB_LAUNCHED();
+  }
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+// Every backward entry after its checks, n_pix > 0, on the workspace `w` lays out: the route's tensor-core kernels
+// and the reductions of their partials, or for kNone (float32 channels-last only) the CUDA-core kernels, tiled where
+// x, dy and dx allow 16-byte loads.  dalpha_depsilon, when not null, comes from the literal-pow kernels' fused
+// partials, and on any other route from the exponent kernel after the rest.
+int backward(const TcRoute& r, bool channels_first, const void* x, const float* gamma, const float* beta,
+             const void* dy, void* dx, float* dgamma, float* dbeta, float* dalpha_depsilon, void* ws,
+             const BwdWorkspace& w, int64_t n_pix, int64_t S, cudaStream_t s) {
+  const int C = r.C;
+  const GdnFlags f = parse_flags(r.flags, r.alpha, r.eps);
+  const float* xf = static_cast<const float*>(x);
+  const float* dyf = static_cast<const float*>(dy);
+  float* dxf = static_cast<float*>(dx);
+  float* q = static_cast<float*>(ws);
+  float* part_g = at(ws, w.part_g);
+  float* part_b = at(ws, w.part_b);
+  float* part_e = at(ws, w.part_e);
+  const bool fused_e = dalpha_depsilon && r.family == TcRoute::kPow;
+  if (r.family != TcRoute::kNone) {
+    float* scratch = channels_first || r.dtype != 0 ? at(ws, w.scratch) : nullptr;
+    int n_parts = 0, n_parts_e = 0;
+    TFCB_TRY(gdn_tc_backward(r, channels_first, x, gamma, beta, dy, dx, q, part_g, part_b, fused_e ? part_e : nullptr,
+                             scratch, n_pix, S, s, &n_parts, &n_parts_e));
+    reduce_dgamma(part_g, part_b, n_parts, C, dgamma, dbeta, s);
+    if (fused_e) {
+      reduce_partials_kernel<<<1, 32, 0, s>>>(part_e, n_parts_e, 2, dalpha_depsilon);
+      TFCB_LAUNCHED();
+    }
+  } else if (fast_c(C) && aligned16(x, dy, dx)) {
+    const size_t smem = fast_smem(C);
+    const long long n_tiles = (n_pix + kTM - 1) / kTM;
+    const int grid = (int)std::min<long long>(n_tiles, sm_count());
+    const int grid_g = (int)std::min<long long>((n_pix + 31) / 32, kMaxParts);
+    DISPATCH_CPL(C, {
+      TFCB_TRY(set_smem(gdn_bwd_q_kernel<CPL>, smem));
+      TFCB_TRY(set_smem(gdn_bwd_dx_kernel<CPL>, smem));
+      gdn_bwd_q_kernel<CPL><<<grid, kThreads, smem, s>>>(xf, gamma, beta, dyf, q, dxf, n_pix, f);
+      gdn_bwd_dx_kernel<CPL><<<grid, kThreads, smem, s>>>(xf, gamma, q, dxf, n_pix, f);
+      gdn_bwd_dgamma_kernel<CPL><<<grid_g, 256, 0, s>>>(xf, q, part_g, part_b, n_pix, f);
+    });
+    TFCB_LAUNCHED();
+    TFCB_LAUNCHED();
+    TFCB_LAUNCHED();
+    reduce_dgamma(part_g, part_b, grid_g, C, dgamma, dbeta, s);
+  } else {
+    const long long blocks = (n_pix + 3) / 4;
+    gdn_bwd_generic_kernel<<<(unsigned)blocks, 128, 0, s>>>(xf, gamma, beta, dyf, q, dxf, n_pix, C, f);
+    const long long e = (long long)C * C + C;
+    gdn_bwd_generic_dgamma_kernel<<<(unsigned)((e + 127) / 128), 128, 0, s>>>(xf, q, dgamma, dbeta, n_pix, C, f);
+    TFCB_LAUNCHED();
+    TFCB_LAUNCHED();
+  }
+  TFCB_CUDA_TRY(cudaGetLastError());
+  if (!dalpha_depsilon || fused_e) return TFCB_OK;
+  return exponent_grads(xf, gamma, beta, dyf, dalpha_depsilon, part_e, n_pix, C, f, s);
+}
+
+}  // namespace
+
+}  // namespace tfcb
+
+using namespace tfcb;
+
 extern "C" {
 
 int tfcb_gdn_forward(const float* x_dev, const float* gamma_dev, const float* beta_dev, float* y_dev,
                      int64_t n_pix, int C, int flags, float alpha, float epsilon, void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
+  TFCB_TRY(check_shape(n_pix, C));
   if (n_pix == 0) return TFCB_OK;
-  if (!x_dev || !gamma_dev || !beta_dev || !y_dev) return fail(TFCB_INVALID_ARGUMENT, "null pointer");
-  cudaStream_t s = as_stream(stream);
-  GdnFlags f;
-  parse_flags(flags, alpha, epsilon, &f);
-  bool handled = false;
-  TFCB_TRY(gdn_tc_forward(x_dev, gamma_dev, beta_dev, y_dev, n_pix, C, flags, alpha, epsilon, s, &handled));
-  if (handled) return TFCB_OK;
-  if (fast_c(C) && aligned16(x_dev, y_dev, nullptr)) {
-    const size_t smem = fast_smem(C);
-    const long long n_tiles = (n_pix + kTM - 1) / kTM;
-    const int grid = (int)std::min<long long>(n_tiles, sm_count());
-    DISPATCH_CPL(C, {
-      TFCB_TRY(set_smem(gdn_fwd_kernel<CPL>, smem));
-      gdn_fwd_kernel<CPL><<<grid, kThreads, smem, s>>>(x_dev, gamma_dev, beta_dev, y_dev, n_pix, f);
-    });
-  } else {
-    const long long blocks = (n_pix + 3) / 4;
-    gdn_fwd_generic_kernel<<<(unsigned)blocks, 128, 0, s>>>(x_dev, gamma_dev, beta_dev, y_dev, n_pix, C, f);
-  }
-  TFCB_LAUNCHED();
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, y_dev));
+  TcRoute r = gdn_tc_route(C, 0, flags, alpha, epsilon);
+  if (!aligned16(x_dev, y_dev, beta_dev)) r.family = TcRoute::kNone;
+  return forward(r, false, x_dev, gamma_dev, beta_dev, y_dev, n_pix, 1, as_stream(stream));
 }
 
 int tfcb_gdn_forward_16bit(const void* x_dev, const float* gamma_dev, const float* beta_dev, void* y_dev, int64_t n_pix,
                            int C, int dtype, int flags, float alpha, float epsilon, void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
+  TFCB_TRY(check_shape(n_pix, C));
   if (dtype != 1 && dtype != 2) return fail(TFCB_INVALID_ARGUMENT, "GDN 16-bit: dtype must be 1 (float16) or 2 (bfloat16)");
-  if (!x_dev || !gamma_dev || !beta_dev || !y_dev) return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, y_dev));
   if (n_pix == 0) return TFCB_OK;
-  bool handled = false;
-  TFCB_TRY(gdn_tc_forward16(x_dev, gamma_dev, beta_dev, y_dev, n_pix, C, flags, alpha, epsilon, dtype, as_stream(stream), &handled));
-  if (!handled)
+  const TcRoute r = gdn_tc_route(C, dtype, flags, alpha, epsilon);
+  if (r.family == TcRoute::kNone || !aligned16(x_dev, y_dev, beta_dev))
     return fail(TFCB_INVALID_ARGUMENT, "GDN 16-bit: only C = 128 or 192 with alpha in {1, 2}, epsilon in {1, 1/2} has a native 16-bit kernel; "
                 "convert to float32 for this configuration");
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  return forward(r, false, x_dev, gamma_dev, beta_dev, y_dev, n_pix, 1, as_stream(stream));
 }
 
-int64_t tfcb_gdn_backward_workspace_bytes(int64_t n_pix, int C) {
-  const int64_t q = ((n_pix + 127) / 128 * 128) * C * (int64_t)sizeof(float);  // whole 128-pixel tiles (the C = 192 tensor-core pair hands q over tile by tile)
-  const int64_t parts = (int64_t)kDgammaGrid * ((int64_t)C * C + C) * (int64_t)sizeof(float);
-  return q + parts + 256;
-}
+int64_t tfcb_gdn_backward_workspace_bytes(int64_t n_pix, int C) { return bwd_workspace(n_pix, C, false, false).bytes; }
 
 int tfcb_gdn_backward(const float* x_dev, const float* gamma_dev, const float* beta_dev, const float* dy_dev,
                       float* dx_dev, float* dgamma_dev, float* dbeta_dev, void* workspace_dev, int64_t n_pix,
                       int C, int flags, float alpha, float epsilon, void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
-  if (!x_dev || !gamma_dev || !beta_dev || !dy_dev || !dx_dev || !dgamma_dev || !dbeta_dev || !workspace_dev)
-    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  TFCB_TRY(check_shape(n_pix, C));
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, workspace_dev));
   cudaStream_t s = as_stream(stream);
-  GdnFlags f;
-  parse_flags(flags, alpha, epsilon, &f);
-  if (n_pix == 0) {
-    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
-    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
-    return TFCB_OK;
-  }
-  float* q = reinterpret_cast<float*>(workspace_dev);
-  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
-  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
-  bool handled = false;
-  int n_parts = 0;
-  TFCB_TRY(gdn_tc_backward(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b, &n_parts, n_pix, C, flags,
-                           alpha, epsilon, s, &handled));
-  if (handled) {
-    reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
-  } else if (fast_c(C) && aligned16(x_dev, dy_dev, dx_dev)) {
-    const size_t smem = fast_smem(C);
-    const long long n_tiles = (n_pix + kTM - 1) / kTM;
-    const int grid = (int)std::min<long long>(n_tiles, sm_count());
-    const int grid_g = (int)std::min<long long>((n_pix + 31) / 32, kDgammaGrid);
-    DISPATCH_CPL(C, {
-      TFCB_TRY(set_smem(gdn_bwd_q_kernel<CPL>, smem));
-      TFCB_TRY(set_smem(gdn_bwd_dx_kernel<CPL>, smem));
-      gdn_bwd_q_kernel<CPL><<<grid, kThreads, smem, s>>>(x_dev, gamma_dev, beta_dev, dy_dev, q, dx_dev, n_pix, f);
-      gdn_bwd_dx_kernel<CPL><<<grid, kThreads, smem, s>>>(x_dev, gamma_dev, q, dx_dev, n_pix, f);
-      gdn_bwd_dgamma_kernel<CPL><<<grid_g, 256, 0, s>>>(x_dev, q, part_g, part_b, n_pix, f);
-    });
-    TFCB_LAUNCHED();
-    TFCB_LAUNCHED();
-    TFCB_LAUNCHED();
-    const long long ng = (long long)C * C;
-    reduce_partials_kernel<<<(unsigned)((ng + 255) / 256), 256, 0, s>>>(part_g, grid_g, ng, dgamma_dev);
-    reduce_partials_kernel<<<(unsigned)((C + 255) / 256), 256, 0, s>>>(part_b, grid_g, C, dbeta_dev);
-    TFCB_LAUNCHED();
-    TFCB_LAUNCHED();
-  } else {
-    const long long blocks = (n_pix + 3) / 4;
-    gdn_bwd_generic_kernel<<<(unsigned)blocks, 128, 0, s>>>(x_dev, gamma_dev, beta_dev, dy_dev, q, dx_dev, n_pix,
-                                                            C, f);
-    const long long e = (long long)C * C + C;
-    gdn_bwd_generic_dgamma_kernel<<<(unsigned)((e + 127) / 128), 128, 0, s>>>(x_dev, q, dgamma_dev, dbeta_dev,
-                                                                             n_pix, C, f);
-    TFCB_LAUNCHED();
-    TFCB_LAUNCHED();
-  }
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  if (n_pix == 0) return zero_grads(dgamma_dev, dbeta_dev, nullptr, C, s);
+  TcRoute r = gdn_tc_route(C, 0, flags, alpha, epsilon);
+  if (!aligned16(x_dev, dy_dev, dx_dev, workspace_dev, beta_dev)) r.family = TcRoute::kNone;
+  return backward(r, false, x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, nullptr, workspace_dev,
+                  bwd_workspace(n_pix, C, false, false), n_pix, 1, s);
 }
 
-// The float32 backward's workspace (q, the partials) followed by the direct-term scratch of the 16-bit dx kernel.
-int64_t tfcb_gdn_backward_16bit_workspace_bytes(int64_t n_pix, int C) {
-  return tfcb_gdn_backward_workspace_bytes(n_pix, C) +
-         (int64_t)gdn_tc_backward16_scratch_floats(n_pix, C) * (int64_t)sizeof(float);
-}
+int64_t tfcb_gdn_backward_16bit_workspace_bytes(int64_t n_pix, int C) { return bwd_workspace(n_pix, C, false, true).bytes; }
 
 int tfcb_gdn_backward_16bit(const void* x_dev, const float* gamma_dev, const float* beta_dev, const void* dy_dev,
                             void* dx_dev, float* dgamma_dev, float* dbeta_dev, void* workspace_dev, int64_t n_pix,
                             int C, int dtype, int flags, float alpha, float epsilon, void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
+  TFCB_TRY(check_shape(n_pix, C));
   if (dtype != 1 && dtype != 2) return fail(TFCB_INVALID_ARGUMENT, "GDN 16-bit: dtype must be 1 (float16) or 2 (bfloat16)");
-  if (!x_dev || !gamma_dev || !beta_dev || !dy_dev || !dx_dev || !dgamma_dev || !dbeta_dev || !workspace_dev)
-    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, workspace_dev));
   cudaStream_t s = as_stream(stream);
-  if (n_pix == 0) {  // as tfcb_gdn_backward: no kernel, dgamma / dbeta are the empty sums
-    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
-    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
-    return TFCB_OK;
-  }
-  // the layout of tfcb_gdn_backward's workspace, then the scratch
-  float* q = reinterpret_cast<float*>(workspace_dev);
-  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
-  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
-  float* scratch = part_b + (size_t)kDgammaGrid * C;
-  bool handled = false;
-  int n_parts = 0;
-  TFCB_TRY(gdn_tc_backward16(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b, scratch, &n_parts, n_pix,
-                             C, flags, alpha, epsilon, dtype, s, &handled));
-  if (!handled)
+  if (n_pix == 0) return zero_grads(dgamma_dev, dbeta_dev, nullptr, C, s);
+  const TcRoute r = gdn_tc_route(C, dtype, flags, alpha, epsilon);
+  const BwdWorkspace w = bwd_workspace(n_pix, C, false, true);
+  if (r.family == TcRoute::kNone ||
+      !aligned16(x_dev, dy_dev, dx_dev, workspace_dev, beta_dev, at(workspace_dev, w.scratch)))
     return fail(TFCB_INVALID_ARGUMENT, "GDN 16-bit backward: only C = 128 or 192 with alpha in {1, 2}, epsilon in {1, 1/2} "
                 "and 16-byte aligned pointers has a native 16-bit kernel; convert to float32 for this configuration");
-  reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  return backward(r, false, x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, nullptr, workspace_dev, w,
+                  n_pix, 1, s);
 }
 
 int64_t tfcb_gdn_exponent_grads_workspace_bytes(void) { return (int64_t)kExpGrid * 2 * (int64_t)sizeof(float); }
@@ -701,97 +705,55 @@ int64_t tfcb_gdn_exponent_grads_workspace_bytes(void) { return (int64_t)kExpGrid
 int tfcb_gdn_exponent_grads(const float* x_dev, const float* gamma_dev, const float* beta_dev, const float* dy_dev,
                             float* dalpha_depsilon_dev, void* workspace_dev, int64_t n_pix, int C, int flags,
                             float alpha, float epsilon, void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
-  if (!x_dev || !gamma_dev || !beta_dev || !dy_dev || !dalpha_depsilon_dev || !workspace_dev)
-    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  TFCB_TRY(check_shape(n_pix, C));
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, dy_dev, dalpha_depsilon_dev, workspace_dev));
   if ((size_t)C * 4 * sizeof(float) > 48 * 1024) return fail(TFCB_INVALID_ARGUMENT, "GDN exponent gradients: C too large");
   cudaStream_t s = as_stream(stream);
-  GdnFlags f;
-  parse_flags(flags, alpha, epsilon, &f);
-  if (n_pix == 0) {
-    TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon_dev, 0, 2 * sizeof(float), s));
-    return TFCB_OK;
-  }
-  const int grid = (int)std::min<long long>((n_pix + 3) / 4, kExpGrid);
-  float* part = reinterpret_cast<float*>(workspace_dev);
-  gdn_bwd_exponents_kernel<<<grid, 128, (size_t)C * 4 * sizeof(float), s>>>(x_dev, gamma_dev, beta_dev, dy_dev, part, n_pix, C, f);
-  reduce_partials_kernel<<<1, 32, 0, s>>>(part, grid, 2, dalpha_depsilon_dev);
-  TFCB_LAUNCHED();
-  TFCB_LAUNCHED();
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  if (n_pix == 0) return zero_grads(nullptr, nullptr, dalpha_depsilon_dev, C, s);
+  return exponent_grads(x_dev, gamma_dev, beta_dev, dy_dev, dalpha_depsilon_dev, static_cast<float*>(workspace_dev),
+                        n_pix, C, parse_flags(flags, alpha, epsilon), s);
 }
 
-// tfcb_gdn_backward's workspace, then the exponent partials [kExpGrid][2] (the exponent kernel's grid bounds the
-// tensor-core kernels' CTA count too).
 int64_t tfcb_gdn_backward_exponents_workspace_bytes(int64_t n_pix, int C) {
-  return tfcb_gdn_backward_workspace_bytes(n_pix, C) + tfcb_gdn_exponent_grads_workspace_bytes();
+  return bwd_workspace(n_pix, C, true, false).bytes;
 }
 
 int tfcb_gdn_backward_exponents(const float* x_dev, const float* gamma_dev, const float* beta_dev, const float* dy_dev,
                                 float* dx_dev, float* dgamma_dev, float* dbeta_dev, float* dalpha_depsilon_dev,
                                 void* workspace_dev, int64_t n_pix, int C, int flags, float alpha, float epsilon,
                                 void* stream) {
-  if (n_pix < 0 || C <= 0) return fail(TFCB_INVALID_ARGUMENT, "bad GDN shape: n_pix=%lld C=%d", (long long)n_pix, C);
-  if (!x_dev || !gamma_dev || !beta_dev || !dy_dev || !dx_dev || !dgamma_dev || !dbeta_dev || !dalpha_depsilon_dev ||
-      !workspace_dev)
-    return fail(TFCB_INVALID_ARGUMENT, "null pointer");
+  TFCB_TRY(check_shape(n_pix, C));
+  TFCB_TRY(check_pointers(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, dalpha_depsilon_dev,
+                          workspace_dev));
   if ((size_t)C * 4 * sizeof(float) > 48 * 1024) return fail(TFCB_INVALID_ARGUMENT, "GDN exponent gradients: C too large");
   cudaStream_t s = as_stream(stream);
-  if (n_pix == 0) {  // the empty sums, no kernel
-    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
-    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
-    TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon_dev, 0, 2 * sizeof(float), s));
-    return TFCB_OK;
-  }
-  float* q = reinterpret_cast<float*>(workspace_dev);
-  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
-  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
-  void* exp_ws = static_cast<uint8_t*>(workspace_dev) + tfcb_gdn_backward_workspace_bytes(n_pix, C);
-  bool handled = false;
-  int n_parts = 0, n_parts_e = 0;
-  TFCB_TRY(gdn_tc_backward_exponents(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b,
-                                     static_cast<float*>(exp_ws), &n_parts, &n_parts_e, n_pix, C, flags, alpha, epsilon,
-                                     s, &handled));
-  if (handled) {
-    reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
-    reduce_partials_kernel<<<1, 32, 0, s>>>(static_cast<const float*>(exp_ws), n_parts_e, 2, dalpha_depsilon_dev);
-    TFCB_LAUNCHED();
-    TFCB_CUDA_TRY(cudaGetLastError());
-    return TFCB_OK;
-  }
-  TFCB_TRY(tfcb_gdn_backward(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, workspace_dev, n_pix, C,
-                             flags, alpha, epsilon, stream));
-  return tfcb_gdn_exponent_grads(x_dev, gamma_dev, beta_dev, dy_dev, dalpha_depsilon_dev, exp_ws, n_pix, C, flags,
-                                 alpha, epsilon, stream);
+  if (n_pix == 0) return zero_grads(dgamma_dev, dbeta_dev, dalpha_depsilon_dev, C, s);
+  TcRoute r = gdn_tc_route(C, 0, flags, alpha, epsilon);
+  if (!aligned16(x_dev, dy_dev, dx_dev, workspace_dev, beta_dev)) r.family = TcRoute::kNone;
+  return backward(r, false, x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, dalpha_depsilon_dev,
+                  workspace_dev, bwd_workspace(n_pix, C, true, false), n_pix, 1, s);
 }
 
 int tfcb_gdn_forward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, void* y_dev, int64_t n_items,
                         int64_t spatial, int C, int dtype, int flags, float alpha, float epsilon, void* stream) {
   int64_t n_pix = 0;
-  bool pow = false;
-  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &pow));
+  TcRoute r{};
+  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &r));
   if (!gamma_dev || !beta_dev || (n_pix > 0 && (!x_dev || !y_dev))) return fail(TFCB_INVALID_ARGUMENT, "null pointer");
-  if (unaligned16(x_dev) || unaligned16(y_dev) || unaligned16(beta_dev))
+  if (!aligned16(x_dev, y_dev, beta_dev))
     return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: x, y and beta must be 16-byte aligned");
   if (n_pix == 0) return TFCB_OK;
-  TFCB_TRY(gdn_tc_forward_cf(x_dev, gamma_dev, beta_dev, y_dev, n_pix, spatial, C, flags, alpha, epsilon, dtype,
-                             as_stream(stream)));
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  return forward(r, true, x_dev, gamma_dev, beta_dev, y_dev, n_pix, spatial, as_stream(stream));
 }
 
-// 16 bits: tfcb_gdn_backward_16bit's workspace (q, the partials, the dx kernel's direct-term scratch); float32:
-// tfcb_gdn_backward_exponents' (q, the partials, the exponent partials) followed by the same scratch, which the
-// channels-first float32 dx kernel uses too.  -1 for arguments the entries reject.
+// 16 bits: tfcb_gdn_backward_16bit's workspace; float32: tfcb_gdn_backward_exponents' followed by the scratch, which
+// the channels-first float32 dx kernel uses too.  -1 for arguments the entries reject.
 int64_t tfcb_gdn_backward_cf_workspace_bytes(int64_t n_items, int64_t spatial, int C, int dtype) {
   int64_t n_pix = 0, elems = 0;
   if (n_items < 0 || spatial < 0 || C <= 0 || dtype < 0 || dtype > 2 ||
       __builtin_mul_overflow(n_items, spatial, &n_pix) || __builtin_mul_overflow(n_pix, (int64_t)C, &elems))
     return -1;
-  return dtype == 0 ? tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C) +
-                          (int64_t)gdn_tc_backward16_scratch_floats(n_pix, C) * (int64_t)sizeof(float)
-                    : tfcb_gdn_backward_16bit_workspace_bytes(n_pix, C);
+  return bwd_workspace(n_pix, C, dtype == 0, true).bytes;
 }
 
 int tfcb_gdn_backward_cf(const void* x_dev, const float* gamma_dev, const float* beta_dev, const void* dy_dev,
@@ -799,45 +761,21 @@ int tfcb_gdn_backward_cf(const void* x_dev, const float* gamma_dev, const float*
                          void* workspace_dev, int64_t n_items, int64_t spatial, int C, int dtype, int flags,
                          float alpha, float epsilon, void* stream) {
   int64_t n_pix = 0;
-  bool pow = false;
-  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &pow));
+  TcRoute r{};
+  TFCB_TRY(cf_check(n_items, spatial, C, dtype, flags, alpha, epsilon, &n_pix, &r));
   const bool want_e = (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) != 0;
   if (!gamma_dev || !beta_dev || !dgamma_dev || !dbeta_dev || !workspace_dev || (want_e && !dalpha_depsilon_dev) ||
       (n_pix > 0 && (!x_dev || !dy_dev || !dx_dev)))
     return fail(TFCB_INVALID_ARGUMENT, "null pointer");
-  if (dalpha_depsilon_dev && !pow)
+  if (dalpha_depsilon_dev && r.family != TcRoute::kPow)
     return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: dalpha_depsilon_dev must be NULL when alpha and epsilon are "
                 "fixed at the shortcut values (alpha in {1, 2}, epsilon in {1, 1/2})");
-  if (unaligned16(x_dev) || unaligned16(dy_dev) || unaligned16(dx_dev) || unaligned16(beta_dev) ||
-      unaligned16(workspace_dev))
+  if (!aligned16(x_dev, dy_dev, dx_dev, beta_dev, workspace_dev))
     return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: x, dy, dx, beta and the workspace must be 16-byte aligned");
   cudaStream_t s = as_stream(stream);
-  if (n_pix == 0) {  // as tfcb_gdn_backward: no kernel, the gradients are the empty sums
-    TFCB_CUDA_TRY(cudaMemsetAsync(dgamma_dev, 0, (size_t)C * C * sizeof(float), s));
-    TFCB_CUDA_TRY(cudaMemsetAsync(dbeta_dev, 0, (size_t)C * sizeof(float), s));
-    if (dalpha_depsilon_dev) TFCB_CUDA_TRY(cudaMemsetAsync(dalpha_depsilon_dev, 0, 2 * sizeof(float), s));
-    return TFCB_OK;
-  }
-  // the channels-last entries' workspace layouts: q, the partials, then the 16-bit dx kernel's scratch (16 bits) or
-  // the exponent partials and the scratch (float32)
-  uint8_t* ws = static_cast<uint8_t*>(workspace_dev);
-  float* q = reinterpret_cast<float*>(ws);
-  float* part_g = q + (size_t)((n_pix + 127) / 128 * 128) * C;
-  float* part_b = part_g + (size_t)kDgammaGrid * C * C;
-  float* part_e = reinterpret_cast<float*>(ws + tfcb_gdn_backward_workspace_bytes(n_pix, C));
-  float* scratch = dtype == 0 ? reinterpret_cast<float*>(ws + tfcb_gdn_backward_exponents_workspace_bytes(n_pix, C))
-                              : part_b + (size_t)kDgammaGrid * C;
-  int n_parts = 0, n_parts_e = 0;
-  TFCB_TRY(gdn_tc_backward_cf(x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, q, part_g, part_b, scratch,
-                              dalpha_depsilon_dev ? part_e : nullptr, &n_parts, &n_parts_e, n_pix, spatial, C, flags,
-                              alpha, epsilon, dtype, s));
-  reduce_tc_partials(part_g, part_b, n_parts, C, dgamma_dev, dbeta_dev, s);
-  if (dalpha_depsilon_dev) {
-    reduce_partials_kernel<<<1, 32, 0, s>>>(part_e, n_parts_e, 2, dalpha_depsilon_dev);
-    TFCB_LAUNCHED();
-  }
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  if (n_pix == 0) return zero_grads(dgamma_dev, dbeta_dev, dalpha_depsilon_dev, C, s);
+  return backward(r, true, x_dev, gamma_dev, beta_dev, dy_dev, dx_dev, dgamma_dev, dbeta_dev, dalpha_depsilon_dev,
+                  workspace_dev, bwd_workspace(n_pix, C, dtype == 0, true), n_pix, spatial, s);
 }
 
 }  // extern "C"

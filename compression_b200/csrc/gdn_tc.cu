@@ -28,19 +28,22 @@
 // gdn.cu.  At C = 128 / 192 the forward, dx and dgamma kernels also take float16 / bfloat16 activations (IO = 1, 2):
 // each element is widened exactly on load, the arithmetic is the float32 kernels', and the only rounding to 16 bits
 // is the final store, so the result is the float32 result of the widened inputs rounded once.
+//
+// Host side: gdn_tc_route decides which of these kernels take a configuration, and gdn_tc_forward / gdn_tc_backward
+// launch them through with_kernels, the one map from a route and a layout to the kernels' template arguments.  The C
+// entry points, their argument checks and the backward workspace are gdn.cu's.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <algorithm>
 #include <type_traits>
 
-#include "common.cuh"
+#include "gdn_tc.cuh"
 
 namespace tfcb {
 namespace {
 
-constexpr int kTileM = 64;     // pixels per warpgroup tile (wgmma M)
-constexpr int kMaxParts = 148;  // per-CTA dgamma partials the workspace holds (kDgammaGrid, gdn.cu)
+constexpr int kTileM = 64;  // pixels per warpgroup tile (wgmma M)
 
 struct TcFlags {
   int inverse, rectify, alpha_mode, eps_mode;  // alpha_mode: 1 |u|, 2 u^2; eps_mode: 1 identity, 2 sqrt
@@ -1303,19 +1306,6 @@ gdn_tc_pow_wide_dgamma_kernel(const float* __restrict__ x, const float* __restri
   tc_wide_dgamma_body<C, false, CF>(x, q, part_g, part_b, n_pix, f, S);
 }
 
-int sm_count_tc() {
-  int dev = 0, n = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 1;
-}
-
-template <typename Kern>
-int reserve_smem(Kern kernel, int bytes) {
-  TFCB_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-  return TFCB_OK;
-}
-
 // The kernels of a configuration: gdn_tc_* for TcFlags, gdn_tc_pow_* (float32, FAST = false) for TcPowFlags, in the
 // activation layout CF.
 template <int C, bool FAST, int IO, bool CF, class F>
@@ -1356,14 +1346,14 @@ auto wide_dgamma_kernel() {
 
 // The launchers take the layout CF and the channels-first item size S (1 channels-last); grids, partial counts and
 // everything else depend on n_pix only, so both layouts run the same CTAs over the same tiles.
-template <int C, bool FAST, int IO, bool CF = false, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 int launch_tc_fwd(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, F f,
-                  cudaStream_t s, long long S = 1) {
+                  cudaStream_t s, long long S) {
   using K = TcCfg<C>;
   const auto kern = fwd_kernel<C, FAST, IO, CF, F>();
-  TFCB_TRY(reserve_smem(kern, K::kSmem));
+  TFCB_TRY(set_smem(kern, K::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
-  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sm_count_tc());
+  const int grid = (int)std::min<long long>((n_tiles + K::kWG - 1) / K::kWG, sm_count());
   kern<<<grid, K::kThreads, K::kSmem, s>>>(x, gamma, beta, y, n_pix, f, S);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
@@ -1381,17 +1371,17 @@ long long bwd16_scratch_floats(long long n_pix) {
 
 // IO != 0: x, dy, dx in 16 bits.  IO != 0 or CF: `scratch` holds bwd16_scratch_floats<C>(n_pix) floats.
 // TcPowFlags: the dx kernel's CTAs write f.part_e[CTA][2] (when not null), *n_parts_e of them (at most kMaxParts).
-template <int C, bool FAST, int IO, bool CF = false, class F>
+template <int C, bool FAST, int IO, bool CF, class F>
 int launch_tc_bwd(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
                   float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, F f,
-                  cudaStream_t s, int* n_parts_e = nullptr, long long S = 1) {
+                  cudaStream_t s, int* n_parts_e, long long S) {
   using K = TcCfg<C>;
   using L = DgCfg<C>;
   const auto dx_kern = bwd_dx_kernel<C, FAST, IO, CF, F>();
   const auto dg_kern = dgamma_kernel<C, FAST, IO, CF, F>();
-  TFCB_TRY(reserve_smem(dx_kern, K::kSmem));
-  TFCB_TRY(reserve_smem(dg_kern, L::kSmem));
-  const int sms = sm_count_tc();
+  TFCB_TRY(set_smem(dx_kern, K::kSmem));
+  TFCB_TRY(set_smem(dg_kern, L::kSmem));
+  const int sms = sm_count();
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   // dx does not depend on the grid (every tile is computed the same way by whichever CTA takes it)
   const bool capped = IO != 0 || CF || kPow<F>;
@@ -1412,16 +1402,16 @@ int launch_tc_bwd(const void* x, const float* gamma, const float* beta, const vo
 template <int C>
 int wide_grid(long long n_tiles_per_group) {
   using W = WideCfg<C>;
-  const long long groups = std::max(1, std::min(sm_count_tc() / W::kBlocks, kMaxParts));
+  const long long groups = std::max(1, std::min(sm_count() / W::kBlocks, kMaxParts));
   return (int)(std::min<long long>(n_tiles_per_group, groups) * W::kBlocks);
 }
 
-template <int C, bool FAST, bool CF = false, class F>
+template <int C, bool FAST, bool CF, class F>
 int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, F f,
-                       cudaStream_t s, long long S = 1) {
+                       cudaStream_t s, long long S) {
   using W = WideCfg<C>;
   const auto kern = wide_fwd_kernel<C, FAST, CF, F>();
-  TFCB_TRY(reserve_smem(kern, W::kSmem));
+  TFCB_TRY(set_smem(kern, W::kSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
   kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, y, n_pix, f, S);
@@ -1432,17 +1422,17 @@ int launch_tc_wide_fwd(const float* x, const float* gamma, const float* beta, fl
 
 // TcPowFlags: CTA b of pass 1 writes f.part_e[b][1] and CTA b of pass 2 f.part_e[b][0] (when not null), *n_parts_e
 // partials (at most kMaxParts * kBlocks).
-template <int C, bool FAST, bool CF = false, class F>
+template <int C, bool FAST, bool CF, class F>
 int launch_tc_wide_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
                        float* part_g, float* part_b, int* n_parts, long long n_pix, F f, cudaStream_t s,
-                       int* n_parts_e = nullptr, long long S = 1) {
+                       int* n_parts_e, long long S) {
   using W = WideCfg<C>;
   const auto q_kern = wide_bwd_q_kernel<C, FAST, CF, F>();
   const auto dp_kern = wide_bwd_dp_kernel<C, FAST, CF, F>();
   const auto dg_kern = wide_dgamma_kernel<C, FAST, CF, F>();
-  TFCB_TRY(reserve_smem(q_kern, W::kSmem));
-  TFCB_TRY(reserve_smem(dp_kern, W::kSmem));
-  TFCB_TRY(reserve_smem(dg_kern, W::kDgSmem));
+  TFCB_TRY(set_smem(q_kern, W::kSmem));
+  TFCB_TRY(set_smem(dp_kern, W::kSmem));
+  TFCB_TRY(set_smem(dg_kern, W::kDgSmem));
   const long long n_tiles = (n_pix + kTileM - 1) / kTileM;
   const int grid = wide_grid<C>((n_tiles + W::kWG - 1) / W::kWG);
   q_kern<<<grid, W::kThreads, W::kSmem, s>>>(x, gamma, beta, dy, dx, q_ws, n_pix, f, S);
@@ -1459,287 +1449,105 @@ int launch_tc_wide_bwd(const float* x, const float* gamma, const float* beta, co
   return TFCB_OK;
 }
 
-// Which configurations have a tensor-core kernel; fills *f.
-bool tc_config(int C, int flags, float alpha, float eps, TcFlags* f) {
-  if (!(C == 128 || C == 192 || C == 256 || C == 320)) return false;
-  if (!(alpha == 1.f || alpha == 2.f) || !(eps == 1.f || eps == 0.5f)) return false;
-  if (flags & (TFCB_GDN_POW_ALPHA | TFCB_GDN_POW_EPSILON)) return false;  // trainable exponents: literal pow
-  if (const char* env = getenv("TFCB_GDN_FP32")) {
-    if (env[0] == '1') return false;  // debugging aid: force the CUDA-core kernels
+// One instantiation of the kernels: the template arguments with_kernels hands to its function.
+template <int C_, bool FAST_, int IO_, bool CF_>
+struct Inst {
+  static constexpr int C = C_, IO = IO_;
+  static constexpr bool FAST = FAST_, CF = CF_;
+};
+
+// TcPowFlags as gdn.cu's parse_flags fills GdnFlags (part_e null); a fixed-exponent route's TcFlags are its modes.
+TcPowFlags route_flags(const TcRoute& r) {
+  return {(r.flags & TFCB_GDN_INVERSE) ? 1 : 0,
+          (r.flags & TFCB_GDN_RECTIFY) ? 1 : 0,
+          (r.flags & TFCB_GDN_POW_ALPHA) ? 0 : (r.alpha == 1.f ? 1 : (r.alpha == 2.f ? 2 : 0)),
+          (r.flags & TFCB_GDN_POW_EPSILON) ? 0 : (r.eps == 1.f ? 1 : (r.eps == 0.5f ? 2 : 0)),
+          r.alpha,
+          r.eps,
+          nullptr};
+}
+
+template <int C, bool CF, class Fn>
+int with_width(const TcRoute& r, Fn& fn) {
+  const TcPowFlags pf = route_flags(r);
+  if (r.family == TcRoute::kPow) return fn(Inst<C, false, 0, CF>{}, pf);
+  const TcFlags f{pf.inverse, pf.rectify, pf.alpha_mode, pf.eps_mode};
+  auto with_io = [&](auto io) {
+    constexpr int IO = decltype(io)::value;
+    return r.fast ? fn(Inst<C, true, IO, CF>{}, f) : fn(Inst<C, false, IO, CF>{}, f);
+  };
+  if constexpr (C <= 192) {
+    if (r.dtype == 1) return with_io(std::integral_constant<int, 1>{});
+    if (r.dtype == 2) return with_io(std::integral_constant<int, 2>{});
   }
-  f->inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
-  f->rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
-  f->alpha_mode = (alpha == 2.f) ? 2 : 1;
-  f->eps_mode = (eps == 0.5f) ? 2 : 1;
-  return true;
+  return with_io(std::integral_constant<int, 0>{});
 }
 
-bool tc_fast(const TcFlags& f) { return f.alpha_mode == 1 && f.eps_mode == 1 && !f.rectify; }
-
-// The configurations of the four widths that tc_config leaves out (a trainable exponent, or a fixed one outside
-// {1, 2} / {1, 1/2}) run the literal-pow kernels; fills *f as gdn.cu's parse_flags does, part_e null.
-bool tc_pow_config(int C, int flags, float alpha, float eps, TcPowFlags* f) {
-  if (!(C == 128 || C == 192 || C == 256 || C == 320)) return false;
-  if (const char* env = getenv("TFCB_GDN_FP32")) {
-    if (env[0] == '1') return false;
-  }
-  TcFlags fixed;
-  if (tc_config(C, flags, alpha, eps, &fixed)) return false;
-  f->inverse = (flags & TFCB_GDN_INVERSE) ? 1 : 0;
-  f->rectify = (flags & TFCB_GDN_RECTIFY) ? 1 : 0;
-  f->alpha_mode = (flags & TFCB_GDN_POW_ALPHA) ? 0 : (alpha == 1.f ? 1 : (alpha == 2.f ? 2 : 0));
-  f->eps_mode = (flags & TFCB_GDN_POW_EPSILON) ? 0 : (eps == 1.f ? 1 : (eps == 0.5f ? 2 : 0));
-  f->alpha = alpha;
-  f->eps = eps;
-  f->part_e = nullptr;
-  return true;
-}
-
-bool misaligned(const void* a, const void* b, const void* c) {
-  return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) != 0;
-}
-
-template <bool CF = false>
-int launch_pow_fwd(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
-                   const TcPowFlags& f, cudaStream_t s, long long S = 1) {
-  if (C == 128) return launch_tc_fwd<128, false, 0, CF>(x, gamma, beta, y, n_pix, f, s, S);
-  if (C == 192) return launch_tc_fwd<192, false, 0, CF>(x, gamma, beta, y, n_pix, f, s, S);
-  if (C == 256) return launch_tc_wide_fwd<256, false, CF>(x, gamma, beta, y, n_pix, f, s, S);
-  return launch_tc_wide_fwd<320, false, CF>(x, gamma, beta, y, n_pix, f, s, S);
-}
-
-// CF: `scratch` as launch_tc_bwd takes it at C = 128 / 192.
-template <bool CF = false>
-int launch_pow_bwd(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                   float* part_g, float* part_b, int* n_parts, int* n_parts_e, long long n_pix, int C,
-                   const TcPowFlags& f, cudaStream_t s, long long S = 1, float* scratch = nullptr) {
-  if (C == 128)
-    return launch_tc_bwd<128, false, 0, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f,
-                                            s, n_parts_e, S);
-  if (C == 192)
-    return launch_tc_bwd<192, false, 0, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f,
-                                            s, n_parts_e, S);
-  if (C == 256)
-    return launch_tc_wide_bwd<256, false, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
-                                              n_parts_e, S);
-  return launch_tc_wide_bwd<320, false, CF>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s,
-                                            n_parts_e, S);
+// The one map from a route and a layout to the kernels: fn(Inst<C, FAST, IO, CF>{}, flags), flags TcFlags or
+// TcPowFlags.  What it instantiates is the kernel set: at C = 128 / 192 the fixed-exponent kernels for FAST x IO and
+// the literal-pow ones for IO = 0; at C = 256 / 320 both families for IO = 0; each in both layouts.
+template <class Fn>
+int with_kernels(const TcRoute& r, bool channels_first, Fn fn) {
+  auto with_layout = [&](auto cf) {
+    constexpr bool CF = decltype(cf)::value;
+    switch (r.C) {
+      case 128: return with_width<128, CF>(r, fn);
+      case 192: return with_width<192, CF>(r, fn);
+      case 256: return with_width<256, CF>(r, fn);
+      default: return with_width<320, CF>(r, fn);
+    }
+  };
+  return channels_first ? with_layout(std::true_type{}) : with_layout(std::false_type{});
 }
 
 }  // namespace
 
-int gdn_tc_forward(const float* x, const float* gamma, const float* beta, float* y, long long n_pix, int C,
-                   int flags, float alpha, float eps, cudaStream_t s, bool* handled) {
-  *handled = false;
-  TcPowFlags pf;
-  if (!misaligned(x, y, beta) && tc_pow_config(C, flags, alpha, eps, &pf)) {
-    *handled = true;
-    return launch_pow_fwd(x, gamma, beta, y, n_pix, C, pf, s);
-  }
-  TcFlags f;
-  if (misaligned(x, y, beta) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
-  *handled = true;
-  const bool fast = tc_fast(f);
-  if (C == 256)
-    return fast ? launch_tc_wide_fwd<256, true>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_wide_fwd<256, false>(x, gamma, beta, y, n_pix, f, s);
-  if (C == 320)
-    return fast ? launch_tc_wide_fwd<320, true>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_wide_fwd<320, false>(x, gamma, beta, y, n_pix, f, s);
-  if (C == 128)
-    return fast ? launch_tc_fwd<128, true, 0>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_fwd<128, false, 0>(x, gamma, beta, y, n_pix, f, s);
-  return fast ? launch_tc_fwd<192, true, 0>(x, gamma, beta, y, n_pix, f, s)
-              : launch_tc_fwd<192, false, 0>(x, gamma, beta, y, n_pix, f, s);
+TcRoute gdn_tc_route(int C, int dtype, int flags, float alpha, float eps) {
+  TcRoute r{TcRoute::kNone, false, C, dtype, flags, alpha, eps};
+  const char* env = getenv("TFCB_GDN_FP32");  // debugging aid: force the CUDA-core kernels
+  if ((env && env[0] == '1') || !(C == 128 || C == 192 || C == 256 || C == 320)) return r;
+  const TcPowFlags f = route_flags(r);
+  const bool pow = f.alpha_mode == 0 || f.eps_mode == 0;
+  if (dtype != 0 && (pow || C > 192 || (dtype != 1 && dtype != 2))) return r;
+  r.family = pow ? TcRoute::kPow : TcRoute::kFixed;
+  r.fast = f.alpha_mode == 1 && f.eps_mode == 1 && !f.rectify;
+  return r;
 }
 
-// 16-bit activations (float16 / bfloat16 in, same type out; parameters and arithmetic float32): the C = 128 / 192
-// kernels reading and writing the 16-bit elements themselves.  *handled = false -> the caller reports the
-// configuration.
-int gdn_tc_forward16(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, int C, int flags,
-                     float alpha, float eps, int dtype, cudaStream_t s, bool* handled) {
-  *handled = false;
-  TcFlags f;
-  if ((C != 128 && C != 192) || (dtype != 1 && dtype != 2) || misaligned(x, y, beta) ||
-      !tc_config(C, flags, alpha, eps, &f))
-    return TFCB_OK;
-  *handled = true;
-  const bool fast = tc_fast(f);
-  if (C == 128) {
-    if (dtype == 1)
-      return fast ? launch_tc_fwd<128, true, 1>(x, gamma, beta, y, n_pix, f, s)
-                  : launch_tc_fwd<128, false, 1>(x, gamma, beta, y, n_pix, f, s);
-    return fast ? launch_tc_fwd<128, true, 2>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_fwd<128, false, 2>(x, gamma, beta, y, n_pix, f, s);
-  }
-  if (dtype == 1)
-    return fast ? launch_tc_fwd<192, true, 1>(x, gamma, beta, y, n_pix, f, s)
-                : launch_tc_fwd<192, false, 1>(x, gamma, beta, y, n_pix, f, s);
-  return fast ? launch_tc_fwd<192, true, 2>(x, gamma, beta, y, n_pix, f, s)
-              : launch_tc_fwd<192, false, 2>(x, gamma, beta, y, n_pix, f, s);
+int gdn_tc_forward(const TcRoute& r, bool channels_first, const void* x, const float* gamma, const float* beta, void* y,
+                   long long n_pix, long long S, cudaStream_t s) {
+  return with_kernels(r, channels_first, [&](auto k, auto f) {
+    using K = decltype(k);
+    if constexpr (K::C > 192) {
+      static_assert(K::IO == 0, "the wide kernels take float32 activations only");
+      return launch_tc_wide_fwd<K::C, K::FAST, K::CF>(static_cast<const float*>(x), gamma, beta, static_cast<float*>(y),
+                                                       n_pix, f, s, S);
+    } else {
+      return launch_tc_fwd<K::C, K::FAST, K::IO, K::CF>(x, gamma, beta, y, n_pix, f, s, S);
+    }
+  });
 }
 
-long long gdn_tc_backward16_scratch_floats(long long n_pix, int C) {
+int gdn_tc_backward(const TcRoute& r, bool channels_first, const void* x, const float* gamma, const float* beta,
+                    const void* dy, void* dx, float* q, float* part_g, float* part_b, float* part_e, float* scratch,
+                    long long n_pix, long long S, cudaStream_t s, int* n_parts, int* n_parts_e) {
+  return with_kernels(r, channels_first, [&](auto k, auto f) {
+    using K = decltype(k);
+    if constexpr (kPow<decltype(f)>) f.part_e = part_e;
+    if constexpr (K::C > 192)
+      return launch_tc_wide_bwd<K::C, K::FAST, K::CF>(static_cast<const float*>(x), gamma, beta,
+                                                       static_cast<const float*>(dy), static_cast<float*>(dx), q,
+                                                       part_g, part_b, n_parts, n_pix, f, s, n_parts_e, S);
+    else
+      return launch_tc_bwd<K::C, K::FAST, K::IO, K::CF>(x, gamma, beta, dy, dx, q, part_g, part_b, scratch, n_parts,
+                                                         n_pix, f, s, n_parts_e, S);
+  });
+}
+
+long long gdn_tc_scratch_floats(long long n_pix, int C) {
   if (C == 128) return bwd16_scratch_floats<128>(n_pix);
   if (C == 192) return bwd16_scratch_floats<192>(n_pix);
   return 0;
-}
-
-// 16-bit backward: x, dy, dx in float16 / bfloat16; q, the partials and `scratch`
-// (gdn_tc_backward16_scratch_floats(n_pix, C) floats) as in gdn_tc_backward.  dx is the float32 backward's dx of the
-// widened inputs rounded once; q and the partials are the float32 backward's, bit for bit.  *handled = false -> the
-// caller reports the configuration.
-int gdn_tc_backward16(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
-                      float* part_g, float* part_b, float* scratch, int* n_parts, long long n_pix, int C, int flags,
-                      float alpha, float eps, int dtype, cudaStream_t s, bool* handled) {
-  *handled = false;
-  TcFlags f;
-  if ((C != 128 && C != 192) || (dtype != 1 && dtype != 2) || misaligned(x, dy, dx) ||
-      misaligned(q_ws, beta, scratch) || !tc_config(C, flags, alpha, eps, &f))
-    return TFCB_OK;
-  *handled = true;
-#define TFCB_BWD16(C_, FAST_, IO_) \
-  launch_tc_bwd<C_, FAST_, IO_>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, scratch, n_parts, n_pix, f, s)
-  const bool fast = tc_fast(f);
-  if (C == 128) {
-    if (dtype == 1) return fast ? TFCB_BWD16(128, true, 1) : TFCB_BWD16(128, false, 1);
-    return fast ? TFCB_BWD16(128, true, 2) : TFCB_BWD16(128, false, 2);
-  }
-  if (dtype == 1) return fast ? TFCB_BWD16(192, true, 1) : TFCB_BWD16(192, false, 1);
-  return fast ? TFCB_BWD16(192, true, 2) : TFCB_BWD16(192, false, 2);
-#undef TFCB_BWD16
-}
-
-// Tensor-core backward: dx, q (workspace) and the per-CTA partial sums (part_g [n_parts][C][C], part_b [n_parts][C])
-// that the caller reduces.  *handled = false -> the caller runs the fp32 kernels.
-int gdn_tc_backward(const float* x, const float* gamma, const float* beta, const float* dy, float* dx, float* q_ws,
-                    float* part_g, float* part_b, int* n_parts, long long n_pix, int C, int flags, float alpha,
-                    float eps, cudaStream_t s, bool* handled) {
-  *handled = false;
-  TcPowFlags pf;
-  if (!misaligned(x, dy, dx) && !misaligned(q_ws, beta, nullptr) && tc_pow_config(C, flags, alpha, eps, &pf)) {
-    *handled = true;
-    int n_parts_e = 0;
-    return launch_pow_bwd(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, &n_parts_e, n_pix, C, pf, s);
-  }
-  TcFlags f;
-  if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_config(C, flags, alpha, eps, &f)) return TFCB_OK;
-  *handled = true;
-  const bool fast = tc_fast(f);
-  if (C == 256)
-    return fast ? launch_tc_wide_bwd<256, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
-                : launch_tc_wide_bwd<256, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
-  if (C == 320)
-    return fast ? launch_tc_wide_bwd<320, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s)
-                : launch_tc_wide_bwd<320, false>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_pix, f, s);
-  if (C == 128)
-    return fast ? launch_tc_bwd<128, true, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s)
-                : launch_tc_bwd<128, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f,
-                                               s);
-  return fast ? launch_tc_bwd<192, true, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s)
-              : launch_tc_bwd<192, false, 0>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, nullptr, n_parts, n_pix, f, s);
-}
-
-// gdn_tc_backward with dL/dalpha and dL/depsilon fused in, for the literal-pow configurations: part_e receives
-// *n_parts_e partials [2] (at most kMaxParts * 5), reduced by the caller.  *handled = false (every other
-// configuration) -> the caller runs the fp32 kernels and the exponent kernel.
-int gdn_tc_backward_exponents(const float* x, const float* gamma, const float* beta, const float* dy, float* dx,
-                              float* q_ws, float* part_g, float* part_b, float* part_e, int* n_parts, int* n_parts_e,
-                              long long n_pix, int C, int flags, float alpha, float eps, cudaStream_t s,
-                              bool* handled) {
-  *handled = false;
-  TcPowFlags pf;
-  if (misaligned(x, dy, dx) || misaligned(q_ws, beta, nullptr) || !tc_pow_config(C, flags, alpha, eps, &pf))
-    return TFCB_OK;
-  *handled = true;
-  pf.part_e = part_e;
-  return launch_pow_bwd(x, gamma, beta, dy, dx, q_ws, part_g, part_b, n_parts, n_parts_e, n_pix, C, pf, s);
-}
-
-// ---- Channels-first activations: x, y, dy, dx [n_pix / S, C, S] ----
-//
-// Covered exactly where the channels-last tensor-core kernels run: float32 (dtype 0) at C in {128, 192, 256, 320}
-// with any exponents (*pow: on the literal-pow kernels), float16 / bfloat16 (dtype 1, 2) at C = 128 / 192 with the
-// fixed exponents' shortcuts; nothing under TFCB_GDN_FP32=1.  The caller checks this before any device work.
-bool gdn_tc_cf_config(int C, int dtype, int flags, float alpha, float eps, bool* pow) {
-  TcPowFlags pf;
-  TcFlags f;
-  *pow = dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf);
-  if (*pow) return true;
-  if (dtype != 0 && !((dtype == 1 || dtype == 2) && (C == 128 || C == 192))) return false;
-  return tc_config(C, flags, alpha, eps, &f);
-}
-
-// A configuration gdn_tc_cf_config accepts, n_pix > 0.  The kernels and grids of the channels-last entries with the
-// channels-first accesses: y is, bit for bit, what they write for the transposed x.
-int gdn_tc_forward_cf(const void* x, const float* gamma, const float* beta, void* y, long long n_pix, long long S,
-                      int C, int flags, float alpha, float eps, int dtype, cudaStream_t s) {
-  const float* xf = static_cast<const float*>(x);
-  float* yf = static_cast<float*>(y);
-  TcPowFlags pf;
-  if (dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf))
-    return launch_pow_fwd<true>(xf, gamma, beta, yf, n_pix, C, pf, s, S);
-  TcFlags f;
-  if (!tc_config(C, flags, alpha, eps, &f))
-    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for this configuration");
-  const bool fast = tc_fast(f);
-#define TFCB_FWD_CF(C_, IO_)                                                 \
-  (fast ? launch_tc_fwd<C_, true, IO_, true>(x, gamma, beta, y, n_pix, f, s, S) \
-        : launch_tc_fwd<C_, false, IO_, true>(x, gamma, beta, y, n_pix, f, s, S))
-  if (dtype == 0) {
-    if (C == 256)
-      return fast ? launch_tc_wide_fwd<256, true, true>(xf, gamma, beta, yf, n_pix, f, s, S)
-                  : launch_tc_wide_fwd<256, false, true>(xf, gamma, beta, yf, n_pix, f, s, S);
-    if (C == 320)
-      return fast ? launch_tc_wide_fwd<320, true, true>(xf, gamma, beta, yf, n_pix, f, s, S)
-                  : launch_tc_wide_fwd<320, false, true>(xf, gamma, beta, yf, n_pix, f, s, S);
-    return C == 128 ? TFCB_FWD_CF(128, 0) : TFCB_FWD_CF(192, 0);
-  }
-  if (C == 128) return dtype == 1 ? TFCB_FWD_CF(128, 1) : TFCB_FWD_CF(128, 2);
-  return dtype == 1 ? TFCB_FWD_CF(192, 1) : TFCB_FWD_CF(192, 2);
-#undef TFCB_FWD_CF
-}
-
-// dx, q and the partials as gdn_tc_backward (float32) / gdn_tc_backward16 (16-bit) write them, for channels-first x,
-// dy, dx; at C = 128 / 192 `scratch` holds gdn_tc_backward16_scratch_floats(n_pix, C) floats in either type.  On the
-// literal-pow kernels part_e, when not null, receives the exponent partials as gdn_tc_backward_exponents writes them
-// (*n_parts_e).
-int gdn_tc_backward_cf(const void* x, const float* gamma, const float* beta, const void* dy, void* dx, float* q_ws,
-                       float* part_g, float* part_b, float* scratch, float* part_e, int* n_parts, int* n_parts_e,
-                       long long n_pix, long long S, int C, int flags, float alpha, float eps, int dtype,
-                       cudaStream_t s) {
-  const float* xf = static_cast<const float*>(x);
-  const float* dyf = static_cast<const float*>(dy);
-  float* dxf = static_cast<float*>(dx);
-  TcPowFlags pf;
-  if (dtype == 0 && tc_pow_config(C, flags, alpha, eps, &pf)) {
-    pf.part_e = part_e;
-    return launch_pow_bwd<true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_parts_e, n_pix, C, pf, s,
-                                S, scratch);
-  }
-  TcFlags f;
-  if (!tc_config(C, flags, alpha, eps, &f))
-    return fail(TFCB_INVALID_ARGUMENT, "GDN channels-first: no kernel for this configuration");
-  const bool fast = tc_fast(f);
-#define TFCB_BWD_CF(C_, IO_, SCRATCH_)                                                                              \
-  (fast ? launch_tc_bwd<C_, true, IO_, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, SCRATCH_, n_parts, n_pix, \
-                                             f, s, nullptr, S)                                                     \
-        : launch_tc_bwd<C_, false, IO_, true>(x, gamma, beta, dy, dx, q_ws, part_g, part_b, SCRATCH_, n_parts,      \
-                                              n_pix, f, s, nullptr, S))
-#define TFCB_WIDE_BWD_CF(C_)                                                                                         \
-  (fast ? launch_tc_wide_bwd<C_, true, true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_pix, f, s, \
-                                             nullptr, S)                                                            \
-        : launch_tc_wide_bwd<C_, false, true>(xf, gamma, beta, dyf, dxf, q_ws, part_g, part_b, n_parts, n_pix, f, s, \
-                                              nullptr, S))
-  if (dtype == 0) {
-    if (C == 256) return TFCB_WIDE_BWD_CF(256);
-    if (C == 320) return TFCB_WIDE_BWD_CF(320);
-    return C == 128 ? TFCB_BWD_CF(128, 0, scratch) : TFCB_BWD_CF(192, 0, scratch);
-  }
-  if (C == 128) return dtype == 1 ? TFCB_BWD_CF(128, 1, scratch) : TFCB_BWD_CF(128, 2, scratch);
-  return dtype == 1 ? TFCB_BWD_CF(192, 1, scratch) : TFCB_BWD_CF(192, 2, scratch);
-#undef TFCB_BWD_CF
-#undef TFCB_WIDE_BWD_CF
 }
 
 }  // namespace tfcb
