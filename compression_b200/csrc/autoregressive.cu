@@ -21,6 +21,7 @@
 //   in increasing k starting from 0.f, where K is the layer's input width.
 #include <cuda_runtime.h>
 
+#include "autoregressive.cuh"
 #include "common.cuh"
 #include "range_decoder.cuh"
 
@@ -28,35 +29,8 @@ namespace tfcb {
 namespace {
 
 constexpr int kArThreads = 512;
-constexpr int kArSlices = 8;      // input slices per dense output (the fixed reduction order above)
-constexpr int kArTaps = 12;       // causal taps of a 5x5 type-A mask
-constexpr int kArMaxM = 384;
-constexpr float kArLeakySlope = 0.01f;
 
 enum : int { kArParams = 0, kArEncode = 1, kArDecode = 2 };
-
-struct ArDims {
-  int M, N2, N3, N4;
-  long long wc, bc, w1, b1, w2, b2, w3, b3, total;  // offsets into the packed buffer, in floats
-};
-
-__host__ __device__ inline ArDims ar_dims(int M) {
-  ArDims d;
-  d.M = M;
-  d.N2 = 2 * M;
-  d.N3 = 10 * M / 3;
-  d.N4 = 8 * M / 3;
-  d.wc = 0;
-  d.bc = d.wc + (long long)kArTaps * M * d.N2;
-  d.w1 = d.bc + d.N2;
-  d.b1 = d.w1 + 4ll * M * d.N3;
-  d.w2 = d.b1 + d.N3;
-  d.b2 = d.w2 + (long long)d.N3 * d.N4;
-  d.w3 = d.b2 + d.N4;
-  d.b3 = d.w3 + (long long)d.N4 * d.N2;
-  d.total = d.b3 + d.N2;
-  return d;
-}
 
 // floats of shared memory for activations: gathered taps, [ψ, ctx], h1, h2, out, and the slice partials
 __host__ __device__ inline long long ar_act_floats(const ArDims& d) {
@@ -106,14 +80,6 @@ __device__ __forceinline__ void ar_dense(const float* in, int nin, const float* 
     out[j] = v;
   }
   __syncthreads();
-}
-
-// ContinuousIndexedEntropyModel._normalize_indexes (maximum with 0, minimum with num_scales - 1, both NaN-
-// propagating like torch.maximum / minimum) followed by .to(torch.int32) on the GPU (truncation; NaN -> 0).
-__device__ __forceinline__ int32_t ar_table_index(float s, int num_scales) {
-  float v = (s != s) ? s : fmaxf(s, 0.f);
-  v = (v != v) ? v : fminf(v, (float)(num_scales - 1));
-  return (int32_t)v;
 }
 
 template <int MODE, bool SMEM_KEYS>
@@ -251,28 +217,6 @@ __global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
     st.pos = c.pos2 >> 1;
     P.state[b] = st;
   }
-}
-
-int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64_t H, int64_t W, int num_scales) {
-  if (M <= 0 || M % 6 != 0 || M > kArMaxM)
-    return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be a positive multiple of 6 and at most %d", M,
-                kArMaxM);
-  if (!packed) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
-  if (packed_floats != ar_dims(M).total)
-    return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, M=%d needs %lld", (long long)packed_floats,
-                M, (long long)ar_dims(M).total);
-  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
-  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
-    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
-  if (num_scales < 1) return fail(TFCB_INVALID_ARGUMENT, "num_scales=%d must be positive", num_scales);
-  return TFCB_OK;
-}
-
-int ar_check_range(int64_t p0, int64_t p1, int64_t H, int64_t W) {
-  if (p0 < 0 || p1 < p0 || p1 > H * W)
-    return fail(TFCB_INVALID_ARGUMENT, "positions [%lld, %lld) outside [0, %lld)", (long long)p0, (long long)p1,
-                (long long)(H * W));
-  return TFCB_OK;
 }
 
 template <int MODE, bool SMEM_KEYS>

@@ -814,7 +814,12 @@ def ar_pack_weights(ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
   """The device layout the parameter kernel reads: the context kernel [5, 5, M, 2M] (masked or not: only its 12
   causal taps are read), then each 1x1 layer as [inputs, outputs] and its bias.  Returns float32 [packed floats] on
   the context kernel's device; the values are copied unchanged."""
-  ctx_kernel = ctx_kernel.detach()
+  return _pack_weights(ctx_kernel.detach(), None, ctx_bias, w1, b1, w2, b2, w3, b3)
+
+
+def _pack_weights(ctx_kernel, taps, ctx_bias, w1, b1, w2, b2, w3, b3):
+  """tfcb_ar_pack_weights of a [5, 5, M, 2M] context kernel, whose first 12 * M * 2M floats the library reads:
+  unchanged (`taps` None) or its taps [(dy + 2, dx + 2), ...] gathered into a contiguous [12, M, 2M]."""
   if ctx_kernel.dim() != 4 or ctx_kernel.shape[:2] != (5, 5) or ctx_kernel.shape[3] != 2 * ctx_kernel.shape[2]:
     raise _lib.InvalidArgumentError(f"context kernel must be [5, 5, M, 2M]: {tuple(ctx_kernel.shape)}")
   M = int(ctx_kernel.shape[2])
@@ -825,6 +830,8 @@ def ar_pack_weights(ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
     raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
   want = ((ctx_bias, (2 * M,)), (w1, (4 * M, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, 2 * M)),
           (b3, (2 * M,)))
+  if taps is not None:
+    ctx_kernel = ctx_kernel[[y for y, _ in taps], [x for _, x in taps]]
   ops = [_f32(ctx_kernel, dev)]
   for t, shape in want:
     t = t.detach()
@@ -940,4 +947,92 @@ def ar_decode_naive(handle, packed, psi, num_scales, cdf_offset):
   for p in range(H * W):
     loc, _, index = ar_params(packed, y_hat, psi, p, num_scales)
     flat[:, p] = decode_index_f32(handle, index, loc, coff)
+  return y_hat
+
+
+# ------------------------------------------------------------------------------------------------
+# Checkerboard context model (He et al. 2021): two parameter passes over the positions of one colour (tfcb_cb_*) on
+# the packed network of ar_pack_weights.  Anchors are the positions (r, c) with r + c even; coding order is the
+# anchors in raster order, then the non-anchors in raster order.  Latents are float32 CUDA [B, H, W, M], psi
+# [B, H, W, 2M]; coding-order tensors are [B, n, M] for one colour and [B, H * W, M] for both.
+# ------------------------------------------------------------------------------------------------
+CB_TAPS = tuple((dy, dx) for dy in range(-2, 3) for dx in range(-2, 3) if (dy + dx) % 2)  # raster order, 12 taps
+
+
+def cb_pack_weights(ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
+  """ar_pack_weights for the checkerboard parameter passes: the 12 checkerboard taps of the context kernel
+  [5, 5, M, 2M] (masked or not: no other tap is read) are packed in raster order where ar_pack_weights puts the
+  causal ones."""
+  return _pack_weights(ctx_kernel.detach(), [(dy + 2, dx + 2) for dy, dx in CB_TAPS], ctx_bias, w1, b1, w2, b2, w3,
+                       b3)
+
+
+def cb_counts(H, W):
+  """(anchors, non-anchors) of an H x W latent: (ceil(H W / 2), floor(H W / 2))."""
+  return (H * W + 1) // 2, H * W // 2
+
+
+def _cb_pass(packed, y_hat, psi, anchors, num_scales, whole, loc, scale, index, y=None, y_cb=None, y_hat_out=None):
+  B, H, W, M, n = _ar_dims(packed, psi)
+  dev = packed.device
+  lib = _lib.lib()
+  nw = int(lib.tfcb_cb_workspace_floats(M, B, H, W, int(bool(anchors))))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
+  check(lib.tfcb_cb_params(_p(packed), n, M, _p(y_hat), _p(psi), B, H, W, int(bool(anchors)), int(num_scales),
+                           _p(work), nw, int(whole), _p(loc), _p(scale), _p(index), _p(y), _p(y_cb), _p(y_hat_out),
+                           _stream()))
+
+
+def cb_params(packed, y_hat, psi, anchors, num_scales):
+  """One parameter pass: (loc, scale_index, index) [B, n, M] (float32, float32, int32) of the n positions of one
+  colour of every image, in coding order.  The non-anchor pass reads the anchors of y_hat [B, H, W, M]; the anchor
+  pass reads no latent (y_hat may be None).  Row b depends only on image b."""
+  B, H, W, M, _ = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  if y_hat is not None or not anchors:
+    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  n = cb_counts(H, W)[0 if anchors else 1]
+  loc = torch.empty((B, n, M), dtype=torch.float32, device=dev)
+  scale = torch.empty_like(loc)
+  index = torch.empty((B, n, M), dtype=torch.int32, device=dev)
+  _cb_pass(packed, y_hat, psi, anchors, num_scales, False, loc, scale, index)
+  return loc, scale, index
+
+
+def cb_encode(packed, y, psi, num_scales, scale_index=False):
+  """The two-pass encoder: returns y_hat [B, H, W, M] and y, loc, index in coding order [B, H * W, M] (and
+  scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc, the anchors' before the
+  non-anchor pass reads them.  The strings are one index-mode encode of the coding-order y with index and loc."""
+  B, H, W, M, _ = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
+  y_cb, loc = (torch.empty((B, H * W, M), dtype=torch.float32, device=dev) for _ in range(2))
+  index = torch.empty((B, H * W, M), dtype=torch.int32, device=dev)
+  scale = torch.empty_like(loc) if scale_index else None
+  for anchors in (True, False):
+    _cb_pass(packed, y_hat, psi, anchors, num_scales, True, loc, scale, index, y, y_cb, y_hat)
+  return (y_hat, y_cb, loc, index) + ((scale,) if scale_index else ())
+
+
+def cb_decode(handle, packed, psi, num_scales, cdf_offset):
+  """The two-pass decoder, continuing `handle` (a DecoderHandle of B index-mode strings in coding order): anchor
+  parameters, decode_index_f32 of the anchors, their latents to [B, H, W, M], non-anchor parameters, decode of the
+  non-anchors, to [B, H, W, M].  Returns y_hat [B, H, W, M].  A fixed number of library launches whatever B, H and W
+  (fewer at H W = 1, where the non-anchor pass is empty) and no host synchronisation; stream errors surface at
+  entropy_decode_finalize."""
+  B, H, W, M, _ = _ar_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  if handle.n_streams != B:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a batch of {B}")
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for anchors in (True, False):
+    loc, _, index = cb_params(packed, y_hat, psi, anchors, num_scales)
+    part = decode_index_f32(handle, index, loc, coff)
+    check(lib.tfcb_cb_scatter(_p(part), B, H, W, M, int(anchors), _p(y_hat), _stream()))
   return y_hat

@@ -28,7 +28,7 @@ from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -672,9 +672,12 @@ class MBT2018Model(_Model):
   def entropy_parameters_of(self, y_ctx, psi):
     """The parallel (training) form of the parameter network: (loc, scale_index) of every position from the latents
     the context model sees and psi."""
-    ctx = self.context_model(y_ctx)
+    ctx = self._context(y_ctx)
     params = self.entropy_parameters(torch.cat([psi, ctx], dim=-1))
     return params[..., :self.latent_depth], params[..., self.latent_depth:]
+
+  def _context(self, y_ctx):
+    return self.context_model(y_ctx)
 
   def forward(self, x, training=True):
     """-> (loss, bpp, mse).  The context model sees y plus uniform noise when training, round(y) otherwise."""
@@ -703,8 +706,10 @@ class MBT2018Model(_Model):
     if any(not layer.built for layer in layers):
       raise RuntimeError("the entropy-parameter layers are not built: call build() first")
     w = [t for layer in layers for t in (layer.kernel.reshape(layer.kernel.shape[-2:]), layer.bias)]
-    self._packed = F.ar_pack_weights(self.context_model.kernel, self.context_model.bias, *w)
+    self._packed = self._pack_weights(self.context_model.kernel, self.context_model.bias, *w)
     return self
+
+  _pack_weights = staticmethod(F.ar_pack_weights)
 
   # -- coding: one latent shape per call --
   def _encode_latents(self, y, psi):
@@ -799,6 +804,69 @@ class MBT2018Model(_Model):
   def decompress_from_tfci(self, data):
     dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
     return self.decompress(*PackedTensors(data).unpack(dtypes))
+
+
+def checkerboard_mask(kernel_size=5):
+  """[k, k]: 1 at the offsets (dy, dx) from the centre with dy + dx odd (12 for k = 5), 0 elsewhere.  Centred on a
+  non-anchor, every such tap is an anchor."""
+  r = torch.arange(kernel_size)
+  return ((r[:, None] + r[None, :]) % 2 == 1).to(torch.float32)
+
+
+def anchor_mask(H, W, device=None, dtype=torch.float32):
+  """[1, H, W, 1]: 1 at the anchors (r + c even), 0 at the non-anchors."""
+  r, c = torch.arange(H, device=device), torch.arange(W, device=device)
+  return ((r[:, None] + c[None, :]) % 2 == 0).to(dtype)[None, :, :, None]
+
+
+class CheckerboardConv2D(MaskedConv2D):
+  """MaskedConv2D with the checkerboard mask: 12 taps of odd parity around the centre."""
+
+  def __init__(self, in_channels, filters):
+    super().__init__(in_channels, filters)
+    self.mask.copy_(checkerboard_mask(5)[:, :, None, None])
+
+
+def checkerboard_context(context_model, y):
+  """The context feature of the training path: nonanchor * context_model(anchor * y).  Anchors get 0 (bias
+  included); a non-anchor gets its context model's output over the anchors around it."""
+  a = anchor_mask(y.shape[1], y.shape[2], y.device, y.dtype)
+  return (1 - a) * context_model(a * y)
+
+
+class CheckerboardModel(MBT2018Model):
+  """MBT2018Model with the checkerboard context model of He, Zheng, Sun, Wang & Qin (CVPR 2021): the same
+  transforms, hyper prior, widths and entropy models; the 5x5 context model sees only the anchors (positions with
+  r + c even), and anchors take a context feature of zero.  So coding is two passes in which every position is
+  independent: the anchors' parameters from psi alone, then the non-anchors' from psi and the decoded anchors.
+
+  Coding runs on the parameter passes (functional.cb_*): the strings are one index-mode encode of y in coding order
+  (each image's anchors in raster order, then its non-anchors), the bytes of
+  `LocationScaleIndexedEntropyModel.compress(y_cb, scale_index_cb, loc_cb)` of the coding-order tensors; the decoder
+  makes two decode_index_f32 calls on one decoder handle."""
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.):
+    super().__init__(lmbda, num_filters, latent_depth, num_scales, scale_min, scale_max)
+    self.context_model = CheckerboardConv2D(self.latent_depth, 2 * self.latent_depth)
+
+  def _context(self, y_ctx):
+    return checkerboard_context(self.context_model, y_ctx)
+
+  _pack_weights = staticmethod(F.cb_pack_weights)
+
+  def _encode_latents(self, y, psi):
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H * W, M]."""
+    em = self.entropy_model
+    y_hat, y_cb, loc, index = F.cb_encode(self._packed, y.contiguous(), psi, self.num_scales)
+    strings = F.compress_f32((y.shape[0],), em._lookup_host(), y_cb, loc, em.cdf_offset.to(y.device), index=index)
+    return strings, y_hat, loc, index
+
+  def _decode_latents(self, strings, psi):
+    em = self.entropy_model
+    handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
+    y_hat = F.cb_decode(handle, self._packed, psi, self.num_scales, em.cdf_offset.to(psi.device))
+    em._finish_decode(handle)
+    return y_hat
 
 
 # ------------------------------------------------------------------------------------------------

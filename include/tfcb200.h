@@ -256,6 +256,33 @@ int tfcb_ar_decode(tfcb_decoder* h, const float* packed_dev, int64_t packed_floa
                    const int32_t* cdf_offset_dev, float* yhat_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Checkerboard context model (He et al. 2021) on the same packed parameters.  A latent position (r, c) is an
+ * anchor when r + c is even, else a non-anchor; an image has ceil(H W / 2) anchors.  Coding order: the anchors in
+ * raster order, then the non-anchors in raster order, M channels per position.  Anchors take ctx = 0 (bias
+ * included); a non-anchor takes ctx = Wc * taps + bc over the 12 taps (dy, dx) in [-2, 2]^2 with dy + dx odd, in
+ * raster order, zeros outside the image.  The packed Wc is those 12 taps [12, M, 2M]: pack them with
+ * tfcb_ar_pack_weights, which reads the first 12 M 2M floats of its context-kernel operand.  The rest of the
+ * network and its float32 order of operations are tfcb_ar_params'.
+ * ---------------------------------------------------------------------------------------------- */
+/* Floats of workspace one tfcb_cb_params pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_cb_workspace_floats(int M, int64_t B, int64_t H, int64_t W, int anchors);
+/* One pass over every position of one colour (anchors != 0: the anchors) of all B images.  The non-anchor pass
+ * reads the anchors' decoded latents from `yhat_dev` [B, H, W, M] (NULL is allowed for the anchor pass).  Writes
+ * loc, scale_index and the table index (each may be NULL) in coding order: [B, n, M] with n the positions of this
+ * colour per image (whole == 0), or [B, H W, M] at this pass's rows (whole != 0).  Encoder epilogue (y_dev not
+ * NULL, [B, H, W, M]): also writes y in coding order to `y_cb_dev` (same layout as loc) and yhat = float(int32(rint(
+ * y - loc))) + loc at this colour's positions of `yhat_out_dev` [B, H, W, M]; loc and index are then required.
+ * Three launches for the anchors, four for the non-anchors, none for an empty pass; no host synchronisation. */
+int tfcb_cb_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,
+                   int64_t B, int64_t H, int64_t W, int anchors, int num_scales, float* work_dev,
+                   int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev, int32_t* index_dev,
+                   const float* y_dev, float* y_cb_dev, float* yhat_out_dev, void* stream);
+/* Moves one colour's latents from coding order [B, n, M] to their positions of `dst_dev` [B, H, W, M] (the
+ * other colour's positions are not written).  One launch; none when the colour has no positions. */
+int tfcb_cb_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int anchors, float* dst_dev,
+                    void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Legacy single-stream ops RangeEncode / RangeDecode (int16 data, broadcastable N-D int32 CDF):
  *   op contract   tensorflow_compression/cc/ops/range_coding_ops.cc:30-124
  *   CPU kernels   tensorflow_compression/cc/kernels/range_coding_kernels.cc:60-379
