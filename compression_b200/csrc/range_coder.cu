@@ -22,10 +22,8 @@
 // The one-warp-per-stream helpers further down (ByteWindow, dec_symbol) serve the legacy single-stream ops only.
 #include <algorithm>
 #include <cstring>
-#include <vector>
-
-#include <cstring>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_bf16.h>
@@ -1865,19 +1863,78 @@ int prepare_ragged(tfcb_encoder* h, const int64_t* sym_off, cudaStream_t s) {
   return TFCB_OK;
 }
 
-// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all, laid out by prepare_ragged.
-// `decoded` / `decoded16`: the kModeDecoded output; `loc16`: the 16-bit loc (EncParams).
+// Value types, numbered as the C ABI's `dtype` / `loc_dtype` (int32 values have no such argument).
+enum Dtype : int { kInt32 = -1, kFloat32 = 0, kFloat16 = 1, kBFloat16 = 2 };
+
+// What one encode or decode codes, besides the values themselves: each public entry converts its own arguments into
+// this, and mode_of alone reads the kernel's mode from it.
+struct Operands {
+  Dtype type = kInt32;             // the value's (decoder: the output's) type
+  bool indexed = false;            // index mode: `index` picks each symbol's table; channel mode: its position does
+  const int32_t* index = nullptr;  // [S, n]
+  const void* off = nullptr;       // channel mode: quantisation offsets [n_rows]; index mode: loc [S, n]; or null
+  Dtype off_type = kFloat32;       // float32, or in index mode also the value's 16-bit type
+  const int32_t* cdf_offset = nullptr;  // float values: [n_rows]
+  void* decoded = nullptr;         // encoder, float values: each symbol's decoded value [S, n], or null
+};
+
+// The kernels' mode for a call.  A 16-bit index-mode call with a float32 loc runs under kModeLocF32, which also makes
+// its decoded values float32 (torch's type promotion); in channel mode the offsets are float32 and the mode has no
+// kModeLocF32.
+int mode_of(const Operands& o) {
+  int mode = (o.indexed ? kModeIndex : 0) | (o.decoded ? kModeDecoded : 0);
+  if (o.type == kFloat32) mode |= kModeF32;
+  if (o.type == kFloat16) mode |= kModeH16;
+  if (o.type == kBFloat16) mode |= kModeB16;
+  if ((mode & kMode16) && o.indexed && o.off && o.off_type == kFloat32) mode |= kModeLocF32;
+  return mode;
+}
+
 template <int MODE>
-int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr,
-                  float* decoded = nullptr, const uint16_t* loc16 = nullptr, uint16_t* decoded16 = nullptr) {
+using Mode = std::integral_constant<int, MODE>;
+
+// The one map from a mode_of mode to the kernels' MODE: returns fn(Mode<MODE>{}).  It lists the modes the kernels are
+// compiled for: decode_kernel's 10 below, and encode_kernel's 18, those 10 and each float one with kModeDecoded.
+template <bool ENCODER, class Fn>
+int with_mode(int mode, Fn fn) {
+  const bool decoded = mode & kModeDecoded;
+  if (decoded && !(ENCODER && (mode & kModeFloat)))
+    return fail(TFCB_INVALID_ARGUMENT, "decoded values need float values");
+  auto with_decoded = [&](auto m) {
+    if constexpr (ENCODER) {
+      if (decoded) return fn(Mode<decltype(m)::value | kModeDecoded>{});
+    }
+    return fn(m);
+  };
+  switch (mode & ~kModeDecoded) {
+    case 0: return fn(Mode<0>{});
+    case kModeIndex: return fn(Mode<kModeIndex>{});
+    case kModeF32: return with_decoded(Mode<kModeF32>{});
+    case kModeIndex | kModeF32: return with_decoded(Mode<kModeIndex | kModeF32>{});
+    case kModeH16: return with_decoded(Mode<kModeH16>{});
+    case kModeIndex | kModeH16: return with_decoded(Mode<kModeIndex | kModeH16>{});
+    case kModeIndex | kModeH16 | kModeLocF32: return with_decoded(Mode<kModeIndex | kModeH16 | kModeLocF32>{});
+    case kModeB16: return with_decoded(Mode<kModeB16>{});
+    case kModeIndex | kModeB16: return with_decoded(Mode<kModeIndex | kModeB16>{});
+    case kModeIndex | kModeB16 | kModeLocF32: return with_decoded(Mode<kModeIndex | kModeB16 | kModeLocF32>{});
+  }
+  return fail(TFCB_INVALID_ARGUMENT, "no kernel for mode %d", mode);
+}
+
+// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all, laid out by prepare_ragged.
+template <int MODE>
+int launch_encode(tfcb_encoder* h, const void* value, const Operands& o, long long n, cudaStream_t s,
+                  const long long* sym_off) {
+  // 16-bit values: a loc (index mode) and the decoded output are in the value's type, unless kModeLocF32
+  constexpr bool in16 = (MODE & kMode16) && !(MODE & kModeLocF32);
+  constexpr bool loc16 = in16 && (MODE & kModeIndex);
   if (h->finalized) return fail(TFCB_INVALID_ARGUMENT, "encoder handle was already finalized");
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
   if (h->lut.n_rows == 0) return fail(TFCB_INVALID_ARGUMENT, "index=0 not in range [0, 0)");
   if (value == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`value` is null");
-  if ((MODE & kModeIndex) && index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
-  if ((MODE & kModeFloat) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  if ((MODE & kModeIndex) && o.index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
+  if ((MODE & kModeFloat) && o.cdf_offset == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
   if (!sym_off) {
     const long long extra = words_bound(h, n);
     TFCB_TRY(ensure_capacity(h, extra, s));
@@ -1889,9 +1946,9 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.n_rows = h->lut.n_rows;
   P.uniform_prec = h->lut.uniform_prec;
   P.value = value;
-  P.index = index;
-  P.qoff = qoff;
-  P.coff = coff;
+  P.index = o.index;
+  P.qoff = (MODE & kModeFloat) && !loc16 ? static_cast<const float*>(o.off) : nullptr;
+  P.coff = (MODE & kModeFloat) ? o.cdf_offset : nullptr;
   P.n = n;
   P.n_streams = h->n_streams;
   P.fresh = h->fresh ? 1 : 0;
@@ -1902,15 +1959,21 @@ int launch_encode(tfcb_encoder* h, const void* value, const int32_t* index, cons
   P.err = h->err;
   P.sym_off = sym_off;
   P.arena_off = h->arena_off;
-  P.decoded = decoded;
-  P.loc16 = loc16;
-  P.decoded16 = decoded16;
+  P.decoded = in16 ? nullptr : static_cast<float*>(o.decoded);
+  P.loc16 = loc16 ? static_cast<const uint16_t*>(o.off) : nullptr;
+  P.decoded16 = in16 ? static_cast<uint16_t*>(o.decoded) : nullptr;
   if (h->n_streams > 0x7FFFFFFFll) return fail(TFCB_INVALID_ARGUMENT, "too many streams");
   encode_kernel<MODE><<<(unsigned)h->n_streams, 192, 0, s>>>(P);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   h->fresh = false;
   return TFCB_OK;
+}
+
+int encode(tfcb_encoder* h, const void* value, const Operands& o, long long n, cudaStream_t s,
+           const long long* sym_off = nullptr) {
+  return with_mode<true>(mode_of(o),
+                         [&](auto m) { return launch_encode<decltype(m)::value>(h, value, o, n, s, sym_off); });
 }
 
 // Host-mapped {total, error} per host thread: written by enc_offsets_kernel, read after the stream synchronises.
@@ -2007,26 +2070,27 @@ int tfcb_encoder_create(const int32_t* lookup_host, int64_t lookup_len, int64_t 
 
 int tfcb_encode_channel(tfcb_encoder* h, const int32_t* value_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
-  return launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, as_stream(stream));
+  return encode(h, value_dev, Operands{}, n, as_stream(stream));
 }
 
 int tfcb_encode_index(tfcb_encoder* h, const int32_t* index_dev, const int32_t* value_dev, int64_t n,
                       void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
-  return launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, as_stream(stream));
+  return encode(h, value_dev, Operands{kInt32, true, index_dev}, n, as_stream(stream));
 }
 
 int tfcb_encode_channel_f32(tfcb_encoder* h, const float* y_dev, const float* quant_offset_dev,
                             const int32_t* cdf_offset_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
-  return launch_encode<kModeF32>(h, y_dev, nullptr, quant_offset_dev, cdf_offset_dev, n, as_stream(stream));
+  return encode(h, y_dev, Operands{kFloat32, false, nullptr, quant_offset_dev, kFloat32, cdf_offset_dev}, n,
+                as_stream(stream));
 }
 
 int tfcb_encode_index_f32(tfcb_encoder* h, const int32_t* index_dev, const float* y_dev,
                           const float* loc_dev, const int32_t* cdf_offset_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not an encoder");
-  return launch_encode<kModeIndex | kModeF32>(h, y_dev, index_dev, loc_dev, cdf_offset_dev, n,
-                                              as_stream(stream));
+  return encode(h, y_dev, Operands{kFloat32, true, index_dev, loc_dev, kFloat32, cdf_offset_dev}, n,
+                as_stream(stream));
 }
 
 int tfcb_encoder_check(tfcb_encoder* h, void* stream) {
@@ -2181,33 +2245,6 @@ int finish_compress(tfcb_encoder* h, int rc, int64_t* offsets_dev, cudaStream_t 
   return TFCB_OK;
 }
 
-// The encode of tfcb_compress, tfcb_compress_ragged and tfcb_compress_ragged_decoded on a checked-out encoder.
-// `decoded` non-null (float values only): the encode also writes the decoded values there.
-int encode_checked_out(tfcb_encoder* h, const int32_t* index_dev, const void* value_dev, int32_t value_is_f32,
-                       const float* qoff_dev, const int32_t* cdf_offset_dev, long long n, const long long* sym_off,
-                       cudaStream_t s, float* decoded = nullptr) {
-  const int mode = (index_dev ? kModeIndex : 0) | (value_is_f32 ? kModeF32 : 0) | (decoded ? kModeDecoded : 0);
-  int rc;
-  switch (mode) {
-    case 0: rc = launch_encode<0>(h, value_dev, nullptr, nullptr, nullptr, n, s, sym_off); break;
-    case kModeIndex: rc = launch_encode<kModeIndex>(h, value_dev, index_dev, nullptr, nullptr, n, s, sym_off); break;
-    case kModeF32: rc = launch_encode<kModeF32>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s, sym_off); break;
-    case kModeIndex | kModeF32:
-      rc = launch_encode<kModeIndex | kModeF32>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s, sym_off);
-      break;
-    case kModeF32 | kModeDecoded:
-      rc = launch_encode<kModeF32 | kModeDecoded>(h, value_dev, nullptr, qoff_dev, cdf_offset_dev, n, s, sym_off,
-                                                   decoded);
-      break;
-    case kModeIndex | kModeF32 | kModeDecoded:
-      rc = launch_encode<kModeIndex | kModeF32 | kModeDecoded>(h, value_dev, index_dev, qoff_dev, cdf_offset_dev, n, s,
-                                                               sym_off, decoded);
-      break;
-    default: rc = fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values"); break;
-  }
-  return rc;
-}
-
 // The 16-bit value types' host-side arguments, checked before any device work: `dtype` 1 float16 or 2 bfloat16;
 // `loc_dtype` 0 (float32), or in index mode also `dtype`; cdf_offset always, and the value (or output) whenever
 // there are symbols.
@@ -2223,45 +2260,40 @@ int check16(int dtype, bool index_mode, int loc_dtype, const void* data, const c
   return TFCB_OK;
 }
 
-// The modes of a 16-bit call: the value's type, index mode, and a float32 loc in index mode (kModeLocF32, which
-// also makes the decoded values float32).  The loc is float32 in channel mode (the quantisation offsets).
-int mode16(int dtype, const int32_t* index, const void* loc, int loc_dtype) {
-  return (dtype == 1 ? kModeH16 : kModeB16) | (index ? kModeIndex : 0) | (index && loc && loc_dtype == 0 ? kModeLocF32 : 0);
-}
-
-template <int MODE>
-int encode16(tfcb_encoder* h, const void* value, const int32_t* index, const void* loc, const int32_t* coff,
-             long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
-  constexpr bool loc16 = (MODE & kModeIndex) && !(MODE & kModeLocF32);
-  return launch_encode<MODE>(h, value, index, loc16 ? nullptr : static_cast<const float*>(loc), coff, n, s, sym_off,
-                             (MODE & kModeLocF32) ? static_cast<float*>(decoded) : nullptr,
-                             loc16 ? static_cast<const uint16_t*>(loc) : nullptr,
-                             (MODE & kModeLocF32) ? nullptr : static_cast<uint16_t*>(decoded));
-}
-
-// One encode of a 16-bit value (`decoded` non-null: kModeDecoded) with the mode mode16 selects.
-template <int DT>
-int encode16_of(int mode, tfcb_encoder* h, const void* value, const int32_t* index, const void* loc,
-                const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
-  switch ((mode & ~kMode16) | (decoded ? kModeDecoded : 0)) {
-    case 0: return encode16<DT>(h, value, index, loc, coff, n, s, sym_off, decoded);
-    case kModeDecoded: return encode16<DT | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off, decoded);
-    case kModeIndex: return encode16<DT | kModeIndex>(h, value, index, loc, coff, n, s, sym_off, decoded);
-    case kModeIndex | kModeDecoded:
-      return encode16<DT | kModeIndex | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off, decoded);
-    case kModeIndex | kModeLocF32:
-      return encode16<DT | kModeIndex | kModeLocF32>(h, value, index, loc, coff, n, s, sym_off, decoded);
-    default:
-      return encode16<DT | kModeIndex | kModeLocF32 | kModeDecoded>(h, value, index, loc, coff, n, s, sym_off,
-                                                                     decoded);
+// The compress of every tfcb_compress* entry, after its argument checks: `n` symbols per stream, or with
+// `sym_off_host` [n_streams + 1] non-null a ragged batch.  A ragged batch's per-stream size limit needs the table's
+// worst case bits per symbol, so the table is parsed for it here, before any device work.  Then one encode on a
+// pooled encoder and finish_compress.
+int compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams, long long n,
+             const int64_t* sym_off_host, const void* value, const Operands& o, int64_t* offsets_dev, void* stream,
+             tfcb_encoder** out, int64_t* total_bytes_host) {
+  if (sym_off_host) {
+    std::vector<HostRow> rows;
+    TFCB_TRY(parse_lookup(lookup_host, lookup_len, lookup_cols, &rows));
+    int max_prec = 0;
+    bool any_overflow = false;
+    for (const HostRow& r : rows) {
+      max_prec = std::max(max_prec, r.prec < 0 ? -r.prec : r.prec);
+      any_overflow |= r.prec < 0;
+    }
+    const long long bits = bits_bound(max_prec, any_overflow);
+    for (long long i = 0; i < n_streams; ++i)
+      if (words_for(bits, sym_off_host[i + 1] - sym_off_host[i]) + 32 >= kMaxStreamWords)
+        return fail(TFCB_INVALID_ARGUMENT, "a single code stream may not exceed 2^31 16-bit words (stream %lld)", i);
   }
-}
-
-int encode16_any(int dtype, tfcb_encoder* h, const void* value, const int32_t* index, const void* loc, int loc_dtype,
-                 const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off, void* decoded) {
-  const int mode = mode16(dtype, index, loc, loc_dtype);
-  if (mode & kModeH16) return encode16_of<kModeH16>(mode, h, value, index, loc, coff, n, s, sym_off, decoded);
-  return encode16_of<kModeB16>(mode, h, value, index, loc, coff, n, s, sym_off, decoded);
+  cudaStream_t s = as_stream(stream);
+  tfcb_encoder* h = nullptr;
+  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
+  if (sym_off_host) {
+    const int rc = prepare_ragged(h, sym_off_host, s);
+    if (rc != TFCB_OK) {
+      tfcb_encoder_destroy(h);
+      return rc;
+    }
+    n = sym_off_host[n_streams];
+  }
+  return finish_compress(h, encode(h, value, o, n, s, sym_off_host ? h->ext : nullptr), offsets_dev, s, out,
+                         total_bytes_host);
 }
 
 }  // namespace
@@ -2277,12 +2309,10 @@ int tfcb_compress(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup
   *total_bytes_host = 0;
   if (n_streams < 0) return fail(TFCB_INVALID_ARGUMENT, "negative stream count");
   if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
-  cudaStream_t s = as_stream(stream);
-  tfcb_encoder* h = nullptr;
-  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
-  return finish_compress(h, encode_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev, n,
-                                               nullptr, s),
-                         offsets_dev, s, out, total_bytes_host);
+  const Operands o{value_is_f32 ? kFloat32 : kInt32, index_dev != nullptr, index_dev, qoff_dev, kFloat32,
+                   cdf_offset_dev};
+  return compress(lookup_host, lookup_len, lookup_cols, n_streams, n, nullptr, value_dev, o, offsets_dev, stream, out,
+                  total_bytes_host);
 }
 
 int tfcb_compress_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
@@ -2296,81 +2326,24 @@ int tfcb_compress_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t 
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
   TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, value_dev, "value", cdf_offset_dev, n_streams * n));
-  cudaStream_t s = as_stream(stream);
-  tfcb_encoder* h = nullptr;
-  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
-  return finish_compress(h, encode16_any(dtype, h, value_dev, index_dev, loc_dev, loc_dtype, cdf_offset_dev, n, s,
-                                         nullptr, nullptr),
-                         offsets_dev, s, out, total_bytes_host);
+  const Operands o{Dtype(dtype), index_dev != nullptr, index_dev, loc_dev, Dtype(loc_dtype), cdf_offset_dev};
+  return compress(lookup_host, lookup_len, lookup_cols, n_streams, n, nullptr, value_dev, o, offsets_dev, stream, out,
+                  total_bytes_host);
 }
-
-}  // extern "C"
-
-namespace {
-
-// What the ragged compress entries share: the host-side checks, an encoder laid out for the batch, then
-// `encode(h, n_symbols, device symbol offsets, stream)` and finish_compress.
-template <typename Encode>
-int compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
-                    const int64_t* symbol_offsets_host, int64_t* offsets_dev, void* stream, tfcb_encoder** out,
-                    int64_t* total_bytes_host, Encode encode) {
-  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
-  *out = nullptr;
-  *total_bytes_host = 0;
-  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
-  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
-  // the per-stream size limit needs the table's worst case bits per symbol: parsed here, before any device work
-  {
-    std::vector<HostRow> rows;
-    TFCB_TRY(parse_lookup(lookup_host, lookup_len, lookup_cols, &rows));
-    int max_prec = 0;
-    bool any_overflow = false;
-    for (const HostRow& r : rows) {
-      max_prec = std::max(max_prec, r.prec < 0 ? -r.prec : r.prec);
-      any_overflow |= r.prec < 0;
-    }
-    const long long bits = bits_bound(max_prec, any_overflow);
-    for (long long i = 0; i < n_streams; ++i)
-      if (words_for(bits, symbol_offsets_host[i + 1] - symbol_offsets_host[i]) + 32 >= kMaxStreamWords)
-        return fail(TFCB_INVALID_ARGUMENT, "a single code stream may not exceed 2^31 16-bit words (stream %lld)", i);
-  }
-  cudaStream_t s = as_stream(stream);
-  tfcb_encoder* h = nullptr;
-  TFCB_TRY(checkout_encoder(lookup_host, lookup_len, lookup_cols, n_streams, s, &h));
-  const int rc = prepare_ragged(h, symbol_offsets_host, s);
-  if (rc != TFCB_OK) {
-    tfcb_encoder_destroy(h);
-    return rc;
-  }
-  return finish_compress(h, encode(h, (long long)symbol_offsets_host[n_streams], h->ext, s), offsets_dev, s, out,
-                         total_bytes_host);
-}
-
-// tfcb_compress_ragged, and tfcb_compress_ragged_decoded with `decoded` non-null.
-int compress_ragged_f32(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
-                        const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
-                        int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
-                        int64_t* offsets_dev, float* decoded, void* stream, tfcb_encoder** out,
-                        int64_t* total_bytes_host) {
-  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, offsets_dev, stream,
-                         out, total_bytes_host,
-                         [&](tfcb_encoder* h, long long n, const long long* sym_off, cudaStream_t s) {
-                           return encode_checked_out(h, index_dev, value_dev, value_is_f32, qoff_dev, cdf_offset_dev,
-                                                     n, sym_off, s, decoded);
-                         });
-}
-
-}  // namespace
-
-extern "C" {
 
 int tfcb_compress_ragged(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
                          const int64_t* symbol_offsets_host, const int32_t* index_dev, const void* value_dev,
                          int32_t value_is_f32, const float* qoff_dev, const int32_t* cdf_offset_dev,
                          int64_t* offsets_dev, void* stream, tfcb_encoder** out, int64_t* total_bytes_host) {
-  return compress_ragged_f32(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev,
-                             value_dev, value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, nullptr, stream, out,
-                             total_bytes_host);
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  *out = nullptr;
+  *total_bytes_host = 0;
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
+  const Operands o{value_is_f32 ? kFloat32 : kInt32, index_dev != nullptr, index_dev, qoff_dev, kFloat32,
+                   cdf_offset_dev};
+  return compress(lookup_host, lookup_len, lookup_cols, n_streams, 0, symbol_offsets_host, value_dev, o, offsets_dev,
+                  stream, out, total_bytes_host);
 }
 
 int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols,
@@ -2383,9 +2356,12 @@ int tfcb_compress_ragged_decoded(const int32_t* lookup_host, int64_t lookup_len,
   if (!value_is_f32) return fail(TFCB_INVALID_ARGUMENT, "decoded values need float32 values (`value_is_f32` is 0)");
   if (!decoded_dev) return fail(TFCB_INVALID_ARGUMENT, "`decoded` is null");
   if (!cdf_offset_dev) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
-  return compress_ragged_f32(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, index_dev,
-                             value_dev, value_is_f32, qoff_dev, cdf_offset_dev, offsets_dev, decoded_dev, stream, out,
-                             total_bytes_host);
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
+  const Operands o{kFloat32, index_dev != nullptr, index_dev, qoff_dev, kFloat32, cdf_offset_dev, decoded_dev};
+  return compress(lookup_host, lookup_len, lookup_cols, n_streams, 0, symbol_offsets_host, value_dev, o, offsets_dev,
+                  stream, out, total_bytes_host);
 }
 
 int tfcb_compress_ragged_16bit(const int32_t* lookup_host, int64_t lookup_len, int64_t lookup_cols, int64_t n_streams,
@@ -2398,12 +2374,12 @@ int tfcb_compress_ragged_16bit(const int32_t* lookup_host, int64_t lookup_len, i
   TFCB_TRY(check_symbol_offsets(symbol_offsets_host, n_streams));
   TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, value_dev, "value", cdf_offset_dev,
                    symbol_offsets_host[n_streams]));
-  return compress_ragged(lookup_host, lookup_len, lookup_cols, n_streams, symbol_offsets_host, offsets_dev, stream,
-                         out, total_bytes_host,
-                         [&](tfcb_encoder* h, long long n, const long long* sym_off, cudaStream_t s) {
-                           return encode16_any(dtype, h, value_dev, index_dev, loc_dev, loc_dtype, cdf_offset_dev, n,
-                                               s, sym_off, decoded_dev);
-                         });
+  if (!out || !total_bytes_host) return fail(TFCB_INVALID_ARGUMENT, "null output pointer");
+  if (!offsets_dev) return fail(TFCB_INVALID_ARGUMENT, "`offsets` is null");
+  const Operands o{Dtype(dtype), index_dev != nullptr, index_dev, loc_dev, Dtype(loc_dtype), cdf_offset_dev,
+                   decoded_dev};
+  return compress(lookup_host, lookup_len, lookup_cols, n_streams, 0, symbol_offsets_host, value_dev, o, offsets_dev,
+                  stream, out, total_bytes_host);
 }
 
 int tfcb_compress_write(tfcb_encoder* h, const int64_t* offsets_dev, uint8_t* bytes_dev, void* stream) {
@@ -2452,17 +2428,18 @@ int tfcb::decoder_view(tfcb_decoder* h, DecoderView* v) {
 
 namespace {
 
-// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all.  `loc16`: DecParams.
+// `sym_off` (device, [n_streams + 1]) non-null: a ragged batch of `n` symbols in all.
 template <int MODE>
-int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float* qoff,
-                  const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off = nullptr,
-                  const uint16_t* loc16 = nullptr) {
+int launch_decode(tfcb_decoder* h, void* out, const Operands& o, long long n, cudaStream_t s,
+                  const long long* sym_off) {
+  // 16-bit index modes: the loc is in the output's type, unless kModeLocF32
+  constexpr bool loc16 = (MODE & kMode16) && (MODE & kModeIndex) && !(MODE & kModeLocF32);
   if (n < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   if (h->n_streams == 0 || n == 0) return TFCB_OK;
   if (h->lut.n_rows == 0) return fail(TFCB_INVALID_ARGUMENT, "index=0 not in range [0, 0)");
   if (out == nullptr) return fail(TFCB_INVALID_ARGUMENT, "output is null");
-  if ((MODE & kModeIndex) && index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
-  if ((MODE & kModeFloat) && coff == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
+  if ((MODE & kModeIndex) && o.index == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`index` is null");
+  if ((MODE & kModeFloat) && o.cdf_offset == nullptr) return fail(TFCB_INVALID_ARGUMENT, "`cdf_offset` is null");
   DecParams P;
   P.lookup = h->lut.lookup;
   P.rows = h->lut.rows;
@@ -2474,16 +2451,16 @@ int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float*
   P.lookup_len = h->lut.len;
   P.bytes = h->bytes;
   P.offsets = h->offsets;
-  P.index = index;
+  P.index = o.index;
   P.out = out;
-  P.qoff = qoff;
-  P.coff = coff;
+  P.qoff = (MODE & kModeFloat) && !loc16 ? static_cast<const float*>(o.off) : nullptr;
+  P.coff = (MODE & kModeFloat) ? o.cdf_offset : nullptr;
   P.n = n;
   P.n_streams = h->n_streams;
   P.state = h->state;
   P.err = h->err;
   P.sym_off = sym_off;
-  P.loc16 = loc16;
+  P.loc16 = loc16 ? static_cast<const uint16_t*>(o.off) : nullptr;
   // Search keys live in shared memory whenever they fit beside the kernel's static 16 KB: up to 96 KB two CTAs
   // (streams) still share an SM; up to 200 KB one CTA per SM (cfg3's 64 NoisyNormal tables up to sigma = 256 take
   // 118 KB: from L1/L2 every slow-path search round cost a global-memory latency on the chain warp).
@@ -2500,32 +2477,6 @@ int launch_decode(tfcb_decoder* h, const int32_t* index, void* out, const float*
   return TFCB_OK;
 }
 
-template <int MODE>
-int decode16(tfcb_decoder* h, const int32_t* index, void* out, const void* loc, const int32_t* coff, long long n,
-             cudaStream_t s, const long long* sym_off) {
-  constexpr bool loc16 = (MODE & kModeIndex) && !(MODE & kModeLocF32);
-  return launch_decode<MODE>(h, index, out, loc16 ? nullptr : static_cast<const float*>(loc), coff, n, s, sym_off,
-                             loc16 ? static_cast<const uint16_t*>(loc) : nullptr);
-}
-
-template <int DT>
-int decode16_of(int mode, tfcb_decoder* h, const int32_t* index, void* out, const void* loc, const int32_t* coff,
-                long long n, cudaStream_t s, const long long* sym_off) {
-  switch (mode & ~kMode16) {
-    case 0: return decode16<DT>(h, index, out, loc, coff, n, s, sym_off);
-    case kModeIndex: return decode16<DT | kModeIndex>(h, index, out, loc, coff, n, s, sym_off);
-    default: return decode16<DT | kModeIndex | kModeLocF32>(h, index, out, loc, coff, n, s, sym_off);
-  }
-}
-
-// One decode of 16-bit values with the mode mode16 selects.
-int decode16_any(int dtype, tfcb_decoder* h, const int32_t* index, void* out, const void* loc, int loc_dtype,
-                 const int32_t* coff, long long n, cudaStream_t s, const long long* sym_off) {
-  const int mode = mode16(dtype, index, loc, loc_dtype);
-  if (mode & kModeH16) return decode16_of<kModeH16>(mode, h, index, out, loc, coff, n, s, sym_off);
-  return decode16_of<kModeB16>(mode, h, index, out, loc, coff, n, s, sym_off);
-}
-
 // A ragged decode's symbol offsets, checked and copied to the decoder (`*n`: the symbols in all; nothing is copied
 // when there are none).
 int upload_symbol_offsets(tfcb_decoder* h, const int64_t* symbol_offsets_host, cudaStream_t s, long long* n) {
@@ -2537,6 +2488,15 @@ int upload_symbol_offsets(tfcb_decoder* h, const int64_t* symbol_offsets_host, c
   TFCB_CUDA_TRY(cudaMemcpyAsync(h->sym_off, symbol_offsets_host, (h->n_streams + 1) * sizeof(long long),
                                 cudaMemcpyHostToDevice, s));
   return TFCB_OK;
+}
+
+// The decode of every tfcb_decode_* entry, after its argument checks: `n` symbols per stream, or with `sym_off_host`
+// [n_streams + 1] non-null a ragged batch.
+int decode(tfcb_decoder* h, long long n, const int64_t* sym_off_host, void* out, const Operands& o, cudaStream_t s) {
+  if (sym_off_host) TFCB_TRY(upload_symbol_offsets(h, sym_off_host, s, &n));
+  return with_mode<false>(mode_of(o), [&](auto m) {
+    return launch_decode<decltype(m)::value>(h, out, o, n, s, sym_off_host ? h->sym_off : nullptr);
+  });
 }
 
 }  // namespace
@@ -2577,43 +2537,35 @@ int tfcb_decoder_create(const uint8_t* bytes_dev, const int64_t* offsets_dev, in
 
 int tfcb_decode_channel(tfcb_decoder* h, int32_t* out_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  return launch_decode<0>(h, nullptr, out_dev, nullptr, nullptr, n, as_stream(stream));
+  return decode(h, n, nullptr, out_dev, Operands{}, as_stream(stream));
 }
 
 int tfcb_decode_index(tfcb_decoder* h, const int32_t* index_dev, int32_t* out_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  return launch_decode<kModeIndex>(h, index_dev, out_dev, nullptr, nullptr, n, as_stream(stream));
+  return decode(h, n, nullptr, out_dev, Operands{kInt32, true, index_dev}, as_stream(stream));
 }
 
 int tfcb_decode_channel_f32(tfcb_decoder* h, float* out_dev, const float* quant_offset_dev,
                             const int32_t* cdf_offset_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  return launch_decode<kModeF32>(h, nullptr, out_dev, quant_offset_dev, cdf_offset_dev, n, as_stream(stream));
+  return decode(h, n, nullptr, out_dev, Operands{kFloat32, false, nullptr, quant_offset_dev, kFloat32, cdf_offset_dev},
+                as_stream(stream));
 }
 
 int tfcb_decode_index_f32(tfcb_decoder* h, const int32_t* index_dev, float* out_dev, const float* loc_dev,
                           const int32_t* cdf_offset_dev, int64_t n, void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  return launch_decode<kModeIndex | kModeF32>(h, index_dev, out_dev, loc_dev, cdf_offset_dev, n,
-                                              as_stream(stream));
+  return decode(h, n, nullptr, out_dev, Operands{kFloat32, true, index_dev, loc_dev, kFloat32, cdf_offset_dev},
+                as_stream(stream));
 }
 
 int tfcb_decode_ragged(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev, void* out_dev,
                        int32_t out_is_f32, const float* quant_offset_dev, const int32_t* cdf_offset_dev,
                        void* stream) {
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
-  cudaStream_t s = as_stream(stream);
-  long long n = 0;
-  TFCB_TRY(upload_symbol_offsets(h, symbol_offsets_host, s, &n));
-  if (n == 0) return TFCB_OK;
-  const float* q = quant_offset_dev;
-  const int32_t* c = cdf_offset_dev;
-  switch ((index_dev ? kModeIndex : 0) | (out_is_f32 ? kModeF32 : 0)) {
-    case 0: return launch_decode<0>(h, nullptr, out_dev, nullptr, nullptr, n, s, h->sym_off);
-    case kModeIndex: return launch_decode<kModeIndex>(h, index_dev, out_dev, nullptr, nullptr, n, s, h->sym_off);
-    case kModeF32: return launch_decode<kModeF32>(h, nullptr, out_dev, q, c, n, s, h->sym_off);
-    default: return launch_decode<kModeIndex | kModeF32>(h, index_dev, out_dev, q, c, n, s, h->sym_off);
-  }
+  const Operands o{out_is_f32 ? kFloat32 : kInt32, index_dev != nullptr, index_dev, quant_offset_dev, kFloat32,
+                   cdf_offset_dev};
+  return decode(h, 0, symbol_offsets_host, out_dev, o, as_stream(stream));
 }
 
 int tfcb_decode_16bit(tfcb_decoder* h, const int32_t* index_dev, void* out_dev, int dtype, const void* loc_dev,
@@ -2621,8 +2573,8 @@ int tfcb_decode_16bit(tfcb_decoder* h, const int32_t* index_dev, void* out_dev, 
   if (!h) return fail(TFCB_INVALID_ARGUMENT, "'handle' is not a decoder");
   if (n_per_stream < 0) return fail(TFCB_INVALID_ARGUMENT, "negative element count");
   TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, out_dev, "out", cdf_offset_dev, h->n_streams * n_per_stream));
-  return decode16_any(dtype, h, index_dev, out_dev, loc_dev, loc_dtype, cdf_offset_dev, n_per_stream,
-                      as_stream(stream), nullptr);
+  const Operands o{Dtype(dtype), index_dev != nullptr, index_dev, loc_dev, Dtype(loc_dtype), cdf_offset_dev};
+  return decode(h, n_per_stream, nullptr, out_dev, o, as_stream(stream));
 }
 
 int tfcb_decode_ragged_16bit(tfcb_decoder* h, const int64_t* symbol_offsets_host, const int32_t* index_dev,
@@ -2632,10 +2584,8 @@ int tfcb_decode_ragged_16bit(tfcb_decoder* h, const int64_t* symbol_offsets_host
   TFCB_TRY(check_symbol_offsets(symbol_offsets_host, h->n_streams));
   TFCB_TRY(check16(dtype, index_dev != nullptr, loc_dtype, out_dev, "out", cdf_offset_dev,
                    symbol_offsets_host[h->n_streams]));
-  cudaStream_t s = as_stream(stream);
-  long long n = 0;
-  TFCB_TRY(upload_symbol_offsets(h, symbol_offsets_host, s, &n));
-  return decode16_any(dtype, h, index_dev, out_dev, loc_dev, loc_dtype, cdf_offset_dev, n, s, h->sym_off);
+  const Operands o{Dtype(dtype), index_dev != nullptr, index_dev, loc_dev, Dtype(loc_dtype), cdf_offset_dev};
+  return decode(h, 0, symbol_offsets_host, out_dev, o, as_stream(stream));
 }
 
 int tfcb_decode_finalize(tfcb_decoder* h, uint8_t* ok_host, void* stream) {
