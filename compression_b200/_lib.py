@@ -77,6 +77,12 @@ SIGNATURES = {
     "tfcb_cb_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64, _int, _vp, _vp, _vp,
                               _vp, _vp, _vp, _vp]),
     "tfcb_cb_scatter": (_int, [_vp, _i64, _i64, _i64, _int, _int, _vp, _vp]),
+    "tfcb_scc_packed_floats": (_i64, [_int, _int, _int, _p(_i64)]),
+    "tfcb_scc_pack_weights": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "tfcb_scc_workspace_floats": (_i64, [_int, _int, _int, _i64, _i64, _i64, _int]),
+    "tfcb_scc_params": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64,
+                               _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_scc_scatter": (_int, [_vp, _i64, _i64, _i64, _int, _int, _int, _int, _vp, _vp]),
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_range_decode": (_int, [_vp, _i64, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),

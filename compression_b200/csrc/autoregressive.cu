@@ -257,15 +257,8 @@ int tfcb_ar_pack_weights(int M, const float* ctx_kernel_dev, const float* ctx_bi
                 M, (long long)d.total);
   const float* src[8] = {ctx_kernel_dev, ctx_bias_dev, w1_dev, b1_dev, w2_dev, b2_dev, w3_dev, b3_dev};
   const long long at[9] = {d.wc, d.bc, d.w1, d.b1, d.w2, d.b2, d.w3, d.b3, d.total};
-  for (int i = 0; i < 8; ++i)
-    if (!src[i]) return fail(TFCB_INVALID_ARGUMENT, "weight operand %d is null", i);
-  if (!packed_dev) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
-  cudaStream_t s = as_stream(stream);
   // the context kernel [5, 5, M, 2M] holds the 12 causal taps first in raster order: [12M][2M] is its prefix
-  for (int i = 0; i < 8; ++i)
-    TFCB_CUDA_TRY(cudaMemcpyAsync(packed_dev + at[i], src[i], (at[i + 1] - at[i]) * sizeof(float),
-                                  cudaMemcpyDeviceToDevice, s));
-  return TFCB_OK;
+  return ar_pack_segments(src, at, packed_dev, as_stream(stream));
 }
 
 int tfcb_ar_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,

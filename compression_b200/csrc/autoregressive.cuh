@@ -1,7 +1,8 @@
-// What the joint autoregressive prior (autoregressive.cu) and the checkerboard context model (checkerboard.cu)
-// share: the packed parameter layout, the constants of the fixed reduction order, the table-index conversion and
-// the argument checks.  Both kernels read the same packed buffer (tfcb_ar_pack_weights) and compute every dense
-// output in the order of autoregressive.cu's file comment.
+// What the joint autoregressive prior (autoregressive.cu) and the checkerboard and space-channel context models
+// (checkerboard.cu) share: the packed parameter layout, the constants of the fixed reduction order, the table-index
+// conversion, the packing copies and the argument checks.  Both files' kernels compute every dense output in the
+// order of autoregressive.cu's file comment; with one channel group they read the same packed buffer
+// (tfcb_ar_pack_weights).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -47,6 +48,14 @@ __device__ __forceinline__ int32_t ar_table_index(float s, int num_scales) {
   return (int32_t)v;
 }
 
+int ar_check_batch(int64_t B, int64_t H, int64_t W, int num_scales) {
+  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
+  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
+    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
+  if (num_scales < 1) return fail(TFCB_INVALID_ARGUMENT, "num_scales=%d must be positive", num_scales);
+  return TFCB_OK;
+}
+
 int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64_t H, int64_t W, int num_scales) {
   if (M <= 0 || M % 6 != 0 || M > kArMaxM)
     return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be a positive multiple of 6 and at most %d", M,
@@ -55,10 +64,18 @@ int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64
   if (packed_floats != ar_dims(M).total)
     return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, M=%d needs %lld", (long long)packed_floats,
                 M, (long long)ar_dims(M).total);
-  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
-  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
-    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
-  if (num_scales < 1) return fail(TFCB_INVALID_ARGUMENT, "num_scales=%d must be positive", num_scales);
+  return ar_check_batch(B, H, W, num_scales);
+}
+
+// Stream-ordered device copies of the eight weight operands (context weights, bias, W1, b1, W2, b2, W3, b3) into
+// `packed` at the offsets at[i], each at[i + 1] - at[i] floats long.
+int ar_pack_segments(const float* const src[8], const long long at[9], float* packed, cudaStream_t s) {
+  for (int i = 0; i < 8; ++i)
+    if (!src[i]) return fail(TFCB_INVALID_ARGUMENT, "weight operand %d is null", i);
+  if (!packed) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
+  for (int i = 0; i < 8; ++i)
+    TFCB_CUDA_TRY(cudaMemcpyAsync(packed + at[i], src[i], (at[i + 1] - at[i]) * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, s));
   return TFCB_OK;
 }
 

@@ -1,21 +1,27 @@
-// Checkerboard context model (He, Zheng, Sun, Wang & Qin, CVPR 2021) on sm_90a: the entropy parameters of one
-// colour of latent positions, all images and positions of that colour at once.
+// Checkerboard context model (He, Zheng, Sun, Wang & Qin, CVPR 2021) and space-channel context model (He, Yang, Peng,
+// Ma, Qin & Wang, CVPR 2022) on sm_90a: the entropy parameters of one colour of latent positions of one channel group,
+// all images and positions of that colour at once.
 //
-// A position (r, c) is an anchor when r + c is even, else a non-anchor.  An image codes its anchors in raster order,
-// then its non-anchors in raster order ("coding order"); the j-th position of colour k (0 anchors, 1 non-anchors)
-// lies in row 2 (j / W) or 2 (j / W) + 1, see cb_position.  Per position (N2 = 2M, N3 = 10M/3, N4 = 8M/3):
-//   ctx   = 0 at an anchor (bias included); at a non-anchor bc + Wc · gather(ŷ, the 12 taps (dy, dx) in [-2, 2]^2
-//           with dy + dx odd, raster order, zeros outside the image), every tap an anchor            [12M] -> [2M]
-//   h1    = leaky(b1 + W1 · [ψ_p, ctx])                                                              [4M]  -> [N3]
-//   h2    = leaky(b2 + W2 · h1)                                                                      [N3]  -> [N4]
-//   out   = b3 + W3 · h2 = [loc, scale_index]                                                        [N4]  -> [2M]
-// with the packed weights of tfcb_ar_pack_weights (Wc: the 12 checkerboard taps, gathered by the caller).
+// A position (r, c) is an anchor when r + c is even, else a non-anchor.  The latent y [B, H, W, M] is split into
+// channel groups; group k holds the C = c_k channels [o, o + C) (the checkerboard model is the one group o = 0,
+// C = M).  An image codes group 0's anchors in raster order, then group 0's non-anchors in raster order, then group
+// 1's anchors, and so on ("coding order"); the j-th position of colour k (0 anchors, 1 non-anchors) lies in row
+// 2 (j / W) or 2 (j / W) + 1, see cb_position.  Per position of group k (CH = 0 for k = 0, else 2C):
+//   ctx   = 0 at an anchor (bias included); at a non-anchor bc + Wc · gather(ŷ[o, o + C), the 12 taps (dy, dx) in
+//           [-2, 2]^2 with dy + dx odd, raster order, zeros outside the image), every tap an anchor  [12C] -> [2C]
+//   h1    = leaky(b1 + W1 · [ψ_p (2M), chctx_p (CH), ctx])                      [K1 = 2M + CH + 2C]  -> [N3 = 5 K1 / 6]
+//   h2    = leaky(b2 + W2 · h1)                                                                      [N3]  -> [N4 = 2 K1 / 3]
+//   out   = b3 + W3 · h2 = [loc, scale_index]                                                        [N4]  -> [2C]
+// (N3 and N4 rounded down; with one group they are 10M/3 and 8M/3) with the packed weights of one group, laid out
+// by cb_net (Wc: the 12 checkerboard taps, gathered by the caller).  The channel context chctx [B, H, W, CH] comes
+// from the caller.
 //
 // Every output is autoregressive.cu's fixed sequence of float32 operations: bias first, then the eight slices
 // [s·K/8, (s+1)·K/8) in order, each an __fmaf_rn chain from +0.f in increasing k, added with __fadd_rn, then the
 // LeakyReLU.  So an output depends only on its own position's inputs, never on the tile, the grid, B or the SM count.
-// At an anchor, layer 1's slices 4-7 are exactly the ctx half [2M, 4M) (4M/8 = M/2), whose chains over zeros are +0
-// for finite weights: they are skipped and +0.f is added in their place (turning a -0 sum into +0, as the chain would).
+// At an anchor, a slice of layer 1 that lies wholly in the ctx segment [2M + CH, K1) is a chain over zeros, which is
+// +0 for finite weights: it is skipped and +0.f is added in its place (turning a -0 sum into +0, as the chain would).
+// Any other slice runs its chain over the zeros.  With one group these are exactly slices 4-7.
 //
 // A pass is one launch per layer (three at anchors, four at non-anchors).  A CTA computes a tile of kCbTP positions ×
 // kCbTN output columns of one layer, staging kCbKC inputs of each position and the matching weight rows in shared
@@ -44,16 +50,17 @@ enum : int { kInTaps = 0, kInPsiCtx = 1, kInPlain = 2 };  // what a layer reads
 enum : int { kOutHidden = 0, kOutParams = 1 };             // what it writes
 
 struct CbPass {
-  int B, H, W, M, colour, num_scales;
-  long long n_k, n_a, HW, P;  // positions of this colour per image, anchors per image, H·W, B·n_k
-  const float* psi;           // [B, H, W, 2M]
-  const float* yhat;          // [B, H, W, M]: the non-anchor pass gathers the anchors' ŷ
-  // params epilogue: [B, out_rows, M] with this pass's rows at out_row0 + j
-  long long out_rows, out_row0;
+  int B, H, W, M, C, o, CH, colour, num_scales;  // latent depth M; the group's C channels from o; CH: chctx width
+  long long n_k, HW, P;                          // positions of this colour per image, H·W, B·n_k
+  const float* psi;                              // [B, H, W, 2M]
+  const float* chctx;                            // [B, H, W, CH] (CH > 0)
+  const float* yhat;                             // [B, H, W, M]: the non-anchor pass gathers the anchors' ŷ
+  // params epilogue: channel c of this pass's j-th position of image b at out_stride·b + out_base + C·j + c
+  long long out_stride, out_base;
   float* loc;
   float* scale;
   int32_t* index;
-  // encoder epilogue (y non-null): y [B, H, W, M] in, y in coding order and ŷ [B, H, W, M] out
+  // encoder epilogue (y non-null): y [B, H, W, M] in, y in coding order and ŷ [B, H, W, M] out, at channels o + c
   const float* y;
   float* y_cb;
   float* yhat_out;
@@ -62,11 +69,38 @@ struct CbPass {
 struct CbLayer {
   const float* W;  // [K, N]
   const float* bias;
-  const float* in;  // kInPsiCtx: ctx [P, 2M]; kInPlain: [P, K]
+  const float* in;  // kInPsiCtx: ctx [P, 2C]; kInPlain: [P, K]
   float* out;       // kOutHidden: [P, N]
   int K, N;
-  bool leaky, ctx_zero;  // ctx_zero: layer 1 at anchors
+  int zero_from;    // kInPsiCtx: inputs [zero_from, K) are zeros (the ctx segment at anchors), else K
+  bool leaky;
 };
+
+// One group's parameter network: its widths and the offsets of its packed buffer, in floats.
+struct CbNet {
+  int C, K1, N3, N4;
+  long long wc, bc, w1, b1, w2, b2, w3, b3, total;
+};
+
+// The packed layout of group [o, o + C) of a latent of depth M: Wc [12C, 2C], bc [2C], W1 [K1, N3], b1, W2 [N3, N4],
+// b2, W3 [N4, 2C], b3.  At o = 0, C = M (M a multiple of 6) it is ar_dims(M)'s, which tfcb_ar_pack_weights packs.
+__host__ __device__ inline CbNet cb_net(int M, int o, int C) {
+  CbNet d;
+  d.C = C;
+  d.K1 = 2 * M + (o > 0 ? 2 * C : 0) + 2 * C;
+  d.N3 = 5 * d.K1 / 6;
+  d.N4 = 2 * d.K1 / 3;
+  d.wc = 0;
+  d.bc = d.wc + (long long)kArTaps * C * 2 * C;
+  d.w1 = d.bc + 2 * C;
+  d.b1 = d.w1 + (long long)d.K1 * d.N3;
+  d.w2 = d.b1 + d.N3;
+  d.b2 = d.w2 + (long long)d.N3 * d.N4;
+  d.w3 = d.b2 + d.N4;
+  d.b3 = d.w3 + (long long)d.N4 * 2 * C;
+  d.total = d.b3 + 2 * C;
+  return d;
+}
 
 // the j-th position of colour k of an image of width W, in raster order
 __host__ __device__ inline void cb_position(long long j, int W, int k, int* r, int* c) {
@@ -86,7 +120,7 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
   __shared__ __align__(16) float xs[kCbKC][kCbTP + 4];  // (+4: a stage's stores hit 8 banks, rows stay 16-byte aligned)
   __shared__ __align__(16) float ws[kCbKC][kCbTN];
   __shared__ long long s_pix[kCbTP];  // b·H·W + r·W + c, or -1 past the last position
-  __shared__ long long s_row[kCbTP];  // the position's row of the params outputs
+  __shared__ long long s_row[kCbTP];  // the position's first element of the params outputs
   __shared__ int s_r[kCbTP], s_c[kCbTP];
   const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   const long long p0 = (long long)blockIdx.x * kCbTP;
@@ -99,7 +133,7 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
       const long long b = p / S.n_k;
       cb_position(p - b * S.n_k, S.W, S.colour, &r, &c);
       pix = b * S.HW + (long long)r * S.W + c;
-      row = b * S.out_rows + S.out_row0 + (p - b * S.n_k);
+      row = b * S.out_stride + S.out_base + (p - b * S.n_k) * S.C;
     }
     s_pix[tid] = pix;
     s_row[tid] = row;
@@ -107,7 +141,7 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
     s_c[tid] = c;
   }
   __syncthreads();
-  const int K = L.K, N = L.N, M = S.M;
+  const int K = L.K, N = L.N, C = S.C;
   float v[4][2], acc[4][2];
 #pragma unroll
   for (int q = 0; q < 2; ++q) {
@@ -118,7 +152,7 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
   }
   for (int s = 0; s < kArSlices; ++s) {
     const int k0 = s * K / kArSlices, k1 = (s + 1) * K / kArSlices;
-    if (L.ctx_zero && s >= kArSlices / 2) {  // the ctx half of [ψ, ctx] at an anchor: a chain over zeros is +0
+    if (k0 >= L.zero_from) {  // wholly in the ctx segment of [ψ, chctx, ctx] at an anchor: a chain over zeros is +0
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -139,12 +173,18 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
         if (kk < n && pix >= 0) {
           const int k = kc + kk;
           if (IN == kInTaps) {
-            const int t = k / M, ch = k - t * M;
+            const int t = k / C, ch = k - t * C;
             const int rr = s_r[pp] + c_cb_dy[t], cc = s_c[pp] + c_cb_dx[t];
             if (rr >= 0 && rr < S.H && cc >= 0 && cc < S.W)
-              x = S.yhat[(pix + (long long)c_cb_dy[t] * S.W + c_cb_dx[t]) * M + ch];
+              x = S.yhat[(pix + (long long)c_cb_dy[t] * S.W + c_cb_dx[t]) * S.M + S.o + ch];
           } else if (IN == kInPsiCtx) {
-            x = k < 2 * M ? __ldg(S.psi + pix * (2 * M) + k) : L.in[(p0 + pp) * (2 * M) + (k - 2 * M)];
+            const int PW = 2 * S.M, CH = S.CH;
+            if (k < PW)
+              x = __ldg(S.psi + pix * PW + k);
+            else if (k < PW + CH)
+              x = __ldg(S.chctx + pix * CH + (k - PW));
+            else if (k < L.zero_from)
+              x = L.in[(p0 + pp) * (2 * C) + (k - PW - CH)];
           } else {
             x = L.in[(p0 + pp) * K + k];
           }
@@ -188,45 +228,128 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
         L.out[p * N + j] = val;
         continue;
       }
-      const long long row = s_row[pp] * M;
-      if (j < M) {
+      const long long row = s_row[pp];
+      if (j < C) {
         if (S.loc) S.loc[row + j] = val;
         if (S.y) {
-          const float yv = __ldg(S.y + pix * M + j);
+          const long long at = pix * S.M + S.o + j;
+          const float yv = __ldg(S.y + at);
           const int q32 = (int)rintf(__fsub_rn(yv, val));
-          S.yhat_out[pix * M + j] = __fadd_rn((float)q32, val);
+          S.yhat_out[at] = __fadd_rn((float)q32, val);
           S.y_cb[row + j] = yv;
         }
       } else {
-        if (S.scale) S.scale[row + j - M] = val;
-        if (S.index) S.index[row + j - M] = ar_table_index(val, S.num_scales);
+        if (S.scale) S.scale[row + j - C] = val;
+        if (S.index) S.index[row + j - C] = ar_table_index(val, S.num_scales);
       }
     }
   }
 }
 
-// ŷ of one colour, [B, n_k, M] in coding order -> its positions of [B, H, W, M]
+// ŷ of one colour of group [o, o + C), [B, n_k, C] in coding order -> its positions and channels of [B, H, W, M]
 __global__ void cb_scatter_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n_k, int W,
-                                  long long HW, int M, int colour, long long total) {
+                                  long long HW, int M, int o, int C, int colour, long long total) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const long long row = e / M, b = row / n_k;
+    const long long row = e / C, b = row / n_k;
     int r, c;
     cb_position(row - b * n_k, W, colour, &r, &c);
-    dst[(b * HW + (long long)r * W + c) * M + (e - row * M)] = src[e];
+    dst[(b * HW + (long long)r * W + c) * M + o + (e - row * C)] = src[e];
   }
 }
 
+constexpr int kSccMaxM = 1024;
+
 long long cb_count(int64_t H, int64_t W, int colour) { return colour ? H * W / 2 : (H * W + 1) / 2; }
 
-long long cb_work_floats(int M, int64_t B, int64_t H, int64_t W, int colour) {
-  const ArDims d = ar_dims(M);
-  return B * cb_count(H, W, colour) * ((colour ? d.N2 : 0) + d.N3 + d.N4);
+long long cb_work_floats(const CbNet& d, int64_t B, int64_t H, int64_t W, int colour) {
+  return B * cb_count(H, W, colour) * ((colour ? 2 * d.C : 0) + d.N3 + d.N4);
+}
+
+bool scc_group_ok(int M, int o, int C) { return M > 0 && M % 2 == 0 && M <= kSccMaxM && o >= 0 && C >= 1 && o + C <= M; }
+
+int scc_check_group(int M, int o, int C) {
+  if (M <= 0 || M % 2 != 0 || M > kSccMaxM)
+    return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be a positive even number and at most %d", M, kSccMaxM);
+  if (o < 0 || C < 1 || o + C > M)
+    return fail(TFCB_INVALID_ARGUMENT, "group of %d channels at offset %d does not fit a latent of depth %d", C, o, M);
+  return TFCB_OK;
 }
 
 template <int IN, int OUT>
 int cb_layer(const CbPass& S, const CbLayer& L, cudaStream_t s) {
   const dim3 grid((unsigned)((S.P + kCbTP - 1) / kCbTP), (unsigned)((L.N + kCbTN - 1) / kCbTN));
   cb_dense_kernel<IN, OUT><<<grid, kCbThreads, 0, s>>>(S, L);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+// One pass over colour `colour` of group [o, o + C) of a latent of depth M, after the caller's checks of M, the group,
+// the packed size, B, H, W and num_scales.  Outputs [B, n_k, C] (whole == 0), or the coding order of every group,
+// [B, H W M], at this pass's block H W o + (colour ? n_a C : 0) (whole != 0).
+int cb_run(const float* packed, int M, int o, int C, const float* yhat, const float* psi, const float* chctx,
+           int64_t B, int64_t H, int64_t W, int colour, int num_scales, float* work, int64_t work_floats, int whole,
+           float* loc, float* scale, int32_t* index, const float* y, float* y_cb, float* yhat_out, void* stream) {
+  if (!psi || (colour && !yhat)) return fail(TFCB_INVALID_ARGUMENT, "`psi` or `yhat` is null");
+  if (o > 0 && !chctx)
+    return fail(TFCB_INVALID_ARGUMENT, "`chctx` is null: the group at channel offset %d needs its channel context", o);
+  const CbNet d = cb_net(M, o, C);
+  const long long need = cb_work_floats(d, B, H, W, colour);
+  if (!work || work_floats < need)
+    return fail(TFCB_INVALID_ARGUMENT, "workspace of %lld floats, this pass needs %lld", work ? (long long)work_floats : 0ll,
+                need);
+  if (y && (!y_cb || !yhat_out || !loc || !index))
+    return fail(TFCB_INVALID_ARGUMENT, "the encoder needs `y_cb`, `yhat_out`, `loc` and `index`");
+  const long long n_k = cb_count(H, W, colour);
+  if (n_k == 0) return TFCB_OK;
+  CbPass S{};
+  S.B = (int)B;
+  S.H = (int)H;
+  S.W = (int)W;
+  S.M = M;
+  S.C = C;
+  S.o = o;
+  S.CH = o > 0 ? 2 * C : 0;
+  S.colour = colour;
+  S.num_scales = num_scales;
+  S.n_k = n_k;
+  S.HW = H * W;
+  S.P = B * n_k;
+  S.psi = psi;
+  S.chctx = chctx;
+  S.yhat = yhat;
+  S.out_stride = whole ? S.HW * M : n_k * C;
+  S.out_base = whole ? S.HW * o + (colour ? cb_count(H, W, 0) * C : 0) : 0;
+  S.loc = loc;
+  S.scale = scale;
+  S.index = index;
+  S.y = y;
+  S.y_cb = y_cb;
+  S.yhat_out = yhat_out;
+  float* ctx = work;
+  float* h1 = ctx + (colour ? S.P * 2 * C : 0);
+  float* h2 = h1 + S.P * d.N3;
+  cudaStream_t s = as_stream(stream);
+  if (colour)
+    TFCB_TRY((cb_layer<kInTaps, kOutHidden>(
+        S, {packed + d.wc, packed + d.bc, nullptr, ctx, kArTaps * C, 2 * C, kArTaps * C, false}, s)));
+  TFCB_TRY((cb_layer<kInPsiCtx, kOutHidden>(
+      S, {packed + d.w1, packed + d.b1, ctx, h1, d.K1, d.N3, colour ? d.K1 : d.K1 - 2 * C, true}, s)));
+  TFCB_TRY((cb_layer<kInPlain, kOutHidden>(S, {packed + d.w2, packed + d.b2, h1, h2, d.N3, d.N4, d.N3, true}, s)));
+  return cb_layer<kInPlain, kOutParams>(S, {packed + d.w3, packed + d.b3, h2, nullptr, d.N4, 2 * C, d.N4, false}, s);
+}
+
+int cb_scatter(const float* src, int64_t B, int64_t H, int64_t W, int M, int o, int C, int colour, float* dst,
+               void* stream) {
+  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
+  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
+    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
+  const long long n_k = cb_count(H, W, colour), total = B * n_k * C;
+  if (total == 0) return TFCB_OK;  // (the non-anchors of a 1x1 latent: empty tensors may have null pointers)
+  if (!src || !dst) return fail(TFCB_INVALID_ARGUMENT, "`src` or `dst` is null");
+  const long long blocks = std::min<long long>((total + 255) / 256, 1ll << 16);
+  cb_scatter_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(src, dst, n_k, (int)W, H * W, M, o, C, colour,
+                                                                     total);
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
@@ -241,7 +364,7 @@ extern "C" {
 
 int64_t tfcb_cb_workspace_floats(int M, int64_t B, int64_t H, int64_t W, int anchors) {
   if (M <= 0 || M % 6 != 0 || M > kArMaxM || B <= 0 || H <= 0 || W <= 0 || H * W > 0x7FFFFFFF) return -1;
-  return cb_work_floats(M, B, H, W, anchors ? 0 : 1);
+  return cb_work_floats(cb_net(M, 0, M), B, H, W, anchors ? 0 : 1);
 }
 
 int tfcb_cb_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,
@@ -249,67 +372,66 @@ int tfcb_cb_params(const float* packed_dev, int64_t packed_floats, int M, const 
                    int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev, int32_t* index_dev,
                    const float* y_dev, float* y_cb_dev, float* yhat_out_dev, void* stream) {
   TFCB_TRY(ar_check(M, packed_dev, packed_floats, B, H, W, num_scales));
-  const int colour = anchors ? 0 : 1;
-  if (!psi_dev || (colour && !yhat_dev)) return fail(TFCB_INVALID_ARGUMENT, "`psi` or `yhat` is null");
-  const long long need = cb_work_floats(M, B, H, W, colour);
-  if (!work_dev || work_floats < need)
-    return fail(TFCB_INVALID_ARGUMENT, "workspace of %lld floats, this pass needs %lld",
-                work_dev ? (long long)work_floats : 0ll, need);
-  if (y_dev && (!y_cb_dev || !yhat_out_dev || !loc_dev || !index_dev))
-    return fail(TFCB_INVALID_ARGUMENT, "the encoder needs `y_cb`, `yhat_out`, `loc` and `index`");
-  const long long n_k = cb_count(H, W, colour);
-  if (n_k == 0) return TFCB_OK;
-  const ArDims d = ar_dims(M);
-  CbPass S{};
-  S.B = (int)B;
-  S.H = (int)H;
-  S.W = (int)W;
-  S.M = M;
-  S.colour = colour;
-  S.num_scales = num_scales;
-  S.n_k = n_k;
-  S.n_a = cb_count(H, W, 0);
-  S.HW = H * W;
-  S.P = B * n_k;
-  S.psi = psi_dev;
-  S.yhat = yhat_dev;
-  S.out_rows = whole ? H * W : n_k;
-  S.out_row0 = whole && colour ? S.n_a : 0;
-  S.loc = loc_dev;
-  S.scale = scale_index_dev;
-  S.index = index_dev;
-  S.y = y_dev;
-  S.y_cb = y_cb_dev;
-  S.yhat_out = yhat_out_dev;
-  float* ctx = work_dev;
-  float* h1 = ctx + (colour ? S.P * d.N2 : 0);
-  float* h2 = h1 + S.P * d.N3;
-  const float* Wp = packed_dev;
-  cudaStream_t s = as_stream(stream);
-  if (colour)
-    TFCB_TRY((cb_layer<kInTaps, kOutHidden>(S, {Wp + d.wc, Wp + d.bc, nullptr, ctx, kArTaps * M, d.N2, false, false},
-                                            s)));
-  TFCB_TRY((cb_layer<kInPsiCtx, kOutHidden>(S, {Wp + d.w1, Wp + d.b1, ctx, h1, 4 * M, d.N3, true, !colour}, s)));
-  TFCB_TRY((cb_layer<kInPlain, kOutHidden>(S, {Wp + d.w2, Wp + d.b2, h1, h2, d.N3, d.N4, true, false}, s)));
-  return cb_layer<kInPlain, kOutParams>(S, {Wp + d.w3, Wp + d.b3, h2, nullptr, d.N4, d.N2, false, false}, s);
+  return cb_run(packed_dev, M, 0, M, yhat_dev, psi_dev, nullptr, B, H, W, anchors ? 0 : 1, num_scales, work_dev,
+                work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev, yhat_out_dev, stream);
 }
 
 int tfcb_cb_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int anchors, float* dst_dev,
                     void* stream) {
   if (M <= 0) return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be positive", M);
-  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
-  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
-    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
-  const int colour = anchors ? 0 : 1;
-  const long long n_k = cb_count(H, W, colour), total = B * n_k * M;
-  if (total == 0) return TFCB_OK;  // (the non-anchors of a 1x1 latent: empty tensors may have null pointers)
-  if (!src_dev || !dst_dev) return fail(TFCB_INVALID_ARGUMENT, "`src` or `dst` is null");
-  const long long blocks = std::min<long long>((total + 255) / 256, 1ll << 16);
-  cb_scatter_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(src_dev, dst_dev, n_k, (int)W, H * W, M, colour,
-                                                                     total);
-  TFCB_LAUNCHED();
-  TFCB_CUDA_TRY(cudaGetLastError());
-  return TFCB_OK;
+  return cb_scatter(src_dev, B, H, W, M, 0, M, anchors ? 0 : 1, dst_dev, stream);
+}
+
+int64_t tfcb_scc_packed_floats(int M, int offset, int C, int64_t* layout) {
+  if (!scc_group_ok(M, offset, C)) return -1;
+  const CbNet d = cb_net(M, offset, C);
+  if (layout) {
+    const int64_t v[11] = {d.K1, d.N3, d.N4, d.wc, d.bc, d.w1, d.b1, d.w2, d.b2, d.w3, d.b3};
+    for (int i = 0; i < 11; ++i) layout[i] = v[i];
+  }
+  return d.total;
+}
+
+int tfcb_scc_pack_weights(int M, int offset, int C, const float* ctx_taps_dev, const float* ctx_bias_dev,
+                          const float* w1_dev, const float* b1_dev, const float* w2_dev, const float* b2_dev,
+                          const float* w3_dev, const float* b3_dev, float* packed_dev, int64_t packed_floats,
+                          void* stream) {
+  TFCB_TRY(scc_check_group(M, offset, C));
+  const CbNet d = cb_net(M, offset, C);
+  if (packed_floats != d.total)
+    return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, the group [%d, %d) of M=%d needs %lld",
+                (long long)packed_floats, offset, offset + C, M, (long long)d.total);
+  const float* src[8] = {ctx_taps_dev, ctx_bias_dev, w1_dev, b1_dev, w2_dev, b2_dev, w3_dev, b3_dev};
+  const long long at[9] = {d.wc, d.bc, d.w1, d.b1, d.w2, d.b2, d.w3, d.b3, d.total};
+  return ar_pack_segments(src, at, packed_dev, as_stream(stream));
+}
+
+int64_t tfcb_scc_workspace_floats(int M, int offset, int C, int64_t B, int64_t H, int64_t W, int anchors) {
+  if (!scc_group_ok(M, offset, C) || B <= 0 || H <= 0 || W <= 0 || H * W > 0x7FFFFFFF) return -1;
+  return cb_work_floats(cb_net(M, offset, C), B, H, W, anchors ? 0 : 1);
+}
+
+int tfcb_scc_params(const float* packed_dev, int64_t packed_floats, int M, int offset, int C, const float* yhat_dev,
+                    const float* psi_dev, const float* chctx_dev, int64_t B, int64_t H, int64_t W, int anchors,
+                    int num_scales, float* work_dev, int64_t work_floats, int whole, float* loc_dev,
+                    float* scale_index_dev, int32_t* index_dev, const float* y_dev, float* y_cb_dev,
+                    float* yhat_out_dev, void* stream) {
+  TFCB_TRY(scc_check_group(M, offset, C));
+  if (!packed_dev) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
+  const long long n = cb_net(M, offset, C).total;
+  if (packed_floats != n)
+    return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, the group [%d, %d) of M=%d needs %lld",
+                (long long)packed_floats, offset, offset + C, M, n);
+  TFCB_TRY(ar_check_batch(B, H, W, num_scales));
+  return cb_run(packed_dev, M, offset, C, yhat_dev, psi_dev, chctx_dev, B, H, W, anchors ? 0 : 1, num_scales,
+                work_dev, work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev, yhat_out_dev,
+                stream);
+}
+
+int tfcb_scc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int offset, int C, int anchors,
+                     float* dst_dev, void* stream) {
+  TFCB_TRY(scc_check_group(M, offset, C));
+  return cb_scatter(src_dev, B, H, W, M, offset, C, anchors ? 0 : 1, dst_dev, stream);
 }
 
 }  // extern "C"

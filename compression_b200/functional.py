@@ -1036,3 +1036,174 @@ def cb_decode(handle, packed, psi, num_scales, cdf_offset):
     part = decode_index_f32(handle, index, loc, coff)
     check(lib.tfcb_cb_scatter(_p(part), B, H, W, M, int(anchors), _p(y_hat), _stream()))
   return y_hat
+
+
+# ------------------------------------------------------------------------------------------------
+# Space-channel context model (He et al. 2022): the checkerboard passes per channel group (tfcb_scc_*).  The groups
+# (c_0, ..., c_{K-1}) split y's M channels; group k is the span (o_k, c_k), channels [o_k, o_k + c_k).  Each group
+# has its own packed network (scc_pack_weights), whose layer 1 reads [psi, the channel context of group k (none for
+# k = 0), its spatial context].  Coding order: per image, group 0's anchors, group 0's non-anchors, group 1's
+# anchors, ..., each in raster order with c_k channels per position; the coding-order tensors are [B, H * W * M].
+# ------------------------------------------------------------------------------------------------
+def scc_spans(groups):
+  """[(offset, channels), ...] of the channel counts `groups`."""
+  spans, o = [], 0
+  for c in groups:
+    spans.append((o, int(c)))
+    o += int(c)
+  return spans
+
+
+def scc_layout(M, group):
+  """The library's packed layout of group (offset, channels) of a depth-M latent: a dict of the widths K1, N3, N4,
+  the offsets of wc, bc, w1, b1, w2, b2, w3, b3 and the `total` floats."""
+  o, c = (int(v) for v in group)
+  out = (C.c_int64 * 11)()
+  n = int(_lib.lib().tfcb_scc_packed_floats(int(M), o, c, out))
+  if n < 0:
+    raise _lib.InvalidArgumentError(f"group of {c} channels at offset {o} of a latent of depth M={M}: M must be a "
+                                    "positive even number at most 1024, with every channel inside it")
+  keys = ("K1", "N3", "N4", "wc", "bc", "w1", "b1", "w2", "b2", "w3", "b3")
+  return dict(zip(keys, (int(v) for v in out)), total=n)
+
+
+def scc_pack_weights(M, group, ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
+  """The device layout of group (offset, channels)'s parameter passes: the 12 checkerboard taps of its context
+  kernel [5, 5, c, 2c] (masked or not: no other tap is read), then each 1x1 layer as [inputs, outputs] and its bias,
+  with the widths scc_layout gives.  Returns float32 [total] on the context kernel's device."""
+  o, c = (int(v) for v in group)
+  lay = scc_layout(M, group)
+  ctx_kernel = ctx_kernel.detach()
+  if tuple(ctx_kernel.shape) != (5, 5, c, 2 * c):
+    raise _lib.InvalidArgumentError(f"context kernel must be [5, 5, {c}, {2 * c}]: {tuple(ctx_kernel.shape)}")
+  dev = ctx_kernel.device
+  if dev.type != "cuda":
+    raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
+  k1, n3, n4 = lay["K1"], lay["N3"], lay["N4"]
+  want = ((ctx_bias, (2 * c,)), (w1, (k1, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, 2 * c)),
+          (b3, (2 * c,)))
+  ops = [_f32(ctx_kernel[[dy + 2 for dy, _ in CB_TAPS], [dx + 2 for _, dx in CB_TAPS]], dev)]
+  for t, shape in want:
+    t = t.detach()
+    if tuple(t.shape) != shape:
+      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where group ({o}, {c}) of M={M} needs "
+                                      f"{shape}")
+    ops.append(_f32(t, dev))
+  packed = torch.empty(lay["total"], dtype=torch.float32, device=dev)
+  check(_lib.lib().tfcb_scc_pack_weights(int(M), o, c, *[_p(t) for t in ops], _p(packed), lay["total"], _stream()))
+  return packed
+
+
+def _scc_dims(packed, group, psi):
+  """(B, H, W, M, offset, channels, packed floats) from psi [B, H, W, 2M], checked against the group's packed
+  buffer."""
+  if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
+    raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
+  B, H, W, M = int(psi.shape[0]), int(psi.shape[1]), int(psi.shape[2]), int(psi.shape[3]) // 2
+  if B == 0 or H == 0 or W == 0:
+    raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
+  o, c = (int(v) for v in group)
+  n = scc_layout(M, group)["total"]
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from scc_pack_weights")
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, group ({o}, {c}) of M={M} needs {n}")
+  if packed.device.type != "cuda" or psi.device != packed.device:
+    raise _lib.InvalidArgumentError(f"`packed` ({packed.device}) and `psi` ({psi.device}) must share a CUDA device")
+  return B, H, W, M, o, c, n
+
+
+def _scc_pass(packed, group, y_hat, psi, ch_ctx, anchors, num_scales, whole, loc, scale, index, y=None, y_cc=None,
+              y_hat_out=None):
+  B, H, W, M, o, c, n = _scc_dims(packed, group, psi)
+  lib = _lib.lib()
+  nw = int(lib.tfcb_scc_workspace_floats(M, o, c, B, H, W, int(bool(anchors))))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=packed.device)
+  check(lib.tfcb_scc_params(_p(packed), n, M, o, c, _p(y_hat), _p(psi), _p(ch_ctx), B, H, W, int(bool(anchors)),
+                            int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale), _p(index), _p(y), _p(y_cc),
+                            _p(y_hat_out), _stream()))
+
+
+def _scc_ch_ctx(ch_ctx, group, shape, dev):
+  """The channel context [B, H, W, 2c] of a group at a positive offset; None at offset 0."""
+  o, c = (int(v) for v in group)
+  if o == 0:
+    if ch_ctx is not None:
+      raise _lib.InvalidArgumentError("the group at offset 0 has no channel context: pass None")
+    return None
+  return _ar_tensor(ch_ctx, "ch_ctx", tuple(shape) + (2 * c,), dev)
+
+
+def scc_params(packed, group, y_hat, psi, ch_ctx, anchors, num_scales):
+  """One parameter pass of group (offset, channels): (loc, scale_index, index) [B, n, c] (float32, float32, int32)
+  of the n positions of one colour of every image, in coding order.  ch_ctx [B, H, W, 2c] is the group's channel
+  context (None at offset 0); the non-anchor pass reads the group's channels of the anchors of y_hat [B, H, W, M]
+  (y_hat may be None for the anchor pass).  Row b depends only on image b."""
+  B, H, W, M, o, c, _ = _scc_dims(packed, group, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  ch_ctx = _scc_ch_ctx(ch_ctx, group, (B, H, W), dev)
+  if y_hat is not None or not anchors:
+    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  n = cb_counts(H, W)[0 if anchors else 1]
+  loc = torch.empty((B, n, c), dtype=torch.float32, device=dev)
+  scale = torch.empty_like(loc)
+  index = torch.empty((B, n, c), dtype=torch.int32, device=dev)
+  _scc_pass(packed, group, y_hat, psi, ch_ctx, anchors, num_scales, False, loc, scale, index)
+  return loc, scale, index
+
+
+def _scc_batch(packed, groups, psi):
+  """(B, H, W, M, spans, psi) of a whole-latent call, with every group's packed buffer checked."""
+  if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
+    raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
+  M = int(psi.shape[3]) // 2
+  spans = scc_spans(groups)
+  if sum(c for _, c in spans) != M or len(packed) != len(spans):
+    raise _lib.InvalidArgumentError(f"{len(packed)} packed networks and groups {tuple(groups)} for a latent of depth "
+                                    f"{M}: one network per group, and the groups must sum to M")
+  for p, g in zip(packed, spans):
+    B, H, W = _scc_dims(p, g, psi)[:3]
+  return B, H, W, M, spans, _ar_tensor(psi, "psi", (B, H, W, 2 * M), psi.device)
+
+
+def scc_encode(packed, groups, y, psi, channel_context, num_scales, scale_index=False):
+  """The group-by-group encoder: `packed` holds one scc_pack_weights buffer per group.  Per group k, its channel
+  context `channel_context(k, y_hat)` [B, H, W, 2c_k] (called for k >= 1, once y_hat holds groups 0 to k - 1), the
+  anchor pass, then the non-anchor pass.  Returns y_hat [B, H, W, M] and y, loc, index in coding order
+  [B, H * W * M] (and scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc.  The
+  strings are one index-mode encode of the coding-order y with index and loc."""
+  B, H, W, M, spans, psi = _scc_batch(packed, groups, psi)
+  dev = psi.device
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
+  y_cc, loc = (torch.empty((B, H * W * M), dtype=torch.float32, device=dev) for _ in range(2))
+  index = torch.empty((B, H * W * M), dtype=torch.int32, device=dev)
+  scale = torch.empty_like(loc) if scale_index else None
+  for k, (p, g) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx(channel_context(k, y_hat) if k else None, g, (B, H, W), dev)
+    for anchors in (True, False):
+      _scc_pass(p, g, y_hat, psi, ch, anchors, num_scales, True, loc, scale, index, y, y_cc, y_hat)
+  return (y_hat, y_cc, loc, index) + ((scale,) if scale_index else ())
+
+
+def scc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_offset):
+  """The group-by-group decoder, continuing `handle` (a DecoderHandle of B index-mode strings in coding order): per
+  group its channel context (as in scc_encode), then per colour the parameter pass, decode_index_f32 and the scatter
+  into y_hat [B, H, W, M], which it returns.  2K decode calls on the handle; per group a fixed number of library
+  launches whatever B, H and W (fewer at H W = 1, where the non-anchor passes are empty), and no host
+  synchronisation; stream errors surface at entropy_decode_finalize."""
+  B, H, W, M, spans, psi = _scc_batch(packed, groups, psi)
+  dev = psi.device
+  if handle.n_streams != B:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a batch of {B}")
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for k, (p, (o, c)) in enumerate(zip(packed, spans)):
+    ch = channel_context(k, y_hat) if k else None
+    for anchors in (True, False):
+      loc, _, index = scc_params(p, (o, c), y_hat, psi, ch, anchors, num_scales)
+      part = decode_index_f32(handle, index, loc, coff)
+      check(lib.tfcb_scc_scatter(_p(part), B, H, W, M, o, c, int(anchors), _p(y_hat), _stream()))
+  return y_hat

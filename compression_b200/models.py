@@ -28,7 +28,7 @@ from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -640,6 +640,15 @@ class MBT2018Model(_Model):
     N, M = int(num_filters), int(latent_depth)
     if M <= 0 or M % 6:
       raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
+    self._init_transforms(lmbda, N, M, num_scales, scale_min, scale_max)
+    self.context_model = MaskedConv2D(M, 2 * M)
+    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
+    self.entropy_parameters = nn.Sequential(
+        ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(2 * M, "layer_2", None))
+    self._init_entropy_models(N)
+
+  def _init_transforms(self, lmbda, N, M, num_scales, scale_min, scale_max):
+    """The analysis, synthesis and hyper transforms and the scale table."""
     self.lmbda = lmbda
     self.num_filters, self.latent_depth, self.num_scales = N, M, int(num_scales)
     offset = math.log(scale_min)
@@ -655,10 +664,8 @@ class MBT2018Model(_Model):
     hs = lambda f, k, name, up, act: _conv(f, k, name, up=up, corr=False, kernel_parameter="variable", activation=act)
     self.hyper_synthesis_transform = nn.Sequential(
         hs(M, 5, "layer_0", 2, _leaky), hs(3 * M // 2, 5, "layer_1", 2, _leaky), hs(2 * M, 3, "layer_2", 1, None))
-    self.context_model = MaskedConv2D(M, 2 * M)
-    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
-    self.entropy_parameters = nn.Sequential(
-        ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(2 * M, "layer_2", None))
+
+  def _init_entropy_models(self, N):
     self.hyperprior = D.NoisyDeepFactorized(batch_shape=(N,))
     self.entropy_model = None
     self.side_entropy_model = None
@@ -702,12 +709,12 @@ class MBT2018Model(_Model):
     self.entropy_model = E.LocationScaleIndexedEntropyModel(D.NoisyNormal, self.num_scales, self.scale_fn,
                                                             coding_rank=3, compression=True).to(dev)
     self.side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3, compression=True).to(dev)
-    layers = list(self.entropy_parameters)
-    if any(not layer.built for layer in layers):
-      raise RuntimeError("the entropy-parameter layers are not built: call build() first")
-    w = [t for layer in layers for t in (layer.kernel.reshape(layer.kernel.shape[-2:]), layer.bias)]
-    self._packed = self._pack_weights(self.context_model.kernel, self.context_model.bias, *w)
+    self._packed = self._pack()
     return self
+
+  def _pack(self):
+    return self._pack_weights(self.context_model.kernel, self.context_model.bias,
+                              *_dense_weights(self.entropy_parameters))
 
   _pack_weights = staticmethod(F.ar_pack_weights)
 
@@ -806,6 +813,14 @@ class MBT2018Model(_Model):
     return self.decompress(*PackedTensors(data).unpack(dtypes))
 
 
+def _dense_weights(layers):
+  """[W1, b1, W2, b2, ...] ([inputs, outputs] and [outputs]) of a stack of built 1x1 convolutions."""
+  layers = list(layers)
+  if any(not layer.built for layer in layers):
+    raise RuntimeError("the entropy-parameter layers are not built: call build() first")
+  return [t for layer in layers for t in (layer.kernel.reshape(layer.kernel.shape[-2:]), layer.bias)]
+
+
 def checkerboard_mask(kernel_size=5):
   """[k, k]: 1 at the offsets (dy, dx) from the centre with dy + dx odd (12 for k = 5), 0 elsewhere.  Centred on a
   non-anchor, every such tap is an anchor."""
@@ -865,6 +880,89 @@ class CheckerboardModel(MBT2018Model):
     em = self.entropy_model
     handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
     y_hat = F.cb_decode(handle, self._packed, psi, self.num_scales, em.cdf_offset.to(psi.device))
+    em._finish_decode(handle)
+    return y_hat
+
+
+class SpaceChannelModel(MBT2018Model):
+  """The space-channel context model (SCCTX) of ELIC (He, Yang, Peng, Ma, Qin & Wang, CVPR 2022) on MBT2018Model's
+  analysis, synthesis and hyper transforms (psi of 2M) and entropy models.  y is split into the uneven channel
+  groups `groups` (c_0, ..., c_{K-1}), summing to M; group k holds channels [o_k, o_k + c_k).  Each group is coded
+  in two checkerboard passes (CheckerboardModel's anchors and taps), conditioned on psi, on the groups before it
+  (the channel context g_ch^k(y_hat[..., :o_k]), 2c_k wide, none for k = 0) and on its own decoded anchors (the
+  spatial context, a CheckerboardConv2D(c_k, 2c_k)).  The group's entropy parameters are three 1x1 layers with
+  LeakyReLU, K1 -> 5 K1 / 6 -> 2 K1 / 3 -> 2c_k on [psi, channel ctx, spatial ctx] of width K1 (MBT2018's ratios,
+  so with one group the widths are MBT2018's).  g_ch^k is MS2020's slice transform stack (5x5 -> 224, 5x5 -> 128,
+  3x3 -> 2c_k); in coding it runs one image at a time, so nothing depends on the batch.
+
+  Coding runs on the group passes (functional.scc_*): one string per image, the bytes of
+  `LocationScaleIndexedEntropyModel.compress(y_cc, scale_index_cc, loc_cc)` of the coding-order tensors [B, H W M]
+  (group 0's anchors, group 0's non-anchors, group 1's anchors, ..., each in raster order); the decoder makes 2K
+  decode_index_f32 calls on one decoder handle."""
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=320, groups=(16, 16, 32, 64, 192), num_scales=64,
+               scale_min=.11, scale_max=256.):
+    _Model.__init__(self)
+    N, M = int(num_filters), int(latent_depth)
+    groups = tuple(int(c) for c in groups)
+    if M <= 0 or M % 2:
+      raise ValueError(f"latent_depth must be a positive even number (3M/2 is a layer width): {M}")
+    if not groups or min(groups) < 1:
+      raise ValueError(f"every group needs at least one channel: {groups}")
+    if sum(groups) != M:
+      raise ValueError(f"the groups {groups} hold {sum(groups)} channels, but latent_depth is {M}")
+    self.groups = groups
+    self.spans = F.scc_spans(groups)
+    self._init_transforms(lmbda, N, M, num_scales, scale_min, scale_max)
+    self.context_models = nn.ModuleList([CheckerboardConv2D(c, 2 * c) for c in groups])
+    self.channel_context_transforms = nn.ModuleList([_MS2020SliceTransform(2 * c) for c in groups[1:]])
+    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
+    stacks = []
+    for k, c in enumerate(groups):
+      k1 = 2 * M + (2 * c if k else 0) + 2 * c
+      stacks.append(nn.Sequential(ep(5 * k1 // 6, "layer_0", _leaky), ep(2 * k1 // 3, "layer_1", _leaky),
+                                  ep(2 * c, "layer_2", None)))
+    self.entropy_parameters = nn.ModuleList(stacks)
+    self._init_entropy_models(N)
+
+  def entropy_parameters_of(self, y_ctx, psi):
+    """The parallel (training) form: (loc, scale_index) [B, H, W, M] of every position from the latents both
+    contexts see and psi."""
+    locs, scales = [], []
+    for k, (o, c) in enumerate(self.spans):
+      parts = [psi]
+      if k:
+        parts.append(self.channel_context_transforms[k - 1](y_ctx[..., :o]))
+      parts.append(checkerboard_context(self.context_models[k], y_ctx[..., o:o + c]))
+      params = self.entropy_parameters[k](torch.cat(parts, dim=-1))
+      locs.append(params[..., :c])
+      scales.append(params[..., c:])
+    return torch.cat(locs, dim=-1), torch.cat(scales, dim=-1)
+
+  def _channel_context(self, k, y_hat):
+    """g_ch^k of y_hat[..., :o_k] [B, H, W, 2c_k], one image at a time."""
+    o = self.spans[k][0]
+    g = self.channel_context_transforms[k - 1]
+    return torch.cat([g(y_hat[i:i + 1, ..., :o]) for i in range(y_hat.shape[0])]).contiguous()
+
+  def _pack(self):
+    M = self.latent_depth
+    return [F.scc_pack_weights(M, span, cm.kernel, cm.bias, *_dense_weights(ep))
+            for span, cm, ep in zip(self.spans, self.context_models, self.entropy_parameters)]
+
+  def _encode_latents(self, y, psi):
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H W M]."""
+    em = self.entropy_model
+    y_hat, y_cc, loc, index = F.scc_encode(self._packed, self.groups, y.contiguous(), psi, self._channel_context,
+                                           self.num_scales)
+    strings = F.compress_f32((y.shape[0],), em._lookup_host(), y_cc, loc, em.cdf_offset.to(y.device), index=index)
+    return strings, y_hat, loc, index
+
+  def _decode_latents(self, strings, psi):
+    em = self.entropy_model
+    handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
+    y_hat = F.scc_decode(handle, self._packed, self.groups, psi, self._channel_context, self.num_scales,
+                         em.cdf_offset.to(psi.device))
     em._finish_decode(handle)
     return y_hat
 

@@ -283,6 +283,48 @@ int tfcb_cb_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M
                     void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Space-channel context model (He et al. 2022): the checkerboard passes per channel group.  M = latent depth, even,
+ * at most 1024; a group is the C >= 1 channels [offset, offset + C) of y, with offset + C <= M.  Per position of a
+ * group, with CH = 0 for the group at offset 0 and CH = 2C otherwise:
+ *   ctx = 0 at an anchor, else Wc * (the group's channels of yhat at the 12 checkerboard taps) + bc   [12C] -> [2C]
+ *   h1 = leaky(W1 * [psi (2M), chctx (CH), ctx (2C)] + b1)                         [K1 = 2M + CH + 2C] -> [5 K1 / 6]
+ *   h2 = leaky(W2 * h1 + b2) -> [2 K1 / 3];  [loc, scale_index] = W3 * h2 + b3 (C each)
+ * (widths rounded down) in tfcb_ar_params' float32 order of operations; chctx [B, H, W, CH] is the caller's channel
+ * context.  At offset 0 with C = M (M a multiple of 6) this is tfcb_cb_params, bit for bit, on the same packed
+ * layout.  Coding order of all groups: per image, group 0's anchors, group 0's non-anchors, group 1's anchors, ...,
+ * each in raster order with C channels per position: [B, H W M] in all.
+ * ---------------------------------------------------------------------------------------------- */
+/* Floats of one group's packed parameters, or -1 if the group is not supported.  If `layout` is not NULL it receives
+ * 11 values: the widths K1, N3, N4, then the offsets of Wc [12, C, 2C], bc [2C], W1 [K1, N3], b1, W2 [N3, N4], b2,
+ * W3 [N4, 2C] and b3 (inputs x outputs, row major); the buffer ends at the returned size. */
+int64_t tfcb_scc_packed_floats(int M, int offset, int C, int64_t* layout);
+/* Packs one group's parameters into `packed_dev`, stream-ordered device copies of the values unchanged, the
+ * context taps already gathered as [12, C, 2C] in raster order of the taps. */
+int tfcb_scc_pack_weights(int M, int offset, int C, const float* ctx_taps_dev, const float* ctx_bias_dev,
+                          const float* w1_dev, const float* b1_dev, const float* w2_dev, const float* b2_dev,
+                          const float* w3_dev, const float* b3_dev, float* packed_dev, int64_t packed_floats,
+                          void* stream);
+/* Floats of workspace one tfcb_scc_params pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_scc_workspace_floats(int M, int offset, int C, int64_t B, int64_t H, int64_t W, int anchors);
+/* One pass over every position of one colour of one group of all B images; tfcb_cb_params' arguments, plus the
+ * group and `chctx_dev` [B, H, W, 2C] (required unless offset is 0).  The non-anchor pass reads the group's
+ * channels of the anchors of `yhat_dev` [B, H, W, M].  Writes loc, scale_index and the table index (each may be
+ * NULL): [B, n, C] with n the positions of this colour (whole == 0), or [B, H W M] in the coding order of all groups
+ * at this pass's block (whole != 0).  Encoder epilogue (y_dev not NULL, [B, H, W, M]): also writes the group's y in
+ * coding order to `y_cb_dev` (same layout as loc) and yhat = float(int32(rint(y - loc))) + loc at this colour's
+ * positions and the group's channels of `yhat_out_dev` [B, H, W, M]; loc and index are then required.  Three
+ * launches for the anchors, four for the non-anchors, none for an empty pass; no host synchronisation. */
+int tfcb_scc_params(const float* packed_dev, int64_t packed_floats, int M, int offset, int C, const float* yhat_dev,
+                    const float* psi_dev, const float* chctx_dev, int64_t B, int64_t H, int64_t W, int anchors,
+                    int num_scales, float* work_dev, int64_t work_floats, int whole, float* loc_dev,
+                    float* scale_index_dev, int32_t* index_dev, const float* y_dev, float* y_cb_dev,
+                    float* yhat_out_dev, void* stream);
+/* Moves one colour of one group from coding order [B, n, C] to its positions and channels of `dst_dev`
+ * [B, H, W, M] (nothing else is written).  One launch; none when the colour has no positions. */
+int tfcb_scc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int offset, int C, int anchors,
+                     float* dst_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Legacy single-stream ops RangeEncode / RangeDecode (int16 data, broadcastable N-D int32 CDF):
  *   op contract   tensorflow_compression/cc/ops/range_coding_ops.cc:30-124
  *   CPU kernels   tensorflow_compression/cc/kernels/range_coding_kernels.cc:60-379
