@@ -73,6 +73,10 @@ SIGNATURES = {
     "tfcb_ar_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp]),
     "tfcb_ar_encode": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp, _vp, _vp]),
     "tfcb_ar_decode": (_int, [_vp, _vp, _i64, _int, _vp, _i64, _i64, _i64, _i64, _i64, _int, _vp, _vp, _vp]),
+    "tfcb_ar_ragged_workspace_floats": (_i64, [_i64]),
+    "tfcb_ar_encode_ragged": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _vp, _vp, _int, _vp, _i64, _vp, _vp, _vp, _vp,
+                                     _vp]),
+    "tfcb_ar_decode_ragged": (_int, [_vp, _vp, _i64, _int, _vp, _i64, _vp, _vp, _int, _vp, _vp, _i64, _vp, _vp]),
     "tfcb_cb_workspace_floats": (_i64, [_int, _i64, _i64, _i64, _int]),
     "tfcb_cb_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64, _int, _vp, _vp, _vp,
                               _vp, _vp, _vp, _vp]),
@@ -83,6 +87,10 @@ SIGNATURES = {
     "tfcb_scc_params": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64,
                                _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tfcb_scc_scatter": (_int, [_vp, _i64, _i64, _i64, _int, _int, _int, _int, _vp, _vp]),
+    "tfcb_scc_ragged_workspace_floats": (_i64, [_int, _int, _int, _i64, _vp, _vp, _int]),
+    "tfcb_scc_params_ragged": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp,
+                                      _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_scc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _int, _int, _vp, _i64, _vp, _vp]),
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_range_decode": (_int, [_vp, _i64, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),

@@ -21,6 +21,8 @@
 //   in increasing k starting from 0.f, where K is the layer's input width.
 #include <cuda_runtime.h>
 
+#include <vector>
+
 #include "autoregressive.cuh"
 #include "common.cuh"
 #include "range_decoder.cuh"
@@ -36,6 +38,12 @@ enum : int { kArParams = 0, kArEncode = 1, kArDecode = 2 };
 __host__ __device__ inline long long ar_act_floats(const ArDims& d) {
   return (long long)kArTaps * d.M + 2ll * d.N2 + d.N3 + d.N4 + d.N2 + (long long)kArSlices * d.N3;
 }
+
+// One image of a ragged list: its first pixel P_i (its elements start at M P_i) and its shape.
+struct ArImage {
+  long long pix;
+  int H, W;
+};
 
 struct ArParams {
   const float* packed;
@@ -56,6 +64,7 @@ struct ArParams {
   const uint8_t* bytes;
   const long long* offsets;
   DecState* state;
+  const ArImage* img;  // ragged list: CTA b runs every position of image b (§3.13)
 };
 
 // out[j] for j < nout, in the fixed order of the file comment.  `in` and `out` are shared; W is [nin][nout].
@@ -82,14 +91,20 @@ __device__ __forceinline__ void ar_dense(const float* in, int nin, const float* 
   __syncthreads();
 }
 
-template <int MODE, bool SMEM_KEYS>
-__global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
+// The CTA of image b: positions [P.p0, P.p1) of B images of P.H × P.W, or (RAGGED) every position of image b of the
+// list P.img.
+template <int MODE, bool SMEM_KEYS, bool RAGGED>
+__device__ __forceinline__ void ar_body(const ArParams& P) {
   extern __shared__ __align__(16) float s_act[];
   __shared__ __align__(16) uint16_t ring_buf[2 * kRing];  // decoder only: 4096-byte aligned ring, as decode_kernel
   const ArDims d = ar_dims(P.M);
   const int M = P.M;
   const long long b = blockIdx.x;
   const long long HW = (long long)P.H * P.W;
+  // a ragged list's image b (the fixed-shape arithmetic below is left exactly as it was when RAGGED is false)
+  ArImage im{};
+  if (RAGGED) im = P.img[b];
+  const long long pix0 = RAGGED ? im.pix : b * HW;  // the image's first pixel
   float* const taps = s_act;                    // [12M]
   float* const x1 = taps + kArTaps * M;         // [4M]: ψ then ctx
   float* const h1 = x1 + 2 * d.N2;              // [N3]
@@ -139,18 +154,19 @@ __global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
     }
   }
 
-  for (int p = P.p0; p < P.p1; ++p) {
-    const int py = p / P.W, px = p - py * P.W;
+  for (int p = RAGGED ? 0 : P.p0; p < (RAGGED ? im.H * im.W : P.p1); ++p) {
+    const int py = p / (RAGGED ? im.W : P.W), px = p - py * (RAGGED ? im.W : P.W);
     // ---- gather: the 12 causal neighbours of p (zeros outside the image) and ψ_p ----
-    const float* yimg = P.yhat + b * HW * M;
+    const float* yimg = P.yhat + (RAGGED ? pix0 * M : b * HW * M);
     for (int i = threadIdx.x; i < kArTaps * M; i += blockDim.x) {
       const int t = i / M, ch = i - t * M;
       const int yy = py + t / 5 - 2, xx = px + t % 5 - 2;
       float v = 0.f;
-      if (yy >= 0 && xx >= 0 && xx < P.W) v = yimg[((long long)yy * P.W + xx) * M + ch];  // (yy <= py always)
+      if (yy >= 0 && xx >= 0 && xx < (RAGGED ? im.W : P.W))
+        v = yimg[((long long)yy * (RAGGED ? im.W : P.W) + xx) * M + ch];  // (yy <= py always)
       taps[i] = v;
     }
-    const float* psi = P.psi + (b * HW + p) * d.N2;
+    const float* psi = P.psi + (RAGGED ? pix0 + p : b * HW + p) * d.N2;
     for (int i = threadIdx.x; i < d.N2; i += blockDim.x) x1[i] = __ldg(psi + i);
     __syncthreads();
     // ---- context model and entropy parameters ----
@@ -159,7 +175,7 @@ __global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
     ar_dense(h1, d.N3, Wp + d.w2, Wp + d.b2, d.N4, part, h2, true);
     ar_dense(h2, d.N4, Wp + d.w3, Wp + d.b3, d.N2, part, out, false);
     // ---- epilogue ----
-    const long long row = (MODE == kArParams) ? b * M : (b * HW + p) * M;
+    const long long row = (MODE == kArParams) ? b * M : (RAGGED ? pix0 + p : b * HW + p) * M;
     if (MODE != kArDecode) {
       for (int ch = threadIdx.x; ch < M; ch += blockDim.x) {
         const float loc = out[ch], sc = out[M + ch];
@@ -220,8 +236,19 @@ __global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
 }
 
 template <int MODE, bool SMEM_KEYS>
+__global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
+  ar_body<MODE, SMEM_KEYS, false>(P);
+}
+
+template <int MODE, bool SMEM_KEYS>
+__global__ void __launch_bounds__(kArThreads) ar_ragged_kernel(const ArParams P) {
+  ar_body<MODE, SMEM_KEYS, true>(P);
+}
+
+template <int MODE, bool SMEM_KEYS, bool RAGGED = false>
 int ar_launch(const ArParams& P, long long B, size_t smem, cudaStream_t s) {
   auto kern = ar_kernel<MODE, SMEM_KEYS>;
+  if constexpr (RAGGED) kern = ar_ragged_kernel<MODE, SMEM_KEYS>;
   TFCB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<(unsigned)B, kArThreads, smem, s>>>(P);
   TFCB_LAUNCHED();
@@ -232,6 +259,53 @@ int ar_launch(const ArParams& P, long long B, size_t smem, cudaStream_t s) {
 constexpr size_t kArSmemLimit = 200 * 1024;  // dynamic shared memory beside the 8 KB ring (227 KB per CTA)
 
 size_t ar_act_bytes(int M) { return (size_t)ar_act_floats(ar_dims(M)) * sizeof(float); }
+
+constexpr long long kArImageFloats = sizeof(ArImage) / sizeof(float);
+
+// Checks the workspace and uploads a ragged list's image table to it (one stream-ordered copy from pageable memory,
+// staged before the call returns).
+int ar_upload_table(int64_t n, const int64_t* hs, const int64_t* ws, float* work, int64_t work_floats, ArParams* P,
+                    cudaStream_t s) {
+  TFCB_TRY(ar_check_table_space(work, work_floats, n * kArImageFloats, alignof(ArImage)));
+  std::vector<ArImage> t((size_t)n);
+  long long pix = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    t[i] = {pix, (int)hs[i], (int)ws[i]};
+    pix += hs[i] * ws[i];
+  }
+  TFCB_CUDA_TRY(cudaMemcpyAsync(work, t.data(), t.size() * sizeof(ArImage), cudaMemcpyHostToDevice, s));
+  P->img = reinterpret_cast<const ArImage*>(work);
+  return TFCB_OK;
+}
+
+// The decoder's launch: search keys in shared memory when they fit beside the activations (64 NoisyNormal tables:
+// 118 KB).
+template <bool RAGGED>
+int ar_launch_decode(const ArParams& P, const DecoderView& v, long long B, cudaStream_t s) {
+  const size_t act = ar_act_bytes(P.M);
+  const size_t keys = (size_t)((v.n_pairs * 8 + 15) & ~15ll) + (size_t)v.n_rows * sizeof(int4);
+  if (act + keys <= kArSmemLimit) return ar_launch<kArDecode, true, RAGGED>(P, B, act + keys, s);
+  return ar_launch<kArDecode, false, RAGGED>(P, B, act, s);
+}
+
+void ar_set_decoder(const DecoderView& v, ArParams* P) {
+  P->pairs = v.pairs;
+  P->rows4 = v.rows4;
+  P->n_rows = v.n_rows;
+  P->n_pairs = v.n_pairs;
+  P->bytes = v.bytes;
+  P->offsets = v.offsets;
+  P->state = v.state;
+}
+
+int ar_check_decoder(const DecoderView& v, int64_t B, int num_scales) {
+  if (v.n_streams != B)
+    return fail(TFCB_INVALID_ARGUMENT, "the decoder holds %lld strings for a batch of %lld", v.n_streams,
+                (long long)B);
+  if (v.n_rows < num_scales)
+    return fail(TFCB_INVALID_ARGUMENT, "the decoder's tables have %d rows for num_scales=%d", v.n_rows, num_scales);
+  return TFCB_OK;
+}
 
 }  // namespace
 }  // namespace tfcb
@@ -315,11 +389,7 @@ int tfcb_ar_decode(tfcb_decoder* h, const float* packed_dev, int64_t packed_floa
   TFCB_TRY(decoder_view(h, &v));
   TFCB_TRY(ar_check(M, packed_dev, packed_floats, B, H, W, num_scales));
   TFCB_TRY(ar_check_range(p_begin, p_end, H, W));
-  if (v.n_streams != B)
-    return fail(TFCB_INVALID_ARGUMENT, "the decoder holds %lld strings for a batch of %lld", v.n_streams,
-                (long long)B);
-  if (v.n_rows < num_scales)
-    return fail(TFCB_INVALID_ARGUMENT, "the decoder's tables have %d rows for num_scales=%d", v.n_rows, num_scales);
+  TFCB_TRY(ar_check_decoder(v, B, num_scales));
   if (!psi_dev || !yhat_dev || !cdf_offset_dev)
     return fail(TFCB_INVALID_ARGUMENT, "`psi`, `yhat` or `cdf_offset` is null");
   if (p_begin == p_end) return TFCB_OK;
@@ -334,19 +404,60 @@ int tfcb_ar_decode(tfcb_decoder* h, const float* packed_dev, int64_t packed_floa
   P.num_scales = num_scales;
   P.p0 = (int)p_begin;
   P.p1 = (int)p_end;
-  P.pairs = v.pairs;
-  P.rows4 = v.rows4;
-  P.n_rows = v.n_rows;
-  P.n_pairs = v.n_pairs;
-  P.bytes = v.bytes;
-  P.offsets = v.offsets;
-  P.state = v.state;
-  // search keys in shared memory when they fit beside the activations (64 NoisyNormal tables: 118 KB)
-  const size_t act = ar_act_bytes(M);
-  const size_t keys = (size_t)((v.n_pairs * 8 + 15) & ~15ll) + (size_t)v.n_rows * sizeof(int4);
+  ar_set_decoder(v, &P);
+  return ar_launch_decode<false>(P, v, B, as_stream(stream));
+}
+
+int64_t tfcb_ar_ragged_workspace_floats(int64_t n_images) {
+  if (n_images <= 0 || n_images > 0x7FFFFFFF) return -1;
+  return n_images * kArImageFloats;
+}
+
+int tfcb_ar_encode_ragged(const float* packed_dev, int64_t packed_floats, int M, const float* y_dev,
+                          const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                          const int64_t* widths_host, int num_scales, float* work_dev, int64_t work_floats,
+                          float* yhat_dev, float* loc_dev, int32_t* index_dev, float* scale_index_dev, void* stream) {
+  TFCB_TRY(ar_check_packed(M, packed_dev, packed_floats));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, num_scales));
+  if (!y_dev || !psi_dev || !yhat_dev || !loc_dev || !index_dev)
+    return fail(TFCB_INVALID_ARGUMENT, "`y`, `psi`, `yhat`, `loc` or `index` is null");
+  ArParams P{};
+  P.packed = packed_dev;
+  P.psi = psi_dev;
+  P.y = y_dev;
+  P.yhat = yhat_dev;
+  P.loc_out = loc_dev;
+  P.scale_out = scale_index_dev;
+  P.index_out = index_dev;
+  P.M = M;
+  P.num_scales = num_scales;
   cudaStream_t s = as_stream(stream);
-  if (act + keys <= kArSmemLimit) return ar_launch<kArDecode, true>(P, B, act + keys, s);
-  return ar_launch<kArDecode, false>(P, B, act, s);
+  TFCB_TRY(ar_upload_table(n_images, heights_host, widths_host, work_dev, work_floats, &P, s));
+  return ar_launch<kArEncode, false, true>(P, n_images, ar_act_bytes(M), s);
+}
+
+int tfcb_ar_decode_ragged(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
+                          int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int num_scales,
+                          const int32_t* cdf_offset_dev, float* work_dev, int64_t work_floats, float* yhat_dev,
+                          void* stream) {
+  DecoderView v;
+  TFCB_TRY(decoder_view(h, &v));
+  TFCB_TRY(ar_check_packed(M, packed_dev, packed_floats));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, num_scales));
+  TFCB_TRY(ar_check_decoder(v, n_images, num_scales));
+  if (!psi_dev || !yhat_dev || !cdf_offset_dev)
+    return fail(TFCB_INVALID_ARGUMENT, "`psi`, `yhat` or `cdf_offset` is null");
+  ArParams P{};
+  P.packed = packed_dev;
+  P.psi = psi_dev;
+  P.yhat = yhat_dev;
+  P.cdf_offset = cdf_offset_dev;
+  P.M = M;
+  P.num_scales = num_scales;
+  ar_set_decoder(v, &P);
+  cudaStream_t s = as_stream(stream);
+  TFCB_TRY(ar_upload_table(n_images, heights_host, widths_host, work_dev, work_floats, &P, s));
+  return ar_launch_decode<true>(P, v, n_images, s);
 }
 
 }  // extern "C"

@@ -7,6 +7,8 @@
 
 #include <cuda_runtime.h>
 
+#include <cstdint>
+
 #include "common.cuh"
 
 namespace tfcb {
@@ -56,7 +58,29 @@ int ar_check_batch(int64_t B, int64_t H, int64_t W, int num_scales) {
   return TFCB_OK;
 }
 
-int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64_t H, int64_t W, int num_scales) {
+// A latent shape of a ragged list: positive sides and H W <= 2^31 - 1.
+bool ar_shape_ok(int64_t H, int64_t W) { return H > 0 && W > 0 && H <= 0x7FFFFFFF && W <= 0x7FFFFFFF / H; }
+
+bool ar_list_ok(int64_t n, const int64_t* hs, const int64_t* ws) {
+  if (n <= 0 || n > 0x7FFFFFFF || !hs || !ws) return false;
+  for (int64_t i = 0; i < n; ++i)
+    if (!ar_shape_ok(hs[i], ws[i])) return false;
+  return true;
+}
+
+// A ragged list of n images of latent shapes hs[i] x ws[i] (host arrays) and num_scales.
+int ar_check_list(int64_t n, const int64_t* hs, const int64_t* ws, int num_scales) {
+  if (n <= 0 || n > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "a list of %lld images", (long long)n);
+  if (!hs || !ws) return fail(TFCB_INVALID_ARGUMENT, "`heights` or `widths` is null");
+  for (int64_t i = 0; i < n; ++i)
+    if (!ar_shape_ok(hs[i], ws[i]))
+      return fail(TFCB_INVALID_ARGUMENT, "image %lld: latent shape %lld x %lld out of range", (long long)i,
+                  (long long)hs[i], (long long)ws[i]);
+  if (num_scales < 1) return fail(TFCB_INVALID_ARGUMENT, "num_scales=%d must be positive", num_scales);
+  return TFCB_OK;
+}
+
+int ar_check_packed(int M, const float* packed, int64_t packed_floats) {
   if (M <= 0 || M % 6 != 0 || M > kArMaxM)
     return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be a positive multiple of 6 and at most %d", M,
                 kArMaxM);
@@ -64,7 +88,22 @@ int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64
   if (packed_floats != ar_dims(M).total)
     return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, M=%d needs %lld", (long long)packed_floats,
                 M, (long long)ar_dims(M).total);
+  return TFCB_OK;
+}
+
+int ar_check(int M, const float* packed, int64_t packed_floats, int64_t B, int64_t H, int64_t W, int num_scales) {
+  TFCB_TRY(ar_check_packed(M, packed, packed_floats));
   return ar_check_batch(B, H, W, num_scales);
+}
+
+// A ragged list's per-image table, at least `need` floats of workspace: null and misaligned workspaces are refused.
+int ar_check_table_space(const void* work, int64_t work_floats, long long need, size_t align) {
+  if (!work || work_floats < need)
+    return fail(TFCB_INVALID_ARGUMENT, "workspace of %lld floats, this call needs %lld",
+                work ? (long long)work_floats : 0ll, need);
+  if (reinterpret_cast<uintptr_t>(work) % align)
+    return fail(TFCB_INVALID_ARGUMENT, "the workspace must be %d-byte aligned", (int)align);
+  return TFCB_OK;
 }
 
 // Stream-ordered device copies of the eight weight operands (context weights, bias, W1, b1, W2, b2, W3, b3) into

@@ -30,6 +30,8 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstdint>
+#include <vector>
 
 #include "autoregressive.cuh"
 #include "common.cuh"
@@ -49,9 +51,18 @@ __constant__ int8_t c_cb_dx[kArTaps] = {-1, 1, -2, 0, 2, -1, 1, -2, 0, 2, -1, 1}
 enum : int { kInTaps = 0, kInPsiCtx = 1, kInPlain = 2 };  // what a layer reads
 enum : int { kOutHidden = 0, kOutParams = 1 };             // what it writes
 
+// One image of a ragged list (§3.13): its first position of this pass (Q_i), its first pixel (P_i), its shape and
+// the first element of its params outputs.
+struct CbImage {
+  long long q, pix, out;
+  int H, W;
+};
+
 struct CbPass {
   int B, H, W, M, C, o, CH, colour, num_scales;  // latent depth M; the group's C channels from o; CH: chctx width
-  long long n_k, HW, P;                          // positions of this colour per image, H·W, B·n_k
+  long long n_k, HW, P;                          // positions of this colour per image, H·W, B·n_k (ragged: Σ n_k,i)
+  const CbImage* img;                            // a ragged list of n_img images, or null: B images of H × W
+  int n_img;
   const float* psi;                              // [B, H, W, 2M]
   const float* chctx;                            // [B, H, W, CH] (CH > 0)
   const float* yhat;                             // [B, H, W, M]: the non-anchor pass gathers the anchors' ŷ
@@ -115,6 +126,20 @@ __host__ __device__ inline void cb_position(long long j, int W, int k, int* r, i
   }
 }
 
+// the image of a ragged list holding the pass's position p: the last i with img[i].q <= p (an image with no
+// positions of this pass shares its q with the next one and is never chosen)
+__device__ inline int cb_image_of(const CbImage* img, int n_img, long long p) {
+  int lo = 0, hi = n_img - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&img[mid].q) <= p)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  return lo;
+}
+
 template <int IN, int OUT>
 __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, const CbLayer L) {
   __shared__ __align__(16) float xs[kCbKC][kCbTP + 4];  // (+4: a stage's stores hit 8 banks, rows stay 16-byte aligned)
@@ -122,23 +147,35 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
   __shared__ long long s_pix[kCbTP];  // b·H·W + r·W + c, or -1 past the last position
   __shared__ long long s_row[kCbTP];  // the position's first element of the params outputs
   __shared__ int s_r[kCbTP], s_c[kCbTP];
+  __shared__ int s_h[kCbTP], s_w[kCbTP];  // the position's image shape (a tile may straddle images of a list)
   const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
   const long long p0 = (long long)blockIdx.x * kCbTP;
   const int j0 = blockIdx.y * kCbTN;
   if (tid < kCbTP) {
     const long long p = p0 + tid;
     long long pix = -1, row = 0;
-    int r = 0, c = 0;
+    int r = 0, c = 0, h = S.H, w = S.W;
     if (p < S.P) {
-      const long long b = p / S.n_k;
-      cb_position(p - b * S.n_k, S.W, S.colour, &r, &c);
-      pix = b * S.HW + (long long)r * S.W + c;
-      row = b * S.out_stride + S.out_base + (p - b * S.n_k) * S.C;
+      if (S.img) {
+        const CbImage im = S.img[cb_image_of(S.img, S.n_img, p)];
+        h = im.H;
+        w = im.W;
+        cb_position(p - im.q, w, S.colour, &r, &c);
+        pix = im.pix + (long long)r * w + c;
+        row = im.out + (p - im.q) * S.C;
+      } else {
+        const long long b = p / S.n_k;
+        cb_position(p - b * S.n_k, S.W, S.colour, &r, &c);
+        pix = b * S.HW + (long long)r * S.W + c;
+        row = b * S.out_stride + S.out_base + (p - b * S.n_k) * S.C;
+      }
     }
     s_pix[tid] = pix;
     s_row[tid] = row;
     s_r[tid] = r;
     s_c[tid] = c;
+    s_h[tid] = h;
+    s_w[tid] = w;
   }
   __syncthreads();
   const int K = L.K, N = L.N, C = S.C;
@@ -174,9 +211,9 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
           const int k = kc + kk;
           if (IN == kInTaps) {
             const int t = k / C, ch = k - t * C;
-            const int rr = s_r[pp] + c_cb_dy[t], cc = s_c[pp] + c_cb_dx[t];
-            if (rr >= 0 && rr < S.H && cc >= 0 && cc < S.W)
-              x = S.yhat[(pix + (long long)c_cb_dy[t] * S.W + c_cb_dx[t]) * S.M + S.o + ch];
+            const int rr = s_r[pp] + c_cb_dy[t], cc = s_c[pp] + c_cb_dx[t], w = s_w[pp];
+            if (rr >= 0 && rr < s_h[pp] && cc >= 0 && cc < w)
+              x = S.yhat[(pix + (long long)c_cb_dy[t] * w + c_cb_dx[t]) * S.M + S.o + ch];
           } else if (IN == kInPsiCtx) {
             const int PW = 2 * S.M, CH = S.CH;
             if (k < PW)
@@ -246,23 +283,71 @@ __global__ void __launch_bounds__(kCbThreads) cb_dense_kernel(const CbPass S, co
   }
 }
 
-// ŷ of one colour of group [o, o + C), [B, n_k, C] in coding order -> its positions and channels of [B, H, W, M]
+// ŷ of one colour of group [o, o + C), [B, n_k, C] in coding order -> its positions and channels of [B, H, W, M];
+// with `img` (a ragged list of n_img images) image i's n_k,i C values at C q_i -> its [H_i, W_i, M] at M pix_i
 __global__ void cb_scatter_kernel(const float* __restrict__ src, float* __restrict__ dst, long long n_k, int W,
-                                  long long HW, int M, int o, int C, int colour, long long total) {
+                                  long long HW, int M, int o, int C, int colour, long long total,
+                                  const CbImage* __restrict__ img, int n_img) {
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const long long row = e / C, b = row / n_k;
+    const long long row = e / C;
     int r, c;
-    cb_position(row - b * n_k, W, colour, &r, &c);
-    dst[(b * HW + (long long)r * W + c) * M + o + (e - row * C)] = src[e];
+    long long pix;
+    if (img) {
+      const CbImage im = img[cb_image_of(img, n_img, row)];
+      cb_position(row - im.q, im.W, colour, &r, &c);
+      pix = im.pix + (long long)r * im.W + c;
+    } else {
+      const long long b = row / n_k;
+      cb_position(row - b * n_k, W, colour, &r, &c);
+      pix = b * HW + (long long)r * W + c;
+    }
+    dst[pix * M + o + (e - row * C)] = src[e];
   }
 }
 
 constexpr int kSccMaxM = 1024;
 
+// The images of a call: B of H × W (hs null), or a ragged list of B images of hs[i] × ws[i] (§3.13).
+struct CbList {
+  int64_t B, H, W;
+  const int64_t* hs;
+  const int64_t* ws;
+};
+
 long long cb_count(int64_t H, int64_t W, int colour) { return colour ? H * W / 2 : (H * W + 1) / 2; }
 
-long long cb_work_floats(const CbNet& d, int64_t B, int64_t H, int64_t W, int colour) {
-  return B * cb_count(H, W, colour) * ((colour ? 2 * d.C : 0) + d.N3 + d.N4);
+// floats of a ragged list's image table at the start of the workspace
+long long cb_table_floats(const CbList& L) { return L.hs ? L.B * (long long)(sizeof(CbImage) / sizeof(float)) : 0; }
+
+long long cb_positions(const CbList& L, int colour) {
+  if (!L.hs) return L.B * cb_count(L.H, L.W, colour);
+  long long n = 0;
+  for (int64_t i = 0; i < L.B; ++i) n += cb_count(L.hs[i], L.ws[i], colour);
+  return n;
+}
+
+long long cb_work_floats(const CbNet& d, const CbList& L, int colour) {
+  return cb_table_floats(L) + cb_positions(L, colour) * ((colour ? 2 * d.C : 0) + d.N3 + d.N4);
+}
+
+// Uploads the image table of colour `colour` of group [o, o + C) of a ragged list to `work` (one stream-ordered copy
+// from pageable memory, staged before the call returns).  Params outputs of image i start at C Q_i (whole == 0), or at
+// M P_i + H_i W_i o + (colour ? n_a,i C : 0) in the coding order of every group (whole != 0).
+int cb_upload_table(const CbList& L, int M, int o, int C, int colour, int whole, float* work, cudaStream_t s) {
+  std::vector<CbImage> t((size_t)L.B);
+  long long q = 0, pix = 0;
+  for (int64_t i = 0; i < L.B; ++i) {
+    const int64_t H = L.hs[i], W = L.ws[i];
+    t[i].q = q;
+    t[i].pix = pix;
+    t[i].out = whole ? M * pix + H * W * o + (colour ? cb_count(H, W, 0) * C : 0) : C * q;
+    t[i].H = (int)H;
+    t[i].W = (int)W;
+    q += cb_count(H, W, colour);
+    pix += H * W;
+  }
+  TFCB_CUDA_TRY(cudaMemcpyAsync(work, t.data(), t.size() * sizeof(CbImage), cudaMemcpyHostToDevice, s));
+  return TFCB_OK;
 }
 
 bool scc_group_ok(int M, int o, int C) { return M > 0 && M % 2 == 0 && M <= kSccMaxM && o >= 0 && C >= 1 && o + C <= M; }
@@ -272,6 +357,15 @@ int scc_check_group(int M, int o, int C) {
     return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be a positive even number and at most %d", M, kSccMaxM);
   if (o < 0 || C < 1 || o + C > M)
     return fail(TFCB_INVALID_ARGUMENT, "group of %d channels at offset %d does not fit a latent of depth %d", C, o, M);
+  return TFCB_OK;
+}
+
+int scc_check_packed(const float* packed, int64_t packed_floats, int M, int o, int C) {
+  if (!packed) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
+  const long long n = cb_net(M, o, C).total;
+  if (packed_floats != n)
+    return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, the group [%d, %d) of M=%d needs %lld",
+                (long long)packed_floats, o, o + C, M, n);
   return TFCB_OK;
 }
 
@@ -285,51 +379,60 @@ int cb_layer(const CbPass& S, const CbLayer& L, cudaStream_t s) {
 }
 
 // One pass over colour `colour` of group [o, o + C) of a latent of depth M, after the caller's checks of M, the group,
-// the packed size, B, H, W and num_scales.  Outputs [B, n_k, C] (whole == 0), or the coding order of every group,
-// [B, H W M], at this pass's block H W o + (colour ? n_a C : 0) (whole != 0).
+// the packed size, the images and num_scales.  Outputs [B, n_k, C] (whole == 0), or the coding order of every group,
+// [B, H W M], at this pass's block H W o + (colour ? n_a C : 0) (whole != 0); for a ragged list, image by image at the
+// offsets of cb_upload_table.
 int cb_run(const float* packed, int M, int o, int C, const float* yhat, const float* psi, const float* chctx,
-           int64_t B, int64_t H, int64_t W, int colour, int num_scales, float* work, int64_t work_floats, int whole,
-           float* loc, float* scale, int32_t* index, const float* y, float* y_cb, float* yhat_out, void* stream) {
+           const CbList& I, int colour, int num_scales, float* work, int64_t work_floats, int whole, float* loc,
+           float* scale, int32_t* index, const float* y, float* y_cb, float* yhat_out, void* stream) {
   if (!psi || (colour && !yhat)) return fail(TFCB_INVALID_ARGUMENT, "`psi` or `yhat` is null");
   if (o > 0 && !chctx)
     return fail(TFCB_INVALID_ARGUMENT, "`chctx` is null: the group at channel offset %d needs its channel context", o);
   const CbNet d = cb_net(M, o, C);
-  const long long need = cb_work_floats(d, B, H, W, colour);
+  const long long need = cb_work_floats(d, I, colour);
   if (!work || work_floats < need)
     return fail(TFCB_INVALID_ARGUMENT, "workspace of %lld floats, this pass needs %lld", work ? (long long)work_floats : 0ll,
                 need);
+  if (I.hs) TFCB_TRY(ar_check_table_space(work, work_floats, need, alignof(CbImage)));
   if (y && (!y_cb || !yhat_out || !loc || !index))
     return fail(TFCB_INVALID_ARGUMENT, "the encoder needs `y_cb`, `yhat_out`, `loc` and `index`");
-  const long long n_k = cb_count(H, W, colour);
-  if (n_k == 0) return TFCB_OK;
+  const long long P = cb_positions(I, colour);
+  if (P == 0) return TFCB_OK;
+  cudaStream_t s = as_stream(stream);
   CbPass S{};
-  S.B = (int)B;
-  S.H = (int)H;
-  S.W = (int)W;
+  S.B = (int)I.B;
   S.M = M;
   S.C = C;
   S.o = o;
   S.CH = o > 0 ? 2 * C : 0;
   S.colour = colour;
   S.num_scales = num_scales;
-  S.n_k = n_k;
-  S.HW = H * W;
-  S.P = B * n_k;
+  S.P = P;
+  if (I.hs) {
+    TFCB_TRY(cb_upload_table(I, M, o, C, colour, whole, work, s));
+    S.img = reinterpret_cast<const CbImage*>(work);
+    S.n_img = (int)I.B;
+  } else {
+    const long long n_k = cb_count(I.H, I.W, colour);
+    S.H = (int)I.H;
+    S.W = (int)I.W;
+    S.n_k = n_k;
+    S.HW = I.H * I.W;
+    S.out_stride = whole ? S.HW * M : n_k * C;
+    S.out_base = whole ? S.HW * o + (colour ? cb_count(I.H, I.W, 0) * C : 0) : 0;
+  }
   S.psi = psi;
   S.chctx = chctx;
   S.yhat = yhat;
-  S.out_stride = whole ? S.HW * M : n_k * C;
-  S.out_base = whole ? S.HW * o + (colour ? cb_count(H, W, 0) * C : 0) : 0;
   S.loc = loc;
   S.scale = scale;
   S.index = index;
   S.y = y;
   S.y_cb = y_cb;
   S.yhat_out = yhat_out;
-  float* ctx = work;
+  float* ctx = work + cb_table_floats(I);
   float* h1 = ctx + (colour ? S.P * 2 * C : 0);
   float* h2 = h1 + S.P * d.N3;
-  cudaStream_t s = as_stream(stream);
   if (colour)
     TFCB_TRY((cb_layer<kInTaps, kOutHidden>(
         S, {packed + d.wc, packed + d.bc, nullptr, ctx, kArTaps * C, 2 * C, kArTaps * C, false}, s)));
@@ -339,17 +442,30 @@ int cb_run(const float* packed, int M, int o, int C, const float* yhat, const fl
   return cb_layer<kInPlain, kOutParams>(S, {packed + d.w3, packed + d.b3, h2, nullptr, d.N4, 2 * C, d.N4, false}, s);
 }
 
-int cb_scatter(const float* src, int64_t B, int64_t H, int64_t W, int M, int o, int C, int colour, float* dst,
-               void* stream) {
-  if (B <= 0 || B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)B);
-  if (H <= 0 || W <= 0 || H * W > 0x7FFFFFFF)
-    return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)H, (long long)W);
-  const long long n_k = cb_count(H, W, colour), total = B * n_k * C;
+// The scatter of one colour of group [o, o + C), after the caller's checks of the group and (for a ragged list) the
+// images; a ragged list's table goes to `work`.
+int cb_scatter(const float* src, const CbList& I, int M, int o, int C, int colour, float* dst, float* work,
+               int64_t work_floats, void* stream) {
+  if (!I.hs) {
+    if (I.B <= 0 || I.B > 0x7FFFFFFF) return fail(TFCB_INVALID_ARGUMENT, "batch size %lld out of range", (long long)I.B);
+    if (I.H <= 0 || I.W <= 0 || I.H * I.W > 0x7FFFFFFF)
+      return fail(TFCB_INVALID_ARGUMENT, "latent shape %lld x %lld out of range", (long long)I.H, (long long)I.W);
+  } else {
+    TFCB_TRY(ar_check_table_space(work, work_floats, cb_table_floats(I), alignof(CbImage)));
+  }
+  const long long total = cb_positions(I, colour) * C;
   if (total == 0) return TFCB_OK;  // (the non-anchors of a 1x1 latent: empty tensors may have null pointers)
   if (!src || !dst) return fail(TFCB_INVALID_ARGUMENT, "`src` or `dst` is null");
+  cudaStream_t s = as_stream(stream);
   const long long blocks = std::min<long long>((total + 255) / 256, 1ll << 16);
-  cb_scatter_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(src, dst, n_k, (int)W, H * W, M, o, C, colour,
-                                                                     total);
+  if (I.hs) {
+    TFCB_TRY(cb_upload_table(I, M, o, C, colour, 0, work, s));
+    cb_scatter_kernel<<<(unsigned)blocks, 256, 0, s>>>(src, dst, 0, 0, 0, M, o, C, colour, total,
+                                                       reinterpret_cast<const CbImage*>(work), (int)I.B);
+  } else {
+    cb_scatter_kernel<<<(unsigned)blocks, 256, 0, s>>>(src, dst, cb_count(I.H, I.W, colour), (int)I.W, I.H * I.W, M, o,
+                                                       C, colour, total, nullptr, 0);
+  }
   TFCB_LAUNCHED();
   TFCB_CUDA_TRY(cudaGetLastError());
   return TFCB_OK;
@@ -364,7 +480,7 @@ extern "C" {
 
 int64_t tfcb_cb_workspace_floats(int M, int64_t B, int64_t H, int64_t W, int anchors) {
   if (M <= 0 || M % 6 != 0 || M > kArMaxM || B <= 0 || H <= 0 || W <= 0 || H * W > 0x7FFFFFFF) return -1;
-  return cb_work_floats(cb_net(M, 0, M), B, H, W, anchors ? 0 : 1);
+  return cb_work_floats(cb_net(M, 0, M), {B, H, W, nullptr, nullptr}, anchors ? 0 : 1);
 }
 
 int tfcb_cb_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,
@@ -372,14 +488,15 @@ int tfcb_cb_params(const float* packed_dev, int64_t packed_floats, int M, const 
                    int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev, int32_t* index_dev,
                    const float* y_dev, float* y_cb_dev, float* yhat_out_dev, void* stream) {
   TFCB_TRY(ar_check(M, packed_dev, packed_floats, B, H, W, num_scales));
-  return cb_run(packed_dev, M, 0, M, yhat_dev, psi_dev, nullptr, B, H, W, anchors ? 0 : 1, num_scales, work_dev,
-                work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev, yhat_out_dev, stream);
+  return cb_run(packed_dev, M, 0, M, yhat_dev, psi_dev, nullptr, {B, H, W, nullptr, nullptr}, anchors ? 0 : 1,
+                num_scales, work_dev, work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev,
+                yhat_out_dev, stream);
 }
 
 int tfcb_cb_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int anchors, float* dst_dev,
                     void* stream) {
   if (M <= 0) return fail(TFCB_INVALID_ARGUMENT, "latent depth M=%d must be positive", M);
-  return cb_scatter(src_dev, B, H, W, M, 0, M, anchors ? 0 : 1, dst_dev, stream);
+  return cb_scatter(src_dev, {B, H, W, nullptr, nullptr}, M, 0, M, anchors ? 0 : 1, dst_dev, nullptr, 0, stream);
 }
 
 int64_t tfcb_scc_packed_floats(int M, int offset, int C, int64_t* layout) {
@@ -408,7 +525,7 @@ int tfcb_scc_pack_weights(int M, int offset, int C, const float* ctx_taps_dev, c
 
 int64_t tfcb_scc_workspace_floats(int M, int offset, int C, int64_t B, int64_t H, int64_t W, int anchors) {
   if (!scc_group_ok(M, offset, C) || B <= 0 || H <= 0 || W <= 0 || H * W > 0x7FFFFFFF) return -1;
-  return cb_work_floats(cb_net(M, offset, C), B, H, W, anchors ? 0 : 1);
+  return cb_work_floats(cb_net(M, offset, C), {B, H, W, nullptr, nullptr}, anchors ? 0 : 1);
 }
 
 int tfcb_scc_params(const float* packed_dev, int64_t packed_floats, int M, int offset, int C, const float* yhat_dev,
@@ -417,21 +534,46 @@ int tfcb_scc_params(const float* packed_dev, int64_t packed_floats, int M, int o
                     float* scale_index_dev, int32_t* index_dev, const float* y_dev, float* y_cb_dev,
                     float* yhat_out_dev, void* stream) {
   TFCB_TRY(scc_check_group(M, offset, C));
-  if (!packed_dev) return fail(TFCB_INVALID_ARGUMENT, "`packed` is null");
-  const long long n = cb_net(M, offset, C).total;
-  if (packed_floats != n)
-    return fail(TFCB_INVALID_ARGUMENT, "packed weights hold %lld floats, the group [%d, %d) of M=%d needs %lld",
-                (long long)packed_floats, offset, offset + C, M, n);
+  TFCB_TRY(scc_check_packed(packed_dev, packed_floats, M, offset, C));
   TFCB_TRY(ar_check_batch(B, H, W, num_scales));
-  return cb_run(packed_dev, M, offset, C, yhat_dev, psi_dev, chctx_dev, B, H, W, anchors ? 0 : 1, num_scales,
-                work_dev, work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev, yhat_out_dev,
-                stream);
+  return cb_run(packed_dev, M, offset, C, yhat_dev, psi_dev, chctx_dev, {B, H, W, nullptr, nullptr}, anchors ? 0 : 1,
+                num_scales, work_dev, work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev, y_cb_dev,
+                yhat_out_dev, stream);
 }
 
 int tfcb_scc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int offset, int C, int anchors,
                      float* dst_dev, void* stream) {
   TFCB_TRY(scc_check_group(M, offset, C));
-  return cb_scatter(src_dev, B, H, W, M, offset, C, anchors ? 0 : 1, dst_dev, stream);
+  return cb_scatter(src_dev, {B, H, W, nullptr, nullptr}, M, offset, C, anchors ? 0 : 1, dst_dev, nullptr, 0, stream);
+}
+
+int64_t tfcb_scc_ragged_workspace_floats(int M, int offset, int C, int64_t n_images, const int64_t* heights_host,
+                                         const int64_t* widths_host, int anchors) {
+  if (!scc_group_ok(M, offset, C) || !ar_list_ok(n_images, heights_host, widths_host)) return -1;
+  return cb_work_floats(cb_net(M, offset, C), {n_images, 0, 0, heights_host, widths_host}, anchors ? 0 : 1);
+}
+
+int tfcb_scc_params_ragged(const float* packed_dev, int64_t packed_floats, int M, int offset, int C,
+                           const float* yhat_dev, const float* psi_dev, const float* chctx_dev, int64_t n_images,
+                           const int64_t* heights_host, const int64_t* widths_host, int anchors, int num_scales,
+                           float* work_dev, int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev,
+                           int32_t* index_dev, const float* y_dev, float* y_cb_dev, float* yhat_out_dev,
+                           void* stream) {
+  TFCB_TRY(scc_check_group(M, offset, C));
+  TFCB_TRY(scc_check_packed(packed_dev, packed_floats, M, offset, C));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, num_scales));
+  return cb_run(packed_dev, M, offset, C, yhat_dev, psi_dev, chctx_dev, {n_images, 0, 0, heights_host, widths_host},
+                anchors ? 0 : 1, num_scales, work_dev, work_floats, whole, loc_dev, scale_index_dev, index_dev, y_dev,
+                y_cb_dev, yhat_out_dev, stream);
+}
+
+int tfcb_scc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_t* heights_host,
+                            const int64_t* widths_host, int M, int offset, int C, int anchors, float* work_dev,
+                            int64_t work_floats, float* dst_dev, void* stream) {
+  TFCB_TRY(scc_check_group(M, offset, C));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, 1));
+  return cb_scatter(src_dev, {n_images, 0, 0, heights_host, widths_host}, M, offset, C, anchors ? 0 : 1, dst_dev,
+                    work_dev, work_floats, stream);
 }
 
 }  // extern "C"

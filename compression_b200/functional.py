@@ -1207,3 +1207,239 @@ def scc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_off
       part = decode_index_f32(handle, index, loc, coff)
       check(lib.tfcb_scc_scatter(_p(part), B, H, W, M, o, c, int(anchors), _p(y_hat), _stream()))
   return y_hat
+
+
+# ------------------------------------------------------------------------------------------------
+# Ragged lists of latents (§3.13): the context models over images of their own latent shapes in one launch sequence.
+# A list holds n images with latents [H_i, W_i, M] and psi [H_i, W_i, 2M] (float32 CUDA tensors); inside the calls
+# they are flat, image after image.  Coding-order tensors are flat too: image i's H_i W_i M values follow image
+# i - 1's, so `compress_ragged(lookup, lengths, y, loc, cdf_offset, index=index)` with the returned lengths makes each
+# image's string, byte for byte the string of the fixed-shape call on that image alone.  Decoded latents are returned
+# as a list of views of one flat buffer.
+# ------------------------------------------------------------------------------------------------
+def _ragged_list(psis):
+  """(heights, widths, M) of a list of psi [H_i, W_i, 2M]; heights and widths are int64 numpy arrays."""
+  import numpy as np
+  if not isinstance(psis, (list, tuple)) or not psis:
+    raise _lib.InvalidArgumentError("a ragged call needs a non-empty list of latents")
+  for psi in psis:
+    if not isinstance(psi, torch.Tensor) or psi.dim() != 3 or psi.shape[-1] % 2 or psi.shape[-1] != psis[0].shape[-1]:
+      raise _lib.InvalidArgumentError("every `psi` must be [H_i, W_i, 2M] with one M")
+    if psi.shape[0] == 0 or psi.shape[1] == 0:
+      raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
+  hs = np.ascontiguousarray([int(p.shape[0]) for p in psis], dtype=np.int64)
+  ws = np.ascontiguousarray([int(p.shape[1]) for p in psis], dtype=np.int64)
+  return hs, ws, int(psis[0].shape[-1]) // 2
+
+
+def _ragged_cat(ts, name, hs, ws, ch, dev):
+  """The flat concatenation of the list `ts` of [H_i, W_i, ch] tensors."""
+  if not isinstance(ts, (list, tuple)) or len(ts) != hs.size:
+    raise _lib.InvalidArgumentError(f"`{name}` must be a list of {hs.size} tensors, one per image")
+  return torch.cat([_ar_tensor(t, name, (int(h), int(w), ch), dev).reshape(-1) for t, h, w in zip(ts, hs, ws)])
+
+
+def _ragged_views(flat, hs, ws, ch):
+  """Image i's [H_i, W_i, ch] view of a flat list."""
+  out, at = [], 0
+  for h, w in zip(hs.tolist(), ws.tolist()):
+    out.append(flat[at:at + h * w * ch].view(h, w, ch))
+    at += h * w * ch
+  return out
+
+
+def _host(a):
+  return a.ctypes.data_as(C.c_void_p)
+
+
+def _ar_ragged(packed, psis):
+  """(heights, widths, M, packed floats, flat psi) of a ragged call of the autoregressive model."""
+  hs, ws, M = _ragged_list(psis)
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from ar_pack_weights")
+  n = ar_packed_floats(M)
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, M={M} needs {n}")
+  if packed.device.type != "cuda":
+    raise _lib.InvalidArgumentError(f"`packed` must be on a CUDA device, not {packed.device}")
+  return hs, ws, M, n, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed.device)
+
+
+def _ar_work(k, dev):
+  nw = int(_lib.lib().tfcb_ar_ragged_workspace_floats(k))
+  return torch.empty(max(nw, 1), dtype=torch.float32, device=dev), nw
+
+
+def ar_encode_ragged(packed, ys, psis, num_scales, scale_index=False):
+  """ar_encode of every position of a list of images of their own shapes, one CTA per image in one launch: returns
+  (y_hats, y, loc, index, lengths), and scale_index last with `scale_index=True`.  y_hats is the list of [H_i, W_i, M];
+  y, loc and index are flat in coding order (raster order, image after image), `lengths` the images' H_i W_i M."""
+  hs, ws, M, n, psi = _ar_ragged(packed, psis)
+  dev = packed.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, loc = torch.empty_like(y), torch.empty_like(y)
+  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
+  scale = torch.empty_like(y) if scale_index else None
+  work, nw = _ar_work(hs.size, dev)
+  check(_lib.lib().tfcb_ar_encode_ragged(_p(packed), n, M, _p(y), _p(psi), hs.size, _host(hs), _host(ws),
+                                         int(num_scales), _p(work), nw, _p(y_hat), _p(loc), _p(index), _p(scale),
+                                         _stream()))
+  return (_ragged_views(y_hat, hs, ws, M), y, loc, index, (hs * ws * M).tolist()) + ((scale,) if scale_index else ())
+
+
+def ar_decode_ragged(handle, packed, psis, num_scales, cdf_offset):
+  """ar_decode of every position of a list of images, continuing `handle` (a DecoderHandle of one index-mode string per
+  image): returns the list of y_hat [H_i, W_i, M].  One launch, one CTA per image, no host synchronisation; stream
+  errors surface at entropy_decode_finalize."""
+  hs, ws, M, n, psi = _ar_ragged(packed, psis)
+  dev = packed.device
+  if handle.n_streams != hs.size:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a list of {hs.size}")
+  y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  work, nw = _ar_work(hs.size, dev)
+  coff = _i32(cdf_offset, dev)
+  check(_lib.lib().tfcb_ar_decode_ragged(handle._h, _p(packed), n, M, _p(psi), hs.size, _host(hs), _host(ws),
+                                         int(num_scales), _p(coff), _p(work), nw, _p(y_hat), _stream()))
+  return _ragged_views(y_hat, hs, ws, M)
+
+
+def _scc_ragged(packed, groups, psis):
+  """(heights, widths, M, spans, flat psi) of a whole-latent ragged call, with every group's packed buffer checked."""
+  hs, ws, M = _ragged_list(psis)
+  spans = scc_spans(groups)
+  if sum(c for _, c in spans) != M or len(packed) != len(spans):
+    raise _lib.InvalidArgumentError(f"{len(packed)} packed networks and groups {tuple(groups)} for a latent of depth "
+                                    f"{M}: one network per group, and the groups must sum to M")
+  for p, g in zip(packed, spans):
+    _scc_check_packed(p, M, g)
+  return hs, ws, M, spans, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed[0].device)
+
+
+def _scc_check_packed(packed, M, group):
+  o, c = (int(v) for v in group)
+  n = scc_layout(M, group)["total"]
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from scc_pack_weights")
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, group ({o}, {c}) of M={M} needs {n}")
+  if packed.device.type != "cuda":
+    raise _lib.InvalidArgumentError(f"`packed` must be on a CUDA device, not {packed.device}")
+  return n
+
+
+def _scc_pass_ragged(packed, group, M, hs, ws, y_hat, psi, ch_ctx, anchors, num_scales, whole=False, loc=None,
+                     scale=None, index=None, y=None, y_cc=None, y_hat_out=None):
+  """One pass of group (offset, channels) over the flat list.  Per-pass outputs (whole False, loc None) are allocated:
+  returns (loc, scale_index, index, lengths, work) with image i's n_k,i c values at c Q_i; the workspace holds the
+  image table for the scatter."""
+  o, c = (int(v) for v in group)
+  n = _scc_check_packed(packed, M, group)
+  dev = packed.device
+  lib = _lib.lib()
+  k = hs.size
+  counts = (hs * ws + 1) // 2 if anchors else hs * ws // 2
+  if loc is None:
+    total = int(counts.sum()) * c
+    loc, scale = (torch.empty(total, dtype=torch.float32, device=dev) for _ in range(2))
+    index = torch.empty(total, dtype=torch.int32, device=dev)
+  nw = int(lib.tfcb_scc_ragged_workspace_floats(M, o, c, k, _host(hs), _host(ws), int(bool(anchors))))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
+  check(lib.tfcb_scc_params_ragged(_p(packed), n, M, o, c, _p(y_hat), _p(psi), _p(ch_ctx), k, _host(hs), _host(ws),
+                                   int(bool(anchors)), int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale),
+                                   _p(index), _p(y), _p(y_cc), _p(y_hat_out), _stream()))
+  return loc, scale, index, (counts * c).tolist(), work
+
+
+def _scc_ch_ctx_ragged(ch_ctx, group, hs, ws, dev):
+  """The flat channel context of a group at a positive offset (a list of [H_i, W_i, 2c]); None at offset 0."""
+  o, c = (int(v) for v in group)
+  if o == 0:
+    if ch_ctx is not None:
+      raise _lib.InvalidArgumentError("the group at offset 0 has no channel context: pass None")
+    return None
+  return _ragged_cat(ch_ctx, "ch_ctx", hs, ws, 2 * c, dev)
+
+
+def scc_params_ragged(packed, group, y_hats, psis, ch_ctx, anchors, num_scales):
+  """scc_params over a list of images of their own shapes in one pass: returns (loc, scale_index, index, lengths),
+  flat, image i's n_i c values (n_i its positions of this colour) after image i - 1's; `lengths` are the n_i c.
+  ch_ctx is a list of [H_i, W_i, 2c] (None at offset 0); y_hats a list of [H_i, W_i, M] (may be None for the anchor
+  pass).  Image i's values equal scc_params on that image alone, bit for bit."""
+  hs, ws, M = _ragged_list(psis)
+  _scc_check_packed(packed, M, group)
+  dev = packed.device
+  psi = _ragged_cat(psis, "psi", hs, ws, 2 * M, dev)
+  ch = _scc_ch_ctx_ragged(ch_ctx, group, hs, ws, dev)
+  y_hat = None if y_hats is None and anchors else _ragged_cat(y_hats, "y_hat", hs, ws, M, dev)
+  return _scc_pass_ragged(packed, group, M, hs, ws, y_hat, psi, ch, anchors, num_scales)[:4]
+
+
+def scc_encode_ragged(packed, groups, ys, psis, channel_context, num_scales, scale_index=False):
+  """scc_encode of a list of images of their own shapes, one pass sequence for the whole list: returns (y_hats, y,
+  loc, index, lengths), and scale_index last with `scale_index=True`.  `channel_context(k, y_hats)` takes and returns
+  lists ([H_i, W_i, 2c_k] per image).  y, loc and index are flat in coding order, image i's H_i W_i M values (its
+  `lengths` entry) after image i - 1's."""
+  hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis)
+  dev = psi.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, y_cc, loc = (torch.empty_like(y) for _ in range(3))
+  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
+  scale = torch.empty_like(y) if scale_index else None
+  views = _ragged_views(y_hat, hs, ws, M)
+  for k, (p, g) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, g, hs, ws, dev)
+    for anchors in (True, False):
+      _scc_pass_ragged(p, g, M, hs, ws, y_hat, psi, ch, anchors, num_scales, True, loc, scale, index, y, y_cc, y_hat)
+  return (views, y_cc, loc, index, (hs * ws * M).tolist()) + ((scale,) if scale_index else ())
+
+
+def scc_decode_ragged(handle, packed, groups, psis, channel_context, num_scales, cdf_offset):
+  """scc_decode of a list of images of their own shapes, continuing `handle` (one index-mode string per image): per
+  group its channel context (as in scc_encode_ragged), then per colour one ragged parameter pass, one decode_ragged
+  and one scatter for the whole list.  Returns the list of y_hat [H_i, W_i, M].  The library launches depend on the
+  groups, not on the images' number or shapes (fewer when every image is 1x1); no host synchronisation."""
+  hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis)
+  dev = psi.device
+  if handle.n_streams != hs.size:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a list of {hs.size}")
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  views = _ragged_views(y_hat, hs, ws, M)
+  lib = _lib.lib()
+  for k, (p, (o, c)) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, (o, c), hs, ws, dev)
+    for anchors in (True, False):
+      loc, _, index, lengths, work = _scc_pass_ragged(p, (o, c), M, hs, ws, y_hat, psi, ch, anchors, num_scales)
+      part = decode_ragged(handle, lengths, index=index, quant_offset=loc, cdf_offset=coff)
+      check(lib.tfcb_scc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, o, c, int(anchors), _p(work),
+                                        work.numel(), _p(y_hat), _stream()))
+  return views
+
+
+def _cb_ragged_check(packed, psis):
+  """The checkerboard model's packed size (M a multiple of 6) before the group (0, M) calls."""
+  M = _ragged_list(psis)[2]
+  n = ar_packed_floats(M)
+  if isinstance(packed, torch.Tensor) and packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, M={M} needs {n}")
+  return M
+
+
+def cb_params_ragged(packed, y_hats, psis, anchors, num_scales):
+  """cb_params over a list of images of their own shapes in one pass: (loc, scale_index, index, lengths) as
+  scc_params_ragged gives them for the group (0, M), which is the checkerboard pass bit for bit."""
+  M = _cb_ragged_check(packed, psis)
+  return scc_params_ragged(packed, (0, M), y_hats, psis, None, anchors, num_scales)
+
+
+def cb_encode_ragged(packed, ys, psis, num_scales, scale_index=False):
+  """cb_encode of a list of images of their own shapes: (y_hats, y, loc, index, lengths) as scc_encode_ragged."""
+  M = _cb_ragged_check(packed, psis)
+  return scc_encode_ragged([packed], (M,), ys, psis, None, num_scales, scale_index)
+
+
+def cb_decode_ragged(handle, packed, psis, num_scales, cdf_offset):
+  """cb_decode of a list of images of their own shapes: two parameter passes, two decode_ragged calls and two
+  scatters for the whole list.  Returns the list of y_hat [H_i, W_i, M]."""
+  M = _cb_ragged_check(packed, psis)
+  return scc_decode_ragged(handle, [packed], (M,), psis, None, num_scales, cdf_offset)

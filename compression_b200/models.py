@@ -760,23 +760,31 @@ class MBT2018Model(_Model):
     x_hat = self.synthesis_transform(y_hat)
     return _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])
 
-  # -- lists of differently sized images: transforms per image, coding grouped by latent shape --
+  # -- lists of differently sized images: transforms per image, one ragged coding call for the whole list --
+  def _encode_ragged(self, ys, psis):
+    """(y, loc, index, lengths) in coding order of latents ys [H_i, W_i, M] with hyper features psis."""
+    return F.ar_encode_ragged(self._packed, ys, psis, self.num_scales)[1:]
+
+  def _decode_ragged(self, handle, psis, cdf_offset):
+    """The list of y_hat [H_i, W_i, M], continuing `handle` (one string per image)."""
+    return F.ar_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset)
+
   @torch.no_grad()
   def compress_images(self, images):
     """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element.
-    The transforms run per image; images of one latent shape share one encoder launch and one range encode."""
+    The transforms run per image; the latents of the whole list, whatever their shapes, share one ragged encoder
+    launch sequence and one range encode."""
     xs = [_as_image(x)[None].to(device=self._device(), dtype=torch.float32) for x in images]
     if not xs:
       raise ValueError("`images` is empty")
     ys = [self.analysis_transform(x) for x in xs]
     zs = [self.hyper_analysis_transform(y) for y in ys]
     side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs]).split()
-    psis = [self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1])) for y, z in zip(ys, zs)]
-    strings = [None] * len(xs)
-    for members in self._groups([tuple(y.shape[1:-1]) for y in ys]):
-      group = self._encode_latents(torch.cat([ys[i] for i in members]), torch.cat([psis[i] for i in members]))[0]
-      for i, s in zip(members, group.split()):
-        strings[i] = s
+    psis = [self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))[0] for y, z in zip(ys, zs)]
+    em = self.entropy_model
+    y_cc, loc, index, lengths = self._encode_ragged([y[0] for y in ys], psis)
+    strings = F.compress_ragged(em._lookup_host(), lengths, y_cc, loc, em.cdf_offset.to(y_cc.device),
+                                index=index).split()
     return [(strings[i], side_strings[i]) + tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
             for i, (x, y, z) in enumerate(zip(xs, ys, zs))]
 
@@ -788,25 +796,17 @@ class MBT2018Model(_Model):
       raise ValueError("`items` is empty")
     z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
                                                        [tuple(int(v) for v in it[4]) for it in items])
-    y_hws = [(int(it[3][0]), int(it[3][1])) for it in items]
-    psis = [self._psi(z_hat[None], hw) for z_hat, hw in zip(z_hats, y_hws)]
-    out = [None] * len(items)
-    for members in self._groups(y_hws):
-      y_hat = self._decode_latents(gen_ops.Strings.concat([items[i][0] for i in members]),
-                                   torch.cat([psis[i] for i in members]))
-      for k, i in enumerate(members):
-        x_shape = items[i][2]
-        x_hat = self.synthesis_transform(y_hat[k:k + 1])
-        out[i] = _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])[0]
+    psis = [self._psi(z_hat[None], (int(it[3][0]), int(it[3][1])))[0] for z_hat, it in zip(z_hats, items)]
+    em = self.entropy_model
+    handle = gen_ops.create_range_decoder(em._strings(gen_ops.Strings.concat([it[0] for it in items])),
+                                          em._lookup_host())
+    y_hats = self._decode_ragged(handle, psis, em.cdf_offset.to(psis[0].device))
+    em._finish_decode(handle)
+    out = []
+    for y_hat, it in zip(y_hats, items):
+      x_hat = self.synthesis_transform(y_hat[None])
+      out.append(_to_uint8(x_hat[:, :int(it[2][0]), :int(it[2][1]), :])[0])
     return out
-
-  @staticmethod
-  def _groups(shapes):
-    """Indexes of the items of each distinct shape, in order of first appearance."""
-    groups = {}
-    for i, s in enumerate(shapes):
-      groups.setdefault(tuple(s), []).append(i)
-    return list(groups.values())
 
   def decompress_from_tfci(self, data):
     dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
@@ -883,6 +883,12 @@ class CheckerboardModel(MBT2018Model):
     em._finish_decode(handle)
     return y_hat
 
+  def _encode_ragged(self, ys, psis):
+    return F.cb_encode_ragged(self._packed, ys, psis, self.num_scales)[1:]
+
+  def _decode_ragged(self, handle, psis, cdf_offset):
+    return F.cb_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset)
+
 
 class SpaceChannelModel(MBT2018Model):
   """The space-channel context model (SCCTX) of ELIC (He, Yang, Peng, Ma, Qin & Wang, CVPR 2022) on MBT2018Model's
@@ -945,6 +951,12 @@ class SpaceChannelModel(MBT2018Model):
     g = self.channel_context_transforms[k - 1]
     return torch.cat([g(y_hat[i:i + 1, ..., :o]) for i in range(y_hat.shape[0])]).contiguous()
 
+  def _channel_contexts(self, k, y_hats):
+    """g_ch^k of each y_hat[..., :o_k] of a list of [H_i, W_i, M]: a list of [H_i, W_i, 2c_k]."""
+    o = self.spans[k][0]
+    g = self.channel_context_transforms[k - 1]
+    return [g(y_hat[None, ..., :o])[0] for y_hat in y_hats]
+
   def _pack(self):
     M = self.latent_depth
     return [F.scc_pack_weights(M, span, cm.kernel, cm.bias, *_dense_weights(ep))
@@ -965,6 +977,13 @@ class SpaceChannelModel(MBT2018Model):
                          em.cdf_offset.to(psi.device))
     em._finish_decode(handle)
     return y_hat
+
+  def _encode_ragged(self, ys, psis):
+    return F.scc_encode_ragged(self._packed, self.groups, ys, psis, self._channel_contexts, self.num_scales)[1:]
+
+  def _decode_ragged(self, handle, psis, cdf_offset):
+    return F.scc_decode_ragged(handle, self._packed, self.groups, psis, self._channel_contexts, self.num_scales,
+                               cdf_offset)
 
 
 # ------------------------------------------------------------------------------------------------

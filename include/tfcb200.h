@@ -254,6 +254,24 @@ int tfcb_ar_encode(const float* packed_dev, int64_t packed_floats, int M, const 
 int tfcb_ar_decode(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
                    int64_t B, int64_t H, int64_t W, int64_t p_begin, int64_t p_end, int num_scales,
                    const int32_t* cdf_offset_dev, float* yhat_dev, void* stream);
+/* Ragged lists: n_images > 0 images of latent shapes heights_host[i] x widths_host[i] (host arrays; every side
+ * positive, H W <= 2^31 - 1).  Latents, yhat, loc, index and scale_index are flat: image i's [H_i, W_i, M] starts at
+ * element M P_i with P_i = sum_{j<i} H_j W_j, psi likewise with 2M channels.  Each image's outputs equal the
+ * fixed-shape call on that image alone, bit for bit.  The entries keep a table of the images in `work_dev`, uploaded
+ * with one stream-ordered copy; there is no host synchronisation. */
+/* Floats of workspace a ragged call over n_images images needs, or -1 if n_images is not positive. */
+int64_t tfcb_ar_ragged_workspace_floats(int64_t n_images);
+/* tfcb_ar_encode over every position of every image of the list, one CTA per image.  One launch. */
+int tfcb_ar_encode_ragged(const float* packed_dev, int64_t packed_floats, int M, const float* y_dev,
+                          const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                          const int64_t* widths_host, int num_scales, float* work_dev, int64_t work_floats,
+                          float* yhat_dev, float* loc_dev, int32_t* index_dev, float* scale_index_dev, void* stream);
+/* tfcb_ar_decode over every position of every image of the list: image i continues stream i of `h`, which must hold
+ * n_images strings.  One launch. */
+int tfcb_ar_decode_ragged(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
+                          int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int num_scales,
+                          const int32_t* cdf_offset_dev, float* work_dev, int64_t work_floats, float* yhat_dev,
+                          void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Checkerboard context model (He et al. 2021) on the same packed parameters.  A latent position (r, c) is an
@@ -323,6 +341,30 @@ int tfcb_scc_params(const float* packed_dev, int64_t packed_floats, int M, int o
  * [B, H, W, M] (nothing else is written).  One launch; none when the colour has no positions. */
 int tfcb_scc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int offset, int C, int anchors,
                      float* dst_dev, void* stream);
+/* Ragged lists (the layout of tfcb_ar_encode_ragged): psi, chctx (2C channels), y and yhat are flat, image i's
+ * starting at P_i times their channel count.  With n_k,i the positions of this colour of image i and
+ * Q_i = sum_{j<i} n_k,j, a pass writes image i's n_k,i C values at C Q_i (whole == 0), or its block of the coding
+ * order of all groups at M P_i + H_i W_i offset + (anchors ? 0 : n_a,i C) (whole != 0), whose streams are the images'
+ * H_i W_i M values.  Each image's outputs equal the fixed-shape call on that image alone, bit for bit; a tile of
+ * positions may span several images.  The checkerboard model is the group (0, M).  The table of the images goes to
+ * `work_dev` with one stream-ordered copy; there is no host synchronisation. */
+/* Floats of workspace one tfcb_scc_params_ragged pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_scc_ragged_workspace_floats(int M, int offset, int C, int64_t n_images, const int64_t* heights_host,
+                                         const int64_t* widths_host, int anchors);
+/* tfcb_scc_params over a ragged list of images in place of B, H, W.  Three launches for the anchors, four for the
+ * non-anchors, none when no image has a position of this colour. */
+int tfcb_scc_params_ragged(const float* packed_dev, int64_t packed_floats, int M, int offset, int C,
+                           const float* yhat_dev, const float* psi_dev, const float* chctx_dev, int64_t n_images,
+                           const int64_t* heights_host, const int64_t* widths_host, int anchors, int num_scales,
+                           float* work_dev, int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev,
+                           int32_t* index_dev, const float* y_dev, float* y_cb_dev, float* yhat_out_dev,
+                           void* stream);
+/* tfcb_scc_scatter of a ragged list: image i's n_k,i C values at C Q_i -> its positions and the group's channels of
+ * its [H_i, W_i, M] in `dst_dev`.  `work_dev` holds at least 8 n_images floats (the workspace of a pass of the list
+ * does).  One launch; none when no image has a position of this colour. */
+int tfcb_scc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_t* heights_host,
+                            const int64_t* widths_host, int M, int offset, int C, int anchors, float* work_dev,
+                            int64_t work_floats, float* dst_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Legacy single-stream ops RangeEncode / RangeDecode (int16 data, broadcastable N-D int32 CDF):

@@ -5,7 +5,9 @@
 
 The model has random weights (seeded) unless --state-dict loads a torch state_dict saved from the same class and
 arguments.  The images are the PNGs of --images DIR (read with PIL, converted to RGB) or, with --synthetic kodak,
-24 seeded smooth-plus-noise images of Kodak's shapes, 12 of 512x768 and 12 of 768x512.
+24 seeded smooth-plus-noise images of Kodak's shapes, 12 of 512x768 and 12 of 768x512; with --synthetic mixed, 24
+such images of seeded, all different shapes (sides multiples of 16 from 256 to 1024), as in a dataset of many image
+sizes.  The context models (mbt2018, checkerboard, space_channel) code such a list with one ragged launch sequence.
 
 --time also measures, alternating the two sides of each pair --reps times after --warmup calls (median ms, CUDA
 events around a synchronised call):
@@ -15,7 +17,7 @@ events around a synchronised call):
 with the library's kernel launches and all CUDA kernels (torch.profiler, one call in a separate pass) of one call of
 each side, and the card's name, power limit and SM clock read in the same run.
 
-  python tools/rd_eval.py --synthetic kodak [--model bmshj2018] [--num-filters 192] [--state-dict F] [--time]
+  python tools/rd_eval.py --synthetic kodak|mixed [--model bmshj2018] [--num-filters 192] [--state-dict F] [--time]
   python tools/rd_eval.py --images DIR ...
 """
 import argparse
@@ -40,10 +42,28 @@ BLOCKS = [  # (metric, colour space, key in the evaluate_images dicts)
 ]
 
 
-def synthetic_kodak(seed):
+MODELS = {"bls2017": models.BLS2017Model, "bmshj2018": models.BMSHJ2018Model, "ms2020": models.MS2020Model,
+          "mbt2018": models.MBT2018Model, "checkerboard": models.CheckerboardModel,
+          "space_channel": models.SpaceChannelModel}
+
+
+def mixed_shapes(seed, n=24):
+  """n seeded image shapes (h, w), sides multiples of 16 from 256 to 1024, no two alike (nor their latents)."""
+  rng = np.random.default_rng(seed)
+  sides = np.arange(256, 1025, 16)
+  out = []
+  while len(out) < n:
+    s = (int(rng.choice(sides)), int(rng.choice(sides)))
+    if s not in out:
+      out.append(s)
+  return out
+
+
+def synthetic(seed, shapes=None):
+  """Seeded smooth-plus-noise images of `shapes` (default: Kodak's, 12 of 512x768 and 12 of 768x512)."""
   g = torch.Generator().manual_seed(seed)
   out = []
-  for h, w in [(512, 768)] * 12 + [(768, 512)] * 12:
+  for h, w in shapes or [(512, 768)] * 12 + [(768, 512)] * 12:
     yy = torch.linspace(0, 1, h)[:, None, None]
     xx = torch.linspace(0, 1, w)[None, :, None]
     f = 2 + 6 * torch.rand(1, 1, 3, generator=g)
@@ -64,7 +84,7 @@ def png_images(directory):
 def make_model(name, num_filters, state_dict, seed):
   torch.manual_seed(seed)
   kw = {} if num_filters is None else {"num_filters": num_filters}
-  m = {"bls2017": models.BLS2017Model, "bmshj2018": models.BMSHJ2018Model, "ms2020": models.MS2020Model}[name](**kw)
+  m = MODELS[name](**kw)
   m.build("cuda")
   if state_dict:
     m.load_state_dict(torch.load(state_dict, map_location="cuda"))
@@ -108,12 +128,12 @@ def launches(fn):
   return n1 - n0, kernels
 
 
-def main():
+def parser():
   p = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
   src = p.add_mutually_exclusive_group(required=True)
   src.add_argument("--images", help="directory of PNG images")
-  src.add_argument("--synthetic", choices=["kodak"], help="seeded synthetic images of a dataset's shapes")
-  p.add_argument("--model", choices=["bls2017", "bmshj2018", "ms2020"], default="bmshj2018")
+  src.add_argument("--synthetic", choices=["kodak", "mixed"], help="seeded synthetic images of a dataset's shapes")
+  p.add_argument("--model", choices=list(MODELS), default="bmshj2018")
   p.add_argument("--num-filters", type=int, default=None, help="the model's num_filters (default: its own)")
   p.add_argument("--state-dict", default=None, help="torch state_dict of the model to load")
   p.add_argument("--seed", type=int, default=0)
@@ -121,11 +141,18 @@ def main():
   p.add_argument("--reps", type=int, default=10)
   p.add_argument("--warmup", type=int, default=2)
   p.add_argument("--out", default=None, help="also write the results as JSON to this file")
-  args = p.parse_args()
+  return p
+
+
+def main():
+  args = parser().parse_args()
   if not torch.cuda.is_available():
     raise SystemExit("rd_eval.py needs a CUDA device")
 
-  images = synthetic_kodak(args.seed) if args.synthetic else png_images(args.images)
+  if args.synthetic:
+    images = synthetic(args.seed, mixed_shapes(args.seed) if args.synthetic == "mixed" else None)
+  else:
+    images = png_images(args.images)
   model = make_model(args.model, args.num_filters, args.state_dict, args.seed)
   per_image = model.evaluate_images(images)
   mean = models.mean_metrics(per_image)
