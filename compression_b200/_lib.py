@@ -91,6 +91,9 @@ SIGNATURES = {
     "tfcb_scc_params_ragged": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp,
                                       _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tfcb_scc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _int, _int, _vp, _i64, _vp, _vp]),
+    "tfcb_substream_layout": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp]),
+    "tfcb_substream_gather_workspace_bytes": (_i64, [_i64, _i64, _i64]),
+    "tfcb_substream_gather": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "tfcb_decoder_destroy": (None, [_vp]),
     "tfcb_range_encode": (_int, [_vp, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),
     "tfcb_range_decode": (_int, [_vp, _i64, _vp, _int, _vp, _vp, _int, _int, _int, _vp, _vp]),

@@ -265,10 +265,47 @@ class ContinuousEntropyModelBase(nn.Module):
   def _coder16(self, dtype, device, off, index, shape):
     return self._coder16_models and F._coder16(dtype, device, off, index, shape)
 
-  def _encode(self, batch_shape, b, off, coff, index=None, fused=True):
+  # substreams (DESIGN §3.14): with S > 1 each coding unit's string holds S independently decodable streams, and every
+  # call runs on the ragged entries over units x S streams.  A unit is one phase of positions: rows of the tables
+  # (channel mode) or of the innermost axis (index mode), so every stream starts at a position.
+  @staticmethod
+  def _substreams(substreams, fused=True):
+    S = gen_ops.check_substreams(substreams)
+    if S > 1 and not fused:
+      raise ValueError("`fused=False` issues the reference's op sequence, which writes one stream per string: "
+                       "substreams must be 1")
+    return S
+
+  @staticmethod
+  def _substream_layout(shapes, coff, index, substreams):
+    """F.substream_layout of single-phase units of the given shapes."""
+    if index is None:
+      widths = [coff.numel()] * len(shapes)
+    else:
+      widths = [max(int(s[-1]), 1) if len(s) else 1 for s in shapes]
+    return F.substream_layout([[gen_ops._prod(s) // w] for s, w in zip(shapes, widths)], [[w] for w in widths],
+                              substreams)
+
+  @staticmethod
+  def _flat_unit_operands(off, index):
+    """off and index flat for the ragged entries (off stays per row in channel mode)."""
+    if index is not None:
+      if off is not None and off.numel() == index.numel():
+        off = off.reshape(-1)
+      index = index.reshape(-1)
+    return off, index
+
+  def _encode(self, batch_shape, b, off, coff, index=None, fused=True, substreams=1):
     """One string per element of `batch_shape` for `b` (in bottleneck_dtype, coding units innermost).  A float32
     bottleneck, and a 16-bit one with the operands _coder16 accepts, is quantised inside the encoder unless
     `fused=False`, which issues the reference's op sequence."""
+    S = self._substreams(substreams, fused)
+    if S > 1:
+      unit = tuple((b if index is None else index).shape[len(batch_shape):])
+      off, index = self._flat_unit_operands(off, index)
+      strings = self._encode_ragged([unit] * gen_ops._prod(batch_shape), b.reshape(-1), off, coff, index,
+                                    substreams=S)
+      return gen_ops.Strings(strings.bytes_dev, strings.offsets_dev, batch_shape)
     if fused and b.dtype == torch.float32:
       return F.compress_f32(batch_shape, self._lookup_host(), b, off, coff, index=index)
     if fused and self._coder16(b.dtype, b.device, off, index, b.shape):
@@ -281,8 +318,13 @@ class ContinuousEntropyModelBase(nn.Module):
       gen_ops.entropy_encode_index(handle, index, symbols)
     return gen_ops.entropy_encode_finalize(handle)
 
-  def _decode(self, strings, shape, off, coff, index=None, fused=True):
+  def _decode(self, strings, shape, off, coff, index=None, fused=True, substreams=1):
     """Inverse of _encode: a tensor of shape strings.shape + `shape` (the coding unit's) in bottleneck_dtype."""
+    S = self._substreams(substreams, fused)
+    if S > 1:
+      off, index = self._flat_unit_operands(off, index)
+      out = self._decode_flat(strings, [tuple(shape)] * strings.numel(), off, coff, index, S)
+      return out.reshape(tuple(strings.shape) + tuple(shape))
     handle = gen_ops.create_range_decoder(strings, self._lookup_host())
     if fused and self.bottleneck_dtype == torch.float32:
       if index is None:
@@ -305,24 +347,42 @@ class ContinuousEntropyModelBase(nn.Module):
     return self._dequantize(symbols, off, coff, index).reshape(strings.shape + shape)
 
   # ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none)
-  def _encode_ragged(self, shapes, b, off, coff, index=None, return_decoded=False):
+  def _encode_ragged(self, shapes, b, off, coff, index=None, return_decoded=False, substreams=1):
     """Strings of shape (k,) for the k items of the given shapes that `b` (in bottleneck_dtype) holds back to back;
     with `return_decoded`, also what _decode_ragged makes of them.  A float32 bottleneck, and a 16-bit one with the
-    operands _coder16 accepts, is quantised inside the encoder, which then also writes the decoded items."""
-    lengths = [gen_ops._prod(s) for s in shapes]
+    operands _coder16 accepts, is quantised inside the encoder, which then also writes the decoded items.  With
+    `substreams` = S > 1 the encode runs over items x S streams, in item order, and the strings are joined."""
+    S = self._substreams(substreams)
+    lengths = [gen_ops._prod(s) for s in shapes] if S == 1 else self._substream_layout(shapes, coff, index, S)[0]
+    fused = b.dtype == torch.float32 or self._coder16(b.dtype, b.device, off, index, b.shape)
     if b.dtype == torch.float32:
       out = F.compress_ragged(self._lookup_host(), lengths, b, off, coff, index=index, decoded=return_decoded)
-      return (out[0], gen_ops._split_items(out[1], shapes)) if return_decoded else out
-    if self._coder16(b.dtype, b.device, off, index, b.shape):
+    elif fused:
       out = F.compress_ragged_16bit(self._lookup_host(), lengths, b, off, coff, index=index, decoded=return_decoded)
-      return (out[0], gen_ops._split_items(out[1], shapes)) if return_decoded else out
-    strings = F.compress_ragged(self._lookup_host(), lengths, self._quantize(b, off, coff, index), index=index)
-    return (strings, self._decode_ragged(strings, shapes, off, coff, index)) if return_decoded else strings
+    else:
+      out = F.compress_ragged(self._lookup_host(), lengths, self._quantize(b, off, coff, index), index=index)
+    strings, decoded = out if fused and return_decoded else (out, None)
+    if S > 1:
+      strings = gen_ops.join_substreams(strings, S, (len(shapes),))
+    if not return_decoded:
+      return strings
+    if decoded is None:
+      return strings, self._decode_ragged(strings, shapes, off, coff, index, S)
+    return strings, gen_ops._split_items(decoded, shapes)
 
-  def _decode_ragged(self, strings, shapes, off, coff, index=None):
+  def _decode_ragged(self, strings, shapes, off, coff, index=None, substreams=1):
     """Inverse of _encode_ragged: the items, views into one allocation."""
-    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
+    S = self._substreams(substreams)
+    return gen_ops._split_items(self._decode_flat(strings, shapes, off, coff, index, S), shapes)
+
+  def _decode_flat(self, strings, shapes, off, coff, index, substreams):
+    """The items of _decode_ragged back to back in one flat tensor.  With substreams the headers are parsed on the
+    host before any device work, and the sanity check of an item is that of all its streams."""
     lengths = [gen_ops._prod(s) for s in shapes]
+    if substreams > 1:
+      lengths = self._substream_layout(shapes, coff, index, substreams)[0]
+      strings = gen_ops.split_substreams(strings, substreams)
+    handle = gen_ops.create_range_decoder(strings, self._lookup_host())
     dtype, dev = self.bottleneck_dtype, strings.bytes_dev.device
     unfused = False
     if dtype == torch.float32:
@@ -335,7 +395,7 @@ class ContinuousEntropyModelBase(nn.Module):
     self._finish_decode(handle)
     if unfused:
       out = self._dequantize(out, off, coff, index).reshape(-1)
-    return gen_ops._split_items(out, shapes)
+    return out
 
 
 class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
@@ -433,9 +493,11 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     qoff = self.quantization_offset
     return coff, (None if qoff is None else qoff.to(device, torch.float32).reshape(-1))
 
-  def compress(self, bottleneck, fused=True):
+  def compress(self, bottleneck, fused=True, *, substreams=1):
     """continuous_batched.py:347-383.  `fused=True` quantises inside the encode kernel (same arithmetic);
-    `fused=False` issues the reference's op sequence literally."""
+    `fused=False` issues the reference's op sequence literally.  `substreams` = S > 1 writes each string as S
+    independently decodable streams behind a small header (DESIGN §3.14; S = 1 is the reference's string), to be
+    decompressed with the same S."""
     self._check_compression()
     bottleneck = torch.as_tensor(bottleneck).to(device=_cuda(), dtype=self.bottleneck_dtype)
     shape = tuple(bottleneck.shape)
@@ -446,21 +508,21 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     if rank_p and shape[-rank_p:] != self.prior_shape:
       bottleneck = torch.broadcast_to(bottleneck, shape[:-rank_p] + self.prior_shape)
     coff, qoff = self._flat_tables(bottleneck.device)
-    return self._encode(batch_shape, bottleneck, qoff, coff, fused=fused)
+    return self._encode(batch_shape, bottleneck, qoff, coff, fused=fused, substreams=substreams)
 
-  def decompress(self, strings, broadcast_shape, fused=True):
+  def decompress(self, strings, broadcast_shape, fused=True, *, substreams=1):
     """continuous_batched.py:385-422."""
     self._check_compression()
     strings = self._strings(strings)
     broadcast_shape = tuple(int(d) for d in np.asarray(broadcast_shape).reshape(-1))
     coff, qoff = self._flat_tables(strings.bytes_dev.device)
-    return self._decode(strings, broadcast_shape + self.prior_shape, qoff, coff, fused=fused)
+    return self._decode(strings, broadcast_shape + self.prior_shape, qoff, coff, fused=fused, substreams=substreams)
 
   # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
-  def compress_ragged(self, bottlenecks, return_decoded=False):
+  def compress_ragged(self, bottlenecks, return_decoded=False, *, substreams=1):
     """Compresses a list of coding units of different shapes in one range-coder launch.  Each item has exactly
     `coding_rank` dimensions ending in `prior_shape` (no broadcasting).  Returns a Strings of shape (k,) whose string
-    i equals `compress(bottlenecks[i])`.
+    i equals `compress(bottlenecks[i], substreams=substreams)`.
 
     `return_decoded=True` returns `(strings, items)` with `items` equal, bit for bit, to
     `decompress_ragged(strings, ...)`: written by the encoder itself for a float32 bottleneck, decoded from the
@@ -478,16 +540,16 @@ class ContinuousBatchedEntropyModel(ContinuousEntropyModelBase):
     coff, qoff = self._flat_tables(dev)
     # every item holds whole rows of prior_shape, so channel mode's rows line up across items
     return self._encode_ragged([tuple(b.shape) for b in items], torch.cat([b.reshape(-1) for b in items]), qoff,
-                               coff, return_decoded=return_decoded)
+                               coff, return_decoded=return_decoded, substreams=substreams)
 
-  def decompress_ragged(self, strings, broadcast_shapes):
+  def decompress_ragged(self, strings, broadcast_shapes, *, substreams=1):
     """Inverse of compress_ragged: item i has shape `broadcast_shapes[i] + prior_shape` and equals
     `decompress(strings[i:i+1], broadcast_shapes[i])[0]`.  The items are views into one allocation."""
     self._check_compression()
     shapes = [tuple(int(d) for d in np.asarray(s).reshape(-1)) + self.prior_shape for s in broadcast_shapes]
     strings = self._strings(strings, len(shapes))
     coff, qoff = self._flat_tables(strings.bytes_dev.device)
-    return self._decode_ragged(strings, shapes, qoff, coff)
+    return self._decode_ragged(strings, shapes, qoff, coff, substreams=substreams)
 
   def get_config(self):
     """continuous_batched.py:424-436."""
@@ -593,8 +655,8 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
   def quantize(self, bottleneck):
     return math_ops.round_st(torch.as_tensor(bottleneck).to(self.bottleneck_dtype))
 
-  def compress(self, bottleneck, indexes, fused=True, _loc=None):
-    """continuous_indexed.py:354-386."""
+  def compress(self, bottleneck, indexes, fused=True, _loc=None, *, substreams=1):
+    """continuous_indexed.py:354-386.  `substreams` as in ContinuousBatchedEntropyModel.compress."""
     self._check_compression()
     dev = _cuda()
     bottleneck = torch.as_tensor(bottleneck).to(device=dev, dtype=self.bottleneck_dtype)
@@ -602,9 +664,9 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     flat = self._flatten_indexes(indexes)
     fshape = tuple(flat.shape)
     return self._encode(fshape[:len(fshape) - self.coding_rank], bottleneck, _loc, self.cdf_offset.to(dev), flat,
-                        fused)
+                        fused, substreams)
 
-  def decompress(self, strings, indexes, fused=True, _loc=None):
+  def decompress(self, strings, indexes, fused=True, _loc=None, *, substreams=1):
     """continuous_indexed.py:388-417."""
     self._check_compression()
     strings = self._strings(strings)
@@ -612,7 +674,8 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     indexes = self._normalize_indexes(torch.as_tensor(indexes).to(device=dev, dtype=self.prior_dtype))
     flat = self._flatten_indexes(indexes)
     fshape = tuple(flat.shape)
-    return self._decode(strings, fshape[len(fshape) - self.coding_rank:], _loc, self.cdf_offset.to(dev), flat, fused)
+    return self._decode(strings, fshape[len(fshape) - self.coding_rank:], _loc, self.cdf_offset.to(dev), flat, fused,
+                        substreams)
 
   # -- ragged batches: items of different shapes, one range-coder launch (an extension; the reference has none) --
   def _ragged_indexes(self, indexes, dev):
@@ -632,7 +695,7 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
         raise ValueError(f"each item needs {self.coding_rank} dimensions: received indexes for shape {s}")
     return flat, shapes
 
-  def compress_ragged(self, bottlenecks, indexes, _loc=None, return_decoded=False):
+  def compress_ragged(self, bottlenecks, indexes, _loc=None, return_decoded=False, *, substreams=1):
     """Compresses a list of coding units of different shapes (each with exactly `coding_rank` dimensions) in one
     range-coder launch.  Returns a Strings of shape (k,) whose string i equals `compress(bottlenecks[i],
     indexes[i])`.
@@ -650,9 +713,9 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     b = torch.cat([b.reshape(-1) for b in items])
     if loc is not None and loc.numel() != b.numel():
       raise ValueError("each `loc` item must have the shape of its bottleneck")
-    return self._encode_ragged(shapes, b, loc, self.cdf_offset.to(dev), flat, return_decoded)
+    return self._encode_ragged(shapes, b, loc, self.cdf_offset.to(dev), flat, return_decoded, substreams)
 
-  def decompress_ragged(self, strings, indexes, _loc=None):
+  def decompress_ragged(self, strings, indexes, _loc=None, *, substreams=1):
     """Inverse of compress_ragged: item i has the coding shape of `indexes[i]`.  The items are views into one
     allocation."""
     self._check_compression()
@@ -660,7 +723,7 @@ class ContinuousIndexedEntropyModel(ContinuousEntropyModelBase):
     dev = strings.bytes_dev.device
     flat, shapes = self._ragged_indexes(indexes, dev)
     loc = None if _loc is None else torch.cat([torch.as_tensor(l).to(dev).reshape(-1) for l in _loc])
-    return self._decode_ragged(strings, shapes, loc, self.cdf_offset.to(dev), flat)
+    return self._decode_ragged(strings, shapes, loc, self.cdf_offset.to(dev), flat, substreams)
 
   def get_config(self):
     raise NotImplementedError("Serializing indexed entropy models is not yet implemented.")
@@ -693,18 +756,19 @@ class LocationScaleIndexedEntropyModel(ContinuousIndexedEntropyModel):
   def quantize(self, bottleneck, loc=None):
     return math_ops.round_st(torch.as_tensor(bottleneck).to(self.bottleneck_dtype), loc)
 
-  def compress(self, bottleneck, scale_indexes, loc=None, fused=True):
-    return super().compress(bottleneck, scale_indexes, fused=fused, _loc=loc)
+  def compress(self, bottleneck, scale_indexes, loc=None, fused=True, *, substreams=1):
+    return super().compress(bottleneck, scale_indexes, fused=fused, _loc=loc, substreams=substreams)
 
-  def decompress(self, strings, scale_indexes, loc=None, fused=True):
-    return super().decompress(strings, scale_indexes, fused=fused, _loc=loc)
+  def decompress(self, strings, scale_indexes, loc=None, fused=True, *, substreams=1):
+    return super().decompress(strings, scale_indexes, fused=fused, _loc=loc, substreams=substreams)
 
-  def compress_ragged(self, bottlenecks, scale_indexes, loc=None, return_decoded=False):
+  def compress_ragged(self, bottlenecks, scale_indexes, loc=None, return_decoded=False, *, substreams=1):
     """`loc`: None or a list with one tensor per item."""
-    return super().compress_ragged(bottlenecks, scale_indexes, _loc=loc, return_decoded=return_decoded)
+    return super().compress_ragged(bottlenecks, scale_indexes, _loc=loc, return_decoded=return_decoded,
+                                   substreams=substreams)
 
-  def decompress_ragged(self, strings, scale_indexes, loc=None):
-    return super().decompress_ragged(strings, scale_indexes, _loc=loc)
+  def decompress_ragged(self, strings, scale_indexes, loc=None, *, substreams=1):
+    return super().decompress_ragged(strings, scale_indexes, _loc=loc, substreams=substreams)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -512,6 +512,64 @@ def decode_ragged(handle, lengths, index=None, quant_offset=None, cdf_offset=Non
 
 
 # ------------------------------------------------------------------------------------------------
+# Substreams (DESIGN §3.14): the library's split of coding units into S streams, and the encoder's gather
+# ------------------------------------------------------------------------------------------------
+def _phase_table(positions, widths):
+  import numpy as np
+  pos = np.ascontiguousarray(np.asarray(positions, dtype=np.int64))
+  wid = np.ascontiguousarray(np.broadcast_to(np.asarray(widths, dtype=np.int64), pos.shape))
+  if pos.ndim != 2 or pos.shape[0] == 0 or pos.shape[1] == 0:
+    raise _lib.InvalidArgumentError(f"`positions` must be [units, phases]: shape {pos.shape}")
+  return pos, wid
+
+
+def substream_layout(positions, widths, substreams):
+  """The split of units into `substreams` = S streams: `positions` [units, phases] (phase p of unit u has that many
+  positions of widths[u, p] symbols; `widths` broadcasts).  Returns (stream_lengths [units S], phase_lengths
+  [phases, units S]) as int64 numpy arrays: stream u S + s's symbols in all (for compress_ragged) and in phase p (for
+  one decode_ragged per phase)."""
+  import numpy as np
+  pos, wid = _phase_table(positions, widths)
+  U, P = pos.shape
+  S = int(substreams)
+  offs = np.zeros(U * S + 1, dtype=np.int64)
+  phase = np.zeros((P, U * S), dtype=np.int64)
+  check(_lib.lib().tfcb_substream_layout(U, P, _host(pos), _host(wid), S, _host(offs), _host(phase)))
+  return np.diff(offs), phase
+
+
+def substream_gather(positions, widths, substreams, y=None, loc=None, index=None):
+  """Units held back to back in coding order -> substream order, in one launch: y and loc (float32) and index
+  (int32), flat, each rewritten as substream_layout splits `positions` / `widths`.  Returns the new (y, loc, index),
+  None where the operand is None."""
+  pos, wid = _phase_table(positions, widths)
+  U, P = pos.shape
+  S = int(substreams)
+  lib = _lib.lib()
+  given = [t for t in (y, loc, index) if t is not None]
+  if not given:
+    raise _lib.InvalidArgumentError("substream_gather needs y, loc or index")
+  dev = given[0].device
+  ins = (_f32(y, dev), _f32(loc, dev), _i32(index, dev))
+  outs = tuple(None if t is None else torch.empty_like(t) for t in ins)
+  nw = int(lib.tfcb_substream_gather_workspace_bytes(U, P, S))
+  work = torch.empty(max(nw // 8, 1), dtype=torch.int64, device=dev)
+  check(lib.tfcb_substream_gather(U, P, _host(pos), _host(wid), S, *[_p(t) for t in ins], *[_p(t) for t in outs],
+                                  _p(work), work.numel() * 8, _stream()))
+  return outs
+
+
+def context_phases(groups, hs, ws):
+  """positions and widths [images, 2K] of the context models' coding order: per group c_k, its anchors, then its
+  non-anchors (the checkerboard model is the one group (M,))."""
+  import numpy as np
+  hw = np.asarray(hs, dtype=np.int64).reshape(-1) * np.asarray(ws, dtype=np.int64).reshape(-1)
+  pos = np.stack([n for _ in groups for n in ((hw + 1) // 2, hw // 2)], axis=1)
+  wid = np.broadcast_to(np.asarray([int(c) for c in groups for _ in range(2)], dtype=np.int64), pos.shape)
+  return pos, wid
+
+
+# ------------------------------------------------------------------------------------------------
 # Universal quantisation: shared noise levels and coding tensors (universal.py:30-62,147-170,446-466)
 # ------------------------------------------------------------------------------------------------
 def _seed_words(seed):
@@ -1000,10 +1058,12 @@ def cb_params(packed, y_hat, psi, anchors, num_scales):
   return loc, scale, index
 
 
-def cb_encode(packed, y, psi, num_scales, scale_index=False):
+def cb_encode(packed, y, psi, num_scales, scale_index=False, substreams=1):
   """The two-pass encoder: returns y_hat [B, H, W, M] and y, loc, index in coding order [B, H * W, M] (and
   scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc, the anchors' before the
-  non-anchor pass reads them.  The strings are one index-mode encode of the coding-order y with index and loc."""
+  non-anchor pass reads them.  The strings are one index-mode encode of the coding-order y with index and loc.  With
+  `substreams` = S > 1 the coding-order tensors are rewritten into substream order by one gather (a second one for
+  scale_index), ready for compress_ragged with the stream lengths of context_substreams."""
   B, H, W, M, _ = _ar_dims(packed, psi)
   dev = packed.device
   psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
@@ -1014,28 +1074,62 @@ def cb_encode(packed, y, psi, num_scales, scale_index=False):
   scale = torch.empty_like(loc) if scale_index else None
   for anchors in (True, False):
     _cb_pass(packed, y_hat, psi, anchors, num_scales, True, loc, scale, index, y, y_cb, y_hat)
-  return (y_hat, y_cb, loc, index) + ((scale,) if scale_index else ())
+  return (y_hat,) + _to_substreams((M,), [H] * B, [W] * B, substreams, y_cb, loc, index, scale)
 
 
-def cb_decode(handle, packed, psi, num_scales, cdf_offset):
+def cb_decode(handle, packed, psi, num_scales, cdf_offset, substreams=1):
   """The two-pass decoder, continuing `handle` (a DecoderHandle of B index-mode strings in coding order): anchor
   parameters, decode_index_f32 of the anchors, their latents to [B, H, W, M], non-anchor parameters, decode of the
   non-anchors, to [B, H, W, M].  Returns y_hat [B, H, W, M].  A fixed number of library launches whatever B, H and W
   (fewer at H W = 1, where the non-anchor pass is empty) and no host synchronisation; stream errors surface at
-  entropy_decode_finalize."""
+  entropy_decode_finalize.  With `substreams` = S > 1 the handle holds B S substreams (gen_ops.split_substreams) and
+  each pass decodes with one decode_ragged in place of decode_index_f32: the same launches."""
   B, H, W, M, _ = _ar_dims(packed, psi)
   dev = packed.device
   psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
-  if handle.n_streams != B:
-    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a batch of {B}")
+  phases = _substream_phases(handle, (M,), [H] * B, [W] * B, substreams)
   coff = _i32(cdf_offset, dev)
   y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
   lib = _lib.lib()
-  for anchors in (True, False):
+  for p, anchors in enumerate((True, False)):
     loc, _, index = cb_params(packed, y_hat, psi, anchors, num_scales)
-    part = decode_index_f32(handle, index, loc, coff)
+    part = _decode_phase(handle, phases, p, index, loc, coff)
     check(lib.tfcb_cb_scatter(_p(part), B, H, W, M, int(anchors), _p(y_hat), _stream()))
   return y_hat
+
+
+def context_substreams(groups, hs, ws, substreams):
+  """(stream_lengths, phase_lengths) of substream_layout for the context models' coding order of images of latent
+  shapes hs[i] x ws[i] with channel groups `groups`."""
+  return substream_layout(*context_phases(groups, hs, ws), substreams)
+
+
+def _to_substreams(groups, hs, ws, substreams, y, loc, index, scale=None):
+  """An encoder's coding-order outputs, rewritten into substream order when `substreams` > 1 (shapes kept)."""
+  out = (y, loc, index) + (() if scale is None else (scale,))
+  if substreams == 1:
+    return out
+  pos, wid = context_phases(groups, hs, ws)
+  moved = substream_gather(pos, wid, substreams, y.reshape(-1), loc.reshape(-1), index.reshape(-1))
+  if scale is not None:
+    moved += (substream_gather(pos, wid, substreams, loc=scale.reshape(-1))[1],)
+  return tuple(m.view(t.shape) for m, t in zip(moved, out))
+
+
+def _substream_phases(handle, groups, hs, ws, substreams, what="batch"):
+  """A context decoder's per-pass decode lengths (None for S = 1), after checking the handle's stream count."""
+  units = len(hs)
+  if handle.n_streams != units * substreams:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a {what} of {units}" +
+                                    ("" if substreams == 1 else f" in {substreams} substreams"))
+  return None if substreams == 1 else context_substreams(groups, hs, ws, substreams)[1]
+
+
+def _decode_phase(handle, phases, p, index, loc, coff):
+  """Pass p's symbols of every image in coding order: one decode_index_f32, or with substreams one decode_ragged."""
+  if phases is None:
+    return decode_index_f32(handle, index, loc, coff)
+  return decode_ragged(handle, phases[p], index=index, quant_offset=loc, cdf_offset=coff)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1167,12 +1261,12 @@ def _scc_batch(packed, groups, psi):
   return B, H, W, M, spans, _ar_tensor(psi, "psi", (B, H, W, 2 * M), psi.device)
 
 
-def scc_encode(packed, groups, y, psi, channel_context, num_scales, scale_index=False):
+def scc_encode(packed, groups, y, psi, channel_context, num_scales, scale_index=False, substreams=1):
   """The group-by-group encoder: `packed` holds one scc_pack_weights buffer per group.  Per group k, its channel
   context `channel_context(k, y_hat)` [B, H, W, 2c_k] (called for k >= 1, once y_hat holds groups 0 to k - 1), the
   anchor pass, then the non-anchor pass.  Returns y_hat [B, H, W, M] and y, loc, index in coding order
   [B, H * W * M] (and scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc.  The
-  strings are one index-mode encode of the coding-order y with index and loc."""
+  strings are one index-mode encode of the coding-order y with index and loc.  `substreams` as in cb_encode."""
   B, H, W, M, spans, psi = _scc_batch(packed, groups, psi)
   dev = psi.device
   y = _ar_tensor(y, "y", (B, H, W, M), dev)
@@ -1184,19 +1278,18 @@ def scc_encode(packed, groups, y, psi, channel_context, num_scales, scale_index=
     ch = _scc_ch_ctx(channel_context(k, y_hat) if k else None, g, (B, H, W), dev)
     for anchors in (True, False):
       _scc_pass(p, g, y_hat, psi, ch, anchors, num_scales, True, loc, scale, index, y, y_cc, y_hat)
-  return (y_hat, y_cc, loc, index) + ((scale,) if scale_index else ())
+  return (y_hat,) + _to_substreams(groups, [H] * B, [W] * B, substreams, y_cc, loc, index, scale)
 
 
-def scc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_offset):
+def scc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_offset, substreams=1):
   """The group-by-group decoder, continuing `handle` (a DecoderHandle of B index-mode strings in coding order): per
   group its channel context (as in scc_encode), then per colour the parameter pass, decode_index_f32 and the scatter
   into y_hat [B, H, W, M], which it returns.  2K decode calls on the handle; per group a fixed number of library
   launches whatever B, H and W (fewer at H W = 1, where the non-anchor passes are empty), and no host
-  synchronisation; stream errors surface at entropy_decode_finalize."""
+  synchronisation; stream errors surface at entropy_decode_finalize.  `substreams` as in cb_decode."""
   B, H, W, M, spans, psi = _scc_batch(packed, groups, psi)
   dev = psi.device
-  if handle.n_streams != B:
-    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a batch of {B}")
+  phases = _substream_phases(handle, groups, [H] * B, [W] * B, substreams)
   coff = _i32(cdf_offset, dev)
   y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
   lib = _lib.lib()
@@ -1204,7 +1297,7 @@ def scc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_off
     ch = channel_context(k, y_hat) if k else None
     for anchors in (True, False):
       loc, _, index = scc_params(p, (o, c), y_hat, psi, ch, anchors, num_scales)
-      part = decode_index_f32(handle, index, loc, coff)
+      part = _decode_phase(handle, phases, 2 * k + (0 if anchors else 1), index, loc, coff)
       check(lib.tfcb_scc_scatter(_p(part), B, H, W, M, o, c, int(anchors), _p(y_hat), _stream()))
   return y_hat
 
@@ -1374,11 +1467,12 @@ def scc_params_ragged(packed, group, y_hats, psis, ch_ctx, anchors, num_scales):
   return _scc_pass_ragged(packed, group, M, hs, ws, y_hat, psi, ch, anchors, num_scales)[:4]
 
 
-def scc_encode_ragged(packed, groups, ys, psis, channel_context, num_scales, scale_index=False):
+def scc_encode_ragged(packed, groups, ys, psis, channel_context, num_scales, scale_index=False, substreams=1):
   """scc_encode of a list of images of their own shapes, one pass sequence for the whole list: returns (y_hats, y,
   loc, index, lengths), and scale_index last with `scale_index=True`.  `channel_context(k, y_hats)` takes and returns
   lists ([H_i, W_i, 2c_k] per image).  y, loc and index are flat in coding order, image i's H_i W_i M values (its
-  `lengths` entry) after image i - 1's."""
+  `lengths` entry) after image i - 1's.  With `substreams` = S > 1 they are in substream order (one gather, a second
+  one for scale_index) and `lengths` holds the n S stream lengths, image i's substream s at i S + s."""
   hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis)
   dev = psi.device
   y = _ragged_cat(ys, "y", hs, ws, M, dev)
@@ -1390,18 +1484,20 @@ def scc_encode_ragged(packed, groups, ys, psis, channel_context, num_scales, sca
     ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, g, hs, ws, dev)
     for anchors in (True, False):
       _scc_pass_ragged(p, g, M, hs, ws, y_hat, psi, ch, anchors, num_scales, True, loc, scale, index, y, y_cc, y_hat)
-  return (views, y_cc, loc, index, (hs * ws * M).tolist()) + ((scale,) if scale_index else ())
+  out = _to_substreams(groups, hs, ws, substreams, y_cc, loc, index, scale)
+  lengths = (hs * ws * M).tolist() if substreams == 1 else context_substreams(groups, hs, ws, substreams)[0].tolist()
+  return (views,) + out[:3] + (lengths,) + out[3:]
 
 
-def scc_decode_ragged(handle, packed, groups, psis, channel_context, num_scales, cdf_offset):
+def scc_decode_ragged(handle, packed, groups, psis, channel_context, num_scales, cdf_offset, substreams=1):
   """scc_decode of a list of images of their own shapes, continuing `handle` (one index-mode string per image): per
   group its channel context (as in scc_encode_ragged), then per colour one ragged parameter pass, one decode_ragged
   and one scatter for the whole list.  Returns the list of y_hat [H_i, W_i, M].  The library launches depend on the
-  groups, not on the images' number or shapes (fewer when every image is 1x1); no host synchronisation."""
+  groups, not on the images' number or shapes (fewer when every image is 1x1); no host synchronisation.  With
+  `substreams` = S > 1 the handle holds n S substreams and each decode_ragged takes that pass's substream lengths."""
   hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis)
   dev = psi.device
-  if handle.n_streams != hs.size:
-    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a list of {hs.size}")
+  phases = _substream_phases(handle, groups, hs, ws, substreams, "list")
   coff = _i32(cdf_offset, dev)
   y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
   views = _ragged_views(y_hat, hs, ws, M)
@@ -1410,6 +1506,8 @@ def scc_decode_ragged(handle, packed, groups, psis, channel_context, num_scales,
     ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, (o, c), hs, ws, dev)
     for anchors in (True, False):
       loc, _, index, lengths, work = _scc_pass_ragged(p, (o, c), M, hs, ws, y_hat, psi, ch, anchors, num_scales)
+      if phases is not None:
+        lengths = phases[2 * k + (0 if anchors else 1)]
       part = decode_ragged(handle, lengths, index=index, quant_offset=loc, cdf_offset=coff)
       check(lib.tfcb_scc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, o, c, int(anchors), _p(work),
                                         work.numel(), _p(y_hat), _stream()))
@@ -1432,14 +1530,14 @@ def cb_params_ragged(packed, y_hats, psis, anchors, num_scales):
   return scc_params_ragged(packed, (0, M), y_hats, psis, None, anchors, num_scales)
 
 
-def cb_encode_ragged(packed, ys, psis, num_scales, scale_index=False):
+def cb_encode_ragged(packed, ys, psis, num_scales, scale_index=False, substreams=1):
   """cb_encode of a list of images of their own shapes: (y_hats, y, loc, index, lengths) as scc_encode_ragged."""
   M = _cb_ragged_check(packed, psis)
-  return scc_encode_ragged([packed], (M,), ys, psis, None, num_scales, scale_index)
+  return scc_encode_ragged([packed], (M,), ys, psis, None, num_scales, scale_index, substreams)
 
 
-def cb_decode_ragged(handle, packed, psis, num_scales, cdf_offset):
+def cb_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1):
   """cb_decode of a list of images of their own shapes: two parameter passes, two decode_ragged calls and two
   scatters for the whole list.  Returns the list of y_hat [H_i, W_i, M]."""
   M = _cb_ragged_check(packed, psis)
-  return scc_decode_ragged(handle, [packed], (M,), psis, None, num_scales, cdf_offset)
+  return scc_decode_ragged(handle, [packed], (M,), psis, None, num_scales, cdf_offset, substreams)

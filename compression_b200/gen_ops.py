@@ -165,6 +165,108 @@ class Strings:
     return self.shape[0] if self.shape else 1
 
 
+# ------------------------------------------------------------------------------------------------
+# Substream strings (DESIGN §3.14).  With S > 1 substreams a coding unit's string is varint(S), varint(len_0) ...
+# varint(len_{S-2}), then the S substreams back to back, the last one running to the end of the string; varints are
+# unsigned LEB128 in minimal form.  S = 1 is the plain range-coded string, with no header.
+# ------------------------------------------------------------------------------------------------
+MAX_SUBSTREAMS = 1024
+
+
+def check_substreams(substreams) -> int:
+  """`substreams` as an int in [1, MAX_SUBSTREAMS]; anything else raises InvalidArgumentError (a ValueError)."""
+  if isinstance(substreams, (bool, np.bool_)) or not isinstance(substreams, (int, np.integer)):
+    raise InvalidArgumentError(f"`substreams` must be an integer: {substreams!r}")
+  if not 1 <= int(substreams) <= MAX_SUBSTREAMS:
+    raise InvalidArgumentError(f"`substreams` must be in [1, {MAX_SUBSTREAMS}]: {int(substreams)}")
+  return int(substreams)
+
+
+def _varint(v: int) -> bytes:
+  out = bytearray()
+  while True:
+    b = v & 0x7F
+    v >>= 7
+    if not v:
+      out.append(b)
+      return bytes(out)
+    out.append(b | 0x80)
+
+
+def substream_header(lengths) -> bytes:
+  """The header of a unit whose S = len(lengths) substreams have these byte lengths (b"" for S = 1)."""
+  lengths = [int(n) for n in lengths]
+  if len(lengths) == 1:
+    return b""
+  return _varint(len(lengths)) + b"".join(_varint(n) for n in lengths[:-1])
+
+
+def _read_varint(s: bytes, at: int, i: int):
+  v, shift, start = 0, 0, at
+  while True:
+    if at >= len(s):
+      raise InvalidArgumentError(f"string {i}: truncated substream header")
+    b = s[at]
+    at += 1
+    v |= (b & 0x7F) << shift
+    if not b & 0x80:
+      break
+    shift += 7
+    if shift > 63:
+      raise InvalidArgumentError(f"string {i}: substream header varint longer than 64 bits")
+  if at - start > 1 and b == 0:
+    raise InvalidArgumentError(f"string {i}: substream header varint not in minimal form")
+  return v, at
+
+
+def parse_substreams(s: bytes, substreams: int, i: int = 0) -> List[bytes]:
+  """The S substreams of string number `i`, `s`, written with `substreams` = S > 1.  A truncated or non-minimal
+  varint, another S, or lengths past the end raise InvalidArgumentError naming the string."""
+  n, at = _read_varint(s, 0, i)
+  if n != substreams:
+    raise InvalidArgumentError(f"string {i}: written with {n} substreams, decoding expects {substreams}")
+  lengths = []
+  for _ in range(substreams - 1):
+    v, at = _read_varint(s, at, i)
+    lengths.append(v)
+  out = []
+  for v in lengths:
+    if at + v > len(s):
+      raise InvalidArgumentError(f"string {i}: substream lengths run past the end of its {len(s)} bytes")
+    out.append(s[at:at + v])
+    at += v
+  return out + [s[at:]]
+
+
+def join_substreams(parts: Strings, substreams: int, shape) -> Strings:
+  """Strings of `shape` from the unit x S substreams `parts` (unit u's substream s at u S + s): each unit's header
+  and its substreams.  One device-to-host copy (the offsets); the bytes stay on the device."""
+  S = substreams
+  n = parts.numel() // S
+  offs = parts.offsets_dev.cpu().numpy()
+  heads = [substream_header(np.diff(offs[u * S:(u + 1) * S + 1])) for u in range(n)]
+  dev = parts.bytes_dev.device
+  hbuf = torch.from_numpy(np.frombuffer(b"".join(heads) + b"\0", dtype=np.uint8).copy()).to(dev)
+  chunks, out_offs, at = [], [0], 0
+  for u, h in enumerate(heads):
+    lo, hi = int(offs[u * S]), int(offs[(u + 1) * S])
+    chunks += [hbuf[at:at + len(h)], parts.bytes_dev[lo:hi]]
+    at += len(h)
+    out_offs.append(out_offs[-1] + len(h) + hi - lo)
+  data = torch.cat(chunks + [torch.zeros(1, dtype=torch.uint8, device=dev)])
+  return Strings(data, torch.tensor(out_offs, dtype=torch.int64).to(dev), shape)
+
+
+def split_substreams(strings: Strings, substreams: int) -> Strings:
+  """The payloads of strings written with `substreams` = S > 1, without their headers, as a Strings of shape
+  (numel S,) (string i's substream s at i S + s): what a decoder handle takes.  Parsed on the host before any device
+  work."""
+  payload = []
+  for i, s in enumerate(strings.tolist()):
+    payload += parse_substreams(s, substreams, i)
+  return Strings.from_bytes(payload, (len(payload),))
+
+
 class EncoderHandle:
   """Stand-in for the DT_VARIANT encoder handle (cc/kernels/range_coder_kernels.cc:62-66)."""
 

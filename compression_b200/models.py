@@ -125,8 +125,20 @@ def mean_metrics(per_image):
 
 class _Model(nn.Module):
 
+  # whether the model's decoders can use substreams (DESIGN §3.14); MBT2018Model's decodes positions serially
+  _substream_decoder = True
+
   def _device(self):
     return next(self.parameters()).device
+
+  def _set_substreams(self, substreams):
+    """`substreams` = S: every string the model writes (y, z, each MS2020 slice) holds S independently decodable
+    streams behind a small header, so that one image decodes on S SMs; S = 1 writes the reference's strings."""
+    S = gen_ops.check_substreams(substreams)
+    if S > 1 and not self._substream_decoder:
+      raise ValueError(f"{type(self).__name__} decodes its positions one after another, so substreams cannot help "
+                       f"it: substreams must be 1, not {S}")
+    self.substreams = S
 
   def build(self, device="cuda", patch=(64, 64)):
     """Keras `self.build((None, None, None, 3))`: creates every variable (the layers build lazily on a first pass)."""
@@ -199,8 +211,9 @@ class _Model(nn.Module):
 class BLS2017Model(_Model):
   """models/bls2017.py:95-190."""
 
-  def __init__(self, lmbda=0.01, num_filters=128):
+  def __init__(self, lmbda=0.01, num_filters=128, substreams=1):
     super().__init__()
+    self._set_substreams(substreams)
     self.lmbda = lmbda
     self.num_filters = int(num_filters)
     self.analysis_transform = AnalysisTransform(num_filters)
@@ -238,11 +251,11 @@ class BLS2017Model(_Model):
     y = self.analysis_transform(x)
     x_shape = torch.tensor(x.shape[1:-1], dtype=torch.int32)
     y_shape = torch.tensor(y.shape[1:-1], dtype=torch.int32)
-    return self.entropy_model.compress(y), x_shape, y_shape
+    return self.entropy_model.compress(y, substreams=self.substreams), x_shape, y_shape
 
   @torch.no_grad()
   def decompress_batch(self, strings, x_shape, y_shape):
-    y_hat = self.entropy_model.decompress(strings, tuple(int(v) for v in y_shape))
+    y_hat = self.entropy_model.decompress(strings, tuple(int(v) for v in y_shape), substreams=self.substreams)
     x_hat = self.synthesis_transform(y_hat)
     x_hat = x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :]
     return _to_uint8(x_hat)
@@ -257,7 +270,7 @@ class BLS2017Model(_Model):
       y = self.analysis_transform(x)
       ys.append(y[0])
       shapes.append((torch.tensor(x.shape[1:-1], dtype=torch.int32), torch.tensor(y.shape[1:-1], dtype=torch.int32)))
-    strings = self.entropy_model.compress_ragged(ys).split()
+    strings = self.entropy_model.compress_ragged(ys, substreams=self.substreams).split()
     return [(s,) + sh for s, sh in zip(strings, shapes)]
 
   @torch.no_grad()
@@ -265,7 +278,8 @@ class BLS2017Model(_Model):
     """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
     items = list(items)
     y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]),
-                                                  [tuple(int(v) for v in it[2]) for it in items])
+                                                  [tuple(int(v) for v in it[2]) for it in items],
+                                                  substreams=self.substreams)
     out = []
     for y_hat, (_, x_shape, _) in zip(y_hats, items):
       x_hat = self.synthesis_transform(y_hat[None])
@@ -281,8 +295,9 @@ class BLS2017Model(_Model):
 class BMSHJ2018Model(_Model):
   """models/bmshj2018.py:141-264 (scale hyperprior)."""
 
-  def __init__(self, lmbda=0.01, num_filters=192, num_scales=64, scale_min=.11, scale_max=256.):
+  def __init__(self, lmbda=0.01, num_filters=192, num_scales=64, scale_min=.11, scale_max=256., substreams=1):
     super().__init__()
+    self._set_substreams(substreams)
     self.lmbda = lmbda
     self.num_scales = int(num_scales)
     offset = math.log(scale_min)
@@ -339,16 +354,16 @@ class BMSHJ2018Model(_Model):
     z_hat = self.side_entropy_model.quantize(z)
     indexes = self.hyper_synthesis_transform(z_hat)
     indexes = indexes[:, :y.shape[1], :y.shape[2], :]
-    side_string = self.side_entropy_model.compress(z)
-    string = self.entropy_model.compress(y, indexes)
+    side_string = self.side_entropy_model.compress(z, substreams=self.substreams)
+    string = self.entropy_model.compress(y, indexes, substreams=self.substreams)
     return string, side_string, x_shape, y_shape, z_shape
 
   @torch.no_grad()
   def decompress_batch(self, string, side_string, x_shape, y_shape, z_shape):
-    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape))
+    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape), substreams=self.substreams)
     indexes = self.hyper_synthesis_transform(z_hat)
     indexes = indexes[:, :int(y_shape[0]), :int(y_shape[1]), :]
-    y_hat = self.entropy_model.decompress(string, indexes)
+    y_hat = self.entropy_model.decompress(string, indexes, substreams=self.substreams)
     x_hat = self.synthesis_transform(y_hat)
     x_hat = x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :]
     return _to_uint8(x_hat)
@@ -367,8 +382,8 @@ class BMSHJ2018Model(_Model):
       zs.append(z[0])
       idxs.append(indexes[0, :y.shape[1], :y.shape[2], :])
       shapes.append(tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z)))
-    side_strings = self.side_entropy_model.compress_ragged(zs).split()
-    strings = self.entropy_model.compress_ragged(ys, idxs).split()
+    side_strings = self.side_entropy_model.compress_ragged(zs, substreams=self.substreams).split()
+    strings = self.entropy_model.compress_ragged(ys, idxs, substreams=self.substreams).split()
     return [(s, side) + sh for s, side, sh in zip(strings, side_strings, shapes)]
 
   @torch.no_grad()
@@ -376,11 +391,13 @@ class BMSHJ2018Model(_Model):
     """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
     items = list(items)
     z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
-                                                       [tuple(int(v) for v in it[4]) for it in items])
+                                                       [tuple(int(v) for v in it[4]) for it in items],
+                                                       substreams=self.substreams)
     idxs = []
     for z_hat, (_, _, _, y_shape, _) in zip(z_hats, items):
       idxs.append(self.hyper_synthesis_transform(z_hat[None])[0, :int(y_shape[0]), :int(y_shape[1]), :])
-    y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]), idxs)
+    y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]), idxs,
+                                                  substreams=self.substreams)
     out = []
     for y_hat, (_, _, x_shape, _, _) in zip(y_hats, items):
       x_hat = self.synthesis_transform(y_hat[None])
@@ -408,8 +425,9 @@ class MS2020Model(_Model):
   encodes AND the matching decodes (ms2020.py:334-389)."""
 
   def __init__(self, lmbda=0.01, num_filters=192, latent_depth=320, hyperprior_depth=192, num_slices=10,
-               max_support_slices=5, num_scales=64, scale_min=.11, scale_max=256.):
+               max_support_slices=5, num_scales=64, scale_min=.11, scale_max=256., substreams=1):
     super().__init__()
+    self._set_substreams(substreams)
     if latent_depth % num_slices:
       raise ValueError("Slices do not evenly divide latent depth (%d / %d)" % (latent_depth, num_slices))
     self.lmbda = lmbda
@@ -491,15 +509,16 @@ class MS2020Model(_Model):
     y = self.analysis_transform(x)
     y_hw = tuple(y.shape[1:-1])
     z = self.hyper_analysis_transform(y)
-    z_string = self.em_z.compress(z)
-    z_hat = self.em_z.decompress(z_string, tuple(z.shape[1:-1]))
+    S = self.substreams
+    z_string = self.em_z.compress(z, substreams=S)
+    z_hat = self.em_z.decompress(z_string, tuple(z.shape[1:-1]), substreams=S)
     latent_scales = self.hyper_synthesis_scale_transform(z_hat)
     latent_means = self.hyper_synthesis_mean_transform(z_hat)
     y_strings, y_hat_slices = [], []
     for i, y_slice in enumerate(torch.chunk(y, self.num_slices, dim=-1)):
       mu, sigma, mean_support = self._slice_params(i, latent_means, latent_scales, y_hat_slices, y_hw)
-      y_strings.append(self.em_y.compress(y_slice.contiguous(), sigma, mu))
-      y_hat_slices.append(self._lrp(i, mean_support, self.em_y.decompress(y_strings[-1], sigma, mu)))
+      y_strings.append(self.em_y.compress(y_slice.contiguous(), sigma, mu, substreams=S))
+      y_hat_slices.append(self._lrp(i, mean_support, self.em_y.decompress(y_strings[-1], sigma, mu, substreams=S)))
     shapes = [torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z)]
     return tuple(shapes) + (z_string,) + tuple(y_strings)
 
@@ -508,13 +527,14 @@ class MS2020Model(_Model):
     """ms2020.py:391-433."""
     assert len(y_strings) == self.num_slices
     y_hw = (int(y_shape[0]), int(y_shape[1]))
-    z_hat = self.em_z.decompress(z_string, tuple(int(v) for v in z_shape))
+    S = self.substreams
+    z_hat = self.em_z.decompress(z_string, tuple(int(v) for v in z_shape), substreams=S)
     latent_scales = self.hyper_synthesis_scale_transform(z_hat)
     latent_means = self.hyper_synthesis_mean_transform(z_hat)
     y_hat_slices = []
     for i, y_string in enumerate(y_strings):
       mu, sigma, mean_support = self._slice_params(i, latent_means, latent_scales, y_hat_slices, y_hw)
-      y_hat_slices.append(self._lrp(i, mean_support, self.em_y.decompress(y_string, sigma, loc=mu)))
+      y_hat_slices.append(self._lrp(i, mean_support, self.em_y.decompress(y_string, sigma, loc=mu, substreams=S)))
     x_hat = self.synthesis_transform(torch.cat(y_hat_slices, dim=-1))
     return _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])
 
@@ -537,7 +557,7 @@ class MS2020Model(_Model):
     ys = [self.analysis_transform(x) for x in xs]
     zs = [self.hyper_analysis_transform(y) for y in ys]
     y_hws = [tuple(y.shape[1:-1]) for y in ys]
-    z_strings, z_hats = self.em_z.compress_ragged([z[0] for z in zs], return_decoded=True)
+    z_strings, z_hats = self.em_z.compress_ragged([z[0] for z in zs], return_decoded=True, substreams=self.substreams)
     z_strings = z_strings.split()
     latents = [(self.hyper_synthesis_mean_transform(z_hat[None]), self.hyper_synthesis_scale_transform(z_hat[None]))
                for z_hat in z_hats]
@@ -547,7 +567,8 @@ class MS2020Model(_Model):
     for i in range(self.num_slices):
       params = [self._slice_params(i, lm, ls, sl, hw) for (lm, ls), sl, hw in zip(latents, y_hat_slices, y_hws)]
       strings, y_hats = self.em_y.compress_ragged([s[i][0] for s in y_slices], [p[1][0] for p in params],
-                                                  loc=[p[0][0] for p in params], return_decoded=True)
+                                                  loc=[p[0][0] for p in params], return_decoded=True,
+                                                  substreams=self.substreams)
       y_strings.append(strings.split())
       for sl, p, y_hat in zip(y_hat_slices, params, y_hats):
         sl.append(self._lrp(i, p[2], y_hat[None]))
@@ -569,14 +590,15 @@ class MS2020Model(_Model):
         raise ValueError(f"each item needs 3 shapes and {self.num_slices + 1} strings: received {len(it)} elements")
     y_hws = [(int(it[1][0]), int(it[1][1])) for it in items]
     z_hats = self.em_z.decompress_ragged(gen_ops.Strings.concat([it[3] for it in items]),
-                                         [tuple(int(v) for v in it[2]) for it in items])
+                                         [tuple(int(v) for v in it[2]) for it in items], substreams=self.substreams)
     latents = [(self.hyper_synthesis_mean_transform(z_hat[None]), self.hyper_synthesis_scale_transform(z_hat[None]))
                for z_hat in z_hats]
     y_hat_slices = [[] for _ in items]
     for i in range(self.num_slices):
       params = [self._slice_params(i, lm, ls, sl, hw) for (lm, ls), sl, hw in zip(latents, y_hat_slices, y_hws)]
       y_hats = self.em_y.decompress_ragged(gen_ops.Strings.concat([it[4 + i] for it in items]),
-                                           [p[1][0] for p in params], loc=[p[0][0] for p in params])
+                                           [p[1][0] for p in params], loc=[p[0][0] for p in params],
+                                           substreams=self.substreams)
       for sl, p, y_hat in zip(y_hat_slices, params, y_hats):
         sl.append(self._lrp(i, p[2], y_hat[None]))
     out = []
@@ -635,8 +657,12 @@ class MBT2018Model(_Model):
   M symbols of each position in one launch.  The hyper synthesis runs per image, so psi, and with it the decoded
   latents, do not depend on how images were batched."""
 
-  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.):
+  _substream_decoder = False
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.,
+               substreams=1):
     super().__init__()
+    self._set_substreams(substreams)
     N, M = int(num_filters), int(latent_depth)
     if M <= 0 or M % 6:
       raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
@@ -734,6 +760,32 @@ class MBT2018Model(_Model):
     em._finish_decode(handle)
     return y_hat
 
+  def _y_decoder(self, strings):
+    """A decoder handle of y strings (their substreams with substreams > 1)."""
+    em = self.entropy_model
+    strings = em._strings(strings)
+    if self.substreams > 1:
+      strings = gen_ops.split_substreams(strings, self.substreams)
+    return gen_ops.create_range_decoder(strings, em._lookup_host())
+
+  def _compress_coding_order(self, y, loc, index, lengths, units):
+    """The y strings of `units` images from an encoder's coding-order tensors (substream order, and `lengths` the
+    stream lengths, with substreams > 1)."""
+    em = self.entropy_model
+    coff = em.cdf_offset.to(y.device)
+    if self.substreams == 1 and lengths is None:
+      return F.compress_f32((units,), em._lookup_host(), y, loc, coff, index=index)
+    strings = F.compress_ragged(em._lookup_host(), lengths, y, loc, coff, index=index)
+    return strings if self.substreams == 1 else gen_ops.join_substreams(strings, self.substreams, (units,))
+
+  def _coded(self, y, loc, index, B, H, W):
+    """The y strings of a batch of B latents of H x W from the context models' coding-order tensors (`_groups()` are
+    their channel groups)."""
+    lengths = None
+    if self.substreams > 1:
+      lengths = F.context_substreams(self._groups(), [H] * B, [W] * B, self.substreams)[0]
+    return self._compress_coding_order(y, loc, index, lengths, B)
+
   def compress(self, x):
     """uint8 [H, W, 3] -> (string, side_string, x_shape, y_shape, z_shape), bmshj2018's signature."""
     return self.compress_batch(_as_image(x)[None])
@@ -747,14 +799,14 @@ class MBT2018Model(_Model):
     y = self.analysis_transform(x)
     z = self.hyper_analysis_transform(y)
     shapes = tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
-    side_string = self.side_entropy_model.compress(z)
+    side_string = self.side_entropy_model.compress(z, substreams=self.substreams)
     psi = self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))
     string = self._encode_latents(y, psi)[0]
     return (string, side_string) + shapes
 
   @torch.no_grad()
   def decompress_batch(self, string, side_string, x_shape, y_shape, z_shape):
-    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape))
+    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape), substreams=self.substreams)
     psi = self._psi(z_hat, (int(y_shape[0]), int(y_shape[1])))
     y_hat = self._decode_latents(string, psi)
     x_hat = self.synthesis_transform(y_hat)
@@ -779,12 +831,10 @@ class MBT2018Model(_Model):
       raise ValueError("`images` is empty")
     ys = [self.analysis_transform(x) for x in xs]
     zs = [self.hyper_analysis_transform(y) for y in ys]
-    side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs]).split()
+    side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs], substreams=self.substreams).split()
     psis = [self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))[0] for y, z in zip(ys, zs)]
-    em = self.entropy_model
     y_cc, loc, index, lengths = self._encode_ragged([y[0] for y in ys], psis)
-    strings = F.compress_ragged(em._lookup_host(), lengths, y_cc, loc, em.cdf_offset.to(y_cc.device),
-                                index=index).split()
+    strings = self._compress_coding_order(y_cc, loc, index, lengths, len(xs)).split()
     return [(strings[i], side_strings[i]) + tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
             for i, (x, y, z) in enumerate(zip(xs, ys, zs))]
 
@@ -795,11 +845,11 @@ class MBT2018Model(_Model):
     if not items:
       raise ValueError("`items` is empty")
     z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
-                                                       [tuple(int(v) for v in it[4]) for it in items])
+                                                       [tuple(int(v) for v in it[4]) for it in items],
+                                                       substreams=self.substreams)
     psis = [self._psi(z_hat[None], (int(it[3][0]), int(it[3][1])))[0] for z_hat, it in zip(z_hats, items)]
     em = self.entropy_model
-    handle = gen_ops.create_range_decoder(em._strings(gen_ops.Strings.concat([it[0] for it in items])),
-                                          em._lookup_host())
+    handle = self._y_decoder(gen_ops.Strings.concat([it[0] for it in items]))
     y_hats = self._decode_ragged(handle, psis, em.cdf_offset.to(psis[0].device))
     em._finish_decode(handle)
     out = []
@@ -860,8 +910,11 @@ class CheckerboardModel(MBT2018Model):
   `LocationScaleIndexedEntropyModel.compress(y_cb, scale_index_cb, loc_cb)` of the coding-order tensors; the decoder
   makes two decode_index_f32 calls on one decoder handle."""
 
-  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.):
-    super().__init__(lmbda, num_filters, latent_depth, num_scales, scale_min, scale_max)
+  _substream_decoder = True
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.,
+               substreams=1):
+    super().__init__(lmbda, num_filters, latent_depth, num_scales, scale_min, scale_max, substreams)
     self.context_model = CheckerboardConv2D(self.latent_depth, 2 * self.latent_depth)
 
   def _context(self, y_ctx):
@@ -869,25 +922,29 @@ class CheckerboardModel(MBT2018Model):
 
   _pack_weights = staticmethod(F.cb_pack_weights)
 
+  def _groups(self):
+    return (self.latent_depth,)
+
   def _encode_latents(self, y, psi):
-    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H * W, M]."""
-    em = self.entropy_model
-    y_hat, y_cb, loc, index = F.cb_encode(self._packed, y.contiguous(), psi, self.num_scales)
-    strings = F.compress_f32((y.shape[0],), em._lookup_host(), y_cb, loc, em.cdf_offset.to(y.device), index=index)
-    return strings, y_hat, loc, index
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H * W, M] (substream
+    order with substreams > 1)."""
+    B, H, W = (int(d) for d in y.shape[:3])
+    y_hat, y_cb, loc, index = F.cb_encode(self._packed, y.contiguous(), psi, self.num_scales,
+                                          substreams=self.substreams)
+    return self._coded(y_cb, loc, index, B, H, W), y_hat, loc, index
 
   def _decode_latents(self, strings, psi):
-    em = self.entropy_model
-    handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
-    y_hat = F.cb_decode(handle, self._packed, psi, self.num_scales, em.cdf_offset.to(psi.device))
-    em._finish_decode(handle)
+    handle = self._y_decoder(strings)
+    y_hat = F.cb_decode(handle, self._packed, psi, self.num_scales, self.entropy_model.cdf_offset.to(psi.device),
+                        substreams=self.substreams)
+    self.entropy_model._finish_decode(handle)
     return y_hat
 
   def _encode_ragged(self, ys, psis):
-    return F.cb_encode_ragged(self._packed, ys, psis, self.num_scales)[1:]
+    return F.cb_encode_ragged(self._packed, ys, psis, self.num_scales, substreams=self.substreams)[1:]
 
   def _decode_ragged(self, handle, psis, cdf_offset):
-    return F.cb_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset)
+    return F.cb_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset, substreams=self.substreams)
 
 
 class SpaceChannelModel(MBT2018Model):
@@ -906,9 +963,12 @@ class SpaceChannelModel(MBT2018Model):
   (group 0's anchors, group 0's non-anchors, group 1's anchors, ..., each in raster order); the decoder makes 2K
   decode_index_f32 calls on one decoder handle."""
 
+  _substream_decoder = True
+
   def __init__(self, lmbda=0.01, num_filters=192, latent_depth=320, groups=(16, 16, 32, 64, 192), num_scales=64,
-               scale_min=.11, scale_max=256.):
+               scale_min=.11, scale_max=256., substreams=1):
     _Model.__init__(self)
+    self._set_substreams(substreams)
     N, M = int(num_filters), int(latent_depth)
     groups = tuple(int(c) for c in groups)
     if M <= 0 or M % 2:
@@ -962,28 +1022,31 @@ class SpaceChannelModel(MBT2018Model):
     return [F.scc_pack_weights(M, span, cm.kernel, cm.bias, *_dense_weights(ep))
             for span, cm, ep in zip(self.spans, self.context_models, self.entropy_parameters)]
 
+  def _groups(self):
+    return self.groups
+
   def _encode_latents(self, y, psi):
-    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H W M]."""
-    em = self.entropy_model
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H W M] (substream order
+    with substreams > 1)."""
+    B, H, W = (int(d) for d in y.shape[:3])
     y_hat, y_cc, loc, index = F.scc_encode(self._packed, self.groups, y.contiguous(), psi, self._channel_context,
-                                           self.num_scales)
-    strings = F.compress_f32((y.shape[0],), em._lookup_host(), y_cc, loc, em.cdf_offset.to(y.device), index=index)
-    return strings, y_hat, loc, index
+                                           self.num_scales, substreams=self.substreams)
+    return self._coded(y_cc, loc, index, B, H, W), y_hat, loc, index
 
   def _decode_latents(self, strings, psi):
-    em = self.entropy_model
-    handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
+    handle = self._y_decoder(strings)
     y_hat = F.scc_decode(handle, self._packed, self.groups, psi, self._channel_context, self.num_scales,
-                         em.cdf_offset.to(psi.device))
-    em._finish_decode(handle)
+                         self.entropy_model.cdf_offset.to(psi.device), substreams=self.substreams)
+    self.entropy_model._finish_decode(handle)
     return y_hat
 
   def _encode_ragged(self, ys, psis):
-    return F.scc_encode_ragged(self._packed, self.groups, ys, psis, self._channel_contexts, self.num_scales)[1:]
+    return F.scc_encode_ragged(self._packed, self.groups, ys, psis, self._channel_contexts, self.num_scales,
+                               substreams=self.substreams)[1:]
 
   def _decode_ragged(self, handle, psis, cdf_offset):
     return F.scc_decode_ragged(handle, self._packed, self.groups, psis, self._channel_contexts, self.num_scales,
-                               cdf_offset)
+                               cdf_offset, substreams=self.substreams)
 
 
 # ------------------------------------------------------------------------------------------------

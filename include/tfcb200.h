@@ -367,6 +367,32 @@ int tfcb_scc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_
                             int64_t work_floats, float* dst_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Substreams (DESIGN §3.14): a coding unit (one string of today's format: one image's y or z, one MS2020 slice)
+ * split into S independently decodable streams.  A unit's symbols are in coding order, in phases p = 0 .. P-1
+ * (the order in which the decoder makes them); phase p of unit u has positions[u P + p] positions of
+ * widths[u P + p] symbols each.  Substream s of unit u is the concatenation, over p in order, of the positions
+ * [floor(s n / S), floor((s + 1) n / S)) of phase p (n = its positions), all symbols of each.  Streams are numbered
+ * u S + s.  1 <= S <= 1024; positions >= 0; widths >= 1.
+ * ------------------------------------------------------------------------------------------------ */
+/* The layout on the host, no device work: `stream_offsets_host` [n_units S + 1] the symbol offsets of the streams
+ * for tfcb_compress_ragged (substream order, unit after unit); `phase_lengths_host` [n_phases][n_units S] the
+ * symbols of stream u S + s in phase p, for one tfcb_decode_ragged per phase (whose output is then phase p's
+ * coding order, unit after unit).  Either output may be NULL. */
+int tfcb_substream_layout(int64_t n_units, int64_t n_phases, const int64_t* positions_host,
+                          const int64_t* widths_host, int64_t substreams, int64_t* stream_offsets_host,
+                          int64_t* phase_lengths_host);
+/* Bytes of workspace tfcb_substream_gather needs, or -1 if the arguments are not supported. */
+int64_t tfcb_substream_gather_workspace_bytes(int64_t n_units, int64_t n_phases, int64_t substreams);
+/* Rewrites units held back to back in coding order (unit u's symbols after unit u - 1's) into substream order:
+ * up to three 4-byte operands (y and loc float32, index int32; a NULL input skips that operand, whose output must
+ * then be NULL too, and at least one is given).  One launch (none when there are no symbols), no host
+ * synchronisation; the segment table goes to `work_dev` (8-byte aligned) with one stream-ordered copy. */
+int tfcb_substream_gather(int64_t n_units, int64_t n_phases, const int64_t* positions_host,
+                          const int64_t* widths_host, int64_t substreams, const float* y_dev, const float* loc_dev,
+                          const int32_t* index_dev, float* y_out_dev, float* loc_out_dev, int32_t* index_out_dev,
+                          void* work_dev, int64_t work_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Legacy single-stream ops RangeEncode / RangeDecode (int16 data, broadcastable N-D int32 CDF):
  *   op contract   tensorflow_compression/cc/ops/range_coding_ops.cc:30-124
  *   CPU kernels   tensorflow_compression/cc/kernels/range_coding_kernels.cc:60-379

@@ -8,6 +8,7 @@ arguments.  The images are the PNGs of --images DIR (read with PIL, converted to
 24 seeded smooth-plus-noise images of Kodak's shapes, 12 of 512x768 and 12 of 768x512; with --synthetic mixed, 24
 such images of seeded, all different shapes (sides multiples of 16 from 256 to 1024), as in a dataset of many image
 sizes.  The context models (mbt2018, checkerboard, space_channel) code such a list with one ragged launch sequence.
+--substreams S writes every string as S independently decodable streams (DESIGN §3.14); bpp includes their headers.
 
 --time also measures, alternating the two sides of each pair --reps times after --warmup calls (median ms, CUDA
 events around a synchronised call):
@@ -17,7 +18,8 @@ events around a synchronised call):
 with the library's kernel launches and all CUDA kernels (torch.profiler, one call in a separate pass) of one call of
 each side, and the card's name, power limit and SM clock read in the same run.
 
-  python tools/rd_eval.py --synthetic kodak|mixed [--model bmshj2018] [--num-filters 192] [--state-dict F] [--time]
+  python tools/rd_eval.py --synthetic kodak|mixed [--model bmshj2018] [--num-filters 192] [--state-dict F]
+                          [--substreams S] [--time]
   python tools/rd_eval.py --images DIR ...
 """
 import argparse
@@ -81,9 +83,11 @@ def png_images(directory):
   return [torch.from_numpy(np.asarray(Image.open(os.path.join(directory, n)).convert("RGB")).copy()) for n in names]
 
 
-def make_model(name, num_filters, state_dict, seed):
+def make_model(name, num_filters, state_dict, seed, substreams=1):
   torch.manual_seed(seed)
   kw = {} if num_filters is None else {"num_filters": num_filters}
+  if substreams != 1:
+    kw["substreams"] = substreams
   m = MODELS[name](**kw)
   m.build("cuda")
   if state_dict:
@@ -137,6 +141,8 @@ def parser():
   p.add_argument("--num-filters", type=int, default=None, help="the model's num_filters (default: its own)")
   p.add_argument("--state-dict", default=None, help="torch state_dict of the model to load")
   p.add_argument("--seed", type=int, default=0)
+  p.add_argument("--substreams", type=int, default=1,
+                 help="independently decodable streams per string (DESIGN §3.14; not mbt2018)")
   p.add_argument("--time", action="store_true")
   p.add_argument("--reps", type=int, default=10)
   p.add_argument("--warmup", type=int, default=2)
@@ -153,7 +159,7 @@ def main():
     images = synthetic(args.seed, mixed_shapes(args.seed) if args.synthetic == "mixed" else None)
   else:
     images = png_images(args.images)
-  model = make_model(args.model, args.num_filters, args.state_dict, args.seed)
+  model = make_model(args.model, args.num_filters, args.state_dict, args.seed, args.substreams)
   per_image = model.evaluate_images(images)
   mean = models.mean_metrics(per_image)
   dataset = args.synthetic or os.path.basename(os.path.normpath(args.images))
@@ -163,7 +169,8 @@ def main():
     print("# The first column contains bits per pixel (bpp) values; means over the images at one lambda.")
     print(f"{mean['bpp']:.6f}, {mean[key]:.6f}")
     print()
-  result = {"model": args.model, "dataset": dataset, "n_images": len(images), "mean": mean}
+  result = {"model": args.model, "dataset": dataset, "n_images": len(images), "substreams": args.substreams,
+            "mean": mean}
 
   if args.time:
     gpu = card()
