@@ -175,18 +175,19 @@ def test_nan_and_inf_positions_equal_the_cuda_core_path(F, fp32_path, C_):
 
 
 def _kernels(fn):
-  """Names of the CUDA kernels `fn` launches (a profiler session that recorded no kernel is taken again, at most
-  twice)."""
+  """Names of the CUDA kernels `fn` launches: the union over three profiler sessions of the same call.  A session of a
+  process that has profiled before can miss device events -- all of them, or only some of the call's kernels -- and
+  `fn` launches the same kernels every time, so the union is what it launches (the tests only ask whether some name
+  is or is not among them)."""
   fn()
   torch.cuda.synchronize()
+  names = {}
   for _ in range(3):
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
       fn()
       torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if e.device_type.name == "CUDA"]
-    if any(not n.startswith(("Memcpy", "Memset")) for n in names):
-      break
-  return names
+    names.update(dict.fromkeys(e.name for e in prof.events() if e.device_type.name == "CUDA"))
+  return list(names)
 
 
 def _misaligned(n_pix, C_, seed):

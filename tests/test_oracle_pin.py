@@ -67,7 +67,42 @@ def coder_fuzz_cases():
     wild = isov & (rng.random((S, N)) < 0.2)
     val[wild] = rng.integers(-300, 300, size=int(wild.sum()))
     batches.append((lookup, val, index))
-  return triples, batches
+  return triples, batches + decoder_edge_batches()
+
+
+def decoder_edge_batches():
+  """Seeded (lookup, values, index) batches on the table families the GPU decoder treats specially
+  (tests/test_range_decoder_paths_gpu.py): zero-width bins (leading, interior runs, trailing, an empty escape bin,
+  all but one), one-bin rows (regular and overflow) and precisions 1 to 4; uniform symbols over the nonzero bins."""
+  from test_range_decoder_paths_gpu import cdf_with_empty_bins, rows_of, uniform_symbols
+  rng = np.random.default_rng(78)
+  out = []
+  for t in range(24):
+    nrows, S, N = int(rng.integers(1, 7)), int(rng.integers(1, 4)), int(rng.integers(1, 300))
+    cdfs, precs, ovf = [], [], []
+    for _ in range(nrows):
+      p = int(rng.integers(1, 5)) if t % 3 == 0 else int(rng.integers(1, 17))
+      n = int(rng.integers(1, min(40, 1 << p) + 1))
+      kind = int(rng.integers(0, 5)) if n > 2 else 0
+      if kind == 1:    # leading
+        empty = range(int(rng.integers(1, n)))
+      elif kind == 2:  # trailing (an overflow row's escape bin among them)
+        empty = range(int(rng.integers(1, n)), n)
+      elif kind == 3:  # anywhere, runs included
+        empty = rng.choice(n, size=int(rng.integers(1, n)), replace=False)
+      elif kind == 4:
+        empty = [i for i in range(n) if i != n // 2]
+      else:
+        empty = []
+      cdfs.append(cdf_with_empty_bins(rng, n, p, empty, peaky=2.0))
+      precs.append(p)
+      ovf.append(bool(rng.integers(0, 2)))
+    two_d = t % 2 or util.ambiguous_1d(precs, ovf)
+    lookup = util.make_lookup_2d(cdfs, precs, ovf) if two_d else util.make_lookup_1d(cdfs, precs, ovf)
+    index = rng.integers(0, nrows, size=(S, N)).astype(np.int32) if t % 4 < 2 else None
+    val = uniform_symbols(rng, cdfs, ovf, rows_of(nrows, S, N, index), esc_prob=0.2, esc_lo=-300, esc_hi=300)
+    out.append((lookup, val, index))
+  return out
 
 
 def test_port_equals_compiled_reference_fuzz():

@@ -38,6 +38,12 @@ def make_lookup_1d(cdfs, precisions, overflow, pad=None):
   return np.asarray(out, dtype=np.int32)
 
 
+def ambiguous_1d(precisions, overflow):
+  """Whether a 1-D lookup of these rows reads differently: the grammar skips every value equal to a row's 2^p after
+  it as padding, so a next row whose precision entry is that value (+2, +4, +8, +16) loses it."""
+  return any(not o and q == 1 << p for p, q, o in zip(precisions, precisions[1:], overflow[1:]))
+
+
 def make_lookup_2d(cdfs, precisions, overflow):
   width = max(len(c) for c in cdfs) + 1
   m = np.zeros((len(cdfs), width), dtype=np.int32)
