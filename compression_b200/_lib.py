@@ -77,6 +77,11 @@ SIGNATURES = {
     "tfcb_ar_encode_ragged": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _vp, _vp, _int, _vp, _i64, _vp, _vp, _vp, _vp,
                                      _vp]),
     "tfcb_ar_decode_ragged": (_int, [_vp, _vp, _i64, _int, _vp, _i64, _vp, _vp, _int, _vp, _vp, _i64, _vp, _vp]),
+    "tfcb_ar_tiles_workspace_floats": (_i64, [_i64, _vp, _vp, _i64]),
+    "tfcb_ar_tiles_schedule": (_int, [_i64, _vp, _vp, _i64, _p(_i64), _vp]),
+    "tfcb_ar_encode_tiles": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _vp, _vp, _i64, _int, _vp, _i64, _vp, _vp, _vp,
+                                    _vp, _vp]),
+    "tfcb_ar_decode_tiles": (_int, [_vp, _vp, _i64, _int, _vp, _i64, _vp, _vp, _i64, _int, _vp, _vp, _i64, _vp, _vp]),
     "tfcb_cb_workspace_floats": (_i64, [_int, _i64, _i64, _i64, _int]),
     "tfcb_cb_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64, _int, _vp, _vp, _vp,
                               _vp, _vp, _vp, _vp]),

@@ -21,6 +21,8 @@
 //   in increasing k starting from 0.f, where K is the layer's input width.
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cstring>
 #include <vector>
 
 #include "autoregressive.cuh"
@@ -91,15 +93,26 @@ __device__ __forceinline__ void ar_dense(const float* in, int nin, const float* 
   __syncthreads();
 }
 
+// One work item of the column-tile kernel (§3.15): columns [c0, c1) of row `row` of image `img`, which is tile `tile`
+// of the image (its stream img T + tile).  `self`, `left` and `upper` index the per-(image, non-empty tile) progress
+// counters: the item's own tile, the tile before it in the row (-1 for the first), and the tile holding column
+// min(W - 1, c1 + 1) (-1 in row 0).
+struct ArTileItem {
+  int img, row, c0, c1;
+  int tile, self, left, upper;
+};
+
 // The CTA of image b: positions [P.p0, P.p1) of B images of P.H × P.W, or (RAGGED) every position of image b of the
-// list P.img.
-template <int MODE, bool SMEM_KEYS, bool RAGGED>
-__device__ __forceinline__ void ar_body(const ArParams& P) {
+// list P.img, or (TILE, with RAGGED) the positions of the work item `it`, continuing the stream of its tile.  With
+// TILE the search keys are already in shared memory (SMEM_KEYS) and ŷ of other items is read with coherent loads.
+template <int MODE, bool SMEM_KEYS, bool RAGGED, bool TILE = false>
+__device__ __forceinline__ void ar_body(const ArParams& P, const ArTileItem& it = ArTileItem{}, int tiles = 1) {
   extern __shared__ __align__(16) float s_act[];
   __shared__ __align__(16) uint16_t ring_buf[2 * kRing];  // decoder only: 4096-byte aligned ring, as decode_kernel
   const ArDims d = ar_dims(P.M);
   const int M = P.M;
-  const long long b = blockIdx.x;
+  const long long b = TILE ? (long long)it.img : (long long)blockIdx.x;
+  const long long strm = TILE ? b * tiles + it.tile : b;  // the decoder's stream
   const long long HW = (long long)P.H * P.W;
   // a ragged list's image b (the fixed-shape arithmetic below is left exactly as it was when RAGGED is false)
   ArImage im{};
@@ -125,17 +138,19 @@ __device__ __forceinline__ void ar_body(const ArParams& P) {
     if (SMEM_KEYS) {
       uint2* sp = reinterpret_cast<uint2*>(part + (long long)kArSlices * d.N3);
       int4* sr = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sp) + ((P.n_pairs * 8 + 15) & ~15ll));
-      for (long long i = threadIdx.x; i < P.n_pairs; i += blockDim.x) sp[i] = P.pairs[i];
-      for (int i = threadIdx.x; i < P.n_rows; i += blockDim.x) sr[i] = P.rows4[i];
+      if (!TILE) {  // (the tile kernel copies them once per CTA: ar_tile_keys)
+        for (long long i = threadIdx.x; i < P.n_pairs; i += blockDim.x) sp[i] = P.pairs[i];
+        for (int i = threadIdx.x; i < P.n_rows; i += blockDim.x) sr[i] = P.rows4[i];
+      }
       pairs = sp;
       rows4 = sr;
-      __syncthreads();
+      if (!TILE) __syncthreads();
     }
     ring = ring_buf + (((4096u - (smem_addr(ring_buf) & 4095u)) & 4095u) >> 1);
     if (threadIdx.x < 32) {
-      bw.p = P.bytes + P.offsets[b];
-      bw.len = P.offsets[b + 1] - P.offsets[b];
-      const DecState st = P.state[b];
+      bw.p = P.bytes + P.offsets[strm];
+      bw.len = P.offsets[strm + 1] - P.offsets[strm];
+      const DecState st = P.state[strm];
       c.lane = lane;
       c.base = st.base;
       c.span = st.span;
@@ -154,7 +169,8 @@ __device__ __forceinline__ void ar_body(const ArParams& P) {
     }
   }
 
-  for (int p = RAGGED ? 0 : P.p0; p < (RAGGED ? im.H * im.W : P.p1); ++p) {
+  for (int p = TILE ? it.row * im.W + it.c0 : (RAGGED ? 0 : P.p0);
+       p < (TILE ? it.row * im.W + it.c1 : (RAGGED ? im.H * im.W : P.p1)); ++p) {
     const int py = p / (RAGGED ? im.W : P.W), px = p - py * (RAGGED ? im.W : P.W);
     // ---- gather: the 12 causal neighbours of p (zeros outside the image) and ψ_p ----
     const float* yimg = P.yhat + (RAGGED ? pix0 * M : b * HW * M);
@@ -162,8 +178,10 @@ __device__ __forceinline__ void ar_body(const ArParams& P) {
       const int t = i / M, ch = i - t * M;
       const int yy = py + t / 5 - 2, xx = px + t % 5 - 2;
       float v = 0.f;
-      if (yy >= 0 && xx >= 0 && xx < (RAGGED ? im.W : P.W))
-        v = yimg[((long long)yy * (RAGGED ? im.W : P.W) + xx) * M + ch];  // (yy <= py always)
+      if (yy >= 0 && xx >= 0 && xx < (RAGGED ? im.W : P.W)) {
+        const float* src = yimg + ((long long)yy * (RAGGED ? im.W : P.W) + xx) * M + ch;  // (yy <= py always)
+        v = TILE ? __ldcg(src) : *src;  // (other CTAs' ŷ: L2, never a stale L1 line)
+      }
       taps[i] = v;
     }
     const float* psi = P.psi + (RAGGED ? pix0 + p : b * HW + p) * d.N2;
@@ -231,7 +249,7 @@ __device__ __forceinline__ void ar_body(const ArParams& P) {
     st.span = c.span;
     st.value = c.value;
     st.pos = c.pos2 >> 1;
-    P.state[b] = st;
+    P.state[strm] = st;
   }
 }
 
@@ -243,6 +261,127 @@ __global__ void __launch_bounds__(kArThreads) ar_kernel(const ArParams P) {
 template <int MODE, bool SMEM_KEYS>
 __global__ void __launch_bounds__(kArThreads) ar_ragged_kernel(const ArParams P) {
   ar_body<MODE, SMEM_KEYS, true>(P);
+}
+
+// ---- column tiles (§3.15): one persistent grid over a ticket-ordered table of (image, row, tile) items ----
+struct ArTileParams {
+  ArParams ar;               // ar.img: the image table
+  const ArTileItem* items;   // in ticket order: sorted by (2 row + tile rank, row, image)
+  int n_items, tiles;
+  int* counters;             // rows done per (image, non-empty tile); kArTileFailed marks a tile with a failed item
+  int* sched;                // [0] the next ticket, [1] the abort word, [2] CTAs that have finished
+};
+
+constexpr int kArTileFailed = 1 << 30;
+constexpr unsigned long long kArTileWaitNs = 10000000000ull;  // 10 s: only a scheduling bug can wait this long
+
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ int ld_acquire(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ int ld_relaxed(const int* p) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void add_release(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// Thread 0: waits until item `it` may run: tile u - 1 has finished row r and the tile holding column c1 + 1 has
+// finished row r - 1.  False when the launch is aborted: the abort word is set, a tile it waits on failed, or the wait
+// passes kArTileWaitNs (the first such CTA sets the abort word).  Every CTA then drains its remaining items.
+__device__ __forceinline__ bool ar_tile_wait(const ArTileParams& T, const ArTileItem& it) {
+  const unsigned long long t0 = global_ns();
+  unsigned ns = 32;
+  for (;;) {
+    if (ld_relaxed(T.sched + 1)) return false;
+    const int l = it.left < 0 ? it.row + 1 : ld_acquire(T.counters + it.left);
+    const int u = it.upper < 0 ? it.row : ld_acquire(T.counters + it.upper);
+    if ((l | u) & kArTileFailed) return false;
+    if (l >= it.row + 1 && u >= it.row) return true;
+    if (global_ns() - t0 > kArTileWaitNs) {
+      atomicExch(T.sched + 1, 1);
+      return false;
+    }
+    __nanosleep(ns);
+    ns = min(ns * 2, 1024u);
+  }
+}
+
+// The decoder's search keys, copied once per CTA to where ar_body<..., SMEM_KEYS> finds them (behind the activations).
+__device__ __forceinline__ void ar_tile_keys(const ArParams& P) {
+  extern __shared__ __align__(16) float s_act[];
+  uint2* sp = reinterpret_cast<uint2*>(s_act + ar_act_floats(ar_dims(P.M)));
+  int4* sr = reinterpret_cast<int4*>(reinterpret_cast<uint8_t*>(sp) + ((P.n_pairs * 8 + 15) & ~15ll));
+  for (long long i = threadIdx.x; i < P.n_pairs; i += blockDim.x) sp[i] = P.pairs[i];
+  for (int i = threadIdx.x; i < P.n_rows; i += blockDim.x) sr[i] = P.rows4[i];
+}
+
+// Each CTA takes the next ticket, waits for the item's two dependencies, runs its positions left to right with
+// ar_body (encoder: writes ŷ, loc, index; decoder: continues stream img T + tile from its saved state and saves it
+// back), then publishes the row: ŷ and the state are written, a barrier, a fence and a release add on the counter.
+// Tickets are in an order in which every item comes after the items it waits for, so the lowest unfinished ticket
+// can always run: the schedule finishes for any grid size.  A failed item (aborted launch) writes no ŷ and marks its
+// tile failed; the encoder sets its table indexes to -1, which the range encode rejects, and the last CTA to finish
+// gives every failed tile's stream a state that tfcb_decode_finalize reports as not OK.
+template <int MODE, bool SMEM_KEYS>
+__global__ void __launch_bounds__(kArThreads) ar_tile_kernel(const ArTileParams T) {
+  __shared__ int s_ticket, s_go;
+  const ArParams& P = T.ar;
+  if (MODE == kArDecode && SMEM_KEYS) ar_tile_keys(P);
+  for (;;) {
+    if (threadIdx.x == 0) s_ticket = atomicAdd(T.sched, 1);
+    __syncthreads();
+    const int k = s_ticket;
+    if (k >= T.n_items) break;
+    const ArTileItem it = T.items[k];
+    if (threadIdx.x == 0) s_go = ar_tile_wait(T, it);
+    __syncthreads();
+    const bool go = s_go;
+    if (go) {
+      ar_body<MODE, SMEM_KEYS, true, true>(P, it, T.tiles);  // (ends with a barrier after the last position's ŷ)
+    } else if (MODE == kArEncode) {
+      const ArImage im = P.img[it.img];
+      const long long at = (im.pix + (long long)it.row * im.W + it.c0) * P.M;
+      for (long long e = threadIdx.x; e < (long long)(it.c1 - it.c0) * P.M; e += blockDim.x) P.index_out[at + e] = -1;
+    }
+    if (threadIdx.x == 0) {
+      if (go) {
+        __threadfence();
+        add_release(T.counters + it.self, 1);
+      } else {
+        atomicOr(T.counters + it.self, kArTileFailed);
+      }
+    }
+  }
+  if (MODE == kArDecode) {
+    __shared__ int s_last;
+    if (threadIdx.x == 0) {
+      __threadfence();
+      s_last = atomicAdd(T.sched + 2, 1) == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (s_last && threadIdx.x == 0 && ld_acquire(T.sched + 1)) {  // every other CTA has saved its states
+      for (int k = 0; k < T.n_items; ++k) {
+        const ArTileItem it = T.items[k];
+        if (ld_relaxed(T.counters + it.self) & kArTileFailed) {
+          DecState st;  // base 0 with value 1 (or not read to the end): RangeDecoder::Finalize fails
+          st.base = 0;
+          st.span = 0;
+          st.value = 1;
+          st.pos = 0x7FFFFFFFu;
+          P.state[(long long)it.img * T.tiles + it.tile] = st;
+        }
+      }
+    }
+  }
 }
 
 template <int MODE, bool SMEM_KEYS, bool RAGGED = false>
@@ -304,6 +443,128 @@ int ar_check_decoder(const DecoderView& v, int64_t B, int num_scales) {
                 (long long)B);
   if (v.n_rows < num_scales)
     return fail(TFCB_INVALID_ARGUMENT, "the decoder's tables have %d rows for num_scales=%d", v.n_rows, num_scales);
+  return TFCB_OK;
+}
+
+// ---- column tiles: the schedule and the workspace (image table, item table, counters, ticket, abort, exits) ----
+constexpr int64_t kArMaxTiles = 1024;  // gen_ops.MAX_SUBSTREAMS: the tiles are the substreams of a string
+
+bool ar_tiles_ok(int64_t T) { return T >= 1 && T <= kArMaxTiles; }
+
+int ar_check_tiles(int64_t T) {
+  if (!ar_tiles_ok(T))
+    return fail(TFCB_INVALID_ARGUMENT, "tiles=%lld must be in [1, %lld]", (long long)T, (long long)kArMaxTiles);
+  return TFCB_OK;
+}
+
+// The items of a checked list in ticket order, and the number of progress counters (non-empty tiles of all images).
+// Tile t of an image of width W holds columns [floor(t W / T), floor((t + 1) W / T)); item (i, r, u) is row r of the
+// u-th non-empty tile.  False when the list has more than 2^31 - 1 items.
+bool ar_tile_schedule(int64_t n, const int64_t* hs, const int64_t* ws, int64_t T, std::vector<ArTileItem>* items,
+                      long long* n_counters) {
+  long long total = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    total += hs[i] * std::min<int64_t>(T, ws[i]);
+    if (total > 0x7FFFFFFF) return false;
+  }
+  struct Keyed {
+    long long diag;  // 2 r + u
+    int row;
+    ArTileItem it;
+  };
+  std::vector<Keyed> keyed;
+  keyed.reserve((size_t)total);
+  long long cbase = 0;
+  std::vector<int> tile, c0, c1;
+  for (int64_t i = 0; i < n; ++i) {
+    const int64_t W = ws[i];
+    tile.clear();
+    c0.clear();
+    c1.clear();
+    for (int64_t t = 0; t < T; ++t) {
+      const int64_t a = t * W / T, b = (t + 1) * W / T;
+      if (b > a) {
+        tile.push_back((int)t);
+        c0.push_back((int)a);
+        c1.push_back((int)b);
+      }
+    }
+    const int U = (int)tile.size();
+    for (int u = 0, ur = 0; u < U; ++u) {
+      const int64_t need = std::min<int64_t>(W - 1, (int64_t)c1[u] + 1);  // column c_last + 2
+      while (c1[ur] <= need) ++ur;
+      for (int64_t r = 0; r < hs[i]; ++r) {
+        const ArTileItem it{(int)i, (int)r, c0[u], c1[u], tile[u], (int)(cbase + u), u ? (int)(cbase + u - 1) : -1,
+                            r ? (int)(cbase + ur) : -1};
+        keyed.push_back({2 * r + u, (int)r, it});
+      }
+    }
+    cbase += U;
+  }
+  std::sort(keyed.begin(), keyed.end(), [](const Keyed& x, const Keyed& y) {
+    if (x.diag != y.diag) return x.diag < y.diag;
+    if (x.row != y.row) return x.row < y.row;
+    return x.it.img < y.it.img;
+  });
+  items->resize(keyed.size());
+  for (size_t k = 0; k < keyed.size(); ++k) (*items)[k] = keyed[k].it;
+  *n_counters = cbase;
+  return true;
+}
+
+// Bytes of each workspace section: the image table, the item table, then counters and the three schedule words.
+struct ArTileSpace {
+  long long images, items, words;
+  long long floats() const { return (images + items + words + 3) / 4; }
+};
+
+ArTileSpace ar_tile_space(int64_t n, long long n_items, long long n_counters) {
+  return {n * (long long)sizeof(ArImage), n_items * (long long)sizeof(ArTileItem), (n_counters + 3) * 4};
+}
+
+// The tiles decoder's launch: keys in shared memory when they fit, as ar_launch_decode.
+template <int MODE, bool SMEM_KEYS>
+int ar_tile_launch(const ArTileParams& T, size_t smem, cudaStream_t s) {
+  auto kern = ar_tile_kernel<MODE, SMEM_KEYS>;
+  TFCB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int dev = 0, sms = 0, per_sm = 0;
+  TFCB_CUDA_TRY(cudaGetDevice(&dev));
+  TFCB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  TFCB_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kArThreads, smem));
+  const long long grid = std::min<long long>(T.n_items, (long long)std::max(per_sm, 1) * std::max(sms, 1));
+  kern<<<(unsigned)grid, kArThreads, smem, s>>>(T);
+  TFCB_LAUNCHED();
+  TFCB_CUDA_TRY(cudaGetLastError());
+  return TFCB_OK;
+}
+
+// Checks the workspace, uploads the image and item tables (one stream-ordered copy from pageable memory, staged
+// before the call returns, as ar_upload_table) and resets the counters and schedule words (one memset).
+int ar_tile_prepare(int64_t n, const int64_t* hs, const int64_t* ws, int64_t T, float* work, int64_t work_floats,
+                    ArTileParams* TP, cudaStream_t s) {
+  std::vector<ArTileItem> items;
+  long long n_counters = 0;
+  if (!ar_tile_schedule(n, hs, ws, T, &items, &n_counters))
+    return fail(TFCB_INVALID_ARGUMENT, "the list has more than 2^31 - 1 (row, tile) items");
+  const ArTileSpace sp = ar_tile_space(n, (long long)items.size(), n_counters);
+  TFCB_TRY(ar_check_table_space(work, work_floats, sp.floats(), alignof(ArImage)));
+  std::vector<uint8_t> host((size_t)(sp.images + sp.items));
+  long long pix = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    const ArImage im{pix, (int)hs[i], (int)ws[i]};
+    std::memcpy(host.data() + i * sizeof(ArImage), &im, sizeof(ArImage));
+    pix += hs[i] * ws[i];
+  }
+  std::memcpy(host.data() + sp.images, items.data(), (size_t)sp.items);
+  uint8_t* base = reinterpret_cast<uint8_t*>(work);
+  TFCB_CUDA_TRY(cudaMemcpyAsync(base, host.data(), host.size(), cudaMemcpyHostToDevice, s));
+  TFCB_CUDA_TRY(cudaMemsetAsync(base + sp.images + sp.items, 0, (size_t)sp.words, s));
+  TP->ar.img = reinterpret_cast<const ArImage*>(base);
+  TP->items = reinterpret_cast<const ArTileItem*>(base + sp.images);
+  TP->n_items = (int)items.size();
+  TP->tiles = (int)T;
+  TP->counters = reinterpret_cast<int*>(base + sp.images + sp.items);
+  TP->sched = TP->counters + n_counters;
   return TFCB_OK;
 }
 
@@ -458,6 +719,92 @@ int tfcb_ar_decode_ragged(tfcb_decoder* h, const float* packed_dev, int64_t pack
   cudaStream_t s = as_stream(stream);
   TFCB_TRY(ar_upload_table(n_images, heights_host, widths_host, work_dev, work_floats, &P, s));
   return ar_launch_decode<true>(P, v, n_images, s);
+}
+
+int64_t tfcb_ar_tiles_workspace_floats(int64_t n_images, const int64_t* heights_host, const int64_t* widths_host,
+                                       int64_t tiles) {
+  if (!ar_list_ok(n_images, heights_host, widths_host) || !ar_tiles_ok(tiles)) return -1;
+  std::vector<ArTileItem> items;
+  long long n_counters = 0;
+  if (!ar_tile_schedule(n_images, heights_host, widths_host, tiles, &items, &n_counters)) return -1;
+  return ar_tile_space(n_images, (long long)items.size(), n_counters).floats();
+}
+
+int tfcb_ar_tiles_schedule(int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int64_t tiles,
+                           int64_t* n_items_host, int64_t* items_host) {
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, 1));
+  TFCB_TRY(ar_check_tiles(tiles));
+  if (!n_items_host) return fail(TFCB_INVALID_ARGUMENT, "`n_items` is null");
+  std::vector<ArTileItem> items;
+  long long n_counters = 0;
+  if (!ar_tile_schedule(n_images, heights_host, widths_host, tiles, &items, &n_counters))
+    return fail(TFCB_INVALID_ARGUMENT, "the list has more than 2^31 - 1 (row, tile) items");
+  *n_items_host = (int64_t)items.size();
+  if (items_host)
+    for (size_t k = 0; k < items.size(); ++k) {
+      int64_t* o = items_host + 5 * k;
+      o[0] = items[k].img;
+      o[1] = items[k].row;
+      o[2] = items[k].tile;
+      o[3] = items[k].c0;
+      o[4] = items[k].c1;
+    }
+  return TFCB_OK;
+}
+
+int tfcb_ar_encode_tiles(const float* packed_dev, int64_t packed_floats, int M, const float* y_dev,
+                         const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                         const int64_t* widths_host, int64_t tiles, int num_scales, float* work_dev,
+                         int64_t work_floats, float* yhat_dev, float* loc_dev, int32_t* index_dev,
+                         float* scale_index_dev, void* stream) {
+  TFCB_TRY(ar_check_packed(M, packed_dev, packed_floats));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, num_scales));
+  TFCB_TRY(ar_check_tiles(tiles));
+  if (!y_dev || !psi_dev || !yhat_dev || !loc_dev || !index_dev)
+    return fail(TFCB_INVALID_ARGUMENT, "`y`, `psi`, `yhat`, `loc` or `index` is null");
+  ArTileParams T{};
+  ArParams& P = T.ar;
+  P.packed = packed_dev;
+  P.psi = psi_dev;
+  P.y = y_dev;
+  P.yhat = yhat_dev;
+  P.loc_out = loc_dev;
+  P.scale_out = scale_index_dev;
+  P.index_out = index_dev;
+  P.M = M;
+  P.num_scales = num_scales;
+  cudaStream_t s = as_stream(stream);
+  TFCB_TRY(ar_tile_prepare(n_images, heights_host, widths_host, tiles, work_dev, work_floats, &T, s));
+  return ar_tile_launch<kArEncode, false>(T, ar_act_bytes(M), s);
+}
+
+int tfcb_ar_decode_tiles(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
+                         int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int64_t tiles,
+                         int num_scales, const int32_t* cdf_offset_dev, float* work_dev, int64_t work_floats,
+                         float* yhat_dev, void* stream) {
+  DecoderView v;
+  TFCB_TRY(decoder_view(h, &v));
+  TFCB_TRY(ar_check_packed(M, packed_dev, packed_floats));
+  TFCB_TRY(ar_check_list(n_images, heights_host, widths_host, num_scales));
+  TFCB_TRY(ar_check_tiles(tiles));
+  TFCB_TRY(ar_check_decoder(v, n_images * tiles, num_scales));
+  if (!psi_dev || !yhat_dev || !cdf_offset_dev)
+    return fail(TFCB_INVALID_ARGUMENT, "`psi`, `yhat` or `cdf_offset` is null");
+  ArTileParams T{};
+  ArParams& P = T.ar;
+  P.packed = packed_dev;
+  P.psi = psi_dev;
+  P.yhat = yhat_dev;
+  P.cdf_offset = cdf_offset_dev;
+  P.M = M;
+  P.num_scales = num_scales;
+  ar_set_decoder(v, &P);
+  cudaStream_t s = as_stream(stream);
+  TFCB_TRY(ar_tile_prepare(n_images, heights_host, widths_host, tiles, work_dev, work_floats, &T, s));
+  const size_t act = ar_act_bytes(M);
+  const size_t keys = (size_t)((v.n_pairs * 8 + 15) & ~15ll) + (size_t)v.n_rows * sizeof(int4);
+  if (act + keys <= kArSmemLimit) return ar_tile_launch<kArDecode, true>(T, act + keys, s);
+  return ar_tile_launch<kArDecode, false>(T, act, s);
 }
 
 }  // extern "C"

@@ -1396,6 +1396,93 @@ def ar_decode_ragged(handle, packed, psis, num_scales, cdf_offset):
   return _ragged_views(y_hat, hs, ws, M)
 
 
+# ------------------------------------------------------------------------------------------------
+# Column tiles (DESIGN §3.15): the autoregressive model's latents as T independent streams per image, tile t holding
+# columns [floor(t W / T), floor((t + 1) W / T)) of every row, encoded and decoded as a wavefront over many CTAs.
+# ------------------------------------------------------------------------------------------------
+def ar_tile_layout(hs, ws, tiles, depth=1):
+  """(positions, widths) [images, max H_i] for substream_layout / substream_gather with S = `tiles`: one phase per
+  latent row of W_i positions of `depth` symbols (M for the y strings); rows past H_i have no positions."""
+  import numpy as np
+  gen_ops.check_substreams(tiles, "tiles")
+  hs = np.asarray(hs, dtype=np.int64).reshape(-1)
+  ws = np.asarray(ws, dtype=np.int64).reshape(-1)
+  if hs.size == 0 or hs.size != ws.size or (hs <= 0).any() or (ws <= 0).any():
+    raise _lib.InvalidArgumentError(f"latent shapes {hs.tolist()} x {ws.tolist()}: one positive pair per image")
+  pos = np.where(np.arange(int(hs.max()))[None, :] < hs[:, None], ws[:, None], 0).astype(np.int64)
+  return pos, np.full(pos.shape, int(depth), dtype=np.int64)
+
+
+def ar_tiles_schedule(hs, ws, tiles):
+  """The library's ticket order of a list: int64 [items, 5] rows (image, row, tile, first column, end column)."""
+  import numpy as np
+  hs = np.ascontiguousarray(hs, dtype=np.int64).reshape(-1)
+  ws = np.ascontiguousarray(ws, dtype=np.int64).reshape(-1)
+  if hs.size != ws.size:
+    raise _lib.InvalidArgumentError(f"{hs.size} heights and {ws.size} widths")
+  n = C.c_int64(0)
+  lib = _lib.lib()
+  check(lib.tfcb_ar_tiles_schedule(hs.size, _host(hs), _host(ws), int(tiles), C.byref(n), None))
+  out = np.zeros((n.value, 5), dtype=np.int64)
+  check(lib.tfcb_ar_tiles_schedule(hs.size, _host(hs), _host(ws), int(tiles), C.byref(n), _host(out)))
+  return out
+
+
+def _ar_tiles_work(hs, ws, tiles, dev):
+  nw = int(_lib.lib().tfcb_ar_tiles_workspace_floats(hs.size, _host(hs), _host(ws), int(tiles)))
+  if nw < 0:
+    raise _lib.InvalidArgumentError(f"tiles={tiles} is not supported for this list (1 <= tiles <= 1024)")
+  return torch.empty((nw + 1) // 2, dtype=torch.float64, device=dev), nw  # (8-byte aligned)
+
+
+def ar_encode_tiles(packed, ys, psis, num_scales, tiles, scale_index=False):
+  """ar_encode_ragged over `tiles` = T column tiles per image, in one launch on many CTAs: returns (y_hats, y, loc,
+  index, lengths), and scale_index last with `scale_index=True`.  y_hats are ar_encode_ragged's bit for bit; y, loc,
+  index (and scale_index) are in tile order (image i's tile t at stream i T + t, as substream_gather makes them from
+  ar_tile_layout) and `lengths` holds the n T stream lengths, ready for compress_ragged.  At T > 1 one gather (two
+  with scale_index) follows the launch.  A schedule that could not finish leaves index -1 at the positions it skipped,
+  which compress_ragged rejects."""
+  T = gen_ops.check_substreams(tiles, "tiles")
+  hs, ws, M, n, psi = _ar_ragged(packed, psis)
+  dev = packed.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, loc = torch.empty_like(y), torch.empty_like(y)
+  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
+  scale = torch.empty_like(y) if scale_index else None
+  work, nw = _ar_tiles_work(hs, ws, T, dev)
+  check(_lib.lib().tfcb_ar_encode_tiles(_p(packed), n, M, _p(y), _p(psi), hs.size, _host(hs), _host(ws), T,
+                                        int(num_scales), _p(work), nw, _p(y_hat), _p(loc), _p(index), _p(scale),
+                                        _stream()))
+  out = (y, loc, index) + ((scale,) if scale_index else ())
+  lengths = (hs * ws * M).tolist()
+  if T > 1:
+    pos, wid = ar_tile_layout(hs, ws, T, M)
+    out = substream_gather(pos, wid, T, y, loc, index)
+    if scale_index:
+      out += (substream_gather(pos, wid, T, loc=scale)[1],)
+    lengths = substream_layout(pos, wid, T)[0].tolist()
+  return (_ragged_views(y_hat, hs, ws, M),) + out[:3] + (lengths,) + out[3:]
+
+
+def ar_decode_tiles(handle, packed, psis, num_scales, cdf_offset, tiles):
+  """ar_decode_ragged of strings written in `tiles` = T column tiles: `handle` holds n T streams (image i's tile t at
+  i T + t, gen_ops.split_substreams of the strings).  Returns the list of y_hat [H_i, W_i, M], ar_decode_ragged's bit
+  for bit.  One launch, no host synchronisation; stream errors, including a schedule that could not finish, surface at
+  entropy_decode_finalize."""
+  T = gen_ops.check_substreams(tiles, "tiles")
+  hs, ws, M, n, psi = _ar_ragged(packed, psis)
+  dev = packed.device
+  if handle.n_streams != hs.size * T:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a list of {hs.size}"
+                                    f" in {T} tiles")
+  y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  work, nw = _ar_tiles_work(hs, ws, T, dev)
+  coff = _i32(cdf_offset, dev)
+  check(_lib.lib().tfcb_ar_decode_tiles(handle._h, _p(packed), n, M, _p(psi), hs.size, _host(hs), _host(ws), T,
+                                        int(num_scales), _p(coff), _p(work), nw, _p(y_hat), _stream()))
+  return _ragged_views(y_hat, hs, ws, M)
+
+
 def _scc_ragged(packed, groups, psis):
   """(heights, widths, M, spans, flat psi) of a whole-latent ragged call, with every group's packed buffer checked."""
   hs, ws, M = _ragged_list(psis)

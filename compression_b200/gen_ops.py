@@ -173,12 +173,13 @@ class Strings:
 MAX_SUBSTREAMS = 1024
 
 
-def check_substreams(substreams) -> int:
-  """`substreams` as an int in [1, MAX_SUBSTREAMS]; anything else raises InvalidArgumentError (a ValueError)."""
+def check_substreams(substreams, name="substreams") -> int:
+  """`substreams` as an int in [1, MAX_SUBSTREAMS]; anything else raises InvalidArgumentError (a ValueError).  `name`
+  is the argument's name in the message (MBT2018Model's `tiles` are the substreams of its y strings)."""
   if isinstance(substreams, (bool, np.bool_)) or not isinstance(substreams, (int, np.integer)):
-    raise InvalidArgumentError(f"`substreams` must be an integer: {substreams!r}")
+    raise InvalidArgumentError(f"`{name}` must be an integer: {substreams!r}")
   if not 1 <= int(substreams) <= MAX_SUBSTREAMS:
-    raise InvalidArgumentError(f"`substreams` must be in [1, {MAX_SUBSTREAMS}]: {int(substreams)}")
+    raise InvalidArgumentError(f"`{name}` must be in [1, {MAX_SUBSTREAMS}]: {int(substreams)}")
   return int(substreams)
 
 

@@ -655,14 +655,23 @@ class MBT2018Model(_Model):
   index-mode encode of y with the kernel's table indexes and loc makes the strings (the bytes of
   `LocationScaleIndexedEntropyModel.compress(y, scale_index, loc)`); the decoder runs the parameter step and the
   M symbols of each position in one launch.  The hyper synthesis runs per image, so psi, and with it the decoded
-  latents, do not depend on how images were batched."""
+  latents, do not depend on how images were batched.
+
+  `tiles` = T > 1 (keyword only, at most 1024) writes every y string as T column tiles (DESIGN §3.15): tile t holds
+  columns [floor(t W / T), floor((t + 1) W / T)) of every latent row, coded as its own stream inside the substream
+  container (gen_ops.join_substreams with S = T), and the encoder and decoder run the positions of one image as a
+  wavefront over many SMs (functional.ar_encode_tiles / ar_decode_tiles).  The latents and reconstructions are those
+  of T = 1 bit for bit; only the y strings change, and they must be decoded with the same T.  The z strings are
+  unchanged.  T = 1 is the one-stream model."""
 
   _substream_decoder = False
+  tiles = 1  # (the subclasses' y strings are never tiled)
 
   def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.,
-               substreams=1):
+               substreams=1, *, tiles=1):
     super().__init__()
     self._set_substreams(substreams)
+    self.tiles = gen_ops.check_substreams(tiles, "tiles")
     N, M = int(num_filters), int(latent_depth)
     if M <= 0 or M % 6:
       raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
@@ -746,37 +755,53 @@ class MBT2018Model(_Model):
 
   # -- coding: one latent shape per call --
   def _encode_latents(self, y, psi):
-    """(strings, y_hat, loc, index) of latents y [B, H, W, M] with hyper feature psi."""
+    """(strings, y_hat, loc, index) of latents y [B, H, W, M] with hyper feature psi (loc and index flat in tile order
+    with tiles > 1)."""
     em = self.entropy_model
     y = y.contiguous()
+    if self.tiles > 1:
+      y_hats, y_t, loc, index, lengths = F.ar_encode_tiles(self._packed, list(y), list(psi), self.num_scales,
+                                                           self.tiles)
+      return self._compress_coding_order(y_t, loc, index, lengths, len(y_hats)), torch.stack(y_hats), loc, index
     y_hat, loc, index = F.ar_encode(self._packed, y, psi, self.num_scales)
     strings = F.compress_f32((y.shape[0],), em._lookup_host(), y, loc, em.cdf_offset.to(y.device), index=index)
     return strings, y_hat, loc, index
 
   def _decode_latents(self, strings, psi):
     em = self.entropy_model
+    if self.tiles > 1:
+      handle = self._y_decoder(strings)
+      y_hats = F.ar_decode_tiles(handle, self._packed, list(psi), self.num_scales, em.cdf_offset.to(psi.device),
+                                 self.tiles)
+      em._finish_decode(handle)
+      return torch.stack(y_hats)
     handle = gen_ops.create_range_decoder(em._strings(strings), em._lookup_host())
     y_hat = F.ar_decode(handle, self._packed, psi, self.num_scales, em.cdf_offset.to(psi.device))
     em._finish_decode(handle)
     return y_hat
 
+  def _y_streams(self):
+    """Streams per y string: the substreams, or MBT2018Model's column tiles (at most one of them is above 1)."""
+    return self.substreams * self.tiles
+
   def _y_decoder(self, strings):
-    """A decoder handle of y strings (their substreams with substreams > 1)."""
+    """A decoder handle of y strings (their substreams or tiles when there are several)."""
     em = self.entropy_model
     strings = em._strings(strings)
-    if self.substreams > 1:
-      strings = gen_ops.split_substreams(strings, self.substreams)
+    if self._y_streams() > 1:
+      strings = gen_ops.split_substreams(strings, self._y_streams())
     return gen_ops.create_range_decoder(strings, em._lookup_host())
 
   def _compress_coding_order(self, y, loc, index, lengths, units):
     """The y strings of `units` images from an encoder's coding-order tensors (substream order, and `lengths` the
-    stream lengths, with substreams > 1)."""
+    stream lengths, with substreams or tiles > 1)."""
     em = self.entropy_model
     coff = em.cdf_offset.to(y.device)
-    if self.substreams == 1 and lengths is None:
+    S = self._y_streams()
+    if S == 1 and lengths is None:
       return F.compress_f32((units,), em._lookup_host(), y, loc, coff, index=index)
     strings = F.compress_ragged(em._lookup_host(), lengths, y, loc, coff, index=index)
-    return strings if self.substreams == 1 else gen_ops.join_substreams(strings, self.substreams, (units,))
+    return strings if S == 1 else gen_ops.join_substreams(strings, S, (units,))
 
   def _coded(self, y, loc, index, B, H, W):
     """The y strings of a batch of B latents of H x W from the context models' coding-order tensors (`_groups()` are
@@ -814,11 +839,16 @@ class MBT2018Model(_Model):
 
   # -- lists of differently sized images: transforms per image, one ragged coding call for the whole list --
   def _encode_ragged(self, ys, psis):
-    """(y, loc, index, lengths) in coding order of latents ys [H_i, W_i, M] with hyper features psis."""
+    """(y, loc, index, lengths) in coding order of latents ys [H_i, W_i, M] with hyper features psis (tile order and
+    the stream lengths with tiles > 1)."""
+    if self.tiles > 1:
+      return F.ar_encode_tiles(self._packed, ys, psis, self.num_scales, self.tiles)[1:]
     return F.ar_encode_ragged(self._packed, ys, psis, self.num_scales)[1:]
 
   def _decode_ragged(self, handle, psis, cdf_offset):
-    """The list of y_hat [H_i, W_i, M], continuing `handle` (one string per image)."""
+    """The list of y_hat [H_i, W_i, M], continuing `handle` (one string per image, or one per tile)."""
+    if self.tiles > 1:
+      return F.ar_decode_tiles(handle, self._packed, psis, self.num_scales, cdf_offset, self.tiles)
     return F.ar_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset)
 
   @torch.no_grad()

@@ -272,6 +272,37 @@ int tfcb_ar_decode_ragged(tfcb_decoder* h, const float* packed_dev, int64_t pack
                           int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int num_scales,
                           const int32_t* cdf_offset_dev, float* work_dev, int64_t work_floats, float* yhat_dev,
                           void* stream);
+/* Column tiles (DESIGN §3.15): image i's latents coded as 1 <= tiles = T <= 1024 independent streams, decoded and
+ * encoded as a wavefront over many CTAs.  Tile t of an image of width W holds columns [floor(t W / T),
+ * floor((t + 1) W / T)) of every row (no columns when T > W); its stream is the tile's rows in order, M symbols per
+ * position in channel order: tfcb_substream_layout with S = T and one phase per latent row of W positions of width M.
+ * A work item is one row of one non-empty tile.  Item (i, r, u), u the tile's rank among the row's non-empty tiles,
+ * waits for (i, r, u - 1) and for (i, r - 1, u_R), u_R the tile holding column min(W - 1, c_last + 2); the items run
+ * in ticket order, sorted by (2 r + u, r, i), on a persistent grid (no co-residency is assumed).  ŷ, loc and index
+ * equal tfcb_ar_encode_ragged's / tfcb_ar_decode_ragged's bit for bit.  Every wait is bounded (10 s) and polls an
+ * abort word; an aborted encode sets the index of every position it skipped to -1 (which the range encode rejects),
+ * an aborted decode leaves each failed tile's stream in a state tfcb_decode_finalize reports as not OK.  Per call:
+ * one table upload, one reset of the counters, one launch; no host synchronisation. */
+/* Floats of workspace a tiles call needs (image table, item table, progress counters and schedule words), or -1 if
+ * the list or `tiles` is not supported.  The workspace must be 8-byte aligned. */
+int64_t tfcb_ar_tiles_workspace_floats(int64_t n_images, const int64_t* heights_host, const int64_t* widths_host,
+                                       int64_t tiles);
+/* The ticket order on the host, no device work: *n_items_host receives the number of items and, if `items_host` is
+ * not NULL, items_host [n_items][5] the items in ticket order as (image, row, tile t, first column, end column). */
+int tfcb_ar_tiles_schedule(int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int64_t tiles,
+                           int64_t* n_items_host, int64_t* items_host);
+/* tfcb_ar_encode_ragged over column tiles: the same outputs in the same raster layout. */
+int tfcb_ar_encode_tiles(const float* packed_dev, int64_t packed_floats, int M, const float* y_dev,
+                         const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                         const int64_t* widths_host, int64_t tiles, int num_scales, float* work_dev,
+                         int64_t work_floats, float* yhat_dev, float* loc_dev, int32_t* index_dev,
+                         float* scale_index_dev, void* stream);
+/* tfcb_ar_decode_ragged over column tiles: tile t of image i continues stream i T + t of `h`, which must hold
+ * n_images T strings. */
+int tfcb_ar_decode_tiles(tfcb_decoder* h, const float* packed_dev, int64_t packed_floats, int M, const float* psi_dev,
+                         int64_t n_images, const int64_t* heights_host, const int64_t* widths_host, int64_t tiles,
+                         int num_scales, const int32_t* cdf_offset_dev, float* work_dev, int64_t work_floats,
+                         float* yhat_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Checkerboard context model (He et al. 2021) on the same packed parameters.  A latent position (r, c) is an

@@ -9,6 +9,7 @@ arguments.  The images are the PNGs of --images DIR (read with PIL, converted to
 such images of seeded, all different shapes (sides multiples of 16 from 256 to 1024), as in a dataset of many image
 sizes.  The context models (mbt2018, checkerboard, space_channel) code such a list with one ragged launch sequence.
 --substreams S writes every string as S independently decodable streams (DESIGN §3.14); bpp includes their headers.
+--tiles T (mbt2018 only) writes every y string as T column tiles, coded as a wavefront over many SMs (DESIGN §3.15).
 
 --time also measures, alternating the two sides of each pair --reps times after --warmup calls (median ms, CUDA
 events around a synchronised call):
@@ -19,7 +20,7 @@ with the library's kernel launches and all CUDA kernels (torch.profiler, one cal
 each side, and the card's name, power limit and SM clock read in the same run.
 
   python tools/rd_eval.py --synthetic kodak|mixed [--model bmshj2018] [--num-filters 192] [--state-dict F]
-                          [--substreams S] [--time]
+                          [--substreams S] [--tiles T] [--time]
   python tools/rd_eval.py --images DIR ...
 """
 import argparse
@@ -83,11 +84,15 @@ def png_images(directory):
   return [torch.from_numpy(np.asarray(Image.open(os.path.join(directory, n)).convert("RGB")).copy()) for n in names]
 
 
-def make_model(name, num_filters, state_dict, seed, substreams=1):
+def make_model(name, num_filters, state_dict, seed, substreams=1, tiles=1):
   torch.manual_seed(seed)
   kw = {} if num_filters is None else {"num_filters": num_filters}
   if substreams != 1:
     kw["substreams"] = substreams
+  if tiles != 1:
+    if name != "mbt2018":
+      raise SystemExit(f"--tiles is for mbt2018 only, not {name}")
+    kw["tiles"] = tiles
   m = MODELS[name](**kw)
   m.build("cuda")
   if state_dict:
@@ -143,6 +148,7 @@ def parser():
   p.add_argument("--seed", type=int, default=0)
   p.add_argument("--substreams", type=int, default=1,
                  help="independently decodable streams per string (DESIGN §3.14; not mbt2018)")
+  p.add_argument("--tiles", type=int, default=1, help="column tiles per y string (DESIGN §3.15; mbt2018 only)")
   p.add_argument("--time", action="store_true")
   p.add_argument("--reps", type=int, default=10)
   p.add_argument("--warmup", type=int, default=2)
@@ -159,7 +165,7 @@ def main():
     images = synthetic(args.seed, mixed_shapes(args.seed) if args.synthetic == "mixed" else None)
   else:
     images = png_images(args.images)
-  model = make_model(args.model, args.num_filters, args.state_dict, args.seed, args.substreams)
+  model = make_model(args.model, args.num_filters, args.state_dict, args.seed, args.substreams, args.tiles)
   per_image = model.evaluate_images(images)
   mean = models.mean_metrics(per_image)
   dataset = args.synthetic or os.path.basename(os.path.normpath(args.images))
@@ -170,7 +176,7 @@ def main():
     print(f"{mean['bpp']:.6f}, {mean[key]:.6f}")
     print()
   result = {"model": args.model, "dataset": dataset, "n_images": len(images), "substreams": args.substreams,
-            "mean": mean}
+            "tiles": args.tiles, "mean": mean}
 
   if args.time:
     gpu = card()
