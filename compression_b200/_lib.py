@@ -96,6 +96,16 @@ SIGNATURES = {
     "tfcb_scc_params_ragged": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp,
                                       _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tfcb_scc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _int, _int, _vp, _i64, _vp, _vp]),
+    "tfcb_msc_packed_floats": (_i64, [_int]),
+    "tfcb_msc_pack_weights": (_int, [_int] + [_vp] * 13 + [_i64, _vp]),
+    "tfcb_msc_workspace_floats": (_i64, [_int, _i64, _i64, _i64, _int]),
+    "tfcb_msc_params": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64, _int, _vp, _vp, _vp,
+                               _vp, _vp, _vp, _vp]),
+    "tfcb_msc_scatter": (_int, [_vp, _i64, _i64, _i64, _int, _int, _vp, _vp]),
+    "tfcb_msc_ragged_workspace_floats": (_i64, [_int, _i64, _vp, _vp, _int]),
+    "tfcb_msc_params_ragged": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp, _i64, _int, _vp, _vp,
+                                      _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_msc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _vp, _i64, _vp, _vp]),
     "tfcb_substream_layout": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp]),
     "tfcb_substream_gather_workspace_bytes": (_i64, [_i64, _i64, _i64]),
     "tfcb_substream_gather": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),

@@ -1628,3 +1628,288 @@ def cb_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1)
   scatters for the whole list.  Returns the list of y_hat [H_i, W_i, M]."""
   M = _cb_ragged_check(packed, psis)
   return scc_decode_ragged(handle, [packed], (M,), psis, None, num_scales, cdf_offset, substreams)
+
+
+# ------------------------------------------------------------------------------------------------
+# Multistage context model (Lin et al. 2023): four parameter passes over the stages of a 2x2 schedule (tfcb_msc_*).
+# Position (r, c) has phase (r mod 2, c mod 2); the phases (0, 0), (1, 1), (0, 1), (1, 0) are stages 0 to 3.  Stage
+# s >= 1 reads the decoded latents at its taps (the offsets whose neighbour is in an earlier stage) through its own
+# context kernel; the three 1x1 entropy-parameter layers are shared.  Coding order: per image, stage 0, 1, 2, 3, each
+# in raster order with M channels per position.  Latents are float32 CUDA [B, H, W, M], psi [B, H, W, 2M];
+# coding-order tensors are [B, n_s, M] for one stage and [B, H * W, M] for all four.
+# ------------------------------------------------------------------------------------------------
+MSC_PHASES = ((0, 0), (1, 1), (0, 1), (1, 0))
+
+
+def msc_stage(r, c):
+  """The stage of latent position (r, c)."""
+  return MSC_PHASES.index((r % 2, c % 2))
+
+
+MSC_TAPS = tuple(tuple((dy, dx) for dy in range(-2, 3) for dx in range(-2, 3)
+                       if (dy, dx) != (0, 0) and msc_stage(a + dy, b + dx) < s)
+                 for s, (a, b) in enumerate(MSC_PHASES))  # per stage, raster order: 0, 4, 12 and 16 taps
+
+
+def msc_packed_floats(M):
+  """Floats of the packed parameter buffer for latent depth M (a multiple of 6 in [6, 384])."""
+  n = int(_lib.lib().tfcb_msc_packed_floats(int(M)))
+  if n < 0:
+    raise _lib.InvalidArgumentError(f"latent depth M={M} must be a positive multiple of 6 and at most 384")
+  return n
+
+
+def msc_pack_weights(ctx_kernels, ctx_biases, w1, b1, w2, b2, w3, b3):
+  """The device layout of the four passes: for stages 1, 2 and 3 the taps of its context kernel [5, 5, M, 2M]
+  (masked or not: no other tap is read), gathered as [T_s, M, 2M], and its bias [2M]; then the shared 1x1 layers
+  as [inputs, outputs] and their biases.  Returns float32 [msc_packed_floats(M)] on the kernels' device."""
+  ctx_kernels, ctx_biases = list(ctx_kernels), list(ctx_biases)
+  if len(ctx_kernels) != 3 or len(ctx_biases) != 3:
+    raise _lib.InvalidArgumentError("one context kernel and one bias for each of stages 1, 2 and 3")
+  k = ctx_kernels[0]
+  if k.dim() != 4 or k.shape[:2] != (5, 5) or k.shape[3] != 2 * k.shape[2]:
+    raise _lib.InvalidArgumentError(f"context kernels must be [5, 5, M, 2M]: {tuple(k.shape)}")
+  M = int(k.shape[2])
+  n = msc_packed_floats(M)
+  dev = k.device
+  if dev.type != "cuda":
+    raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
+  n3, n4 = 10 * M // 3, 8 * M // 3
+
+  def operand(t, shape):
+    t = t.detach()
+    if tuple(t.shape) != shape:
+      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where M={M} needs {shape}")
+    return _f32(t, dev)
+
+  ops = []
+  for s, (kernel, bias) in enumerate(zip(ctx_kernels, ctx_biases), 1):
+    kernel = operand(kernel, (5, 5, M, 2 * M))
+    taps = MSC_TAPS[s]
+    ops += [kernel[[dy + 2 for dy, _ in taps], [dx + 2 for _, dx in taps]].contiguous(), operand(bias, (2 * M,))]
+  for t, shape in ((w1, (4 * M, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, 2 * M)), (b3, (2 * M,))):
+    ops.append(operand(t, shape))
+  packed = torch.empty(n, dtype=torch.float32, device=dev)
+  check(_lib.lib().tfcb_msc_pack_weights(M, *[_p(t) for t in ops], _p(packed), n, _stream()))
+  return packed
+
+
+def msc_counts(H, W):
+  """Positions of stages 0 to 3 of an H x W latent: ceil((H - a) / 2) * ceil((W - b) / 2) at phase (a, b)."""
+  return tuple(((H - a + 1) // 2) * ((W - b + 1) // 2) for a, b in MSC_PHASES)
+
+
+def _msc_dims(packed, psi):
+  """(B, H, W, M, packed floats) from psi [B, H, W, 2M], checked against the packed buffer."""
+  if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
+    raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
+  B, H, W, M = int(psi.shape[0]), int(psi.shape[1]), int(psi.shape[2]), int(psi.shape[3]) // 2
+  if B == 0 or H == 0 or W == 0:
+    raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
+  _msc_check_packed(packed, M)
+  if psi.device != packed.device:
+    raise _lib.InvalidArgumentError(f"`packed` ({packed.device}) and `psi` ({psi.device}) must share a CUDA device")
+  return B, H, W, M, packed.numel()
+
+
+def _msc_check_packed(packed, M):
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from msc_pack_weights")
+  n = msc_packed_floats(M)
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, M={M} needs {n}")
+  if packed.device.type != "cuda":
+    raise _lib.InvalidArgumentError(f"`packed` must be on a CUDA device, not {packed.device}")
+  return n
+
+
+def _msc_stage_arg(stage):
+  if int(stage) not in range(4):
+    raise _lib.InvalidArgumentError(f"stage {stage} outside [0, 4)")
+  return int(stage)
+
+
+def _msc_pass(packed, y_hat, psi, stage, num_scales, whole, loc, scale, index, y=None, y_ms=None, y_hat_out=None):
+  B, H, W, M, n = _msc_dims(packed, psi)
+  lib = _lib.lib()
+  nw = int(lib.tfcb_msc_workspace_floats(M, B, H, W, int(stage)))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=packed.device)
+  check(lib.tfcb_msc_params(_p(packed), n, M, _p(y_hat), _p(psi), B, H, W, int(stage), int(num_scales), _p(work), nw,
+                            int(whole), _p(loc), _p(scale), _p(index), _p(y), _p(y_ms), _p(y_hat_out), _stream()))
+
+
+def msc_params(packed, y_hat, psi, stage, num_scales):
+  """One parameter pass: (loc, scale_index, index) [B, n_s, M] (float32, float32, int32) of the n_s positions of
+  stage `stage` of every image, in coding order.  Stages 1-3 read the earlier stages' positions of y_hat
+  [B, H, W, M]; stage 0 reads no latent (y_hat may be None).  Row b depends only on image b."""
+  stage = _msc_stage_arg(stage)
+  B, H, W, M, _ = _msc_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  if y_hat is not None or stage:
+    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  n = msc_counts(H, W)[stage]
+  loc = torch.empty((B, n, M), dtype=torch.float32, device=dev)
+  scale = torch.empty_like(loc)
+  index = torch.empty((B, n, M), dtype=torch.int32, device=dev)
+  _msc_pass(packed, y_hat, psi, stage, num_scales, False, loc, scale, index)
+  return loc, scale, index
+
+
+def msc_phases(hs, ws, M):
+  """positions and widths [images, 4] of the multistage coding order for substream_layout: per image its positions
+  of stages 0 to 3, M symbols each."""
+  import numpy as np
+  hs = np.asarray(hs, dtype=np.int64).reshape(-1)
+  ws = np.asarray(ws, dtype=np.int64).reshape(-1)
+  pos = np.stack([((hs - a + 1) // 2) * ((ws - b + 1) // 2) for a, b in MSC_PHASES], axis=1)
+  return pos, np.full(pos.shape, int(M), dtype=np.int64)
+
+
+def msc_substreams(hs, ws, M, substreams):
+  """(stream_lengths, phase_lengths) of substream_layout for the multistage coding order of images of latent shapes
+  hs[i] x ws[i] and depth M, four phases per image."""
+  return substream_layout(*msc_phases(hs, ws, M), substreams)
+
+
+def _msc_to_substreams(hs, ws, M, substreams, y, loc, index, scale=None):
+  """An encoder's coding-order outputs, rewritten into substream order when `substreams` > 1 (shapes kept)."""
+  out = (y, loc, index) + (() if scale is None else (scale,))
+  if substreams == 1:
+    return out
+  pos, wid = msc_phases(hs, ws, M)
+  moved = substream_gather(pos, wid, substreams, y.reshape(-1), loc.reshape(-1), index.reshape(-1))
+  if scale is not None:
+    moved += (substream_gather(pos, wid, substreams, loc=scale.reshape(-1))[1],)
+  return tuple(m.view(t.shape) for m, t in zip(moved, out))
+
+
+def _msc_phase_lengths(handle, hs, ws, M, substreams, what="batch"):
+  """The decoder's per-stage decode lengths (None for S = 1), after checking the handle's stream count."""
+  S = gen_ops.check_substreams(substreams)
+  units = len(hs)
+  if handle.n_streams != units * S:
+    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a {what} of {units}" +
+                                    ("" if S == 1 else f" in {S} substreams"))
+  return None if S == 1 else msc_substreams(hs, ws, M, S)[1]
+
+
+def msc_encode(packed, y, psi, num_scales, scale_index=False, substreams=1):
+  """The four-pass encoder: returns y_hat [B, H, W, M] and y, loc, index in coding order [B, H * W, M] (and
+  scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc, each stage's before the
+  next stage reads it.  The strings are one index-mode encode of the coding-order y with index and loc.  With
+  `substreams` = S > 1 the coding-order tensors are rewritten into substream order by one gather (a second one for
+  scale_index), ready for compress_ragged with the stream lengths of msc_substreams."""
+  S = gen_ops.check_substreams(substreams)
+  B, H, W, M, _ = _msc_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
+  y_ms, loc = (torch.empty((B, H * W, M), dtype=torch.float32, device=dev) for _ in range(2))
+  index = torch.empty((B, H * W, M), dtype=torch.int32, device=dev)
+  scale = torch.empty_like(loc) if scale_index else None
+  for stage in range(4):
+    _msc_pass(packed, y_hat, psi, stage, num_scales, True, loc, scale, index, y, y_ms, y_hat)
+  return (y_hat,) + _msc_to_substreams([H] * B, [W] * B, M, S, y_ms, loc, index, scale)
+
+
+def msc_decode(handle, packed, psi, num_scales, cdf_offset, substreams=1):
+  """The four-pass decoder, continuing `handle` (a DecoderHandle of B index-mode strings in coding order): per stage
+  its parameters, decode_index_f32 of its positions and their latents to y_hat [B, H, W, M], which it returns.  A
+  fixed number of library launches whatever B, H and W (fewer when a stage is empty, at H = 1 or W = 1) and no host
+  synchronisation; stream errors surface at entropy_decode_finalize.  With `substreams` = S > 1 the handle holds B S
+  substreams (gen_ops.split_substreams) and each stage decodes with one decode_ragged: the same launches."""
+  B, H, W, M, _ = _msc_dims(packed, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  phases = _msc_phase_lengths(handle, [H] * B, [W] * B, M, substreams)
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for stage in range(4):
+    loc, _, index = msc_params(packed, y_hat, psi, stage, num_scales)
+    part = _decode_phase(handle, phases, stage, index, loc, coff)
+    check(lib.tfcb_msc_scatter(_p(part), B, H, W, M, stage, _p(y_hat), _stream()))
+  return y_hat
+
+
+def _msc_ragged(packed, psis):
+  """(heights, widths, M, flat psi) of a ragged multistage call."""
+  hs, ws, M = _ragged_list(psis)
+  _msc_check_packed(packed, M)
+  return hs, ws, M, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed.device)
+
+
+def _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales, whole=False, loc=None, scale=None, index=None,
+                     y=None, y_ms=None, y_hat_out=None):
+  """One stage over the flat list.  Per-stage outputs (whole False, loc None) are allocated: returns (loc,
+  scale_index, index, lengths, work) with image i's n_s,i M values at M Q_i; the workspace holds the image table for
+  the scatter."""
+  n = _msc_check_packed(packed, M)
+  dev = packed.device
+  lib = _lib.lib()
+  k = hs.size
+  a, b = MSC_PHASES[stage]
+  counts = ((hs - a + 1) // 2) * ((ws - b + 1) // 2)
+  if loc is None:
+    total = int(counts.sum()) * M
+    loc, scale = (torch.empty(total, dtype=torch.float32, device=dev) for _ in range(2))
+    index = torch.empty(total, dtype=torch.int32, device=dev)
+  nw = int(lib.tfcb_msc_ragged_workspace_floats(M, k, _host(hs), _host(ws), int(stage)))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
+  check(lib.tfcb_msc_params_ragged(_p(packed), n, M, _p(y_hat), _p(psi), k, _host(hs), _host(ws), int(stage),
+                                   int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale), _p(index), _p(y),
+                                   _p(y_ms), _p(y_hat_out), _stream()))
+  return loc, scale, index, (counts * M).tolist(), work
+
+
+def msc_params_ragged(packed, y_hats, psis, stage, num_scales):
+  """msc_params over a list of images of their own shapes in one pass: returns (loc, scale_index, index, lengths),
+  flat, image i's n_s,i M values after image i - 1's; `lengths` are the n_s,i M.  y_hats is a list of [H_i, W_i, M]
+  (may be None at stage 0).  Image i's values equal msc_params on that image alone, bit for bit."""
+  stage = _msc_stage_arg(stage)
+  hs, ws, M, psi = _msc_ragged(packed, psis)
+  y_hat = None if y_hats is None and not stage else _ragged_cat(y_hats, "y_hat", hs, ws, M, packed.device)
+  return _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales)[:4]
+
+
+def msc_encode_ragged(packed, ys, psis, num_scales, scale_index=False, substreams=1):
+  """msc_encode of a list of images of their own shapes, one four-pass sequence for the whole list: returns (y_hats,
+  y, loc, index, lengths), and scale_index last with `scale_index=True`.  y, loc and index are flat in coding order,
+  image i's H_i W_i M values (its `lengths` entry) after image i - 1's.  With `substreams` = S > 1 they are in
+  substream order (one gather, a second one for scale_index) and `lengths` holds the n S stream lengths, image i's
+  substream s at i S + s."""
+  S = gen_ops.check_substreams(substreams)
+  hs, ws, M, psi = _msc_ragged(packed, psis)
+  dev = psi.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, y_ms, loc = (torch.empty_like(y) for _ in range(3))
+  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
+  scale = torch.empty_like(y) if scale_index else None
+  for stage in range(4):
+    _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales, True, loc, scale, index, y, y_ms, y_hat)
+  out = _msc_to_substreams(hs, ws, M, S, y_ms, loc, index, scale)
+  lengths = (hs * ws * M).tolist() if S == 1 else msc_substreams(hs, ws, M, S)[0].tolist()
+  return (_ragged_views(y_hat, hs, ws, M),) + out[:3] + (lengths,) + out[3:]
+
+
+def msc_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1):
+  """msc_decode of a list of images of their own shapes, continuing `handle` (one index-mode string per image, or S
+  substreams per image): per stage one ragged parameter pass, one decode_ragged and one scatter for the whole list.
+  Returns the list of y_hat [H_i, W_i, M].  The library launches do not depend on the images' number or shapes
+  (fewer when a stage is empty in every image); no host synchronisation."""
+  hs, ws, M, psi = _msc_ragged(packed, psis)
+  dev = psi.device
+  phases = _msc_phase_lengths(handle, hs, ws, M, substreams, "list")
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for stage in range(4):
+    loc, _, index, lengths, work = _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales)
+    if phases is not None:
+      lengths = phases[stage]
+    part = decode_ragged(handle, lengths, index=index, quant_offset=loc, cdf_offset=coff)
+    check(lib.tfcb_msc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, stage, _p(work), work.numel(),
+                                      _p(y_hat), _stream()))
+  return _ragged_views(y_hat, hs, ws, M)

@@ -28,7 +28,7 @@ from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MultistageModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -1077,6 +1077,109 @@ class SpaceChannelModel(MBT2018Model):
   def _decode_ragged(self, handle, psis, cdf_offset):
     return F.scc_decode_ragged(handle, self._packed, self.groups, psis, self._channel_contexts, self.num_scales,
                                cdf_offset, substreams=self.substreams)
+
+
+def multistage_mask(stage, kernel_size=5):
+  """[k, k]: 1 at the offsets (dy, dx) from the centre whose neighbour lies in a stage before `stage` of the 2x2
+  schedule (functional.MSC_TAPS: 0, 4, 12 and 16 taps at k = 5), 0 elsewhere.  The mask is the same at every
+  position of the stage."""
+  h = kernel_size // 2
+  m = torch.zeros(kernel_size, kernel_size)
+  for dy, dx in F.MSC_TAPS[stage]:
+    if abs(dy) <= h and abs(dx) <= h:
+      m[dy + h, dx + h] = 1
+  return m
+
+
+def multistage_stage_map(H, W, device=None):
+  """[H, W] int64: the stage of each position, (0,0) -> 0, (1,1) -> 1, (0,1) -> 2, (1,0) -> 3 on (r mod 2, c mod 2)."""
+  r, c = torch.arange(H, device=device) % 2, torch.arange(W, device=device) % 2
+  table = torch.tensor([[0, 2], [3, 1]], device=device)
+  return table[r[:, None], c[None, :]]
+
+
+class MultistageConv2D(MaskedConv2D):
+  """MaskedConv2D with the mask of one stage s >= 1 of the 2x2 schedule (multistage_mask(s))."""
+
+  def __init__(self, in_channels, filters, stage):
+    super().__init__(in_channels, filters)
+    self.stage = int(stage)
+    self.mask.copy_(multistage_mask(self.stage)[:, :, None, None])
+
+
+def multistage_context(context_models, y):
+  """The context feature of the training path: sum over s of [stage(p) = s] * context_models[s - 1](y)(p) for the
+  stages s = 1, 2, 3.  Stage 0 gets 0 (bias included); a position of stage s gets its stage's masked convolution,
+  which reads only positions of earlier stages."""
+  stage = multistage_stage_map(y.shape[1], y.shape[2], y.device)[None, :, :, None]
+  out = torch.zeros(y.shape[:3] + (2 * y.shape[3],), device=y.device, dtype=y.dtype)
+  for s, cm in enumerate(context_models, 1):
+    out = out + (stage == s).to(y.dtype) * cm(y)
+  return out
+
+
+class MultistageModel(MBT2018Model):
+  """MBT2018Model with a multistage spatial context (after Lin et al., ICASSP 2023): the same transforms, hyper
+  prior, widths and entropy models.  Each 2x2 patch of the latent is coded in four stages, (0,0), (1,1), (0,1),
+  (1,0) by (r mod 2, c mod 2); stage 0 takes a context feature of zero, and stage s >= 1 has its own 5x5 context
+  model M -> 2M (a MultistageConv2D) that sees the stages before it: 4, 12 and 16 taps.  The three 1x1 entropy-
+  parameter layers are shared by the stages.  All positions of a stage are independent, so coding is four parallel
+  passes, and only a quarter of the positions code without spatial context (half with CheckerboardModel).
+
+  Coding runs on the parameter passes (functional.msc_*): the strings are one index-mode encode of y in coding order
+  (each image's stage 0 in raster order, then stages 1, 2 and 3), the bytes of
+  `LocationScaleIndexedEntropyModel.compress(y_ms, scale_index_ms, loc_ms)` of the coding-order tensors; the decoder
+  makes four decode_index_f32 calls on one decoder handle."""
+
+  _substream_decoder = True
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_scales=64, scale_min=.11, scale_max=256.,
+               substreams=1):
+    _Model.__init__(self)
+    self._set_substreams(substreams)
+    N, M = int(num_filters), int(latent_depth)
+    if M <= 0 or M % 6:
+      raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
+    self._init_transforms(lmbda, N, M, num_scales, scale_min, scale_max)
+    self.context_models = nn.ModuleList([MultistageConv2D(M, 2 * M, s) for s in (1, 2, 3)])
+    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
+    self.entropy_parameters = nn.Sequential(
+        ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(2 * M, "layer_2", None))
+    self._init_entropy_models(N)
+
+  def _context(self, y_ctx):
+    return multistage_context(self.context_models, y_ctx)
+
+  def _pack(self):
+    return F.msc_pack_weights([cm.kernel for cm in self.context_models], [cm.bias for cm in self.context_models],
+                              *_dense_weights(self.entropy_parameters))
+
+  def _coded(self, y, loc, index, B, H, W):
+    lengths = None
+    if self.substreams > 1:
+      lengths = F.msc_substreams([H] * B, [W] * B, self.latent_depth, self.substreams)[0]
+    return self._compress_coding_order(y, loc, index, lengths, B)
+
+  def _encode_latents(self, y, psi):
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H * W, M] (substream
+    order with substreams > 1)."""
+    B, H, W = (int(d) for d in y.shape[:3])
+    y_hat, y_ms, loc, index = F.msc_encode(self._packed, y.contiguous(), psi, self.num_scales,
+                                           substreams=self.substreams)
+    return self._coded(y_ms, loc, index, B, H, W), y_hat, loc, index
+
+  def _decode_latents(self, strings, psi):
+    handle = self._y_decoder(strings)
+    y_hat = F.msc_decode(handle, self._packed, psi, self.num_scales, self.entropy_model.cdf_offset.to(psi.device),
+                         substreams=self.substreams)
+    self.entropy_model._finish_decode(handle)
+    return y_hat
+
+  def _encode_ragged(self, ys, psis):
+    return F.msc_encode_ragged(self._packed, ys, psis, self.num_scales, substreams=self.substreams)[1:]
+
+  def _decode_ragged(self, handle, psis, cdf_offset):
+    return F.msc_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset, substreams=self.substreams)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -398,6 +398,61 @@ int tfcb_scc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_
                             int64_t work_floats, float* dst_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Multistage context model (Lin et al. 2023): four position-parallel stages of a 2x2 schedule.  M = latent depth, a
+ * multiple of 6, at most 384.  Position (r, c) has phase (r mod 2, c mod 2) and stage (0,0) -> 0, (1,1) -> 1,
+ * (0,1) -> 2, (1,0) -> 3.  Stage s with phase (a, b) has ceil((H - a) / 2) W_s positions, W_s = ceil((W - b) / 2), the
+ * j-th at (a + 2 floor(j / W_s), b + 2 (j mod W_s)); a stage may be empty (H = 1 or W = 1).  Coding order: per image,
+ * stage 0, 1, 2, 3, each in raster order with M channels per position: [B, H W M] in all.  Per position of stage s:
+ *   ctx = 0 at stage 0 (bias included), else Wc_s * (yhat at the stage's T_s taps) + bc_s            [T_s M] -> [2M]
+ * with the taps (dy, dx) in [-2, 2]^2 whose neighbour lies in an earlier stage, in raster order, zeros outside the
+ * image: T_1 = 4 (dy, dx both odd), T_2 = 12 (dy + dx odd), T_3 = 16 (dy, dx not both even).  Then tfcb_ar_params'
+ * network on [psi, ctx] (4M -> 10M/3 -> 8M/3 -> [loc, scale_index]), shared by the stages, in its float32 order of
+ * operations; stage 0 is tfcb_cb_params' anchor pass bit for bit on the same shared network.
+ * ---------------------------------------------------------------------------------------------- */
+/* Floats of the packed parameters, or -1 if M is not supported: Wc_1 [4, M, 2M], bc_1 [2M], Wc_2 [12, M, 2M], bc_2,
+ * Wc_3 [16, M, 2M], bc_3, W1 [4M, 10M/3], b1, W2 [10M/3, 8M/3], b2, W3 [8M/3, 2M], b3, back to back. */
+int64_t tfcb_msc_packed_floats(int M);
+/* Packs the parameters into `packed_dev`, stream-ordered device copies of the values unchanged; each stage's context
+ * taps already gathered as [T_s, M, 2M] in raster order of its taps. */
+int tfcb_msc_pack_weights(int M, const float* wc1_dev, const float* bc1_dev, const float* wc2_dev,
+                          const float* bc2_dev, const float* wc3_dev, const float* bc3_dev, const float* w1_dev,
+                          const float* b1_dev, const float* w2_dev, const float* b2_dev, const float* w3_dev,
+                          const float* b3_dev, float* packed_dev, int64_t packed_floats, void* stream);
+/* Floats of workspace one tfcb_msc_params pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_msc_workspace_floats(int M, int64_t B, int64_t H, int64_t W, int stage);
+/* One pass over every position of stage `stage` (0 to 3) of all B images.  Stages 1-3 read the earlier stages'
+ * decoded latents from `yhat_dev` [B, H, W, M] (NULL is allowed for stage 0).  Writes loc, scale_index and the table
+ * index (each may be NULL): [B, n_s, M] (whole == 0), or [B, H W M] in coding order at this stage's block
+ * (whole != 0).  Encoder epilogue (y_dev not NULL, [B, H, W, M]): also writes y in coding order to `y_ms_dev` (same
+ * layout as loc) and yhat = float(int32(rint(y - loc))) + loc at this stage's positions of `yhat_out_dev`
+ * [B, H, W, M]; loc and index are then required.  Three launches at stage 0, four at stages 1-3, none for an empty
+ * stage; no host synchronisation. */
+int tfcb_msc_params(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev, const float* psi_dev,
+                    int64_t B, int64_t H, int64_t W, int stage, int num_scales, float* work_dev, int64_t work_floats,
+                    int whole, float* loc_dev, float* scale_index_dev, int32_t* index_dev, const float* y_dev,
+                    float* y_ms_dev, float* yhat_out_dev, void* stream);
+/* Moves one stage's latents from coding order [B, n_s, M] to their positions of `dst_dev` [B, H, W, M] (nothing
+ * else is written).  One launch; none for an empty stage. */
+int tfcb_msc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int stage, float* dst_dev,
+                     void* stream);
+/* Ragged lists, in the layout of tfcb_scc_params_ragged: image i's n_s,i M values at M Q_i (whole == 0), or its
+ * block of its coding order at M (P_i + its positions of the earlier stages) (whole != 0).  Each image's outputs
+ * equal the fixed-shape call on that image alone, bit for bit.  The image table goes to `work_dev` with one
+ * stream-ordered copy; there is no host synchronisation. */
+int64_t tfcb_msc_ragged_workspace_floats(int M, int64_t n_images, const int64_t* heights_host,
+                                         const int64_t* widths_host, int stage);
+int tfcb_msc_params_ragged(const float* packed_dev, int64_t packed_floats, int M, const float* yhat_dev,
+                           const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                           const int64_t* widths_host, int stage, int num_scales, float* work_dev,
+                           int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev, int32_t* index_dev,
+                           const float* y_dev, float* y_ms_dev, float* yhat_out_dev, void* stream);
+/* tfcb_msc_scatter of a ragged list: image i's n_s,i M values at M Q_i -> its [H_i, W_i, M] in `dst_dev`.
+ * `work_dev` holds at least 8 n_images floats (the workspace of a pass of the list does). */
+int tfcb_msc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_t* heights_host,
+                            const int64_t* widths_host, int M, int stage, float* work_dev, int64_t work_floats,
+                            float* dst_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Substreams (DESIGN §3.14): a coding unit (one string of today's format: one image's y or z, one MS2020 slice)
  * split into S independently decodable streams.  A unit's symbols are in coding order, in phases p = 0 .. P-1
  * (the order in which the decoder makes them); phase p of unit u has positions[u P + p] positions of
