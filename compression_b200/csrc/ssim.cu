@@ -58,7 +58,9 @@ struct Window {
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
-__device__ __forceinline__ float to_f32(uint8_t v) { return (float)v * (1.0f / 255.0f); }
+// One rounded multiply, never contracted into a following add: the pool kernel's sum of converted texels must be
+// convert_image_dtype's float32 values added, or the uint8 pyramid differs from the converted images' by roundings.
+__device__ __forceinline__ float to_f32(uint8_t v) { return __fmul_rn((float)v, 1.0f / 255.0f); }
 
 template <typename T>
 __device__ __forceinline__ T from_f32(float v);
@@ -663,13 +665,16 @@ int check_params(float max_val, float filter_sigma) {
   return TFCB_OK;
 }
 
+// The exponent is taken relative to the smallest squared offset m^2 (0 for odd F, 1/4 for even F), as a softmax
+// subtracts its maximum: the central taps are exp(0) = 1 for any sigma, so a tiny sigma at even F gives the box of the
+// central taps instead of 0 / 0.  The difference is exact in double, and for odd F it leaves the window's bits alone.
 Window make_window(int F, float sigma) {
   Window w;
   w.size = F;
   double g[kMaxFilter], sum = 0.0;
-  const double s2 = (double)sigma * sigma, mid = 0.5 * (F - 1);
+  const double s2 = (double)sigma * sigma, mid = 0.5 * (F - 1), m2 = F % 2 ? 0.0 : 0.25;
   for (int k = 0; k < F; ++k) {
-    g[k] = exp(-0.5 * (k - mid) * (k - mid) / s2);
+    g[k] = exp(-0.5 * ((k - mid) * (k - mid) - m2) / s2);
     sum += g[k];
   }
   for (int k = 0; k < kMaxFilter; ++k) w.g[k] = k < F ? g[k] / sum : 0.0;

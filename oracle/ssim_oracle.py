@@ -6,8 +6,13 @@ Images are [..., H, W, C] channels-last.  uint8 is converted as convert_image_dt
 float32(1/255)) before the widening to `dtype`, and so is max_val after a cast to the image dtype; float images are
 cast to float32 first, then widened.  The window is the softmax of -(i^2 + j^2) / (2 sigma^2) over coordinates centred
 at (size - 1) / 2, applied per channel with VALID padding as one 2-D convolution (no separability is assumed).  The
-moments are formed on raw values, S(x^2) - mx^2, which float64 keeps exact enough for the tests.  `dtype` and
+moments are formed on raw values, S(x^2) - mx^2, which float64 keeps exact enough for the gradient tests.  `dtype` and
 `device` let the same graph run in float32 on a GPU as the eager baseline of tools/msssim_bench.py.
+
+`ssim_stats(..., pool="float32")` is the tight reference of the statistics: TF pools in float64 (here) or float32
+(in TF) with its own summation order, while the kernels store every pyramid level as a float32 sum in a fixed order,
+so from scale 1 on, TF and the kernels filter planes that differ by float32 roundings.  The float32 option builds the kernels'
+pyramid bit for bit and computes each scale's statistics in float64 from it, on values centred per plane.
 """
 import math
 
@@ -46,14 +51,16 @@ def filter_valid(x, size, sigma):
   return y.permute(0, 2, 3, 1)
 
 
-def _ssim_per_channel(x, y, max_val, size, sigma, k1, k2):
-  """(mean(l * cs), mean(cs)) over the valid positions, [N, C] each."""
+def _ssim_per_channel(x, y, max_val, size, sigma, k1, k2, shift=0.0):
+  """(mean(l * cs), mean(cs)) over the valid positions, [N, C] each.  cs is formed from x - shift and y - shift (a
+  constant per plane, [N, 1, 1, C]), on which the variances and the covariance are the same; shift = 0 is TF's graph."""
   c1 = (k1 * max_val)**2
   c2 = (k2 * max_val)**2
+  x, y = x - shift, y - shift
   mx, my = filter_valid(x, size, sigma), filter_valid(y, size, sigma)
   num0 = mx * my * 2.0
   den0 = mx**2 + my**2
-  luminance = (num0 + c1) / (den0 + c1)
+  luminance = ((mx + shift) * (my + shift) * 2.0 + c1) / ((mx + shift)**2 + (my + shift)**2 + c1)
   num1 = filter_valid(x * y, size, sigma) * 2.0
   den1 = filter_valid(x**2 + y**2, size, sigma)
   cs = (num1 - num0 + c2) / (den1 - den0 + c2)
@@ -77,20 +84,45 @@ def downsample(x):
   return 0.25 * (x[:, 0::2, 0::2] + x[:, 1::2, 0::2] + x[:, 0::2, 1::2] + x[:, 1::2, 1::2])
 
 
+def downsample32(x):
+  """The pyramid level the kernels store, from float32 x [N, H, W, C]: with the last row / column repeated where H or
+  W is odd, ((x[2r, 2c] + x[2r, 2c + 1]) + (x[2r + 1, 2c] + x[2r + 1, 2c + 1])) * 0.25, each operation one float32
+  rounding in that order."""
+  assert x.dtype == torch.float32
+  h, w = x.shape[1], x.shape[2]
+  x = torch.cat([x, x[:, -1:]], 1) if h % 2 else x
+  x = torch.cat([x, x[:, :, -1:]], 2) if w % 2 else x
+  return ((x[:, 0::2, 0::2] + x[:, 0::2, 1::2]) + (x[:, 1::2, 0::2] + x[:, 1::2, 1::2])) * 0.25
+
+
 def ssim_stats(img1, img2, max_val, n_scales=1, filter_size=11, filter_sigma=1.5, k1=0.01, k2=0.03,
-               dtype=torch.float64):
-  """[..., C, n_scales, 2]: (mean(cs), mean(l * cs)) per channel and scale, the statistics the kernels return."""
+               dtype=torch.float64, pool="float64"):
+  """[..., C, n_scales, 2]: (mean(cs), mean(l * cs)) per channel and scale, the statistics the kernels return.
+
+  pool="float64" is TF's graph in `dtype` (the gradient reference).  pool="float32" computes what the kernels are
+  given: filter_sigma, k1 and k2 rounded to float32 as the library's arguments are, the float32 images and the float32
+  pyramid of `downsample32`, each level widened to float64 and centred on the mean of its two planes before the
+  moments, so the float64 statistics keep their digits on bright content."""
   assert img1.shape == img2.shape and img1.dtype == img2.dtype and img1.dim() >= 3
+  assert pool in ("float64", "float32")
   check_size(img1.shape, n_scales, filter_size)
+  if pool == "float32":
+    filter_sigma, k1, k2 = (float(torch.tensor(v, dtype=torch.float32)) for v in (filter_sigma, k1, k2))
   mv = convert_max_val(max_val, img1.dtype)
   batch = img1.shape[:-3]
-  x = convert(img1, dtype).reshape((-1,) + tuple(img1.shape[-3:]))
-  y = convert(img2, dtype).reshape((-1,) + tuple(img2.shape[-3:]))
+  level = torch.float32 if pool == "float32" else dtype
+  x = convert(img1, level).reshape((-1,) + tuple(img1.shape[-3:]))
+  y = convert(img2, level).reshape((-1,) + tuple(img2.shape[-3:]))
   out = []
   for s in range(n_scales):
     if s:
-      x, y = downsample(x), downsample(y)
-    lcs, cs = _ssim_per_channel(x, y, mv, filter_size, filter_sigma, k1, k2)
+      x, y = (downsample32(x), downsample32(y)) if pool == "float32" else (downsample(x), downsample(y))
+    if pool == "float32":
+      x64, y64 = x.double(), y.double()
+      shift = 0.5 * (x64.mean((1, 2), keepdim=True) + y64.mean((1, 2), keepdim=True))
+      lcs, cs = _ssim_per_channel(x64, y64, mv, filter_size, filter_sigma, k1, k2, shift)
+    else:
+      lcs, cs = _ssim_per_channel(x, y, mv, filter_size, filter_sigma, k1, k2)
     out.append(torch.stack([cs, lcs], -1))
   return torch.stack(out, -2).reshape(tuple(batch) + (img1.shape[-1], n_scales, 2))
 
