@@ -106,6 +106,16 @@ SIGNATURES = {
     "tfcb_msc_params_ragged": (_int, [_vp, _i64, _int, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp, _i64, _int, _vp, _vp,
                                       _vp, _vp, _vp, _vp, _vp]),
     "tfcb_msc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _vp, _i64, _vp, _vp]),
+    "tfcb_mscc_packed_floats": (_i64, [_int, _int, _int, _p(_i64)]),
+    "tfcb_mscc_pack_weights": (_int, [_int, _int, _int] + [_vp] * 13 + [_i64, _vp]),
+    "tfcb_mscc_workspace_floats": (_i64, [_int, _int, _int, _i64, _i64, _i64, _int]),
+    "tfcb_mscc_params": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _i64, _i64, _int, _int, _vp, _i64,
+                                _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_mscc_scatter": (_int, [_vp, _i64, _i64, _i64, _int, _int, _int, _int, _vp, _vp]),
+    "tfcb_mscc_ragged_workspace_floats": (_i64, [_int, _int, _int, _i64, _vp, _vp, _int]),
+    "tfcb_mscc_params_ragged": (_int, [_vp, _i64, _int, _int, _int, _vp, _vp, _vp, _i64, _vp, _vp, _int, _int, _vp,
+                                       _i64, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_mscc_scatter_ragged": (_int, [_vp, _i64, _vp, _vp, _int, _int, _int, _int, _vp, _i64, _vp, _vp]),
     "tfcb_substream_layout": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp]),
     "tfcb_substream_gather_workspace_bytes": (_i64, [_i64, _i64, _i64]),
     "tfcb_substream_gather": (_int, [_i64, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),

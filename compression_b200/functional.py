@@ -559,13 +559,19 @@ def substream_gather(positions, widths, substreams, y=None, loc=None, index=None
   return outs
 
 
-def context_phases(groups, hs, ws):
+def context_phases(groups, hs, ws, multistage=False):
   """positions and widths [images, 2K] of the context models' coding order: per group c_k, its anchors, then its
-  non-anchors (the checkerboard model is the one group (M,))."""
+  non-anchors (the checkerboard model is the one group (M,)).  With `multistage`, [images, 4K]: per group its
+  stages 0 to 3 of the 2x2 schedule (the multistage model is the one group (M,))."""
   import numpy as np
-  hw = np.asarray(hs, dtype=np.int64).reshape(-1) * np.asarray(ws, dtype=np.int64).reshape(-1)
-  pos = np.stack([n for _ in groups for n in ((hw + 1) // 2, hw // 2)], axis=1)
-  wid = np.broadcast_to(np.asarray([int(c) for c in groups for _ in range(2)], dtype=np.int64), pos.shape)
+  hs = np.asarray(hs, dtype=np.int64).reshape(-1)
+  ws = np.asarray(ws, dtype=np.int64).reshape(-1)
+  if multistage:
+    passes = [((hs - a + 1) // 2) * ((ws - b + 1) // 2) for a, b in MSC_PHASES]
+  else:
+    passes = [(hs * ws + 1) // 2, hs * ws // 2]
+  pos = np.stack([n for _ in groups for n in passes], axis=1)
+  wid = np.broadcast_to(np.asarray([int(c) for c in groups for _ in passes], dtype=np.int64), pos.shape)
   return pos, wid
 
 
@@ -1098,31 +1104,31 @@ def cb_decode(handle, packed, psi, num_scales, cdf_offset, substreams=1):
   return y_hat
 
 
-def context_substreams(groups, hs, ws, substreams):
+def context_substreams(groups, hs, ws, substreams, multistage=False):
   """(stream_lengths, phase_lengths) of substream_layout for the context models' coding order of images of latent
-  shapes hs[i] x ws[i] with channel groups `groups`."""
-  return substream_layout(*context_phases(groups, hs, ws), substreams)
+  shapes hs[i] x ws[i] with channel groups `groups` (`multistage` as in context_phases)."""
+  return substream_layout(*context_phases(groups, hs, ws, multistage), substreams)
 
 
-def _to_substreams(groups, hs, ws, substreams, y, loc, index, scale=None):
+def _to_substreams(groups, hs, ws, substreams, y, loc, index, scale=None, multistage=False):
   """An encoder's coding-order outputs, rewritten into substream order when `substreams` > 1 (shapes kept)."""
   out = (y, loc, index) + (() if scale is None else (scale,))
   if substreams == 1:
     return out
-  pos, wid = context_phases(groups, hs, ws)
+  pos, wid = context_phases(groups, hs, ws, multistage)
   moved = substream_gather(pos, wid, substreams, y.reshape(-1), loc.reshape(-1), index.reshape(-1))
   if scale is not None:
     moved += (substream_gather(pos, wid, substreams, loc=scale.reshape(-1))[1],)
   return tuple(m.view(t.shape) for m, t in zip(moved, out))
 
 
-def _substream_phases(handle, groups, hs, ws, substreams, what="batch"):
+def _substream_phases(handle, groups, hs, ws, substreams, what="batch", multistage=False):
   """A context decoder's per-pass decode lengths (None for S = 1), after checking the handle's stream count."""
   units = len(hs)
   if handle.n_streams != units * substreams:
     raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a {what} of {units}" +
                                     ("" if substreams == 1 else f" in {substreams} substreams"))
-  return None if substreams == 1 else context_substreams(groups, hs, ws, substreams)[1]
+  return None if substreams == 1 else context_substreams(groups, hs, ws, substreams, multistage)[1]
 
 
 def _decode_phase(handle, phases, p, index, loc, coff):
@@ -1188,18 +1194,18 @@ def scc_pack_weights(M, group, ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
   return packed
 
 
-def _scc_dims(packed, group, psi):
+def _scc_dims(packed, group, psi, layout=scc_layout):
   """(B, H, W, M, offset, channels, packed floats) from psi [B, H, W, 2M], checked against the group's packed
-  buffer."""
+  buffer (of scc_layout, or mscc_layout for the space-channel multistage model)."""
   if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
     raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
   B, H, W, M = int(psi.shape[0]), int(psi.shape[1]), int(psi.shape[2]), int(psi.shape[3]) // 2
   if B == 0 or H == 0 or W == 0:
     raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
   o, c = (int(v) for v in group)
-  n = scc_layout(M, group)["total"]
+  n = layout(M, group)["total"]
   if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
-    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from scc_pack_weights")
+    raise _lib.InvalidArgumentError(f"`packed` must be a float32 vector from {_PACKERS[layout]}")
   if packed.numel() != n:
     raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, group ({o}, {c}) of M={M} needs {n}")
   if packed.device.type != "cuda" or psi.device != packed.device:
@@ -1247,7 +1253,7 @@ def scc_params(packed, group, y_hat, psi, ch_ctx, anchors, num_scales):
   return loc, scale, index
 
 
-def _scc_batch(packed, groups, psi):
+def _scc_batch(packed, groups, psi, layout=scc_layout):
   """(B, H, W, M, spans, psi) of a whole-latent call, with every group's packed buffer checked."""
   if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
     raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
@@ -1257,7 +1263,7 @@ def _scc_batch(packed, groups, psi):
     raise _lib.InvalidArgumentError(f"{len(packed)} packed networks and groups {tuple(groups)} for a latent of depth "
                                     f"{M}: one network per group, and the groups must sum to M")
   for p, g in zip(packed, spans):
-    B, H, W = _scc_dims(p, g, psi)[:3]
+    B, H, W = _scc_dims(p, g, psi, layout)[:3]
   return B, H, W, M, spans, _ar_tensor(psi, "psi", (B, H, W, 2 * M), psi.device)
 
 
@@ -1483,7 +1489,7 @@ def ar_decode_tiles(handle, packed, psis, num_scales, cdf_offset, tiles):
   return _ragged_views(y_hat, hs, ws, M)
 
 
-def _scc_ragged(packed, groups, psis):
+def _scc_ragged(packed, groups, psis, layout=scc_layout):
   """(heights, widths, M, spans, flat psi) of a whole-latent ragged call, with every group's packed buffer checked."""
   hs, ws, M = _ragged_list(psis)
   spans = scc_spans(groups)
@@ -1491,15 +1497,15 @@ def _scc_ragged(packed, groups, psis):
     raise _lib.InvalidArgumentError(f"{len(packed)} packed networks and groups {tuple(groups)} for a latent of depth "
                                     f"{M}: one network per group, and the groups must sum to M")
   for p, g in zip(packed, spans):
-    _scc_check_packed(p, M, g)
+    _scc_check_packed(p, M, g, layout)
   return hs, ws, M, spans, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed[0].device)
 
 
-def _scc_check_packed(packed, M, group):
+def _scc_check_packed(packed, M, group, layout=scc_layout):
   o, c = (int(v) for v in group)
-  n = scc_layout(M, group)["total"]
+  n = layout(M, group)["total"]
   if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
-    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from scc_pack_weights")
+    raise _lib.InvalidArgumentError(f"`packed` must be a float32 vector from {_PACKERS[layout]}")
   if packed.numel() != n:
     raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, group ({o}, {c}) of M={M} needs {n}")
   if packed.device.type != "cuda":
@@ -1671,27 +1677,35 @@ def msc_pack_weights(ctx_kernels, ctx_biases, w1, b1, w2, b2, w3, b3):
     raise _lib.InvalidArgumentError(f"context kernels must be [5, 5, M, 2M]: {tuple(k.shape)}")
   M = int(k.shape[2])
   n = msc_packed_floats(M)
-  dev = k.device
+  ops = _ms_operands(M, 4 * M, ctx_kernels, ctx_biases, (w1, b1, w2, b2, w3, b3), f"M={M}")
+  packed = torch.empty(n, dtype=torch.float32, device=ops[0].device)
+  check(_lib.lib().tfcb_msc_pack_weights(M, *[_p(t) for t in ops], _p(packed), n, _stream()))
+  return packed
+
+
+def _ms_operands(c, k1, ctx_kernels, ctx_biases, dense, where):
+  """The twelve operands of a multistage network of c channels whose layer 1 is k1 wide, in the library's order:
+  per stage 1-3 the taps of its context kernel [5, 5, c, 2c] gathered as [T_s, c, 2c] and its bias [2c]; then the
+  1x1 layers (W1, b1, W2, b2, W3, b3) as [inputs, outputs] and their biases, K1 -> 5 K1 / 6 -> 2 K1 / 3 -> 2c."""
+  dev = ctx_kernels[0].device
   if dev.type != "cuda":
     raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
-  n3, n4 = 10 * M // 3, 8 * M // 3
+  n3, n4 = 5 * k1 // 6, 2 * k1 // 3
 
   def operand(t, shape):
     t = t.detach()
     if tuple(t.shape) != shape:
-      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where M={M} needs {shape}")
+      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where {where} needs {shape}")
     return _f32(t, dev)
 
   ops = []
   for s, (kernel, bias) in enumerate(zip(ctx_kernels, ctx_biases), 1):
-    kernel = operand(kernel, (5, 5, M, 2 * M))
+    kernel = operand(kernel, (5, 5, c, 2 * c))
     taps = MSC_TAPS[s]
-    ops += [kernel[[dy + 2 for dy, _ in taps], [dx + 2 for _, dx in taps]].contiguous(), operand(bias, (2 * M,))]
-  for t, shape in ((w1, (4 * M, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, 2 * M)), (b3, (2 * M,))):
+    ops += [kernel[[dy + 2 for dy, _ in taps], [dx + 2 for _, dx in taps]].contiguous(), operand(bias, (2 * c,))]
+  for t, shape in zip(dense, ((k1, n3), (n3,), (n3, n4), (n4,), (n4, 2 * c), (2 * c,))):
     ops.append(operand(t, shape))
-  packed = torch.empty(n, dtype=torch.float32, device=dev)
-  check(_lib.lib().tfcb_msc_pack_weights(M, *[_p(t) for t in ops], _p(packed), n, _stream()))
-  return packed
+  return ops
 
 
 def msc_counts(H, W):
@@ -1729,69 +1743,26 @@ def _msc_stage_arg(stage):
   return int(stage)
 
 
-def _msc_pass(packed, y_hat, psi, stage, num_scales, whole, loc, scale, index, y=None, y_ms=None, y_hat_out=None):
-  B, H, W, M, n = _msc_dims(packed, psi)
-  lib = _lib.lib()
-  nw = int(lib.tfcb_msc_workspace_floats(M, B, H, W, int(stage)))
-  work = torch.empty(max(nw, 1), dtype=torch.float32, device=packed.device)
-  check(lib.tfcb_msc_params(_p(packed), n, M, _p(y_hat), _p(psi), B, H, W, int(stage), int(num_scales), _p(work), nw,
-                            int(whole), _p(loc), _p(scale), _p(index), _p(y), _p(y_ms), _p(y_hat_out), _stream()))
-
-
 def msc_params(packed, y_hat, psi, stage, num_scales):
   """One parameter pass: (loc, scale_index, index) [B, n_s, M] (float32, float32, int32) of the n_s positions of
   stage `stage` of every image, in coding order.  Stages 1-3 read the earlier stages' positions of y_hat
-  [B, H, W, M]; stage 0 reads no latent (y_hat may be None).  Row b depends only on image b."""
+  [B, H, W, M]; stage 0 reads no latent (y_hat may be None).  Row b depends only on image b.  (mscc_params of the
+  one group (0, M), bit for bit.)"""
   stage = _msc_stage_arg(stage)
-  B, H, W, M, _ = _msc_dims(packed, psi)
-  dev = packed.device
-  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
-  if y_hat is not None or stage:
-    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
-  n = msc_counts(H, W)[stage]
-  loc = torch.empty((B, n, M), dtype=torch.float32, device=dev)
-  scale = torch.empty_like(loc)
-  index = torch.empty((B, n, M), dtype=torch.int32, device=dev)
-  _msc_pass(packed, y_hat, psi, stage, num_scales, False, loc, scale, index)
-  return loc, scale, index
+  M = _msc_dims(packed, psi)[3]
+  return mscc_params(packed, (0, M), y_hat, psi, None, stage, num_scales)
 
 
 def msc_phases(hs, ws, M):
   """positions and widths [images, 4] of the multistage coding order for substream_layout: per image its positions
   of stages 0 to 3, M symbols each."""
-  import numpy as np
-  hs = np.asarray(hs, dtype=np.int64).reshape(-1)
-  ws = np.asarray(ws, dtype=np.int64).reshape(-1)
-  pos = np.stack([((hs - a + 1) // 2) * ((ws - b + 1) // 2) for a, b in MSC_PHASES], axis=1)
-  return pos, np.full(pos.shape, int(M), dtype=np.int64)
+  return context_phases((M,), hs, ws, multistage=True)
 
 
 def msc_substreams(hs, ws, M, substreams):
   """(stream_lengths, phase_lengths) of substream_layout for the multistage coding order of images of latent shapes
   hs[i] x ws[i] and depth M, four phases per image."""
-  return substream_layout(*msc_phases(hs, ws, M), substreams)
-
-
-def _msc_to_substreams(hs, ws, M, substreams, y, loc, index, scale=None):
-  """An encoder's coding-order outputs, rewritten into substream order when `substreams` > 1 (shapes kept)."""
-  out = (y, loc, index) + (() if scale is None else (scale,))
-  if substreams == 1:
-    return out
-  pos, wid = msc_phases(hs, ws, M)
-  moved = substream_gather(pos, wid, substreams, y.reshape(-1), loc.reshape(-1), index.reshape(-1))
-  if scale is not None:
-    moved += (substream_gather(pos, wid, substreams, loc=scale.reshape(-1))[1],)
-  return tuple(m.view(t.shape) for m, t in zip(moved, out))
-
-
-def _msc_phase_lengths(handle, hs, ws, M, substreams, what="batch"):
-  """The decoder's per-stage decode lengths (None for S = 1), after checking the handle's stream count."""
-  S = gen_ops.check_substreams(substreams)
-  units = len(hs)
-  if handle.n_streams != units * S:
-    raise _lib.InvalidArgumentError(f"the decoder holds {handle.n_streams} strings for a {what} of {units}" +
-                                    ("" if S == 1 else f" in {S} substreams"))
-  return None if S == 1 else msc_substreams(hs, ws, M, S)[1]
+  return context_substreams((M,), hs, ws, substreams, multistage=True)
 
 
 def msc_encode(packed, y, psi, num_scales, scale_index=False, substreams=1):
@@ -1802,16 +1773,8 @@ def msc_encode(packed, y, psi, num_scales, scale_index=False, substreams=1):
   scale_index), ready for compress_ragged with the stream lengths of msc_substreams."""
   S = gen_ops.check_substreams(substreams)
   B, H, W, M, _ = _msc_dims(packed, psi)
-  dev = packed.device
-  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
-  y = _ar_tensor(y, "y", (B, H, W, M), dev)
-  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
-  y_ms, loc = (torch.empty((B, H * W, M), dtype=torch.float32, device=dev) for _ in range(2))
-  index = torch.empty((B, H * W, M), dtype=torch.int32, device=dev)
-  scale = torch.empty_like(loc) if scale_index else None
-  for stage in range(4):
-    _msc_pass(packed, y_hat, psi, stage, num_scales, True, loc, scale, index, y, y_ms, y_hat)
-  return (y_hat,) + _msc_to_substreams([H] * B, [W] * B, M, S, y_ms, loc, index, scale)
+  out = mscc_encode([packed], (M,), y, psi, None, num_scales, scale_index, S)
+  return out[:1] + tuple(t.view(B, H * W, M) for t in out[1:])
 
 
 def msc_decode(handle, packed, psi, num_scales, cdf_offset, substreams=1):
@@ -1820,48 +1783,15 @@ def msc_decode(handle, packed, psi, num_scales, cdf_offset, substreams=1):
   fixed number of library launches whatever B, H and W (fewer when a stage is empty, at H = 1 or W = 1) and no host
   synchronisation; stream errors surface at entropy_decode_finalize.  With `substreams` = S > 1 the handle holds B S
   substreams (gen_ops.split_substreams) and each stage decodes with one decode_ragged: the same launches."""
-  B, H, W, M, _ = _msc_dims(packed, psi)
-  dev = packed.device
-  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
-  phases = _msc_phase_lengths(handle, [H] * B, [W] * B, M, substreams)
-  coff = _i32(cdf_offset, dev)
-  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
-  lib = _lib.lib()
-  for stage in range(4):
-    loc, _, index = msc_params(packed, y_hat, psi, stage, num_scales)
-    part = _decode_phase(handle, phases, stage, index, loc, coff)
-    check(lib.tfcb_msc_scatter(_p(part), B, H, W, M, stage, _p(y_hat), _stream()))
-  return y_hat
+  M = _msc_dims(packed, psi)[3]
+  return mscc_decode(handle, [packed], (M,), psi, None, num_scales, cdf_offset, gen_ops.check_substreams(substreams))
 
 
-def _msc_ragged(packed, psis):
-  """(heights, widths, M, flat psi) of a ragged multistage call."""
-  hs, ws, M = _ragged_list(psis)
+def _msc_ragged_check(packed, psis):
+  """M of a ragged multistage call, with the packed buffer checked."""
+  M = _ragged_list(psis)[2]
   _msc_check_packed(packed, M)
-  return hs, ws, M, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed.device)
-
-
-def _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales, whole=False, loc=None, scale=None, index=None,
-                     y=None, y_ms=None, y_hat_out=None):
-  """One stage over the flat list.  Per-stage outputs (whole False, loc None) are allocated: returns (loc,
-  scale_index, index, lengths, work) with image i's n_s,i M values at M Q_i; the workspace holds the image table for
-  the scatter."""
-  n = _msc_check_packed(packed, M)
-  dev = packed.device
-  lib = _lib.lib()
-  k = hs.size
-  a, b = MSC_PHASES[stage]
-  counts = ((hs - a + 1) // 2) * ((ws - b + 1) // 2)
-  if loc is None:
-    total = int(counts.sum()) * M
-    loc, scale = (torch.empty(total, dtype=torch.float32, device=dev) for _ in range(2))
-    index = torch.empty(total, dtype=torch.int32, device=dev)
-  nw = int(lib.tfcb_msc_ragged_workspace_floats(M, k, _host(hs), _host(ws), int(stage)))
-  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
-  check(lib.tfcb_msc_params_ragged(_p(packed), n, M, _p(y_hat), _p(psi), k, _host(hs), _host(ws), int(stage),
-                                   int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale), _p(index), _p(y),
-                                   _p(y_ms), _p(y_hat_out), _stream()))
-  return loc, scale, index, (counts * M).tolist(), work
+  return M
 
 
 def msc_params_ragged(packed, y_hats, psis, stage, num_scales):
@@ -1869,9 +1799,8 @@ def msc_params_ragged(packed, y_hats, psis, stage, num_scales):
   flat, image i's n_s,i M values after image i - 1's; `lengths` are the n_s,i M.  y_hats is a list of [H_i, W_i, M]
   (may be None at stage 0).  Image i's values equal msc_params on that image alone, bit for bit."""
   stage = _msc_stage_arg(stage)
-  hs, ws, M, psi = _msc_ragged(packed, psis)
-  y_hat = None if y_hats is None and not stage else _ragged_cat(y_hats, "y_hat", hs, ws, M, packed.device)
-  return _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales)[:4]
+  M = _msc_ragged_check(packed, psis)
+  return mscc_params_ragged(packed, (0, M), y_hats, psis, None, stage, num_scales)
 
 
 def msc_encode_ragged(packed, ys, psis, num_scales, scale_index=False, substreams=1):
@@ -1881,17 +1810,8 @@ def msc_encode_ragged(packed, ys, psis, num_scales, scale_index=False, substream
   substream order (one gather, a second one for scale_index) and `lengths` holds the n S stream lengths, image i's
   substream s at i S + s."""
   S = gen_ops.check_substreams(substreams)
-  hs, ws, M, psi = _msc_ragged(packed, psis)
-  dev = psi.device
-  y = _ragged_cat(ys, "y", hs, ws, M, dev)
-  y_hat, y_ms, loc = (torch.empty_like(y) for _ in range(3))
-  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
-  scale = torch.empty_like(y) if scale_index else None
-  for stage in range(4):
-    _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales, True, loc, scale, index, y, y_ms, y_hat)
-  out = _msc_to_substreams(hs, ws, M, S, y_ms, loc, index, scale)
-  lengths = (hs * ws * M).tolist() if S == 1 else msc_substreams(hs, ws, M, S)[0].tolist()
-  return (_ragged_views(y_hat, hs, ws, M),) + out[:3] + (lengths,) + out[3:]
+  M = _msc_ragged_check(packed, psis)
+  return mscc_encode_ragged([packed], (M,), ys, psis, None, num_scales, scale_index, S)
 
 
 def msc_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1):
@@ -1899,17 +1819,208 @@ def msc_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1
   substreams per image): per stage one ragged parameter pass, one decode_ragged and one scatter for the whole list.
   Returns the list of y_hat [H_i, W_i, M].  The library launches do not depend on the images' number or shapes
   (fewer when a stage is empty in every image); no host synchronisation."""
-  hs, ws, M, psi = _msc_ragged(packed, psis)
+  M = _msc_ragged_check(packed, psis)
+  return mscc_decode_ragged(handle, [packed], (M,), psis, None, num_scales, cdf_offset,
+                            gen_ops.check_substreams(substreams))
+
+
+# ------------------------------------------------------------------------------------------------
+# Space-channel multistage context model (DESIGN §3.17): the space-channel model's channel groups (scc_spans), each
+# coded in the four stages of the multistage schedule (tfcb_mscc_*).  Group k has its own packed network
+# (mscc_pack_weights): a context kernel per stage 1-3 over its own c_k channels, and three 1x1 layers shared by its
+# stages whose layer 1 reads [psi, the channel context of group k (none for k = 0), its spatial context].  Coding
+# order: per image, group 0's stages 0, 1, 2, 3, then group 1's, ..., each stage in raster order with c_k channels
+# per position; the coding-order tensors are [B, H * W * M].  The multistage model (msc_*) is the one group (M,).
+# ------------------------------------------------------------------------------------------------
+def mscc_layout(M, group):
+  """The library's packed layout of group (offset, channels) of a depth-M latent: a dict of the widths K1, N3, N4,
+  the offsets of wc1, bc1, wc2, bc2, wc3, bc3, w1, b1, w2, b2, w3, b3 and the `total` floats."""
+  o, c = (int(v) for v in group)
+  out = (C.c_int64 * 15)()
+  n = int(_lib.lib().tfcb_mscc_packed_floats(int(M), o, c, out))
+  if n < 0:
+    raise _lib.InvalidArgumentError(f"group of {c} channels at offset {o} of a latent of depth M={M}: M must be a "
+                                    "positive even number at most 1024, with every channel inside it")
+  keys = ("K1", "N3", "N4", "wc1", "bc1", "wc2", "bc2", "wc3", "bc3", "w1", "b1", "w2", "b2", "w3", "b3")
+  return dict(zip(keys, (int(v) for v in out)), total=n)
+
+
+_PACKERS = {scc_layout: "scc_pack_weights", mscc_layout: "mscc_pack_weights"}
+
+
+def mscc_pack_weights(M, group, ctx_kernels, ctx_biases, w1, b1, w2, b2, w3, b3):
+  """The device layout of group (offset, channels)'s four passes: for stages 1, 2 and 3 the taps of its context
+  kernel [5, 5, c, 2c] (masked or not: no other tap is read), gathered as [T_s, c, 2c], and its bias [2c]; then the
+  group's 1x1 layers as [inputs, outputs] and their biases, with the widths mscc_layout gives.  Returns float32
+  [total] on the kernels' device."""
+  o, c = (int(v) for v in group)
+  lay = mscc_layout(M, group)
+  ctx_kernels, ctx_biases = list(ctx_kernels), list(ctx_biases)
+  if len(ctx_kernels) != 3 or len(ctx_biases) != 3:
+    raise _lib.InvalidArgumentError("one context kernel and one bias for each of stages 1, 2 and 3")
+  ops = _ms_operands(c, lay["K1"], ctx_kernels, ctx_biases, (w1, b1, w2, b2, w3, b3), f"group ({o}, {c}) of M={M}")
+  packed = torch.empty(lay["total"], dtype=torch.float32, device=ops[0].device)
+  check(_lib.lib().tfcb_mscc_pack_weights(int(M), o, c, *[_p(t) for t in ops], _p(packed), lay["total"], _stream()))
+  return packed
+
+
+def _mscc_pass(packed, group, y_hat, psi, ch_ctx, stage, num_scales, whole, loc, scale, index, y=None, y_cc=None,
+               y_hat_out=None):
+  B, H, W, M, o, c, n = _scc_dims(packed, group, psi, mscc_layout)
+  lib = _lib.lib()
+  nw = int(lib.tfcb_mscc_workspace_floats(M, o, c, B, H, W, int(stage)))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=packed.device)
+  check(lib.tfcb_mscc_params(_p(packed), n, M, o, c, _p(y_hat), _p(psi), _p(ch_ctx), B, H, W, int(stage),
+                             int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale), _p(index), _p(y), _p(y_cc),
+                             _p(y_hat_out), _stream()))
+
+
+def mscc_params(packed, group, y_hat, psi, ch_ctx, stage, num_scales):
+  """One parameter pass of group (offset, channels): (loc, scale_index, index) [B, n_s, c] (float32, float32, int32)
+  of the n_s positions of stage `stage` of every image, in coding order.  ch_ctx [B, H, W, 2c] is the group's
+  channel context (None at offset 0); stages 1-3 read the group's channels of the earlier stages' positions of y_hat
+  [B, H, W, M] (y_hat may be None at stage 0).  Row b depends only on image b."""
+  stage = _msc_stage_arg(stage)
+  B, H, W, M, o, c, _ = _scc_dims(packed, group, psi, mscc_layout)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  ch_ctx = _scc_ch_ctx(ch_ctx, group, (B, H, W), dev)
+  if y_hat is not None or stage:
+    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  n = msc_counts(H, W)[stage]
+  loc = torch.empty((B, n, c), dtype=torch.float32, device=dev)
+  scale = torch.empty_like(loc)
+  index = torch.empty((B, n, c), dtype=torch.int32, device=dev)
+  _mscc_pass(packed, group, y_hat, psi, ch_ctx, stage, num_scales, False, loc, scale, index)
+  return loc, scale, index
+
+
+def mscc_encode(packed, groups, y, psi, channel_context, num_scales, scale_index=False, substreams=1):
+  """The group-by-group, stage-by-stage encoder: `packed` holds one mscc_pack_weights buffer per group.  Per group k,
+  its channel context `channel_context(k, y_hat)` [B, H, W, 2c_k] (called for k >= 1, once y_hat holds groups 0 to
+  k - 1), then its stages 0 to 3.  Returns y_hat [B, H, W, M] and y, loc, index in coding order [B, H * W * M] (and
+  scale_index last with `scale_index=True`).  y_hat = float(int32(rint(y - loc))) + loc.  The strings are one
+  index-mode encode of the coding-order y with index and loc.  With `substreams` = S > 1 the coding-order tensors
+  are rewritten into substream order (4K phases per image), ready for compress_ragged with the stream lengths of
+  context_substreams(groups, ..., multistage=True)."""
+  S = gen_ops.check_substreams(substreams)
+  B, H, W, M, spans, psi = _scc_batch(packed, groups, psi, mscc_layout)
   dev = psi.device
-  phases = _msc_phase_lengths(handle, hs, ws, M, substreams, "list")
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
+  y_cc, loc = (torch.empty((B, H * W * M), dtype=torch.float32, device=dev) for _ in range(2))
+  index = torch.empty((B, H * W * M), dtype=torch.int32, device=dev)
+  scale = torch.empty_like(loc) if scale_index else None
+  for k, (p, g) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx(channel_context(k, y_hat) if k else None, g, (B, H, W), dev)
+    for stage in range(4):
+      _mscc_pass(p, g, y_hat, psi, ch, stage, num_scales, True, loc, scale, index, y, y_cc, y_hat)
+  return (y_hat,) + _to_substreams(groups, [H] * B, [W] * B, S, y_cc, loc, index, scale, multistage=True)
+
+
+def mscc_decode(handle, packed, groups, psi, channel_context, num_scales, cdf_offset, substreams=1):
+  """The group-by-group, stage-by-stage decoder, continuing `handle` (a DecoderHandle of B index-mode strings in
+  coding order, or B S substreams): per group its channel context (as in mscc_encode), then per stage the parameter
+  pass, one decode call and the scatter into y_hat [B, H, W, M], which it returns.  4K decode calls on the handle;
+  per group a fixed number of library launches whatever B, H and W (fewer when a stage is empty, at H = 1 or W = 1),
+  and no host synchronisation; stream errors surface at entropy_decode_finalize."""
+  B, H, W, M, spans, psi = _scc_batch(packed, groups, psi, mscc_layout)
+  dev = psi.device
+  phases = _substream_phases(handle, groups, [H] * B, [W] * B, substreams, multistage=True)
+  coff = _i32(cdf_offset, dev)
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for k, (p, (o, c)) in enumerate(zip(packed, spans)):
+    ch = channel_context(k, y_hat) if k else None
+    for stage in range(4):
+      loc, _, index = mscc_params(p, (o, c), y_hat, psi, ch, stage, num_scales)
+      part = _decode_phase(handle, phases, 4 * k + stage, index, loc, coff)
+      check(lib.tfcb_mscc_scatter(_p(part), B, H, W, M, o, c, stage, _p(y_hat), _stream()))
+  return y_hat
+
+
+def _mscc_pass_ragged(packed, group, M, hs, ws, y_hat, psi, ch_ctx, stage, num_scales, whole=False, loc=None,
+                      scale=None, index=None, y=None, y_cc=None, y_hat_out=None):
+  """One stage of group (offset, channels) over the flat list.  Per-stage outputs (whole False, loc None) are
+  allocated: returns (loc, scale_index, index, lengths, work) with image i's n_s,i c values at c Q_i; the workspace
+  holds the image table for the scatter."""
+  o, c = (int(v) for v in group)
+  n = _scc_check_packed(packed, M, group, mscc_layout)
+  dev = packed.device
+  lib = _lib.lib()
+  k = hs.size
+  a, b = MSC_PHASES[stage]
+  counts = ((hs - a + 1) // 2) * ((ws - b + 1) // 2)
+  if loc is None:
+    total = int(counts.sum()) * c
+    loc, scale = (torch.empty(total, dtype=torch.float32, device=dev) for _ in range(2))
+    index = torch.empty(total, dtype=torch.int32, device=dev)
+  nw = int(lib.tfcb_mscc_ragged_workspace_floats(M, o, c, k, _host(hs), _host(ws), int(stage)))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
+  check(lib.tfcb_mscc_params_ragged(_p(packed), n, M, o, c, _p(y_hat), _p(psi), _p(ch_ctx), k, _host(hs), _host(ws),
+                                    int(stage), int(num_scales), _p(work), nw, int(whole), _p(loc), _p(scale),
+                                    _p(index), _p(y), _p(y_cc), _p(y_hat_out), _stream()))
+  return loc, scale, index, (counts * c).tolist(), work
+
+
+def mscc_params_ragged(packed, group, y_hats, psis, ch_ctx, stage, num_scales):
+  """mscc_params over a list of images of their own shapes in one pass: returns (loc, scale_index, index, lengths),
+  flat, image i's n_s,i c values after image i - 1's; `lengths` are the n_s,i c.  ch_ctx is a list of [H_i, W_i, 2c]
+  (None at offset 0); y_hats a list of [H_i, W_i, M] (may be None at stage 0).  Image i's values equal mscc_params
+  on that image alone, bit for bit."""
+  stage = _msc_stage_arg(stage)
+  hs, ws, M = _ragged_list(psis)
+  _scc_check_packed(packed, M, group, mscc_layout)
+  dev = packed.device
+  psi = _ragged_cat(psis, "psi", hs, ws, 2 * M, dev)
+  ch = _scc_ch_ctx_ragged(ch_ctx, group, hs, ws, dev)
+  y_hat = None if y_hats is None and not stage else _ragged_cat(y_hats, "y_hat", hs, ws, M, dev)
+  return _mscc_pass_ragged(packed, group, M, hs, ws, y_hat, psi, ch, stage, num_scales)[:4]
+
+
+def mscc_encode_ragged(packed, groups, ys, psis, channel_context, num_scales, scale_index=False, substreams=1):
+  """mscc_encode of a list of images of their own shapes, one pass sequence for the whole list: returns (y_hats, y,
+  loc, index, lengths), and scale_index last with `scale_index=True`.  `channel_context(k, y_hats)` takes and
+  returns lists ([H_i, W_i, 2c_k] per image).  y, loc and index are flat in coding order, image i's H_i W_i M values
+  (its `lengths` entry) after image i - 1's.  With `substreams` = S > 1 they are in substream order and `lengths`
+  holds the n S stream lengths, image i's substream s at i S + s."""
+  S = gen_ops.check_substreams(substreams)
+  hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis, mscc_layout)
+  dev = psi.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, y_cc, loc = (torch.empty_like(y) for _ in range(3))
+  index = torch.empty(y.shape, dtype=torch.int32, device=dev)
+  scale = torch.empty_like(y) if scale_index else None
+  views = _ragged_views(y_hat, hs, ws, M)
+  for k, (p, g) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, g, hs, ws, dev)
+    for stage in range(4):
+      _mscc_pass_ragged(p, g, M, hs, ws, y_hat, psi, ch, stage, num_scales, True, loc, scale, index, y, y_cc, y_hat)
+  out = _to_substreams(groups, hs, ws, S, y_cc, loc, index, scale, multistage=True)
+  lengths = (hs * ws * M).tolist() if S == 1 else context_substreams(groups, hs, ws, S, multistage=True)[0].tolist()
+  return (views,) + out[:3] + (lengths,) + out[3:]
+
+
+def mscc_decode_ragged(handle, packed, groups, psis, channel_context, num_scales, cdf_offset, substreams=1):
+  """mscc_decode of a list of images of their own shapes, continuing `handle` (one index-mode string per image, or S
+  substreams per image): per group its channel context (as in mscc_encode_ragged), then per stage one ragged
+  parameter pass, one decode_ragged and one scatter for the whole list.  Returns the list of y_hat [H_i, W_i, M].
+  The library launches depend on the groups, not on the images' number or shapes (fewer when a stage is empty in
+  every image); no host synchronisation."""
+  hs, ws, M, spans, psi = _scc_ragged(packed, groups, psis, mscc_layout)
+  dev = psi.device
+  phases = _substream_phases(handle, groups, hs, ws, substreams, "list", multistage=True)
   coff = _i32(cdf_offset, dev)
   y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  views = _ragged_views(y_hat, hs, ws, M)
   lib = _lib.lib()
-  for stage in range(4):
-    loc, _, index, lengths, work = _msc_pass_ragged(packed, M, hs, ws, y_hat, psi, stage, num_scales)
-    if phases is not None:
-      lengths = phases[stage]
-    part = decode_ragged(handle, lengths, index=index, quant_offset=loc, cdf_offset=coff)
-    check(lib.tfcb_msc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, stage, _p(work), work.numel(),
-                                      _p(y_hat), _stream()))
-  return _ragged_views(y_hat, hs, ws, M)
+  for k, (p, (o, c)) in enumerate(zip(packed, spans)):
+    ch = _scc_ch_ctx_ragged(channel_context(k, views) if k else None, (o, c), hs, ws, dev)
+    for stage in range(4):
+      loc, _, index, lengths, work = _mscc_pass_ragged(p, (o, c), M, hs, ws, y_hat, psi, ch, stage, num_scales)
+      if phases is not None:
+        lengths = phases[4 * k + stage]
+      part = decode_ragged(handle, lengths, index=index, quant_offset=loc, cdf_offset=coff)
+      check(lib.tfcb_mscc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, o, c, stage, _p(work),
+                                         work.numel(), _p(y_hat), _stream()))
+  return views

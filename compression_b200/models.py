@@ -1010,7 +1010,7 @@ class SpaceChannelModel(MBT2018Model):
     self.groups = groups
     self.spans = F.scc_spans(groups)
     self._init_transforms(lmbda, N, M, num_scales, scale_min, scale_max)
-    self.context_models = nn.ModuleList([CheckerboardConv2D(c, 2 * c) for c in groups])
+    self.context_models = nn.ModuleList([self._spatial_context_model(c) for c in groups])
     self.channel_context_transforms = nn.ModuleList([_MS2020SliceTransform(2 * c) for c in groups[1:]])
     ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
     stacks = []
@@ -1029,11 +1029,20 @@ class SpaceChannelModel(MBT2018Model):
       parts = [psi]
       if k:
         parts.append(self.channel_context_transforms[k - 1](y_ctx[..., :o]))
-      parts.append(checkerboard_context(self.context_models[k], y_ctx[..., o:o + c]))
+      parts.append(self._spatial_context(k, y_ctx[..., o:o + c]))
       params = self.entropy_parameters[k](torch.cat(parts, dim=-1))
       locs.append(params[..., :c])
       scales.append(params[..., c:])
     return torch.cat(locs, dim=-1), torch.cat(scales, dim=-1)
+
+  @staticmethod
+  def _spatial_context_model(c):
+    """The spatial context model of a group of c channels."""
+    return CheckerboardConv2D(c, 2 * c)
+
+  def _spatial_context(self, k, y):
+    """The training form's spatial context [B, H, W, 2c_k] of group k from its channels y [B, H, W, c_k]."""
+    return checkerboard_context(self.context_models[k], y)
 
   def _channel_context(self, k, y_hat):
     """g_ch^k of y_hat[..., :o_k] [B, H, W, 2c_k], one image at a time."""
@@ -1180,6 +1189,62 @@ class MultistageModel(MBT2018Model):
 
   def _decode_ragged(self, handle, psis, cdf_offset):
     return F.msc_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset, substreams=self.substreams)
+
+
+class SpaceChannelMultistageModel(SpaceChannelModel):
+  """SpaceChannelModel with each channel group coded in the four stages of MultistageModel's 2x2 schedule (DESIGN
+  §3.17): the same transforms, channel groups, channel-context stacks, entropy-parameter stacks and entropy models.
+  Group k's spatial context is 0 at stage 0 and, at stage s >= 1, its own MultistageConv2D(c_k, 2c_k, s) over the
+  group's channels at the earlier stages' positions (4, 12 and 16 taps); `context_models[k]` holds the three.  The
+  group's entropy-parameter layers are shared by its four stages.  So only a quarter of each group's positions code
+  without spatial context (half with SpaceChannelModel), and every stage is position-parallel.
+
+  Coding runs on the group passes (functional.mscc_*): one string per image, the bytes of
+  `LocationScaleIndexedEntropyModel.compress(y_cc, scale_index_cc, loc_cc)` of the coding-order tensors [B, H W M]
+  (group 0's stages 0, 1, 2, 3, then group 1's, ..., each in raster order); the decoder makes 4K decode_index_f32
+  calls on one decoder handle.  With groups = (M,) and M a multiple of 6 the strings are MultistageModel's with the
+  same weights."""
+
+  @staticmethod
+  def _spatial_context_model(c):
+    return nn.ModuleList([MultistageConv2D(c, 2 * c, s) for s in (1, 2, 3)])
+
+  def _spatial_context(self, k, y):
+    return multistage_context(self.context_models[k], y)
+
+  def _pack(self):
+    M = self.latent_depth
+    return [F.mscc_pack_weights(M, span, [cm.kernel for cm in cms], [cm.bias for cm in cms], *_dense_weights(ep))
+            for span, cms, ep in zip(self.spans, self.context_models, self.entropy_parameters)]
+
+  def _coded(self, y, loc, index, B, H, W):
+    lengths = None
+    if self.substreams > 1:
+      lengths = F.context_substreams(self.groups, [H] * B, [W] * B, self.substreams, multistage=True)[0]
+    return self._compress_coding_order(y, loc, index, lengths, B)
+
+  def _encode_latents(self, y, psi):
+    """(strings, y_hat, loc, index): y_hat [B, H, W, M]; loc and index in coding order [B, H W M] (substream order
+    with substreams > 1)."""
+    B, H, W = (int(d) for d in y.shape[:3])
+    y_hat, y_cc, loc, index = F.mscc_encode(self._packed, self.groups, y.contiguous(), psi, self._channel_context,
+                                            self.num_scales, substreams=self.substreams)
+    return self._coded(y_cc, loc, index, B, H, W), y_hat, loc, index
+
+  def _decode_latents(self, strings, psi):
+    handle = self._y_decoder(strings)
+    y_hat = F.mscc_decode(handle, self._packed, self.groups, psi, self._channel_context, self.num_scales,
+                          self.entropy_model.cdf_offset.to(psi.device), substreams=self.substreams)
+    self.entropy_model._finish_decode(handle)
+    return y_hat
+
+  def _encode_ragged(self, ys, psis):
+    return F.mscc_encode_ragged(self._packed, self.groups, ys, psis, self._channel_contexts, self.num_scales,
+                                substreams=self.substreams)[1:]
+
+  def _decode_ragged(self, handle, psis, cdf_offset):
+    return F.mscc_decode_ragged(handle, self._packed, self.groups, psis, self._channel_contexts, self.num_scales,
+                                cdf_offset, substreams=self.substreams)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -453,6 +453,70 @@ int tfcb_msc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_
                             float* dst_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Space-channel multistage context model (DESIGN §3.17): the space-channel model's channel groups, each coded in the
+ * four stages of the multistage schedule.  M = latent depth, even, at most 1024; group [offset, offset + C) of it.
+ * Per position of stage s of the group (CH = 0 at offset 0, else 2C):
+ *   ctx = 0 at stage 0 (bias included), else Wc_s * (the group's channels of yhat at the stage's T_s taps) + bc_s
+ *                                                                                                 [T_s C] -> [2C]
+ *   h1 = leaky(W1 * [psi (2M), chctx (CH), ctx (2C)] + b1) -> [N3 = 5 K1 / 6], K1 = 2M + CH + 2C;
+ *   h2 = leaky(W2 * h1 + b2) -> [N4 = 2 K1 / 3];  [loc, scale_index] = W3 * h2 + b3 (C each)
+ * (widths rounded down) with tfcb_msc_params' stages, taps and float32 order of operations; chctx [B, H, W, CH] is
+ * the caller's channel context.  At offset 0 with C = M (M a multiple of 6) this is tfcb_msc_params, bit for bit, on
+ * the same packed layout; stage 0 is tfcb_scc_params' anchor pass of the group at its positions.  Coding order of
+ * all groups: per image, group 0's stages 0, 1, 2, 3, then group 1's, ..., each stage in raster order with C channels
+ * per position: [B, H W M] in all.
+ * ---------------------------------------------------------------------------------------------- */
+/* Floats of one group's packed parameters, or -1 if the group is not supported.  If `layout` is not NULL it receives
+ * 15 values: the widths K1, N3, N4, then the offsets of Wc_1 [4, C, 2C], bc_1 [2C], Wc_2 [12, C, 2C], bc_2,
+ * Wc_3 [16, C, 2C], bc_3, W1 [K1, N3], b1, W2 [N3, N4], b2, W3 [N4, 2C] and b3 (inputs x outputs, row major); the
+ * buffer ends at the returned size. */
+int64_t tfcb_mscc_packed_floats(int M, int offset, int C, int64_t* layout);
+/* Packs one group's parameters into `packed_dev`, stream-ordered device copies of the values unchanged; each stage's
+ * context taps already gathered as [T_s, C, 2C] in raster order of its taps. */
+int tfcb_mscc_pack_weights(int M, int offset, int C, const float* wc1_dev, const float* bc1_dev, const float* wc2_dev,
+                           const float* bc2_dev, const float* wc3_dev, const float* bc3_dev, const float* w1_dev,
+                           const float* b1_dev, const float* w2_dev, const float* b2_dev, const float* w3_dev,
+                           const float* b3_dev, float* packed_dev, int64_t packed_floats, void* stream);
+/* Floats of workspace one tfcb_mscc_params pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_mscc_workspace_floats(int M, int offset, int C, int64_t B, int64_t H, int64_t W, int stage);
+/* One pass over every position of stage `stage` (0 to 3) of one group of all B images; tfcb_msc_params' arguments,
+ * plus the group and `chctx_dev` [B, H, W, 2C] (required unless offset is 0).  Stages 1-3 read the group's channels
+ * of the earlier stages' positions of `yhat_dev` [B, H, W, M].  Writes loc, scale_index and the table index (each may
+ * be NULL): [B, n_s, C] (whole == 0), or [B, H W M] in the coding order of all groups at this pass's block
+ * H W offset + C (the positions of the earlier stages) (whole != 0).  Encoder epilogue (y_dev not NULL,
+ * [B, H, W, M]): also writes the group's y in coding order to `y_cc_dev` (same layout as loc) and
+ * yhat = float(int32(rint(y - loc))) + loc at this stage's positions and the group's channels of `yhat_out_dev`
+ * [B, H, W, M]; loc and index are then required.  Three launches at stage 0, four at stages 1-3, none for an empty
+ * stage; no host synchronisation. */
+int tfcb_mscc_params(const float* packed_dev, int64_t packed_floats, int M, int offset, int C, const float* yhat_dev,
+                     const float* psi_dev, const float* chctx_dev, int64_t B, int64_t H, int64_t W, int stage,
+                     int num_scales, float* work_dev, int64_t work_floats, int whole, float* loc_dev,
+                     float* scale_index_dev, int32_t* index_dev, const float* y_dev, float* y_cc_dev,
+                     float* yhat_out_dev, void* stream);
+/* Moves one stage of one group from coding order [B, n_s, C] to its positions and channels of `dst_dev`
+ * [B, H, W, M] (nothing else is written).  One launch; none for an empty stage. */
+int tfcb_mscc_scatter(const float* src_dev, int64_t B, int64_t H, int64_t W, int M, int offset, int C, int stage,
+                      float* dst_dev, void* stream);
+/* Ragged lists, in the layout of tfcb_scc_params_ragged: image i's n_s,i C values at C Q_i (whole == 0), or its block
+ * of the coding order of all groups at M P_i + H_i W_i offset + C (its positions of the earlier stages)
+ * (whole != 0).  Each image's outputs equal the fixed-shape call on that image alone, bit for bit.  The image table
+ * goes to `work_dev` with one stream-ordered copy; there is no host synchronisation. */
+int64_t tfcb_mscc_ragged_workspace_floats(int M, int offset, int C, int64_t n_images, const int64_t* heights_host,
+                                          const int64_t* widths_host, int stage);
+int tfcb_mscc_params_ragged(const float* packed_dev, int64_t packed_floats, int M, int offset, int C,
+                            const float* yhat_dev, const float* psi_dev, const float* chctx_dev, int64_t n_images,
+                            const int64_t* heights_host, const int64_t* widths_host, int stage, int num_scales,
+                            float* work_dev, int64_t work_floats, int whole, float* loc_dev, float* scale_index_dev,
+                            int32_t* index_dev, const float* y_dev, float* y_cc_dev, float* yhat_out_dev,
+                            void* stream);
+/* tfcb_mscc_scatter of a ragged list: image i's n_s,i C values at C Q_i -> its positions and the group's channels of
+ * its [H_i, W_i, M] in `dst_dev`.  `work_dev` holds at least 8 n_images floats (the workspace of a pass of the list
+ * does).  One launch; none when no image has a position of this stage. */
+int tfcb_mscc_scatter_ragged(const float* src_dev, int64_t n_images, const int64_t* heights_host,
+                             const int64_t* widths_host, int M, int offset, int C, int stage, float* work_dev,
+                             int64_t work_floats, float* dst_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Substreams (DESIGN §3.14): a coding unit (one string of today's format: one image's y or z, one MS2020 slice)
  * split into S independently decodable streams.  A unit's symbols are in coding order, in phases p = 0 .. P-1
  * (the order in which the decoder makes them); phase p of unit u has positions[u P + p] positions of
