@@ -128,6 +128,13 @@ SIGNATURES = {
     "tfcb_unbounded_index_range_encoder_destroy": (None, [_vp]),
     "tfcb_unbounded_index_range_decode_ragged": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _int, _vp, _i64, _vp,
                                                         _i64, _int, _int, _int, _vp, _vp]),
+    "tfcb_mixture_tables": (_int, [_vp, _vp, _vp, _i64, _int, _int, _int, C.c_double, _int, _vp, _vp, _vp, _vp, _vp]),
+    "tfcb_mixture_encode_ragged": (_int, [_vp, _vp, _vp, _vp, _int, _int, _int, C.c_double, _int, _i64, _vp, _vp, _vp,
+                                          _p(_vp), _p(_i64)]),
+    "tfcb_mixture_write": (_int, [_vp, _vp, _vp]),
+    "tfcb_mixture_encoder_destroy": (None, [_vp]),
+    "tfcb_mixture_decode_ragged": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _int, _int, _int, C.c_double, _int, _vp,
+                                          _vp]),
     "tfcb_pmf_to_quantized_cdf": (_int, [_vp, _i64, _i64, _int, _vp, _vp]),
     "tfcb_build_lookup": (_int, [_vp, _i64, _i64, _vp, _int, _vp, _vp]),
     "tfcb_run_length_encode": (_int, [_vp, _i64, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),

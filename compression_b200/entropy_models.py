@@ -23,7 +23,7 @@ from compression_b200 import gen_ops, math_ops
 __all__ = [
     "ContinuousEntropyModelBase", "ContinuousBatchedEntropyModel", "ContinuousIndexedEntropyModel",
     "LocationScaleIndexedEntropyModel", "UniversalBatchedEntropyModel", "UniversalIndexedEntropyModel",
-    "EntropyBottleneck",
+    "EntropyBottleneck", "MixtureEntropyModel",
 ]
 
 
@@ -1171,6 +1171,157 @@ class UniversalIndexedEntropyModel(ContinuousEntropyModelBase):
 
   def get_config(self):
     raise NotImplementedError()
+
+
+class MixtureEntropyModel(nn.Module):
+  """Every element coded under its own mixture of K Normal or Logistic components (Cheng et al. 2020), with its CDF
+  built on the device from (weight, loc, scale) (DESIGN §3.18).  There are no tables: `weight`, `loc` and `scale`
+  have the bottleneck's shape plus a last axis of K components; the weights need not sum to 1 and are normalised.
+  The string of a coding unit (the last `coding_rank` axes) is one range-coded stream, or S independently decodable
+  ones with `substreams` = S (DESIGN §3.14).  float32 only."""
+
+  decode_sanity_check = True
+
+  def __init__(self, family="normal", coding_rank=0, tail_mass=2**-8, range_coder_precision=16, max_support=256):
+    super().__init__()
+    if family not in F.MIXTURE_FAMILIES:
+      raise ValueError(f"`family` must be one of {sorted(F.MIXTURE_FAMILIES)}: {family!r}")
+    if int(coding_rank) < 0:
+      raise ValueError("`coding_rank` must be at least 0.")
+    if not 0 < tail_mass < 1:
+      raise ValueError("`tail_mass` must be between 0 and 1.")
+    if not 1 <= int(max_support) <= 256:
+      raise ValueError(f"`max_support` must be in [1, 256]: {max_support}")
+    if not 1 <= int(range_coder_precision) <= 16 or (1 << int(range_coder_precision)) <= int(max_support):
+      raise ValueError(f"`range_coder_precision` must be in [1, 16] with 2^precision > max_support: "
+                       f"{range_coder_precision}")
+    self.family = family
+    self.coding_rank = int(coding_rank)
+    self.tail_mass = float(tail_mass)
+    self.range_coder_precision = int(range_coder_precision)
+    self.max_support = int(max_support)
+
+  def _prior(self, weight, loc, scale):
+    cls = D.NoisyNormalMixture if self.family == "normal" else D.NoisyLogisticMixture
+    return cls(loc, scale, weight / weight.sum(-1, keepdim=True))
+
+  def _check(self, bottleneck, weight, loc, scale):
+    for name, t in (("bottleneck", bottleneck), ("weight", weight), ("loc", loc), ("scale", scale)):
+      if t is None and name == "bottleneck":  # (decompress: the parameters alone give the shape)
+        continue
+      if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+        raise ValueError(f"MixtureEntropyModel codes float32 only: `{name}` is "
+                         f"{getattr(t, 'dtype', type(t).__name__)}")
+    if weight.dim() < 1 or weight.shape != loc.shape or weight.shape != scale.shape:
+      raise ValueError(f"weight, loc and scale must share one shape: {tuple(weight.shape)}, {tuple(loc.shape)}, "
+                       f"{tuple(scale.shape)}")
+    if bottleneck is not None and tuple(bottleneck.shape) != tuple(weight.shape[:-1]):
+      raise ValueError(f"the parameters' shape {tuple(weight.shape)} must be the bottleneck's "
+                       f"{tuple(bottleneck.shape)} plus the components")
+    if weight.dim() - 1 < self.coding_rank:
+      raise ValueError(f"coding_rank {self.coding_rank} exceeds the bottleneck's rank {weight.dim() - 1}")
+
+  @staticmethod
+  def _components(weights):
+    """The one component count K of a list of items' parameters; items with different K are rejected."""
+    ks = {int(w.shape[-1]) for w in weights}
+    if len(ks) != 1:
+      raise ValueError(f"every item must have the same number of components: {sorted(ks)}")
+    return ks.pop()
+
+  def forward(self, bottleneck, weight, loc, scale, training=True):
+    """(perturbed or rounded bottleneck, bits per coding unit) through the NoisyNormalMixture /
+    NoisyLogisticMixture graph: the rate term training already uses."""
+    self._check(bottleneck, weight, loc, scale)
+    prior = self._prior(weight, loc, scale)
+    if training:
+      log_probs, perturbed = math_ops.perturb_and_apply(lambda x: prior.log_prob(x), bottleneck,
+                                                        expected_grads=False)
+    else:
+      perturbed = math_ops.round_st(bottleneck)
+      log_probs = prior.log_prob(perturbed)
+    axes = tuple(range(-self.coding_rank, 0))
+    bits = (log_probs.sum(dim=axes) if axes else log_probs) / -math.log(2.)
+    return perturbed, bits
+
+  def _coder_args(self):
+    return dict(family=self.family, precision=self.range_coder_precision, tail_mass=self.tail_mass,
+                max_support=self.max_support)
+
+  @staticmethod
+  def _lengths(shapes, substreams):
+    """Stream lengths of coding units of these shapes: one stream each, or substream_layout's split of the unit's
+    positions along its last axis."""
+    if substreams == 1:
+      return [gen_ops._prod(s) for s in shapes]
+    widths = [max(int(s[-1]), 1) if len(s) else 1 for s in shapes]
+    return F.substream_layout([[gen_ops._prod(s) // w] for s, w in zip(shapes, widths)], [[w] for w in widths],
+                              substreams)[0]
+
+  def _encode(self, shapes, y, weight, loc, scale, substreams):
+    S = gen_ops.check_substreams(substreams)
+    strings = F.mixture_encode_ragged(y.reshape(-1), weight, loc, scale, self._lengths(shapes, S),
+                                      **self._coder_args())
+    return gen_ops.join_substreams(strings, S, (len(shapes),)) if S > 1 else strings
+
+  def _decode(self, strings, shapes, weight, loc, scale, substreams):
+    S = gen_ops.check_substreams(substreams)
+    if S > 1:
+      strings = gen_ops.split_substreams(strings, S)
+    return F.mixture_decode_ragged(strings, weight, loc, scale, self._lengths(shapes, S), **self._coder_args())
+
+  def compress(self, bottleneck, weight, loc, scale, *, substreams=1):
+    """One string per coding unit: Strings of shape bottleneck.shape[:-coding_rank]."""
+    self._check(bottleneck, weight, loc, scale)
+    r = self.coding_rank
+    batch = tuple(bottleneck.shape[:bottleneck.dim() - r])
+    unit = tuple(bottleneck.shape[bottleneck.dim() - r:])
+    s = self._encode([unit] * gen_ops._prod(batch), bottleneck, weight, loc, scale, substreams)
+    return gen_ops.Strings(s.bytes_dev, s.offsets_dev, batch)
+
+  def decompress(self, strings, weight, loc, scale, *, substreams=1):
+    """Inverse of compress: float32 of weight.shape[:-1]."""
+    self._check(None, weight, loc, scale)
+    r = self.coding_rank
+    shape = tuple(weight.shape[:-1])
+    batch, unit = shape[:len(shape) - r], shape[len(shape) - r:]
+    n = gen_ops._prod(batch)
+    if not isinstance(strings, gen_ops.Strings):
+      strings = gen_ops.Strings.from_bytes(strings)
+    if strings.numel() != n:
+      raise ValueError(f"{strings.numel()} strings for a batch of {n} coding units")
+    flat = gen_ops.Strings(strings.bytes_dev, strings.offsets_dev, (n,))
+    return self._decode(flat, [unit] * n, weight, loc, scale, substreams).reshape(shape)
+
+  def compress_ragged(self, bottlenecks, weights, locs, scales, *, substreams=1):
+    """One string per item of a list of differently shaped bottlenecks (each item one coding unit), in one launch
+    sequence; string i equals the string of item i alone."""
+    items = list(zip(bottlenecks, weights, locs, scales))
+    if not items or len({len(bottlenecks), len(weights), len(locs), len(scales)}) != 1:
+      raise ValueError("compress_ragged needs at least one item, and as many parameters as bottlenecks")
+    for b, w, l, s in items:
+      self._check(b, w, l, s)
+    K = self._components(weights)
+    cat = lambda ts: torch.cat([t.reshape(-1) for t in ts])
+    w, l, s = (cat(ts).reshape(-1, K) for ts in (weights, locs, scales))
+    return self._encode([tuple(b.shape) for b in bottlenecks], cat(bottlenecks), w, l, s, substreams)
+
+  def decompress_ragged(self, strings, weights, locs, scales, *, substreams=1):
+    """Inverse of compress_ragged: a list of float32 items shaped weights[i].shape[:-1]."""
+    items = list(zip(weights, locs, scales))
+    if not items or len({len(weights), len(locs), len(scales)}) != 1:
+      raise ValueError("decompress_ragged needs at least one item, and as many locs and scales as weights")
+    for w, l, s in items:
+      self._check(None, w, l, s)
+    K = self._components(weights)
+    shapes = [tuple(w.shape[:-1]) for w in weights]
+    if not isinstance(strings, gen_ops.Strings):
+      strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+    if strings.numel() != len(items):
+      raise ValueError(f"{strings.numel()} strings for {len(items)} items")
+    cat = lambda ts: torch.cat([t.reshape(-1) for t in ts]).reshape(-1, K)
+    out = self._decode(strings, shapes, cat(weights), cat(locs), cat(scales), substreams)
+    return gen_ops._split_items(out, shapes)
 
 
 def EntropyBottleneck(num_channels=None, prior=None, coding_rank=3, compression=True, **kwargs):

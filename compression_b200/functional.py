@@ -862,6 +862,91 @@ def unbounded_index_range_decode_ragged(strings, index, lengths, cdf, cdf_size, 
 
 
 # ------------------------------------------------------------------------------------------------
+# Mixture priors (DESIGN §3.18): every element coded under its own Normal or Logistic mixture, its row built on the
+# device (tfcb_mixture_*).  weight / loc / scale are float32 [elements, K], components innermost.
+# ------------------------------------------------------------------------------------------------
+MIXTURE_FAMILIES = {"normal": 0, "logistic": 1}
+
+
+def _mixture_args(weight, loc, scale, family, n=None):
+  """(weight, loc, scale, K, family code) as contiguous float32 CUDA tensors [elements, K], checked on the host."""
+  if family not in MIXTURE_FAMILIES:
+    raise _lib.InvalidArgumentError(f"`family` must be one of {sorted(MIXTURE_FAMILIES)}: {family!r}")
+  ts = (weight, loc, scale)
+  for name, t in zip(("weight", "loc", "scale"), ts):
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda:
+      raise _lib.InvalidArgumentError(f"`{name}` must be a float32 CUDA tensor")
+    if t.dim() < 1 or t.shape != weight.shape:
+      raise _lib.InvalidArgumentError(f"weight, loc and scale must share one shape [..., K]: {tuple(t.shape)}")
+  K = int(weight.shape[-1])
+  m = weight.numel() // K if K else 0
+  if n is not None and m != n:
+    raise _lib.InvalidArgumentError(f"{n} elements, but the parameters hold {m} mixtures")
+  return (*(t.reshape(-1, K).contiguous() for t in ts), K, MIXTURE_FAMILIES[family])
+
+
+def mixture_tables(weight, loc, scale, family="normal", precision=16, tail_mass=2**-8, max_support=256):
+  """The rows the mixture coder builds, for tests and for the reference coder: (start int32 [n], size int32 [n], mass
+  int64 [n, max_support + 1], rows int32 [n, max_support + 3]).  Row e is [-precision, c_0, .., c_{L+1}] padded with
+  2^precision; mass[e] holds m_0 .. m_{L-1}, the escape mass m_L, then zeros."""
+  w, l, s, K, fam = _mixture_args(weight, loc, scale, family)
+  n = w.shape[0]
+  dev = w.device
+  start = torch.empty(n, dtype=torch.int32, device=dev)
+  size = torch.empty(n, dtype=torch.int32, device=dev)
+  mass = torch.empty((n, int(max_support) + 1), dtype=torch.int64, device=dev)
+  rows = torch.empty((n, int(max_support) + 3), dtype=torch.int32, device=dev)
+  check(_lib.lib().tfcb_mixture_tables(_p(w), _p(l), _p(s), n, K, fam, int(precision), float(tail_mass),
+                                       int(max_support), _p(start), _p(size), _p(mass), _p(rows), _stream()))
+  return start, size, mass, rows
+
+
+def mixture_encode_ragged(y, weight, loc, scale, lengths, family="normal", precision=16, tail_mass=2**-8,
+                          max_support=256):
+  """String i codes the next `lengths[i]` elements of the flat float32 `y` (CUDA), each quantised to int32(rint(y))
+  and coded under its own mixture.  Returns a Strings of shape (len(lengths),); one host synchronisation."""
+  offs = _symbol_offsets(lengths)
+  n = int(offs[-1])
+  if not isinstance(y, torch.Tensor) or y.dtype != torch.float32 or not y.is_cuda:
+    raise _lib.InvalidArgumentError("`y` must be a float32 CUDA tensor")
+  if y.numel() != n:
+    raise _lib.InvalidArgumentError(f"ragged batch of {n} elements, but `y` has {y.numel()}")
+  w, l, s, K, fam = _mixture_args(weight, loc, scale, family, n)
+  y = y.reshape(-1).contiguous()
+  k = offs.size - 1
+  offsets = torch.empty(k + 1, dtype=torch.int64, device=y.device)
+  h, total = C.c_void_p(), C.c_int64(0)
+  L = _lib.lib()
+  check(L.tfcb_mixture_encode_ragged(_p(y), _p(w), _p(l), _p(s), K, fam, int(precision), float(tail_mass),
+                                     int(max_support), k, offs.ctypes.data_as(C.c_void_p), _p(offsets), _stream(),
+                                     C.byref(h), C.byref(total)))
+  try:
+    out = torch.empty(max(int(total.value), 1), dtype=torch.uint8, device=y.device)
+  except BaseException:
+    L.tfcb_mixture_encoder_destroy(h)
+    raise
+  check(L.tfcb_mixture_write(h, _p(out), _stream()))
+  return gen_ops.Strings(out, offsets, (k,))
+
+
+def mixture_decode_ragged(strings, weight, loc, scale, lengths, family="normal", precision=16, tail_mass=2**-8,
+                          max_support=256):
+  """Inverse of mixture_encode_ragged: float32 [sum(lengths)] on the parameters' device, string after string."""
+  offs = _symbol_offsets(lengths)
+  n = int(offs[-1])
+  w, l, s, K, fam = _mixture_args(weight, loc, scale, family, n)
+  if not isinstance(strings, gen_ops.Strings):
+    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+  if strings.numel() != offs.size - 1:
+    raise _lib.InvalidArgumentError(f"{strings.numel()} strings for {offs.size - 1} lengths")
+  out = torch.empty(n, dtype=torch.float32, device=w.device)
+  check(_lib.lib().tfcb_mixture_decode_ragged(_p(strings.bytes_dev), _p(strings.offsets_dev), offs.size - 1,
+                                              offs.ctypes.data_as(C.c_void_p), _p(w), _p(l), _p(s), K, fam,
+                                              int(precision), float(tail_mass), int(max_support), _p(out), _stream()))
+  return out
+
+
+# ------------------------------------------------------------------------------------------------
 # Joint autoregressive + hierarchical prior (Minnen 2018): the packed parameter network and the parameter, encoder and
 # decoder steps over latent positions in raster order (tfcb_ar_*).  Latents are float32 CUDA [B, H, W, M], the hyper
 # feature psi [B, H, W, 2M].

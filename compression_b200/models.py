@@ -23,12 +23,12 @@ from torch import nn
 from compression_b200 import distributions as D
 from compression_b200 import entropy_models as E
 from compression_b200 import functional as F
-from compression_b200 import gen_ops
+from compression_b200 import gen_ops, math_ops
 from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MultistageModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MultistageModel", "MixtureHyperpriorModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -682,8 +682,9 @@ class MBT2018Model(_Model):
         ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(2 * M, "layer_2", None))
     self._init_entropy_models(N)
 
-  def _init_transforms(self, lmbda, N, M, num_scales, scale_min, scale_max):
-    """The analysis, synthesis and hyper transforms and the scale table."""
+  def _init_transforms(self, lmbda, N, M, num_scales, scale_min, scale_max, psi_width=None):
+    """The analysis, synthesis and hyper transforms and the scale table; the hyper synthesis ends in `psi_width`
+    channels (2M by default)."""
     self.lmbda = lmbda
     self.num_filters, self.latent_depth, self.num_scales = N, M, int(num_scales)
     offset = math.log(scale_min)
@@ -698,7 +699,8 @@ class MBT2018Model(_Model):
         _conv(N, 5, "layer_2", down=2, use_bias=False))
     hs = lambda f, k, name, up, act: _conv(f, k, name, up=up, corr=False, kernel_parameter="variable", activation=act)
     self.hyper_synthesis_transform = nn.Sequential(
-        hs(M, 5, "layer_0", 2, _leaky), hs(3 * M // 2, 5, "layer_1", 2, _leaky), hs(2 * M, 3, "layer_2", 1, None))
+        hs(M, 5, "layer_0", 2, _leaky), hs(3 * M // 2, 5, "layer_1", 2, _leaky),
+        hs(psi_width or 2 * M, 3, "layer_2", 1, None))
 
   def _init_entropy_models(self, N):
     self.hyperprior = D.NoisyDeepFactorized(batch_shape=(N,))
@@ -882,6 +884,129 @@ class MBT2018Model(_Model):
     handle = self._y_decoder(gen_ops.Strings.concat([it[0] for it in items]))
     y_hats = self._decode_ragged(handle, psis, em.cdf_offset.to(psis[0].device))
     em._finish_decode(handle)
+    out = []
+    for y_hat, it in zip(y_hats, items):
+      x_hat = self.synthesis_transform(y_hat[None])
+      out.append(_to_uint8(x_hat[:, :int(it[2][0]), :int(it[2][1]), :])[0])
+    return out
+
+  def decompress_from_tfci(self, data):
+    dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
+    return self.decompress(*PackedTensors(data).unpack(dtypes))
+
+
+class MixtureHyperpriorModel(_Model):
+  """Hyperprior with a discretized mixture prior on y (Cheng et al., CVPR 2020, without the attention modules and the
+  context model).  N = num_filters, M = latent_depth, K = num_components.  MBT2018Model's analysis, synthesis and
+  hyper transforms, the hyper synthesis widened to 3KM channels: channel c of y reads its K logits, K locs and K
+  scales, in that order, from channels 3Kc .. 3Kc + 3K - 1; weights = softmax(logits), scales bounded below at 0.11.
+  z is coded with a NoisyDeepFactorized prior as in MBT2018Model, y by entropy_models.MixtureEntropyModel
+  (coding_rank 3), whose rows are built on the device (DESIGN §3.18).  The hyper synthesis runs per image, so the
+  strings of an image do not depend on its batch or list."""
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_components=3, family="normal", substreams=1):
+    super().__init__()
+    self._set_substreams(substreams)
+    N, M, K = int(num_filters), int(latent_depth), int(num_components)
+    if M <= 0 or M % 2:
+      raise ValueError(f"latent_depth must be a positive even number (3M/2 is a layer width): {M}")
+    if K < 1 or K > 64:
+      raise ValueError(f"num_components must be in [1, 64]: {K}")
+    if family not in F.MIXTURE_FAMILIES:
+      raise ValueError(f"`family` must be one of {sorted(F.MIXTURE_FAMILIES)}: {family!r}")
+    self.num_components, self.family = K, family
+    MBT2018Model._init_transforms(self, lmbda, N, M, 64, .11, 256., psi_width=3 * K * M)
+    self.hyperprior = D.NoisyDeepFactorized(batch_shape=(N,))
+    self.entropy_model = E.MixtureEntropyModel(family, coding_rank=3)
+    self.side_entropy_model = None
+
+  def mixture_parameters(self, psi):
+    """(weight, loc, scale), each [B, H, W, M, K], from the hyper feature psi [B, H, W, 3KM]."""
+    K = self.num_components
+    p = psi.reshape(psi.shape[:-1] + (self.latent_depth, 3, K))
+    weight = torch.softmax(p[..., 0, :], dim=-1)
+    scale = math_ops.lower_bound(p[..., 2, :], .11)
+    return weight.contiguous(), p[..., 1, :].contiguous(), scale.contiguous()
+
+  def _params(self, z_hat, y_hw):
+    """The mixture parameters of each image, the hyper synthesis run one image at a time and cropped to y's size."""
+    psi = torch.cat([self.hyper_synthesis_transform(z_hat[i:i + 1])[:, :y_hw[0], :y_hw[1], :]
+                     for i in range(z_hat.shape[0])])
+    return self.mixture_parameters(psi)
+
+  def forward(self, x, training=True):
+    """-> (loss, bpp, mse), with the rate of y through the NoisyNormalMixture / NoisyLogisticMixture graph."""
+    side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3, compression=False)
+    x = x.to(torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    z_hat, side_bits = side_entropy_model(z, training=training)
+    psi = self.hyper_synthesis_transform(z_hat)[:, :y.shape[1], :y.shape[2], :]
+    y_hat, bits = self.entropy_model(y, *self.mixture_parameters(psi), training=training)
+    self._last_x_hat = self.synthesis_transform(y_hat)[:, :x.shape[1], :x.shape[2], :]
+    return self.rate_distortion(x, bits.sum() + side_bits.sum())
+
+  def fix_tables(self):
+    """Builds z's coding tables from the trained hyperprior (y needs none)."""
+    self.side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3,
+                                                              compression=True).to(self._device())
+    return self
+
+  def compress(self, x):
+    """uint8 [H, W, 3] -> (string, side_string, x_shape, y_shape, z_shape), bmshj2018's signature."""
+    return self.compress_batch(_as_image(x)[None])
+
+  def decompress(self, string, side_string, x_shape, y_shape, z_shape):
+    return self.decompress_batch(string, side_string, x_shape, y_shape, z_shape)[0]
+
+  @torch.no_grad()
+  def compress_batch(self, x):
+    x = _as_batch(x).to(device=self._device(), dtype=torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    shapes = tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+    side_string = self.side_entropy_model.compress(z, substreams=self.substreams)
+    params = self._params(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))
+    string = self.entropy_model.compress(y.contiguous(), *params, substreams=self.substreams)
+    return (string, side_string) + shapes
+
+  @torch.no_grad()
+  def decompress_batch(self, string, side_string, x_shape, y_shape, z_shape):
+    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape), substreams=self.substreams)
+    params = self._params(z_hat, (int(y_shape[0]), int(y_shape[1])))
+    y_hat = self.entropy_model.decompress(string, *params, substreams=self.substreams)
+    x_hat = self.synthesis_transform(y_hat)
+    return _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])
+
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element.  The
+    transforms run per image; z and y of the whole list are each coded in one ragged launch sequence."""
+    xs = [_as_image(x)[None].to(device=self._device(), dtype=torch.float32) for x in images]
+    if not xs:
+      raise ValueError("`images` is empty")
+    ys = [self.analysis_transform(x) for x in xs]
+    zs = [self.hyper_analysis_transform(y) for y in ys]
+    side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs], substreams=self.substreams).split()
+    params = [self._params(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1])) for y, z in zip(ys, zs)]
+    ws, ls, ss = ([p[j][0] for p in params] for j in range(3))
+    strings = self.entropy_model.compress_ragged([y[0] for y in ys], ws, ls, ss, substreams=self.substreams).split()
+    return [(strings[i], side_strings[i]) + tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+            for i, (x, y, z) in enumerate(zip(xs, ys, zs))]
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
+    items = list(items)
+    if not items:
+      raise ValueError("`items` is empty")
+    z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
+                                                       [tuple(int(v) for v in it[4]) for it in items],
+                                                       substreams=self.substreams)
+    params = [self._params(z_hat[None], (int(it[3][0]), int(it[3][1]))) for z_hat, it in zip(z_hats, items)]
+    ws, ls, ss = ([p[j][0] for p in params] for j in range(3))
+    y_hats = self.entropy_model.decompress_ragged(gen_ops.Strings.concat([it[0] for it in items]), ws, ls, ss,
+                                                  substreams=self.substreams)
     out = []
     for y_hat, it in zip(y_hats, items):
       x_hat = self.synthesis_transform(y_hat[None])

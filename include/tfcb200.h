@@ -599,6 +599,43 @@ int tfcb_unbounded_index_range_decode_ragged(const uint8_t* bytes_dev, const int
                                              int overflow_width, int debug_level, int32_t* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Mixture priors (Cheng et al. 2020), DESIGN.md §3.18: element e is coded under its own mixture of K components of
+ * one family (0 Normal, 1 Logistic) with float32 weight_dev, loc_dev and scale_dev [n, K] (components innermost; the
+ * weights need not sum to 1).  The row of element e, built on the device, is the index-mode overflow row
+ * [-precision, c_0, .., c_n] of the support start_e .. start_e + L_e - 1 plus the escape bin; y is quantised as
+ * int32(rint(y)) (saturating, NaN -> 0) and coded as the reference RangeEncoder codes y - start_e with that row,
+ * escapes with the Elias-gamma payload, so every int32 codes.  The decoded value is float32 of that int32.
+ * Checked before any device work (TFCB_INVALID_ARGUMENT): family, K in [1, 64], max_support in [1, 256], precision
+ * in [1, 16] with 2^precision > max_support, tail_mass in (0, 1), null pointers and the item offsets as for
+ * tfcb_compress_ragged.  On the device: non-finite parameters, a scale <= 0, a negative weight, all weights 0 and
+ * weights summing below 2^-126;
+ * failures name the lowest failing string and element.
+ * tfcb_mixture_tables writes start_dev / size_dev int32 [n], the masses mass_dev int64 [n, max_support + 1] (m_0 ..
+ * m_{L-1}, the escape mass m_L, zeros after) and rows_dev int32 [n, max_support + 3] (the row, padded with
+ * 2^precision: a 2-D lookup the reference coder takes), and synchronises once.
+ * tfcb_mixture_encode_ragged codes item u (elements [item_offsets_host[u], item_offsets_host[u+1]) of y_dev and the
+ * parameters) into string u, writes where each string starts to offsets_dev int64 [n_items + 1], synchronises once
+ * and returns the total size and a handle; tfcb_mixture_write writes the strings back to back into bytes_dev
+ * (asynchronous) and takes the handle back, also when it fails; tfcb_mixture_encoder_destroy releases a handle that
+ * is never written.  tfcb_mixture_decode_ragged decodes string u into out_dev float32 [item_offsets_host[u] ..) and
+ * synchronises once; a damaged string decodes to what the reference decoder gives on the same rows.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct tfcb_mixture_encoder tfcb_mixture_encoder;
+int tfcb_mixture_tables(const float* weight_dev, const float* loc_dev, const float* scale_dev, int64_t n, int K,
+                        int family, int precision, double tail_mass, int max_support, int32_t* start_dev,
+                        int32_t* size_dev, int64_t* mass_dev, int32_t* rows_dev, void* stream);
+int tfcb_mixture_encode_ragged(const float* y_dev, const float* weight_dev, const float* loc_dev,
+                               const float* scale_dev, int K, int family, int precision, double tail_mass,
+                               int max_support, int64_t n_items, const int64_t* item_offsets_host, int64_t* offsets_dev,
+                               void* stream, tfcb_mixture_encoder** out, int64_t* total_bytes_host);
+int tfcb_mixture_write(tfcb_mixture_encoder* h, uint8_t* bytes_dev, void* stream);
+void tfcb_mixture_encoder_destroy(tfcb_mixture_encoder* h);
+int tfcb_mixture_decode_ragged(const uint8_t* bytes_dev, const int64_t* offsets_dev, int64_t n_items,
+                               const int64_t* item_offsets_host, const float* weight_dev, const float* loc_dev,
+                               const float* scale_dev, int K, int family, int precision, double tail_mass,
+                               int max_support, float* out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * PmfToQuantizedCdf:
  *   op contract   tensorflow_compression/cc/ops/pmf_to_cdf_ops.cc:28-57
  *   CPU kernel    tensorflow_compression/cc/kernels/pmf_to_cdf_kernels.cc:58-208
