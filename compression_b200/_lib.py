@@ -135,6 +135,13 @@ SIGNATURES = {
     "tfcb_mixture_encoder_destroy": (None, [_vp]),
     "tfcb_mixture_decode_ragged": (_int, [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _int, _int, _int, C.c_double, _int, _vp,
                                           _vp]),
+    "tfcb_cbm_packed_floats": (_i64, [_int, _int, _p(_i64)]),
+    "tfcb_cbm_pack_weights": (_int, [_int, _int] + [_vp] * 9 + [_i64, _vp]),
+    "tfcb_cbm_workspace_floats": (_i64, [_int, _int, _i64, _i64, _i64, _int]),
+    "tfcb_cbm_params": (_int, [_vp, _i64, _int, _int, _vp, _vp, _i64, _i64, _i64, _int, _vp, _i64, _int] + [_vp] * 7),
+    "tfcb_cbm_ragged_workspace_floats": (_i64, [_int, _int, _i64, _vp, _vp, _int]),
+    "tfcb_cbm_params_ragged": (_int, [_vp, _i64, _int, _int, _vp, _vp, _i64, _vp, _vp, _int, _vp, _i64, _int]
+                               + [_vp] * 7),
     "tfcb_pmf_to_quantized_cdf": (_int, [_vp, _i64, _i64, _int, _vp, _vp]),
     "tfcb_build_lookup": (_int, [_vp, _i64, _i64, _vp, _int, _vp, _vp]),
     "tfcb_run_length_encode": (_int, [_vp, _i64, _int, _int, _int, _vp, _i64, _p(_i64), _vp]),

@@ -1722,6 +1722,300 @@ def cb_decode_ragged(handle, packed, psis, num_scales, cdf_offset, substreams=1)
 
 
 # ------------------------------------------------------------------------------------------------
+# Checkerboard context model with mixture priors (DESIGN §3.19): the checkerboard's two parameter passes on a network
+# whose last layer has 3KM outputs, each ending in the per-latent mixtures of the mixture coder (tfcb_cbm_*).  Coding
+# order is the checkerboard's.  One image's y string is varint(len A) ‖ A ‖ N, A and N the strings
+# mixture_encode_ragged writes for its anchors' and its non-anchors' coding-order latents (with S substreams each
+# when substreams = S > 1).  Latents are float32 CUDA [B, H, W, M], psi [B, H, W, 2M]; mixture parameters are
+# [..., M, K], components innermost.
+# ------------------------------------------------------------------------------------------------
+CBM_LAYOUT_KEYS = ("K1", "N3", "N4", "NO", "wc", "bc", "w1", "b1", "w2", "b2", "w3", "b3")
+
+
+def cbm_layout(M, K):
+  """The packed network of latent depth M (a multiple of 6 in [6, 384]) with K components (in [1, 64]): widths K1,
+  N3, N4, NO = 3KM, the offsets of its eight operands and `total`, in floats."""
+  lay = np.zeros(len(CBM_LAYOUT_KEYS), dtype=np.int64)
+  n = int(_lib.lib().tfcb_cbm_packed_floats(int(M), int(K), lay.ctypes.data_as(C.POINTER(C.c_int64))))
+  if n < 0:
+    raise _lib.InvalidArgumentError(f"latent depth M={M} must be a positive multiple of 6 and at most 384, and K={K} "
+                                    f"in [1, 64]")
+  return dict(zip(CBM_LAYOUT_KEYS, (int(v) for v in lay)), total=n)
+
+
+def cbm_pack_weights(ctx_kernel, ctx_bias, w1, b1, w2, b2, w3, b3):
+  """cb_pack_weights for the mixture network: the 12 checkerboard taps of the context kernel [5, 5, M, 2M], then the
+  1x1 layers [4M, 10M/3], [10M/3, 8M/3], [8M/3, 3KM] and their biases; K is read from W3's width.  Returns float32
+  [total] on the context kernel's device, the values copied unchanged."""
+  ctx_kernel = ctx_kernel.detach()
+  if ctx_kernel.dim() != 4 or ctx_kernel.shape[:2] != (5, 5) or ctx_kernel.shape[3] != 2 * ctx_kernel.shape[2]:
+    raise _lib.InvalidArgumentError(f"context kernel must be [5, 5, M, 2M]: {tuple(ctx_kernel.shape)}")
+  M = int(ctx_kernel.shape[2])
+  if w3.dim() != 2 or M <= 0 or w3.shape[1] % (3 * M):
+    raise _lib.InvalidArgumentError(f"W3 of shape {tuple(w3.shape)} must be [8M/3, 3KM] for M={M}")
+  K = int(w3.shape[1]) // (3 * M)
+  lay = cbm_layout(M, K)
+  dev = ctx_kernel.device
+  if dev.type != "cuda":
+    raise _lib.InvalidArgumentError(f"the parameters must be on a CUDA device, not {dev}")
+  n3, n4, no = lay["N3"], lay["N4"], lay["NO"]
+  want = ((ctx_bias, (2 * M,)), (w1, (4 * M, n3)), (b1, (n3,)), (w2, (n3, n4)), (b2, (n4,)), (w3, (n4, no)),
+          (b3, (no,)))
+  ops = [_f32(ctx_kernel[[dy + 2 for dy, _ in CB_TAPS], [dx + 2 for _, dx in CB_TAPS]], dev)]
+  for t, shape in want:
+    t = t.detach()
+    if tuple(t.shape) != shape:
+      raise _lib.InvalidArgumentError(f"parameter of shape {tuple(t.shape)} where M={M}, K={K} needs {shape}")
+    ops.append(_f32(t, dev))
+  packed = torch.empty(lay["total"], dtype=torch.float32, device=dev)
+  check(_lib.lib().tfcb_cbm_pack_weights(M, K, *[_p(t) for t in ops], _p(packed), lay["total"], _stream()))
+  return packed
+
+
+def _cbm_check_packed(packed, M, K):
+  n = cbm_layout(M, K)["total"]
+  if not isinstance(packed, torch.Tensor) or packed.dim() != 1 or packed.dtype != torch.float32:
+    raise _lib.InvalidArgumentError("`packed` must be a float32 vector from cbm_pack_weights")
+  if packed.numel() != n:
+    raise _lib.InvalidArgumentError(f"packed weights hold {packed.numel()} floats, M={M} with K={K} needs {n}")
+  if packed.device.type != "cuda":
+    raise _lib.InvalidArgumentError(f"`packed` must be on a CUDA device, not {packed.device}")
+  return n
+
+
+def _cbm_dims(packed, K, psi):
+  """(B, H, W, M, packed floats) from psi [B, H, W, 2M], checked against the packed buffer."""
+  if not isinstance(psi, torch.Tensor) or psi.dim() != 4 or psi.shape[-1] % 2:
+    raise _lib.InvalidArgumentError("`psi` must be [B, H, W, 2M]")
+  B, H, W, M = int(psi.shape[0]), int(psi.shape[1]), int(psi.shape[2]), int(psi.shape[3]) // 2
+  if B == 0 or H == 0 or W == 0:
+    raise _lib.InvalidArgumentError(f"empty latents: psi has shape {tuple(psi.shape)}")
+  n = _cbm_check_packed(packed, M, K)
+  if psi.device != packed.device:
+    raise _lib.InvalidArgumentError(f"`packed` ({packed.device}) and `psi` ({psi.device}) must share a CUDA device")
+  return B, H, W, M, n
+
+
+def _cbm_coder(family, precision, tail_mass, max_support):
+  if family not in MIXTURE_FAMILIES:
+    raise _lib.InvalidArgumentError(f"`family` must be one of {sorted(MIXTURE_FAMILIES)}: {family!r}")
+  return dict(family=family, precision=precision, tail_mass=tail_mass, max_support=max_support)
+
+
+def _cbm_lengths(counts, M, substreams):
+  """The stream lengths of items of counts[u] positions of M latents: one stream each, or S substreams each as
+  MixtureEntropyModel splits a [positions, M] coding unit."""
+  if substreams == 1:
+    return [int(c) * M for c in counts]
+  return substream_layout([[int(c)] for c in counts], M, substreams)[0].tolist()
+
+
+def cbm_join(parts):
+  """The y strings of B images from the 2B strings `parts` (image b's anchors at 2b, its non-anchors at 2b + 1):
+  varint(len A) ‖ A ‖ N each.  One device-to-host copy (the offsets); the bytes stay on the device."""
+  offs = parts.offsets_dev.cpu().numpy()
+  n = parts.numel() // 2
+  heads = [gen_ops._varint(int(offs[2 * b + 1] - offs[2 * b])) for b in range(n)]
+  dev = parts.bytes_dev.device
+  hbuf = torch.from_numpy(np.frombuffer(b"".join(heads) + b"\0", dtype=np.uint8).copy()).to(dev)
+  chunks, out_offs, at = [], [0], 0
+  for b, h in enumerate(heads):
+    lo, hi = int(offs[2 * b]), int(offs[2 * b + 2])
+    chunks += [hbuf[at:at + len(h)], parts.bytes_dev[lo:hi]]
+    at += len(h)
+    out_offs.append(out_offs[-1] + len(h) + hi - lo)
+  data = torch.cat(chunks + [torch.zeros(1, dtype=torch.uint8, device=dev)])
+  return gen_ops.Strings(data, torch.tensor(out_offs, dtype=torch.int64).to(dev), (n,))
+
+
+def cbm_split(s, i=0):
+  """(A, N) of string number `i`, `s` (bytes).  A truncated or non-minimal varint, or an anchor part that runs past
+  the end of the string, raises InvalidArgumentError naming the string."""
+  s = bytes(s)
+  v, shift, at = 0, 0, 0
+  while True:
+    if at >= len(s):
+      raise _lib.InvalidArgumentError(f"string {i}: truncated length of its anchor part")
+    b = s[at]
+    at += 1
+    v |= (b & 0x7F) << shift
+    if not b & 0x80:
+      break
+    shift += 7
+    if shift > 63:
+      raise _lib.InvalidArgumentError(f"string {i}: anchor length varint longer than 64 bits")
+  if at > 1 and b == 0:
+    raise _lib.InvalidArgumentError(f"string {i}: anchor length varint not in minimal form")
+  if v > len(s) - at:
+    raise _lib.InvalidArgumentError(f"string {i}: an anchor part of {v} bytes runs past the end of its {len(s)} bytes")
+  return s[at:at + v], s[at + v:]
+
+
+def _cbm_parts(strings, n, substreams):
+  """Both colours' strings of n y strings, split on the host before any device work: (anchors, non-anchors), each a
+  Strings of their payloads (n S substreams with S > 1)."""
+  if not isinstance(strings, gen_ops.Strings):
+    strings = gen_ops.Strings.from_bytes(list(strings), (len(strings),))
+  if strings.numel() != n:
+    raise _lib.InvalidArgumentError(f"{strings.numel()} strings for {n} images")
+  split = [cbm_split(s, i) for i, s in enumerate(strings.tolist())]
+  out = []
+  for c in range(2):
+    part = gen_ops.Strings.from_bytes([p[c] for p in split], (n,))
+    out.append(gen_ops.split_substreams(part, substreams) if substreams > 1 else part)
+  return out
+
+
+def _cbm_pass(packed, K, y_hat, psi, anchors, whole, weight, loc, scale, y=None, y_cb=None, y_hat_out=None):
+  B, H, W, M, n = _cbm_dims(packed, K, psi)
+  lib = _lib.lib()
+  nw = int(lib.tfcb_cbm_workspace_floats(M, int(K), B, H, W, int(bool(anchors))))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=packed.device)
+  check(lib.tfcb_cbm_params(_p(packed), n, M, int(K), _p(y_hat), _p(psi), B, H, W, int(bool(anchors)), _p(work), nw,
+                            int(whole), _p(weight), _p(loc), _p(scale), _p(y), _p(y_cb), _p(y_hat_out), _stream()))
+
+
+def cbm_params(packed, K, y_hat, psi, anchors):
+  """One parameter pass: (weight, loc, scale) [B, n, M, K] of the n positions of one colour of every image, in coding
+  order, as the mixture coder takes them (weights unnormalised, the largest 1).  The non-anchor pass reads the
+  anchors of y_hat [B, H, W, M]; the anchor pass reads no latent (y_hat may be None)."""
+  B, H, W, M, _ = _cbm_dims(packed, K, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  if y_hat is not None or not anchors:
+    y_hat = _ar_tensor(y_hat, "y_hat", (B, H, W, M), dev)
+  n = cb_counts(H, W)[0 if anchors else 1]
+  weight, loc, scale = (torch.empty((B, n, M, int(K)), dtype=torch.float32, device=dev) for _ in range(3))
+  _cbm_pass(packed, K, y_hat, psi, anchors, False, weight, loc, scale)
+  return weight, loc, scale
+
+
+def cbm_encode(packed, K, y, psi, family="normal", substreams=1, precision=16, tail_mass=2**-8, max_support=256):
+  """The two-pass encoder: returns (y_hat [B, H, W, M], strings of shape (B,)).  y_hat = float(int32(rint(y)))
+  (saturating, NaN -> 0), the anchors' before the non-anchor pass reads them; then one mixture_encode_ragged of the
+  coding-order y over the 2B items (image, colour) and one join."""
+  coder = _cbm_coder(family, precision, tail_mass, max_support)
+  S = gen_ops.check_substreams(substreams)
+  B, H, W, M, _ = _cbm_dims(packed, K, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  y = _ar_tensor(y, "y", (B, H, W, M), dev)
+  y_hat = torch.empty((B, H, W, M), dtype=torch.float32, device=dev)
+  y_cb = torch.empty((B, H * W, M), dtype=torch.float32, device=dev)
+  weight, loc, scale = (torch.empty((B, H * W, M, int(K)), dtype=torch.float32, device=dev) for _ in range(3))
+  for anchors in (True, False):
+    _cbm_pass(packed, K, y_hat, psi, anchors, True, weight, loc, scale, y, y_cb, y_hat)
+  parts = mixture_encode_ragged(y_cb, weight, loc, scale, _cbm_lengths(cb_counts(H, W) * B, M, S), **coder)
+  if S > 1:
+    parts = gen_ops.join_substreams(parts, S, (2 * B,))
+  return y_hat, cbm_join(parts)
+
+
+def cbm_decode(strings, packed, K, psi, family="normal", substreams=1, precision=16, tail_mass=2**-8,
+               max_support=256):
+  """Inverse of cbm_encode: anchor parameters, one mixture decode of every image's anchors, their latents to
+  [B, H, W, M], non-anchor parameters, one decode of the non-anchors, to [B, H, W, M].  Returns y_hat [B, H, W, M].
+  The strings are split on the host first; a length that overruns its string or a wrong `substreams` raises
+  InvalidArgumentError before any device work."""
+  coder = _cbm_coder(family, precision, tail_mass, max_support)
+  S = gen_ops.check_substreams(substreams)
+  B, H, W, M, _ = _cbm_dims(packed, K, psi)
+  dev = packed.device
+  psi = _ar_tensor(psi, "psi", (B, H, W, 2 * M), dev)
+  parts = _cbm_parts(strings, B, S)
+  y_hat = torch.zeros((B, H, W, M), dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for c, anchors in enumerate((True, False)):
+    n = cb_counts(H, W)[c]
+    if n == 0:
+      continue
+    weight, loc, scale = cbm_params(packed, K, y_hat, psi, anchors)
+    part = mixture_decode_ragged(parts[c], weight, loc, scale, _cbm_lengths([n] * B, M, S), **coder)
+    check(lib.tfcb_cb_scatter(_p(part), B, H, W, M, int(anchors), _p(y_hat), _stream()))
+  return y_hat
+
+
+def _cbm_ragged(packed, K, psis):
+  """(heights, widths, M, packed floats, flat psi) of a ragged call."""
+  hs, ws, M = _ragged_list(psis)
+  n = _cbm_check_packed(packed, M, K)
+  return hs, ws, M, n, _ragged_cat(psis, "psi", hs, ws, 2 * M, packed.device)
+
+
+def _cbm_pass_ragged(packed, K, M, n, hs, ws, y_hat, psi, anchors, whole=False, weight=None, loc=None, scale=None,
+                     y=None, y_cb=None, y_hat_out=None):
+  """One pass over the flat list.  Per-pass outputs (weight None) are allocated: returns (weight, loc, scale, counts,
+  work) with image i's n_k,i M rows at M Q_i; the workspace holds the image table for the scatter."""
+  dev = packed.device
+  lib = _lib.lib()
+  k = hs.size
+  counts = (hs * ws + 1) // 2 if anchors else hs * ws // 2
+  if weight is None:
+    weight, loc, scale = (torch.empty((int(counts.sum()) * M, int(K)), dtype=torch.float32, device=dev)
+                          for _ in range(3))
+  nw = int(lib.tfcb_cbm_ragged_workspace_floats(M, int(K), k, _host(hs), _host(ws), int(bool(anchors))))
+  work = torch.empty(max(nw, 1), dtype=torch.float32, device=dev)
+  check(lib.tfcb_cbm_params_ragged(_p(packed), n, M, int(K), _p(y_hat), _p(psi), k, _host(hs), _host(ws),
+                                   int(bool(anchors)), _p(work), nw, int(whole), _p(weight), _p(loc), _p(scale), _p(y),
+                                   _p(y_cb), _p(y_hat_out), _stream()))
+  return weight, loc, scale, counts, work
+
+
+def cbm_params_ragged(packed, K, y_hats, psis, anchors):
+  """cbm_params over a list of images of their own shapes in one pass: (weight, loc, scale, lengths), the first three
+  [sum n_i M, K] with image i's n_i M rows (n_i its positions of this colour) after image i - 1's; `lengths` are the
+  n_i M.  y_hats is a list of [H_i, W_i, M] (may be None for the anchor pass).  Image i's values equal cbm_params on
+  that image alone, bit for bit."""
+  hs, ws, M, n, psi = _cbm_ragged(packed, K, psis)
+  dev = packed.device
+  y_hat = None if y_hats is None and anchors else _ragged_cat(y_hats, "y_hat", hs, ws, M, dev)
+  weight, loc, scale, counts, _ = _cbm_pass_ragged(packed, K, M, n, hs, ws, y_hat, psi, anchors)
+  return weight, loc, scale, (counts * M).tolist()
+
+
+def cbm_encode_ragged(packed, K, ys, psis, family="normal", substreams=1, precision=16, tail_mass=2**-8,
+                      max_support=256):
+  """cbm_encode of a list of images of their own shapes, one pass sequence and one mixture encode for the whole list:
+  returns (y_hats, strings of shape (n,)), y_hats the list of [H_i, W_i, M].  String i equals cbm_encode's string of
+  image i alone."""
+  coder = _cbm_coder(family, precision, tail_mass, max_support)
+  S = gen_ops.check_substreams(substreams)
+  hs, ws, M, n, psi = _cbm_ragged(packed, K, psis)
+  dev = packed.device
+  y = _ragged_cat(ys, "y", hs, ws, M, dev)
+  y_hat, y_cb = torch.empty_like(y), torch.empty_like(y)
+  weight, loc, scale = (torch.empty((y.numel(), int(K)), dtype=torch.float32, device=dev) for _ in range(3))
+  for anchors in (True, False):
+    _cbm_pass_ragged(packed, K, M, n, hs, ws, y_hat, psi, anchors, True, weight, loc, scale, y, y_cb, y_hat)
+  counts = np.stack([(hs * ws + 1) // 2, hs * ws // 2], 1).reshape(-1)
+  parts = mixture_encode_ragged(y_cb, weight, loc, scale, _cbm_lengths(counts, M, S), **coder)
+  if S > 1:
+    parts = gen_ops.join_substreams(parts, S, (2 * hs.size,))
+  return _ragged_views(y_hat, hs, ws, M), cbm_join(parts)
+
+
+def cbm_decode_ragged(strings, packed, K, psis, family="normal", substreams=1, precision=16, tail_mass=2**-8,
+                      max_support=256):
+  """cbm_decode of a list of images of their own shapes, one string per image: per colour one ragged parameter pass,
+  one mixture decode and one scatter for the whole list.  Returns the list of y_hat [H_i, W_i, M]."""
+  coder = _cbm_coder(family, precision, tail_mass, max_support)
+  S = gen_ops.check_substreams(substreams)
+  hs, ws, M, n, psi = _cbm_ragged(packed, K, psis)
+  dev = packed.device
+  parts = _cbm_parts(strings, hs.size, S)
+  y_hat = torch.zeros(int((hs * ws).sum()) * M, dtype=torch.float32, device=dev)
+  lib = _lib.lib()
+  for c, anchors in enumerate((True, False)):
+    weight, loc, scale, counts, work = _cbm_pass_ragged(packed, K, M, n, hs, ws, y_hat, psi, anchors)
+    if not counts.any():
+      continue
+    part = mixture_decode_ragged(parts[c], weight, loc, scale, _cbm_lengths(counts, M, S), **coder)
+    check(lib.tfcb_scc_scatter_ragged(_p(part), hs.size, _host(hs), _host(ws), M, 0, M, int(anchors), _p(work),
+                                      work.numel(), _p(y_hat), _stream()))
+  return _ragged_views(y_hat, hs, ws, M)
+
+
+# ------------------------------------------------------------------------------------------------
 # Multistage context model (Lin et al. 2023): four parameter passes over the stages of a 2x2 schedule (tfcb_msc_*).
 # Position (r, c) has phase (r mod 2, c mod 2); the phases (0, 0), (1, 1), (0, 1), (1, 0) are stages 0 to 3.  Stage
 # s >= 1 reads the decoded latents at its taps (the offsets whose neighbour is in an earlier stage) through its own

@@ -28,7 +28,7 @@ from compression_b200.gdn import GDN
 from compression_b200.packed_tensors import PackedTensors
 from compression_b200.signal_conv import SignalConv2D
 
-__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MultistageModel", "MixtureHyperpriorModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
+__all__ = ["BLS2017Model", "BMSHJ2018Model", "MS2020Model", "MBT2018Model", "CheckerboardModel", "SpaceChannelModel", "MultistageModel", "MixtureHyperpriorModel", "CheckerboardMixtureModel", "MaskedConv2D", "AnalysisTransform", "SynthesisTransform", "HyperAnalysisTransform",
            "HyperSynthesisTransform", "bench_model_paths", "mean_metrics"]
 
 
@@ -1100,6 +1100,143 @@ class CheckerboardModel(MBT2018Model):
 
   def _decode_ragged(self, handle, psis, cdf_offset):
     return F.cb_decode_ragged(handle, self._packed, psis, self.num_scales, cdf_offset, substreams=self.substreams)
+
+
+class CheckerboardMixtureModel(_Model):
+  """The checkerboard context model with a discretized mixture prior on y (Cheng et al., CVPR 2020, without the
+  attention modules).  N = num_filters, M = latent_depth (a multiple of 6), K = num_components (in [1, 64]).
+  CheckerboardModel's transforms, psi of width 2M and CheckerboardConv2D(M, 2M) context model; the entropy-parameter
+  layers are 1x1 4M -> 10M/3 -> 8M/3 -> 3KM with LeakyReLU between them, channel c reading its K logits, K locs and K
+  scales from outputs 3Kc .. 3Kc + 3K - 1 as MixtureHyperpriorModel reads its hyper synthesis.  z is coded as in
+  MixtureHyperpriorModel, y by entropy_models.MixtureEntropyModel's coder.
+
+  Coding runs on the checkerboard's two parameter passes (functional.cbm_*, DESIGN §3.19): every latent is coded as
+  int32(rint(y)), so y_hat does not depend on the parameters; the anchors' mixtures come from psi alone, the
+  non-anchors' from psi and the decoded anchors.  An image's y string is varint(len A) ‖ A ‖ N, A and N the
+  MixtureEntropyModel strings of its anchors' and its non-anchors' coding-order latents (each with `substreams`
+  substreams).  The hyper synthesis runs per image, so an image's strings do not depend on its batch or list."""
+
+  def __init__(self, lmbda=0.01, num_filters=192, latent_depth=192, num_components=3, family="normal", substreams=1):
+    super().__init__()
+    self._set_substreams(substreams)
+    N, M, K = int(num_filters), int(latent_depth), int(num_components)
+    if M <= 0 or M % 6:
+      raise ValueError(f"latent_depth must be a positive multiple of 6 (3M/2, 10M/3 and 8M/3 are layer widths): {M}")
+    if K < 1 or K > 64:
+      raise ValueError(f"num_components must be in [1, 64]: {K}")
+    if family not in F.MIXTURE_FAMILIES:
+      raise ValueError(f"`family` must be one of {sorted(F.MIXTURE_FAMILIES)}: {family!r}")
+    self.num_components, self.family = K, family
+    MBT2018Model._init_transforms(self, lmbda, N, M, 64, .11, 256.)
+    self.context_model = CheckerboardConv2D(M, 2 * M)
+    ep = lambda f, name, act: _conv(f, 1, name, kernel_parameter="variable", activation=act)
+    self.entropy_parameters = nn.Sequential(
+        ep(10 * M // 3, "layer_0", _leaky), ep(8 * M // 3, "layer_1", _leaky), ep(3 * K * M, "layer_2", None))
+    self.hyperprior = D.NoisyDeepFactorized(batch_shape=(N,))
+    self.entropy_model = E.MixtureEntropyModel(family, coding_rank=3)
+    self.side_entropy_model = None
+    self._packed = None
+
+  _psi = MBT2018Model._psi
+
+  def mixture_parameters(self, y_ctx, psi):
+    """The parallel (training) form of the parameter network: (weight, loc, scale), each [B, H, W, M, K], from the
+    latents the context model sees and psi [B, H, W, 2M]; weights are a softmax, scales bounded below at 0.11."""
+    params = self.entropy_parameters(torch.cat([psi, checkerboard_context(self.context_model, y_ctx)], dim=-1))
+    return MixtureHyperpriorModel.mixture_parameters(self, params)
+
+  def forward(self, x, training=True):
+    """-> (loss, bpp, mse).  The context model sees y plus uniform noise when training, round(y) otherwise; the rate
+    of y goes through the NoisyNormalMixture / NoisyLogisticMixture graph."""
+    side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3, compression=False)
+    x = x.to(torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    z_hat, side_bits = side_entropy_model(z, training=training)
+    psi = self.hyper_synthesis_transform(z_hat)[:, :y.shape[1], :y.shape[2], :]
+    y_ctx = y + torch.empty_like(y).uniform_(-.5, .5) if training else torch.round(y)
+    y_hat, bits = self.entropy_model(y, *self.mixture_parameters(y_ctx, psi), training=training)
+    self._last_x_hat = self.synthesis_transform(y_hat)[:, :x.shape[1], :x.shape[2], :]
+    return self.rate_distortion(x, bits.sum() + side_bits.sum())
+
+  def fix_tables(self):
+    """Builds z's coding tables and packs the parameter network for the coding kernels (call again after the weights
+    change)."""
+    self.side_entropy_model = E.ContinuousBatchedEntropyModel(self.hyperprior, coding_rank=3,
+                                                              compression=True).to(self._device())
+    self._packed = F.cbm_pack_weights(self.context_model.kernel, self.context_model.bias,
+                                      *_dense_weights(self.entropy_parameters))
+    return self
+
+  def _coder(self):
+    return dict(substreams=self.substreams, **self.entropy_model._coder_args())
+
+  def compress(self, x):
+    """uint8 [H, W, 3] -> (string, side_string, x_shape, y_shape, z_shape), bmshj2018's signature."""
+    return self.compress_batch(_as_image(x)[None])
+
+  def decompress(self, string, side_string, x_shape, y_shape, z_shape):
+    return self.decompress_batch(string, side_string, x_shape, y_shape, z_shape)[0]
+
+  @torch.no_grad()
+  def compress_batch(self, x):
+    x = _as_batch(x).to(device=self._device(), dtype=torch.float32)
+    y = self.analysis_transform(x)
+    z = self.hyper_analysis_transform(y)
+    shapes = tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+    side_string = self.side_entropy_model.compress(z, substreams=self.substreams)
+    psi = self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))
+    string = F.cbm_encode(self._packed, self.num_components, y.contiguous(), psi, **self._coder())[1]
+    return (string, side_string) + shapes
+
+  @torch.no_grad()
+  def decompress_batch(self, string, side_string, x_shape, y_shape, z_shape):
+    z_hat = self.side_entropy_model.decompress(side_string, tuple(int(v) for v in z_shape), substreams=self.substreams)
+    psi = self._psi(z_hat, (int(y_shape[0]), int(y_shape[1])))
+    if not isinstance(string, gen_ops.Strings):
+      string = gen_ops.Strings.from_bytes(string)
+    y_hat = F.cbm_decode(gen_ops.Strings(string.bytes_dev, string.offsets_dev, (string.numel(),)), self._packed,
+                         self.num_components, psi, **self._coder())
+    x_hat = self.synthesis_transform(y_hat)
+    return _to_uint8(x_hat[:, :int(x_shape[0]), :int(x_shape[1]), :])
+
+  @torch.no_grad()
+  def compress_images(self, images):
+    """images: list of uint8 [H_i, W_i, 3] -> the list of what `compress(image)` returns, element for element.  The
+    transforms run per image; z and y of the whole list are each coded in one ragged launch sequence."""
+    xs = [_as_image(x)[None].to(device=self._device(), dtype=torch.float32) for x in images]
+    if not xs:
+      raise ValueError("`images` is empty")
+    ys = [self.analysis_transform(x) for x in xs]
+    zs = [self.hyper_analysis_transform(y) for y in ys]
+    side_strings = self.side_entropy_model.compress_ragged([z[0] for z in zs], substreams=self.substreams).split()
+    psis = [self._psi(self.side_entropy_model.quantize(z), tuple(y.shape[1:-1]))[0] for y, z in zip(ys, zs)]
+    strings = F.cbm_encode_ragged(self._packed, self.num_components, [y[0] for y in ys], psis,
+                                  **self._coder())[1].split()
+    return [(strings[i], side_strings[i]) + tuple(torch.tensor(t.shape[1:-1], dtype=torch.int32) for t in (x, y, z))
+            for i, (x, y, z) in enumerate(zip(xs, ys, zs))]
+
+  @torch.no_grad()
+  def decompress_images(self, items):
+    """items: tuples as `compress_images` returns them -> list of uint8 [H_i, W_i, 3]."""
+    items = list(items)
+    if not items:
+      raise ValueError("`items` is empty")
+    z_hats = self.side_entropy_model.decompress_ragged(gen_ops.Strings.concat([it[1] for it in items]),
+                                                       [tuple(int(v) for v in it[4]) for it in items],
+                                                       substreams=self.substreams)
+    psis = [self._psi(z_hat[None], (int(it[3][0]), int(it[3][1])))[0] for z_hat, it in zip(z_hats, items)]
+    y_hats = F.cbm_decode_ragged(gen_ops.Strings.concat([it[0] for it in items]), self._packed, self.num_components,
+                                 psis, **self._coder())
+    out = []
+    for y_hat, it in zip(y_hats, items):
+      x_hat = self.synthesis_transform(y_hat[None])
+      out.append(_to_uint8(x_hat[:, :int(it[2][0]), :int(it[2][1]), :])[0])
+    return out
+
+  def decompress_from_tfci(self, data):
+    dtypes = [bytes, bytes, torch.int32, torch.int32, torch.int32]
+    return self.decompress(*PackedTensors(data).unpack(dtypes))
 
 
 class SpaceChannelModel(MBT2018Model):

@@ -636,6 +636,45 @@ int tfcb_mixture_decode_ragged(const uint8_t* bytes_dev, const int64_t* offsets_
                                int max_support, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Checkerboard context model with mixture priors, DESIGN.md §3.19: the two checkerboard passes of tfcb_cb_params
+ * (anchors r + c even, then non-anchors; coding order and float32 order as there) on a network whose last layer has
+ * 3KM outputs, followed by an epilogue that writes each (position, channel)'s K components for the mixture coder:
+ * weight_k = expf(l_k - max_j l_j) (unnormalised), loc_k, scale_k = fmaxf(raw, 0.11f), channel c reading its K logits,
+ * K locs and K scales from outputs 3Kc .. 3Kc + 3K - 1.  M is a multiple of 6 in [6, 384], K in [1, 64].
+ * tfcb_cbm_packed_floats returns the packed size (-1 if unsupported) and, with `layout`, writes int64 [12]: K1, N3,
+ * N4, NO = 3KM and the offsets of Wc [12M, 2M] (the 12 checkerboard taps, raster order), bc, W1 [4M, N3], b1,
+ * W2 [N3, N4], b2, W3 [N4, 3KM], b3; tfcb_cbm_pack_weights copies the eight operands there.
+ * tfcb_cbm_params runs one pass over every position of one colour of B images of H x W: weight_dev, loc_dev and
+ * scale_dev float32 [B, n_k, M, K] in coding order (whole == 0), or each image's [H W, M, K] block of both colours at
+ * this pass's rows (whole != 0).  The non-anchor pass reads the anchors of yhat_dev [B, H, W, M].  With y_dev
+ * [B, H, W, M] (the encoder, whole != 0) it also writes y in coding order to y_cb_dev [B, H W, M] and
+ * float((int)rintf(y)) at this pass's positions of yhat_out_dev [B, H, W, M].  Four launches for the anchors, five
+ * for the non-anchors, none for an empty pass.  The _ragged forms take a list of n_images latents of
+ * heights_host[i] x widths_host[i] back to back, per-pass outputs at M Q_i K (Q_i: the images before i's positions
+ * of this colour), whole outputs at M P_i K (+ n_a,i M K for the non-anchors); the workspace holds the image table,
+ * which tfcb_scc_scatter_ragged (offset 0, C = M) reads for the scatter of decoded latents.  Every argument is
+ * checked before any launch (TFCB_INVALID_ARGUMENT).
+ * ---------------------------------------------------------------------------------------------- */
+int64_t tfcb_cbm_packed_floats(int M, int K, int64_t* layout);
+int tfcb_cbm_pack_weights(int M, int K, const float* ctx_taps_dev, const float* ctx_bias_dev, const float* w1_dev,
+                          const float* b1_dev, const float* w2_dev, const float* b2_dev, const float* w3_dev,
+                          const float* b3_dev, float* packed_dev, int64_t packed_floats, void* stream);
+/* Floats of workspace one tfcb_cbm_params pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_cbm_workspace_floats(int M, int K, int64_t B, int64_t H, int64_t W, int anchors);
+int tfcb_cbm_params(const float* packed_dev, int64_t packed_floats, int M, int K, const float* yhat_dev,
+                    const float* psi_dev, int64_t B, int64_t H, int64_t W, int anchors, float* work_dev,
+                    int64_t work_floats, int whole, float* weight_dev, float* loc_dev, float* scale_dev,
+                    const float* y_dev, float* y_cb_dev, float* yhat_out_dev, void* stream);
+/* Floats of workspace one tfcb_cbm_params_ragged pass needs, or -1 if the arguments are not supported. */
+int64_t tfcb_cbm_ragged_workspace_floats(int M, int K, int64_t n_images, const int64_t* heights_host,
+                                         const int64_t* widths_host, int anchors);
+int tfcb_cbm_params_ragged(const float* packed_dev, int64_t packed_floats, int M, int K, const float* yhat_dev,
+                           const float* psi_dev, int64_t n_images, const int64_t* heights_host,
+                           const int64_t* widths_host, int anchors, float* work_dev, int64_t work_floats, int whole,
+                           float* weight_dev, float* loc_dev, float* scale_dev, const float* y_dev, float* y_cb_dev,
+                           float* yhat_out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * PmfToQuantizedCdf:
  *   op contract   tensorflow_compression/cc/ops/pmf_to_cdf_ops.cc:28-57
  *   CPU kernel    tensorflow_compression/cc/kernels/pmf_to_cdf_kernels.cc:58-208

@@ -7,8 +7,8 @@ The model has random weights (seeded) unless --state-dict loads a torch state_di
 arguments.  The images are the PNGs of --images DIR (read with PIL, converted to RGB) or, with --synthetic kodak,
 24 seeded smooth-plus-noise images of Kodak's shapes, 12 of 512x768 and 12 of 768x512; with --synthetic mixed, 24
 such images of seeded, all different shapes (sides multiples of 16 from 256 to 1024), as in a dataset of many image
-sizes.  The context models (mbt2018, checkerboard, space_channel, multistage, space_channel_multistage) code such a
-list with one ragged launch sequence.
+sizes.  The context models (mbt2018, checkerboard, space_channel, multistage, space_channel_multistage,
+checkerboard_mixture) code such a list with one ragged launch sequence.
 --substreams S writes every string as S independently decodable streams (DESIGN §3.14); bpp includes their headers.
 --tiles T (mbt2018 only) writes every y string as T column tiles, coded as a wavefront over many SMs (DESIGN §3.15).
 
@@ -49,7 +49,8 @@ BLOCKS = [  # (metric, colour space, key in the evaluate_images dicts)
 MODELS = {"bls2017": models.BLS2017Model, "bmshj2018": models.BMSHJ2018Model, "ms2020": models.MS2020Model,
           "mbt2018": models.MBT2018Model, "checkerboard": models.CheckerboardModel,
           "space_channel": models.SpaceChannelModel, "multistage": models.MultistageModel,
-          "space_channel_multistage": models.SpaceChannelMultistageModel}
+          "space_channel_multistage": models.SpaceChannelMultistageModel,
+          "checkerboard_mixture": models.CheckerboardMixtureModel}
 
 
 def mixed_shapes(seed, n=24):
